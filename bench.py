@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the B200-native compositor (contract: see DESIGN.md section 6).
+"""bench.py -- headline benchmark of the H100-native compositor (contract: see DESIGN.md section 6).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--workload cfg3] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--workload cfg3] [--impl ours|reference] [--dump-outputs DIR]
 
 A "step" is one pass of the hot path over one batch of synthetic input: one output frame of the
 workload (default: BASELINE config 3, 16 x 4K NV12 -> 4K NV12 mosaic with per-input Lanczos3 4:1
@@ -13,6 +13,9 @@ composites its own output stream (weak scaling, no data-path collective: outputs
 `roofline`  dominant kernel: algorithmic bytes per launch / its device time (events inside the library).
 `cpu_baseline` / `--impl reference`: the CPU oracle (restatement of the reference's wgpu path; the
             reference itself is Rust + wgpu and cannot run here) timed on the host cores, bounded sample.
+`--dump-outputs DIR`: the output planes of the last timed step as DIR/output_<k>_{y,uv}.npy (float32; a fixed seeded
+            sample of the elements when all of them would exceed 64 MB), so that two builds can be compared on the same
+            inputs.
 """
 import argparse
 import ctypes as C
@@ -126,7 +129,7 @@ SETUP_SECONDS = 0.3   # untimed set-up ticks before the W warm-up steps (clock r
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,clocks.mem,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -260,6 +263,26 @@ def run_reference(args, wl):
             "e2e": {"value": fps, "unit": "frames/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
             "gpu_launches": 0}
     print(json.dumps(line))
+
+
+DUMP_LIMIT_BYTES = 64_000_000
+DUMP_SEED = 0x5EED
+
+
+def dump_outputs(out_dir, planes):
+    """planes: {name: uint8 device tensor}.  Writes out_dir/<name>.npy as float32.  When all elements together exceed
+    DUMP_LIMIT_BYTES, every plane keeps the same share of its elements, at positions drawn once from a fixed seed."""
+    os.makedirs(out_dir, exist_ok=True)
+    total = sum(t.numel() for t in planes.values())
+    budget = (DUMP_LIMIT_BYTES - 4096 * len(planes)) // 4   # float32 elements, .npy headers set aside
+    for j, (name, t) in enumerate(planes.items()):
+        a = t.cpu().numpy().reshape(-1)
+        if total > budget:
+            m = t.numel() * budget // total
+            a = a[np.sort(np.random.default_rng(DUMP_SEED + j).choice(a.size, m, replace=False))]
+        else:
+            a = a.reshape(tuple(t.shape))
+        np.save(os.path.join(out_dir, f"{name}.npy"), a.astype(np.float32))
 
 
 class _DevMem:
@@ -431,6 +454,8 @@ def main():
     ap.add_argument("--no-secondary", action="store_true", help="N > 1: skip the cfg4 (NVLink exchange) leg")
     ap.add_argument("--exchange", default="all", choices=["all", "nccl", "peer_copy", "peer_direct"],
                     help="N > 1, cfg4 leg: how the shared inputs reach the other GPUs (all: measure each, report the fastest)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the output planes of the last timed step to DIR/<name>.npy (float32)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     wl = workload(args.workload)
@@ -577,6 +602,11 @@ def main():
     barrier()
     ms = e0.elapsed_time(e1)
     launches = r.stats()["kernel_launches"] - launches0
+    if args.dump_outputs and rank == 0:   # before any later leg overwrites the output planes
+        planes = {}
+        for k in range(n_out):
+            planes[f"output_{k + 1}_y"], planes[f"output_{k + 1}_uv"] = out_y[k], out_uv[k]
+        dump_outputs(args.dump_outputs, planes)
     ms_by_rank = [ms]
     if dist is not None:
         g = [torch.zeros(2, device=dev) for _ in range(world)]
@@ -601,7 +631,7 @@ def main():
     if os.path.exists(peaks_path):
         peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (of measured)"
     else:
-        peak, peak_src = 6650.0, "B200_PROFILING.md fallback (of fallback)"
+        peak, peak_src = 3350.0, "H100 SXM data sheet HBM3 bandwidth (not measured)"
     per_kernel = {}
     for name, (tot, cnt) in kt.items():
         if cnt:
@@ -611,16 +641,12 @@ def main():
                                 "ms_per_frame": tot / args.steps}
     dom = max(per_kernel, key=lambda k: per_kernel[k]["ms_per_frame"]) if per_kernel else None
     gpu_ms_frame = sum(v["ms_per_frame"] for v in per_kernel.values())
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "traffic.json")   # dram bytes per launch from the committed ncu capture
-    if os.path.exists(tpath) and dom:
-        traffic = json.load(open(tpath)).get(wl["name"], {}).get(dom)
     roofline = None
     if dom:
         # one launch of the dominant kernel processes one whole output frame's worth of its stage
         ach = wl["alg_bytes"] / (per_kernel[dom]["ms_per_frame"] * 1e-3) / 1e9
         roofline = {"bound": "hbm", "kernel": dom, "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-                    "traffic": traffic, "peak_source": peak_src,
+                    "peak_source": peak_src,
                     "algorithmic_bytes_per_launch": wl["alg_bytes"] // max(1, round(per_kernel[dom]["launches_per_frame"])),
                     "kernel_share_of_gpu_time": per_kernel[dom]["ms_per_frame"] / gpu_ms_frame,
                     "whole_frame": {"achieved": wl["alg_bytes"] / (ms_per_step * 1e-3) / 1e9,
@@ -647,7 +673,7 @@ def main():
                 arr[k].mem_kind = F.MEM_HOST
                 arr[k].planes[0], arr[k].planes[1] = hys[b][k].data_ptr(), huvs[b][k].data_ptr()
             host_out.append(arr)
-        ke = max(5, min(args.steps, 200))   # enough ticks that one host hiccup cannot dominate sub-ms ticks
+        ke = max(args.steps, DEPTH)   # the same K timed steps; at least one per buffer set of the pipeline
         def step_host(k, wait):
             for a in host_in[k % hv]:
                 a.pts_ns = k * frame_ns          # fresh frames every tick (a frame older than the fallback timeout is dropped)
@@ -721,7 +747,8 @@ def main():
                 "config": {"workload": wl["name"], "detail": wl["desc"], "outputs_per_gpu": n_out,
                            "nvlink_broadcast_bytes_per_tick": (n * iw * ih * 3 // 2) * (world - 1) if roots is not None else (secondary or {}).get("nvlink_broadcast_bytes_per_tick", 0),
                            "l2_policy": f"inputs larger than L2: {nvar} distinct frame sets of "
-                                        f"{wl['alg_bytes'] / 1e6:.0f} MB cycled (> 126 MB L2)",
+                                        f"{wl['alg_bytes'] / 1e6:.0f} MB cycled "
+                                        f"(L2: {torch.cuda.get_device_properties(dev).L2_cache_size / 1e6:.0f} MB)",
                            "algorithmic_bytes_per_frame": wl["alg_bytes"], "wall_s_timed_region": t_wall,
                            "device_ms_per_step_by_rank": [m / args.steps for m in ms_by_rank],
                            "host_submit_ms_per_step_by_rank": [m / args.steps for m in submit_by_rank],

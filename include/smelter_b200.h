@@ -1,5 +1,5 @@
 /*
- * smelter_b200.h -- C ABI of the B200-native per-output-frame compositor.
+ * smelter_b200.h -- C ABI of the H100-native per-output-frame compositor.
  *
  * Drop-in boundary: this library replaces `smelter_render::Renderer`
  * (reference: smelter-render/src/state.rs:95-193).  There is no C ABI in the reference (it is a Rust
@@ -13,7 +13,7 @@
  * untouched until the smr_render_end that retires that tick (smr_render has no such window: it returns when the tick
  * it submitted is complete); a handle is
  * internally synchronised exactly like the reference's `Arc<Mutex<InnerRenderer>>` (state.rs:54-55).
- * The product path has NO CPU fallback: every pixel is produced by sm_100a CUDA kernels.
+ * The product path has NO CPU fallback: every pixel is produced by sm_90a CUDA kernels.
  */
 #ifndef SMELTER_B200_H
 #define SMELTER_B200_H

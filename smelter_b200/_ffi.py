@@ -4,7 +4,7 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# SMR_LIB_PATH: a differently built copy of the same library (what-if builds of tools/exp_variants.sh)
+# SMR_LIB_PATH: a differently built copy of the same library (what-if builds with -DSMR_EXP_* switches)
 LIB_PATH = os.environ.get("SMR_LIB_PATH") or os.path.join(_HERE, "libsmelter_b200.so")
 
 SMR_OK = 0
@@ -144,7 +144,7 @@ def lib():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"{LIB_PATH} is missing: build it with `python -m smelter_b200.build` "
-            "(the B200 compositor has no CPU fallback)")
+            "(the H100 compositor has no CPU fallback)")
     L = C.CDLL(LIB_PATH)
     vp = C.c_void_p
     L.smr_create.argtypes = [C.POINTER(Options), C.POINTER(vp)]

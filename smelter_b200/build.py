@@ -1,4 +1,4 @@
-"""Builds libsmelter_b200.so (C-ABI library: C++ host + sm_100a CUDA kernels) in-tree with nvcc.
+"""Builds libsmelter_b200.so (C-ABI library: C++ host + sm_90a CUDA kernels) in-tree with nvcc.
 
 No torch, no JIT cache: the .so sits next to this file so that it travels to the GPU box.
 """
@@ -14,7 +14,7 @@ HEADERS = ["kernels.h", "scene.h", "ptx_helpers.cuh", "resample_tma.cuh", "resam
 
 NVCC_FLAGS = [
     "-std=c++17", "-O3",
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo",
     "-fmad=false",            # numeric contract: only explicit fmaf() is fused
     "-prec-div=true", "-prec-sqrt=true", "-ftz=false",

@@ -1,4 +1,4 @@
-// kernels.cu -- hand-written sm_100a kernels of the per-output-frame compositor.
+// kernels.cu -- hand-written sm_90a kernels of the per-output-frame compositor.
 //
 // Replaces the reference's WGSL shader set (SURVEY 2.2 K1..K11):
 //   k_convert     planar_yuv_to_rgba.wgsl / nv12_to_rgba.wgsl / bgra / argb           (K1,K2,K4)
@@ -527,7 +527,7 @@ int launch_resample(const ResampleJob *jobs_dev, const ResampleJob *jobs_host, i
 
 __constant__ float c_wint[5][32];   // [S][tap]
 __constant__ float c_winv[5];       // 1 / weight_sum
-__constant__ float2 c_wpair[5][32]; // [S][tap] = (w[tap], w[tap - S]): the b-channel FFMA2 of two adjacent output columns
+__constant__ float2 c_wpair[5][32]; // [S][tap] = (w[tap], w[tap - S]): the b-channel FMA pair of two adjacent output columns
 
 void set_int_weights(int S, const float *weights_dev, const float *inv_dev, int taps, Stream s) {
     cudaMemcpyToSymbolAsync(c_wint, weights_dev, sizeof(float) * taps, sizeof(float) * 32 * S, cudaMemcpyDeviceToDevice, (cudaStream_t)s);

@@ -1,4 +1,4 @@
-// kernels.h -- device-side job descriptors + launchers of the sm_100a compositor kernels.
+// kernels.h -- device-side job descriptors + launchers of the sm_90a compositor kernels.
 // Host code (renderer.cpp, g++) and kernels.cu (nvcc) share this header; it is plain C++.
 #pragma once
 

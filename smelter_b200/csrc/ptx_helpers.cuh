@@ -1,5 +1,5 @@
 // ptx_helpers.cuh -- inline-PTX wrappers shared by the kernels (included by kernels.cu inside smr::dev): mbarrier / TMA,
-// volatile shared-memory loads of TMA stages, and the packed FP32 pairs of sm_100 (FFMA2 / FMUL2 / FADD2).
+// volatile shared-memory loads of TMA stages, and FP32 pair helpers.
 #pragma once
 
 namespace v5 {
@@ -57,7 +57,9 @@ __device__ __forceinline__ float lds_tab(uint32_t a) {
     return x;
 }
 
-// ---- packed FP32 (sm_100: FFMA2 / FMUL2 / FADD2), IEEE round-to-nearest per component --------------------------
+// ---- FP32 pairs, IEEE round-to-nearest per component ------------------------------------------------------------
+// sm_90 has no packed FP32 arithmetic: a pair is two scalar FFMA / FMUL / FADD.  The _rn intrinsics are never contracted,
+// so every component is rounded exactly where the expression says, as in the oracle.
 __device__ __forceinline__ unsigned long long pk(float2 a) {
     unsigned long long r;
     asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a.x), "f"(a.y));
@@ -69,34 +71,20 @@ __device__ __forceinline__ float2 upk(unsigned long long r) {
     return a;
 }
 __device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
-    unsigned long long d;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(pk(a)), "l"(pk(b)), "l"(pk(c)));
-    return upk(d);
+    return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
-__device__ __forceinline__ float2 mul2(float2 a, float2 b) {
-    unsigned long long d;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(pk(a)), "l"(pk(b)));
-    return upk(d);
-}
-__device__ __forceinline__ float2 add2(float2 a, float2 b) {
-    unsigned long long d;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(pk(a)), "l"(pk(b)));
-    return upk(d);
-}
+__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 __device__ __forceinline__ float2 splat(float a) { return make_float2(a, a); }
-// the packed operands as they stand (no unpack / repack the compiler could turn into second copies of the registers)
+// a pair held as one 64-bit register pair (the layout of the weight pairs and of the shared-memory loads below)
 __device__ __forceinline__ unsigned long long fma2q(unsigned long long a, unsigned long long b, unsigned long long c) {
-    unsigned long long d;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-    return d;
+    return pk(fma2(upk(a), upk(b), upk(c)));
 }
 __device__ __forceinline__ void lds128q(uint32_t addr, unsigned long long &lo, unsigned long long &hi) {
     asm volatile("ld.shared.v2.b64 {%0, %1}, [%2];" : "=l"(lo), "=l"(hi) : "r"(addr));
 }
-// a + c for an `a` that is the result of mul2(): ptxas contracts mul.rn.f32x2 + add.rn.f32x2 into one FFMA2 even under
-// --fmad=false (it does not for the scalar forms), which would round once instead of twice.  a * 1 + c as an explicit
-// fma is the same value as a + c and leaves the product alone.
-__device__ __forceinline__ float2 add2_after_mul(float2 a, float2 c) { return fma2(a, splat(1.0f), c); }
+// a + c for an `a` that is the result of mul2(): the product is rounded on its own, then the sum
+__device__ __forceinline__ float2 add2_after_mul(float2 a, float2 c) { return add2(a, c); }
 
 
 }  // namespace v5

@@ -4,7 +4,7 @@
 // (populate_inputs / run_transforms / read_outputs), state/render_graph.rs, state/{input,node,output}_texture.rs
 // and transformations/layout.rs (LayoutNode::render, resample_scaled_children) + layout/params.rs.
 //
-// B200 design: no per-node textures and no per-pass submits.  Per tick the host flattens every
+// Design: no per-node textures and no per-pass submits.  Per tick the host flattens every
 // output's scene (CPU, as in the reference), packs ALL device-side descriptors of the tick into one
 // pinned arena, ships it with one async copy, and issues a fixed short sequence of launches on one
 // stream: [convert inputs that feed a Lanczos pass] -> [weights for new mappings] -> [box passes] ->
@@ -420,7 +420,7 @@ class Renderer {
     std::deque<int> inflight_;
     int slot_ = 0;
     bool uploaded_ = false;
-    int sm_count_ = 148;
+    int sm_count_ = 132;
     void drain() {
         if (stream_) cudaStreamSynchronize(stream_);
         if (copy_stream_) cudaStreamSynchronize(copy_stream_);
@@ -503,12 +503,20 @@ smr_status Renderer::init() {
     int n = 0;
     cudaError_t e = cudaGetDeviceCount(&n);
     if (e != cudaSuccess || n <= 0) {
-        set_error("no CUDA device: the B200 compositor has no CPU fallback");
+        set_error("no CUDA device: the H100 compositor has no CPU fallback");
         return SMR_ERR_CUDA;
     }
     if (opts_.cuda_device < 0 || opts_.cuda_device >= n) {
         set_error("cuda_device out of range");
         return SMR_ERR_INVALID_ARGUMENT;
+    }
+    int cc_major = 0, cc_minor = 0;
+    CUDA_OK(cudaDeviceGetAttribute(&cc_major, cudaDevAttrComputeCapabilityMajor, opts_.cuda_device));
+    CUDA_OK(cudaDeviceGetAttribute(&cc_minor, cudaDevAttrComputeCapabilityMinor, opts_.cuda_device));
+    if (cc_major != 9 || cc_minor != 0) {  // sm_90a code loads on compute capability 9.0 alone: say so up front
+        set_error("device has compute capability " + std::to_string(cc_major) + "." + std::to_string(cc_minor) +
+                  "; this library is built for sm_90a (H100) only");
+        return SMR_ERR_UNSUPPORTED;
     }
     CUDA_OK(cudaSetDevice(opts_.cuda_device));
     CUDA_OK(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
@@ -2439,7 +2447,7 @@ smr_status smr_host_unregister(void *ptr) {
     return SMR_OK;
 }
 const char *smr_last_error(smr_renderer *r) { return r ? r->impl.last_error() : g_create_error.c_str(); }
-const char *smr_version(void) { return "smelter_b200 0.1 (sm_100a)"; }
+const char *smr_version(void) { return "smelter_b200 0.1 (sm_90a)"; }
 
 smr_status smr_debug_tile_plan(const int32_t *boxes, uint32_t n_layers, uint32_t width, uint32_t height, int32_t sorted,
                                int32_t *owner_layer, uint32_t owner_cap, uint32_t *tiles, uint32_t tiles_cap, uint32_t *n_tiles) {

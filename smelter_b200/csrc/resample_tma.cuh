@@ -1,4 +1,4 @@
-// resample_tma.cuh -- K1/K2 + K8 (horizontal) + K8 (vertical) fused, Blackwell data movement (included by kernels.cu).
+// resample_tma.cuh -- K1/K2 + K8 (horizontal) + K8 (vertical) fused, TMA data movement (included by kernels.cu).
 //
 // Same arithmetic, same quantisation points and the same per-output accumulation order as k_resample_fused_int
 // (resample.wgsl:42-86 twice, planar_yuv_to_rgba.wgsl / nv12_to_rgba.wgsl in front), so the bytes are identical;
@@ -7,8 +7,8 @@
 //   * the strip's source rows arrive by TMA: one elected thread issues cp.async.bulk.tensor.2d copies of a
 //     (272 B x 32 rows) luma box and the matching chroma box per chunk into a double-buffered shared-memory
 //     stage, completion on an mbarrier; the loads of chunk c+1 are in flight while chunk c is converted.  A box may
-//     start at a negative coordinate but only at a 16-byte boundary of the row (anything else raises an illegal
-//     instruction, measured with tools/probe/tma_probe.cu), so the tile starts at the strip's first pixel rounded down
+//     start at a negative coordinate but only at a 16-byte boundary of the row (the TMA unit's alignment rule for
+//     the global address of a box), so the tile starts at the strip's first pixel rounded down
 //     to 16 and every lane realigns its bytes with one funnel shift per word; out-of-image bytes (zero-filled by
 //     the TMA unit) are replaced by the edge texels (resample.wgsl clamps the tap index);
 //   * no shared-memory row buffer and no per-tap LDS in the horizontal pass: lane l owns the 8 consecutive source
@@ -17,13 +17,13 @@
 //     taps: they start in the lane that owns tap 0, take that lane's pixels in tap order, hop to lane + 1 with
 //     SHFL.UP, and so on (4 lanes for the 25 taps of a 4:1 pass) -- a systolic array along the warp.  Every
 //     accumulator still sees its taps in the order t = 0 .. TAPS-1, one fma each, so the sum is bit-identical;
-//   * FP32 pairs: fma/mul/add.f32x2 (FFMA2 / FMUL2 / FADD2 on sm_100) process two pixels (conversion), the r and g
-//     channel of one output, or two output columns per instruction;
+//   * FP32 pairs (fma2 / mul2 / add2, two scalar IEEE operations each on sm_90) hold two pixels (conversion), the
+//     r and g channel of one output, or two output columns;
 //   * integer -> float without the conversion unit: a byte or a 16-bit field is PRMT-ed under the exponent of 2^23
 //     and 2^23 is subtracted (exact); float -> index by adding 1.5 * 2^23 (round-to-nearest-even, exactly
 //     __float2int_rn for |x| < 2^22); the clamp of NC-2 is folded into a decode table that is extended on both sides;
 //   * the horizontal results of a row (f16-quantised, NC-5) go to a ring of rows in shared memory as f32, each lane
-//     into its own slot, and the vertical pass reads them back with LDS.64 / LDS.128 + FFMA2.
+//     into its own slot, and the vertical pass reads them back with LDS.64 / LDS.128 + FMA pairs.
 //
 // Template parameter S in {2, 4}: integer horizontal ratio with zero crop offset (first(o) = S * o + const).
 // SRC: 0 planar 4:2:0, 1 NV12.

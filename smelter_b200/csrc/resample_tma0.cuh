@@ -4,7 +4,7 @@
 // margins, transitions), ratio 3, crops.  Everything up to the decoded pixels is k_resample_tma3 (TMA tiles, packed FP32
 // K1/K2, lane-replicated decode table); the horizontal pass cannot be systolic here -- every output column has its own
 // weights and window -- so each warp parks the decoded row in a shared-memory row buffer and every lane runs the union
-// window of its two adjacent output columns out of it, one LDS.128 per source pixel feeding three FFMA2, with the
+// window of its two adjacent output columns out of it, one LDS.128 per source pixel feeding six FFMA, with the
 // lane's weights held in registers for the whole strip (54 of the 128 registers of this kernel: two 8-warp groups per
 // SM).  Strips are at most 64 columns and are narrowed by the host so that a strip's source span fits the 256 pixels
 // a warp converts per row.  The vertical pass is the general one (per-row weights from global memory).
@@ -424,7 +424,7 @@ __global__ void __launch_bounds__(32 * kWarps * kGroups, 1) k_resample_tma0(cons
                 // A2: horizontal Lanczos, two adjacent output columns per lane.  The lane's weights live in registers for
                 // the whole piece: wq[j] = (weight of column 2 lane, weight of column 2 lane + 1 shifted by the distance of the
                 // two windows), zeros outside -- one LDS.128 per source pixel (r, g, b, b) of the union window feeds four FFMA
-                // and one FFMA2 (the weight pair is the packed operand as it stands; a splat pair per weight would not fit the
+                // and one FMA pair (the weight pair is the packed operand as it stands; a splat pair per weight would not fit the
                 // register file); the nonzero taps of a column are taken in the shader's order t = 0 .. taps-1, a zero tap
                 // leaves the sum alone
                 {

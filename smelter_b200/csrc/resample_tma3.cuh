@@ -5,7 +5,7 @@
 //     mbarriers, own ring, own list of pieces -- each group is what a block of k_resample_tma was), so that the
 //     sRGB decode table can be shared by all of them and REPLICATED per lane: entry i of lane l sits at word
 //     32 i + l, i.e. in bank l, and the 24 data-dependent lookups of a row never conflict (they were 3-way on average,
-//     44 % of the shared-memory wavefronts of k_resample_tma; profiles/r02_*).  The table has exactly 256 entries, so
+//     a large share of the shared-memory wavefronts of k_resample_tma).  The table has exactly 256 entries, so
 //     the clamp of NC-2 moves back in front of the rounding as the .SAT of the matrix row's last fma;
 //   * ONE 32-row TMA stage per group (a whole 8-output-row step of a 4:1 pass): it is refilled right after the
 //     horizontal pass has consumed it, i.e. while the vertical pass runs; three groups' stages + rings fit in 227 KB;
@@ -416,7 +416,7 @@ __global__ void __launch_bounds__(32 * kWarps * kGroups, 1) k_resample_tma3(cons
         // loads refill the stage while the vertical pass runs
         group_sync(grp);
         if (tid == 0) issue(parked->nxt);
-#ifdef SMR_EXP_NO_B      // what-if build (tools/exp_variants.sh): no vertical pass -- measures what phase B costs; output is garbage
+#ifdef SMR_EXP_NO_B      // what-if build (-DSMR_EXP_NO_B): no vertical pass -- measures what phase B costs; output is garbage
         if (false) {
 #else
         if (cur.last) {

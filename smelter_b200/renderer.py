@@ -4,7 +4,7 @@ Names, argument meaning and error behaviour follow `smelter_render::Renderer`
 (smelter-render/src/state.rs:95-193), `scene::Component` (scene/components.rs) and
 `Frame/FrameData/FrameSet` (types.rs:21-119) so the parity tests read like the reference's render tests
 (integration-tests/src/render_tests/harness/test_case.rs).  Nothing here computes pixels: every call
-goes to libsmelter_b200.so (hand-written sm_100a kernels).
+goes to libsmelter_b200.so (hand-written sm_90a kernels).
 """
 import ctypes as C
 from dataclasses import dataclass, field

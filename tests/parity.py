@@ -1,4 +1,4 @@
-"""Shared parity harness: run a scene through the product (C ABI -> sm_100a kernels) and through the
+"""Shared parity harness: run a scene through the product (C ABI -> sm_90a kernels) and through the
 CPU oracle on the same inputs, return both outputs.  Test infrastructure (imports oracle/)."""
 import numpy as np
 

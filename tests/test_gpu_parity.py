@@ -1,7 +1,7 @@
 """Parity tests proper: the CUDA path (through the C ABI) against the CPU oracle, BIT-EXACT on every
 output byte, on scenes re-typed from the reference's render tests
 (integration-tests/src/render_tests/{simple,tiles,view,rescaler,transition}.rs) with the reference's
-procedural inputs (harness/input.rs).  Run with `-m gpu` on a B200."""
+procedural inputs (harness/input.rs).  Run with `-m gpu` on an H100."""
 import numpy as np
 import pytest
 

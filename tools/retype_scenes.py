@@ -2,11 +2,11 @@
 """Re-types the reference's render-test scene catalogue as Python (tests/golden/ref_scenes.py).
 
 Reads integration-tests/src/render_tests/{simple,view,rescaler,tiles,transition,tiles_transitions}.rs of the
-reference checkout (this container only) and translates the small Rust subset those files use -- struct literals with
+reference checkout given on the command line and translates the small Rust subset those files use -- struct literals with
 `..Default::default()`, enum variants, vec!, Some/None, closures, helper functions, format! -- into Python source
 that builds the same scenes through tests/ref_scene_rt.py.  The output is committed; tests never read the reference.
 
-  python tools/retype_scenes.py [/root/reference] > tests/golden/ref_scenes.py
+  python tools/retype_scenes.py REFERENCE_CHECKOUT > tests/golden/ref_scenes.py
 """
 import os
 import re
@@ -400,7 +400,9 @@ class P:
 
 
 def main():
-    ref = sys.argv[1] if len(sys.argv) > 1 else "/root/reference"
+    if len(sys.argv) != 2:
+        raise SystemExit("usage: retype_scenes.py REFERENCE_CHECKOUT > tests/golden/ref_scenes.py")
+    ref = sys.argv[1]
     base = os.path.join(ref, "integration-tests", "src", "render_tests")
     print('"""GENERATED by tools/retype_scenes.py from the reference\'s render tests (integration-tests/src/render_tests/')
     print('{' + ",".join(FILES) + '}.rs): the scene catalogue re-typed as Python.  Do not edit by hand."""')
