@@ -4,7 +4,7 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# SMR_LIB_PATH: a differently built copy of the same library (what-if builds with -DSMR_EXP_* switches)
+# SMR_LIB_PATH: a differently built copy of the same library (e.g. another revision's build, for an A/B comparison)
 LIB_PATH = os.environ.get("SMR_LIB_PATH") or os.path.join(_HERE, "libsmelter_b200.so")
 
 SMR_OK = 0

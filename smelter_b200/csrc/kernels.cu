@@ -884,7 +884,7 @@ __device__ __forceinline__ float to_v(float r, float g, float b) {
 // very operations of the composite's fused output stage: Y per pixel from the raw bytes, chroma from the exact mean of
 // the four bytes (NC-6u at the .5 / .5 taps of an even-sized target).  (X, Y) even: frame position of the block.
 __device__ __forceinline__ void emit_yuv_2x2(const FusedJob &J, int X, int Y, uint32_t p00, uint32_t p10, uint32_t p01, uint32_t p11) {
-    using namespace v5;
+    using namespace tma;
     // The arithmetic of the composite's output stage, operation for operation, two values per instruction (packed FP32) and
     // without the conversion unit (I2F / F2I run at a fraction of the FP32 rate): a byte or 16-bit field goes under the
     // exponent of 2^23 by PRMT and 2^23 is subtracted (exact); the UNORM8 store rounds by the magic add (== __float2int_rn
@@ -940,11 +940,11 @@ static bool launch_tma0(const FusedJob *jobs_dev, const FusedPiece *pieces, cons
     cudaGetDevice(&dev);
     const unsigned long long bit = 1ull << (dev & 63);
     if (!(done.load(std::memory_order_acquire) & bit)) {
-        cudaFuncSetAttribute(v7::k_resample_tma0<SRC, WINP, BOX>, cudaFuncAttributeMaxDynamicSharedMemorySize, v7::Cfg::SMEM);
+        cudaFuncSetAttribute(tma_any::k_resample_tma0<SRC, WINP, BOX>, cudaFuncAttributeMaxDynamicSharedMemorySize, tma_any::Cfg::SMEM);
         done.fetch_or(bit, std::memory_order_release);
     }
-    const int grid = (nblocks + v7::kGroups - 1) / v7::kGroups;
-    v7::k_resample_tma0<SRC, WINP, BOX><<<grid, dim3(32, v7::kWarps * v7::kGroups), v7::Cfg::SMEM, s>>>(jobs_dev, pieces, piece_begin, nblocks);
+    const int grid = (nblocks + tma_any::kGroups - 1) / tma_any::kGroups;
+    tma_any::k_resample_tma0<SRC, WINP, BOX><<<grid, dim3(32, tma::kWarps * tma_any::kGroups), tma_any::Cfg::SMEM, s>>>(jobs_dev, pieces, piece_begin, nblocks);
     return check_launch("k_resample_tma0");
 }
 
@@ -955,26 +955,12 @@ static bool launch_tma3(const FusedJob *jobs_dev, const FusedPiece *pieces, cons
     cudaGetDevice(&dev);
     const unsigned long long bit = 1ull << (dev & 63);
     if (!(done.load(std::memory_order_acquire) & bit)) {
-        cudaFuncSetAttribute(v6::k_resample_tma3<S, SRC>, cudaFuncAttributeMaxDynamicSharedMemorySize, v6::Cfg<S>::SMEM);
+        cudaFuncSetAttribute(tma_int::k_resample_tma3<S, SRC>, cudaFuncAttributeMaxDynamicSharedMemorySize, tma_int::Cfg<S>::SMEM);
         done.fetch_or(bit, std::memory_order_release);
     }
-    const int grid = (nblocks + v6::kGroups - 1) / v6::kGroups;   // the host cut the work for `nblocks` eight-warp groups
-    v6::k_resample_tma3<S, SRC><<<grid, dim3(32, v6::kWarps * v6::kGroups), v6::Cfg<S>::SMEM, s>>>(jobs_dev, pieces, piece_begin, nblocks);
+    const int grid = (nblocks + tma_int::kGroups - 1) / tma_int::kGroups;   // the host cut the work for `nblocks` eight-warp groups
+    tma_int::k_resample_tma3<S, SRC><<<grid, dim3(32, tma::kWarps * tma_int::kGroups), tma_int::Cfg<S>::SMEM, s>>>(jobs_dev, pieces, piece_begin, nblocks);
     return check_launch("k_resample_tma3");
-}
-
-template <int S, int SRC>
-static bool launch_tma(const FusedJob *jobs_dev, const FusedPiece *pieces, const int *piece_begin, int nblocks, cudaStream_t s) {
-    static std::atomic<unsigned long long> done{0};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    const unsigned long long bit = 1ull << (dev & 63);
-    if (!(done.load(std::memory_order_acquire) & bit)) {
-        cudaFuncSetAttribute(v5::k_resample_tma<S, SRC>, cudaFuncAttributeMaxDynamicSharedMemorySize, v5::Cfg<S>::SMEM);
-        done.fetch_or(bit, std::memory_order_release);
-    }
-    v5::k_resample_tma<S, SRC><<<nblocks, dim3(32, v5::kWarps), v5::Cfg<S>::SMEM, s>>>(jobs_dev, pieces, piece_begin);
-    return check_launch("k_resample_tma");
 }
 
 // src: 0 planar 4:2:0, 1 NV12, 2 UYVY, 3 YUYV (fused_source_class)
@@ -983,13 +969,12 @@ int launch_resample_fused(int variant, int src, const FusedJob *jobs_dev, const 
     if (nblocks <= 0) return 0;
     cudaStream_t st = (cudaStream_t)s;
     bool ok = false;
-    static_assert(v5::Cfg<4>::NOUT == kTmaStripCols4 && v5::Cfg<2>::NOUT == kTmaStripCols2, "strip widths");
-    static_assert(v6::Cfg<4>::NOUT == kTmaStripCols4 && v6::Cfg<2>::NOUT == kTmaStripCols2 && v6::Cfg<4>::RROWS == kTmaRing4 &&
-                  v6::Cfg<2>::RROWS == kTmaRing2 && v6::kChunkRows == kTma3LumaBoxH && v6::kChromaRows == kTma3ChromaBoxH, "grouped kernel");
-    static_assert(v5::Cfg<4>::RROWS == kTmaRing4 && v5::Cfg<2>::RROWS == kTmaRing2, "ring rows");
-    static_assert(v7::kGroups == kTma0Groups && v7::Cfg::MAXT == kTma0MaxTaps && v7::Cfg::WINP_MAX == kTma0Window[3] && v7::Cfg::RROWS == kTmaRing4 && v7::kChunkRows == kTma3LumaBoxH, "any-ratio kernel");
-    static_assert(v5::kLumaBox == 2 * kTmaLumaBoxW && v5::kChunkRows == kTmaLumaBoxH && v5::kNv12Box == 2 * kTmaNv12BoxW &&
-                  v5::kPlanarBox == kTmaPlanarBoxW && v5::kChromaRows == kTmaChromaBoxH, "TMA boxes");
+    static_assert(tma_int::Cfg<4>::NOUT == kTmaStripCols4 && tma_int::Cfg<2>::NOUT == kTmaStripCols2 &&
+                  tma_int::Cfg<4>::RROWS == kTmaRing4 && tma_int::Cfg<2>::RROWS == kTmaRing2, "integer-ratio kernel");
+    static_assert(tma_any::kGroups == kTma0Groups && tma_any::Cfg::MAXT == kTma0MaxTaps && tma_any::Cfg::WINP_MAX == kTma0Window[3] &&
+                  tma_any::Cfg::RROWS == kTmaRing4, "any-ratio kernel");
+    static_assert(tma::kLumaBox == 2 * kTmaLumaBoxW && tma::kChunkRows == kTmaLumaBoxH && tma::kNv12Box == 2 * kTmaNv12BoxW &&
+                  tma::kPlanarBox == kTmaPlanarBoxW && tma::kChromaRows == kTmaChromaBoxH, "TMA boxes");
     switch (variant) {
 #define SMR_TMA0_CASE(B) \
         case 30 + B: ok = src == 1 ? launch_tma0<1, kTma0Window[B], 0>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, st) \
@@ -1002,10 +987,6 @@ int launch_resample_fused(int variant, int src, const FusedJob *jobs_dev, const 
                                : launch_tma3<2, 0>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
         case 24: ok = src == 1 ? launch_tma3<4, 1>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, st)
                                : launch_tma3<4, 0>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
-        case 12: ok = src == 1 ? launch_tma<2, 1>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, st)
-                               : launch_tma<2, 0>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
-        case 14: ok = src == 1 ? launch_tma<4, 1>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, st)
-                               : launch_tma<4, 0>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
         case 2: ok = launch_fused_src<2>(src, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
         case 3: ok = launch_fused_src<3>(src, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
         case 4: ok = launch_fused_src<4>(src, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
@@ -1016,12 +997,21 @@ int launch_resample_fused(int variant, int src, const FusedJob *jobs_dev, const 
 
 // ------------------------------------------------------------------------------------------------
 // FAST_HALF: K1/K2 of one source row of an aligned 8-pixel run (x0 even, interior: 2 <= x0, x0 + 9 <= W - 1, chroma rows
-// inside), packed FP32 as in resample_tma.cuh; the bytes of pixels (2i, 2i + 1) are ADDED to sums[i][c].  The result of
-// yuv_to_rgba8() bit for bit (same operations, two pixels per instruction).
+// inside), the conversion of the TMA-staged kernels (tma::convert_pair); the bytes of pixels (2i, 2i + 1) are ADDED to
+// sums[i][c].  The result of yuv_to_rgba8() bit for bit (same operations, two pixels per instruction).
 // ------------------------------------------------------------------------------------------------
 // one source row: yw = its 8 luma bytes, v[k] = 3 * heavy + light chroma texel cx - 1 + k (u in bits 0..15, v in 16..31)
 __device__ __forceinline__ void half_row_convert(const uint32_t (&yw)[2], const uint32_t (&v)[6], float nk16, float rcp_y, float rcp_c,
-                                                 int (&sums)[4][3]);
+                                                 int (&sums)[4][3]) {
+#pragma unroll
+    for (int p = 0; p < 4; p++) {
+        float2 qr, qg, qb;
+        tma::convert_pair(yw, v, p, nk16, rcp_y, rcp_c, qr, qg, qb);
+        sums[p][0] += (int)(__float_as_uint(qr.x) & 0xffu) + (int)(__float_as_uint(qr.y) & 0xffu);
+        sums[p][1] += (int)(__float_as_uint(qg.x) & 0xffu) + (int)(__float_as_uint(qg.y) & 0xffu);
+        sums[p][2] += (int)(__float_as_uint(qb.x) & 0xffu) + (int)(__float_as_uint(qb.y) & 0xffu);
+    }
+}
 
 template <bool NV12>
 __device__ __forceinline__ void half_row_sums(const Tex &S, int x0, int r, float nk16, float rcp_y, float rcp_c, int (&sums)[4][3]) {
@@ -1067,41 +1057,6 @@ __device__ __forceinline__ void half_pair_sums_nv12(const Tex &S, int x0, int r,
         const uint32_t *yrow = reinterpret_cast<const uint32_t *>(S.p0 + (size_t)(r + half) * S.pitch0 + x0);
         const uint32_t yw[2] = {__ldg(yrow), __ldg(yrow + 1)};
         half_row_convert(yw, v, nk16, rcp_y, rcp_c, sums);
-    }
-}
-
-__device__ __forceinline__ void half_row_convert(const uint32_t (&yw)[2], const uint32_t (&v)[6], float nk16, float rcp_y, float rcp_c,
-                                                 int (&sums)[4][3]) {
-#pragma unroll
-    for (int p = 0; p < 4; p++) {
-        const uint32_t ne = v[p] + 3u * v[p + 1], no = 3u * v[p + 1] + v[p + 2];
-        const float m23 = -8388608.0f;
-        float2 nu = v5::add2(make_float2(__uint_as_float(__byte_perm(ne, 0x4B000000u, 0x7610)), __uint_as_float(__byte_perm(no, 0x4B000000u, 0x7610))), v5::splat(m23));
-        float2 nv = v5::add2(make_float2(__uint_as_float(__byte_perm(ne, 0x4B000000u, 0x7632)), __uint_as_float(__byte_perm(no, 0x4B000000u, 0x7632))), v5::splat(m23));
-        const uint32_t ywd = yw[p >> 1];
-        float2 ny = v5::add2(make_float2(__uint_as_float(__byte_perm(ywd, 0x4B000000u, (p & 1) ? 0x7642 : 0x7640)),
-                                         __uint_as_float(__byte_perm(ywd, 0x4B000000u, (p & 1) ? 0x7643 : 0x7641))), v5::splat(m23));
-        const float c1 = __uint_as_float(0x3b808081u), lo1 = __uint_as_float(0xaf7efeffu);
-        const float c16 = __uint_as_float(0x39808081u), lo16 = __uint_as_float(0xad7efeffu);
-        float2 y = v5::fma2(ny, v5::splat(c1), v5::mul2(ny, v5::splat(lo1)));
-        float2 u = v5::fma2(nu, v5::splat(c16), v5::mul2(nu, v5::splat(lo16)));
-        float2 w = v5::fma2(nv, v5::splat(c16), v5::mul2(nv, v5::splat(lo16)));
-        y = v5::add2(y, v5::splat(nk16)); u = v5::add2(u, v5::splat(nk16)); w = v5::add2(w, v5::splat(nk16));
-        y = make_float2(__saturatef(y.x * rcp_y), __saturatef(y.y * rcp_y));
-        u = make_float2(__saturatef(u.x * rcp_c), __saturatef(u.y * rcp_c));
-        w = make_float2(__saturatef(w.x * rcp_c), __saturatef(w.y * rcp_c));
-        const float2 um = v5::add2(u, v5::splat(-0.5f)), vm = v5::add2(w, v5::splat(-0.5f));
-        const float2 gi = v5::fma2(v5::splat(-0.1873f), um, y);
-        const float2 rr = make_float2(__saturatef(fmaf(1.5748f, vm.x, y.x)), __saturatef(fmaf(1.5748f, vm.y, y.y)));
-        const float2 gg = make_float2(__saturatef(fmaf(-0.4681f, vm.x, gi.x)), __saturatef(fmaf(-0.4681f, vm.y, gi.y)));
-        const float2 bb = make_float2(__saturatef(fmaf(1.8556f, um.x, y.x)), __saturatef(fmaf(1.8556f, um.y, y.y)));
-        const float magic = 12582912.0f;   // 1.5 * 2^23: the add rounds to the nearest-even integer (NC-2)
-        const float2 qr = v5::add2_after_mul(v5::mul2(rr, v5::splat(255.0f)), v5::splat(magic));
-        const float2 qg = v5::add2_after_mul(v5::mul2(gg, v5::splat(255.0f)), v5::splat(magic));
-        const float2 qb = v5::add2_after_mul(v5::mul2(bb, v5::splat(255.0f)), v5::splat(magic));
-        sums[p][0] += (int)(__float_as_uint(qr.x) & 0xffu) + (int)(__float_as_uint(qr.y) & 0xffu);
-        sums[p][1] += (int)(__float_as_uint(qg.x) & 0xffu) + (int)(__float_as_uint(qg.y) & 0xffu);
-        sums[p][2] += (int)(__float_as_uint(qb.x) & 0xffu) + (int)(__float_as_uint(qb.y) & 0xffu);
     }
 }
 

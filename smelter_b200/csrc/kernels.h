@@ -133,10 +133,9 @@ struct FusedJob {
     const float *w_v, *inv_v;
     const int32_t *first_v;
     int32_t variant;        // 0: any ratio (weights from smem); 2,3,4: integer horizontal ratio (constant-bank weights);
-                            // 12, 14: integer ratio 2 / 4 on the TMA-staged kernel (k_resample_tma, resample_tma.cuh);
-                            // 22, 24: the same on its one-block-per-SM form (k_resample_tma3, resample_tma3.cuh);
+                            // 22, 24: integer ratio 2 / 4 on the TMA-staged kernel (k_resample_tma3, resample_tma3.cuh);
                             // 30 + b: any ratio <= 4 on the TMA-staged kernel (k_resample_tma0, resample_tma0.cuh) with a
-                            //         tap loop of kTma0Window[b] slots
+                            //         tap loop of kTma0Window[b] slots; 40 + b: the same on a source box-reduced 2:1
     // TMA variants: device copies of the CUtensorMap of each source plane (luma; NV12 chroma as u16 texels, or U; V)
     const void *tm0, *tm1, *tm2;
     int32_t v_same;         // TMA variants: the vertical mapping is the same integer ratio with zero offset (weights = c_wint[S])
@@ -166,10 +165,9 @@ constexpr int kFusedStripCols = 64, kFusedWarps = 8, kFusedRing = 64, kFusedSpan
 constexpr int kTmaStripCols4 = 58, kTmaStripCols2 = 122, kTmaRing4 = 54, kTmaRing2 = 28;
 // luma and NV12 chroma are addressed in 2-byte elements (a box may be at most 256 elements wide), planar chroma in bytes
 constexpr int kTmaLumaBoxW = 136, kTmaLumaBoxH = 32, kTmaNv12BoxW = 144, kTmaPlanarBoxW = 160, kTmaChromaBoxH = 18;
-constexpr int kTma3LumaBoxH = 32, kTma3ChromaBoxH = 18;   // the grouped kernel (resample_tma3.cuh, variants 22 / 24)
 constexpr int kTma0Groups = 2, kTma0MaxSpan = 256, kTma0MaxTaps = 25;
 constexpr int kTma0Window[4] = {20, 25, 29, 33};
-inline int fused_strip_cols(int variant) { return (variant % 10 == 4 && variant > 10) ? kTmaStripCols4 : (variant % 10 == 2 && variant > 10) ? kTmaStripCols2 : kFusedStripCols; }
+inline int fused_strip_cols(int variant) { return variant == 24 ? kTmaStripCols4 : variant == 22 ? kTmaStripCols2 : kFusedStripCols; }
 
 struct WeightJob {          // resample.wgsl:42-86 evaluated once per output coordinate
     float scale, offset;

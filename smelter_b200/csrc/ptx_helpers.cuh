@@ -2,7 +2,7 @@
 // volatile shared-memory loads of TMA stages, and FP32 pair helpers.
 #pragma once
 
-namespace v5 {
+namespace tma {
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -87,4 +87,4 @@ __device__ __forceinline__ void lds128q(uint32_t addr, unsigned long long &lo, u
 __device__ __forceinline__ float2 add2_after_mul(float2 a, float2 c) { return add2(a, c); }
 
 
-}  // namespace v5
+}  // namespace tma

@@ -215,7 +215,7 @@ static bool nccl_load(std::string &err) {
     return true;
 }
 
-// TMA descriptors of the input planes (k_resample_tma): cuTensorMapEncodeTiled through the runtime's driver entry
+// TMA descriptors of the input planes (k_resample_tma3 / k_resample_tma0): cuTensorMapEncodeTiled through the runtime's driver entry
 // point, so libcuda is not a link-time dependency.  2-D, no swizzle, zero fill outside the plane.
 typedef CUresult (*tmap_encode_fn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
                                    const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -385,7 +385,6 @@ class Renderer {
     bool direct_k11_ = true;                   // SMR_DIRECT_K11=0: A/B switch, every tile goes through the composite
     bool tile_sort_ = true;                    // SMR_TILE_SORT=0: the compacted composite launch keeps row-major order
     bool disable_tma_ = false;                 // SMR_DISABLE_TMA=1: A/B switch back to the LDG-staged kernels
-    bool tma_grouped_ = true;                  // SMR_TMA_GROUPED=0: the three-blocks-per-SM form of the TMA kernel
     std::vector<dev::FusedJob> fused_jobs_;
     std::vector<std::pair<int, size_t>> fused_src_dst_;   // (raw tex index, frame offset of dst)
     std::vector<dev::WeightJob> weight_jobs_;
@@ -499,7 +498,6 @@ smr_status Renderer::init() {
     if (const char *e = getenv("SMR_DISABLE_TMA")) disable_tma_ = e[0] == '1';
     if (const char *e = getenv("SMR_DIRECT_K11")) direct_k11_ = e[0] != '0';
     if (const char *e = getenv("SMR_TILE_SORT")) tile_sort_ = e[0] != '0';
-    if (const char *e = getenv("SMR_TMA_GROUPED")) tma_grouped_ = e[0] != '0';
     int n = 0;
     cudaError_t e = cudaGetDeviceCount(&n);
     if (e != cudaSuccess || n <= 0) {
@@ -786,7 +784,7 @@ int Renderer::try_fused_resample(Input &in, const AxisMapping &hm_in, const Axis
     const int lv_h = hm_in.predecimate_levels(), lv_v = vm_in.predecimate_levels();
     const bool box = lv_h == 1 && lv_v == 1;
     if (!box && (lv_h != 0 || lv_v != 0)) return -1;
-    if (box && (disable_tma_ || !tma_grouped_ || src_class >= 2 || (dw & 1))) return -1;
+    if (box && (disable_tma_ || src_class >= 2 || (dw & 1))) return -1;
     const AxisMapping hm = box ? hm_in.on_reduced_source(1) : hm_in, vm = box ? vm_in.on_reduced_source(1) : vm_in;
     KernelPass passes[2];
     if (plan_passes(hm, vm, passes) != 2 || passes[0].mapping.axis != 0) return -1;
@@ -827,20 +825,19 @@ int Renderer::try_fused_resample(Input &in, const AxisMapping &hm_in, const Axis
             (int)std::ceil((dev::kFusedWarps - 1) * sv) + tv + 1 <= ring) {
             CUtensorMap m[3];
             memset(m, 0, sizeof(m));
-            const int gk = tma_grouped_ ? 4 : 0;
-            bool ok = plane_tmap(t.p0, t.pitch0, t.width, t.height, 0 | gk, &m[0]);
-            if (src_class == 1) ok = ok && plane_tmap(t.p1, t.pitch1, t.width / 2, t.height / 2, 1 | gk, &m[1]);
-            else ok = ok && plane_tmap(t.p1, t.pitch1, t.width / 2, t.height / 2, 2 | gk, &m[1]) &&
-                      plane_tmap(t.p2, t.pitch2, t.width / 2, t.height / 2, 2 | gk, &m[2]);
+            bool ok = plane_tmap(t.p0, t.pitch0, t.width, t.height, 0, &m[0]);
+            if (src_class == 1) ok = ok && plane_tmap(t.p1, t.pitch1, t.width / 2, t.height / 2, 1, &m[1]);
+            else ok = ok && plane_tmap(t.p1, t.pitch1, t.width / 2, t.height / 2, 2, &m[1]) &&
+                      plane_tmap(t.p2, t.pitch2, t.width / 2, t.height / 2, 2, &m[2]);
             if (ok) {
                 tmap_idx = (int)tick_tmaps_.size();
                 tick_tmaps_.insert(tick_tmaps_.end(), m, m + 3);
                 j.v_same = vm.crop_offset == 0.0f && sv == sh && tv == th;
-                j.variant += tma_grouped_ ? 20 : 10;
+                j.variant += 20;
             }
         }
     }
-    if (j.variant < 10 && !disable_tma_ && tma_grouped_ && src_class < 2 && (dw & 1) == 0 && th <= dev::kTma0MaxTaps &&
+    if (j.variant < 10 && !disable_tma_ && src_class < 2 && (dw & 1) == 0 && th <= dev::kTma0MaxTaps &&
         (int)std::ceil((dev::kFusedWarps - 1) * sv) + tv + 1 <= dev::kTmaRing4) {
         // any other ratio <= 4 (fractional, 3, with a crop offset): the any-ratio TMA kernel; its strips are narrowed so that
         // a strip's source span fits the 256 pixels a warp converts per row
@@ -857,10 +854,10 @@ int Renderer::try_fused_resample(Input &in, const AxisMapping &hm_in, const Axis
         CUtensorMap m[3];
         memset(m, 0, sizeof(m));
         bool ok = bucket < 4 && (int)std::ceil((cols - 1) * sh) + th + 3 <= max_span &&
-                  plane_tmap(t.p0, t.pitch0, t.width, t.height, 4, &m[0]);
-        if (ok && src_class == 1) ok = plane_tmap(t.p1, t.pitch1, t.width / 2, t.height / 2, 1 | 4, &m[1]);
-        else if (ok) ok = plane_tmap(t.p1, t.pitch1, t.width / 2, t.height / 2, 2 | 4, &m[1]) &&
-                          plane_tmap(t.p2, t.pitch2, t.width / 2, t.height / 2, 2 | 4, &m[2]);
+                  plane_tmap(t.p0, t.pitch0, t.width, t.height, 0, &m[0]);
+        if (ok && src_class == 1) ok = plane_tmap(t.p1, t.pitch1, t.width / 2, t.height / 2, 1, &m[1]);
+        else if (ok) ok = plane_tmap(t.p1, t.pitch1, t.width / 2, t.height / 2, 2, &m[1]) &&
+                          plane_tmap(t.p2, t.pitch2, t.width / 2, t.height / 2, 2, &m[2]);
         if (ok) {
             tmap_idx = (int)tick_tmaps_.size();
             tick_tmaps_.insert(tick_tmaps_.end(), m, m + 3);
@@ -935,11 +932,10 @@ bool Renderer::plane_tmap(const uint8_t *p, int pitch, int w, int h, int kind, C
     TmapKey key{(uintptr_t)p, pitch, w, h, kind};
     auto it = tmap_cache_.find(key);
     if (it != tmap_cache_.end()) { *out = it->second; return true; }
-    // kind: 0 luma, 1 NV12 chroma, 2 planar chroma; + 4 for the 16-row chunks of the grouped kernel
-    const int lh = (kind & 4) ? dev::kTma3LumaBoxH : dev::kTmaLumaBoxH, chh = (kind & 4) ? dev::kTma3ChromaBoxH : dev::kTmaChromaBoxH;
-    bool ok = (kind & 3) == 0   ? encode_plane_tmap(p, pitch, w / 2, h, 2, dev::kTmaLumaBoxW, lh, out)
-              : (kind & 3) == 1 ? encode_plane_tmap(p, pitch, w, h, 2, dev::kTmaNv12BoxW, chh, out)
-                                : encode_plane_tmap(p, pitch, w, h, 1, dev::kTmaPlanarBoxW, chh, out);
+    // kind: 0 luma, 1 NV12 chroma, 2 planar chroma
+    bool ok = kind == 0   ? encode_plane_tmap(p, pitch, w / 2, h, 2, dev::kTmaLumaBoxW, dev::kTmaLumaBoxH, out)
+              : kind == 1 ? encode_plane_tmap(p, pitch, w, h, 2, dev::kTmaNv12BoxW, dev::kTmaChromaBoxH, out)
+                          : encode_plane_tmap(p, pitch, w, h, 1, dev::kTmaPlanarBoxW, dev::kTmaChromaBoxH, out);
     if (!ok) return false;
     if (tmap_cache_.size() > 2048) tmap_cache_.clear();
     tmap_cache_[key] = *out;
