@@ -4,7 +4,8 @@
 //   k_convert     planar_yuv_to_rgba.wgsl / nv12_to_rgba.wgsl / bgra / argb           (K1,K2,K4)
 //   k_weights     the per-output-coordinate part of resample.wgsl:42-86               (K8 setup)
 //   k_resample    resample.wgsl (Lanczos3 pass) and downsample.wgsl (box pass)         (K7,K8)
-//   k_composite   apply_layouts.wgsl: every layout of an output in ONE launch, painter's order kept per
+//   k_composite_p / k_composite_multi
+//                 apply_layouts.wgsl: every layout of every output in ONE launch, painter's order kept per
 //                 pixel in registers, fixed-function sRGB blend emulated per layer, fused with
 //                 rgba_to_yuv.wgsl / rgba_to_nv12.wgsl on the way out                   (K9,K10,K11)
 //   k_output      rgba_to_yuv / rgba_to_nv12 stand-alone (root size != output size, odd sizes)
@@ -948,6 +949,15 @@ static bool launch_tma0(const FusedJob *jobs_dev, const FusedPiece *pieces, cons
     return check_launch("k_resample_tma0");
 }
 
+template <int WINP>
+static bool launch_tma0_src(int src, int box, const FusedJob *jobs_dev, const FusedPiece *pieces, const int *piece_begin, int nblocks,
+                            cudaStream_t s) {
+    if (box) return src == 1 ? launch_tma0<1, WINP, 1>(jobs_dev, pieces, piece_begin, nblocks, s)
+                             : launch_tma0<0, WINP, 1>(jobs_dev, pieces, piece_begin, nblocks, s);
+    return src == 1 ? launch_tma0<1, WINP, 0>(jobs_dev, pieces, piece_begin, nblocks, s)
+                    : launch_tma0<0, WINP, 0>(jobs_dev, pieces, piece_begin, nblocks, s);
+}
+
 template <int S, int SRC>
 static bool launch_tma3(const FusedJob *jobs_dev, const FusedPiece *pieces, const int *piece_begin, int nblocks, cudaStream_t s) {
     static std::atomic<unsigned long long> done{0};
@@ -964,7 +974,7 @@ static bool launch_tma3(const FusedJob *jobs_dev, const FusedPiece *pieces, cons
 }
 
 // src: 0 planar 4:2:0, 1 NV12, 2 UYVY, 3 YUYV (fused_source_class)
-int launch_resample_fused(int variant, int src, const FusedJob *jobs_dev, const FusedPiece *pieces_dev,
+int launch_resample_fused(const FusedKernel &k, int src, const FusedJob *jobs_dev, const FusedPiece *pieces_dev,
                           const int *piece_begin_dev, int nblocks, Stream s) {
     if (nblocks <= 0) return 0;
     cudaStream_t st = (cudaStream_t)s;
@@ -975,22 +985,28 @@ int launch_resample_fused(int variant, int src, const FusedJob *jobs_dev, const 
                   tma_any::Cfg::RROWS == kTmaRing4, "any-ratio kernel");
     static_assert(tma::kLumaBox == 2 * kTmaLumaBoxW && tma::kChunkRows == kTmaLumaBoxH && tma::kNv12Box == 2 * kTmaNv12BoxW &&
                   tma::kPlanarBox == kTmaPlanarBoxW && tma::kChromaRows == kTmaChromaBoxH, "TMA boxes");
-    switch (variant) {
-#define SMR_TMA0_CASE(B) \
-        case 30 + B: ok = src == 1 ? launch_tma0<1, kTma0Window[B], 0>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, st) \
-                                   : launch_tma0<0, kTma0Window[B], 0>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break; \
-        case 40 + B: ok = src == 1 ? launch_tma0<1, kTma0Window[B], 1>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, st) \
-                                   : launch_tma0<0, kTma0Window[B], 1>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
-        SMR_TMA0_CASE(0) SMR_TMA0_CASE(1) SMR_TMA0_CASE(2) SMR_TMA0_CASE(3)
-#undef SMR_TMA0_CASE
-        case 22: ok = src == 1 ? launch_tma3<2, 1>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, st)
-                               : launch_tma3<2, 0>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
-        case 24: ok = src == 1 ? launch_tma3<4, 1>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, st)
-                               : launch_tma3<4, 0>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
-        case 2: ok = launch_fused_src<2>(src, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
-        case 3: ok = launch_fused_src<3>(src, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
-        case 4: ok = launch_fused_src<4>(src, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
-        default: ok = launch_fused_src<0>(src, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
+    switch (k.kind) {
+        case FusedKernel::TMA_ANY:
+            switch (k.window) {
+                case 0: ok = launch_tma0_src<kTma0Window[0]>(src, k.box, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
+                case 1: ok = launch_tma0_src<kTma0Window[1]>(src, k.box, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
+                case 2: ok = launch_tma0_src<kTma0Window[2]>(src, k.box, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
+                default: ok = launch_tma0_src<kTma0Window[3]>(src, k.box, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
+            }
+            break;
+        case FusedKernel::TMA_INT:
+            if (k.ratio == 4) ok = src == 1 ? launch_tma3<4, 1>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, st)
+                                            : launch_tma3<4, 0>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, st);
+            else ok = src == 1 ? launch_tma3<2, 1>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, st)
+                               : launch_tma3<2, 0>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, st);
+            break;
+        default:
+            switch (k.ratio) {
+                case 2: ok = launch_fused_src<2>(src, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
+                case 3: ok = launch_fused_src<3>(src, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
+                case 4: ok = launch_fused_src<4>(src, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
+                default: ok = launch_fused_src<0>(src, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
+            }
     }
     return ok ? 1 : -1;
 }
@@ -1728,7 +1744,6 @@ __device__ __forceinline__ void composite_body(const CompositeJob &J, const Laye
     }  // it
 }
 
-__global__ void __launch_bounds__(CB_X *CB_Y, SMR_COMPOSITE_BLOCKS) k_composite(CompositeJob J) { composite_body<false>(J, J.layers); }
 __global__ void __launch_bounds__(CB_X *CB_Y, SMR_COMPOSITE_BLOCKS) k_composite_p(const __grid_constant__ CompositeParams P) {
     composite_body<true>(P.job, P.layers);
 }
@@ -1748,34 +1763,25 @@ __global__ void __launch_bounds__(CB_X *CB_Y, SMR_COMPOSITE_BLOCKS) k_composite_
     composite_body<false>(J, J.layers);
 }
 
-int launch_composite_multi(const CompositeJob *jobs_dev, const CompositeJob *jobs_host, int n, Stream s) {
+int launch_composite(const CompositeJob *jobs_dev, const CompositeJob *jobs_host, const LayerDev *layers0_host, int n, Stream s) {
     static_assert(sizeof(CompositeJob) % 4 == 0 && sizeof(CompositeJob) / 4 <= CB_X * CB_Y, "job copied by one block pass");
     int gx = 0, gy = 0;
     for (int i = 0; i < n; i++) {
+        // a tile list leaves out the tiles the resample kernel has written already (all of them: no launch)
         if (jobs_host[i].tile_list != nullptr) { gx = max(gx, jobs_host[i].n_tiles); gy = max(gy, jobs_host[i].n_tiles > 0 ? 1 : 0); continue; }
         gx = max(gx, (jobs_host[i].width + CB_X * CT_W - 1) / (CB_X * CT_W));
         gy = max(gy, (jobs_host[i].height + CB_Y * CT_H * CT_ITERS - 1) / (CB_Y * CT_H * CT_ITERS));
     }
     if (n <= 0 || gx == 0 || gy == 0) return 0;
-    k_composite_multi<<<dim3(gx, gy, n), dim3(CB_X, CB_Y), 0, (cudaStream_t)s>>>(jobs_dev);
-    return check_launch("k_composite_multi") ? 1 : -1;
-}
-
-int launch_composite(const CompositeJob &job, Stream s) {
-    dim3 b(CB_X, CB_Y), g((job.width + CB_X * CT_W - 1) / (CB_X * CT_W), (job.height + CB_Y * CT_H * CT_ITERS - 1) / (CB_Y * CT_H * CT_ITERS));
-    if (job.tile_list != nullptr) {
-        if (job.n_tiles <= 0) return 0;   // every tile of the frame was written by the resample kernel
-        g = dim3(job.n_tiles, 1);
-    }
-    if (job.n_layers <= PARAM_LAYERS && job.layers_host != nullptr) {
+    if (n == 1 && jobs_host[0].n_layers <= PARAM_LAYERS) {
         CompositeParams P;   // ~26 KB on the host stack; the driver copies the parameter block at launch
-        P.job = job;
-        memcpy(P.layers, job.layers_host, sizeof(LayerDev) * (size_t)job.n_layers);
-        k_composite_p<<<g, b, 0, (cudaStream_t)s>>>(P);
+        P.job = jobs_host[0];
+        memcpy(P.layers, layers0_host, sizeof(LayerDev) * (size_t)P.job.n_layers);
+        k_composite_p<<<dim3(gx, gy), dim3(CB_X, CB_Y), 0, (cudaStream_t)s>>>(P);
         return check_launch("k_composite_p") ? 1 : -1;
     }
-    k_composite<<<g, b, 0, (cudaStream_t)s>>>(job);
-    return check_launch("k_composite") ? 1 : -1;
+    k_composite_multi<<<dim3(gx, gy, n), dim3(CB_X, CB_Y), 0, (cudaStream_t)s>>>(jobs_dev);
+    return check_launch("k_composite_multi") ? 1 : -1;
 }
 
 // ------------------------------------------------------------------------------------------------

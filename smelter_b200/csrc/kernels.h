@@ -81,12 +81,15 @@ struct alignas(16) LayerDev {
 // -- every output pixel is the weight-1/2 bilinear tap of one aligned 2x2 texel quad: texel = (2 (px + tx_off), 2 (py + ty_off))
 enum : int32_t { FAST_IDENT = 1, FAST_CONST = 2, FAST_LUT = 4, FAST_OPAQUE = 8, FAST_SAMPLE = 16, FAST_HALF = 32 };
 
+// field order matters for speed: k_composite_multi's instruction schedule follows the offsets of its shared copy of the job
 struct CompositeJob {
     int32_t width, height;           // render target (root node texture) size
     int32_t mode;                    // 0 GpuOptimized (sRGB target, linear blend), 1 CpuOptimized
     int32_t n_layers;
     const LayerDev *layers;          // device copy
-    const LayerDev *layers_host;     // host copy: small lists are passed in the kernel parameter block instead
+    // with direct tiles in the tick the launch covers only the tiles that are left: block b works on tile
+    // (tile_list[b] & 0xffff, tile_list[b] >> 16), row-major order; nullptr: block (x, y) = tile (x, y)
+    const uint32_t *tile_list;
     const MaskDev *masks;
     const Tex *textures;
     // outputs: RGBA8 target and/or fused YUV planes (K10/K11)
@@ -98,10 +101,7 @@ struct CompositeJob {
     // resample kernel has already written its Y / chroma bytes (FusedJob.direct_map), the composite skips the tile
     const uint8_t *direct_map;
     int32_t map_w;
-    // with direct tiles in the tick the launch covers only the tiles that are left: block b works on tile
-    // (tile_list[b] & 0xffff, tile_list[b] >> 16), row-major order; nullptr: block (x, y) = tile (x, y)
-    const uint32_t *tile_list;
-    int32_t n_tiles;
+    int32_t n_tiles;                 // entries of tile_list
 };
 constexpr int kDirectTileW = 128, kDirectTileH = 16;   // = the composite's block tile (CB_X * CT_W x CB_Y * CT_H)
 
@@ -132,16 +132,12 @@ struct FusedJob {
     const int32_t *first_h;
     const float *w_v, *inv_v;
     const int32_t *first_v;
-    int32_t variant;        // 0: any ratio (weights from smem); 2,3,4: integer horizontal ratio (constant-bank weights);
-                            // 22, 24: integer ratio 2 / 4 on the TMA-staged kernel (k_resample_tma3, resample_tma3.cuh);
-                            // 30 + b: any ratio <= 4 on the TMA-staged kernel (k_resample_tma0, resample_tma0.cuh) with a
-                            //         tap loop of kTma0Window[b] slots; 40 + b: the same on a source box-reduced 2:1
-    // TMA variants: device copies of the CUtensorMap of each source plane (luma; NV12 chroma as u16 texels, or U; V)
+    // TMA kernels: device copies of the CUtensorMap of each source plane (luma; NV12 chroma as u16 texels, or U; V)
     const void *tm0, *tm1, *tm2;
-    int32_t v_same;         // TMA variants: the vertical mapping is the same integer ratio with zero offset (weights = c_wint[S])
-    int32_t strip_cols;     // variants 30..33 (any-ratio TMA kernel): output columns per strip of THIS job (<= 64, even)
-    const uint8_t *lane_perm;   // variants 30..33: [strip][32] which pair of the strip's columns each lane owns (nullptr: lane l owns pair l)
-    // variants 22 / 24 with v_same: K10 / K11 straight out of the vertical pass.  Where the child is shown 1:1, opaque and
+    int32_t v_same;         // TMA kernels: the vertical mapping is the same integer ratio with zero offset (weights = c_wint[S])
+    int32_t strip_cols;     // any-ratio TMA kernel: output columns per strip of THIS job (<= 64, even)
+    const uint8_t *lane_perm;   // any-ratio TMA kernel: [strip][32] which pair of the strip's columns each lane owns (nullptr: lane l owns pair l)
+    // integer-ratio TMA kernel with v_same: K10 / K11 straight out of the vertical pass.  Where the child is shown 1:1, opaque and
     // uncovered (the composite's direct tiles, CompositeJob.direct_map), a resampled pixel IS the output frame's pixel:
     // its Y and the chroma of its 2 x 2 block are written here, from the registers that hold the encoded bytes, and
     // the composite never reads them back.  (fx, fy): frame position of dst (0, 0), both even; dst_w, dst_h even.
@@ -160,14 +156,35 @@ struct FusedPiece {
 };
 // limits the host checks before choosing the fused kernel (mirrors FS_* in kernels.cu)
 constexpr int kFusedStripCols = 64, kFusedWarps = 8, kFusedRing = 64, kFusedSpan = 280, kFusedMaxTaps = 25;
-// TMA-staged variants: output columns per strip, ring rows (>= taps_v + ceil(7 * vertical scale)), box sizes of the
+// TMA-staged kernels: output columns per strip, ring rows (>= taps_v + ceil(7 * vertical scale)), box sizes of the
 // tensor maps the host encodes (bytes x rows; NV12 chroma in u16 texels)
 constexpr int kTmaStripCols4 = 58, kTmaStripCols2 = 122, kTmaRing4 = 54, kTmaRing2 = 28;
 // luma and NV12 chroma are addressed in 2-byte elements (a box may be at most 256 elements wide), planar chroma in bytes
 constexpr int kTmaLumaBoxW = 136, kTmaLumaBoxH = 32, kTmaNv12BoxW = 144, kTmaPlanarBoxW = 160, kTmaChromaBoxH = 18;
 constexpr int kTma0Groups = 2, kTma0MaxSpan = 256, kTma0MaxTaps = 25;
 constexpr int kTma0Window[4] = {20, 25, 29, 33};
-inline int fused_strip_cols(int variant) { return variant == 24 ? kTmaStripCols4 : variant == 22 ? kTmaStripCols2 : kFusedStripCols; }
+
+// Which kernel resamples a FusedJob (host side only; every job of one launch has the same kernel and source class)
+struct FusedKernel {
+    enum Kind : int32_t {
+        LDG,      // k_resample_fused_int: LDG-staged, weights from smem (ratio 0) or the constant bank (integer ratio 2 / 3 / 4)
+        TMA_INT,  // k_resample_tma3 (resample_tma3.cuh): integer ratio 2 / 4, TMA-staged
+        TMA_ANY,  // k_resample_tma0 (resample_tma0.cuh): any ratio <= 4, TMA-staged, a tap loop of kTma0Window[window] slots;
+                  // with `box` on a source box-reduced 2:1
+    } kind = LDG;
+    int32_t ratio = 0, window = 0, box = 0;
+    bool operator==(const FusedKernel &o) const { return kind == o.kind && ratio == o.ratio && window == o.window && box == o.box; }
+};
+// What a launch of a fused kernel needs to know: output columns per strip of job `j`, blocks (eight-warp groups) per SM
+// of the persistent grid, and the rows a block's share of the partition is a multiple of
+struct FusedShape { int strip_cols, groups_per_sm, row_gran; };
+inline FusedShape fused_shape(const FusedKernel &k, const FusedJob &j) {
+    switch (k.kind) {
+        case FusedKernel::TMA_INT: return {k.ratio == 4 ? kTmaStripCols4 : kTmaStripCols2, 3, 2};
+        case FusedKernel::TMA_ANY: return {j.strip_cols, kTma0Groups, 8};
+        default: return {kFusedStripCols, 3, 8};
+    }
+}
 
 struct WeightJob {          // resample.wgsl:42-86 evaluated once per output coordinate
     float scale, offset;
@@ -221,13 +238,13 @@ inline int fused_source_class(int tex_kind) {
 int launch_preprocess(const Tex &src, int mode, int rescale, uint8_t *out, int out_pitch, int out_w, int out_h, Stream s);
 // text node texture: clear + glyph quads alpha-blended in list order
 int launch_text(const TextJob &job, Stream s);
-int launch_resample_fused(int variant, int src, const FusedJob *jobs_dev, const FusedPiece *pieces_dev,
+int launch_resample_fused(const FusedKernel &k, int src, const FusedJob *jobs_dev, const FusedPiece *pieces_dev,
                           const int *piece_begin_dev, int nblocks, Stream s);
-// integer-ratio variant: the (single-phase) weight row of ratio S goes to constant memory, once per mapping
+// integer-ratio LDG kernel: the (single-phase) weight row of ratio S goes to constant memory, once per mapping
 void set_int_weights(int S, const float *weights_dev, const float *inv_dev, int taps, Stream s);
-int launch_composite(const CompositeJob &job, Stream s);
-// every output of a tick in one launch; jobs_dev[i] == jobs_host[i], layers / masks / textures device pointers
-int launch_composite_multi(const CompositeJob *jobs_dev, const CompositeJob *jobs_host, int n, Stream s);
+// every output of a tick in one launch; jobs_dev[i] == jobs_host[i], layers / masks / textures device pointers.  One output
+// with a short layer list (layers0_host: host copy of jobs_host[0].layers) passes job and layers in the parameter block
+int launch_composite(const CompositeJob *jobs_dev, const CompositeJob *jobs_host, const LayerDev *layers0_host, int n, Stream s);
 int launch_output(const OutputJob &job, Stream s);
 int launch_fill_yuv(uint8_t *p0, uint8_t *p1, uint8_t *p2, int pitch0, int pitch1, int pitch2, int w, int h,
                     int out_format, uint8_t y, uint8_t u, uint8_t v, Stream s);

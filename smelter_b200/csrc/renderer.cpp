@@ -320,9 +320,21 @@ class Renderer {
     };
 
     // arenas ----------------------------------------------------------------------------------
-    size_t param_alloc(size_t bytes) {  // returns offset in the param arena
+    size_t param_alloc(size_t bytes) {  // returns offset in the param arena (256-byte aligned: tensor maps need 64)
         size_t off = (param_used_ + 255) & ~(size_t)255;
         param_used_ = off + bytes;
+        if (param_host_.size() < param_used_) param_host_.resize(param_used_ * 2);
+        return off;
+    }
+    size_t param_put(const void *p, size_t bytes) {
+        size_t off = param_alloc(bytes);
+        if (bytes) memcpy(param_host_.data() + off, p, bytes);
+        return off;
+    }
+    // the device structs of a list of host records as one array
+    template <class Rec, class Dev> size_t param_put_all(const std::vector<Rec> &recs, Dev Rec::*dev) {
+        size_t off = param_alloc(sizeof(Dev) * recs.size());
+        for (size_t i = 0; i < recs.size(); i++) memcpy(param_host_.data() + off + i * sizeof(Dev), &(recs[i].*dev), sizeof(Dev));
         return off;
     }
     size_t frame_alloc(size_t bytes) {
@@ -336,6 +348,11 @@ class Renderer {
     smr_status get_weights(const KernelPass &p, WeightEntry &out);
     int materialised_input(Input &in);
     int try_fused_resample(Input &in, const struct AxisMapping &hm, const struct AxisMapping &vm, int dw, int dh);
+    int source_tmaps(const dev::Tex &t, int src_class);
+    int add_texture(const dev::Tex &t, bool opaque, size_t frame_off = SIZE_MAX, int fused_job = -1) {
+        plan_.tex.push_back({t, opaque, frame_off, fused_job});
+        return (int)plan_.tex.size() - 1;
+    }
     void prepare_layer(const RenderLayout &l, int W, int H, int tex_index, int tex_w, int tex_h, dev::LayerDev &d, bool &skip);
     void shader_color(const RGBA &c, float out[4]) const;
 
@@ -348,27 +365,64 @@ class Renderer {
     smr_stats stats_ = {};
     uint64_t tick_ = 0;
 
-    // per-tick build state (host mirrors; device addresses = base + offset, fixed up before launch)
-    struct PendingComposite {
+    // per-tick plan: host records; frame-arena and parameter-arena offsets become device addresses in render_begin once
+    // both arenas are sized
+    struct TexRec {             // one entry of the tick's texture table
+        dev::Tex tex;
+        bool opaque;            // every texel's alpha is 255 by construction
+        size_t frame_off;       // p0 lives in the frame arena at this offset (SIZE_MAX: tex.p0 is a device pointer already)
+        int fused_job;          // the fused resample that writes it, or -1
+    };
+    struct FusedRec {
+        dev::FusedJob job;
+        dev::FusedKernel kernel;
+        int src_tex;            // the job's source (texture table)
+        size_t dst_off;         // frame-arena offset of its RGBA8 output
+        int tmap_idx;           // first of its three entries in `tmaps`, or -1
+        size_t direct_off;      // param-arena offset of the direct-tile map it writes for (SIZE_MAX: none)
+    };
+    struct StageRec {           // one generic resample pass
+        dev::ResampleJob job;
+        int src_tex;            // source from the texture table, or -1: the frame-arena f16 at src_off
+        size_t src_off, dst_off;
+    };
+    struct OutputRec { dev::OutputJob job; int src_tex; };
+    struct CompositeRec {
         dev::CompositeJob job; size_t layers_off, masks_off;
+        size_t out_frame_off = SIZE_MAX;  // the target is an RGBA8 frame-arena texture (SIZE_MAX: the caller's planes)
         size_t direct_off = SIZE_MAX;     // param-arena offset of the direct-tile map (SIZE_MAX: none)
         std::vector<int> direct_owner;    // per tile: the fused job that writes its output bytes, or -1
         bool use_list = false;            // compacted launch over `list` (tiles left for the composite, most expensive first)
         std::vector<uint32_t> list;
+        size_t list_off = SIZE_MAX;       // param-arena offset of `list`
     };
     struct PendingCopy { void *dst; size_t dpitch; const void *src; size_t spitch; size_t width, height; };
-    void plan_tiles(Output &o, PendingComposite &pc, const std::vector<dev::LayerDev> &layers, int W, int H);
-    std::vector<dev::Tex> tex_table_;
-    std::vector<uint8_t> tex_opaque_;  // per table entry: every texel's alpha is 255 by construction
-    std::vector<size_t> tex_frame_off_;       // for textures living in the frame arena: offset of p0 (else SIZE_MAX)
-    std::vector<dev::ResampleJob> stage_jobs_[3];
-    std::vector<std::pair<size_t, size_t>> stage_frame_off_[3];  // (src offset or SIZE_MAX, dst offset)
-    std::vector<int> stage_src_tex_[3];       // texture-table index of the source, or -1 when src is a frame-arena f16
+    struct Fill { uint8_t *p[3]; int pitch[3]; int w, h, fmt; uint8_t yuv[3]; };
+    struct TickPlan {
+        std::vector<TexRec> tex;
+        std::vector<StageRec> stages[3];      // box passes, first passes, last passes
+        std::vector<FusedRec> fused;
+        std::vector<CUtensorMap> tmaps;       // three per TMA job
+        std::vector<dev::WeightJob> weight_jobs;
+        std::vector<std::pair<int, size_t>> convert_jobs;  // (raw tex index, frame offset of RGBA8)
+        std::vector<CompositeRec> composites;
+        std::vector<OutputRec> outputs;
+        std::vector<Fill> fills;
+        std::vector<PendingCopy> d2h;
+        std::map<std::tuple<int, uint32_t, uint32_t, uint32_t, uint32_t, int, int>, int> resample_cache;
+        void clear() {   // keeps the vectors' capacity
+            tex.clear();
+            for (auto &s : stages) s.clear();
+            fused.clear(); tmaps.clear(); weight_jobs.clear(); convert_jobs.clear();
+            composites.clear(); outputs.clear(); fills.clear(); d2h.clear(); resample_cache.clear();
+        }
+    } plan_;
+    void plan_tiles(Output &o, CompositeRec &pc, const std::vector<dev::LayerDev> &layers, int W, int H);
     bool int_weights_set_[5] = {false, false, false, false, false};
     std::vector<std::pair<int, WeightEntry>> pending_int_weights_;
     std::vector<WeightKey> new_weight_keys_;   // cache entries whose k_weights launch is not enqueued yet
     void rollback_weights();                   // a tick that fails before that launch must not leave them behind
-    // TMA variants of the fused resample: descriptors of the source planes, cached per (pointer, pitch, size, kind)
+    // TMA kernels of the fused resample: descriptors of the source planes, cached per (pointer, pitch, size, kind)
     struct TmapKey {
         uintptr_t p; int pitch, w, h, kind;
         bool operator<(const TmapKey &o) const { return std::tie(p, pitch, w, h, kind) < std::tie(o.p, o.pitch, o.w, o.h, o.kind); }
@@ -378,24 +432,7 @@ class Renderer {
     std::map<std::tuple<uint32_t, uint32_t, int32_t, int32_t>, uint8_t *> lane_perms_;
     const uint8_t *lane_perm(float scale, float offset, int n_out, int cols);
     bool plane_tmap(const uint8_t *p, int pitch, int w, int h, int kind, CUtensorMap *out);
-    std::vector<CUtensorMap> tick_tmaps_;      // three per TMA job
-    std::vector<int> fused_tmap_idx_;          // per fused job: first of its three entries in tick_tmaps_, or -1
-    std::vector<size_t> fused_direct_off_;     // per fused job: param-arena offset of the direct-tile map it writes for (SIZE_MAX: none)
-    std::map<int, int> tex_fused_job_;         // texture-table index of a fused resample's output -> its index in fused_jobs_
     bool direct_k11_ = true;                   // SMR_DIRECT_K11=0: A/B switch, every tile goes through the composite
-    bool tile_sort_ = true;                    // SMR_TILE_SORT=0: the compacted composite launch keeps row-major order
-    bool disable_tma_ = false;                 // SMR_DISABLE_TMA=1: A/B switch back to the LDG-staged kernels
-    std::vector<dev::FusedJob> fused_jobs_;
-    std::vector<std::pair<int, size_t>> fused_src_dst_;   // (raw tex index, frame offset of dst)
-    std::vector<dev::WeightJob> weight_jobs_;
-    std::vector<std::pair<int, size_t>> convert_jobs_;  // (raw tex index, frame offset of RGBA8)
-    std::vector<PendingComposite> composites_;
-    std::vector<dev::OutputJob> output_jobs_;
-    std::vector<int> output_src_tex_;
-    struct Fill { uint8_t *p[3]; int pitch[3]; int w, h, fmt; uint8_t yuv[3]; };
-    std::vector<Fill> fills_;
-    std::vector<PendingCopy> d2h_;
-    std::map<std::tuple<int, uint32_t, uint32_t, uint32_t, uint32_t, int, int>, int> resample_cache_;
 
     std::vector<uint8_t> param_host_;  // built here, copied to pinned, then to device
     size_t param_used_ = 0;
@@ -495,9 +532,7 @@ smr_status Renderer::init() {
     if (opts_.max_layouts_count == 0) opts_.max_layouts_count = 100;  // DEFAULT_MAX_LAYOUTS_COUNT
     if (opts_.max_layouts_count > 1024) opts_.max_layouts_count = 1024;
     if (opts_.cuda_device == -1) { host_only_ = true; return SMR_OK; }  // scene/layout inspection only
-    if (const char *e = getenv("SMR_DISABLE_TMA")) disable_tma_ = e[0] == '1';
     if (const char *e = getenv("SMR_DIRECT_K11")) direct_k11_ = e[0] != '0';
-    if (const char *e = getenv("SMR_TILE_SORT")) tile_sort_ = e[0] != '0';
     int n = 0;
     cudaError_t e = cudaGetDeviceCount(&n);
     if (e != cudaSuccess || n <= 0) {
@@ -743,10 +778,7 @@ smr_status Renderer::populate_inputs(uint64_t pts, const smr_input_frame *in, ui
         I.tex = t;
         I.res = {f->width, f->height};
         I.has_frame = true;
-        I.raw_tex = (int)tex_table_.size();
-        tex_table_.push_back(t);
-        tex_opaque_.push_back(t.kind == dev::TEX_YUV420 || t.kind == dev::TEX_NV12 || t.kind >= dev::TEX_YUV422);
-        tex_frame_off_.push_back(SIZE_MAX);
+        I.raw_tex = add_texture(t, t.kind == dev::TEX_YUV420 || t.kind == dev::TEX_NV12 || t.kind >= dev::TEX_YUV422);
     }
     return SMR_OK;
 }
@@ -761,11 +793,8 @@ int Renderer::materialised_input(Input &in) {
     t.kind = dev::TEX_RGBA8;
     t.width = in.tex.width; t.height = in.tex.height;
     t.pitch0 = (int)pitch;
-    in.node_tex = (int)tex_table_.size();
-    tex_table_.push_back(t);
-    tex_opaque_.push_back(in.tex.kind == dev::TEX_YUV420 || in.tex.kind == dev::TEX_NV12 || in.tex.kind >= dev::TEX_YUV422);
-    tex_frame_off_.push_back(off);
-    convert_jobs_.push_back({in.raw_tex, off});
+    in.node_tex = add_texture(t, plan_.tex[in.raw_tex].opaque, off);
+    plan_.convert_jobs.push_back({in.raw_tex, off});
     return in.node_tex;
 }
 
@@ -784,7 +813,7 @@ int Renderer::try_fused_resample(Input &in, const AxisMapping &hm_in, const Axis
     const int lv_h = hm_in.predecimate_levels(), lv_v = vm_in.predecimate_levels();
     const bool box = lv_h == 1 && lv_v == 1;
     if (!box && (lv_h != 0 || lv_v != 0)) return -1;
-    if (box && (disable_tma_ || src_class >= 2 || (dw & 1))) return -1;
+    if (box && (src_class >= 2 || (dw & 1))) return -1;
     const AxisMapping hm = box ? hm_in.on_reduced_source(1) : hm_in, vm = box ? vm_in.on_reduced_source(1) : vm_in;
     KernelPass passes[2];
     if (plan_passes(hm, vm, passes) != 2 || passes[0].mapping.axis != 0) return -1;
@@ -810,34 +839,24 @@ int Renderer::try_fused_resample(Input &in, const AxisMapping &hm_in, const Axis
     j.taps_h = wh.taps; j.taps_v = wv.taps;
     j.w_h = wh.weights; j.inv_h = wh.inv; j.first_h = wh.first;
     j.w_v = wv.weights; j.inv_v = wv.inv; j.first_v = wv.first;
-    j.variant = 0;
+    dev::FusedKernel k;   // LDG, weights from smem
     int tmap_idx = -1;
     if (!box && hm.crop_offset == 0.0f && (sh == 2.0f || sh == 3.0f || sh == 4.0f)) {
-        j.variant = (int)sh;
-        if (!int_weights_set_[j.variant]) {   // enqueued after k_weights of this tick (same stream)
-            int_weights_set_[j.variant] = true;
-            pending_int_weights_.push_back({j.variant, wh});
+        k.ratio = (int)sh;   // LDG, constant-bank weights
+        if (!int_weights_set_[k.ratio]) {   // enqueued after k_weights of this tick (same stream)
+            int_weights_set_[k.ratio] = true;
+            pending_int_weights_.push_back({k.ratio, wh});
         }
         // TMA-staged kernel: ratio 2 or 4, planar 4:2:0 / NV12 planes a descriptor can address (16-byte aligned rows),
         // even target width, the vertical footprint of 8 output rows inside the ring
-        const int ring = j.variant == 4 ? dev::kTmaRing4 : dev::kTmaRing2;
-        if (!disable_tma_ && (j.variant == 2 || j.variant == 4) && src_class < 2 && (dw & 1) == 0 &&
-            (int)std::ceil((dev::kFusedWarps - 1) * sv) + tv + 1 <= ring) {
-            CUtensorMap m[3];
-            memset(m, 0, sizeof(m));
-            bool ok = plane_tmap(t.p0, t.pitch0, t.width, t.height, 0, &m[0]);
-            if (src_class == 1) ok = ok && plane_tmap(t.p1, t.pitch1, t.width / 2, t.height / 2, 1, &m[1]);
-            else ok = ok && plane_tmap(t.p1, t.pitch1, t.width / 2, t.height / 2, 2, &m[1]) &&
-                      plane_tmap(t.p2, t.pitch2, t.width / 2, t.height / 2, 2, &m[2]);
-            if (ok) {
-                tmap_idx = (int)tick_tmaps_.size();
-                tick_tmaps_.insert(tick_tmaps_.end(), m, m + 3);
-                j.v_same = vm.crop_offset == 0.0f && sv == sh && tv == th;
-                j.variant += 20;
-            }
+        const int ring = k.ratio == 4 ? dev::kTmaRing4 : dev::kTmaRing2;
+        if ((k.ratio == 2 || k.ratio == 4) && src_class < 2 && (dw & 1) == 0 &&
+            (int)std::ceil((dev::kFusedWarps - 1) * sv) + tv + 1 <= ring && (tmap_idx = source_tmaps(t, src_class)) >= 0) {
+            j.v_same = vm.crop_offset == 0.0f && sv == sh && tv == th;
+            k.kind = dev::FusedKernel::TMA_INT;
         }
     }
-    if (j.variant < 10 && !disable_tma_ && src_class < 2 && (dw & 1) == 0 && th <= dev::kTma0MaxTaps &&
+    if (k.kind == dev::FusedKernel::LDG && src_class < 2 && (dw & 1) == 0 && th <= dev::kTma0MaxTaps &&
         (int)std::ceil((dev::kFusedWarps - 1) * sv) + tv + 1 <= dev::kTmaRing4) {
         // any other ratio <= 4 (fractional, 3, with a crop offset): the any-ratio TMA kernel; its strips are narrowed so that
         // a strip's source span fits the 256 pixels a warp converts per row
@@ -851,34 +870,31 @@ int Renderer::try_fused_resample(Input &in, const AxisMapping &hm_in, const Axis
         const int win = th + gmax, winp = win + ((7 + win - 1) >> 3);
         int bucket = 0;
         while (bucket < 4 && dev::kTma0Window[bucket] < winp) bucket++;
-        CUtensorMap m[3];
-        memset(m, 0, sizeof(m));
-        bool ok = bucket < 4 && (int)std::ceil((cols - 1) * sh) + th + 3 <= max_span &&
-                  plane_tmap(t.p0, t.pitch0, t.width, t.height, 0, &m[0]);
-        if (ok && src_class == 1) ok = plane_tmap(t.p1, t.pitch1, t.width / 2, t.height / 2, 1, &m[1]);
-        else if (ok) ok = plane_tmap(t.p1, t.pitch1, t.width / 2, t.height / 2, 2, &m[1]) &&
-                          plane_tmap(t.p2, t.pitch2, t.width / 2, t.height / 2, 2, &m[2]);
-        if (ok) {
-            tmap_idx = (int)tick_tmaps_.size();
-            tick_tmaps_.insert(tick_tmaps_.end(), m, m + 3);
+        if (bucket < 4 && (int)std::ceil((cols - 1) * sh) + th + 3 <= max_span && (tmap_idx = source_tmaps(t, src_class)) >= 0) {
             j.strip_cols = cols;
             j.lane_perm = lane_perm(sh, hm.crop_offset, dw, cols);   // nullptr (identity) if the table could not be made
-            j.variant = (box ? 40 : 30) + bucket;
+            k = {dev::FusedKernel::TMA_ANY, 0, bucket, box ? 1 : 0};
         }
     }
-    if (box && j.variant < 40) return -1;   // no other fused kernel reduces (the arena bytes stay unused this tick): generic passes
-    fused_jobs_.push_back(j);
-    fused_tmap_idx_.push_back(tmap_idx);
-    fused_direct_off_.push_back(SIZE_MAX);
-    fused_src_dst_.push_back({in.raw_tex, dst_off});
+    if (box && k.kind != dev::FusedKernel::TMA_ANY) return -1;   // no other fused kernel reduces (the arena bytes stay unused this tick): generic passes
+    plan_.fused.push_back({j, k, in.raw_tex, dst_off, tmap_idx, SIZE_MAX});
     dev::Tex out;
     out.kind = dev::TEX_RGBA8; out.width = dw; out.height = dh; out.pitch0 = dw * 4;
-    int idx = (int)tex_table_.size();
-    tex_fused_job_[idx] = (int)fused_jobs_.size() - 1;
-    tex_table_.push_back(out);
-    tex_opaque_.push_back(1);   // the fused kernel reads YUV and writes alpha 255
-    tex_frame_off_.push_back(dst_off);
-    return idx;
+    return add_texture(out, true, dst_off, (int)plan_.fused.size() - 1);   // the fused kernel reads YUV and writes alpha 255
+}
+
+// The tensor maps of a planar 4:2:0 / NV12 source (luma; NV12 chroma, or U and V) for the TMA kernels, added to the tick's
+// list: the index of the first of the three, or -1 when a plane cannot be described
+int Renderer::source_tmaps(const dev::Tex &t, int src_class) {
+    CUtensorMap m[3];
+    memset(m, 0, sizeof(m));
+    bool ok = plane_tmap(t.p0, t.pitch0, t.width, t.height, 0, &m[0]);
+    if (src_class == 1) ok = ok && plane_tmap(t.p1, t.pitch1, t.width / 2, t.height / 2, 1, &m[1]);
+    else ok = ok && plane_tmap(t.p1, t.pitch1, t.width / 2, t.height / 2, 2, &m[1]) &&
+              plane_tmap(t.p2, t.pitch2, t.width / 2, t.height / 2, 2, &m[2]);
+    if (!ok) return -1;
+    plan_.tmaps.insert(plan_.tmaps.end(), m, m + 3);
+    return (int)plan_.tmaps.size() - 3;
 }
 
 // The deal of a strip's 32 column pairs to the 32 lanes (resample_tma0.cuh): a tap of the horizontal pass is one LDS.128
@@ -954,7 +970,7 @@ void Renderer::rollback_weights() {
     new_weight_keys_.clear();
     for (auto &pw : pending_int_weights_) int_weights_set_[pw.first] = false;
     pending_int_weights_.clear();
-    weight_jobs_.clear();
+    plan_.weight_jobs.clear();
 }
 
 void Renderer::shader_color(const RGBA &c, float out[4]) const {  // wgpu/utils.rs:51-71 + params.rs:353-361
@@ -1106,18 +1122,18 @@ void Renderer::prepare_layer(const RenderLayout &l, int W, int H, int tex_index,
                 // 1:1 mapping on whole texels: the NC-6 tap is texel (px - left, py - top) with weight exactly 1
                 // (|coordinate error| < 1e-3 << 1/512, the 8-bit weight rounds to 0 or 1)
                 d.fast |= dev::FAST_IDENT;
-                if (tex_opaque_[tex_index]) d.fast |= dev::FAST_OPAQUE;
+                if (plan_.tex[tex_index].opaque) d.fast |= dev::FAST_OPAQUE;
                 d.tx_off = -(int)l.left; d.ty_off = -(int)l.top;
-            } else if (l.kind == RenderLayout::ChildNode && tex_index >= 0 && tex_opaque_[tex_index] && l.width > 0.0f &&
+            } else if (l.kind == RenderLayout::ChildNode && tex_index >= 0 && plan_.tex[tex_index].opaque && l.width > 0.0f &&
                        l.height > 0.0f &&
-                       (tex_table_[tex_index].kind == dev::TEX_RGBA8 ||
+                       (plan_.tex[tex_index].tex.kind == dev::TEX_RGBA8 ||
                         (opts_.rendering_mode == SMR_MODE_CPU_OPTIMIZED &&
-                         (tex_table_[tex_index].kind == dev::TEX_NV12 || tex_table_[tex_index].kind == dev::TEX_YUV420)))) {
+                         (plan_.tex[tex_index].tex.kind == dev::TEX_NV12 || plan_.tex[tex_index].tex.kind == dev::TEX_YUV420)))) {
                 // opaque child at a fractional position / size: filtered sample alone, target ignored.  RGBA8: a
                 // resampled child; planar 4:2:0 / NV12 in CpuOptimized: the layout shader's own bilinear scaling of
                 // the (virtual) node texture, K1/K2 evaluated per tap quad
                 d.fast |= dev::FAST_SAMPLE | dev::FAST_OPAQUE;
-                const dev::Tex &tt = tex_table_[tex_index];
+                const dev::Tex &tt = plan_.tex[tex_index].tex;
                 if (tt.kind != dev::TEX_RGBA8 && ((tex_w | tex_h) & 1) == 0 && tex_w <= 4096 && tex_h <= 4096 &&
                     l.width * 2.0f == (float)tex_w && l.height * 2.0f == (float)tex_h && l.crop.left == 0.0f && l.crop.top == 0.0f &&
                     l.crop.width == (float)tex_w && l.crop.height == (float)tex_h && integral(l.left) && integral(l.top) &&
@@ -1302,7 +1318,7 @@ smr_status Renderer::get_weights(const KernelPass &p, WeightEntry &out) {
     dev::WeightJob j;
     j.scale = scale; j.offset = offset; j.n_out = key.n_out; j.taps = e.taps;
     j.weights = e.weights; j.inv_wsum = e.inv; j.first = e.first;
-    weight_jobs_.push_back(j);
+    plan_.weight_jobs.push_back(j);
     weights_[key] = e;
     out = e;
     return SMR_OK;
@@ -1390,7 +1406,7 @@ void plan_tiles_core(const TileLayerBox *boxes, int n_layers, int W, int H, bool
     for (size_t k = 0; k < keyed.size(); k++) list[k] = keyed[k].second;
 }
 
-void Renderer::plan_tiles(Output &o, PendingComposite &pc, const std::vector<dev::LayerDev> &layers, int W, int H) {
+void Renderer::plan_tiles(Output &o, CompositeRec &pc, const std::vector<dev::LayerDev> &layers, int W, int H) {
     const int TW = dev::kDirectTileW, TH = dev::kDirectTileH;
     const int tx_n = (W + TW - 1) / TW, ty_n = (H + TH - 1) / TH;
     if (tx_n > 0xffff || ty_n > 0xffff) return;
@@ -1403,19 +1419,20 @@ void Renderer::plan_tiles(Output &o, PendingComposite &pc, const std::vector<dev
         for (size_t li = 0; li < layers.size(); li++) {
             const dev::LayerDev &L = layers[li];
             if (L.type != 0 || (L.fast & (dev::FAST_IDENT | dev::FAST_OPAQUE)) != (dev::FAST_IDENT | dev::FAST_OPAQUE)) continue;
-            auto it = tex_fused_job_.find(L.tex);
-            if (it == tex_fused_job_.end() || it->second >= 255) continue;   // the map holds the owner as one byte
-            const dev::FusedJob &fj = fused_jobs_[it->second];
+            const int ji = plan_.tex[L.tex].fused_job;   // FAST_IDENT: L.tex >= 0
+            if (ji < 0 || ji >= 255) continue;   // the map holds the owner as one byte
+            const FusedRec &f = plan_.fused[ji];
+            const dev::FusedJob &fj = f.job;
             // 4:1 only: per OUTPUT pixel the emission costs the resample kernel about what it saves the composite; at 2:1 a
             // quarter as many source pixels stand behind each output pixel and the vertical pass (four of a group's eight
             // warps) becomes the longer leg -- measured: 4:1 grid +4 %, 2:1 grid -2 %
-            if (fj.variant != 24 || !fj.v_same || ((fj.dst_w | fj.dst_h) & 1)) continue;
+            if (f.kernel.kind != dev::FusedKernel::TMA_INT || f.kernel.ratio != 4 || !fj.v_same || ((fj.dst_w | fj.dst_h) & 1)) continue;
             if ((L.tx_off & 1) || (L.ty_off & 1)) continue;   // frame position of texel (0, 0) = (-tx_off, -ty_off)
             // the whole child inside the frame: the kernel maps EVERY pixel of the job to a tile of the map, so a child hanging
             // over an edge (overflow: visible, absolute positions) would index tiles that do not exist
             if (L.tx_off > 0 || L.ty_off > 0 || -L.tx_off + fj.dst_w > W || -L.ty_off + fj.dst_h > H) continue;
-            if (fused_direct_off_[it->second] != SIZE_MAX) continue;   // serves another output (or an earlier layer) already
-            job_of[li] = it->second;
+            if (f.direct_off != SIZE_MAX) continue;   // serves another output (or an earlier layer) already
+            job_of[li] = ji;
         }
     uint64_t key = 1469598103934665603ull;
     fnv1a(key, &W, sizeof(W)); fnv1a(key, &H, sizeof(H));
@@ -1429,7 +1446,7 @@ void Renderer::plan_tiles(Output &o, PendingComposite &pc, const std::vector<dev
             boxes[li] = {L.px0, L.px1, L.py0, L.py1, L.ix0, L.ix1, L.iy0, L.iy1, L.jx0, L.jx1, L.jy0, L.jy1,
                          (L.fast & dev::FAST_OPAQUE) ? 1 : 0, job_of[li]};
         }
-        plan_tiles_core(boxes.data(), (int)boxes.size(), W, H, tile_sort_, o.tile_owner_layer, o.tile_list);
+        plan_tiles_core(boxes.data(), (int)boxes.size(), W, H, true, o.tile_owner_layer, o.tile_list);
         o.tile_key = key; o.tile_key_valid = true;
     }
     pc.use_list = true;
@@ -1449,9 +1466,9 @@ void Renderer::plan_tiles(Output &o, PendingComposite &pc, const std::vector<dev
     if (!any) { pc.direct_owner.clear(); return; }
     pc.direct_off = param_alloc(n_tiles);
     for (auto &jl : claimed) {
-        dev::FusedJob &fj = fused_jobs_[jl.first];
+        dev::FusedJob &fj = plan_.fused[jl.first].job;
         const dev::LayerDev &L = layers[jl.second];
-        fused_direct_off_[jl.first] = pc.direct_off;
+        plan_.fused[jl.first].direct_off = pc.direct_off;
         fj.map_w = tx_n;
         fj.direct_id = jl.first + 1;
         fj.fx = -L.tx_off; fj.fy = -L.ty_off;
@@ -1485,7 +1502,7 @@ smr_status Renderer::plan_output(Output &o, smr_output_frame &of, uint64_t pts) 
             CUDA_OK(stage.ensure(dp * rows[p]));
             dst[p] = stage.p;
             pitch[p] = (int)dp;
-            d2h_.push_back({of.planes[p], user_pitch, dst[p], dp, row_bytes[p], rows[p]});
+            plan_.d2h.push_back({of.planes[p], user_pitch, dst[p], dp, row_bytes[p], rows[p]});
             stats_.d2h_bytes += row_bytes[p] * rows[p];
         }
     }
@@ -1494,15 +1511,14 @@ smr_status Renderer::plan_output(Output &o, smr_output_frame &of, uint64_t pts) 
         for (int p = 0; p < 3; p++) { f.p[p] = dst[p]; f.pitch[p] = pitch[p]; }
         f.w = (int)of.width; f.h = (int)of.height; f.fmt = o.format;
         black_yuv(f.yuv);
-        fills_.push_back(f);
+        plan_.fills.push_back(f);
     };
-    auto push_output_job = [&](int src_tex, size_t /*unused*/) {
+    auto push_output_job = [&](int src_tex) {
         dev::OutputJob j;
         j.out_w = (int)of.width; j.out_h = (int)of.height; j.out_format = o.format;
         j.out0 = dst[0]; j.out1 = dst[1]; j.out2 = dst[2];
         j.out_pitch0 = pitch[0]; j.out_pitch1 = pitch[1]; j.out_pitch2 = pitch[2];
-        output_jobs_.push_back(j);
-        output_src_tex_.push_back(src_tex);
+        plan_.outputs.push_back({j, src_tex});
     };
 
     if (!o.flat && o.node.root_is_input) {  // pass-through: the root texture IS the input's node texture
@@ -1527,21 +1543,19 @@ smr_status Renderer::plan_output(Output &o, smr_output_frame &of, uint64_t pts) 
             dev::LayerDev d;
             bool skip;
             prepare_layer(l, (int)of.width, (int)of.height, in.raw_tex, (int)of.width, (int)of.height, d, skip);
-            PendingComposite pc;
+            CompositeRec pc;
             memset(&pc.job, 0, sizeof(pc.job));
             pc.job.width = (int)of.width; pc.job.height = (int)of.height; pc.job.mode = mode;
             pc.job.n_layers = skip ? 0 : 1;
-            pc.layers_off = param_alloc(sizeof(dev::LayerDev));
+            pc.layers_off = param_put(&d, sizeof(d));
             pc.masks_off = param_alloc(sizeof(dev::MaskDev));
-            if (param_host_.size() < param_used_) param_host_.resize(param_used_ * 2);
-            memcpy(param_host_.data() + pc.layers_off, &d, sizeof(d));
             pc.job.out_format = o.format;
             pc.job.out0 = dst[0]; pc.job.out1 = dst[1]; pc.job.out2 = dst[2];
             pc.job.out_pitch0 = pitch[0]; pc.job.out_pitch1 = pitch[1]; pc.job.out_pitch2 = pitch[2];
-            composites_.push_back(pc);
+            plan_.composites.push_back(pc);
             return SMR_OK;
         }
-        push_output_job(in.raw_tex, 0);
+        push_output_job(in.raw_tex);
         return SMR_OK;
     }
 
@@ -1578,28 +1592,26 @@ smr_status Renderer::plan_output(Output &o, smr_output_frame &of, uint64_t pts) 
                         memcpy(&cb[0], &l.crop.left, 4); memcpy(&cb[1], &l.crop.top, 4);
                         memcpy(&cb[2], &l.crop.width, 4); memcpy(&cb[3], &l.crop.height, 4);
                         auto key = std::make_tuple(in->raw_tex, cb[0], cb[1], cb[2], cb[3], dw, dh);
-                        auto hit = resample_cache_.find(key);
-                        if (hit != resample_cache_.end()) {
+                        auto hit = plan_.resample_cache.find(key);
+                        if (hit != plan_.resample_cache.end()) {
                             tex_index = hit->second;  // same input/crop/size already resampled this tick
                         } else if (int fused_tex = try_fused_resample(*in, hm, vm, dw, dh); fused_tex != -1) {
                             if (fused_tex < -1) return SMR_ERR_CUDA;
                             tex_index = fused_tex;
-                            resample_cache_[key] = tex_index;
+                            plan_.resample_cache[key] = tex_index;
                         } else {
                             int src_tex = materialised_input(*in);
                             int levels[2] = {hm.predecimate_levels(), vm.predecimate_levels()};
                             int fac[2] = {1 << levels[0], 1 << levels[1]};
                             int cur_w = in->tex.width, cur_h = in->tex.height;
-                            size_t cur_off = SIZE_MAX;  // SIZE_MAX: source is tex_table_[src_tex]
+                            size_t cur_off = SIZE_MAX;  // SIZE_MAX: source is plan_.tex[src_tex]
                             if (fac[0] != 1 || fac[1] != 1) {
                                 int rwid = (cur_w + fac[0] - 1) / fac[0], rhei = (cur_h + fac[1] - 1) / fac[1];
                                 size_t off = frame_alloc((size_t)rwid * rhei * 8);
                                 dev::ResampleJob j{};
                                 j.box_fx = fac[0]; j.box_fy = fac[1];
                                 j.dst_w = rwid; j.dst_h = rhei; j.dst_f16 = 1; j.dst_pitch = rwid * 8;
-                                stage_jobs_[0].push_back(j);
-                                stage_frame_off_[0].push_back({SIZE_MAX, off});
-                                stage_src_tex_[0].push_back(src_tex);
+                                plan_.stages[0].push_back({j, src_tex, SIZE_MAX, off});
                                 cur_w = rwid; cur_h = rhei; cur_off = off;
                             }
                             AxisMapping rh_ = hm.on_reduced_source(levels[0]), rv_ = vm.on_reduced_source(levels[1]);
@@ -1630,19 +1642,13 @@ smr_status Renderer::plan_output(Output &o, smr_output_frame &of, uint64_t pts) 
                                 if (cur_off != SIZE_MAX) {
                                     j.src.kind = dev::TEX_F16; j.src.width = cur_w; j.src.height = cur_h; j.src.pitch0 = cur_w * 8;
                                 }
-                                int stage = last ? 2 : 1;
-                                stage_jobs_[stage].push_back(j);
-                                stage_frame_off_[stage].push_back({cur_off, out_off});
-                                stage_src_tex_[stage].push_back(cur_off == SIZE_MAX ? src_tex : -1);
+                                plan_.stages[last ? 2 : 1].push_back({j, cur_off == SIZE_MAX ? src_tex : -1, cur_off, out_off});
                                 if (!last) { cur_w = j.dst_w; cur_h = j.dst_h; cur_off = out_off; }
                             }
                             dev::Tex t;
                             t.kind = dev::TEX_RGBA8; t.width = dw; t.height = dh; t.pitch0 = dw * 4;
-                            tex_index = (int)tex_table_.size();
-                            tex_table_.push_back(t);
-                            tex_opaque_.push_back(0);
-                            tex_frame_off_.push_back(dst_off);
-                            resample_cache_[key] = tex_index;
+                            tex_index = add_texture(t, false, dst_off);
+                            plan_.resample_cache[key] = tex_index;
                         }
                         tex_w = dw; tex_h = dh;
                         l.crop = {0.0f, 0.0f, (float)dw, (float)dh};  // ResampledChild::output_crop
@@ -1668,15 +1674,12 @@ smr_status Renderer::plan_output(Output &o, smr_output_frame &of, uint64_t pts) 
         layers.push_back(d);
     }
 
-    PendingComposite pc;
+    CompositeRec pc;
     memset(&pc.job, 0, sizeof(pc.job));
     pc.job.width = W; pc.job.height = H; pc.job.mode = mode;
     pc.job.n_layers = (int)layers.size();
-    pc.layers_off = param_alloc(sizeof(dev::LayerDev) * std::max<size_t>(layers.size(), 1));
-    pc.masks_off = param_alloc(sizeof(dev::MaskDev) * std::max<size_t>(masks.size(), 1));
-    if (param_host_.size() < param_used_) param_host_.resize(param_used_ * 2);
-    if (!layers.empty()) memcpy(param_host_.data() + pc.layers_off, layers.data(), sizeof(dev::LayerDev) * layers.size());
-    if (!masks.empty()) memcpy(param_host_.data() + pc.masks_off, masks.data(), sizeof(dev::MaskDev) * masks.size());
+    pc.layers_off = param_put(layers.data(), sizeof(dev::LayerDev) * layers.size());
+    pc.masks_off = param_put(masks.data(), sizeof(dev::MaskDev) * masks.size());
 
     bool same_size = (size_t)W == o.res.width && (size_t)H == o.res.height;
     bool fused_fmt = o.format == SMR_OUT_PLANAR_YUV420 || o.format == SMR_OUT_NV12;
@@ -1685,23 +1688,17 @@ smr_status Renderer::plan_output(Output &o, smr_output_frame &of, uint64_t pts) 
         pc.job.out_format = o.format;
         pc.job.out0 = dst[0]; pc.job.out1 = dst[1]; pc.job.out2 = dst[2];
         pc.job.out_pitch0 = pitch[0]; pc.job.out_pitch1 = pitch[1]; pc.job.out_pitch2 = pitch[2];
-        if (fused_fmt && (direct_k11_ || tile_sort_)) plan_tiles(o, pc, layers, W, H);
-        composites_.push_back(pc);
+        if (fused_fmt) plan_tiles(o, pc, layers, W, H);
+        plan_.composites.push_back(pc);
     } else {
         if (o.format == SMR_OUT_RGBA8) { set_error("RGBA output must match the root layout resolution"); return SMR_ERR_UNSUPPORTED; }
-        size_t off = frame_alloc((size_t)W * H * 4);
+        pc.out_frame_off = frame_alloc((size_t)W * H * 4);
         pc.job.out_format = -1;
-        pc.job.out0 = (uint8_t *)(uintptr_t)off;  // frame offset, fixed up in render_begin
         pc.job.out_pitch0 = W * 4;
-        pc.job.out1 = (uint8_t *)(uintptr_t)1;      // marker: out0 is a frame offset
-        composites_.push_back(pc);
+        plan_.composites.push_back(pc);
         dev::Tex t;
         t.kind = dev::TEX_RGBA8; t.width = W; t.height = H; t.pitch0 = W * 4;
-        int ti = (int)tex_table_.size();
-        tex_table_.push_back(t);
-        tex_opaque_.push_back(0);
-        tex_frame_off_.push_back(off);
-        push_output_job(ti, 0);
+        push_output_job(add_texture(t, false, pc.out_frame_off));
     }
     return SMR_OK;
 }
@@ -1723,13 +1720,8 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
         inflight_.pop_front();
     }
     uploaded_ = false;
-    tex_table_.clear(); tex_opaque_.clear(); tex_frame_off_.clear();
-    for (int s = 0; s < 3; s++) { stage_jobs_[s].clear(); stage_frame_off_[s].clear(); stage_src_tex_[s].clear(); }
-    fused_jobs_.clear(); fused_src_dst_.clear(); fused_tmap_idx_.clear(); tick_tmaps_.clear();
-    fused_direct_off_.clear(); tex_fused_job_.clear();
     rollback_weights();   // leftovers of a tick that failed before its weight launch (normally empty)
-    weight_jobs_.clear(); convert_jobs_.clear(); composites_.clear(); output_jobs_.clear(); output_src_tex_.clear();
-    fills_.clear(); d2h_.clear(); resample_cache_.clear();
+    plan_.clear();
     param_used_ = 0; frame_used_ = 0;
     uint64_t launches = 0;
     cudaStream_t done_on = stream_;   // the stream the tick's last operation goes to
@@ -1775,82 +1767,69 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
     if (frame_used_ + 512 > frame_dev_.cap && !inflight_.empty()) CUDA_OK(cudaStreamSynchronize(stream_));
     CUDA_OK(frame_dev_.ensure(frame_used_ + 512));
     uint8_t *fb = frame_dev_.p;
-    for (size_t i = 0; i < tex_table_.size(); i++)
-        if (tex_frame_off_[i] != SIZE_MAX) tex_table_[i].p0 = fb + tex_frame_off_[i];
-    for (int s = 0; s < 3; s++)
-        for (size_t i = 0; i < stage_jobs_[s].size(); i++) {
-            dev::ResampleJob &j = stage_jobs_[s][i];
-            if (stage_src_tex_[s][i] >= 0) j.src = tex_table_[stage_src_tex_[s][i]];
-            else j.src.p0 = fb + stage_frame_off_[s][i].first;
-            j.dst = fb + stage_frame_off_[s][i].second;
+    for (TexRec &t : plan_.tex)
+        if (t.frame_off != SIZE_MAX) t.tex.p0 = fb + t.frame_off;
+    for (auto &stage : plan_.stages)
+        for (StageRec &r : stage) {
+            if (r.src_tex >= 0) r.job.src = plan_.tex[r.src_tex].tex;
+            else r.job.src.p0 = fb + r.src_off;
+            r.job.dst = fb + r.dst_off;
         }
-    for (size_t i = 0; i < output_jobs_.size(); i++) output_jobs_[i].src = tex_table_[output_src_tex_[i]];
-    for (size_t i = 0; i < fused_jobs_.size(); i++) {
-        fused_jobs_[i].src = tex_table_[fused_src_dst_[i].first];
-        fused_jobs_[i].dst = fb + fused_src_dst_[i].second;
+    for (OutputRec &r : plan_.outputs) r.job.src = plan_.tex[r.src_tex].tex;
+    for (FusedRec &f : plan_.fused) {
+        f.job.src = plan_.tex[f.src_tex].tex;
+        f.job.dst = fb + f.dst_off;
     }
+    for (CompositeRec &c : plan_.composites)
+        if (c.out_frame_off != SIZE_MAX) c.job.out0 = fb + c.out_frame_off;
 
     // ---- pack the parameter arena and ship it in one copy -------------------------------------
-    size_t tex_off = param_alloc(sizeof(dev::Tex) * std::max<size_t>(tex_table_.size(), 1));
-    size_t stage_off[3], wj_off;
-    for (int s = 0; s < 3; s++) stage_off[s] = param_alloc(sizeof(dev::ResampleJob) * std::max<size_t>(stage_jobs_[s].size(), 1));
-    wj_off = param_alloc(sizeof(dev::WeightJob) * std::max<size_t>(weight_jobs_.size(), 1));
-    size_t fj_off = param_alloc(sizeof(dev::FusedJob) * std::max<size_t>(fused_jobs_.size(), 1));
-    const size_t tm_off = param_alloc(sizeof(CUtensorMap) * std::max<size_t>(tick_tmaps_.size(), 1));   // 256-byte aligned
-    // partition the fused resamples of the tick over a persistent grid, one launch per kernel variant
-    struct FusedLaunch { int variant; int src; size_t pieces_off, begin_off; int nblocks; };
+    // partition the fused resamples of the tick over a persistent grid, one launch per kernel and source class
+    struct FusedLaunch { dev::FusedKernel kernel; int src; size_t pieces_off, begin_off; int nblocks; };
     std::vector<FusedLaunch> fused_launches;
     {
-        std::vector<std::pair<int, int>> variants;
-        for (const dev::FusedJob &j : fused_jobs_) {
-            std::pair<int, int> v{j.variant, dev::fused_source_class(j.src.kind)};
-            if (std::find(variants.begin(), variants.end(), v) == variants.end()) variants.push_back(v);
+        std::vector<std::pair<dev::FusedKernel, int>> kernels;
+        for (const FusedRec &f : plan_.fused) {
+            std::pair<dev::FusedKernel, int> v{f.kernel, dev::fused_source_class(f.job.src.kind)};
+            if (std::find(kernels.begin(), kernels.end(), v) == kernels.end()) kernels.push_back(v);
         }
-        for (auto &v : variants) {
+        for (auto &v : kernels) {
             std::vector<int> idx, widths, heights, cols;
-            for (size_t ji = 0; ji < fused_jobs_.size(); ji++) {
-                const dev::FusedJob &j = fused_jobs_[ji];
-                if (j.variant != v.first || dev::fused_source_class(j.src.kind) != v.second) continue;
-                idx.push_back((int)ji); widths.push_back(j.dst_w); heights.push_back(j.dst_h);
-                cols.push_back(v.first >= 30 ? j.strip_cols : dev::fused_strip_cols(v.first));
+            dev::FusedShape shape{};
+            for (size_t ji = 0; ji < plan_.fused.size(); ji++) {
+                const FusedRec &f = plan_.fused[ji];
+                if (!(f.kernel == v.first) || dev::fused_source_class(f.job.src.kind) != v.second) continue;
+                shape = dev::fused_shape(f.kernel, f.job);
+                idx.push_back((int)ji); widths.push_back(f.job.dst_w); heights.push_back(f.job.dst_h); cols.push_back(shape.strip_cols);
             }
             std::vector<dev::FusedPiece> pieces;
             std::vector<int> begin;
-            partition_fused_rows(idx.data(), widths.data(), heights.data(), (int)idx.size(),
-                                 sm_count_ * (v.first >= 30 ? dev::kTma0Groups : 3), pieces, begin, dev::kFusedStripCols, cols.data(),
-                                 (v.first == 22 || v.first == 24) ? 2 : 8);
+            partition_fused_rows(idx.data(), widths.data(), heights.data(), (int)idx.size(), sm_count_ * shape.groups_per_sm, pieces,
+                                 begin, dev::kFusedStripCols, cols.data(), shape.row_gran);
             if (pieces.empty()) continue;
             // direct tiles: the vertical pass emits K10 / K11 per PAIR of output rows, so a job's pieces must hold whole pairs
             // (they do whenever every job of the launch has an even height); a job cut at an odd row writes nothing directly
             for (const dev::FusedPiece &pp : pieces)
-                if (fused_direct_off_[pp.job] != SIZE_MAX && ((pp.oy_begin | pp.oy_end) & 1)) {
-                    fused_direct_off_[pp.job] = SIZE_MAX;
-                    for (PendingComposite &pc : composites_)
+                if (plan_.fused[pp.job].direct_off != SIZE_MAX && ((pp.oy_begin | pp.oy_end) & 1)) {
+                    plan_.fused[pp.job].direct_off = SIZE_MAX;
+                    for (CompositeRec &pc : plan_.composites)
                         for (size_t t = 0; t < pc.direct_owner.size(); t++)
                             if (pc.direct_owner[t] == pp.job) {   // back to the composite (cheap interior tiles: at the end of the list)
                                 pc.direct_owner[t] = -1;
                                 pc.list.push_back((uint32_t)(t % (size_t)pc.job.map_w) | ((uint32_t)(t / (size_t)pc.job.map_w) << 16));
                             }
                 }
-            FusedLaunch fl;
-            fl.variant = v.first; fl.src = v.second; fl.nblocks = (int)begin.size() - 1;
-            fl.pieces_off = param_alloc(sizeof(dev::FusedPiece) * pieces.size());
-            fl.begin_off = param_alloc(sizeof(int) * begin.size());
-            if (param_host_.size() < param_used_) param_host_.resize(param_used_ * 2);
-            memcpy(param_host_.data() + fl.pieces_off, pieces.data(), sizeof(dev::FusedPiece) * pieces.size());
-            memcpy(param_host_.data() + fl.begin_off, begin.data(), sizeof(int) * begin.size());
-            fused_launches.push_back(fl);
+            fused_launches.push_back({v.first, v.second, param_put(pieces.data(), sizeof(dev::FusedPiece) * pieces.size()),
+                                      param_put(begin.data(), sizeof(int) * begin.size()), (int)begin.size() - 1});
         }
     }
-    if (param_host_.size() < param_used_) param_host_.resize(param_used_ * 2);
-    if (!tex_table_.empty()) memcpy(param_host_.data() + tex_off, tex_table_.data(), sizeof(dev::Tex) * tex_table_.size());
-    for (int s = 0; s < 3; s++)
-        if (!stage_jobs_[s].empty())
-            memcpy(param_host_.data() + stage_off[s], stage_jobs_[s].data(), sizeof(dev::ResampleJob) * stage_jobs_[s].size());
-    if (!weight_jobs_.empty()) memcpy(param_host_.data() + wj_off, weight_jobs_.data(), sizeof(dev::WeightJob) * weight_jobs_.size());
-    if (!tick_tmaps_.empty()) memcpy(param_host_.data() + tm_off, tick_tmaps_.data(), sizeof(CUtensorMap) * tick_tmaps_.size());
+    const size_t tex_off = param_put_all(plan_.tex, &TexRec::tex);
+    size_t stage_off[3];
+    for (int s = 0; s < 3; s++) stage_off[s] = param_put_all(plan_.stages[s], &StageRec::job);
+    const size_t wj_off = param_put(plan_.weight_jobs.data(), sizeof(dev::WeightJob) * plan_.weight_jobs.size());
+    const size_t tm_off = param_put(plan_.tmaps.data(), sizeof(CUtensorMap) * plan_.tmaps.size());
     uint64_t direct_tiles = 0;
-    for (PendingComposite &pc : composites_) {   // direct-tile maps (one byte per tile: the owner's id) and tile lists
+    for (CompositeRec &pc : plan_.composites) {   // direct-tile maps (one byte per tile: the owner's id) and tile lists
         if (pc.direct_off != SIZE_MAX) {
             bool any = false;
             for (size_t t = 0; t < pc.direct_owner.size(); t++) {
@@ -1861,102 +1840,87 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
             if (!any) pc.direct_off = SIZE_MAX;
         }
         if (pc.use_list) {
-            const size_t off = param_alloc(sizeof(uint32_t) * std::max<size_t>(pc.list.size(), 1));
-            if (param_host_.size() < param_used_) param_host_.resize(param_used_ * 2);
-            if (!pc.list.empty()) memcpy(param_host_.data() + off, pc.list.data(), sizeof(uint32_t) * pc.list.size());
-            pc.job.tile_list = (const uint32_t *)(uintptr_t)off;   // arena offset for now: the arena may still grow
+            pc.list_off = param_put(pc.list.data(), sizeof(uint32_t) * pc.list.size());
             pc.job.n_tiles = (int)pc.list.size();
         }
     }
-    // composite jobs: their device pointers are known once the arena is sized; with two or more outputs in the tick
-    // the jobs travel in the arena and run as ONE launch
-    const size_t cj_off = param_alloc(sizeof(dev::CompositeJob) * std::max<size_t>(composites_.size(), 1));
-    if (param_host_.size() < param_used_) param_host_.resize(param_used_ * 2);
+    const size_t fj_off = param_put_all(plan_.fused, &FusedRec::job);
+    const size_t cj_off = param_put_all(plan_.composites, &CompositeRec::job);   // read by k_composite_multi
+    // the arena is sized: its offsets become device pointers in the packed jobs
     CUDA_OK(param_pinned_[slot_].ensure(param_used_));
     CUDA_OK(param_dev_[slot_].ensure(param_used_));
-    for (size_t i = 0; i < fused_jobs_.size(); i++)
-        if (fused_tmap_idx_[i] >= 0) {
-            const uint8_t *m = param_dev_[slot_].p + tm_off + sizeof(CUtensorMap) * (size_t)fused_tmap_idx_[i];
-            fused_jobs_[i].tm0 = m; fused_jobs_[i].tm1 = m + sizeof(CUtensorMap); fused_jobs_[i].tm2 = m + 2 * sizeof(CUtensorMap);
+    uint8_t *pd = param_dev_[slot_].p;
+    auto dev_ptr = [&](size_t off) -> uint8_t * { return off != SIZE_MAX ? pd + off : nullptr; };
+    dev::FusedJob *fj = reinterpret_cast<dev::FusedJob *>(param_host_.data() + fj_off);
+    for (size_t i = 0; i < plan_.fused.size(); i++) {
+        const FusedRec &f = plan_.fused[i];
+        if (f.tmap_idx >= 0) {
+            const uint8_t *m = pd + tm_off + sizeof(CUtensorMap) * (size_t)f.tmap_idx;
+            fj[i].tm0 = m; fj[i].tm1 = m + sizeof(CUtensorMap); fj[i].tm2 = m + 2 * sizeof(CUtensorMap);
         }
-    for (PendingComposite &pc : composites_) {   // arena offsets -> device pointers
-        pc.job.direct_map = pc.direct_off != SIZE_MAX ? param_dev_[slot_].p + pc.direct_off : nullptr;
-        if (pc.use_list) pc.job.tile_list = (const uint32_t *)(param_dev_[slot_].p + (size_t)(uintptr_t)pc.job.tile_list);
+        fj[i].direct_map = dev_ptr(f.direct_off);
     }
-    for (size_t i = 0; i < fused_jobs_.size(); i++)
-        fused_jobs_[i].direct_map = fused_direct_off_[i] != SIZE_MAX ? param_dev_[slot_].p + fused_direct_off_[i] : nullptr;
-    if (!fused_jobs_.empty()) memcpy(param_host_.data() + fj_off, fused_jobs_.data(), sizeof(dev::FusedJob) * fused_jobs_.size());
-    {
-        uint8_t *pd0 = param_dev_[slot_].p;
-        for (size_t i = 0; i < composites_.size(); i++) {
-            PendingComposite &pc = composites_[i];
-            pc.job.layers = (const dev::LayerDev *)(pd0 + pc.layers_off);
-            pc.job.layers_host = (const dev::LayerDev *)(param_host_.data() + pc.layers_off);
-            pc.job.masks = (const dev::MaskDev *)(pd0 + pc.masks_off);
-            pc.job.textures = (const dev::Tex *)(pd0 + tex_off);
-            if (pc.job.out_format == -1 && pc.job.out1 == (uint8_t *)(uintptr_t)1) {
-                pc.job.out0 = fb + (size_t)(uintptr_t)pc.job.out0;
-                pc.job.out1 = nullptr;
-            }
-            memcpy(param_host_.data() + cj_off + i * sizeof(dev::CompositeJob), &pc.job, sizeof(dev::CompositeJob));
-        }
+    dev::CompositeJob *cj = reinterpret_cast<dev::CompositeJob *>(param_host_.data() + cj_off);
+    for (size_t i = 0; i < plan_.composites.size(); i++) {
+        const CompositeRec &c = plan_.composites[i];
+        cj[i].layers = (const dev::LayerDev *)(pd + c.layers_off);
+        cj[i].masks = (const dev::MaskDev *)(pd + c.masks_off);
+        cj[i].textures = (const dev::Tex *)(pd + tex_off);
+        cj[i].direct_map = dev_ptr(c.direct_off);
+        cj[i].tile_list = (const uint32_t *)dev_ptr(c.list_off);
     }
     memcpy(param_pinned_[slot_].p, param_host_.data(), param_used_);
-    CUDA_OK(cudaMemcpyAsync(param_dev_[slot_].p, param_pinned_[slot_].p, param_used_, cudaMemcpyHostToDevice, stream_));
-    uint8_t *pd = param_dev_[slot_].p;
+    CUDA_OK(cudaMemcpyAsync(pd, param_pinned_[slot_].p, param_used_, cudaMemcpyHostToDevice, stream_));
 
     // ---- launches -----------------------------------------------------------------------------
     auto launched = [&](int n) -> bool { if (n < 0) return false; launches += (uint64_t)n; return true; };
     prof_mark(-1);
-    for (auto &cj : convert_jobs_) {
-        const dev::Tex &src = tex_table_[cj.first];
-        if (!launched(dev::launch_convert_to_rgba(src, fb + cj.second, src.width * 4, stream_))) goto fail;
+    for (auto &cv : plan_.convert_jobs) {
+        const dev::Tex &src = plan_.tex[cv.first].tex;
+        if (!launched(dev::launch_convert_to_rgba(src, fb + cv.second, src.width * 4, stream_))) goto fail;
         prof_mark(SMR_KERNEL_CONVERT);
     }
-    if (!launched(dev::launch_weights((const dev::WeightJob *)(pd + wj_off), weight_jobs_.data(), (int)weight_jobs_.size(), stream_))) goto fail;
-    if (!weight_jobs_.empty()) prof_mark(SMR_KERNEL_WEIGHTS);
+    if (!launched(dev::launch_weights((const dev::WeightJob *)(pd + wj_off), plan_.weight_jobs.data(), (int)plan_.weight_jobs.size(),
+                                      stream_))) goto fail;
+    if (!plan_.weight_jobs.empty()) prof_mark(SMR_KERNEL_WEIGHTS);
     for (auto &pw : pending_int_weights_) dev::set_int_weights(pw.first, pw.second.weights, pw.second.inv, pw.second.taps, stream_);
     pending_int_weights_.clear();
     new_weight_keys_.clear();
     weight_guard.armed = false;   // the tables are being computed on the stream: the cache entries are good
     for (const FusedLaunch &fl : fused_launches) {
-        if (!launched(dev::launch_resample_fused(fl.variant, fl.src, (const dev::FusedJob *)(pd + fj_off),
+        if (!launched(dev::launch_resample_fused(fl.kernel, fl.src, (const dev::FusedJob *)(pd + fj_off),
                                                  (const dev::FusedPiece *)(pd + fl.pieces_off), (const int *)(pd + fl.begin_off),
                                                  fl.nblocks, stream_))) goto fail;
         prof_mark(SMR_KERNEL_RESAMPLE_FUSED);
     }
     for (int s = 0; s < 3; s++) {
-        if (!launched(dev::launch_resample((const dev::ResampleJob *)(pd + stage_off[s]), stage_jobs_[s].data(),
-                                           (int)stage_jobs_[s].size(), stream_))) goto fail;
-        if (!stage_jobs_[s].empty()) prof_mark(SMR_KERNEL_RESAMPLE_BOX + s);
+        if (!launched(dev::launch_resample((const dev::ResampleJob *)(pd + stage_off[s]),
+                                           (const dev::ResampleJob *)(param_host_.data() + stage_off[s]), (int)plan_.stages[s].size(),
+                                           stream_))) goto fail;
+        if (!plan_.stages[s].empty()) prof_mark(SMR_KERNEL_RESAMPLE_BOX + s);
     }
-    if (composites_.size() >= 2) {
-        if (!launched(dev::launch_composite_multi((const dev::CompositeJob *)(pd + cj_off),
-                                                  (const dev::CompositeJob *)(param_host_.data() + cj_off),
-                                                  (int)composites_.size(), stream_))) goto fail;
+    if (!plan_.composites.empty()) {   // ONE launch for every output of the tick
+        if (!launched(dev::launch_composite((const dev::CompositeJob *)(pd + cj_off), cj,
+                                            (const dev::LayerDev *)(param_host_.data() + plan_.composites[0].layers_off),
+                                            (int)plan_.composites.size(), stream_))) goto fail;
         prof_mark(SMR_KERNEL_COMPOSITE);
-    } else {
-        for (PendingComposite &pc : composites_) {
-            if (!launched(dev::launch_composite(pc.job, stream_))) goto fail;
-            prof_mark(SMR_KERNEL_COMPOSITE);
-        }
     }
-    for (dev::OutputJob &oj : output_jobs_) {
-        if (!launched(dev::launch_output(oj, stream_))) goto fail;
+    for (OutputRec &o : plan_.outputs) {
+        if (!launched(dev::launch_output(o.job, stream_))) goto fail;
         prof_mark(SMR_KERNEL_OUTPUT);
     }
-    for (Fill &f : fills_) {
+    for (Fill &f : plan_.fills) {
         if (!launched(dev::launch_fill_yuv(f.p[0], f.p[1], f.p[2], f.pitch[0], f.pitch[1], f.pitch[2], f.w, f.h, f.fmt,
                                            f.yuv[0], f.yuv[1], f.yuv[2], stream_))) goto fail;
         prof_mark(SMR_KERNEL_FILL);
     }
     // read-back on its own stream: the staging planes are per slot, so the next tick's kernels need not wait for it
-    if (!d2h_.empty() && !profiling_) {
+    if (!plan_.d2h.empty() && !profiling_) {
         CUDA_OK(cudaEventRecord(kernels_done_[slot_], stream_));
         CUDA_OK(cudaStreamWaitEvent(d2h_stream_, kernels_done_[slot_], 0));
         done_on = d2h_stream_;
     }
-    for (PendingCopy &c : d2h_)
+    for (PendingCopy &c : plan_.d2h)
         if (c.dpitch == c.width && c.spitch == c.width)
             CUDA_OK(cudaMemcpyAsync(c.dst, c.src, c.width * c.height, cudaMemcpyDeviceToHost, done_on));
         else
