@@ -15,6 +15,7 @@
 #include <dlfcn.h>
 
 #include <algorithm>
+#include <array>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -248,6 +249,17 @@ static bool encode_plane_tmap(const uint8_t *p, int pitch, int width_elems, int 
                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
+// A caller's smr_input_frame once Renderer::read_frame has checked it.  Nothing is uploaded: tex holds the caller's plane
+// pointers and pitches, which a reader of host frames replaces with those of its device copies.
+struct FrameView {
+    dev::Tex tex;
+    struct Plane {
+        const uint8_t *p = nullptr;   // nullptr: the format has no such plane
+        size_t pitch = 0, row_bytes = 0, rows = 0;
+        size_t span() const { return pitch * (rows - 1) + row_bytes; }   // first to last byte of the plane
+    } plane[3];
+};
+
 // ------------------------------------------------------------------------------------------------
 class Renderer {
   public:
@@ -343,8 +355,17 @@ class Renderer {
         return off;
     }
 
-    smr_status populate_inputs(uint64_t pts, const smr_input_frame *in, uint32_t n_in);
+    smr_status check_output(uint32_t w, uint32_t h, int32_t fmt);
+    smr_status read_frame(const smr_input_frame &f, FrameView &v);
+    template <class Use> smr_status select_inputs(uint64_t pts, const smr_input_frame *in, uint32_t n_in, Use use);
+    smr_status upload_input(Input &I, const smr_input_frame &f);
+    Resolution output_children(const Output &o, const OutputNode &node, uint64_t pts, std::vector<Input *> &child_in,
+                               std::vector<std::optional<Resolution>> &child_res);
+    std::vector<RenderLayout> output_layouts(const Output &o, OutputNode &node, uint64_t pts,
+                                             const std::vector<std::optional<Resolution>> &child_res, Resolution root);
     smr_status plan_output(Output &o, smr_output_frame &of, uint64_t pts);
+    smr_status child_texture(Input &in, RenderLayout &l, int &tex_index, int &tex_w, int &tex_h);
+    template <class Launch> smr_status write_rgba(void *rgba, uint32_t pitch, int32_t mem_kind, uint32_t w, uint32_t h, Launch launch);
     smr_status get_weights(const KernelPass &p, WeightEntry &out);
     int materialised_input(Input &in);
     int try_fused_resample(Input &in, const struct AxisMapping &hm, const struct AxisMapping &vm, int dw, int dh);
@@ -522,11 +543,14 @@ Renderer::~Renderer() {
     }
 }
 
-static double srgb_to_linear_f64(uint8_t c) {  // wgpu/utils.rs:74-81
-    double x = (double)c / 255.0;
-    return x < 0.04045 ? x / 12.92 : std::pow((x + 0.055) / 1.055, 2.4);
-}
-static double eotf_f64(double c) { return c <= 0.04045 ? c / 12.92 : std::pow((c + 0.055) / 1.055, 2.4); }
+static double eotf_f64(double c) { return c <= 0.04045 ? c / 12.92 : std::pow((c + 0.055) / 1.055, 2.4); }  // wgpu/utils.rs:74-81
+// sRGB encode thresholds (numeric contract NC-4): byte k + 1 starts where linear light reaches eotf((k + 0.5) / 255); the
+// device table and the host encoder use the same values
+static const std::array<float, 255> kSrgbEncodeThr = [] {
+    std::array<float, 255> thr;
+    for (int k = 0; k < 255; k++) thr[k] = (float)eotf_f64(((double)k + 0.5) / 255.0);
+    return thr;
+}();
 
 smr_status Renderer::init() {
     if (opts_.max_layouts_count == 0) opts_.max_layouts_count = 100;  // DEFAULT_MAX_LAYOUTS_COUNT
@@ -566,13 +590,12 @@ smr_status Renderer::init() {
         CUDA_OK(cudaEventCreateWithFlags(&h2d_done_[i], cudaEventDisableTiming));
         CUDA_OK(cudaEventCreateWithFlags(&tick_done_[i], cudaEventDisableTiming));
     }
-    float u8n[256], dec[256], thr[255];
+    float u8n[256], dec[256];
     for (int b = 0; b < 256; b++) {
         u8n[b] = (float)b / 255.0f;
         dec[b] = (float)eotf_f64((double)b / 255.0);
     }
-    for (int k = 0; k < 255; k++) thr[k] = (float)eotf_f64(((double)k + 0.5) / 255.0);
-    dev::upload_tables(u8n, dec, thr);
+    dev::upload_tables(u8n, dec, kSrgbEncodeThr.data());
     CUDA_OK(cudaGetLastError());
     return SMR_OK;
 }
@@ -601,17 +624,16 @@ smr_status Renderer::unregister_output(const char *id) {
     return SMR_OK;
 }
 
+smr_status Renderer::check_output(uint32_t w, uint32_t h, int32_t fmt) {
+    if (fmt < SMR_OUT_PLANAR_YUV420 || fmt > SMR_OUT_NV12) { set_error("unsupported output format"); return SMR_ERR_UNSUPPORTED; }
+    if (w == 0 || h == 0 || w > 16384 || h > 16384) { set_error("output resolution out of range"); return SMR_ERR_INVALID_ARGUMENT; }
+    return SMR_OK;
+}
+
 smr_status Renderer::update_scene(const char *output_id, uint32_t w, uint32_t h, int32_t fmt, const smr_component *root) {
     if (!output_id || !root) return SMR_ERR_INVALID_ARGUMENT;
     std::lock_guard<std::mutex> g(mu_);
-    if (fmt < SMR_OUT_PLANAR_YUV420 || fmt > SMR_OUT_NV12) {
-        set_error("unsupported output format");
-        return SMR_ERR_UNSUPPORTED;
-    }
-    if (w == 0 || h == 0 || w > 16384 || h > 16384) {
-        set_error("output resolution out of range");
-        return SMR_ERR_INVALID_ARGUMENT;
-    }
+    if (smr_status st = check_output(w, h, fmt); st != SMR_OK) return st;
     Component c;
     std::string err;
     if (!component_from_c(root, c, err)) {
@@ -638,8 +660,7 @@ smr_status Renderer::set_layouts(const char *output_id, uint32_t w, uint32_t h, 
                                  const char *const *child_ids, uint32_t n_children, const smr_render_layout *layouts, uint32_t n) {
     if (!output_id || (n && !layouts) || (n_children && !child_ids)) return SMR_ERR_INVALID_ARGUMENT;
     std::lock_guard<std::mutex> g(mu_);
-    if (fmt < SMR_OUT_PLANAR_YUV420 || fmt > SMR_OUT_NV12) { set_error("unsupported output format"); return SMR_ERR_UNSUPPORTED; }
-    if (w == 0 || h == 0 || w > 16384 || h > 16384) { set_error("output resolution out of range"); return SMR_ERR_INVALID_ARGUMENT; }
+    if (smr_status st = check_output(w, h, fmt); st != SMR_OK) return st;
     std::vector<RenderLayout> ls(n);
     for (uint32_t i = 0; i < n; i++) {
         const smr_render_layout &d = layouts[i];
@@ -723,63 +744,81 @@ static bool tex_kind_of_format(int fmt, dev::Tex &t) {   // FrameData variant ->
     }
 }
 
-smr_status Renderer::populate_inputs(uint64_t pts, const smr_input_frame *in, uint32_t n_in) {
+static void set_tex_plane(dev::Tex &t, int p, const uint8_t *ptr, size_t pitch) {
+    (p == 0 ? t.p0 : p == 1 ? t.p1 : t.p2) = ptr;
+    (p == 0 ? t.pitch0 : p == 1 ? t.pitch1 : t.pitch2) = (int)pitch;
+}
+
+static bool frame_size_ok(const smr_input_frame &f) { return f.width >= 2 && f.height >= 2 && f.width <= 16384 && f.height <= 16384; }
+
+// The checks every reader of a caller's frame applies (smr_render, smr_preprocess_frame, the exchange calls)
+smr_status Renderer::read_frame(const smr_input_frame &f, FrameView &v) {
+    if (!frame_size_ok(f)) { set_error("input frame resolution out of range"); return SMR_ERR_INVALID_ARGUMENT; }
+    v = FrameView();
+    if (!tex_kind_of_format(f.format, v.tex)) { set_error("unsupported input frame format"); return SMR_ERR_UNSUPPORTED; }
+    v.tex.width = (int)f.width; v.tex.height = (int)f.height;
+    // the kernels read these as one 4-byte word per texel
+    const bool texel4 = f.format == SMR_FRAME_UYVY422 || f.format == SMR_FRAME_YUYV422 || f.format == SMR_FRAME_RGBA8 ||
+                        f.format == SMR_FRAME_BGRA || f.format == SMR_FRAME_ARGB;
+    for (int p = 0; p < 3; p++) {
+        FrameView::Plane &P = v.plane[p];
+        if (!plane_layout(f.format, f.width, f.height, p, P.row_bytes, P.rows)) continue;
+        if (!f.planes[p]) { set_error("input plane pointer is null"); return SMR_ERR_INVALID_ARGUMENT; }
+        P.pitch = f.pitch[p] ? f.pitch[p] : P.row_bytes;
+        if (P.pitch < P.row_bytes) { set_error("input plane pitch is smaller than a row"); return SMR_ERR_INVALID_ARGUMENT; }
+        if (f.mem_kind == SMR_MEM_DEVICE && texel4 && (((uintptr_t)f.planes[p] | P.pitch) & 3)) {
+            set_error("4-byte texel planes must be 4-byte aligned (pointer and pitch)");
+            return SMR_ERR_INVALID_ARGUMENT;
+        }
+        P.p = (const uint8_t *)f.planes[p];
+        set_tex_plane(v.tex, p, P.p, P.pitch);
+    }
+    return SMR_OK;
+}
+
+// A frame set as the scene and the render loop see it: the scene records the input resolutions (state.rs:233-239), and a
+// registered input has a live frame when the set holds one with its id -- the last such -- that is not stale
+// (Duration::saturating_sub(frame_set.pts, timeout) > frame.pts, render_loop.rs:29-32).  `use(input, frame or nullptr)` runs
+// for every registered input before it is marked live; the first status other than SMR_OK ends the walk.
+template <class Use> smr_status Renderer::select_inputs(uint64_t pts, const smr_input_frame *in, uint32_t n_in, Use use) {
+    std::map<std::string, Resolution> res_map;
+    for (uint32_t i = 0; i < n_in; i++)
+        if (in[i].input_id) res_map[in[i].input_id] = {in[i].width, in[i].height};
+    scene_.register_render_event(pts, std::move(res_map));
+    const uint64_t lim = pts > opts_.stream_fallback_timeout_ns ? pts - opts_.stream_fallback_timeout_ns : 0;
     for (auto &kv : inputs_) {
         Input &I = kv.second;
-        I.has_frame = false;
-        I.node_tex = I.raw_tex = -1;
         const smr_input_frame *f = nullptr;
         for (uint32_t i = 0; i < n_in; i++)
             if (in[i].input_id && kv.first == in[i].input_id) f = &in[i];
-        if (!f) continue;
-        // Duration::saturating_sub(frame_set.pts, timeout) > frame.pts  => stale, render_loop.rs:29-32
-        uint64_t lim = pts > opts_.stream_fallback_timeout_ns ? pts - opts_.stream_fallback_timeout_ns : 0;
-        if (lim > f->pts_ns) continue;
-        if (f->width < 2 || f->height < 2 || f->width > 16384 || f->height > 16384) {
-            set_error("input frame resolution out of range");
-            return SMR_ERR_INVALID_ARGUMENT;
-        }
-        dev::Tex t;
-        if (!tex_kind_of_format(f->format, t)) { set_error("unsupported input frame format"); return SMR_ERR_UNSUPPORTED; }
-        t.width = (int)f->width; t.height = (int)f->height;
-        const uint8_t *ptrs[3] = {nullptr, nullptr, nullptr};
-        int pitches[3] = {0, 0, 0};
-        for (int p = 0; p < 3; p++) {
-            size_t row_bytes = 0, rows = 0;
-            if (!plane_layout(f->format, f->width, f->height, p, row_bytes, rows)) continue;
-            if (!f->planes[p]) { set_error("input plane pointer is null"); return SMR_ERR_INVALID_ARGUMENT; }
-            size_t spitch = f->pitch[p] ? f->pitch[p] : row_bytes;
-            if (spitch < row_bytes) { set_error("input plane pitch is smaller than a row"); return SMR_ERR_INVALID_ARGUMENT; }
-            if (f->mem_kind == SMR_MEM_DEVICE && (f->format == SMR_FRAME_UYVY422 || f->format == SMR_FRAME_YUYV422 ||
-                                                  f->format == SMR_FRAME_RGBA8 || f->format == SMR_FRAME_BGRA || f->format == SMR_FRAME_ARGB) &&
-                (((uintptr_t)f->planes[p] | spitch) & 3)) {
-                set_error("4-byte texel planes must be 4-byte aligned (pointer and pitch)");
-                return SMR_ERR_INVALID_ARGUMENT;
-            }
-            if (f->mem_kind == SMR_MEM_DEVICE) {
-                ptrs[p] = (const uint8_t *)f->planes[p];
-                pitches[p] = (int)spitch;
-            } else {
-                CUDA_OK(I.planes[slot_][p].ensure(row_bytes * rows));
-                cudaStream_t cs = (upload_rr_++ & 1) ? copy_stream2_ : copy_stream_;
-                if (spitch == row_bytes)   // tightly packed (the reference's bytes::Bytes planes): one linear DMA
-                    CUDA_OK(cudaMemcpyAsync(I.planes[slot_][p].p, f->planes[p], row_bytes * rows, cudaMemcpyHostToDevice, cs));
-                else
-                    CUDA_OK(cudaMemcpy2DAsync(I.planes[slot_][p].p, row_bytes, f->planes[p], spitch, row_bytes, rows,
-                                              cudaMemcpyHostToDevice, cs));
-                uploaded_ = true;
-                stats_.h2d_bytes += row_bytes * rows;
-                ptrs[p] = I.planes[slot_][p].p;
-                pitches[p] = (int)row_bytes;
-            }
-        }
-        t.p0 = ptrs[0]; t.p1 = ptrs[1]; t.p2 = ptrs[2];
-        t.pitch0 = pitches[0]; t.pitch1 = pitches[1]; t.pitch2 = pitches[2];
-        I.tex = t;
-        I.res = {f->width, f->height};
-        I.has_frame = true;
-        I.raw_tex = add_texture(t, t.kind == dev::TEX_YUV420 || t.kind == dev::TEX_NV12 || t.kind >= dev::TEX_YUV422);
+        if (f && lim > f->pts_ns) f = nullptr;
+        I.has_frame = false;
+        if (smr_status st = use(I, f); st != SMR_OK) return st;
+        if (f) { I.has_frame = true; I.res = {f->width, f->height}; }
     }
+    return SMR_OK;
+}
+
+// a live frame, checked and uploaded: host planes go to the slot's buffers on alternating copy streams
+smr_status Renderer::upload_input(Input &I, const smr_input_frame &f) {
+    FrameView v;
+    if (smr_status st = read_frame(f, v); st != SMR_OK) return st;
+    for (int p = 0; p < 3 && f.mem_kind != SMR_MEM_DEVICE; p++) {
+        const FrameView::Plane &P = v.plane[p];
+        if (!P.p) continue;
+        DevBuf &buf = I.planes[slot_][p];
+        CUDA_OK(buf.ensure(P.row_bytes * P.rows));
+        cudaStream_t cs = (upload_rr_++ & 1) ? copy_stream2_ : copy_stream_;
+        if (P.pitch == P.row_bytes)   // tightly packed (the reference's bytes::Bytes planes): one linear DMA
+            CUDA_OK(cudaMemcpyAsync(buf.p, P.p, P.row_bytes * P.rows, cudaMemcpyHostToDevice, cs));
+        else
+            CUDA_OK(cudaMemcpy2DAsync(buf.p, P.row_bytes, P.p, P.pitch, P.row_bytes, P.rows, cudaMemcpyHostToDevice, cs));
+        uploaded_ = true;
+        stats_.h2d_bytes += P.row_bytes * P.rows;
+        set_tex_plane(v.tex, p, buf.p, P.row_bytes);
+    }
+    I.tex = v.tex;
+    I.raw_tex = add_texture(v.tex, v.tex.kind == dev::TEX_YUV420 || v.tex.kind == dev::TEX_NV12 || v.tex.kind >= dev::TEX_YUV422);
     return SMR_OK;
 }
 
@@ -976,9 +1015,9 @@ void Renderer::rollback_weights() {
 void Renderer::shader_color(const RGBA &c, float out[4]) const {  // wgpu/utils.rs:51-71 + params.rs:353-361
     double a = (double)c.a / 255.0;
     if (opts_.rendering_mode == SMR_MODE_GPU_OPTIMIZED) {
-        out[0] = (float)(a * srgb_to_linear_f64(c.r));
-        out[1] = (float)(a * srgb_to_linear_f64(c.g));
-        out[2] = (float)(a * srgb_to_linear_f64(c.b));
+        out[0] = (float)(a * eotf_f64((double)c.r / 255.0));
+        out[1] = (float)(a * eotf_f64((double)c.g / 255.0));
+        out[2] = (float)(a * eotf_f64((double)c.b / 255.0));
     } else {
         out[0] = (float)(a * (double)c.r / 255.0);
         out[1] = (float)(a * (double)c.g / 255.0);
@@ -987,19 +1026,13 @@ void Renderer::shader_color(const RGBA &c, float out[4]) const {  // wgpu/utils.
     out[3] = (float)a;
 }
 
-static float g_thr_host[255];
-static bool g_thr_init = false;
 static uint8_t unorm8_host(float x) { return (uint8_t)std::rint(std::fmin(std::fmax(x, 0.0f), 1.0f) * 255.0f); }
 static uint8_t srgb_encode_host(float lin) {  // numeric contract NC-4, same thresholds as the device table
-    if (!g_thr_init) {
-        for (int k = 0; k < 255; k++) g_thr_host[k] = (float)eotf_f64(((double)k + 0.5) / 255.0);
-        g_thr_init = true;
-    }
     float x = std::fmin(std::fmax(lin, 0.0f), 1.0f);
     int lo = 0, hi = 255;
     while (lo < hi) {
         int mid = (lo + hi) >> 1;
-        if (x >= g_thr_host[mid]) lo = mid + 1; else hi = mid;
+        if (x >= kSrgbEncodeThr[mid]) lo = mid + 1; else hi = mid;
     }
     return (uint8_t)lo;
 }
@@ -1149,6 +1182,30 @@ void Renderer::prepare_layer(const RenderLayout &l, int W, int H, int tex_index,
     skip = false;
 }
 
+// An RGBA8 result of w x h for the caller: `launch` writes it into `rgba` itself (device memory) or into pre_out_, which is
+// copied back (host memory).  Returns once the result is complete, like the reference's device.poll
+// (frame_pre_processor.rs:171-176); the caller's host buffers are borrowed for the call only.
+template <class Launch>
+smr_status Renderer::write_rgba(void *rgba, uint32_t pitch, int32_t mem_kind, uint32_t w, uint32_t h, Launch launch) {
+    const size_t row = (size_t)w * 4, user_pitch = pitch ? pitch : row;
+    if (user_pitch < row) { set_error("output pitch smaller than a row"); return SMR_ERR_BUFFER_TOO_SMALL; }
+    uint8_t *dst = (uint8_t *)rgba;
+    size_t dpitch = user_pitch;
+    if (mem_kind != SMR_MEM_DEVICE) {
+        if (row * h > pre_out_.cap) CUDA_OK(cudaStreamSynchronize(stream_));
+        CUDA_OK(pre_out_.ensure(row * h));
+        dst = pre_out_.p; dpitch = row;
+    } else if ((dpitch & 3) || ((uintptr_t)dst & 3)) { set_error("device RGBA8 planes are 4-byte aligned"); return SMR_ERR_INVALID_ARGUMENT; }
+    if (launch(dst, (int)dpitch) < 0) { set_error(dev::last_launch_error()); return SMR_ERR_CUDA; }
+    stats_.kernel_launches++;
+    if (mem_kind != SMR_MEM_DEVICE) {
+        CUDA_OK(cudaMemcpy2DAsync(rgba, user_pitch, dst, dpitch, row, h, cudaMemcpyDeviceToHost, stream_));
+        stats_.d2h_bytes += row * h;
+    }
+    CUDA_OK(cudaStreamSynchronize(stream_));
+    return SMR_OK;
+}
+
 // FramePreProcessor::process_to_bytes / process_to_texture (state/frame_pre_processor.rs:60-100)
 smr_status Renderer::preprocess_frame(const smr_input_frame *f, uint32_t ow, uint32_t oh, void *rgba, uint32_t pitch,
                                       int32_t mem_kind, bool premultiply) {
@@ -1160,58 +1217,28 @@ smr_status Renderer::preprocess_frame(const smr_input_frame *f, uint32_t ow, uin
     std::lock_guard<std::mutex> g(mu_);
     if (host_only_) { set_error("host-only handle (cuda_device = -1) has no device: no CPU fallback"); return SMR_ERR_CUDA; }
     CUDA_OK(cudaSetDevice(opts_.cuda_device));
-    if (f->width < 2 || f->height < 2 || f->width > 16384 || f->height > 16384) {
-        set_error("input frame resolution out of range");
+    const bool rescale = ow != 0 || oh != 0;
+    // the output size is checked after the input size and before the rest of the frame
+    if (rescale && frame_size_ok(*f) && (ow == 0 || oh == 0 || ow > 16384 || oh > 16384)) {
+        set_error("output resolution out of range");
         return SMR_ERR_INVALID_ARGUMENT;
     }
-    const bool rescale = ow != 0 || oh != 0;
+    FrameView v;
+    if (smr_status st = read_frame(*f, v); st != SMR_OK) return st;
     if (!rescale) { ow = f->width; oh = f->height; }
-    if (ow == 0 || oh == 0 || ow > 16384 || oh > 16384) { set_error("output resolution out of range"); return SMR_ERR_INVALID_ARGUMENT; }
-    dev::Tex t;
-    if (!tex_kind_of_format(f->format, t)) { set_error("unsupported input frame format"); return SMR_ERR_UNSUPPORTED; }
-    t.width = (int)f->width; t.height = (int)f->height;
-    const uint8_t *ptrs[3] = {nullptr, nullptr, nullptr};
-    int pitches[3] = {0, 0, 0};
-    for (int p = 0; p < 3; p++) {
-        size_t row_bytes = 0, rows = 0;
-        if (!plane_layout(f->format, f->width, f->height, p, row_bytes, rows)) continue;
-        if (!f->planes[p]) { set_error("input plane pointer is null"); return SMR_ERR_INVALID_ARGUMENT; }
-        size_t spitch = f->pitch[p] ? f->pitch[p] : row_bytes;
-        if (f->mem_kind == SMR_MEM_DEVICE) {
-            ptrs[p] = (const uint8_t *)f->planes[p];
-            pitches[p] = (int)spitch;
-        } else {
-            if (row_bytes * rows > pre_planes_[p].cap) CUDA_OK(cudaStreamSynchronize(stream_));
-            CUDA_OK(pre_planes_[p].ensure(row_bytes * rows));
-            CUDA_OK(cudaMemcpy2DAsync(pre_planes_[p].p, row_bytes, f->planes[p], spitch, row_bytes, rows,
-                                      cudaMemcpyHostToDevice, stream_));
-            stats_.h2d_bytes += row_bytes * rows;
-            ptrs[p] = pre_planes_[p].p;
-            pitches[p] = (int)row_bytes;
-        }
+    for (int p = 0; p < 3 && f->mem_kind != SMR_MEM_DEVICE; p++) {
+        const FrameView::Plane &P = v.plane[p];
+        if (!P.p) continue;
+        if (P.row_bytes * P.rows > pre_planes_[p].cap) CUDA_OK(cudaStreamSynchronize(stream_));
+        CUDA_OK(pre_planes_[p].ensure(P.row_bytes * P.rows));
+        CUDA_OK(cudaMemcpy2DAsync(pre_planes_[p].p, P.row_bytes, P.p, P.pitch, P.row_bytes, P.rows, cudaMemcpyHostToDevice, stream_));
+        stats_.h2d_bytes += P.row_bytes * P.rows;
+        set_tex_plane(v.tex, p, pre_planes_[p].p, P.row_bytes);
     }
-    t.p0 = ptrs[0]; t.p1 = ptrs[1]; t.p2 = ptrs[2];
-    t.pitch0 = pitches[0]; t.pitch1 = pitches[1]; t.pitch2 = pitches[2];
-    const size_t row = (size_t)ow * 4, user_pitch = pitch ? pitch : row;
-    if (user_pitch < row) { set_error("output pitch smaller than a row"); return SMR_ERR_BUFFER_TOO_SMALL; }
-    uint8_t *dst = (uint8_t *)rgba;
-    size_t dpitch = user_pitch;
-    if (mem_kind != SMR_MEM_DEVICE) {
-        if (row * oh > pre_out_.cap) CUDA_OK(cudaStreamSynchronize(stream_));
-        CUDA_OK(pre_out_.ensure(row * oh));
-        dst = pre_out_.p; dpitch = row;
-    }
-    if (dev::launch_preprocess(t, opts_.rendering_mode, premultiply ? 2 : (rescale ? 1 : 0), dst, (int)dpitch, (int)ow, (int)oh, stream_) < 0) {
-        set_error(dev::last_launch_error());
-        return SMR_ERR_CUDA;
-    }
-    stats_.kernel_launches++;
-    if (mem_kind != SMR_MEM_DEVICE) {
-        CUDA_OK(cudaMemcpy2DAsync(rgba, user_pitch, dst, dpitch, row, oh, cudaMemcpyDeviceToHost, stream_));
-        stats_.d2h_bytes += row * oh;
-    }
-    CUDA_OK(cudaStreamSynchronize(stream_));   // the reference blocks in device.poll (frame_pre_processor.rs:171-176)
-    return SMR_OK;
+    const int kind = premultiply ? 2 : (rescale ? 1 : 0);
+    return write_rgba(rgba, pitch, mem_kind, ow, oh, [&](uint8_t *dst, int dpitch) {
+        return dev::launch_preprocess(v.tex, opts_.rendering_mode, kind, dst, dpitch, (int)ow, (int)oh, stream_);
+    });
 }
 
 // TextRendererNode::render (transformations/text_renderer.rs:72-167): clear + glyphon's glyph quads
@@ -1261,24 +1288,10 @@ smr_status Renderer::render_text(uint32_t w, uint32_t h, smr_rgba bg, const smr_
         stats_.h2d_bytes += bytes;
         J.glyphs = reinterpret_cast<const dev::GlyphDev *>(pre_planes_[2].p);
     }
-    const size_t row = (size_t)w * 4, user_pitch = pitch ? pitch : row;
-    if (user_pitch < row) { set_error("output pitch smaller than a row"); return SMR_ERR_BUFFER_TOO_SMALL; }
-    uint8_t *dst = (uint8_t *)rgba;
-    size_t dpitch = user_pitch;
-    if (mem_kind != SMR_MEM_DEVICE) {
-        if (row * h > pre_out_.cap) CUDA_OK(cudaStreamSynchronize(stream_));
-        CUDA_OK(pre_out_.ensure(row * h));
-        dst = pre_out_.p; dpitch = row;
-    } else if ((dpitch & 3) || ((size_t)dst & 3)) { set_error("device RGBA8 planes are 4-byte aligned"); return SMR_ERR_INVALID_ARGUMENT; }
-    J.out = dst; J.out_pitch = (int)dpitch;
-    if (dev::launch_text(J, stream_) < 0) { set_error(dev::last_launch_error()); return SMR_ERR_CUDA; }
-    stats_.kernel_launches++;
-    if (mem_kind != SMR_MEM_DEVICE) {
-        CUDA_OK(cudaMemcpy2DAsync(rgba, user_pitch, dst, dpitch, row, h, cudaMemcpyDeviceToHost, stream_));
-        stats_.d2h_bytes += row * h;
-    }
-    CUDA_OK(cudaStreamSynchronize(stream_));   // the glyph list and the atlases are borrowed for the call only
-    return SMR_OK;
+    return write_rgba(rgba, pitch, mem_kind, w, h, [&](uint8_t *dst, int dpitch) {
+        J.out = dst; J.out_pitch = dpitch;
+        return dev::launch_text(J, stream_);
+    });
 }
 
 smr_status Renderer::get_weights(const KernelPass &p, WeightEntry &out) {
@@ -1325,11 +1338,10 @@ smr_status Renderer::get_weights(const KernelPass &p, WeightEntry &out) {
 }
 
 static void black_yuv(uint8_t out[3]) {  // RGBColor::BLACK.to_yuv() through an R8Unorm store
-    auto q = [](float x) { return (uint8_t)std::rint(std::fmin(std::fmax(x, 0.0f), 1.0f) * 255.0f); };
     float y = 0.0f, u = 0.0f, v = 0.0f;
-    out[0] = q((y * 0.85882354f) + (16.0f / 255.0f));
-    out[1] = q(((u + 0.5f) * 0.8784314f) + (16.0f / 255.0f));
-    out[2] = q(((v + 0.5f) * 0.8784314f) + (16.0f / 255.0f));
+    out[0] = unorm8_host((y * 0.85882354f) + (16.0f / 255.0f));
+    out[1] = unorm8_host(((u + 0.5f) * 0.8784314f) + (16.0f / 255.0f));
+    out[2] = unorm8_host(((v + 0.5f) * 0.8784314f) + (16.0f / 255.0f));
 }
 
 static void out_plane_layout(int fmt, uint32_t w, uint32_t h, size_t row_bytes[3], size_t rows[3]) {
@@ -1478,6 +1490,104 @@ void Renderer::plan_tiles(Output &o, CompositeRec &pc, const std::vector<dev::La
     }
 }
 
+// An output's children at `pts` (sources[i].resolution(), layout.rs:176-179): the input behind each (nullptr: no live frame)
+// and its resolution.  Returns the root resolution.
+Resolution Renderer::output_children(const Output &o, const OutputNode &node, uint64_t pts, std::vector<Input *> &child_in,
+                                     std::vector<std::optional<Resolution>> &child_res) {
+    for (const std::string &id : (o.flat ? o.flat_children : node.child_input_ids)) {
+        auto it = inputs_.find(id);
+        Input *in = it != inputs_.end() && it->second.has_frame ? &it->second : nullptr;
+        child_in.push_back(in);
+        child_res.push_back(in ? std::optional<Resolution>(in->res) : std::nullopt);
+    }
+    return o.flat ? o.flat_root : node.layout_resolution(pts);
+}
+
+// Its flattened layouts (layout.rs:180-181), untruncated.  Evaluating them advances Tiles::last_layout of `node`: o.node
+// when rendering, a copy for inspection.
+std::vector<RenderLayout> Renderer::output_layouts(const Output &o, OutputNode &node, uint64_t pts,
+                                                   const std::vector<std::optional<Resolution>> &child_res, Resolution root) {
+    return o.flat ? o.flat_layouts : node.layouts(pts, child_res).flatten(child_res, root);
+}
+
+// The texture a child layer samples: the input's own, or in GpuOptimized mode its copy resampled to the layer's size, whose
+// crop then replaces the layer's (resample_scaled_children, layout.rs:238-278)
+smr_status Renderer::child_texture(Input &in, RenderLayout &l, int &tex_index, int &tex_w, int &tex_h) {
+    tex_index = in.raw_tex; tex_w = in.tex.width; tex_h = in.tex.height;
+    if (opts_.rendering_mode != SMR_MODE_GPU_OPTIMIZED) return SMR_OK;
+    float rw = std::round(l.width), rh = std::round(l.height);
+    int dw = rw >= 1.0f ? (rw > 16384.0f ? 16384 : (int)rw) : 1;
+    int dh = rh >= 1.0f ? (rh > 16384.0f ? 16384 : (int)rh) : 1;
+    AxisMapping hm{0, l.crop.left, l.crop.width, dw}, vm{1, l.crop.top, l.crop.height, dh};
+    KernelPass passes[2];
+    if (plan_passes(hm, vm, passes) == 0) return SMR_OK;
+    uint32_t cb[4];
+    memcpy(&cb[0], &l.crop.left, 4); memcpy(&cb[1], &l.crop.top, 4);
+    memcpy(&cb[2], &l.crop.width, 4); memcpy(&cb[3], &l.crop.height, 4);
+    auto key = std::make_tuple(in.raw_tex, cb[0], cb[1], cb[2], cb[3], dw, dh);
+    auto hit = plan_.resample_cache.find(key);
+    if (hit != plan_.resample_cache.end()) {
+        tex_index = hit->second;  // same input/crop/size already resampled this tick
+    } else if (int fused_tex = try_fused_resample(in, hm, vm, dw, dh); fused_tex != -1) {
+        if (fused_tex < -1) return SMR_ERR_CUDA;
+        tex_index = fused_tex;
+        plan_.resample_cache[key] = tex_index;
+    } else {
+        int src_tex = materialised_input(in);
+        int levels[2] = {hm.predecimate_levels(), vm.predecimate_levels()};
+        int fac[2] = {1 << levels[0], 1 << levels[1]};
+        int cur_w = in.tex.width, cur_h = in.tex.height;
+        size_t cur_off = SIZE_MAX;  // SIZE_MAX: source is plan_.tex[src_tex]
+        if (fac[0] != 1 || fac[1] != 1) {
+            int rwid = (cur_w + fac[0] - 1) / fac[0], rhei = (cur_h + fac[1] - 1) / fac[1];
+            size_t off = frame_alloc((size_t)rwid * rhei * 8);
+            dev::ResampleJob j{};
+            j.box_fx = fac[0]; j.box_fy = fac[1];
+            j.dst_w = rwid; j.dst_h = rhei; j.dst_f16 = 1; j.dst_pitch = rwid * 8;
+            plan_.stages[0].push_back({j, src_tex, SIZE_MAX, off});
+            cur_w = rwid; cur_h = rhei; cur_off = off;
+        }
+        AxisMapping rh_ = hm.on_reduced_source(levels[0]), rv_ = vm.on_reduced_source(levels[1]);
+        int np = plan_passes(rh_, rv_, passes);
+        if (np == 0) { set_error("resampler planning failed"); return SMR_ERR_INVALID_ARGUMENT; }
+        size_t dst_off = frame_alloc((size_t)dw * dh * 4);
+        for (int pi = 0; pi < np; pi++) {
+            const KernelPass &kp = passes[pi];
+            bool last = pi == np - 1;
+            WeightEntry we;
+            smr_status st = get_weights(kp, we);
+            if (st != SMR_OK) return st;
+            dev::ResampleJob j{};
+            j.axis = kp.mapping.axis; j.perp_offset = kp.perp_offset; j.taps = we.taps;
+            j.weights = we.weights; j.inv_wsum = we.inv; j.first = we.first;
+            j.box_fx = j.box_fy = 1;
+            size_t out_off;
+            if (last) {
+                j.dst_w = dw; j.dst_h = dh; j.dst_f16 = 0; j.dst_pitch = dw * 4;
+                out_off = dst_off;
+            } else {
+                j.dst_w = kp.mapping.axis == 0 ? kp.mapping.dst_len : cur_w;  // output_size
+                j.dst_h = kp.mapping.axis == 1 ? kp.mapping.dst_len : cur_h;
+                j.dst_f16 = 1; j.dst_pitch = j.dst_w * 8;
+                out_off = frame_alloc((size_t)j.dst_w * j.dst_h * 8);
+            }
+            // f16 sources carry their geometry in the job; RGBA8/YUV sources come from the table
+            if (cur_off != SIZE_MAX) {
+                j.src.kind = dev::TEX_F16; j.src.width = cur_w; j.src.height = cur_h; j.src.pitch0 = cur_w * 8;
+            }
+            plan_.stages[last ? 2 : 1].push_back({j, cur_off == SIZE_MAX ? src_tex : -1, cur_off, out_off});
+            if (!last) { cur_w = j.dst_w; cur_h = j.dst_h; cur_off = out_off; }
+        }
+        dev::Tex t;
+        t.kind = dev::TEX_RGBA8; t.width = dw; t.height = dh; t.pitch0 = dw * 4;
+        tex_index = add_texture(t, false, dst_off);
+        plan_.resample_cache[key] = tex_index;
+    }
+    tex_w = dw; tex_h = dh;
+    l.crop = {0.0f, 0.0f, (float)dw, (float)dh};  // ResampledChild::output_crop
+    return SMR_OK;
+}
+
 smr_status Renderer::plan_output(Output &o, smr_output_frame &of, uint64_t pts) {
     const int mode = opts_.rendering_mode;
     of.width = (uint32_t)o.res.width; of.height = (uint32_t)o.res.height;
@@ -1559,17 +1669,11 @@ smr_status Renderer::plan_output(Output &o, smr_output_frame &of, uint64_t pts) 
         return SMR_OK;
     }
 
-    // child node resolutions (sources[i].resolution(), layout.rs:176-179)
-    std::vector<std::optional<Resolution>> child_res;
     std::vector<Input *> child_in;
-    for (const std::string &id : (o.flat ? o.flat_children : o.node.child_input_ids)) {
-        auto it = inputs_.find(id);
-        if (it != inputs_.end() && it->second.has_frame) { child_res.push_back(it->second.res); child_in.push_back(&it->second); }
-        else { child_res.push_back(std::nullopt); child_in.push_back(nullptr); }
-    }
-    Resolution root = o.flat ? o.flat_root : o.node.layout_resolution(pts);
+    std::vector<std::optional<Resolution>> child_res;
+    const Resolution root = output_children(o, o.node, pts, child_in, child_res);
     if (root.width == 0 || root.height == 0 || root.width > 16384 || root.height > 16384) { push_fill(); return SMR_OK; }
-    std::vector<RenderLayout> layouts = o.flat ? o.flat_layouts : o.node.layouts(pts, child_res).flatten(child_res, root);
+    std::vector<RenderLayout> layouts = output_layouts(o, o.node, pts, child_res, root);
     if (layouts.size() > opts_.max_layouts_count) layouts.resize(opts_.max_layouts_count);  // params.rs:176-182
 
     const int W = (int)root.width, H = (int)root.height;
@@ -1577,84 +1681,10 @@ smr_status Renderer::plan_output(Output &o, smr_output_frame &of, uint64_t pts) 
     std::vector<dev::MaskDev> masks;
     for (RenderLayout &l : layouts) {
         int tex_index = -1, tex_w = 1, tex_h = 1;
-        if (l.kind == RenderLayout::ChildNode) {
-            Input *in = l.index < child_in.size() ? child_in[l.index] : nullptr;
-            if (in) {
-                tex_index = in->raw_tex; tex_w = in->tex.width; tex_h = in->tex.height;
-                if (mode == SMR_MODE_GPU_OPTIMIZED) {  // resample_scaled_children, layout.rs:238-278
-                    float rw = std::round(l.width), rh = std::round(l.height);
-                    int dw = rw >= 1.0f ? (rw > 16384.0f ? 16384 : (int)rw) : 1;
-                    int dh = rh >= 1.0f ? (rh > 16384.0f ? 16384 : (int)rh) : 1;
-                    AxisMapping hm{0, l.crop.left, l.crop.width, dw}, vm{1, l.crop.top, l.crop.height, dh};
-                    KernelPass passes[2];
-                    if (plan_passes(hm, vm, passes) != 0) {
-                        uint32_t cb[4];
-                        memcpy(&cb[0], &l.crop.left, 4); memcpy(&cb[1], &l.crop.top, 4);
-                        memcpy(&cb[2], &l.crop.width, 4); memcpy(&cb[3], &l.crop.height, 4);
-                        auto key = std::make_tuple(in->raw_tex, cb[0], cb[1], cb[2], cb[3], dw, dh);
-                        auto hit = plan_.resample_cache.find(key);
-                        if (hit != plan_.resample_cache.end()) {
-                            tex_index = hit->second;  // same input/crop/size already resampled this tick
-                        } else if (int fused_tex = try_fused_resample(*in, hm, vm, dw, dh); fused_tex != -1) {
-                            if (fused_tex < -1) return SMR_ERR_CUDA;
-                            tex_index = fused_tex;
-                            plan_.resample_cache[key] = tex_index;
-                        } else {
-                            int src_tex = materialised_input(*in);
-                            int levels[2] = {hm.predecimate_levels(), vm.predecimate_levels()};
-                            int fac[2] = {1 << levels[0], 1 << levels[1]};
-                            int cur_w = in->tex.width, cur_h = in->tex.height;
-                            size_t cur_off = SIZE_MAX;  // SIZE_MAX: source is plan_.tex[src_tex]
-                            if (fac[0] != 1 || fac[1] != 1) {
-                                int rwid = (cur_w + fac[0] - 1) / fac[0], rhei = (cur_h + fac[1] - 1) / fac[1];
-                                size_t off = frame_alloc((size_t)rwid * rhei * 8);
-                                dev::ResampleJob j{};
-                                j.box_fx = fac[0]; j.box_fy = fac[1];
-                                j.dst_w = rwid; j.dst_h = rhei; j.dst_f16 = 1; j.dst_pitch = rwid * 8;
-                                plan_.stages[0].push_back({j, src_tex, SIZE_MAX, off});
-                                cur_w = rwid; cur_h = rhei; cur_off = off;
-                            }
-                            AxisMapping rh_ = hm.on_reduced_source(levels[0]), rv_ = vm.on_reduced_source(levels[1]);
-                            int np = plan_passes(rh_, rv_, passes);
-                            if (np == 0) { set_error("resampler planning failed"); return SMR_ERR_INVALID_ARGUMENT; }
-                            size_t dst_off = frame_alloc((size_t)dw * dh * 4);
-                            for (int pi = 0; pi < np; pi++) {
-                                const KernelPass &kp = passes[pi];
-                                bool last = pi == np - 1;
-                                WeightEntry we;
-                                smr_status st = get_weights(kp, we);
-                                if (st != SMR_OK) return st;
-                                dev::ResampleJob j{};
-                                j.axis = kp.mapping.axis; j.perp_offset = kp.perp_offset; j.taps = we.taps;
-                                j.weights = we.weights; j.inv_wsum = we.inv; j.first = we.first;
-                                j.box_fx = j.box_fy = 1;
-                                size_t out_off;
-                                if (last) {
-                                    j.dst_w = dw; j.dst_h = dh; j.dst_f16 = 0; j.dst_pitch = dw * 4;
-                                    out_off = dst_off;
-                                } else {
-                                    j.dst_w = kp.mapping.axis == 0 ? kp.mapping.dst_len : cur_w;  // output_size
-                                    j.dst_h = kp.mapping.axis == 1 ? kp.mapping.dst_len : cur_h;
-                                    j.dst_f16 = 1; j.dst_pitch = j.dst_w * 8;
-                                    out_off = frame_alloc((size_t)j.dst_w * j.dst_h * 8);
-                                }
-                                // f16 sources carry their geometry in the job; RGBA8/YUV sources come from the table
-                                if (cur_off != SIZE_MAX) {
-                                    j.src.kind = dev::TEX_F16; j.src.width = cur_w; j.src.height = cur_h; j.src.pitch0 = cur_w * 8;
-                                }
-                                plan_.stages[last ? 2 : 1].push_back({j, cur_off == SIZE_MAX ? src_tex : -1, cur_off, out_off});
-                                if (!last) { cur_w = j.dst_w; cur_h = j.dst_h; cur_off = out_off; }
-                            }
-                            dev::Tex t;
-                            t.kind = dev::TEX_RGBA8; t.width = dw; t.height = dh; t.pitch0 = dw * 4;
-                            tex_index = add_texture(t, false, dst_off);
-                            plan_.resample_cache[key] = tex_index;
-                        }
-                        tex_w = dw; tex_h = dh;
-                        l.crop = {0.0f, 0.0f, (float)dw, (float)dh};  // ResampledChild::output_crop
-                    }
-                }
-            }
+        Input *in = l.kind == RenderLayout::ChildNode && l.index < child_in.size() ? child_in[l.index] : nullptr;
+        if (in) {
+            smr_status st = child_texture(*in, l, tex_index, tex_w, tex_h);
+            if (st != SMR_OK) return st;
         }
         dev::LayerDev d;
         bool skip;
@@ -1726,17 +1756,14 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
     uint64_t launches = 0;
     cudaStream_t done_on = stream_;   // the stream the tick's last operation goes to
 
-    // scene.register_render_event(pts, input_resolutions), state.rs:233-239
-    std::map<std::string, Resolution> res_map;
-    for (uint32_t i = 0; i < n_in; i++)
-        if (in[i].input_id) res_map[in[i].input_id] = {in[i].width, in[i].height};
-    scene_.register_render_event(pts, std::move(res_map));
-
     struct WeightGuard {   // any return before the k_weights launch is enqueued drops this tick's new cache entries
         Renderer *r; bool armed = true;
         ~WeightGuard() { if (armed) r->rollback_weights(); }
     } weight_guard{this};
-    smr_status st = populate_inputs(pts, in, n_in);
+    smr_status st = select_inputs(pts, in, n_in, [&](Input &I, const smr_input_frame *f) {
+        I.node_tex = I.raw_tex = -1;
+        return f ? upload_input(I, *f) : SMR_OK;
+    });
     if (st != SMR_OK) return st;
     for (uint32_t i = 0; i < n_out; i++) {
         if (!out[i].output_id) return SMR_ERR_INVALID_ARGUMENT;
@@ -1938,26 +1965,11 @@ fail:
     return SMR_ERR_CUDA;
 }
 
-// inspection: what populate_inputs + register_render_event would record for this FrameSet (no copies)
+// inspection: what smr_render records for this FrameSet (select_inputs), without reading or copying the frames
 smr_status Renderer::debug_set_inputs(uint64_t pts, const smr_input_frame *in, uint32_t n_in) {
     if (n_in && !in) return SMR_ERR_INVALID_ARGUMENT;
     std::lock_guard<std::mutex> g(mu_);
-    std::map<std::string, Resolution> res_map;
-    for (uint32_t i = 0; i < n_in; i++)
-        if (in[i].input_id) res_map[in[i].input_id] = {in[i].width, in[i].height};
-    scene_.register_render_event(pts, std::move(res_map));
-    for (auto &kv : inputs_) {
-        Input &I = kv.second;
-        I.has_frame = false;
-        for (uint32_t i = 0; i < n_in; i++) {
-            if (!in[i].input_id || kv.first != in[i].input_id) continue;
-            uint64_t lim = pts > opts_.stream_fallback_timeout_ns ? pts - opts_.stream_fallback_timeout_ns : 0;
-            if (lim > in[i].pts_ns) continue;
-            I.has_frame = true;
-            I.res = {in[i].width, in[i].height};
-        }
-    }
-    return SMR_OK;
+    return select_inputs(pts, in, n_in, [](Input &, const smr_input_frame *) { return SMR_OK; });
 }
 
 smr_status Renderer::render_end() {   // retires the OLDEST tick in flight
@@ -2065,14 +2077,12 @@ smr_status Renderer::comm_exchange(const smr_input_frame *frames, uint32_t n, co
         if (f.mem_kind != SMR_MEM_DEVICE) { set_error("the exchange needs device-resident planes"); return SMR_ERR_INVALID_ARGUMENT; }
         if (roots[i] < 0 || roots[i] >= comm_size_) return SMR_ERR_INVALID_ARGUMENT;
         const uint64_t mask = ((consumers ? consumers[i] : all) | (1ull << roots[i])) & all;
-        for (int p = 0; p < 3; p++) {
-            size_t row_bytes = 0, rows = 0;
-            if (!plane_layout(f.format, f.width, f.height, p, row_bytes, rows)) continue;
-            if (!f.planes[p]) { set_error("input plane pointer is null"); return SMR_ERR_INVALID_ARGUMENT; }
-            size_t pitch = f.pitch[p] ? f.pitch[p] : row_bytes;
-            if (pitch < row_bytes) { set_error("input plane pitch is smaller than a row"); return SMR_ERR_INVALID_ARGUMENT; }
-            size_t bytes = pitch * (rows - 1) + row_bytes;
-            uint8_t *ptr = (uint8_t *)f.planes[p];
+        FrameView v;
+        if (smr_status st = read_frame(f, v); st != SMR_OK) return st;
+        for (const FrameView::Plane &P : v.plane) {
+            if (!P.p) continue;
+            const size_t bytes = P.span();
+            uint8_t *ptr = (uint8_t *)P.p;
             if ((flags & SMR_COMM_POOLED) && !runs.empty() && runs.back().root == roots[i] && runs.back().mask == mask &&
                 runs.back().p + runs.back().bytes == ptr)
                 runs.back().bytes += bytes;
@@ -2133,15 +2143,16 @@ smr_status Renderer::comm_pull(const smr_input_frame *frames, const smr_input_fr
         if (consumers && !((consumers[i] >> comm_rank_) & 1ull)) continue;
         if (f.mem_kind != SMR_MEM_DEVICE || pf.mem_kind != SMR_MEM_DEVICE) { set_error("the exchange needs device-resident planes"); return SMR_ERR_INVALID_ARGUMENT; }
         if (pf.format != f.format || pf.width != f.width || pf.height != f.height) { set_error("peer frame geometry differs"); return SMR_ERR_INVALID_ARGUMENT; }
+        FrameView v, pv;
+        st = read_frame(f, v);
+        if (st == SMR_OK) st = read_frame(pf, pv);
+        if (st != SMR_OK) return st;
         for (int p = 0; p < 3; p++) {
-            size_t row_bytes = 0, rows = 0;
-            if (!plane_layout(f.format, f.width, f.height, p, row_bytes, rows)) continue;
-            if (!f.planes[p] || !pf.planes[p]) { set_error("input plane pointer is null"); return SMR_ERR_INVALID_ARGUMENT; }
-            const size_t pitch = f.pitch[p] ? f.pitch[p] : row_bytes, ppitch = pf.pitch[p] ? pf.pitch[p] : row_bytes;
-            if (pitch != ppitch || pitch < row_bytes) { set_error("peer frame pitch differs"); return SMR_ERR_INVALID_ARGUMENT; }
-            const size_t bytes = pitch * (rows - 1) + row_bytes;
-            uint8_t *d = (uint8_t *)f.planes[p];
-            const uint8_t *sp = (const uint8_t *)pf.planes[p];
+            if (!v.plane[p].p) continue;
+            if (v.plane[p].pitch != pv.plane[p].pitch) { set_error("peer frame pitch differs"); return SMR_ERR_INVALID_ARGUMENT; }
+            const size_t bytes = v.plane[p].span();
+            uint8_t *d = (uint8_t *)v.plane[p].p;
+            const uint8_t *sp = pv.plane[p].p;
             if (!runs.empty() && runs.back().dst + runs.back().bytes == d && runs.back().src + runs.back().bytes == sp) runs.back().bytes += bytes;
             else runs.push_back({d, sp, bytes});
         }
@@ -2237,16 +2248,12 @@ smr_status Renderer::debug_layouts(const char *output_id, uint64_t pts, smr_rend
     *n = 0;
     if (!o.flat && o.node.root_is_input) { if (rw) *rw = 0; if (rh) *rh = 0; return SMR_OK; }
     OutputNode copy = o.node;  // do not advance Tiles::last_layout
+    std::vector<Input *> child_in;
     std::vector<std::optional<Resolution>> child_res;
-    for (const std::string &id : copy.child_input_ids) {
-        auto ii = inputs_.find(id);
-        if (ii != inputs_.end() && ii->second.has_frame) child_res.push_back(ii->second.res);
-        else child_res.push_back(std::nullopt);
-    }
-    Resolution root = o.flat ? o.flat_root : copy.layout_resolution(pts);
+    const Resolution root = output_children(o, copy, pts, child_in, child_res);
     if (rw) *rw = (uint32_t)root.width;
     if (rh) *rh = (uint32_t)root.height;
-    std::vector<RenderLayout> layouts = o.flat ? o.flat_layouts : copy.layouts(pts, child_res).flatten(child_res, root);
+    std::vector<RenderLayout> layouts = output_layouts(o, copy, pts, child_res, root);
     *n = (uint32_t)layouts.size();
     if (!out) return SMR_OK;
     if (cap < layouts.size()) return SMR_ERR_BUFFER_TOO_SMALL;

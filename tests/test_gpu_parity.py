@@ -605,6 +605,9 @@ def test_pitch_smaller_than_a_row_is_refused():
     arr[0].pitch[0] = 0
     out[0].pitch[1] = 100                      # chroma rows are 320 bytes
     assert r._lib.smr_render(r._h, 0, arr, 1, out, 1) == 1
+    arr[0].pitch[0] = 320                      # the frame pre-processor reads frames by the same rules
+    rgba = np.empty(640 * 360 * 4, np.uint8)
+    assert r._lib.smr_preprocess_frame(r._h, arr, 0, 0, rgba.ctypes.data, 0, F.MEM_HOST) == 1
 
 
 def glyph_like_rgba(w, h, seed):

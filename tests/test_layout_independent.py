@@ -74,6 +74,23 @@ def diff(got, exp):
     return None
 
 
+@pytest.mark.parametrize("width", [20000.0, 0.5])
+def test_root_outside_the_renderable_range(width):
+    """a root too wide to render, or one whose width truncates to 0: smr_render draws only the fallback fill, but
+    smr_debug_layouts still reports the root and its layouts as the scene defines them"""
+    scene = s.ViewComponent(position=s.Position.Static(width=width, height=300.0), children=[
+        s.ViewComponent(position=s.Position.Static(width=100.0, height=100.0), background_color=s.RGBAColor(200, 30, 30, 255)),
+        s.InputStreamComponent(input_id="input_1")])
+    r = s.Renderer(s.RendererOptions(cuda_device=-1))
+    r.register_input("input_1")
+    r.update_scene("output_1", s.Resolution(640, 360), s.OutputFrameFormat.PlanarYuv420Bytes, scene)
+    r.debug_set_inputs(0.0, {"input_1": s.Resolution(640, 360)})
+    got, root = product_layouts(r, 0.0)
+    exp_l, exp_root = LR.layouts(scene, 640, 360, {"input_1": (640, 360)})
+    assert root == exp_root and not (0 < root[0] <= 16384)
+    assert got and diff(got, ref_layouts(exp_l)) is None, diff(got, ref_layouts(exp_l))
+
+
 @pytest.mark.parametrize("module,name", CASES)
 def test_scene_catalogue_layouts(module, name):
     rec = rt.record(ref_scenes.MODULES[module][name])
