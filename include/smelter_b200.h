@@ -296,6 +296,11 @@ smr_status smr_debug_partition(const int32_t *dst_w, const int32_t *dst_h, uint3
  * bars), opaque (the interior replaces the target), job (fused resample job that could write the layer's tiles itself, -1:
  * none)}.  owner_layer[t]: the layer whose job finishes tile t directly, or -1; tiles[]: the tiles left for the composite
  * ((ty << 16) | tx), most expensive first when `sorted` != 0, row-major otherwise. */
+/* inspection (needs a device): the Lanczos3 weights the weight kernel computes for output coordinate out_coord of the
+ * mapping (scale, offset), read back: *taps of them into weights (when they fit in cap) and 1 / weight_sum into *inv. */
+smr_status smr_debug_weights(float scale, float offset, uint32_t out_coord, float *weights, uint32_t cap, uint32_t *taps,
+                             float *inv);
+
 smr_status smr_debug_tile_plan(const int32_t *boxes, uint32_t n_layers, uint32_t width, uint32_t height, int32_t sorted,
                                int32_t *owner_layer, uint32_t owner_cap, uint32_t *tiles, uint32_t tiles_cap, uint32_t *n_tiles);
 

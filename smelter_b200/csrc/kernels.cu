@@ -23,6 +23,7 @@
 #include <cstring>
 
 #include "kernels.h"
+#include "int_weights.h"
 
 namespace smr {
 namespace dev {
@@ -406,6 +407,28 @@ __global__ void k_weights(const WeightJob *jobs) {
     J.first[o] = (int)fc;
 }
 
+// k_weights of one mapping read back: the taps weights of output coordinate out_coord and its 1 / weight_sum
+int debug_weights(float scale, float offset, int out_coord, float *w_host, int cap, int *taps_out, float *inv_host) {
+    const float ks = fmaxf(scale, 1.0f);
+    const int taps = (int)ceilf(2.0f * (3.0f * ks)) + 1, n_out = out_coord + 1;
+    *taps_out = taps;
+    if (out_coord < 0 || taps > cap) return 0;
+    const size_t nw = (size_t)n_out * taps;
+    unsigned char *d = nullptr;
+    if (cudaMalloc(&d, sizeof(WeightJob) + sizeof(float) * (nw + n_out) + sizeof(int32_t) * n_out) != cudaSuccess) return -1;
+    WeightJob j{};
+    j.scale = scale; j.offset = offset; j.n_out = n_out; j.taps = taps;
+    j.weights = reinterpret_cast<float *>(d + sizeof(WeightJob));
+    j.inv_wsum = j.weights + nw;
+    j.first = reinterpret_cast<int32_t *>(j.inv_wsum + n_out);
+    bool ok = cudaMemcpy(d, &j, sizeof(j), cudaMemcpyHostToDevice) == cudaSuccess &&
+              launch_weights(reinterpret_cast<const WeightJob *>(d), &j, 1, nullptr) == 1 &&
+              cudaMemcpy(w_host, j.weights + (size_t)out_coord * taps, sizeof(float) * taps, cudaMemcpyDeviceToHost) == cudaSuccess &&
+              cudaMemcpy(inv_host, j.inv_wsum + out_coord, sizeof(float), cudaMemcpyDeviceToHost) == cudaSuccess;
+    cudaFree(d);
+    return ok ? 1 : -1;
+}
+
 int launch_weights(const WeightJob *jobs_dev, const WeightJob *jobs_host, int n, Stream s) {
     if (n <= 0) return 0;
     int max_out = 1;
@@ -526,22 +549,13 @@ int launch_resample(const ResampleJob *jobs_dev, const ResampleJob *jobs_host, i
 #define W64_WARPS 8
 #define W64_RING 64
 
+// k_resample_fused_int's weights (k_resample_tma3 has them compiled in: int_weights.h)
 __constant__ float c_wint[5][32];   // [S][tap]
 __constant__ float c_winv[5];       // 1 / weight_sum
-__constant__ float2 c_wpair[5][32]; // [S][tap] = (w[tap], w[tap - S]): the b-channel FMA pair of two adjacent output columns
 
 void set_int_weights(int S, const float *weights_dev, const float *inv_dev, int taps, Stream s) {
     cudaMemcpyToSymbolAsync(c_wint, weights_dev, sizeof(float) * taps, sizeof(float) * 32 * S, cudaMemcpyDeviceToDevice, (cudaStream_t)s);
     cudaMemcpyToSymbolAsync(c_winv, inv_dev, sizeof(float), sizeof(float) * S, cudaMemcpyDeviceToDevice, (cudaStream_t)s);
-    // (w[t], w[t - S]) pairs: two strided device-to-device copies into the float2 table (taps below S keep y = 0)
-    float *pair = nullptr;
-    cudaGetSymbolAddress((void **)&pair, c_wpair);
-    pair += 2 * 32 * S;
-    cudaMemsetAsync(pair, 0, sizeof(float2) * 32, (cudaStream_t)s);
-    cudaMemcpy2DAsync(pair, sizeof(float2), weights_dev, sizeof(float), sizeof(float), taps, cudaMemcpyDeviceToDevice, (cudaStream_t)s);
-    if (taps > S)
-        cudaMemcpy2DAsync(pair + 2 * S + 1, sizeof(float2), weights_dev, sizeof(float), sizeof(float), taps - S,
-                          cudaMemcpyDeviceToDevice, (cudaStream_t)s);
 }
 
 template <int S>   // S = 0: any ratio <= 4 (weights per column from shared memory)
@@ -959,7 +973,8 @@ static bool launch_tma0_src(int src, int box, const FusedJob *jobs_dev, const Fu
 }
 
 template <int S, int SRC>
-static bool launch_tma3(const FusedJob *jobs_dev, const FusedPiece *pieces, const int *piece_begin, int nblocks, cudaStream_t s) {
+static bool launch_tma3(const FusedJob *jobs_dev, const FusedPiece *pieces, const int *piece_begin, int nblocks, int full_range,
+                        cudaStream_t s) {
     static std::atomic<unsigned long long> done{0};
     int dev = 0;
     cudaGetDevice(&dev);
@@ -969,12 +984,13 @@ static bool launch_tma3(const FusedJob *jobs_dev, const FusedPiece *pieces, cons
         done.fetch_or(bit, std::memory_order_release);
     }
     const int grid = (nblocks + tma_int::kGroups - 1) / tma_int::kGroups;   // the host cut the work for `nblocks` eight-warp groups
-    tma_int::k_resample_tma3<S, SRC><<<grid, dim3(32, tma::kWarps * tma_int::kGroups), tma_int::Cfg<S>::SMEM, s>>>(jobs_dev, pieces, piece_begin, nblocks);
+    tma_int::k_resample_tma3<S, SRC><<<grid, dim3(32, tma::kWarps * tma_int::kGroups), tma_int::Cfg<S>::SMEM, s>>>(jobs_dev, pieces, piece_begin, nblocks,
+                                                                                                            full_range);
     return check_launch("k_resample_tma3");
 }
 
 // src: 0 planar 4:2:0, 1 NV12, 2 UYVY, 3 YUYV (fused_source_class)
-int launch_resample_fused(const FusedKernel &k, int src, const FusedJob *jobs_dev, const FusedPiece *pieces_dev,
+int launch_resample_fused(const FusedKernel &k, int src, int full_range, const FusedJob *jobs_dev, const FusedPiece *pieces_dev,
                           const int *piece_begin_dev, int nblocks, Stream s) {
     if (nblocks <= 0) return 0;
     cudaStream_t st = (cudaStream_t)s;
@@ -995,10 +1011,10 @@ int launch_resample_fused(const FusedKernel &k, int src, const FusedJob *jobs_de
             }
             break;
         case FusedKernel::TMA_INT:
-            if (k.ratio == 4) ok = src == 1 ? launch_tma3<4, 1>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, st)
-                                            : launch_tma3<4, 0>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, st);
-            else ok = src == 1 ? launch_tma3<2, 1>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, st)
-                               : launch_tma3<2, 0>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, st);
+            if (k.ratio == 4) ok = src == 1 ? launch_tma3<4, 1>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, full_range, st)
+                                            : launch_tma3<4, 0>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, full_range, st);
+            else ok = src == 1 ? launch_tma3<2, 1>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, full_range, st)
+                               : launch_tma3<2, 0>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, full_range, st);
             break;
         default:
             switch (k.ratio) {

@@ -134,7 +134,7 @@ struct FusedJob {
     const int32_t *first_v;
     // TMA kernels: device copies of the CUtensorMap of each source plane (luma; NV12 chroma as u16 texels, or U; V)
     const void *tm0, *tm1, *tm2;
-    int32_t v_same;         // TMA kernels: the vertical mapping is the same integer ratio with zero offset (weights = c_wint[S])
+    int32_t v_same;         // TMA kernels: the vertical mapping is the same integer ratio with zero offset (weights = int_weight<S>)
     int32_t strip_cols;     // any-ratio TMA kernel: output columns per strip of THIS job (<= 64, even)
     const uint8_t *lane_perm;   // any-ratio TMA kernel: [strip][32] which pair of the strip's columns each lane owns (nullptr: lane l owns pair l)
     // integer-ratio TMA kernel with v_same: K10 / K11 straight out of the vertical pass.  Where the child is shown 1:1, opaque and
@@ -164,11 +164,12 @@ constexpr int kTmaLumaBoxW = 136, kTmaLumaBoxH = 32, kTmaNv12BoxW = 144, kTmaPla
 constexpr int kTma0Groups = 2, kTma0MaxSpan = 256, kTma0MaxTaps = 25;
 constexpr int kTma0Window[4] = {20, 25, 29, 33};
 
-// Which kernel resamples a FusedJob (host side only; every job of one launch has the same kernel and source class)
+// Which kernel resamples a FusedJob (host side only; every job of one launch has the same kernel, source class and
+// launch range)
 struct FusedKernel {
     enum Kind : int32_t {
         LDG,      // k_resample_fused_int: LDG-staged, weights from smem (ratio 0) or the constant bank (integer ratio 2 / 3 / 4)
-        TMA_INT,  // k_resample_tma3 (resample_tma3.cuh): integer ratio 2 / 4, TMA-staged
+        TMA_INT,  // k_resample_tma3 (resample_tma3.cuh): integer ratio 2 / 4, TMA-staged, weights from int_weights.h
         TMA_ANY,  // k_resample_tma0 (resample_tma0.cuh): any ratio <= 4, TMA-staged, a tap loop of kTma0Window[window] slots;
                   // with `box` on a source box-reduced 2:1
     } kind = LDG;
@@ -178,6 +179,11 @@ struct FusedKernel {
 // What a launch of a fused kernel needs to know: output columns per strip of job `j`, blocks (eight-warp groups) per SM
 // of the persistent grid, and the rows a block's share of the partition is a multiple of
 struct FusedShape { int strip_cols, groups_per_sm, row_gran; };
+// The source range a launch of kernel k is specialised for: the integer-ratio TMA kernel builds a luma table for one
+// range (1 full, 0 limited), so its launches are single-range; every other kernel reads the range per job (0)
+inline int fused_launch_range(const FusedKernel &k, const FusedJob &j) {
+    return k.kind == FusedKernel::TMA_INT && j.src.full_range ? 1 : 0;
+}
 inline FusedShape fused_shape(const FusedKernel &k, const FusedJob &j) {
     switch (k.kind) {
         case FusedKernel::TMA_INT: return {k.ratio == 4 ? kTmaStripCols4 : kTmaStripCols2, 3, 2};
@@ -229,6 +235,9 @@ typedef void *Stream;  // cudaStream_t
 // each returns the number of kernels it launched (for smr_stats / bench gpu_launches)
 int launch_convert_to_rgba(const Tex &src, uint8_t *dst, int dst_pitch, Stream s);
 int launch_weights(const WeightJob *jobs_dev, const WeightJob *jobs_host, int n_jobs, Stream s);
+// k_weights for one mapping on the current device, synchronously: output coordinate out_coord's weights (*taps of them,
+// when they fit in cap) and 1 / weight_sum.  1 done, 0 cap too small, -1 CUDA error
+int debug_weights(float scale, float offset, int out_coord, float *w_host, int cap, int *taps, float *inv_host);
 int launch_resample(const ResampleJob *jobs_dev, const ResampleJob *jobs_host, int n_jobs, Stream s);
 // source class of the fused kernel's template: 0 planar 4:2:0, 1 NV12, 2 UYVY, 3 YUYV; -1 not supported
 inline int fused_source_class(int tex_kind) {
@@ -238,9 +247,11 @@ inline int fused_source_class(int tex_kind) {
 int launch_preprocess(const Tex &src, int mode, int rescale, uint8_t *out, int out_pitch, int out_w, int out_h, Stream s);
 // text node texture: clear + glyph quads alpha-blended in list order
 int launch_text(const TextJob &job, Stream s);
-int launch_resample_fused(const FusedKernel &k, int src, const FusedJob *jobs_dev, const FusedPiece *pieces_dev,
+// full_range: fused_launch_range of every job of the launch
+int launch_resample_fused(const FusedKernel &k, int src, int full_range, const FusedJob *jobs_dev, const FusedPiece *pieces_dev,
                           const int *piece_begin_dev, int nblocks, Stream s);
-// integer-ratio LDG kernel: the (single-phase) weight row of ratio S goes to constant memory, once per mapping
+// integer-ratio LDG kernel: the (single-phase) weight row of ratio S goes to constant memory, once per mapping (the
+// TMA kernel has it compiled in: int_weights.h)
 void set_int_weights(int S, const float *weights_dev, const float *inv_dev, int taps, Stream s);
 // every output of a tick in one launch; jobs_dev[i] == jobs_host[i], layers / masks / textures device pointers.  One output
 // with a short layer list (layers0_host: host copy of jobs_host[0].layers) passes job and layers in the parameter block

@@ -1811,21 +1811,26 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
         if (c.out_frame_off != SIZE_MAX) c.job.out0 = fb + c.out_frame_off;
 
     // ---- pack the parameter arena and ship it in one copy -------------------------------------
-    // partition the fused resamples of the tick over a persistent grid, one launch per kernel and source class
-    struct FusedLaunch { dev::FusedKernel kernel; int src; size_t pieces_off, begin_off; int nblocks; };
+    // partition the fused resamples of the tick over a persistent grid, one launch per kernel, source class and launch range
+    struct FusedKey {
+        dev::FusedKernel kernel; int src, range;
+        bool operator==(const FusedKey &o) const { return kernel == o.kernel && src == o.src && range == o.range; }
+    };
+    auto key_of = [](const FusedRec &f) {
+        return FusedKey{f.kernel, dev::fused_source_class(f.job.src.kind), dev::fused_launch_range(f.kernel, f.job)};
+    };
+    struct FusedLaunch { FusedKey key; size_t pieces_off, begin_off; int nblocks; };
     std::vector<FusedLaunch> fused_launches;
     {
-        std::vector<std::pair<dev::FusedKernel, int>> kernels;
-        for (const FusedRec &f : plan_.fused) {
-            std::pair<dev::FusedKernel, int> v{f.kernel, dev::fused_source_class(f.job.src.kind)};
-            if (std::find(kernels.begin(), kernels.end(), v) == kernels.end()) kernels.push_back(v);
-        }
-        for (auto &v : kernels) {
+        std::vector<FusedKey> keys;
+        for (const FusedRec &f : plan_.fused)
+            if (std::find(keys.begin(), keys.end(), key_of(f)) == keys.end()) keys.push_back(key_of(f));
+        for (const FusedKey &v : keys) {
             std::vector<int> idx, widths, heights, cols;
             dev::FusedShape shape{};
             for (size_t ji = 0; ji < plan_.fused.size(); ji++) {
                 const FusedRec &f = plan_.fused[ji];
-                if (!(f.kernel == v.first) || dev::fused_source_class(f.job.src.kind) != v.second) continue;
+                if (!(key_of(f) == v)) continue;
                 shape = dev::fused_shape(f.kernel, f.job);
                 idx.push_back((int)ji); widths.push_back(f.job.dst_w); heights.push_back(f.job.dst_h); cols.push_back(shape.strip_cols);
             }
@@ -1846,7 +1851,7 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
                                 pc.list.push_back((uint32_t)(t % (size_t)pc.job.map_w) | ((uint32_t)(t / (size_t)pc.job.map_w) << 16));
                             }
                 }
-            fused_launches.push_back({v.first, v.second, param_put(pieces.data(), sizeof(dev::FusedPiece) * pieces.size()),
+            fused_launches.push_back({v, param_put(pieces.data(), sizeof(dev::FusedPiece) * pieces.size()),
                                       param_put(begin.data(), sizeof(int) * begin.size()), (int)begin.size() - 1});
         }
     }
@@ -1915,7 +1920,7 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
     new_weight_keys_.clear();
     weight_guard.armed = false;   // the tables are being computed on the stream: the cache entries are good
     for (const FusedLaunch &fl : fused_launches) {
-        if (!launched(dev::launch_resample_fused(fl.kernel, fl.src, (const dev::FusedJob *)(pd + fj_off),
+        if (!launched(dev::launch_resample_fused(fl.key.kernel, fl.key.src, fl.key.range, (const dev::FusedJob *)(pd + fj_off),
                                                  (const dev::FusedPiece *)(pd + fl.pieces_off), (const int *)(pd + fl.begin_off),
                                                  fl.nblocks, stream_))) goto fail;
         prof_mark(SMR_KERNEL_RESAMPLE_FUSED);
@@ -2348,6 +2353,13 @@ smr_status smr_debug_partition(const int32_t *dst_w, const int32_t *dst_h, uint3
     }
     for (size_t i = 0; i < bg.size(); i++) begin[i] = bg[i];
     return SMR_OK;
+}
+smr_status smr_debug_weights(float scale, float offset, uint32_t out_coord, float *weights, uint32_t cap, uint32_t *taps, float *inv) {
+    if (!weights || !taps || !inv || out_coord > (1u << 24)) return SMR_ERR_INVALID_ARGUMENT;
+    int n = 0;
+    const int rc = smr::dev::debug_weights(scale, offset, (int)out_coord, weights, (int)cap, &n, inv);
+    *taps = (uint32_t)n;
+    return rc > 0 ? SMR_OK : rc == 0 ? SMR_ERR_BUFFER_TOO_SMALL : SMR_ERR_CUDA;
 }
 smr_status smr_preprocess_frame(smr_renderer *r, const smr_input_frame *f, uint32_t ow, uint32_t oh, void *rgba, uint32_t pitch,
                                 int32_t mem_kind) { SMR_GUARD(r->impl.preprocess_frame(f, ow, oh, rgba, pitch, mem_kind)) }

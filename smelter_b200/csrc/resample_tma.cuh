@@ -46,6 +46,10 @@ constexpr int kKaddrOff = kBarOff + 64;
 constexpr int kStashOff = kBarOff + 128;
 constexpr int kStashBytes = 1024;
 constexpr int kTailBytes = kStashOff + kStashBytes;
+// the luma table of the integer-ratio kernel, behind the tail: K1/K2 luma of every byte for the launch's range, 16
+// copies (entry n of copy c at word 16 n + c, lane l reads copy l % 16), so two lanes at most share a bank
+constexpr int kLumaRep = 16;
+constexpr int kLumaTabBytes = 256 * kLumaRep * 4;
 
 // strips of the integer-ratio kernel: output columns per strip, and the offset that makes the tile's first source pixel
 // first_h(strip) - kLead<S> even
@@ -293,11 +297,35 @@ __device__ __forceinline__ void fetch_row(uint32_t sb, const LaneWords<NV12> &lw
     }
 }
 
+// exact n / 255 of a byte n held as a float: fma(n, c, n * lo)
+constexpr uint32_t kDiv255C = 0x3b808081u, kDiv255Lo = 0xaf7efeffu;
+
+// K1/K2 luma of byte n (ny = n as a float): clamp01((n / 255 - 16/255) * rcp_y), or n / 255 for a full range source
+// (nk16 = 0, rcp_y = 1) -- each operation is one component of convert_pair's pair arithmetic
+__device__ __forceinline__ float luma_of(float ny, float nk16, float rcp_y) {
+    const float y = __fmaf_rn(ny, __uint_as_float(kDiv255C), __fmul_rn(ny, __uint_as_float(kDiv255Lo)));
+    return __saturatef(__fmul_rn(__fadd_rn(y, nk16), rcp_y));
+}
+
+// The luma table behind the tail (kLumaTabBytes, filled by the block before its first __syncthreads) and this lane's
+// lookup base: the entry of byte n is [(float bits of (n + 2^23)) << 6 + base]  (mod 2^32), so that the PRMT which puts
+// the byte under the exponent of 2^23 plus one LEA make the address.
+__device__ __forceinline__ void fill_luma_table(unsigned char *tail, float nk16, float rcp_y) {
+    float *s_y = reinterpret_cast<float *>(tail + kTailBytes);
+    const int btid = threadIdx.y * 32 + threadIdx.x, bn = blockDim.x * blockDim.y;
+    for (int i = btid; i < 256 * kLumaRep; i += bn) s_y[i] = luma_of((float)(i / kLumaRep), nk16, rcp_y);
+}
+__device__ __forceinline__ uint32_t luma_base(unsigned char *tail) {
+    return smem_u32(tail + kTailBytes) - (0x4B000000u << 6) + 4u * (threadIdx.x % kLumaRep);
+}
+
 // K1/K2 -> u8 of pixels 2p and 2p + 1 of an 8-pixel run (yw: its luma bytes, v: its combined chroma as fetch_row makes it),
 // two pixels per instruction: q = 1.5 * 2^23 + the byte.  nk16, rcp_y, rcp_c: -16/255 and the limited-range scales, or
-// 0, 1, 1 for a full-range source.
+// 0, 1, 1 for a full-range source.  YTAB: the luma comes from the luma table (ybase from luma_base, filled for the same
+// nk16 and rcp_y) instead of the arithmetic.
+template <bool YTAB = false>
 __device__ __forceinline__ void convert_pair(const uint32_t (&yw)[2], const uint32_t (&v)[6], int p, float nk16, float rcp_y,
-                                             float rcp_c, float2 &qr, float2 &qg, float2 &qb) {
+                                             float rcp_c, float2 &qr, float2 &qg, float2 &qb, uint32_t ybase = 0) {
     // 16 x chroma of the even / odd pixel of the pair (NC-6u with the .25 / .75 taps)
     const uint32_t ne = v[p] + 3u * v[p + 1], no = 3u * v[p + 1] + v[p + 2];
     const float m23 = -8388608.0f;
@@ -306,17 +334,24 @@ __device__ __forceinline__ void convert_pair(const uint32_t (&yw)[2], const uint
     float2 nv = add2(make_float2(__uint_as_float(__byte_perm(ne, 0x4B000000u, 0x7632)),
                                  __uint_as_float(__byte_perm(no, 0x4B000000u, 0x7632))), splat(m23));
     const uint32_t ywd = yw[p >> 1];
-    float2 ny = add2(make_float2(__uint_as_float(__byte_perm(ywd, 0x4B000000u, (p & 1) ? 0x7642 : 0x7640)),
-                                 __uint_as_float(__byte_perm(ywd, 0x4B000000u, (p & 1) ? 0x7643 : 0x7641))), splat(m23));
+    const uint32_t by0 = __byte_perm(ywd, 0x4B000000u, (p & 1) ? 0x7642 : 0x7640);
+    const uint32_t by1 = __byte_perm(ywd, 0x4B000000u, (p & 1) ? 0x7643 : 0x7641);
     // exact n / 255 and n / (255 * 16): fma(n, c, n * lo)
-    const float c1 = __uint_as_float(0x3b808081u), lo1 = __uint_as_float(0xaf7efeffu);
+    const float c1 = __uint_as_float(kDiv255C), lo1 = __uint_as_float(kDiv255Lo);
     const float c16 = __uint_as_float(0x39808081u), lo16 = __uint_as_float(0xad7efeffu);
-    float2 y = fma2(ny, splat(c1), mul2(ny, splat(lo1)));
+    float2 y;
+    if (YTAB) {
+        y = make_float2(lds_tab((by0 << 6) + ybase), lds_tab((by1 << 6) + ybase));
+    } else {
+        const float2 ny = add2(make_float2(__uint_as_float(by0), __uint_as_float(by1)), splat(m23));
+        y = fma2(ny, splat(c1), mul2(ny, splat(lo1)));
+    }
     float2 u = fma2(nu, splat(c16), mul2(nu, splat(lo16)));
     float2 w = fma2(nv, splat(c16), mul2(nv, splat(lo16)));
     // limited range: clamp01((x - 16/255) * rcp); full range: (x - 0) * 1 and the clamp are identities on [0, 1]
-    y = add2(y, splat(nk16)); u = add2(u, splat(nk16)); w = add2(w, splat(nk16));
-    y = make_float2(__saturatef(y.x * rcp_y), __saturatef(y.y * rcp_y));
+    if (!YTAB) y = add2(y, splat(nk16));
+    u = add2(u, splat(nk16)); w = add2(w, splat(nk16));
+    if (!YTAB) y = make_float2(__saturatef(y.x * rcp_y), __saturatef(y.y * rcp_y));
     u = make_float2(__saturatef(u.x * rcp_c), __saturatef(u.y * rcp_c));
     w = make_float2(__saturatef(w.x * rcp_c), __saturatef(w.y * rcp_c));
     const float2 um = add2(u, splat(-0.5f)), vm = add2(w, splat(-0.5f));
@@ -332,13 +367,14 @@ __device__ __forceinline__ void convert_pair(const uint32_t (&yw)[2], const uint
 }
 
 // K1/K2 -> u8 -> sRGB decode of the node-texture fetch (NC-3) of an 8-pixel run: (r, g) and b of pixel i, looked up in
-// this lane's copy of the decode table (kaddr from setup_block)
+// this lane's copy of the decode table (kaddr from setup_block); YTAB, ybase: as in convert_pair
+template <bool YTAB = false>
 __device__ __forceinline__ void convert_run(const uint32_t (&yw)[2], const uint32_t (&v)[6], float nk16, float rcp_y, float rcp_c,
-                                            uint32_t kaddr, float2 (&prg)[8], float (&pb)[8]) {
+                                            uint32_t kaddr, float2 (&prg)[8], float (&pb)[8], uint32_t ybase = 0) {
 #pragma unroll
     for (int p = 0; p < 4; p++) {
         float2 qr, qg, qb;
-        convert_pair(yw, v, p, nk16, rcp_y, rcp_c, qr, qg, qb);
+        convert_pair<YTAB>(yw, v, p, nk16, rcp_y, rcp_c, qr, qg, qb, ybase);
         prg[2 * p] = make_float2(lds_tab((__float_as_uint(qr.x) << 7) + kaddr), lds_tab((__float_as_uint(qg.x) << 7) + kaddr));
         prg[2 * p + 1] = make_float2(lds_tab((__float_as_uint(qr.y) << 7) + kaddr), lds_tab((__float_as_uint(qg.y) << 7) + kaddr));
         pb[2 * p] = lds_tab((__float_as_uint(qb.x) << 7) + kaddr);

@@ -45,12 +45,12 @@ struct Cfg {
     static constexpr int RROW_BYTES = 32 * 3 * OUT * 4;
     static constexpr int RING_BYTES = RROWS * RROW_BYTES;
     static constexpr int GROUP_BYTES = kStageBytes + RING_BYTES;   // ONE stage: it is refilled while the vertical pass runs
-    static constexpr int SMEM = kGroups * GROUP_BYTES + kTailBytes;
+    static constexpr int SMEM = kGroups * GROUP_BYTES + kTailBytes + kLumaTabBytes;
 };
 
 template <int S, int SRC>
 __global__ void __launch_bounds__(32 * kWarps * kGroups, 1) k_resample_tma3(const FusedJob *jobs, const FusedPiece *pieces, const int *piece_begin,
-                                                                            int n_virtual_blocks) {
+                                                                            int n_virtual_blocks, int full_range) {
     using K = Cfg<S>;
     using It = ChunkIter<S, 1>;
     constexpr int P = K::P, OUT = K::OUT, TAPS = K::TAPS, A = K::A, NST = K::NST;
@@ -63,7 +63,10 @@ __global__ void __launch_bounds__(32 * kWarps * kGroups, 1) k_resample_tma3(cons
     const uint32_t stage0 = smem_u32(smem);
     float *ring = reinterpret_cast<float *>(smem + kStageBytes);
     const uint32_t bar0 = smem_u32(tail + kBarOff) + 16u * (uint32_t)grp;
-    const uint32_t kaddr = setup_block<kGroups>(tail, [] {});
+    // every source of the launch has the range full_range (the host keys the launches by it): the luma table is the block's
+    const float nk16 = full_range ? 0.0f : -K16, rcp_y = full_range ? 1.0f : RCP_Y, rcp_c = full_range ? 1.0f : RCP_C;
+    const uint32_t kaddr = setup_block<kGroups>(tail, [&] { fill_luma_table(tail, nk16, rcp_y); });
+    const uint32_t ybase = luma_base(tail);
     const int vb = blockIdx.x * kGroups + grp;         // the host cut the launch for SMs x 3 eight-warp blocks
     if (vb >= n_virtual_blocks) return;
 
@@ -86,8 +89,6 @@ __global__ void __launch_bounds__(32 * kWarps * kGroups, 1) k_resample_tma3(cons
         const bool cur_tma = cur.nrows > 0;
         const FusedJob &J = jobs[cur.job];
         const int W = J.src.width, H = J.src.height, chei = H >> 1;
-        const bool full_range = J.src.full_range != 0;
-        const float nk16 = full_range ? 0.0f : -K16, rcp_y = full_range ? 1.0f : RCP_Y, rcp_c = full_range ? 1.0f : RCP_C;
         const uint32_t sb = stage0;
         if (cur_tma) {
             mbar_wait(bar0, nchunk & 1u);
@@ -97,11 +98,12 @@ __global__ void __launch_bounds__(32 * kWarps * kGroups, 1) k_resample_tma3(cons
             for (int r = cur.r0 + warp; r < cur.r0 + cur.nrows; r += kWarps) {
                 uint32_t yw[2], v[6];
                 fetch_row<NV12>(sb, lw, r, cur.r0, chei, yw, v);
-                // A1: K1/K2 -> u8 -> sRGB decode, two pixels per instruction
+                // A1: K1/K2 -> u8 -> sRGB decode, two pixels per instruction, luma from the luma table
                 float2 prg[P];   // (r, g) of pixel i
                 float pb[P];     // b of pixel i
-                convert_run(yw, v, nk16, rcp_y, rcp_c, kaddr, prg, pb);
-                // A2: horizontal Lanczos along the warp.  acc j of the lane that owns tap 0 of output OUT * lane + j
+                convert_run<true>(yw, v, nk16, rcp_y, rcp_c, kaddr, prg, pb, ybase);
+                // A2: horizontal Lanczos along the warp.  acc j of the lane that owns tap 0 of output OUT * lane + j.
+                // The weights are compile-time constants (int_weights.h): every FFMA takes its weight as an immediate.
                 float2 arg[OUT];          // (r, g)
                 float ab[OUT];            // b
 #pragma unroll
@@ -113,19 +115,9 @@ __global__ void __launch_bounds__(32 * kWarps * kGroups, 1) k_resample_tma3(cons
 #pragma unroll
                         for (int j = 0; j < OUT; j++) {
                             const int t = P * s + i - A - S * j;   // compile-time after unrolling
-                            if (t >= 0 && t < TAPS) arg[j] = fma2(prg[i], splat(c_wint[S][t]), arg[j]);
-                        }
-#pragma unroll
-                        for (int j = 0; j < OUT; j += 2) {
-                            const int t0 = P * s + i - A - S * j, t1 = t0 - S;
-                            const bool a0 = t0 >= 0 && t0 < TAPS, a1 = t1 >= 0 && t1 < TAPS;
-                            if (a0 && a1) {
-                                const float2 d = fma2(splat(pb[i]), c_wpair[S][a0 ? t0 : 0], make_float2(ab[j], ab[j + 1]));
-                                ab[j] = d.x; ab[j + 1] = d.y;
-                            } else if (a0) {
-                                ab[j] = fmaf(pb[i], c_wint[S][a0 ? t0 : 0], ab[j]);
-                            } else if (a1) {
-                                ab[j + 1] = fmaf(pb[i], c_wint[S][a1 ? t1 : 0], ab[j + 1]);
+                            if (t >= 0 && t < TAPS) {
+                                arg[j] = fma2(prg[i], splat(int_weight<S>(t)), arg[j]);
+                                ab[j] = __fmaf_rn(pb[i], int_weight<S>(t), ab[j]);
                             }
                         }
                     }
@@ -141,7 +133,7 @@ __global__ void __launch_bounds__(32 * kWarps * kGroups, 1) k_resample_tma3(cons
                 }
                 // normalise, quantise to f16 (NC-5) and park the row in the ring: [row][lane][channel][j]
                 {
-                    const float inv = c_winv[S];
+                    constexpr float inv = int_inv<S>();
                     float *dst = ring + (size_t)(r % K::RROWS) * (K::RROW_BYTES / 4) + lane * 3 * OUT;
 #pragma unroll
                     for (int j = 0; j < OUT; j += 2) {
@@ -208,7 +200,7 @@ __global__ void __launch_bounds__(32 * kWarps * kGroups, 1) k_resample_tma3(cons
             if (J.v_same) {
                 // same integer ratio vertically: rows o and o + 1 share TAPS - S of their TAPS ring rows.  Four warps (one
                 // per scheduler) take two output rows each: every ring row is loaded once for both, the weights are the
-                // constant-bank row, the loop unrolls; the ring wraps at most once inside the window.
+                // compile-time row of int_weights.h, the loop unrolls; the ring wraps at most once inside the window.
                 if (warp < kWarps / 2) {
                     const int oa = cur.o0 + 2 * warp, ob = oa + 1;
                     const int fa = __ldg(J.first_v) + S * oa;               // first_v(oa); first_v(ob) = fa + S
@@ -228,11 +220,11 @@ __global__ void __launch_bounds__(32 * kWarps * kGroups, 1) k_resample_tma3(cons
                             for (int k = 0; k < 3 * OUT / 2; k++) v[k] = *reinterpret_cast<const float2 *>(p + 2 * k);
                             if (u < TAPS) {
 #pragma unroll
-                                for (int k = 0; k < 3 * OUT / 2; k++) aa[k] = fma2(v[k], splat(c_wint[S][u < TAPS ? u : 0]), aa[k]);
+                                for (int k = 0; k < 3 * OUT / 2; k++) aa[k] = fma2(v[k], splat(int_weight<S>(u < TAPS ? u : 0)), aa[k]);
                             }
                             if (u >= S) {
 #pragma unroll
-                                for (int k = 0; k < 3 * OUT / 2; k++) bb2[k] = fma2(v[k], splat(c_wint[S][u >= S ? u - S : 0]), bb2[k]);
+                                for (int k = 0; k < 3 * OUT / 2; k++) bb2[k] = fma2(v[k], splat(int_weight<S>(u >= S ? u - S : 0)), bb2[k]);
                             }
                         }
                         uint32_t pa[OUT], pb[OUT];
