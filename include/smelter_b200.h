@@ -150,6 +150,11 @@ typedef struct {                   /* one entry of FrameSet<InputId> */
     uint32_t pitch[3];             /* bytes per row */
     int32_t mem_kind;              /* smr_mem_kind; DEVICE = zero-copy (Nv12WgpuTexture analogue) */
 } smr_input_frame;
+/* Alignment of SMR_MEM_DEVICE planes (pointer and pitch alike; SMR_ERR_INVALID_ARGUMENT otherwise):
+ *  - 4-byte texel formats (RGBA8, BGRA, ARGB, UYVY, YUYV): 4-byte aligned.
+ *  - Planar 4:2:0 (YUV420, YUVJ420) and NV12: the luma plane, and the NV12 chroma plane, 2-byte aligned (the kernels
+ *    read pixel pairs and {u, v} pairs); planar U and V planes may start at any byte.
+ * Host planes are copied into aligned buffers and have no such rule. */
 
 typedef enum {                     /* OutputFrameFormat, types.rs:187-194 */
     SMR_OUT_PLANAR_YUV420 = 0,     /* PlanarYuv420Bytes */
@@ -303,6 +308,30 @@ smr_status smr_debug_weights(float scale, float offset, uint32_t out_coord, floa
 
 smr_status smr_debug_tile_plan(const int32_t *boxes, uint32_t n_layers, uint32_t width, uint32_t height, int32_t sorted,
                                int32_t *owner_layer, uint32_t owner_cap, uint32_t *tiles, uint32_t tiles_cap, uint32_t *n_tiles);
+
+/* inspection (no device access): the fused resample jobs of the handle's most recently planned tick, one record per job in
+ * plan order, as they were launched -- after the partition, so `direct` already reflects a job sent back to the
+ * composite because its piece of the launch was cut at an odd row.  *n is the job count; records go to `out` when they
+ * fit in cap (SMR_ERR_BUFFER_TOO_SMALL otherwise; out = NULL asks for the count). */
+typedef enum {
+    SMR_FUSED_LDG = 0,             /* k_resample_fused_int<ratio, src_class> */
+    SMR_FUSED_TMA_INT = 1,         /* k_resample_tma3<ratio, src_class> */
+    SMR_FUSED_TMA_ANY = 2          /* k_resample_tma0<src_class, window, box> */
+} smr_fused_kernel;
+typedef struct {
+    int32_t kernel;                /* smr_fused_kernel */
+    int32_t ratio;                 /* template ratio: 2 / 3 / 4, or 0 (any ratio; always 0 for SMR_FUSED_TMA_ANY) */
+    int32_t window;                /* SMR_FUSED_TMA_ANY: slots of a lane's tap window (20, 25, 29 or 33); else 0 */
+    int32_t box;                   /* SMR_FUSED_TMA_ANY: 1 when the source is box-reduced 2:1 on the fly */
+    int32_t src_class;             /* 0 planar 4:2:0, 1 NV12, 2 UYVY, 3 YUYV */
+    int32_t full_range;            /* the source's range (1 full, 0 limited) */
+    int32_t v_same;                /* SMR_FUSED_TMA_INT: the vertical mapping is the horizontal one (compiled-in weights) */
+    int32_t strip_cols;            /* output columns per strip of the launch's partition */
+    uint32_t src_width, src_height, dst_width, dst_height;
+    int32_t taps_h, taps_v;
+    int32_t direct;                /* the job writes the output bytes of its direct tiles itself */
+} smr_fused_job_info;
+smr_status smr_debug_fused_jobs(smr_renderer *r, smr_fused_job_info *out, uint32_t cap, uint32_t *n);
 
 /* byte sizes of the planes smr_render writes for an output (0 for unused planes) */
 smr_status smr_output_plane_sizes(uint32_t width, uint32_t height, int32_t output_format, size_t sizes[3]);

@@ -117,6 +117,16 @@ class Stats(C.Structure):
                 ("d2h_bytes", C.c_uint64), ("last_render_kernel_launches", C.c_uint64), ("last_render_direct_tiles", C.c_uint64)]
 
 
+FUSED_LDG, FUSED_TMA_INT, FUSED_TMA_ANY = 0, 1, 2
+
+
+class FusedJobInfo(C.Structure):   # smr_fused_job_info
+    _fields_ = [("kernel", C.c_int32), ("ratio", C.c_int32), ("window", C.c_int32), ("box", C.c_int32),
+                ("src_class", C.c_int32), ("full_range", C.c_int32), ("v_same", C.c_int32), ("strip_cols", C.c_int32),
+                ("src_width", C.c_uint32), ("src_height", C.c_uint32), ("dst_width", C.c_uint32), ("dst_height", C.c_uint32),
+                ("taps_h", C.c_int32), ("taps_v", C.c_int32), ("direct", C.c_int32)]
+
+
 KERNEL_CLASSES = ["convert", "weights", "resample_box", "resample_first", "resample_last", "composite", "output",
                   "fill", "resample_fused"]
 
@@ -127,7 +137,7 @@ class KernelTimes(C.Structure):
 
 EXPORTS = [
     "smr_create", "smr_destroy", "smr_register_input", "smr_unregister_input", "smr_update_scene",
-    "smr_unregister_output", "smr_set_layouts", "smr_render", "smr_render_begin", "smr_render_end", "smr_preprocess_frame", "smr_premultiply_rgba8", "smr_render_text", "smr_debug_partition", "smr_debug_tile_plan", "smr_debug_weights", "smr_output_plane_sizes",
+    "smr_unregister_output", "smr_set_layouts", "smr_render", "smr_render_begin", "smr_render_end", "smr_preprocess_frame", "smr_premultiply_rgba8", "smr_render_text", "smr_debug_partition", "smr_debug_tile_plan", "smr_debug_weights", "smr_debug_fused_jobs", "smr_output_plane_sizes",
     "smr_component_default", "smr_debug_layouts", "smr_debug_set_inputs", "smr_get_stats", "smr_set_profiling", "smr_get_kernel_times",
     "smr_comm_get_unique_id", "smr_comm_init", "smr_comm_broadcast_inputs", "smr_comm_exchange_inputs", "smr_comm_pull_inputs", "smr_peer_pool_alloc", "smr_peer_pool_open", "smr_peer_pool_close", "smr_peer_pool_free", "smr_comm_destroy", "smr_host_register", "smr_host_unregister", "smr_cuda_stream", "smr_last_error",
     "smr_version",
@@ -173,6 +183,8 @@ def lib():
     L.smr_debug_weights.argtypes = [C.c_float, C.c_float, C.c_uint32, C.POINTER(C.c_float), C.c_uint32, C.POINTER(C.c_uint32),
                                     C.POINTER(C.c_float)]
     L.smr_debug_weights.restype = C.c_int32
+    L.smr_debug_fused_jobs.argtypes = [vp, C.POINTER(FusedJobInfo), C.c_uint32, C.POINTER(C.c_uint32)]
+    L.smr_debug_fused_jobs.restype = C.c_int32
     L.smr_output_plane_sizes.argtypes = [C.c_uint32, C.c_uint32, C.c_int32, C.POINTER(C.c_size_t * 3)]
     L.smr_component_default.argtypes = [C.c_int32, C.POINTER(Component)]
     L.smr_component_default.restype = None

@@ -283,6 +283,7 @@ class Renderer {
     smr_status debug_set_inputs(uint64_t pts, const smr_input_frame *in, uint32_t n_in);
     smr_status debug_layouts(const char *output_id, uint64_t pts, smr_render_layout *out, uint32_t cap, uint32_t *n,
                              uint32_t *rw, uint32_t *rh);
+    smr_status debug_fused_jobs(smr_fused_job_info *out, uint32_t cap, uint32_t *n);
     void stats(smr_stats *s) { std::lock_guard<std::mutex> g(mu_); *s = stats_; }
     void *stream() { return (void *)stream_; }
     const char *last_error() { return err_.c_str(); }
@@ -760,6 +761,9 @@ smr_status Renderer::read_frame(const smr_input_frame &f, FrameView &v) {
     // the kernels read these as one 4-byte word per texel
     const bool texel4 = f.format == SMR_FRAME_UYVY422 || f.format == SMR_FRAME_YUYV422 || f.format == SMR_FRAME_RGBA8 ||
                         f.format == SMR_FRAME_BGRA || f.format == SMR_FRAME_ARGB;
+    // 4:2:0 luma is read a pixel pair (2 bytes) at a time, NV12 chroma a {u, v} pair at a time (node_texel, yuv_quad,
+    // k_resample_fused_int, half_row_sums); planar U / V are read byte by byte
+    const bool yuv420 = f.format == SMR_FRAME_PLANAR_YUV420 || f.format == SMR_FRAME_PLANAR_YUVJ420 || f.format == SMR_FRAME_NV12;
     for (int p = 0; p < 3; p++) {
         FrameView::Plane &P = v.plane[p];
         if (!plane_layout(f.format, f.width, f.height, p, P.row_bytes, P.rows)) continue;
@@ -768,6 +772,10 @@ smr_status Renderer::read_frame(const smr_input_frame &f, FrameView &v) {
         if (P.pitch < P.row_bytes) { set_error("input plane pitch is smaller than a row"); return SMR_ERR_INVALID_ARGUMENT; }
         if (f.mem_kind == SMR_MEM_DEVICE && texel4 && (((uintptr_t)f.planes[p] | P.pitch) & 3)) {
             set_error("4-byte texel planes must be 4-byte aligned (pointer and pitch)");
+            return SMR_ERR_INVALID_ARGUMENT;
+        }
+        if (f.mem_kind == SMR_MEM_DEVICE && yuv420 && (p == 0 || f.format == SMR_FRAME_NV12) && (((uintptr_t)f.planes[p] | P.pitch) & 1)) {
+            set_error("4:2:0 luma and NV12 chroma planes must be 2-byte aligned (pointer and pitch)");
             return SMR_ERR_INVALID_ARGUMENT;
         }
         P.p = (const uint8_t *)f.planes[p];
@@ -1977,6 +1985,35 @@ smr_status Renderer::debug_set_inputs(uint64_t pts, const smr_input_frame *in, u
     return select_inputs(pts, in, n_in, [](Input &, const smr_input_frame *) { return SMR_OK; });
 }
 
+// inspection: the fused resample jobs of the last planned tick, as render_begin packed and launched them
+smr_status Renderer::debug_fused_jobs(smr_fused_job_info *out, uint32_t cap, uint32_t *n) {
+    if (!n) return SMR_ERR_INVALID_ARGUMENT;
+    std::lock_guard<std::mutex> g(mu_);
+    *n = (uint32_t)plan_.fused.size();
+    if (!out) return SMR_OK;
+    if (cap < plan_.fused.size()) return SMR_ERR_BUFFER_TOO_SMALL;
+    for (size_t i = 0; i < plan_.fused.size(); i++) {
+        const FusedRec &f = plan_.fused[i];
+        const dev::FusedJob &j = f.job;
+        smr_fused_job_info &o = out[i];
+        o.kernel = f.kernel.kind == dev::FusedKernel::TMA_INT   ? SMR_FUSED_TMA_INT
+                   : f.kernel.kind == dev::FusedKernel::TMA_ANY ? SMR_FUSED_TMA_ANY
+                                                                : SMR_FUSED_LDG;
+        o.ratio = f.kernel.ratio;
+        o.window = f.kernel.kind == dev::FusedKernel::TMA_ANY ? dev::kTma0Window[f.kernel.window] : 0;
+        o.box = f.kernel.box;
+        o.src_class = dev::fused_source_class(j.src.kind);
+        o.full_range = j.src.full_range;
+        o.v_same = j.v_same;
+        o.strip_cols = dev::fused_shape(f.kernel, j).strip_cols;
+        o.src_width = (uint32_t)j.src.width; o.src_height = (uint32_t)j.src.height;
+        o.dst_width = (uint32_t)j.dst_w; o.dst_height = (uint32_t)j.dst_h;
+        o.taps_h = j.taps_h; o.taps_v = j.taps_v;
+        o.direct = f.direct_off != SIZE_MAX ? 1 : 0;
+    }
+    return SMR_OK;
+}
+
 smr_status Renderer::render_end() {   // retires the OLDEST tick in flight
     std::lock_guard<std::mutex> g(mu_);
     if (inflight_.empty()) return SMR_OK;
@@ -2380,6 +2417,7 @@ smr_status smr_render(smr_renderer *r, uint64_t pts, const smr_input_frame *in, 
 smr_status smr_debug_layouts(smr_renderer *r, const char *output_id, uint64_t pts, smr_render_layout *out, uint32_t cap,
                              uint32_t *n, uint32_t *rw, uint32_t *rh) { SMR_GUARD(r->impl.debug_layouts(output_id, pts, out, cap, n, rw, rh)) }
 smr_status smr_debug_set_inputs(smr_renderer *r, uint64_t pts, const smr_input_frame *in, uint32_t n_in) { SMR_GUARD(r->impl.debug_set_inputs(pts, in, n_in)) }
+smr_status smr_debug_fused_jobs(smr_renderer *r, smr_fused_job_info *out, uint32_t cap, uint32_t *n) { SMR_GUARD(r->impl.debug_fused_jobs(out, cap, n)) }
 smr_status smr_comm_get_unique_id(uint8_t id[128]) {
     if (!id) return SMR_ERR_INVALID_ARGUMENT;
     std::string err;

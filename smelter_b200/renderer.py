@@ -624,6 +624,24 @@ class Renderer:
                                                 C.byref(rw), C.byref(rh)))
         return [arr[i] for i in range(n.value)], (rw.value, rh.value)
 
+    def debug_fused_jobs(self):
+        """The fused resample jobs of the last planned tick (smr_debug_fused_jobs), one dict per job in plan order:
+        kernel ("ldg" / "tma_int" / "tma_any"), ratio, window, box, src_class, full_range, v_same, strip_cols,
+        src (w, h), dst (w, h), taps_h, taps_v, direct."""
+        n = C.c_uint32()
+        self._check(self._lib.smr_debug_fused_jobs(self._h, None, 0, C.byref(n)))
+        arr = (F.FusedJobInfo * max(1, n.value))()
+        self._check(self._lib.smr_debug_fused_jobs(self._h, arr, n.value, C.byref(n)))
+        kinds = {F.FUSED_LDG: "ldg", F.FUSED_TMA_INT: "tma_int", F.FUSED_TMA_ANY: "tma_any"}
+        out = []
+        for j in arr[:n.value]:
+            d = {k: getattr(j, k) for k, _ in F.FusedJobInfo._fields_}
+            d["kernel"] = kinds[j.kernel]
+            d["src"] = (d.pop("src_width"), d.pop("src_height"))
+            d["dst"] = (d.pop("dst_width"), d.pop("dst_height"))
+            out.append(d)
+        return out
+
     def stats(self):
         s = F.Stats()
         self._check(self._lib.smr_get_stats(self._h, C.byref(s)))
