@@ -154,7 +154,9 @@ typedef struct {                   /* one entry of FrameSet<InputId> */
  *  - 4-byte texel formats (RGBA8, BGRA, ARGB, UYVY, YUYV): 4-byte aligned.
  *  - Planar 4:2:0 (YUV420, YUVJ420) and NV12: the luma plane, and the NV12 chroma plane, 2-byte aligned (the kernels
  *    read pixel pairs and {u, v} pairs); planar U and V planes may start at any byte.
- * Host planes are copied into aligned buffers and have no such rule. */
+ * Host planes are copied into aligned buffers and have no such rule.
+ * The same holds for SMR_MEM_DEVICE planes of smr_output_frame: an RGBA8 output plane is 4-byte aligned, pointer and
+ * pitch (SMR_ERR_INVALID_ARGUMENT before any kernel is launched otherwise); YUV output planes may start at any byte. */
 
 typedef enum {                     /* OutputFrameFormat, types.rs:187-194 */
     SMR_OUT_PLANAR_YUV420 = 0,     /* PlanarYuv420Bytes */
@@ -332,6 +334,42 @@ typedef struct {
     int32_t direct;                /* the job writes the output bytes of its direct tiles itself */
 } smr_fused_job_info;
 smr_status smr_debug_fused_jobs(smr_renderer *r, smr_fused_job_info *out, uint32_t cap, uint32_t *n);
+
+/* inspection (no device needed): the composite's interior proof for one layout drawn into a width x height target.
+ * Inside it every alpha factor of the fragment shader is exactly 1, so the layer paints its bare colour or sample there.
+ * box: 12 ints {px0, px1, py0, py1 (pixel bounding box), ix0, ix1, iy0, iy1, jx0, jx1, jy0, jy1 (the two interior bars,
+ * which pick the layer's fast class and its direct tiles)}, all 0 when the layer covers no pixel.  shortcut (width *
+ * height bytes, row-major; may be NULL): 1 where the composite's general path skips the fragment shader. */
+smr_status smr_debug_interior(const smr_render_layout *layout, uint32_t width, uint32_t height, int32_t box[12],
+                              uint8_t *shortcut);
+
+/* inspection (no device access): the layers of every composite job of the handle's most recently planned tick, as they
+ * were launched, one record per layer in job order, then painter's order (layers that cover no pixel are left out).  *n is
+ * the record count; records go to `out` when they fit in cap (SMR_ERR_BUFFER_TOO_SMALL otherwise; out = NULL asks for
+ * the count). */
+typedef enum {
+    SMR_COMPOSITE_PARAM = 0,       /* k_composite_p: one job, its layers in the kernel's parameter block */
+    SMR_COMPOSITE_MULTI = 1        /* k_composite_multi: several jobs, or more layers than the parameter block holds */
+} smr_composite_kernel;
+typedef struct {
+    int32_t job;                   /* composite job (outputs of the tick in smr_render order, those that composite) */
+    int32_t kernel;                /* smr_composite_kernel */
+    int32_t layer;                 /* index in the job's layer list */
+    int32_t type;                  /* 0 texture, 1 colour, 2 box shadow */
+    int32_t rotated;
+    int32_t fast;                  /* fast-class bits: 1 IDENT, 2 CONST, 4 LUT, 8 OPAQUE (occludes), 16 SAMPLE, 32 HALF */
+    int32_t box[12];               /* as smr_debug_interior */
+    int32_t tx_off, ty_off;        /* IDENT / HALF: texel offset of pixel (0, 0) */
+    int32_t mask_count;
+    int32_t tex_kind;              /* the texture the kernel reads: 0 none, 1 RGBA8, 2 planar 4:2:0, 3 NV12, 5 BGRA, 6 ARGB,
+                                      7 planar 4:2:2, 8 planar 4:4:4, 9 UYVY, 10 YUYV */
+    int32_t tex_width, tex_height;
+    int32_t tex_pitch[3];          /* bytes per row of each plane (0: unused) */
+    int32_t tex_align[3];          /* each plane's address mod 16 */
+    int32_t width, height;         /* the job's target */
+    int32_t out_format;            /* smr_output_format of the fused K10 / K11 stores, or -1: an RGBA8 frame for k_output */
+} smr_composite_layer_info;
+smr_status smr_debug_composite_layers(smr_renderer *r, smr_composite_layer_info *out, uint32_t cap, uint32_t *n);
 
 /* byte sizes of the planes smr_render writes for an output (0 for unused planes) */
 smr_status smr_output_plane_sizes(uint32_t width, uint32_t height, int32_t output_format, size_t sizes[3]);

@@ -302,6 +302,14 @@ def apply_layouts(out_w, out_h, layouts, textures, mode=MODE_GPU_OPTIMIZED, max_
     return out
 
 
+def bare_map(out_w, out_h, layout, mode=MODE_GPU_OPTIMIZED):
+    """(out_h, out_w) bool: where `layout` covers the pixel and its fragment is the bare colour or sample (every alpha
+    factor exactly 1, no border colour mixed in)."""
+    out = np.empty((out_h, out_w), np.uint8)
+    lib().orc_bare_map(out_w, out_h, C.byref(layout), mode, _p(out))
+    return out.astype(bool)
+
+
 def render_layout_node(out_w, out_h, layouts, nodes, mode=MODE_GPU_OPTIMIZED, max_layouts=100):
     """LayoutNode::render: nodes[i] = premultiplied RGBA8 node texture (h, w, 4) or None."""
     arr = (Layout * max(1, len(layouts)))(*layouts)

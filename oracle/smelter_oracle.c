@@ -782,89 +782,136 @@ static inline void blend_store(uint8_t *dst, const float src_in[4], int mode) {
     dst[3] = orc_unorm8(fmaf(g_u8n[dst[3]], ia, s[3]));
 }
 
-static void draw_layout(int W, int H, const orc_layout *L, const orc_texture *tex, int mode, uint8_t *out) {
-    float left = L->left, top = L->top, w = L->width, h = L->height;
+/* One layout as draw_layout sees it: the quad, the shader colours, the texture */
+typedef struct {
+    const orc_layout *L;
+    const orc_texture *tex;
+    quad q;
+    float left, top, w, h;      /* the quad (box shadow: grown by blur_radius) */
+    float color[4], border_color[4];
+    int tw, th, nmask, mode;
+} layer_ctx;
+
+static int layer_setup(layer_ctx *c, int W, int H, const orc_layout *L, const orc_texture *tex, int mode) {
+    c->L = L; c->tex = tex; c->mode = mode;
+    c->left = L->left; c->top = L->top; c->w = L->width; c->h = L->height;
     if (L->type == ORC_LAYOUT_BOX_SHADOW) { /* apply_layouts.wgsl:215-229 */
         float bw = L->width + 2.0f * L->blur_radius, bh = L->height + 2.0f * L->blur_radius;
-        left = L->left - L->blur_radius; top = L->top - L->blur_radius; w = bw; h = bh;
+        c->left = L->left - L->blur_radius; c->top = L->top - L->blur_radius; c->w = bw; c->h = bh;
     }
-    quad q;
-    if (!quad_setup(&q, left, top, w, h, L->rotation_degrees, W, H)) return;
-    float color[4], border_color[4];
-    shader_color(L->color, mode, color);
-    shader_color(L->border_color, mode, border_color);
-    int tw = tex && tex->data ? tex->width : 1, th = tex && tex->data ? tex->height : 1;
-    int nmask = L->masks_len < ORC_MAX_MASKS ? L->masks_len : ORC_MAX_MASKS;
+    if (!quad_setup(&c->q, c->left, c->top, c->w, c->h, L->rotation_degrees, W, H)) return 0;
+    shader_color(L->color, mode, c->color);
+    shader_color(L->border_color, mode, c->border_color);
+    c->tw = tex && tex->data ? tex->width : 1; c->th = tex && tex->data ? tex->height : 1;
+    c->nmask = L->masks_len < ORC_MAX_MASKS ? L->masks_len : ORC_MAX_MASKS;
+    return 1;
+}
 
+/* vs_main's interpolated attributes + fs_main (apply_layouts.wgsl:258-377) at a covered pixel: the premultiplied source.
+ * *bare = 1 when every alpha factor is exactly 1 and the branch taken does not mix in the border colour, so the source
+ * is the layer's bare colour or sample. */
+static void fragment(const layer_ctx *c, int px, int py, float src[4], int *bare) {
+    const orc_layout *L = c->L;
+    const quad *q = &c->q;
+    float pcx = (float)px + 0.5f, pcy = (float)py + 0.5f;
+    /* interpolated vertex attributes */
+    float lx, ly, u, v;
+    if (!q->rotated) {
+        lx = (pcx - c->left) - c->w * 0.5f;
+        ly = c->h * 0.5f - (pcy - c->top);
+        u = (pcx - c->left) / c->w;
+        v = (pcy - c->top) / c->h;
+    } else {
+        float dx = pcx - q->cx, dyu = q->cy - pcy;
+        lx = dx * q->cs + dyu * q->sn;
+        ly = dyu * q->cs - dx * q->sn;
+        u = lx / c->w + 0.5f;
+        v = 0.5f - ly / c->h;
+    }
+    float mask_alpha = 1.0f;
+    for (int i = 0; i < c->nmask; i++) {
+        const orc_mask *m = &L->masks[i];
+        float d = rounded_rect_sdf((m->left + m->width / 2.0f) - pcx, (m->top + m->height / 2.0f) - pcy,
+                                   m->width, m->height, m->radius);
+        mask_alpha = mask_alpha * smoothstep_f(-0.5f, 0.5f, -d);
+    }
+    for (int ch = 0; ch < 4; ch++) src[ch] = 0.0f;
+    *bare = 0;
+    if (L->type == ORC_LAYOUT_TEXTURE) {
+        float tx = u * (L->crop_width / (float)c->tw) + (L->crop_left / (float)c->tw);
+        float ty = v * (L->crop_height / (float)c->th) + (L->crop_top / (float)c->th);
+        float sample[4];
+        sample_node(c->tex, c->mode, tx, ty, sample);
+        float edge = -rounded_rect_sdf(lx, ly, L->width, L->height, L->border_radius);
+        float bw = L->border_width;
+        if (bw < 1.0f) {
+            float ca = smoothstep_f(-0.5f, 0.5f, edge);
+            for (int ch = 0; ch < 4; ch++) src[ch] = (sample[ch] * ca) * mask_alpha;
+            *bare = ca == 1.0f && mask_alpha == 1.0f;
+        } else if (mask_alpha < 0.01f) {
+            /* transparent */
+        } else if (edge > bw / 2.0f) {
+            float ba = smoothstep_f(bw - 0.5f, bw + 0.5f, edge);
+            for (int ch = 0; ch < 4; ch++)
+                src[ch] = (c->border_color[ch] * (1.0f - ba) + sample[ch] * ba) * mask_alpha;
+            *bare = ba == 1.0f && mask_alpha == 1.0f;
+        } else {
+            float ca = smoothstep_f(-0.5f, 0.5f, edge);
+            for (int ch = 0; ch < 4; ch++) src[ch] = (c->border_color[ch] * ca) * mask_alpha;
+        }
+    } else if (L->type == ORC_LAYOUT_COLOR) {
+        float edge = -rounded_rect_sdf(lx, ly, L->width, L->height, L->border_radius);
+        float bw = L->border_width;
+        if (bw < 1.0f) {
+            float ca = smoothstep_f(-0.5f, 0.5f, edge);
+            for (int ch = 0; ch < 4; ch++) src[ch] = (c->color[ch] * ca) * mask_alpha;
+            *bare = ca == 1.0f && mask_alpha == 1.0f;
+        } else if (edge > bw / 2.0f) {
+            float ba = smoothstep_f(bw, bw + 1.0f, edge);
+            for (int ch = 0; ch < 4; ch++)
+                src[ch] = (c->border_color[ch] * (1.0f - ba) + c->color[ch] * ba) * mask_alpha;
+            *bare = ba == 1.0f && mask_alpha == 1.0f;
+        } else {
+            float ca = smoothstep_f(-0.5f, 0.5f, edge);
+            for (int ch = 0; ch < 4; ch++) src[ch] = (c->border_color[ch] * ca) * mask_alpha;
+        }
+    } else {
+        float edge = -rounded_rect_sdf(lx, ly, L->width, L->height, L->border_radius);
+        float br = L->blur_radius;
+        float ba = smoothstep_f(-br / 2.0f, br / 2.0f, edge) * mask_alpha;
+        for (int ch = 0; ch < 4; ch++) src[ch] = c->color[ch] * ba;
+    }
+}
+
+static void draw_layout(int W, int H, const orc_layout *L, const orc_texture *tex, int mode, uint8_t *out) {
+    layer_ctx c;
+    if (!layer_setup(&c, W, H, L, tex, mode)) return;
 #pragma omp parallel for schedule(static)
-    for (int py = q.by0; py < q.by1; py++)
-        for (int px = q.bx0; px < q.bx1; px++) {
-            if (!quad_covers(&q, px, py)) continue;
-            float pcx = (float)px + 0.5f, pcy = (float)py + 0.5f;
-            /* interpolated vertex attributes */
-            float lx, ly, u, v;
-            if (!q.rotated) {
-                lx = (pcx - left) - w * 0.5f;
-                ly = h * 0.5f - (pcy - top);
-                u = (pcx - left) / w;
-                v = (pcy - top) / h;
-            } else {
-                float dx = pcx - q.cx, dyu = q.cy - pcy;
-                lx = dx * q.cs + dyu * q.sn;
-                ly = dyu * q.cs - dx * q.sn;
-                u = lx / w + 0.5f;
-                v = 0.5f - ly / h;
-            }
-            /* fs_main, apply_layouts.wgsl:258-377 */
-            float mask_alpha = 1.0f;
-            for (int i = 0; i < nmask; i++) {
-                const orc_mask *m = &L->masks[i];
-                float d = rounded_rect_sdf((m->left + m->width / 2.0f) - pcx, (m->top + m->height / 2.0f) - pcy,
-                                           m->width, m->height, m->radius);
-                mask_alpha = mask_alpha * smoothstep_f(-0.5f, 0.5f, -d);
-            }
-            float src[4] = {0, 0, 0, 0};
-            if (L->type == ORC_LAYOUT_TEXTURE) {
-                float tx = u * (L->crop_width / (float)tw) + (L->crop_left / (float)tw);
-                float ty = v * (L->crop_height / (float)th) + (L->crop_top / (float)th);
-                float sample[4];
-                sample_node(tex, mode, tx, ty, sample);
-                float edge = -rounded_rect_sdf(lx, ly, L->width, L->height, L->border_radius);
-                float bw = L->border_width;
-                if (bw < 1.0f) {
-                    float ca = smoothstep_f(-0.5f, 0.5f, edge);
-                    for (int c = 0; c < 4; c++) src[c] = (sample[c] * ca) * mask_alpha;
-                } else if (mask_alpha < 0.01f) {
-                    /* transparent */
-                } else if (edge > bw / 2.0f) {
-                    float ba = smoothstep_f(bw - 0.5f, bw + 0.5f, edge);
-                    for (int c = 0; c < 4; c++)
-                        src[c] = (border_color[c] * (1.0f - ba) + sample[c] * ba) * mask_alpha;
-                } else {
-                    float ca = smoothstep_f(-0.5f, 0.5f, edge);
-                    for (int c = 0; c < 4; c++) src[c] = (border_color[c] * ca) * mask_alpha;
-                }
-            } else if (L->type == ORC_LAYOUT_COLOR) {
-                float edge = -rounded_rect_sdf(lx, ly, L->width, L->height, L->border_radius);
-                float bw = L->border_width;
-                if (bw < 1.0f) {
-                    float ca = smoothstep_f(-0.5f, 0.5f, edge);
-                    for (int c = 0; c < 4; c++) src[c] = (color[c] * ca) * mask_alpha;
-                } else if (edge > bw / 2.0f) {
-                    float ba = smoothstep_f(bw, bw + 1.0f, edge);
-                    for (int c = 0; c < 4; c++)
-                        src[c] = (border_color[c] * (1.0f - ba) + color[c] * ba) * mask_alpha;
-                } else {
-                    float ca = smoothstep_f(-0.5f, 0.5f, edge);
-                    for (int c = 0; c < 4; c++) src[c] = (border_color[c] * ca) * mask_alpha;
-                }
-            } else {
-                float edge = -rounded_rect_sdf(lx, ly, L->width, L->height, L->border_radius);
-                float br = L->blur_radius;
-                float ba = smoothstep_f(-br / 2.0f, br / 2.0f, edge) * mask_alpha;
-                for (int c = 0; c < 4; c++) src[c] = color[c] * ba;
-            }
+    for (int py = c.q.by0; py < c.q.by1; py++)
+        for (int px = c.q.bx0; px < c.q.bx1; px++) {
+            if (!quad_covers(&c.q, px, py)) continue;
+            float src[4];
+            int bare;
+            fragment(&c, px, py, src, &bare);
             blend_store(out + ((size_t)py * W + px) * 4, src, mode);
+        }
+}
+
+/* Per pixel of a W x H target: 1 where the layout covers the pixel and its fragment is the bare colour or sample (every
+ * alpha factor exactly 1, no border colour mixed in), else 0.  The layer interiors the compositor proves must lie inside. */
+void orc_bare_map(int W, int H, const orc_layout *L, int mode, uint8_t *out) {
+    orc_init();
+    memset(out, 0, (size_t)W * H);
+    layer_ctx c;
+    if (!layer_setup(&c, W, H, L, NULL, mode)) return;
+#pragma omp parallel for schedule(static)
+    for (int py = c.q.by0; py < c.q.by1; py++)
+        for (int px = c.q.bx0; px < c.q.bx1; px++) {
+            if (!quad_covers(&c.q, px, py)) continue;
+            float src[4];
+            int bare;
+            fragment(&c, px, py, src, &bare);
+            out[(size_t)py * W + px] = (uint8_t)bare;
         }
 }
 

@@ -122,6 +122,9 @@ int orc_resample_weights(float scale, float offset, int out_coord, float *weight
 void orc_apply_layouts(int out_w, int out_h, const orc_layout *layouts,
                        const orc_texture *textures, int n, int max_layouts, int mode,
                        uint8_t *out_rgba);
+/* One layout's fragment, per pixel of a W x H target: 1 where the layout covers the pixel and its fragment is the bare
+ * colour or sample -- every alpha factor exactly 1 and no border colour mixed in -- else 0. */
+void orc_bare_map(int out_w, int out_h, const orc_layout *layout, int mode, uint8_t *out);
 
 /* --- LayoutNode::render (transformations/layout.rs:169-278): resample scaled children, then
  * apply_layouts. nodes[] are the child node textures indexed by orc_layout.child_index. */

@@ -127,6 +127,17 @@ class FusedJobInfo(C.Structure):   # smr_fused_job_info
                 ("taps_h", C.c_int32), ("taps_v", C.c_int32), ("direct", C.c_int32)]
 
 
+COMPOSITE_PARAM, COMPOSITE_MULTI = 0, 1
+
+
+class CompositeLayerInfo(C.Structure):   # smr_composite_layer_info
+    _fields_ = [("job", C.c_int32), ("kernel", C.c_int32), ("layer", C.c_int32), ("type", C.c_int32), ("rotated", C.c_int32),
+                ("fast", C.c_int32), ("box", C.c_int32 * 12), ("tx_off", C.c_int32), ("ty_off", C.c_int32),
+                ("mask_count", C.c_int32), ("tex_kind", C.c_int32), ("tex_width", C.c_int32), ("tex_height", C.c_int32),
+                ("tex_pitch", C.c_int32 * 3), ("tex_align", C.c_int32 * 3), ("width", C.c_int32), ("height", C.c_int32),
+                ("out_format", C.c_int32)]
+
+
 KERNEL_CLASSES = ["convert", "weights", "resample_box", "resample_first", "resample_last", "composite", "output",
                   "fill", "resample_fused"]
 
@@ -137,7 +148,7 @@ class KernelTimes(C.Structure):
 
 EXPORTS = [
     "smr_create", "smr_destroy", "smr_register_input", "smr_unregister_input", "smr_update_scene",
-    "smr_unregister_output", "smr_set_layouts", "smr_render", "smr_render_begin", "smr_render_end", "smr_preprocess_frame", "smr_premultiply_rgba8", "smr_render_text", "smr_debug_partition", "smr_debug_tile_plan", "smr_debug_weights", "smr_debug_fused_jobs", "smr_output_plane_sizes",
+    "smr_unregister_output", "smr_set_layouts", "smr_render", "smr_render_begin", "smr_render_end", "smr_preprocess_frame", "smr_premultiply_rgba8", "smr_render_text", "smr_debug_partition", "smr_debug_tile_plan", "smr_debug_weights", "smr_debug_fused_jobs", "smr_debug_composite_layers", "smr_debug_interior", "smr_output_plane_sizes",
     "smr_component_default", "smr_debug_layouts", "smr_debug_set_inputs", "smr_get_stats", "smr_set_profiling", "smr_get_kernel_times",
     "smr_comm_get_unique_id", "smr_comm_init", "smr_comm_broadcast_inputs", "smr_comm_exchange_inputs", "smr_comm_pull_inputs", "smr_peer_pool_alloc", "smr_peer_pool_open", "smr_peer_pool_close", "smr_peer_pool_free", "smr_comm_destroy", "smr_host_register", "smr_host_unregister", "smr_cuda_stream", "smr_last_error",
     "smr_version",
@@ -185,6 +196,10 @@ def lib():
     L.smr_debug_weights.restype = C.c_int32
     L.smr_debug_fused_jobs.argtypes = [vp, C.POINTER(FusedJobInfo), C.c_uint32, C.POINTER(C.c_uint32)]
     L.smr_debug_fused_jobs.restype = C.c_int32
+    L.smr_debug_composite_layers.argtypes = [vp, C.POINTER(CompositeLayerInfo), C.c_uint32, C.POINTER(C.c_uint32)]
+    L.smr_debug_composite_layers.restype = C.c_int32
+    L.smr_debug_interior.argtypes = [C.POINTER(RenderLayout), C.c_uint32, C.c_uint32, C.POINTER(C.c_int32 * 12), C.c_void_p]
+    L.smr_debug_interior.restype = C.c_int32
     L.smr_output_plane_sizes.argtypes = [C.c_uint32, C.c_uint32, C.c_int32, C.POINTER(C.c_size_t * 3)]
     L.smr_component_default.argtypes = [C.c_int32, C.POINTER(Component)]
     L.smr_component_default.restype = None

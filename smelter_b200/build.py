@@ -10,7 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libsmelter_b200.so")
 SOURCES = ["kernels.cu", "renderer.cpp", "scene.cpp"]
-HEADERS = ["kernels.h", "int_weights.h", "scene.h", "ptx_helpers.cuh", "resample_tma.cuh", "resample_tma3.cuh", "resample_tma0.cuh", os.path.join("..", "..", "include", "smelter_b200.h")]
+HEADERS = ["kernels.h", "interior.h", "int_weights.h", "scene.h", "ptx_helpers.cuh", "resample_tma.cuh", "resample_tma3.cuh", "resample_tma0.cuh", os.path.join("..", "..", "include", "smelter_b200.h")]
 
 NVCC_FLAGS = [
     "-std=c++17", "-O3",

@@ -23,6 +23,7 @@
 #include <cstring>
 
 #include "kernels.h"
+#include "interior.h"
 #include "int_weights.h"
 
 namespace smr {
@@ -1280,55 +1281,30 @@ __device__ __forceinline__ uchar4 blend(const Tables &T, int mode, uchar4 dst, f
 
 // general per-pixel path: full fragment shader + fixed-function blend.  Kept out of line: the fast paths of
 // k_composite cover almost every pixel and the instruction cache matters more than the call.
-// true when the rounded-rect alpha of fs_main is provably exactly 1 at this pixel centre: at least `shr`
-// inside every edge and outside the four corner squares of side rmax+2 (there the SDF is the plain edge
-// distance, >= 2 > .5, so smoothstep(-.5,.5,.) == 1)
-__device__ __forceinline__ bool rect_alpha_one(float pcx, float pcy, float left, float top, float w, float h,
-                                               float rmax, float shr) {
-    const float hx = w * 0.5f, hy = h * 0.5f;
-    const float dx = fabsf(pcx - (left + hx)), dy = fabsf(pcy - (top + hy));
-    const bool inside = dx <= hx - shr && dy <= hy - shr;
-    const bool corner = dx > hx - rmax - 2.0f && dy > hy - rmax - 2.0f;
-    return inside && !corner;
-}
-
-// general per-pixel path: full fragment shader + fixed-function blend.  Kept out of line: the fast paths of
-// k_composite cover almost every pixel and the instruction cache matters more than the call.
 __device__ __noinline__ uchar4 shade_blend(const Tables &T, const CompositeJob &J, const LayerDev &L, int X, int Y,
                                            uchar4 dst) {
-    if (!L.rotated && L.type != 2) {
-        // per-pixel version of the host's interior classification (LayerDev::ix0..): straight edges of rounded
-        // layers and masks need no SDF -- only the corner squares do
-        const float pcx = (float)X + 0.5f, pcy = (float)Y + 0.5f;
-        const float rmax = fmaxf(fmaxf(L.border_radius[0], L.border_radius[1]), fmaxf(L.border_radius[2], L.border_radius[3]));
-        const float shr = 2.0f + (L.border_width >= 1.0f ? L.border_width + 1.0f : 0.0f);
-        bool one = rect_alpha_one(pcx, pcy, L.left, L.top, L.content_w, L.content_h, fmaxf(rmax, 0.0f), shr);
-        for (int i = 0; one && i < L.mask_count; i++) {
-            const MaskDev &m = J.masks[L.mask_begin + i];
-            const float mr = fmaxf(fmaxf(m.radius[0], m.radius[1]), fmaxf(m.radius[2], m.radius[3]));
-            one = rect_alpha_one(pcx, pcy, m.left, m.top, m.width, m.height, fmaxf(mr, 0.0f), 2.0f);
+    // per-pixel version of the host's interior bars (LayerDev::ix0..): straight edges of rounded layers and masks need
+    // no SDF -- only the corner squares do
+    if (interior_shortcut(L, J.masks + L.mask_begin, X, Y)) {
+        if (L.type == 1) {  // bare colour
+            if (L.fast & FAST_CONST) return *reinterpret_cast<const uchar4 *>(&L.const_bytes);
+            return blend(T, J.mode, dst, make_float4(L.color[0], L.color[1], L.color[2], L.color[3]));
         }
-        if (one) {
-            if (L.type == 1) {  // bare colour
-                if (L.fast & FAST_CONST) return *reinterpret_cast<const uchar4 *>(&L.const_bytes);
-                return blend(T, J.mode, dst, make_float4(L.color[0], L.color[1], L.color[2], L.color[3]));
-            }
-            bool exact;
-            uchar4 texel;
-            float4 sample;
-            if (L.fast & FAST_IDENT) {
-                texel = node_texel(T, J.textures[L.tex], X + L.tx_off, Y + L.ty_off);
-                exact = true;
-                const float *lut = J.mode == 0 ? T.dec : T.u8n;
-                sample = make_float4(lut[texel.x], lut[texel.y], lut[texel.z], T.u8n[texel.w]);
-            } else {
-                const float u = (pcx - L.left) / L.width, v = (pcy - L.top) / L.height;
-                sample = sample_node(T, L.tex >= 0 ? &J.textures[L.tex] : nullptr, J.mode, u * L.crop_sx + L.crop_ox,
-                                     v * L.crop_sy + L.crop_oy, exact, texel);
-            }
-            if (exact && texel.w == 255) return texel;  // encode(decode(b)) == b
-            return blend(T, J.mode, dst, sample);
+        bool exact;
+        uchar4 texel;
+        float4 sample;
+        if (L.fast & FAST_IDENT) {
+            texel = node_texel(T, J.textures[L.tex], X + L.tx_off, Y + L.ty_off);
+            exact = true;
+            const float *lut = J.mode == 0 ? T.dec : T.u8n;
+            sample = make_float4(lut[texel.x], lut[texel.y], lut[texel.z], T.u8n[texel.w]);
+        } else {
+            const float u = (((float)X + 0.5f) - L.left) / L.width, v = (((float)Y + 0.5f) - L.top) / L.height;
+            sample = sample_node(T, L.tex >= 0 ? &J.textures[L.tex] : nullptr, J.mode, u * L.crop_sx + L.crop_ox,
+                                 v * L.crop_sy + L.crop_oy, exact, texel);
         }
+        if (exact && texel.w == 255) return texel;  // encode(decode(b)) == b
+        return blend(T, J.mode, dst, sample);
     }
     bool pass;
     uchar4 texel;
@@ -1349,7 +1325,7 @@ __device__ __noinline__ uchar4 shade_blend(const Tables &T, const CompositeJob &
 
 // PARAM: the layer list travels in the kernel parameter block (constant bank): the per-tile culling and the
 // per-pixel loop read it with no global round trip and no shared-memory copy; used whenever it fits.
-#define PARAM_LAYERS 96
+#define PARAM_LAYERS kCompositeParamLayers
 #define MAX_LUT 4          // translucent colour layers of a tile that get a blend table (FAST_LUT)
 struct CompositeParams {
     CompositeJob job;
@@ -1697,12 +1673,15 @@ __device__ __forceinline__ void composite_body(const CompositeJob &J, const Laye
 
     if (x0 >= J.width || y0 >= J.height) continue;
     if (J.out_format < 0 || J.out_format == 3) {  // RGBA8 node texture / RgbaWgpuTexture analogue
+        // a caller's device plane is 4-byte aligned (host-checked), not necessarily 16: with x0 a multiple of 4 pixels,
+        // every 16-byte store of the plane is aligned when its start and its pitch are
+        const bool vec16 = (((uintptr_t)J.out0 | (uintptr_t)J.out_pitch0) & 15) == 0;
 #pragma unroll
         for (int j = 0; j < CT_H; j++) {
             int Y = y0 + j;
             if (Y >= J.height) break;
             uchar4 *row = reinterpret_cast<uchar4 *>(J.out0 + (size_t)Y * J.out_pitch0);
-            if (x0 + CT_W <= J.width && (J.out_pitch0 & 15) == 0) {
+            if (x0 + CT_W <= J.width && vec16) {
                 uint4 v;
                 v.x = *reinterpret_cast<unsigned int *>(&px[j][0]);
                 v.y = *reinterpret_cast<unsigned int *>(&px[j][1]);
@@ -1722,7 +1701,9 @@ __device__ __forceinline__ void composite_body(const CompositeJob &J, const Laye
 #pragma unroll
         for (int i = 0; i < CT_W; i++)
             yv[j][i] = (unsigned char)unorm8(to_y(T.u8n[px[j][i].x], T.u8n[px[j][i].y], T.u8n[px[j][i].z]));
-    const bool full = (x0 + CT_W <= J.width) && ((J.out_pitch0 & 3) == 0);
+    // YUV planes may start at any byte; x0 is a multiple of 4 (cx of 2), so a plane's vector stores are aligned when its
+    // start and its pitch are
+    const bool full = (x0 + CT_W <= J.width) && (((uintptr_t)J.out0 | (uintptr_t)J.out_pitch0) & 3) == 0;
 #pragma unroll
     for (int j = 0; j < CT_H; j++) {
         int Y = y0 + j;
@@ -1746,12 +1727,12 @@ __device__ __forceinline__ void composite_body(const CompositeJob &J, const Laye
     const int cx = x0 / 2, cy = y0 / 2, cw = J.width / 2;
     if (J.out_format == 4) {  // NV12
         unsigned char *row = J.out1 + (size_t)cy * J.out_pitch1 + cx * 2;
-        if (cx + 1 < cw && (J.out_pitch1 & 3) == 0) *reinterpret_cast<uchar4 *>(row) = make_uchar4(uo[0], vo[0], uo[1], vo[1]);
+        if (cx + 1 < cw && (((uintptr_t)J.out1 | (uintptr_t)J.out_pitch1) & 3) == 0) *reinterpret_cast<uchar4 *>(row) = make_uchar4(uo[0], vo[0], uo[1], vo[1]);
         else
             for (int c = 0; c < 2 && cx + c < cw; c++) { row[2 * c] = uo[c]; row[2 * c + 1] = vo[c]; }
     } else {  // planar 4:2:0
         unsigned char *ru = J.out1 + (size_t)cy * J.out_pitch1 + cx, *rv = J.out2 + (size_t)cy * J.out_pitch2 + cx;
-        if (cx + 1 < cw && (J.out_pitch1 & 1) == 0 && (J.out_pitch2 & 1) == 0) {
+        if (cx + 1 < cw && (((uintptr_t)J.out1 | (uintptr_t)J.out2 | (uintptr_t)(J.out_pitch1 | J.out_pitch2)) & 1) == 0) {
             *reinterpret_cast<uchar2 *>(ru) = make_uchar2(uo[0], uo[1]);
             *reinterpret_cast<uchar2 *>(rv) = make_uchar2(vo[0], vo[1]);
         } else

@@ -45,6 +45,7 @@ struct Tex {
 struct MaskDev {
     float radius[4];
     float top, left, width, height;
+    float edge, corner;              // its interior (interior.h); edge = +inf: none
 };
 
 // One flattened RenderLayout, prepared on the host for the composite kernel
@@ -71,6 +72,7 @@ struct alignas(16) LayerDev {
     int32_t fast;                    // FAST_* bits
     int32_t tx_off, ty_off;          // FAST_IDENT: texel = (px + tx_off, py + ty_off)
     uint32_t const_bytes;            // FAST_CONST: bytes an opaque colour leaves in the target (RGBA little endian)
+    float int_edge, int_corner;      // the layer rect's interior (interior.h); int_edge = +inf: none
 };
 // FAST_LUT: translucent bare colour -- inside the bars the blend is a per-channel function of the target byte
 // FAST_OPAQUE: inside the bars the layer REPLACES the target bytes (opaque constant, or 1:1 texels of a texture
@@ -104,6 +106,9 @@ struct CompositeJob {
     int32_t n_tiles;                 // entries of tile_list
 };
 constexpr int kDirectTileW = 128, kDirectTileH = 16;   // = the composite's block tile (CB_X * CT_W x CB_Y * CT_H)
+// launch_composite runs k_composite_p (job and layers in the parameter block) for one job of at most this many layers,
+// k_composite_multi otherwise
+constexpr int kCompositeParamLayers = 96;
 
 // one Lanczos pass (resample.wgsl) or box pass (downsample.wgsl)
 struct ResampleJob {

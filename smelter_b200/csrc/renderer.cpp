@@ -28,6 +28,7 @@
 #include <vector>
 
 #include "../../include/smelter_b200.h"
+#include "interior.h"
 #include "kernels.h"
 #include "scene.h"
 
@@ -284,6 +285,7 @@ class Renderer {
     smr_status debug_layouts(const char *output_id, uint64_t pts, smr_render_layout *out, uint32_t cap, uint32_t *n,
                              uint32_t *rw, uint32_t *rh);
     smr_status debug_fused_jobs(smr_fused_job_info *out, uint32_t cap, uint32_t *n);
+    smr_status debug_composite_layers(smr_composite_layer_info *out, uint32_t cap, uint32_t *n);
     void stats(smr_stats *s) { std::lock_guard<std::mutex> g(mu_); *s = stats_; }
     void *stream() { return (void *)stream_; }
     const char *last_error() { return err_.c_str(); }
@@ -654,6 +656,26 @@ smr_status Renderer::update_scene(const char *output_id, uint32_t w, uint32_t h,
     return SMR_OK;
 }
 
+// One smr_render_layout (type and masks_len checked by the caller)
+static RenderLayout layout_from_c(const smr_render_layout &d) {
+    RenderLayout l;
+    l.kind = (RenderLayout::Kind)d.type;
+    l.top = d.top; l.left = d.left; l.width = d.width; l.height = d.height; l.rotation_degrees = d.rotation_degrees;
+    l.border_radius = {d.border_radius[0], d.border_radius[1], d.border_radius[2], d.border_radius[3]};
+    l.color = {d.color.r, d.color.g, d.color.b, d.color.a};
+    l.border_color = {d.border_color.r, d.border_color.g, d.border_color.b, d.border_color.a};
+    l.border_width = d.border_width; l.blur_radius = d.blur_radius;
+    l.index = (size_t)std::max(d.child_index, 0);
+    l.crop = {d.crop_top, d.crop_left, d.crop_width, d.crop_height};
+    for (int m = 0; m < d.masks_len; m++) {
+        Mask mk;
+        mk.radius = {d.masks[m].radius[0], d.masks[m].radius[1], d.masks[m].radius[2], d.masks[m].radius[3]};
+        mk.top = d.masks[m].top; mk.left = d.masks[m].left; mk.width = d.masks[m].width; mk.height = d.masks[m].height;
+        l.masks.push_back(mk);
+    }
+    return l;
+}
+
 // The flattened boundary (SURVEY 8b, second form): RenderLayout[] exactly as NestedLayout::flatten returns them and
 // LayoutNodeParams consumes them (transformations/layout/params.rs:169-333), child node indices resolved through
 // `child_ids` (the node's children in DFS order, scene/layout.rs:84-93).
@@ -668,20 +690,7 @@ smr_status Renderer::set_layouts(const char *output_id, uint32_t w, uint32_t h, 
         RenderLayout &l = ls[i];
         if (d.type < 0 || d.type > 2 || d.masks_len < 0 || d.masks_len > SMR_MAX_MASKS) { set_error("malformed layout"); return SMR_ERR_INVALID_ARGUMENT; }
         if (d.type == 0 && (d.child_index < 0 || (uint32_t)d.child_index >= n_children)) { set_error("child index outside child_ids"); return SMR_ERR_INVALID_ARGUMENT; }
-        l.kind = (RenderLayout::Kind)d.type;
-        l.top = d.top; l.left = d.left; l.width = d.width; l.height = d.height; l.rotation_degrees = d.rotation_degrees;
-        l.border_radius = {d.border_radius[0], d.border_radius[1], d.border_radius[2], d.border_radius[3]};
-        l.color = {d.color.r, d.color.g, d.color.b, d.color.a};
-        l.border_color = {d.border_color.r, d.border_color.g, d.border_color.b, d.border_color.a};
-        l.border_width = d.border_width; l.blur_radius = d.blur_radius;
-        l.index = (size_t)std::max(d.child_index, 0);
-        l.crop = {d.crop_top, d.crop_left, d.crop_width, d.crop_height};
-        for (int m = 0; m < d.masks_len; m++) {
-            Mask mk;
-            mk.radius = {d.masks[m].radius[0], d.masks[m].radius[1], d.masks[m].radius[2], d.masks[m].radius[3]};
-            mk.top = d.masks[m].top; mk.left = d.masks[m].left; mk.width = d.masks[m].width; mk.height = d.masks[m].height;
-            l.masks.push_back(mk);
-        }
+        l = layout_from_c(d);
     }
     Output &o = outputs_[output_id];
     o.format = fmt;
@@ -1051,19 +1060,19 @@ static inline long long ceil_div256(long long a) {  // ceil(a / 256)
     return q + (r > 0 ? 1 : 0);
 }
 
-// vertex stage of apply_layouts.wgsl:174-243 + rasteriser (numeric contract NC-7), on the host
-void Renderer::prepare_layer(const RenderLayout &l, int W, int H, int tex_index, int tex_w, int tex_h,
-                             dev::LayerDev &d, bool &skip) {
+// The geometry of a layer drawn into a W x H target: the vertex stage of apply_layouts.wgsl:174-243 + rasteriser (numeric
+// contract NC-7) and the interior proof (interior.h).  Fills the geometric fields of `d` (pixel box, rect, radii, border
+// width, the two bars); false when the layer covers no pixel.
+static bool layer_geometry(const RenderLayout &l, int W, int H, dev::LayerDev &d) {
     memset(&d, 0, sizeof(d));
-    skip = true;
     float left = l.left, top = l.top, w = l.width, h = l.height;
     if (l.kind == RenderLayout::BoxShadow) {
         float bw = l.width + 2.0f * l.blur_radius, bh = l.height + 2.0f * l.blur_radius;
         left = l.left - l.blur_radius; top = l.top - l.blur_radius; w = bw; h = bh;
     }
     float rot = l.rotation_degrees;
-    if (!(left == left) || !(top == top) || !(w == w) || !(h == h) || !(rot == rot)) return;
-    if (std::fabs(left) > 1e7f || std::fabs(top) > 1e7f || std::fabs(w) > 1e7f || std::fabs(h) > 1e7f) return;
+    if (!(left == left) || !(top == top) || !(w == w) || !(h == h) || !(rot == rot)) return false;
+    if (std::fabs(left) > 1e7f || std::fabs(top) > 1e7f || std::fabs(w) > 1e7f || std::fabs(h) > 1e7f) return false;
     d.type = (int)l.kind;
     d.left = left; d.top = top; d.width = w; d.height = h;
     d.content_w = l.width; d.content_h = l.height;
@@ -1095,99 +1104,113 @@ void Renderer::prepare_layer(const RenderLayout &l, int W, int H, int tex_index,
         d.px0 = (int)std::fmax(fx0, 0.0f); d.py0 = (int)std::fmax(fy0, 0.0f);
         d.px1 = (int)std::fmin(fx1, (float)W); d.py1 = (int)std::fmin(fy1, (float)H);
     }
-    if (d.px0 >= d.px1 || d.py0 >= d.py1) return;
+    if (d.px0 >= d.px1 || d.py0 >= d.py1) return false;
     d.border_radius[0] = l.border_radius.top_left; d.border_radius[1] = l.border_radius.top_right;
     d.border_radius[2] = l.border_radius.bottom_right; d.border_radius[3] = l.border_radius.bottom_left;
-    shader_color(l.color, d.color);
-    shader_color(l.border_color, d.border_color);
     d.border_width = l.border_width;
     d.blur_radius = l.blur_radius;
+    // ---- fast interior (see LayerDev): only where every alpha factor of fs_main is provably exactly 1 ----
+    // The layer and each mask prove the pixel centres at least `edge` inside their straight edges and outside their
+    // corner squares (interior.h).  The intersection of those regions contains two bars: core x range x edge y range,
+    // and the transpose.
+    dev::interior_margins(l.left, l.top, l.width, l.height, d.border_radius, d.border_width, d.int_edge, d.int_corner);
+    if (d.rotated || l.kind == RenderLayout::BoxShadow) return true;
+    dev::InteriorRect k;
+    if (!dev::interior_rect(l.left, l.top, l.width, l.height, d.border_radius, d.border_width, k)) return true;
+    float cx0 = l.left + k.core, cx1 = l.left + l.width - k.core, cy0 = l.top + k.core, cy1 = l.top + l.height - k.core;
+    float ex0 = l.left + k.edge, ex1 = l.left + l.width - k.edge, ey0 = l.top + k.edge, ey1 = l.top + l.height - k.edge;
+    size_t nm = std::min<size_t>(l.masks.size(), SMR_MAX_MASKS);
+    for (size_t i = 0; i < nm; i++) {
+        const Mask &mk = l.masks[i];
+        const float r[4] = {mk.radius.top_left, mk.radius.top_right, mk.radius.bottom_right, mk.radius.bottom_left};
+        if (!dev::interior_rect(mk.left, mk.top, mk.width, mk.height, r, 0.0f, k)) return true;
+        cx0 = std::fmax(cx0, mk.left + k.core); cx1 = std::fmin(cx1, mk.left + mk.width - k.core);
+        cy0 = std::fmax(cy0, mk.top + k.core); cy1 = std::fmin(cy1, mk.top + mk.height - k.core);
+        ex0 = std::fmax(ex0, mk.left + k.edge); ex1 = std::fmin(ex1, mk.left + mk.width - k.edge);
+        ey0 = std::fmax(ey0, mk.top + k.edge); ey1 = std::fmin(ey1, mk.top + mk.height - k.edge);
+    }
+    // pixel X is inside iff lo <= X + .5 <= hi
+    auto bar = [&](float lx, float hx, float ly, float hy, int32_t &x0, int32_t &x1, int32_t &y0, int32_t &y1) {
+        if (!(lx < hx && ly < hy)) return;
+        int ax0 = std::max((int)std::ceil(lx - 0.5f), d.px0), ax1 = std::min((int)std::floor(hx - 0.5f) + 1, d.px1);
+        int ay0 = std::max((int)std::ceil(ly - 0.5f), d.py0), ay1 = std::min((int)std::floor(hy - 0.5f) + 1, d.py1);
+        if (ax0 >= ax1 || ay0 >= ay1) return;
+        x0 = ax0; x1 = ax1; y0 = ay0; y1 = ay1;
+    };
+    bar(cx0, cx1, ey0, ey1, d.ix0, d.ix1, d.iy0, d.iy1);
+    bar(ex0, ex1, cy0, cy1, d.jx0, d.jx1, d.jy0, d.jy1);
+    return true;
+}
+
+// Appends the masks of `l` the shader sees (params.rs:284-294); returns their count
+static int layer_masks(const RenderLayout &l, std::vector<dev::MaskDev> &masks) {
+    size_t nm = std::min<size_t>(l.masks.size(), SMR_MAX_MASKS);
+    for (size_t i = 0; i < nm; i++) {
+        const Mask &m = l.masks[i];
+        dev::MaskDev md;
+        md.radius[0] = m.radius.top_left; md.radius[1] = m.radius.top_right;
+        md.radius[2] = m.radius.bottom_right; md.radius[3] = m.radius.bottom_left;
+        md.top = m.top; md.left = m.left; md.width = m.width; md.height = m.height;
+        dev::interior_margins(md.left, md.top, md.width, md.height, md.radius, 0.0f, md.edge, md.corner);
+        masks.push_back(md);
+    }
+    return (int)nm;
+}
+
+// One layer as the composite draws it: its geometry (layer_geometry), colours, texture mapping and fast class
+void Renderer::prepare_layer(const RenderLayout &l, int W, int H, int tex_index, int tex_w, int tex_h,
+                             dev::LayerDev &d, bool &skip) {
+    skip = !layer_geometry(l, W, H, d);
+    if (skip) return;
+    shader_color(l.color, d.color);
+    shader_color(l.border_color, d.border_color);
     d.tex = tex_index;
     if (l.kind == RenderLayout::ChildNode) {
         d.crop_sx = l.crop.width / (float)tex_w; d.crop_ox = l.crop.left / (float)tex_w;
         d.crop_sy = l.crop.height / (float)tex_h; d.crop_oy = l.crop.top / (float)tex_h;
     }
-    // ---- fast interior (see LayerDev): only where every alpha factor of fs_main is provably exactly 1 ----
-    d.ix0 = d.ix1 = d.iy0 = d.iy1 = 0;
-    d.jx0 = d.jx1 = d.jy0 = d.jy1 = 0;
-    if (!d.rotated && l.kind != RenderLayout::BoxShadow) {
-        // Every rounded rect k (the layer itself and each mask) has alpha exactly 1 at least e_k inside its
-        // straight edges and outside its four corner squares of side r_k + 2 (rect_alpha_one in kernels.cu).
-        // The intersection of those regions contains two bars: core x range x edge y range, and the transpose.
-        const float m = 2.0f;
-        float rmax = std::fmax(std::fmax(l.border_radius.top_left, l.border_radius.top_right),
-                               std::fmax(l.border_radius.bottom_left, l.border_radius.bottom_right));
-        float edge = m + (l.border_width >= 1.0f ? l.border_width + 1.0f : 0.0f);
-        float core = edge + std::fmax(rmax, 0.0f);
-        float cx0 = l.left + core, cx1 = l.left + l.width - core, cy0 = l.top + core, cy1 = l.top + l.height - core;
-        float ex0 = l.left + edge, ex1 = l.left + l.width - edge, ey0 = l.top + edge, ey1 = l.top + l.height - edge;
-        size_t nm = std::min<size_t>(l.masks.size(), SMR_MAX_MASKS);
-        for (size_t i = 0; i < nm; i++) {
-            const Mask &k = l.masks[i];
-            float mr = std::fmax(std::fmax(k.radius.top_left, k.radius.top_right),
-                                 std::fmax(k.radius.bottom_left, k.radius.bottom_right));
-            float ms = std::fmax(mr, 0.0f) + m;
-            cx0 = std::fmax(cx0, k.left + ms); cx1 = std::fmin(cx1, k.left + k.width - ms);
-            cy0 = std::fmax(cy0, k.top + ms); cy1 = std::fmin(cy1, k.top + k.height - ms);
-            ex0 = std::fmax(ex0, k.left + m); ex1 = std::fmin(ex1, k.left + k.width - m);
-            ey0 = std::fmax(ey0, k.top + m); ey1 = std::fmin(ey1, k.top + k.height - m);
-        }
-        // pixel X is inside iff lo <= X + .5 <= hi
-        auto bar = [&](float lx, float hx, float ly, float hy, int32_t &x0, int32_t &x1, int32_t &y0, int32_t &y1) {
-            x0 = x1 = y0 = y1 = 0;
-            if (!(lx == lx && hx == hx && ly == ly && hy == hy && lx < hx && ly < hy)) return;
-            int ax0 = std::max((int)std::ceil(lx - 0.5f), d.px0), ax1 = std::min((int)std::floor(hx - 0.5f) + 1, d.px1);
-            int ay0 = std::max((int)std::ceil(ly - 0.5f), d.py0), ay1 = std::min((int)std::floor(hy - 0.5f) + 1, d.py1);
-            if (ax0 >= ax1 || ay0 >= ay1) return;
-            x0 = ax0; x1 = ax1; y0 = ay0; y1 = ay1;
-        };
-        bar(cx0, cx1, ey0, ey1, d.ix0, d.ix1, d.iy0, d.iy1);
-        bar(ex0, ex1, cy0, cy1, d.jx0, d.jx1, d.jy0, d.jy1);
-        if (d.ix0 < d.ix1 || d.jx0 < d.jx1) {
-            if (l.kind == RenderLayout::Color && l.color.a == 255) {
-                // opaque colour: fma(dst, 0, src) == src, so the target bytes are a constant of the layer
-                d.fast |= dev::FAST_CONST | dev::FAST_OPAQUE;
-                uint8_t b[4];
-                for (int c = 0; c < 3; c++)
-                    b[c] = opts_.rendering_mode == SMR_MODE_GPU_OPTIMIZED ? srgb_encode_host(d.color[c]) : unorm8_host(d.color[c]);
-                b[3] = 255;
-                memcpy(&d.const_bytes, b, 4);
-            } else if (l.kind == RenderLayout::Color) {
-                d.fast |= dev::FAST_LUT;
-            }
-            auto integral = [](float v) { return v == std::rint(v) && std::fabs(v) <= 4096.0f; };
-            if (l.kind == RenderLayout::ChildNode && tex_index >= 0 && tex_w <= 4096 && tex_h <= 4096 &&
-                l.width == (float)tex_w && l.crop.width == (float)tex_w && l.height == (float)tex_h &&
-                l.crop.height == (float)tex_h && integral(l.left) && integral(l.top) && l.crop.left == 0.0f &&
-                l.crop.top == 0.0f) {
-                // 1:1 mapping on whole texels: the NC-6 tap is texel (px - left, py - top) with weight exactly 1
-                // (|coordinate error| < 1e-3 << 1/512, the 8-bit weight rounds to 0 or 1)
-                d.fast |= dev::FAST_IDENT;
-                if (plan_.tex[tex_index].opaque) d.fast |= dev::FAST_OPAQUE;
-                d.tx_off = -(int)l.left; d.ty_off = -(int)l.top;
-            } else if (l.kind == RenderLayout::ChildNode && tex_index >= 0 && plan_.tex[tex_index].opaque && l.width > 0.0f &&
-                       l.height > 0.0f &&
-                       (plan_.tex[tex_index].tex.kind == dev::TEX_RGBA8 ||
-                        (opts_.rendering_mode == SMR_MODE_CPU_OPTIMIZED &&
-                         (plan_.tex[tex_index].tex.kind == dev::TEX_NV12 || plan_.tex[tex_index].tex.kind == dev::TEX_YUV420)))) {
-                // opaque child at a fractional position / size: filtered sample alone, target ignored.  RGBA8: a
-                // resampled child; planar 4:2:0 / NV12 in CpuOptimized: the layout shader's own bilinear scaling of
-                // the (virtual) node texture, K1/K2 evaluated per tap quad
-                d.fast |= dev::FAST_SAMPLE | dev::FAST_OPAQUE;
-                const dev::Tex &tt = plan_.tex[tex_index].tex;
-                if (tt.kind != dev::TEX_RGBA8 && ((tex_w | tex_h) & 1) == 0 && tex_w <= 4096 && tex_h <= 4096 &&
-                    l.width * 2.0f == (float)tex_w && l.height * 2.0f == (float)tex_h && l.crop.left == 0.0f && l.crop.top == 0.0f &&
-                    l.crop.width == (float)tex_w && l.crop.height == (float)tex_h && integral(l.left) && integral(l.top) &&
-                    ((int)l.left & 1) == 0 && (tt.pitch0 & 3) == 0 && ((uintptr_t)tt.p0 & 3) == 0) {
-                    // exact 2:1 on whole pixels (a 2x2 grid of same-size inputs): sample coordinate = 2 k + 1/2 with an error
-                    // far below the 1/512 weight step, so the taps are the aligned texel quad at weights exactly 1/2
-                    d.fast |= dev::FAST_HALF;
-                    d.tx_off = -(int)l.left; d.ty_off = -(int)l.top;
-                }
-            }
+    if (d.ix0 >= d.ix1 && d.jx0 >= d.jx1) return;
+    if (l.kind == RenderLayout::Color && l.color.a == 255) {
+        // opaque colour: fma(dst, 0, src) == src, so the target bytes are a constant of the layer
+        d.fast |= dev::FAST_CONST | dev::FAST_OPAQUE;
+        uint8_t b[4];
+        for (int c = 0; c < 3; c++)
+            b[c] = opts_.rendering_mode == SMR_MODE_GPU_OPTIMIZED ? srgb_encode_host(d.color[c]) : unorm8_host(d.color[c]);
+        b[3] = 255;
+        memcpy(&d.const_bytes, b, 4);
+    } else if (l.kind == RenderLayout::Color) {
+        d.fast |= dev::FAST_LUT;
+    }
+    auto integral = [](float v) { return v == std::rint(v) && std::fabs(v) <= 4096.0f; };
+    if (l.kind == RenderLayout::ChildNode && tex_index >= 0 && tex_w <= 4096 && tex_h <= 4096 &&
+        l.width == (float)tex_w && l.crop.width == (float)tex_w && l.height == (float)tex_h &&
+        l.crop.height == (float)tex_h && integral(l.left) && integral(l.top) && l.crop.left == 0.0f &&
+        l.crop.top == 0.0f) {
+        // 1:1 mapping on whole texels: the NC-6 tap is texel (px - left, py - top) with weight exactly 1
+        // (|coordinate error| < 1e-3 << 1/512, the 8-bit weight rounds to 0 or 1)
+        d.fast |= dev::FAST_IDENT;
+        if (plan_.tex[tex_index].opaque) d.fast |= dev::FAST_OPAQUE;
+        d.tx_off = -(int)l.left; d.ty_off = -(int)l.top;
+    } else if (l.kind == RenderLayout::ChildNode && tex_index >= 0 && plan_.tex[tex_index].opaque && l.width > 0.0f &&
+               l.height > 0.0f &&
+               (plan_.tex[tex_index].tex.kind == dev::TEX_RGBA8 ||
+                (opts_.rendering_mode == SMR_MODE_CPU_OPTIMIZED &&
+                 (plan_.tex[tex_index].tex.kind == dev::TEX_NV12 || plan_.tex[tex_index].tex.kind == dev::TEX_YUV420)))) {
+        // opaque child at a fractional position / size: filtered sample alone, target ignored.  RGBA8: a
+        // resampled child; planar 4:2:0 / NV12 in CpuOptimized: the layout shader's own bilinear scaling of
+        // the (virtual) node texture, K1/K2 evaluated per tap quad
+        d.fast |= dev::FAST_SAMPLE | dev::FAST_OPAQUE;
+        const dev::Tex &tt = plan_.tex[tex_index].tex;
+        if (tt.kind != dev::TEX_RGBA8 && ((tex_w | tex_h) & 1) == 0 && tex_w <= 4096 && tex_h <= 4096 &&
+            l.width * 2.0f == (float)tex_w && l.height * 2.0f == (float)tex_h && l.crop.left == 0.0f && l.crop.top == 0.0f &&
+            l.crop.width == (float)tex_w && l.crop.height == (float)tex_h && integral(l.left) && integral(l.top) &&
+            ((int)l.left & 1) == 0 && (tt.pitch0 & 3) == 0 && ((uintptr_t)tt.p0 & 3) == 0) {
+            // exact 2:1 on whole pixels (a 2x2 grid of same-size inputs): sample coordinate = 2 k + 1/2 with an error
+            // far below the 1/512 weight step, so the taps are the aligned texel quad at weights exactly 1/2
+            d.fast |= dev::FAST_HALF;
+            d.tx_off = -(int)l.left; d.ty_off = -(int)l.top;
         }
     }
-    skip = false;
 }
 
 // An RGBA8 result of w x h for the caller: `launch` writes it into `rgba` itself (device memory) or into pre_out_, which is
@@ -1612,6 +1635,11 @@ smr_status Renderer::plan_output(Output &o, smr_output_frame &of, uint64_t pts) 
         size_t user_pitch = of.pitch[p] ? of.pitch[p] : row_bytes[p];
         if (user_pitch < row_bytes[p]) { set_error("output plane pitch is smaller than a row"); return SMR_ERR_INVALID_ARGUMENT; }
         if (of.mem_kind == SMR_MEM_DEVICE) {
+            // every kernel that writes RGBA8 stores whole pixels (4-byte words); YUV planes may start at any byte
+            if (o.format == SMR_OUT_RGBA8 && (((uintptr_t)of.planes[p] | user_pitch) & 3)) {
+                set_error("device RGBA8 output planes are 4-byte aligned (pointer and pitch)");
+                return SMR_ERR_INVALID_ARGUMENT;
+            }
             dst[p] = (uint8_t *)of.planes[p];
             pitch[p] = (int)user_pitch;
         } else {
@@ -1699,16 +1727,7 @@ smr_status Renderer::plan_output(Output &o, smr_output_frame &of, uint64_t pts) 
         prepare_layer(l, W, H, tex_index, tex_w, tex_h, d, skip);
         if (skip) continue;
         d.mask_begin = (int)masks.size();
-        size_t nm = std::min<size_t>(l.masks.size(), SMR_MAX_MASKS);  // params.rs:284-294
-        for (size_t i = 0; i < nm; i++) {
-            const Mask &m = l.masks[i];
-            dev::MaskDev md;
-            md.radius[0] = m.radius.top_left; md.radius[1] = m.radius.top_right;
-            md.radius[2] = m.radius.bottom_right; md.radius[3] = m.radius.bottom_left;
-            md.top = m.top; md.left = m.left; md.width = m.width; md.height = m.height;
-            masks.push_back(md);
-        }
-        d.mask_count = (int)nm;
+        d.mask_count = layer_masks(l, masks);
         layers.push_back(d);
     }
 
@@ -2010,6 +2029,49 @@ smr_status Renderer::debug_fused_jobs(smr_fused_job_info *out, uint32_t cap, uin
         o.dst_width = (uint32_t)j.dst_w; o.dst_height = (uint32_t)j.dst_h;
         o.taps_h = j.taps_h; o.taps_v = j.taps_v;
         o.direct = f.direct_off != SIZE_MAX ? 1 : 0;
+    }
+    return SMR_OK;
+}
+
+// inspection: the layers of the last planned tick's composite jobs, as render_begin packed and launched them
+smr_status Renderer::debug_composite_layers(smr_composite_layer_info *out, uint32_t cap, uint32_t *n) {
+    if (!n) return SMR_ERR_INVALID_ARGUMENT;
+    std::lock_guard<std::mutex> g(mu_);
+    size_t total = 0;
+    for (const CompositeRec &c : plan_.composites) total += (size_t)c.job.n_layers;
+    *n = (uint32_t)total;
+    if (!out) return SMR_OK;
+    if (cap < total) return SMR_ERR_BUFFER_TOO_SMALL;
+    // launch_composite's choice
+    const int kernel = plan_.composites.size() == 1 && plan_.composites[0].job.n_layers <= dev::kCompositeParamLayers
+                           ? SMR_COMPOSITE_PARAM : SMR_COMPOSITE_MULTI;
+    size_t k = 0;
+    for (size_t ci = 0; ci < plan_.composites.size(); ci++) {
+        const CompositeRec &c = plan_.composites[ci];
+        const dev::LayerDev *layers = reinterpret_cast<const dev::LayerDev *>(param_host_.data() + c.layers_off);
+        for (int li = 0; li < c.job.n_layers; li++, k++) {
+            const dev::LayerDev &L = layers[li];
+            smr_composite_layer_info &o = out[k];
+            memset(&o, 0, sizeof(o));
+            o.job = (int32_t)ci; o.kernel = kernel; o.layer = li;
+            o.type = L.type; o.rotated = L.rotated; o.fast = L.fast;
+            const int32_t box[12] = {L.px0, L.px1, L.py0, L.py1, L.ix0, L.ix1, L.iy0, L.iy1, L.jx0, L.jx1, L.jy0, L.jy1};
+            memcpy(o.box, box, sizeof(box));
+            o.tx_off = L.tx_off; o.ty_off = L.ty_off;
+            o.mask_count = L.mask_count;
+            if (L.type == 0 && L.tex >= 0) {
+                const dev::Tex &t = plan_.tex[L.tex].tex;
+                const uint8_t *p[3] = {t.p0, t.p1, t.p2};
+                const int32_t pitch[3] = {t.pitch0, t.pitch1, t.pitch2};
+                o.tex_kind = t.kind; o.tex_width = t.width; o.tex_height = t.height;
+                for (int pl = 0; pl < 3; pl++) {
+                    o.tex_pitch[pl] = p[pl] ? pitch[pl] : 0;
+                    o.tex_align[pl] = (int32_t)((uintptr_t)p[pl] & 15);
+                }
+            }
+            o.width = c.job.width; o.height = c.job.height;
+            o.out_format = c.job.out_format;
+        }
     }
     return SMR_OK;
 }
@@ -2418,6 +2480,29 @@ smr_status smr_debug_layouts(smr_renderer *r, const char *output_id, uint64_t pt
                              uint32_t *n, uint32_t *rw, uint32_t *rh) { SMR_GUARD(r->impl.debug_layouts(output_id, pts, out, cap, n, rw, rh)) }
 smr_status smr_debug_set_inputs(smr_renderer *r, uint64_t pts, const smr_input_frame *in, uint32_t n_in) { SMR_GUARD(r->impl.debug_set_inputs(pts, in, n_in)) }
 smr_status smr_debug_fused_jobs(smr_renderer *r, smr_fused_job_info *out, uint32_t cap, uint32_t *n) { SMR_GUARD(r->impl.debug_fused_jobs(out, cap, n)) }
+smr_status smr_debug_composite_layers(smr_renderer *r, smr_composite_layer_info *out, uint32_t cap, uint32_t *n) {
+    SMR_GUARD(r->impl.debug_composite_layers(out, cap, n))
+}
+smr_status smr_debug_interior(const smr_render_layout *layout, uint32_t width, uint32_t height, int32_t box[12], uint8_t *shortcut) {
+    if (!layout || !box || width == 0 || height == 0 || width > 16384 || height > 16384) return SMR_ERR_INVALID_ARGUMENT;
+    if (layout->type < 0 || layout->type > 2 || layout->masks_len < 0 || layout->masks_len > SMR_MAX_MASKS) return SMR_ERR_INVALID_ARGUMENT;
+    try {
+        const smr::RenderLayout l = smr::layout_from_c(*layout);
+        smr::dev::LayerDev d;
+        const bool drawn = smr::layer_geometry(l, (int)width, (int)height, d);
+        const int32_t b[12] = {d.px0, d.px1, d.py0, d.py1, d.ix0, d.ix1, d.iy0, d.iy1, d.jx0, d.jx1, d.jy0, d.jy1};
+        for (int i = 0; i < 12; i++) box[i] = drawn ? b[i] : 0;
+        if (shortcut) {
+            memset(shortcut, 0, (size_t)width * height);
+            std::vector<smr::dev::MaskDev> masks;
+            d.mask_count = smr::layer_masks(l, masks);
+            for (int y = drawn ? d.py0 : 0; y < (drawn ? d.py1 : 0); y++)
+                for (int x = d.px0; x < d.px1; x++)   // an axis-aligned layer covers its whole box
+                    shortcut[(size_t)y * width + x] = smr::dev::interior_shortcut(d, masks.data(), x, y) ? 1 : 0;
+        }
+        return SMR_OK;
+    } catch (...) { return SMR_ERR_OUT_OF_MEMORY; }
+}
 smr_status smr_comm_get_unique_id(uint8_t id[128]) {
     if (!id) return SMR_ERR_INVALID_ARGUMENT;
     std::string err;

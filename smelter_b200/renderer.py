@@ -642,6 +642,24 @@ class Renderer:
             out.append(d)
         return out
 
+    def debug_composite_layers(self):
+        """The layers of the last planned tick's composite jobs (smr_debug_composite_layers), one dict per layer in job
+        order, then painter's order: job, kernel ("p" / "multi"), layer, type, rotated, fast, box (12 ints: pixel box and
+        both interior bars), tx_off, ty_off, mask_count, tex_kind, tex_width, tex_height, tex_pitch, tex_align, width,
+        height, out_format."""
+        n = C.c_uint32()
+        self._check(self._lib.smr_debug_composite_layers(self._h, None, 0, C.byref(n)))
+        arr = (F.CompositeLayerInfo * max(1, n.value))()
+        self._check(self._lib.smr_debug_composite_layers(self._h, arr, n.value, C.byref(n)))
+        out = []
+        for j in arr[:n.value]:
+            d = {k: getattr(j, k) for k, _ in F.CompositeLayerInfo._fields_}
+            for k in ("box", "tex_pitch", "tex_align"):
+                d[k] = tuple(d[k])
+            d["kernel"] = "p" if j.kernel == F.COMPOSITE_PARAM else "multi"
+            out.append(d)
+        return out
+
     def stats(self):
         s = F.Stats()
         self._check(self._lib.smr_get_stats(self._h, C.byref(s)))
