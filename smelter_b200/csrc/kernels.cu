@@ -536,7 +536,7 @@ int launch_resample(const ResampleJob *jobs_dev, const ResampleJob *jobs_host, i
 // Template parameter S: 0 = any ratio <= 4 (per-column weights and first-tap indices from shared memory);
 // 2, 3, 4 = INTEGER horizontal ratio with a zero crop offset -- every grid / mosaic of the BASELINE configs.  Then first(o) = S*o + const and every output column
 // has the same TAPS = 6S+1 weights (exact small-integer arithmetic in resample.wgsl:45-50), which allows:
-//   * weights in CONSTANT memory: the FFMA reads them as c[bank][offset] operands, no register, no load;
+//   * weights as immediates: every FFMA takes int_weight<S>(j) from int_weights.h, as k_resample_tma3 does;
 //   * register blocking: a lane produces 2 adjacent output columns from one (S+TAPS)-long window;
 //   * 64-column strips (less horizontal halo), one source row per warp step, so only ~4 KB of shared memory
 //     per warp and 3 blocks (24 warps) per SM;
@@ -549,15 +549,6 @@ int launch_resample(const ResampleJob *jobs_dev, const ResampleJob *jobs_host, i
 #define W64_TW 64
 #define W64_WARPS 8
 #define W64_RING 64
-
-// k_resample_fused_int's weights (k_resample_tma3 has them compiled in: int_weights.h)
-__constant__ float c_wint[5][32];   // [S][tap]
-__constant__ float c_winv[5];       // 1 / weight_sum
-
-void set_int_weights(int S, const float *weights_dev, const float *inv_dev, int taps, Stream s) {
-    cudaMemcpyToSymbolAsync(c_wint, weights_dev, sizeof(float) * taps, sizeof(float) * 32 * S, cudaMemcpyDeviceToDevice, (cudaStream_t)s);
-    cudaMemcpyToSymbolAsync(c_winv, inv_dev, sizeof(float), sizeof(float) * S, cudaMemcpyDeviceToDevice, (cudaStream_t)s);
-}
 
 template <int S>   // S = 0: any ratio <= 4 (weights per column from shared memory)
 struct W64 {
@@ -575,6 +566,11 @@ struct W64 {
     // pixels) start 2*S+1 float4 apart -- conflict-free LDS.128; any-ratio rows are stored densely
     static __device__ __forceinline__ int pos(int i) { return S == 0 ? i : i + i / (2 * SS); }
 };
+// The host sends a job here at any ratio <= 4 with at most kFusedMaxTaps taps per axis and checks no span or ring bound:
+// at those limits a strip's source span, ceil(63 * ratio) + taps + 2 pixels, fits a row, and the source rows of eight
+// output rows, ceil(7 * ratio) + taps + 2, fit the ring.
+static_assert((W64_TW - 1) * 4 + kFusedMaxTaps + 2 <= W64<0>::SPAN, "a strip's source span must fit a row");
+static_assert((W64_WARPS - 1) * 4 + kFusedMaxTaps + 2 <= W64_RING, "eight output rows' source rows must fit the ring");
 
 // Pull [p, p + bytes) towards L2, clipped to the plane [lo, hi): one bulk prefetch of exactly the span (16-byte
 // granules) instead of whole 128-byte lines -- neighbouring strips' lines are not dragged in a second time.
@@ -629,7 +625,7 @@ __global__ void __launch_bounds__(32 * W64_WARPS, 3) k_resample_fused_int(const 
         }
         __syncthreads();
     } else {
-        inv0 = inv1 = c_winv[S];
+        inv0 = inv1 = int_inv<S>();
     }
     // S > 0: the strip's pair count is a constant (d0 = 1 needs one pair less for S = 3; the extra one is harmless)
     constexpr int NP = ((W64_TW - 1) * K::SS + TAPS + 2) >> 1, NIT = (NP + 31) / 32;
@@ -800,8 +796,8 @@ __global__ void __launch_bounds__(32 * W64_WARPS, 3) k_resample_fused_int(const 
 #pragma unroll
                     for (int j = 0; j < WIN; j++) {
                         const float4 v = sp[K::pos(j)];
-                        if (j < TAPS) { const float w = c_wint[S][j]; r0 = fmaf(v.x, w, r0); g0 = fmaf(v.y, w, g0); b0 = fmaf(v.z, w, b0); }
-                        if (j >= S) { const float w = c_wint[S][j - S]; r1 = fmaf(v.x, w, r1); g1 = fmaf(v.y, w, g1); b1 = fmaf(v.z, w, b1); }
+                        if (j < TAPS) { const float w = int_weight<S>(j); r0 = fmaf(v.x, w, r0); g0 = fmaf(v.y, w, g0); b0 = fmaf(v.z, w, b0); }
+                        if (j >= S) { const float w = int_weight<S>(j - S); r1 = fmaf(v.x, w, r1); g1 = fmaf(v.y, w, g1); b1 = fmaf(v.z, w, b1); }
                     }
                 }
                 ringrow[lane] = __floats2half2_rn(r0 * inv0, r1 * inv1);  // NC-5

@@ -159,8 +159,9 @@ struct FusedJob {
 struct FusedPiece {
     int32_t job, strip, oy_begin, oy_end;
 };
-// limits the host checks before choosing the fused kernel (mirrors FS_* in kernels.cu)
-constexpr int kFusedStripCols = 64, kFusedWarps = 8, kFusedRing = 64, kFusedSpan = 280, kFusedMaxTaps = 25;
+// LDG-staged kernel: output columns per strip, warps per block, and the taps per axis the host admits to any fused kernel
+// (kernels.cu asserts that the LDG kernel's row and ring hold every ratio <= 4 within them)
+constexpr int kFusedStripCols = 64, kFusedWarps = 8, kFusedMaxTaps = 25;
 // TMA-staged kernels: output columns per strip, ring rows (>= taps_v + ceil(7 * vertical scale)), box sizes of the
 // tensor maps the host encodes (bytes x rows; NV12 chroma in u16 texels)
 constexpr int kTmaStripCols4 = 58, kTmaStripCols2 = 122, kTmaRing4 = 54, kTmaRing2 = 28;
@@ -173,7 +174,7 @@ constexpr int kTma0Window[4] = {20, 25, 29, 33};
 // launch range)
 struct FusedKernel {
     enum Kind : int32_t {
-        LDG,      // k_resample_fused_int: LDG-staged, weights from smem (ratio 0) or the constant bank (integer ratio 2 / 3 / 4)
+        LDG,      // k_resample_fused_int: LDG-staged, weights from smem (ratio 0) or from int_weights.h (integer ratio 2 / 3 / 4)
         TMA_INT,  // k_resample_tma3 (resample_tma3.cuh): integer ratio 2 / 4, TMA-staged, weights from int_weights.h
         TMA_ANY,  // k_resample_tma0 (resample_tma0.cuh): any ratio <= 4, TMA-staged, a tap loop of kTma0Window[window] slots;
                   // with `box` on a source box-reduced 2:1
@@ -255,9 +256,6 @@ int launch_text(const TextJob &job, Stream s);
 // full_range: fused_launch_range of every job of the launch
 int launch_resample_fused(const FusedKernel &k, int src, int full_range, const FusedJob *jobs_dev, const FusedPiece *pieces_dev,
                           const int *piece_begin_dev, int nblocks, Stream s);
-// integer-ratio LDG kernel: the (single-phase) weight row of ratio S goes to constant memory, once per mapping (the
-// TMA kernel has it compiled in: int_weights.h)
-void set_int_weights(int S, const float *weights_dev, const float *inv_dev, int taps, Stream s);
 // every output of a tick in one launch; jobs_dev[i] == jobs_host[i], layers / masks / textures device pointers.  One output
 // with a short layer list (layers0_host: host copy of jobs_host[0].layers) passes job and layers in the parameter block
 int launch_composite(const CompositeJob *jobs_dev, const CompositeJob *jobs_host, const LayerDev *layers0_host, int n, Stream s);

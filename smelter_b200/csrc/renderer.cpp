@@ -442,8 +442,6 @@ class Renderer {
         }
     } plan_;
     void plan_tiles(Output &o, CompositeRec &pc, const std::vector<dev::LayerDev> &layers, int W, int H);
-    bool int_weights_set_[5] = {false, false, false, false, false};
-    std::vector<std::pair<int, WeightEntry>> pending_int_weights_;
     std::vector<WeightKey> new_weight_keys_;   // cache entries whose k_weights launch is not enqueued yet
     void rollback_weights();                   // a tick that fails before that launch must not leave them behind
     // TMA kernels of the fused resample: descriptors of the source planes, cached per (pointer, pitch, size, kind)
@@ -876,17 +874,35 @@ int Renderer::try_fused_resample(Input &in, const AxisMapping &hm_in, const Axis
     float sh = hm.scale(), sv = vm.scale();
     if (!(sh > 0.0f) || !(sv > 0.0f) || !(sh <= 4.001f) || !(sv <= 4.001f)) return -1;
     int th = resample_taps(sh), tv = resample_taps(sv);
+    // at most kFusedMaxTaps taps keeps both ratios <= 4, where the LDG kernel takes any job (kernels.cu asserts its bounds)
     if (th > dev::kFusedMaxTaps || tv > dev::kFusedMaxTaps) return -1;
-    if (!box) {
-        if ((int)std::ceil((dev::kFusedStripCols - 1) * sh) + th + 2 > dev::kFusedSpan) return -1;
-        if ((int)std::ceil((dev::kFusedWarps - 1) * sv) + tv + 2 > dev::kFusedRing) return -1;
-    } else {
-        int cols = 64;
-        const int max_span = dev::kTma0MaxSpan / 2;
-        while (cols > 2 && (int)std::ceil((cols - 1) * sh) + th + 3 > max_span) cols -= 2;
-        if ((int)std::ceil((cols - 1) * sh) + th + 3 > max_span) return -1;
-        if ((int)std::ceil((dev::kFusedWarps - 1) * sv) + tv + 1 > dev::kTmaRing4) return -1;
+    // the kernel is chosen before anything is allocated for it.  TMA-staged kernels: planar 4:2:0 / NV12 planes a
+    // descriptor can address (16-byte aligned rows), even target width, the vertical footprint of 8 output rows inside the ring
+    const bool tma = src_class < 2 && (dw & 1) == 0;
+    const int rows8 = (int)std::ceil((dev::kFusedWarps - 1) * sv) + tv + 1;
+    dev::FusedKernel k;   // LDG, weights from smem
+    int tmap_idx = -1, cols = 64;
+    if (!box && hm.crop_offset == 0.0f && (sh == 2.0f || sh == 3.0f || sh == 4.0f)) k.ratio = (int)sh;   // LDG, int_weights.h
+    if (tma && (k.ratio == 2 || k.ratio == 4) && rows8 <= (k.ratio == 4 ? dev::kTmaRing4 : dev::kTmaRing2) &&
+        (tmap_idx = source_tmaps(t, src_class)) >= 0) {
+        k.kind = dev::FusedKernel::TMA_INT;
+    } else if (tma && th <= dev::kTma0MaxTaps && rows8 <= dev::kTmaRing4) {
+        // any other ratio <= 4 (fractional, 3, with a crop offset, box-reduced): the any-ratio TMA kernel; its strips are
+        // narrowed so that a strip's source span fits the 256 pixels a warp converts per row (= 128 reduced ones)
+        const int max_span = box ? dev::kTma0MaxSpan / 2 : dev::kTma0MaxSpan;
+        auto span = [&](int c) { return (int)std::ceil((c - 1) * sh) + th + 3; };
+        while (cols > 2 && span(cols) > max_span) cols -= 2;
+        // slots of a lane's window: taps + the widest distance of two adjacent columns' first taps + the pad slots crossed
+        // (an integer ratio without offset is exact in f32: the distance is the ratio; otherwise floor + 1 bounds it, and the
+        // kernel traps rather than drop a tap should rounding ever exceed that)
+        const int gmax = (sh == std::floor(sh) && hm.crop_offset == 0.0f) ? (int)sh : (int)std::floor(sh) + 1;
+        const int win = th + gmax, winp = win + ((7 + win - 1) >> 3);
+        int bucket = 0;
+        while (bucket < 4 && dev::kTma0Window[bucket] < winp) bucket++;
+        if (bucket < 4 && span(cols) <= max_span && (tmap_idx = source_tmaps(t, src_class)) >= 0)
+            k = {dev::FusedKernel::TMA_ANY, 0, bucket, box ? 1 : 0};
     }
+    if (box && k.kind != dev::FusedKernel::TMA_ANY) return -1;   // no other fused kernel reduces: generic passes
     WeightEntry wh, wv;
     if (get_weights(passes[0], wh) != SMR_OK || get_weights(passes[1], wv) != SMR_OK) return -2;
     size_t dst_off = frame_alloc((size_t)dw * dh * 4);
@@ -895,44 +911,11 @@ int Renderer::try_fused_resample(Input &in, const AxisMapping &hm_in, const Axis
     j.taps_h = wh.taps; j.taps_v = wv.taps;
     j.w_h = wh.weights; j.inv_h = wh.inv; j.first_h = wh.first;
     j.w_v = wv.weights; j.inv_v = wv.inv; j.first_v = wv.first;
-    dev::FusedKernel k;   // LDG, weights from smem
-    int tmap_idx = -1;
-    if (!box && hm.crop_offset == 0.0f && (sh == 2.0f || sh == 3.0f || sh == 4.0f)) {
-        k.ratio = (int)sh;   // LDG, constant-bank weights
-        if (!int_weights_set_[k.ratio]) {   // enqueued after k_weights of this tick (same stream)
-            int_weights_set_[k.ratio] = true;
-            pending_int_weights_.push_back({k.ratio, wh});
-        }
-        // TMA-staged kernel: ratio 2 or 4, planar 4:2:0 / NV12 planes a descriptor can address (16-byte aligned rows),
-        // even target width, the vertical footprint of 8 output rows inside the ring
-        const int ring = k.ratio == 4 ? dev::kTmaRing4 : dev::kTmaRing2;
-        if ((k.ratio == 2 || k.ratio == 4) && src_class < 2 && (dw & 1) == 0 &&
-            (int)std::ceil((dev::kFusedWarps - 1) * sv) + tv + 1 <= ring && (tmap_idx = source_tmaps(t, src_class)) >= 0) {
-            j.v_same = vm.crop_offset == 0.0f && sv == sh && tv == th;
-            k.kind = dev::FusedKernel::TMA_INT;
-        }
+    if (k.kind == dev::FusedKernel::TMA_INT) j.v_same = vm.crop_offset == 0.0f && sv == sh && tv == th;
+    if (k.kind == dev::FusedKernel::TMA_ANY) {
+        j.strip_cols = cols;
+        j.lane_perm = lane_perm(sh, hm.crop_offset, dw, cols);   // nullptr (identity) if the table could not be made
     }
-    if (k.kind == dev::FusedKernel::LDG && src_class < 2 && (dw & 1) == 0 && th <= dev::kTma0MaxTaps &&
-        (int)std::ceil((dev::kFusedWarps - 1) * sv) + tv + 1 <= dev::kTmaRing4) {
-        // any other ratio <= 4 (fractional, 3, with a crop offset): the any-ratio TMA kernel; its strips are narrowed so that
-        // a strip's source span fits the 256 pixels a warp converts per row
-        int cols = 64;
-        const int max_span = box ? dev::kTma0MaxSpan / 2 : dev::kTma0MaxSpan;   // the row buffer holds 256 source pixels = 128 reduced ones
-        while (cols > 2 && (int)std::ceil((cols - 1) * sh) + th + 3 > max_span) cols -= 2;
-        // slots of a lane's window: taps + the widest distance of two adjacent columns' first taps + the pad slots crossed
-        // (an integer ratio without offset is exact in f32: the distance is the ratio; otherwise floor + 1 bounds it, and the
-        // kernel traps rather than drop a tap should rounding ever exceed that)
-        const int gmax = (sh == std::floor(sh) && hm.crop_offset == 0.0f) ? (int)sh : (int)std::floor(sh) + 1;
-        const int win = th + gmax, winp = win + ((7 + win - 1) >> 3);
-        int bucket = 0;
-        while (bucket < 4 && dev::kTma0Window[bucket] < winp) bucket++;
-        if (bucket < 4 && (int)std::ceil((cols - 1) * sh) + th + 3 <= max_span && (tmap_idx = source_tmaps(t, src_class)) >= 0) {
-            j.strip_cols = cols;
-            j.lane_perm = lane_perm(sh, hm.crop_offset, dw, cols);   // nullptr (identity) if the table could not be made
-            k = {dev::FusedKernel::TMA_ANY, 0, bucket, box ? 1 : 0};
-        }
-    }
-    if (box && k.kind != dev::FusedKernel::TMA_ANY) return -1;   // no other fused kernel reduces (the arena bytes stay unused this tick): generic passes
     plan_.fused.push_back({j, k, in.raw_tex, dst_off, tmap_idx, SIZE_MAX});
     dev::Tex out;
     out.kind = dev::TEX_RGBA8; out.width = dw; out.height = dh; out.pitch0 = dw * 4;
@@ -1014,8 +997,8 @@ bool Renderer::plane_tmap(const uint8_t *p, int pitch, int w, int h, int kind, C
     return true;
 }
 
-// Weight tables created by a tick whose k_weights launch was never enqueued hold uninitialised memory: drop them
-// (and the constant-bank flags that tick set) so that the next tick computes them.
+// Weight tables created by a tick whose k_weights launch was never enqueued hold uninitialised memory: drop them so that
+// the next tick computes them.
 void Renderer::rollback_weights() {
     for (const WeightKey &k : new_weight_keys_) {
         auto it = weights_.find(k);
@@ -1024,8 +1007,6 @@ void Renderer::rollback_weights() {
         weights_.erase(it);
     }
     new_weight_keys_.clear();
-    for (auto &pw : pending_int_weights_) int_weights_set_[pw.first] = false;
-    pending_int_weights_.clear();
     plan_.weight_jobs.clear();
 }
 
@@ -1942,8 +1923,6 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
     if (!launched(dev::launch_weights((const dev::WeightJob *)(pd + wj_off), plan_.weight_jobs.data(), (int)plan_.weight_jobs.size(),
                                       stream_))) goto fail;
     if (!plan_.weight_jobs.empty()) prof_mark(SMR_KERNEL_WEIGHTS);
-    for (auto &pw : pending_int_weights_) dev::set_int_weights(pw.first, pw.second.weights, pw.second.inv, pw.second.taps, stream_);
-    pending_int_weights_.clear();
     new_weight_keys_.clear();
     weight_guard.armed = false;   // the tables are being computed on the stream: the cache entries are good
     for (const FusedLaunch &fl : fused_launches) {

@@ -28,7 +28,7 @@ def device_weights(scale, offset, out_coord):
     return np.array(w[:taps.value], np.float32), np.float32(inv.value)
 
 
-@pytest.mark.parametrize("S", [2, 4])
+@pytest.mark.parametrize("S", [2, 3, 4])
 def test_header_weights_are_the_device_weights(S):
     w, inv = header_tables()[S]
     for o in (0, 5, 1919):

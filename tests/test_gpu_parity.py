@@ -570,7 +570,8 @@ def test_many_layers_beyond_the_parameter_bank():
 def test_failed_tick_does_not_poison_the_weight_cache():
     """A tick that fails AFTER planning (its second output is not registered) created Lanczos weight-cache entries whose
     k_weights launch never ran; the next good tick must recompute them (ADVICE r1: the cache used to keep the
-    uninitialised tables forever)."""
+    uninitialised tables forever).  Two scenes: a grid of two planar inputs, and one UYVY input at exactly 2:1 with a
+    zero crop offset, which the LDG-staged kernel resamples at integer ratio 2."""
     fr = inputs(2)
     scene = s.TilesComponent(children=streams(2), background_color=BG)
     r = TrackedRenderer()
@@ -583,6 +584,21 @@ def test_failed_tick_does_not_poison_the_weight_cache():
     del r._outputs["ghost"]
     got, exp, _ = run_case(scene, fr, renderer=r)
     assert_identical(got, exp, "good tick after a failed one")
+
+    # set_layouts makes the ratio exact: the crop is the whole 640 x 360 frame, the child 320 x 180
+    from tests.test_gpu_fused_variants import Job, check as check_fused, make_frame, scene_of
+    jobs = [Job("input_1", (0.0, 0.0, 640.0, 360.0), (320, 180))]
+    fr = {"input_1": make_frame("uyvy", "extreme", 23, 640, 360)}
+    W, H, ids, layouts, _ = scene_of(jobs)
+    r = s.Renderer()
+    r.register_input("input_1")
+    r.set_layouts(OUTPUT_ID, s.Resolution(W, H), RGBA, (W, H), ids, layouts)
+    r._outputs["ghost"] = (RES, YUV)
+    with pytest.raises(s.RenderSceneError):
+        r.render(s.FrameSet(frames=fr, pts=0.0), outputs=[OUTPUT_ID, "ghost"])
+    assert [(f["kernel"], f["ratio"]) for f in r.debug_fused_jobs()] == [("ldg", 2)]   # planned by the failed tick
+    del r._outputs["ghost"]
+    check_fused(jobs, fr, expect=[{"kernel": "ldg", "ratio": 2}], renderer=r, what="UYVY 2:1 good tick after a failed one")
 
 
 def test_pitch_smaller_than_a_row_is_refused():

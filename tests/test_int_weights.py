@@ -1,4 +1,4 @@
-"""The compiled-in weights of the integer-ratio TMA kernel (smelter_b200/csrc/int_weights.h) against the oracle's weight
+"""The compiled-in weights of the integer-ratio kernels (smelter_b200/csrc/int_weights.h) against the oracle's weight
 code, bit for bit, and the header against its generator (tools/gen_int_weights.py)."""
 import os
 import re
@@ -22,7 +22,7 @@ def header_tables():
     return res
 
 
-@pytest.mark.parametrize("S", [2, 4])
+@pytest.mark.parametrize("S", [2, 3, 4])
 def test_header_weights_are_the_oracle_weights(S):
     """every tap and 1 / weight_sum of the S:1 mapping, at several output coordinates (the table is the same for all)"""
     w, inv = header_tables()[S]
