@@ -156,7 +156,11 @@ typedef struct {                   /* one entry of FrameSet<InputId> */
  *    read pixel pairs and {u, v} pairs); planar U and V planes may start at any byte.
  * Host planes are copied into aligned buffers and have no such rule.
  * The same holds for SMR_MEM_DEVICE planes of smr_output_frame: an RGBA8 output plane is 4-byte aligned, pointer and
- * pitch (SMR_ERR_INVALID_ARGUMENT before any kernel is launched otherwise); YUV output planes may start at any byte. */
+ * pitch (SMR_ERR_INVALID_ARGUMENT before any kernel is launched otherwise); YUV output planes may start at any byte.
+ * Crops of texture layouts (smr_set_layouts): every crop field must be finite (SMR_ERR_INVALID_ARGUMENT otherwise).  A crop
+ * shrunk by more than 4:1 is first box-averaged by a power of two per axis; smr_render refuses, with
+ * SMR_ERR_INVALID_ARGUMENT before any kernel is launched, a layout whose box pass would average more than 2^24 source
+ * texels per reduced texel -- the most a crop inside a 16384 x 16384 frame needs to reach one pixel. */
 
 typedef enum {                     /* OutputFrameFormat, types.rs:187-194 */
     SMR_OUT_PLANAR_YUV420 = 0,     /* PlanarYuv420Bytes */
@@ -303,10 +307,15 @@ smr_status smr_debug_partition(const int32_t *dst_w, const int32_t *dst_h, uint3
  * bars), opaque (the interior replaces the target), job (fused resample job that could write the layer's tiles itself, -1:
  * none)}.  owner_layer[t]: the layer whose job finishes tile t directly, or -1; tiles[]: the tiles left for the composite
  * ((ty << 16) | tx), most expensive first when `sorted` != 0, row-major otherwise. */
-/* inspection (needs a device): the Lanczos3 weights the weight kernel computes for output coordinate out_coord of the
- * mapping (scale, offset), read back: *taps of them into weights (when they fit in cap) and 1 / weight_sum into *inv. */
-smr_status smr_debug_weights(float scale, float offset, uint32_t out_coord, float *weights, uint32_t cap, uint32_t *taps,
-                             float *inv);
+/* inspection (needs a device): the Lanczos3 weight table the weight kernel computes for output coordinates 0 .. n_out - 1
+ * (1 <= n_out <= 16384) of the mapping (scale, offset), 0 < scale <= 1024, read back.  *taps is the tap count; weights
+ * receives n_out x *taps floats, row by row (SMR_ERR_BUFFER_TOO_SMALL when that exceeds cap); inv and first receive, per
+ * output coordinate, 1 / weight_sum and the index of the first tap. */
+smr_status smr_debug_weights(float scale, float offset, uint32_t n_out, float *weights, size_t cap, uint32_t *taps, float *inv,
+                             int32_t *first);
+/* inspection (needs a device): the weight kernel's sin and cos (f32 argument, evaluated in fp64, rounded to f32) of n
+ * host values x into host arrays s and c. */
+smr_status smr_debug_sincos(const float *x, uint32_t n, float *s, float *c);
 
 smr_status smr_debug_tile_plan(const int32_t *boxes, uint32_t n_layers, uint32_t width, uint32_t height, int32_t sorted,
                                int32_t *owner_layer, uint32_t owner_cap, uint32_t *tiles, uint32_t tiles_cap, uint32_t *n_tiles);
@@ -334,6 +343,31 @@ typedef struct {
     int32_t direct;                /* the job writes the output bytes of its direct tiles itself */
 } smr_fused_job_info;
 smr_status smr_debug_fused_jobs(smr_renderer *r, smr_fused_job_info *out, uint32_t cap, uint32_t *n);
+
+/* inspection (no device access): the generic resample passes of the handle's most recently planned tick -- every
+ * resampled child the fused kernels do not take -- one record per pass: box passes, then first passes, then last passes,
+ * each in plan order.  *n is the record count; records go to `out` when it is not NULL.  *n_convert is the number of
+ * k_convert jobs (input -> RGBA8 node texture) of the tick; convert_kinds, when not NULL, receives the texture kind each
+ * reads.  SMR_ERR_BUFFER_TOO_SMALL when a list does not fit its cap. */
+typedef enum { SMR_STAGE_BOX = 0, SMR_STAGE_FIRST = 1, SMR_STAGE_LAST = 2 } smr_resample_stage;
+typedef enum {
+    SMR_STAGE_SRC_RAW = 0,         /* the input's own texture (an RGBA8 input) */
+    SMR_STAGE_SRC_CONVERTED = 1,   /* the RGBA8 node texture k_convert wrote from an input of kind src_kind */
+    SMR_STAGE_SRC_F16 = 2          /* the half-precision result of the previous pass (src_kind 4) */
+} smr_stage_source;
+typedef struct {
+    int32_t stage;                 /* smr_resample_stage */
+    int32_t axis;                  /* Lanczos pass: 0 horizontal, 1 vertical; box pass: -1 */
+    int32_t box_fx, box_fy;        /* box pass: source texels averaged per axis; 1 x 1 for a Lanczos pass */
+    int32_t taps;                  /* Lanczos taps per output texel (0 for a box pass) */
+    int32_t perp_offset;           /* one-pass plan: integer offset along the other axis */
+    int32_t source;                /* smr_stage_source */
+    int32_t src_kind;              /* texture kind, as smr_composite_layer_info.tex_kind (4: half-precision RGBA) */
+    uint32_t src_width, src_height, dst_width, dst_height;
+    int32_t dst_f16;               /* 1: writes half-precision RGBA for the next pass, 0: the sRGB RGBA8 result */
+} smr_resample_stage_info;
+smr_status smr_debug_resample_stages(smr_renderer *r, smr_resample_stage_info *out, uint32_t cap, uint32_t *n,
+                                     int32_t *convert_kinds, uint32_t convert_cap, uint32_t *n_convert);
 
 /* inspection (no device needed): the composite's interior proof for one layout drawn into a width x height target.
  * Inside it every alpha factor of the fragment shader is exactly 1, so the layer paints its bare colour or sample there.

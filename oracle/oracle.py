@@ -75,6 +75,10 @@ def lib():
         _lib.orc_plan_passes.argtypes = [C.c_float] * 4 + [C.c_int, C.c_int, C.c_void_p, C.c_void_p]
         _lib.orc_resample_taps.argtypes = [C.c_float]
         _lib.orc_resample_weights.argtypes = [C.c_float, C.c_float, C.c_int, C.c_void_p, C.c_void_p]
+        _lib.orc_resample_table.argtypes = [C.c_float, C.c_float, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+        _lib.orc_resample_table.restype = None
+        _lib.orc_sincos_cr.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+        _lib.orc_sincos_cr.restype = None
         _lib.orc_resample.argtypes = [C.POINTER(Texture)] + [C.c_float] * 4 + [C.c_int, C.c_int, C.c_void_p]
     return _lib
 
@@ -252,6 +256,25 @@ def resample_weights(scale, offset, out_coord):
     ws = C.c_float()
     first = lib().orc_resample_weights(scale, offset, out_coord, _p(w), C.byref(ws))
     return first, w, ws.value
+
+
+def resample_table(scale, offset, n_out):
+    """every output coordinate of one mapping: (first (n_out,) int32, weights (n_out, taps) float32, 1 / weight_sum
+    (n_out,) float32), the reciprocal taken in f32 as the weight kernel does"""
+    taps = lib().orc_resample_taps(scale)
+    w = np.zeros((n_out, taps), np.float32)
+    first = np.empty(n_out, np.int32)
+    inv = np.empty(n_out, np.float32)
+    lib().orc_resample_table(scale, offset, n_out, _p(w), _p(inv), _p(first))
+    return first, w, inv
+
+
+def sincos_cr(x):
+    """NC-8: (sin, cos) of float32 array x, each correctly rounded to f32"""
+    x = np.ascontiguousarray(x, np.float32)
+    s, c = np.empty_like(x), np.empty_like(x)
+    lib().orc_sincos_cr(_p(x), x.size, _p(s), _p(c))
+    return s, c
 
 
 def resample(src_rgba, crop_left, crop_top, crop_w, crop_h, dst_w, dst_h):

@@ -118,6 +118,14 @@ float orc_f16_to_f32(uint16_t h) {
 static inline float sin_cr(float x) { return (float)sin((double)x); } /* NC-8 */
 static inline float cos_cr(float x) { return (float)cos((double)x); }
 
+void orc_sincos_cr(const float *x, int n, float *s, float *c) {
+#pragma omp parallel for schedule(static)
+    for (int i = 0; i < n; i++) {
+        s[i] = sin_cr(x[i]);
+        c[i] = cos_cr(x[i]);
+    }
+}
+
 /* ------------------------------------------------------------------------------------------ */
 /* NC-6: the one sampler the reference uses everywhere (wgpu/common_pipeline.rs:56-65):        */
 /* min/mag Linear, ClampToEdge                                                                 */
@@ -449,6 +457,15 @@ int orc_resample_weights(float scale, float offset, int out_coord, float *weight
     return (int)first;
 }
 
+void orc_resample_table(float scale, float offset, int n_out, float *weights, float *inv_wsum, int *first) {
+    int taps = orc_resample_taps(scale);
+    for (int o = 0; o < n_out; o++) {
+        float ws;
+        first[o] = orc_resample_weights(scale, offset, o, weights + (size_t)o * taps, &ws);
+        inv_wsum[o] = 1.0f / ws; /* `sum / weight_sum` evaluated as sum * (1/weight_sum) */
+    }
+}
+
 /* a linear-light float texture view used inside the resampler */
 typedef struct {
     int w, h;
@@ -474,11 +491,7 @@ static void rs_kernel_pass(const rs_src *s, int axis, float scale, float offset,
     float *wtab = (float *)malloc(sizeof(float) * (size_t)taps * n_out);
     float *inv = (float *)malloc(sizeof(float) * n_out);
     int *first = (int *)malloc(sizeof(int) * n_out);
-    for (int o = 0; o < n_out; o++) {
-        float ws;
-        first[o] = orc_resample_weights(scale, offset, o, wtab + (size_t)o * taps, &ws);
-        inv[o] = 1.0f / ws; /* `sum / weight_sum` evaluated as sum * (1/weight_sum) */
-    }
+    orc_resample_table(scale, offset, n_out, wtab, inv, first);
     int max_src = (axis == 1 ? s->h : s->w) - 1;
     int max_perp = (axis == 1 ? s->w : s->h) - 1;
 #pragma omp parallel for schedule(static)

@@ -114,6 +114,10 @@ int orc_resample(const orc_texture *src, float crop_left, float crop_top, float 
 int orc_resample_taps(float scale);
 int orc_resample_weights(float scale, float offset, int out_coord, float *weights,
                          float *weight_sum);
+/* the same for output coordinates 0 .. n_out - 1: weights (n_out x taps), 1 / weight_sum and first tap of each */
+void orc_resample_table(float scale, float offset, int n_out, float *weights, float *inv_wsum, int *first);
+/* NC-8, the sin / cos the weights use: s[i], c[i] = sin, cos of x[i] correctly rounded to f32 */
+void orc_sincos_cr(const float *x, int n, float *s, float *c);
 
 /* --- K9: apply_layouts (layout/shader.rs:93-167, params.rs:169-333, apply_layouts.wgsl) ---- */
 /* Draws `n` layouts (at most max_layouts, shader.rs:152) in order onto a transparent W x H

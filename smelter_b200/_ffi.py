@@ -127,6 +127,16 @@ class FusedJobInfo(C.Structure):   # smr_fused_job_info
                 ("taps_h", C.c_int32), ("taps_v", C.c_int32), ("direct", C.c_int32)]
 
 
+STAGE_BOX, STAGE_FIRST, STAGE_LAST = 0, 1, 2
+STAGE_SRC_RAW, STAGE_SRC_CONVERTED, STAGE_SRC_F16 = 0, 1, 2
+
+
+class ResampleStageInfo(C.Structure):   # smr_resample_stage_info
+    _fields_ = [("stage", C.c_int32), ("axis", C.c_int32), ("box_fx", C.c_int32), ("box_fy", C.c_int32), ("taps", C.c_int32),
+                ("perp_offset", C.c_int32), ("source", C.c_int32), ("src_kind", C.c_int32), ("src_width", C.c_uint32),
+                ("src_height", C.c_uint32), ("dst_width", C.c_uint32), ("dst_height", C.c_uint32), ("dst_f16", C.c_int32)]
+
+
 COMPOSITE_PARAM, COMPOSITE_MULTI = 0, 1
 
 
@@ -148,7 +158,7 @@ class KernelTimes(C.Structure):
 
 EXPORTS = [
     "smr_create", "smr_destroy", "smr_register_input", "smr_unregister_input", "smr_update_scene",
-    "smr_unregister_output", "smr_set_layouts", "smr_render", "smr_render_begin", "smr_render_end", "smr_preprocess_frame", "smr_premultiply_rgba8", "smr_render_text", "smr_debug_partition", "smr_debug_tile_plan", "smr_debug_weights", "smr_debug_fused_jobs", "smr_debug_composite_layers", "smr_debug_interior", "smr_output_plane_sizes",
+    "smr_unregister_output", "smr_set_layouts", "smr_render", "smr_render_begin", "smr_render_end", "smr_preprocess_frame", "smr_premultiply_rgba8", "smr_render_text", "smr_debug_partition", "smr_debug_tile_plan", "smr_debug_weights", "smr_debug_sincos", "smr_debug_fused_jobs", "smr_debug_resample_stages", "smr_debug_composite_layers", "smr_debug_interior", "smr_output_plane_sizes",
     "smr_component_default", "smr_debug_layouts", "smr_debug_set_inputs", "smr_get_stats", "smr_set_profiling", "smr_get_kernel_times",
     "smr_comm_get_unique_id", "smr_comm_init", "smr_comm_broadcast_inputs", "smr_comm_exchange_inputs", "smr_comm_pull_inputs", "smr_peer_pool_alloc", "smr_peer_pool_open", "smr_peer_pool_close", "smr_peer_pool_free", "smr_comm_destroy", "smr_host_register", "smr_host_unregister", "smr_cuda_stream", "smr_last_error",
     "smr_version",
@@ -191,11 +201,16 @@ def lib():
     L.smr_debug_tile_plan.argtypes = [C.POINTER(C.c_int32), C.c_uint32, C.c_uint32, C.c_uint32, C.c_int32, C.POINTER(C.c_int32), C.c_uint32,
                                       C.POINTER(C.c_uint32), C.c_uint32, C.POINTER(C.c_uint32)]
     L.smr_debug_tile_plan.restype = C.c_int32
-    L.smr_debug_weights.argtypes = [C.c_float, C.c_float, C.c_uint32, C.POINTER(C.c_float), C.c_uint32, C.POINTER(C.c_uint32),
-                                    C.POINTER(C.c_float)]
+    L.smr_debug_weights.argtypes = [C.c_float, C.c_float, C.c_uint32, C.c_void_p, C.c_size_t, C.POINTER(C.c_uint32), C.c_void_p,
+                                    C.c_void_p]
     L.smr_debug_weights.restype = C.c_int32
+    L.smr_debug_sincos.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
+    L.smr_debug_sincos.restype = C.c_int32
     L.smr_debug_fused_jobs.argtypes = [vp, C.POINTER(FusedJobInfo), C.c_uint32, C.POINTER(C.c_uint32)]
     L.smr_debug_fused_jobs.restype = C.c_int32
+    L.smr_debug_resample_stages.argtypes = [vp, C.POINTER(ResampleStageInfo), C.c_uint32, C.POINTER(C.c_uint32),
+                                            C.POINTER(C.c_int32), C.c_uint32, C.POINTER(C.c_uint32)]
+    L.smr_debug_resample_stages.restype = C.c_int32
     L.smr_debug_composite_layers.argtypes = [vp, C.POINTER(CompositeLayerInfo), C.c_uint32, C.POINTER(C.c_uint32)]
     L.smr_debug_composite_layers.restype = C.c_int32
     L.smr_debug_interior.argtypes = [C.POINTER(RenderLayout), C.c_uint32, C.c_uint32, C.POINTER(C.c_int32 * 12), C.c_void_p]

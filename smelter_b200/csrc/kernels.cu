@@ -244,7 +244,7 @@ __device__ __forceinline__ uchar4 node_texel(const Tables &T, const Tex &s, int 
             int cw = s.width / 2, ch = s.height / 2;
             if (((s.width | s.height) & 1) == 0) {
                 // Even sizes: the NC-6 taps are exactly texel (x,y) for luma and the .25/.75 pair for chroma
-                // (proved for every even size <= 8192 by oracle test test_even_size_sampler_phases_exhaustive).
+                // (proved for every even size <= 16384 by oracle test test_even_size_sampler_phases_exhaustive).
                 int x0 = (x & 1) ? (x >> 1) : max((x >> 1) - 1, 0), x1 = (x & 1) ? min((x >> 1) + 1, cw - 1) : (x >> 1);
                 int y0 = (y & 1) ? (y >> 1) : max((y >> 1) - 1, 0), y1 = (y & 1) ? min((y >> 1) + 1, ch - 1) : (y >> 1);
                 const int kx = (x & 1) ? 1 : 3, ky = (y & 1) ? 1 : 3;   // weight of the second tap, in quarters
@@ -408,13 +408,15 @@ __global__ void k_weights(const WeightJob *jobs) {
     J.first[o] = (int)fc;
 }
 
-// k_weights of one mapping read back: the taps weights of output coordinate out_coord and its 1 / weight_sum
-int debug_weights(float scale, float offset, int out_coord, float *w_host, int cap, int *taps_out, float *inv_host) {
+// k_weights of one mapping read back: the whole table, n_out x taps weights, and per output coordinate its 1 / weight_sum
+// and first tap
+int debug_weights(float scale, float offset, int n_out, float *w_host, size_t cap, int *taps_out, float *inv_host,
+                  int32_t *first_host) {
     const float ks = fmaxf(scale, 1.0f);
-    const int taps = (int)ceilf(2.0f * (3.0f * ks)) + 1, n_out = out_coord + 1;
+    const int taps = (int)ceilf(2.0f * (3.0f * ks)) + 1;
     *taps_out = taps;
-    if (out_coord < 0 || taps > cap) return 0;
     const size_t nw = (size_t)n_out * taps;
+    if (nw > cap) return 0;
     unsigned char *d = nullptr;
     if (cudaMalloc(&d, sizeof(WeightJob) + sizeof(float) * (nw + n_out) + sizeof(int32_t) * n_out) != cudaSuccess) return -1;
     WeightJob j{};
@@ -424,8 +426,31 @@ int debug_weights(float scale, float offset, int out_coord, float *w_host, int c
     j.first = reinterpret_cast<int32_t *>(j.inv_wsum + n_out);
     bool ok = cudaMemcpy(d, &j, sizeof(j), cudaMemcpyHostToDevice) == cudaSuccess &&
               launch_weights(reinterpret_cast<const WeightJob *>(d), &j, 1, nullptr) == 1 &&
-              cudaMemcpy(w_host, j.weights + (size_t)out_coord * taps, sizeof(float) * taps, cudaMemcpyDeviceToHost) == cudaSuccess &&
-              cudaMemcpy(inv_host, j.inv_wsum + out_coord, sizeof(float), cudaMemcpyDeviceToHost) == cudaSuccess;
+              cudaMemcpy(w_host, j.weights, sizeof(float) * nw, cudaMemcpyDeviceToHost) == cudaSuccess &&
+              cudaMemcpy(inv_host, j.inv_wsum, sizeof(float) * n_out, cudaMemcpyDeviceToHost) == cudaSuccess &&
+              cudaMemcpy(first_host, j.first, sizeof(int32_t) * n_out, cudaMemcpyDeviceToHost) == cudaSuccess;
+    cudaFree(d);
+    return ok ? 1 : -1;
+}
+
+__global__ void k_debug_sincos(const float *x, int n, float *s, float *c) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    s[i] = sin_cr(x[i]);
+    c[i] = cos_cr(x[i]);
+}
+
+// sin_cr / cos_cr, the NC-8 functions k_weights calls, on n host values
+int debug_sincos(const float *x_host, int n, float *s_host, float *c_host) {
+    float *d = nullptr;
+    if (cudaMalloc(&d, sizeof(float) * 3 * (size_t)n) != cudaSuccess) return -1;
+    bool ok = cudaMemcpy(d, x_host, sizeof(float) * n, cudaMemcpyHostToDevice) == cudaSuccess;
+    if (ok) {
+        k_debug_sincos<<<(n + 255) / 256, 256>>>(d, n, d + n, d + 2 * (size_t)n);
+        ok = check_launch("k_debug_sincos") &&
+             cudaMemcpy(s_host, d + n, sizeof(float) * n, cudaMemcpyDeviceToHost) == cudaSuccess &&
+             cudaMemcpy(c_host, d + 2 * (size_t)n, sizeof(float) * n, cudaMemcpyDeviceToHost) == cudaSuccess;
+    }
     cudaFree(d);
     return ok ? 1 : -1;
 }
@@ -475,7 +500,7 @@ __global__ void __launch_bounds__(256) k_resample(const ResampleJob *jobs) {
     int px = blockIdx.x * blockDim.x + threadIdx.x, py = blockIdx.y * blockDim.y + threadIdx.y;
     if (px >= J.dst_w || py >= J.dst_h) return;
     const Tex &S = J.src;
-    if (J.box_fx * J.box_fy > 1) {  // downsample.wgsl:28-41
+    if ((unsigned)J.box_fx * (unsigned)J.box_fy > 1u) {  // downsample.wgsl:28-41
         float4 sum = make_float4(0.f, 0.f, 0.f, 0.f);
         for (int dy = 0; dy < J.box_fy; dy++)
             for (int dx = 0; dx < J.box_fx; dx++) {

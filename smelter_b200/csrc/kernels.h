@@ -110,6 +110,10 @@ constexpr int kDirectTileW = 128, kDirectTileH = 16;   // = the composite's bloc
 // k_composite_multi otherwise
 constexpr int kCompositeParamLayers = 96;
 
+// Most source texels one box-pass texel averages: a crop inside a 16384 x 16384 source shrunk to one pixel needs
+// 2^12 x 2^12.  Planning refuses a layout that would need more (the box loop's trip count, which must fit 32 bits).
+constexpr uint64_t kMaxBoxTexels = 1ull << 24;
+
 // one Lanczos pass (resample.wgsl) or box pass (downsample.wgsl)
 struct ResampleJob {
     Tex src;                // TEX_RGBA8 (decoded through the srgb view), TEX_F16, or a YUV kind (fused K1/K2)
@@ -123,7 +127,7 @@ struct ResampleJob {
     const float *weights;   // [n_out][taps]
     const float *inv_wsum;  // [n_out]
     const int32_t *first;   // [n_out]
-    int32_t box_fx, box_fy; // box pass when box_fx*box_fy > 1 (then weights unused)
+    int32_t box_fx, box_fy; // box pass when box_fx*box_fy > 1 (then weights unused); the host keeps the product <= kMaxBoxTexels
 };
 
 // K1/K2 + both Lanczos passes fused (YUV source, horizontal pass first): see k_resample_fused
@@ -241,9 +245,11 @@ typedef void *Stream;  // cudaStream_t
 // each returns the number of kernels it launched (for smr_stats / bench gpu_launches)
 int launch_convert_to_rgba(const Tex &src, uint8_t *dst, int dst_pitch, Stream s);
 int launch_weights(const WeightJob *jobs_dev, const WeightJob *jobs_host, int n_jobs, Stream s);
-// k_weights for one mapping on the current device, synchronously: output coordinate out_coord's weights (*taps of them,
-// when they fit in cap) and 1 / weight_sum.  1 done, 0 cap too small, -1 CUDA error
-int debug_weights(float scale, float offset, int out_coord, float *w_host, int cap, int *taps, float *inv_host);
+// k_weights for one mapping on the current device, synchronously: the n_out x *taps weights (when they fit in cap), and
+// 1 / weight_sum and the first tap of every output coordinate.  1 done, 0 cap too small, -1 CUDA error
+int debug_weights(float scale, float offset, int n_out, float *w_host, size_t cap, int *taps, float *inv_host, int32_t *first_host);
+// NC-8's sin_cr / cos_cr (the functions k_weights calls) on n host values, synchronously.  1 done, -1 CUDA error
+int debug_sincos(const float *x_host, int n, float *s_host, float *c_host);
 int launch_resample(const ResampleJob *jobs_dev, const ResampleJob *jobs_host, int n_jobs, Stream s);
 // source class of the fused kernel's template: 0 planar 4:2:0, 1 NV12, 2 UYVY, 3 YUYV; -1 not supported
 inline int fused_source_class(int tex_kind) {

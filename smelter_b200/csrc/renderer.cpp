@@ -286,6 +286,8 @@ class Renderer {
                              uint32_t *rw, uint32_t *rh);
     smr_status debug_fused_jobs(smr_fused_job_info *out, uint32_t cap, uint32_t *n);
     smr_status debug_composite_layers(smr_composite_layer_info *out, uint32_t cap, uint32_t *n);
+    smr_status debug_resample_stages(smr_resample_stage_info *out, uint32_t cap, uint32_t *n, int32_t *convert_kinds,
+                                     uint32_t convert_cap, uint32_t *n_convert);
     void stats(smr_stats *s) { std::lock_guard<std::mutex> g(mu_); *s = stats_; }
     void *stream() { return (void *)stream_; }
     const char *last_error() { return err_.c_str(); }
@@ -688,6 +690,11 @@ smr_status Renderer::set_layouts(const char *output_id, uint32_t w, uint32_t h, 
         RenderLayout &l = ls[i];
         if (d.type < 0 || d.type > 2 || d.masks_len < 0 || d.masks_len > SMR_MAX_MASKS) { set_error("malformed layout"); return SMR_ERR_INVALID_ARGUMENT; }
         if (d.type == 0 && (d.child_index < 0 || (uint32_t)d.child_index >= n_children)) { set_error("child index outside child_ids"); return SMR_ERR_INVALID_ARGUMENT; }
+        if (d.type == 0 && !(std::isfinite(d.crop_top) && std::isfinite(d.crop_left) && std::isfinite(d.crop_width) &&
+                             std::isfinite(d.crop_height))) {
+            set_error("texture layout crop is not finite");
+            return SMR_ERR_INVALID_ARGUMENT;
+        }
         l = layout_from_c(d);
     }
     Output &o = outputs_[output_id];
@@ -757,7 +764,12 @@ static void set_tex_plane(dev::Tex &t, int p, const uint8_t *ptr, size_t pitch) 
     (p == 0 ? t.pitch0 : p == 1 ? t.pitch1 : t.pitch2) = (int)pitch;
 }
 
-static bool frame_size_ok(const smr_input_frame &f) { return f.width >= 2 && f.height >= 2 && f.width <= 16384 && f.height <= 16384; }
+// The largest input frame side.  The kernels' fixed .25 / .75 chroma taps for even 4:2:0 sizes are proved up to this bound
+// (tests/test_oracle_kat.py reads it from here).
+static constexpr uint32_t kMaxFrameDim = 16384;
+static bool frame_size_ok(const smr_input_frame &f) {
+    return f.width >= 2 && f.height >= 2 && f.width <= kMaxFrameDim && f.height <= kMaxFrameDim;
+}
 
 // The checks every reader of a caller's frame applies (smr_render, smr_preprocess_frame, the exchange calls)
 smr_status Renderer::read_frame(const smr_input_frame &f, FrameView &v) {
@@ -1545,9 +1557,13 @@ smr_status Renderer::child_texture(Input &in, RenderLayout &l, int &tex_index, i
         tex_index = fused_tex;
         plan_.resample_cache[key] = tex_index;
     } else {
-        int src_tex = materialised_input(in);
         int levels[2] = {hm.predecimate_levels(), vm.predecimate_levels()};
         int fac[2] = {1 << levels[0], 1 << levels[1]};
+        if ((uint64_t)fac[0] * (uint64_t)fac[1] > dev::kMaxBoxTexels) {
+            set_error("texture layout crop is too large for its size: the box pass would average more than 2^24 texels");
+            return SMR_ERR_INVALID_ARGUMENT;
+        }
+        int src_tex = materialised_input(in);
         int cur_w = in.tex.width, cur_h = in.tex.height;
         size_t cur_off = SIZE_MAX;  // SIZE_MAX: source is plan_.tex[src_tex]
         if (fac[0] != 1 || fac[1] != 1) {
@@ -2012,6 +2028,49 @@ smr_status Renderer::debug_fused_jobs(smr_fused_job_info *out, uint32_t cap, uin
     return SMR_OK;
 }
 
+// inspection: the generic resample passes and k_convert jobs of the last planned tick
+smr_status Renderer::debug_resample_stages(smr_resample_stage_info *out, uint32_t cap, uint32_t *n, int32_t *convert_kinds,
+                                           uint32_t convert_cap, uint32_t *n_convert) {
+    if (!n || !n_convert) return SMR_ERR_INVALID_ARGUMENT;
+    std::lock_guard<std::mutex> g(mu_);
+    size_t total = 0;
+    for (const auto &stage : plan_.stages) total += stage.size();
+    *n = (uint32_t)total;
+    *n_convert = (uint32_t)plan_.convert_jobs.size();
+    if ((out && cap < total) || (convert_kinds && convert_cap < plan_.convert_jobs.size())) return SMR_ERR_BUFFER_TOO_SMALL;
+    if (convert_kinds)
+        for (size_t i = 0; i < plan_.convert_jobs.size(); i++) convert_kinds[i] = plan_.tex[plan_.convert_jobs[i].first].tex.kind;
+    if (!out) return SMR_OK;
+    size_t k = 0;
+    for (int s = 0; s < 3; s++)
+        for (const StageRec &r : plan_.stages[s]) {
+            const dev::ResampleJob &j = r.job;
+            smr_resample_stage_info &o = out[k++];
+            memset(&o, 0, sizeof(o));
+            o.stage = s;
+            o.axis = s == 0 ? -1 : j.axis;
+            o.box_fx = j.box_fx; o.box_fy = j.box_fy;
+            o.taps = s == 0 ? 0 : j.taps;
+            o.perp_offset = j.perp_offset;
+            dev::Tex src = j.src;   // the f16 intermediate's geometry is in the job
+            o.source = SMR_STAGE_SRC_F16;
+            if (r.src_tex >= 0) {
+                src = plan_.tex[r.src_tex].tex;
+                o.source = SMR_STAGE_SRC_RAW;
+                for (const auto &cv : plan_.convert_jobs)
+                    if (plan_.tex[r.src_tex].frame_off == cv.second) {
+                        o.source = SMR_STAGE_SRC_CONVERTED;
+                        src.kind = plan_.tex[cv.first].tex.kind;
+                    }
+            }
+            o.src_kind = src.kind;
+            o.src_width = (uint32_t)src.width; o.src_height = (uint32_t)src.height;
+            o.dst_width = (uint32_t)j.dst_w; o.dst_height = (uint32_t)j.dst_h;
+            o.dst_f16 = j.dst_f16;
+        }
+    return SMR_OK;
+}
+
 // inspection: the layers of the last planned tick's composite jobs, as render_begin packed and launched them
 smr_status Renderer::debug_composite_layers(smr_composite_layer_info *out, uint32_t cap, uint32_t *n) {
     if (!n) return SMR_ERR_INVALID_ARGUMENT;
@@ -2432,12 +2491,23 @@ smr_status smr_debug_partition(const int32_t *dst_w, const int32_t *dst_h, uint3
     for (size_t i = 0; i < bg.size(); i++) begin[i] = bg[i];
     return SMR_OK;
 }
-smr_status smr_debug_weights(float scale, float offset, uint32_t out_coord, float *weights, uint32_t cap, uint32_t *taps, float *inv) {
-    if (!weights || !taps || !inv || out_coord > (1u << 24)) return SMR_ERR_INVALID_ARGUMENT;
+smr_status smr_debug_weights(float scale, float offset, uint32_t n_out, float *weights, size_t cap, uint32_t *taps, float *inv,
+                             int32_t *first) {
+    if (!weights || !taps || !inv || !first || n_out == 0 || n_out > 16384 || !(scale > 0.0f && scale <= 1024.0f))
+        return SMR_ERR_INVALID_ARGUMENT;
     int n = 0;
-    const int rc = smr::dev::debug_weights(scale, offset, (int)out_coord, weights, (int)cap, &n, inv);
+    const int rc = smr::dev::debug_weights(scale, offset, (int)n_out, weights, cap, &n, inv, first);
     *taps = (uint32_t)n;
     return rc > 0 ? SMR_OK : rc == 0 ? SMR_ERR_BUFFER_TOO_SMALL : SMR_ERR_CUDA;
+}
+smr_status smr_debug_sincos(const float *x, uint32_t n, float *s, float *c) {
+    if ((n && (!x || !s || !c)) || n > (1u << 28)) return SMR_ERR_INVALID_ARGUMENT;
+    if (n == 0) return SMR_OK;
+    return smr::dev::debug_sincos(x, (int)n, s, c) > 0 ? SMR_OK : SMR_ERR_CUDA;
+}
+smr_status smr_debug_resample_stages(smr_renderer *r, smr_resample_stage_info *out, uint32_t cap, uint32_t *n,
+                                     int32_t *convert_kinds, uint32_t convert_cap, uint32_t *n_convert) {
+    SMR_GUARD(r->impl.debug_resample_stages(out, cap, n, convert_kinds, convert_cap, n_convert))
 }
 smr_status smr_preprocess_frame(smr_renderer *r, const smr_input_frame *f, uint32_t ow, uint32_t oh, void *rgba, uint32_t pitch,
                                 int32_t mem_kind) { SMR_GUARD(r->impl.preprocess_frame(f, ow, oh, rgba, pitch, mem_kind)) }

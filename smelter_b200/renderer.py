@@ -642,6 +642,29 @@ class Renderer:
             out.append(d)
         return out
 
+    def debug_resample_stages(self):
+        """The generic resample passes and k_convert jobs of the last planned tick (smr_debug_resample_stages):
+        (stages, convert_kinds).  stages: one dict per pass -- box passes, first passes, last passes, each in plan order --
+        with stage ("box" / "first" / "last"), axis (-1 for a box pass), box_fx, box_fy, taps, perp_offset, source ("raw" /
+        "converted" / "f16"), src_kind, src (w, h), dst (w, h), dst_f16.  convert_kinds: the texture kind each k_convert
+        job reads."""
+        n, nc = C.c_uint32(), C.c_uint32()
+        self._check(self._lib.smr_debug_resample_stages(self._h, None, 0, C.byref(n), None, 0, C.byref(nc)))
+        arr = (F.ResampleStageInfo * max(1, n.value))()
+        kinds = (C.c_int32 * max(1, nc.value))()
+        self._check(self._lib.smr_debug_resample_stages(self._h, arr, n.value, C.byref(n), kinds, nc.value, C.byref(nc)))
+        stage_names = {F.STAGE_BOX: "box", F.STAGE_FIRST: "first", F.STAGE_LAST: "last"}
+        source_names = {F.STAGE_SRC_RAW: "raw", F.STAGE_SRC_CONVERTED: "converted", F.STAGE_SRC_F16: "f16"}
+        out = []
+        for j in arr[:n.value]:
+            d = {k: getattr(j, k) for k, _ in F.ResampleStageInfo._fields_}
+            d["stage"] = stage_names[j.stage]
+            d["source"] = source_names[j.source]
+            d["src"] = (d.pop("src_width"), d.pop("src_height"))
+            d["dst"] = (d.pop("dst_width"), d.pop("dst_height"))
+            out.append(d)
+        return out, list(kinds[:nc.value])
+
     def debug_composite_layers(self):
         """The layers of the last planned tick's composite jobs (smr_debug_composite_layers), one dict per layer in job
         order, then painter's order: job, kernel ("p" / "multi"), layer, type, rotated, fast, box (12 ints: pixel box and

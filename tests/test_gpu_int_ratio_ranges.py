@@ -1,6 +1,7 @@
 """The integer-ratio TMA kernel (k_resample_tma3) with its compiled-in weights and its per-launch luma table.
 
-- The weights of int_weights.h are what the weight kernel computes on the device for the same mapping, bit for bit.
+- The weights of int_weights.h are what the weight kernel computes on the device for the same mapping, bit for bit, at
+  every output column.
 - One tick with full-range and limited-range sources at 2:1 and 4:1 is byte-identical to the oracle.  The luma table
   is built for one range per launch, so planar sources of both ranges take one launch each and NV12 (limited) a third."""
 import ctypes as C
@@ -19,22 +20,28 @@ pytestmark = pytest.mark.gpu
 NV12 = s.OutputFrameFormat.Nv12WgpuTexture
 
 
-def device_weights(scale, offset, out_coord):
+def device_weights(scale, offset, n_out):
+    """the weight kernel's table of one mapping: (first (n_out,), weights (n_out, taps), 1 / weight_sum (n_out,))"""
     L = _ffi.lib()
-    w = (C.c_float * 64)()
-    taps, inv = C.c_uint32(), C.c_float()
-    st = L.smr_debug_weights(scale, offset, out_coord, w, 64, C.byref(taps), C.byref(inv))
-    assert st == 0, st
-    return np.array(w[:taps.value], np.float32), np.float32(inv.value)
+    taps = int(np.ceil(np.float32(6.0) * np.float32(max(scale, 1.0)))) + 1
+    w = np.zeros((n_out, taps), np.float32)
+    inv = np.zeros(n_out, np.float32)
+    first = np.zeros(n_out, np.int32)
+    nt = C.c_uint32()
+    st = L.smr_debug_weights(scale, offset, n_out, w.ctypes.data, w.size, C.byref(nt), inv.ctypes.data, first.ctypes.data)
+    assert st == 0 and nt.value == taps, (st, nt.value, taps)
+    return first, w, inv
 
 
 @pytest.mark.parametrize("S", [2, 3, 4])
-def test_header_weights_are_the_device_weights(S):
+def test_header_weights_are_the_device_table(S):
+    """every row of the weight kernel's S:1 table of a 3840-wide output is the header's row, bit for bit, and its first tap
+    moves by S per output column"""
     w, inv = header_tables()[S]
-    for o in (0, 5, 1919):
-        dw, dinv = device_weights(float(S), 0.0, o)
-        assert np.array_equal(dw.view(np.uint32), w.view(np.uint32)), (S, o)
-        assert dinv.view(np.uint32) == inv.view(np.uint32), (S, o)
+    first, dw, dinv = device_weights(float(S), 0.0, 3840)
+    assert np.array_equal(dw.view(np.uint32), np.broadcast_to(w.view(np.uint32), dw.shape)), S
+    assert np.array_equal(dinv.view(np.uint32), np.full(3840, inv.view(np.uint32))), S
+    assert np.array_equal(first, first[0] + S * np.arange(3840)), S
 
 
 def full_range_frame(planes, w, h):

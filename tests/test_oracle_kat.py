@@ -175,13 +175,25 @@ def test_chroma_upsample_phase_is_quarter():
     assert b[6] == b[7] and b[5] == b[8] and b[4] == b[9] and b[6] > b[5] > b[4]
 
 
+def max_frame_dim():
+    """the largest input frame side the renderer accepts: kMaxFrameDim, the bound frame_size_ok checks"""
+    import os
+    import re
+    src = open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "smelter_b200", "csrc",
+                            "renderer.cpp")).read()
+    dim = int(re.search(r"constexpr uint32_t kMaxFrameDim = (\d+);", src).group(1))
+    body = re.search(r"static bool frame_size_ok\(const smr_input_frame &f\) \{([^}]*)\}", src).group(1)
+    assert body.count("kMaxFrameDim") == 2 and not re.search(r"\d{3,}", body), body
+    return dim
+
+
 def test_even_size_sampler_phases_exhaustive():
     """The CUDA fast paths hard-code the NC-6 taps for even plane sizes; prove the generic formula the
-    oracle evaluates gives exactly those taps for EVERY even size up to 8192 and every coordinate."""
+    oracle evaluates gives exactly those taps for EVERY even size the renderer accepts and every coordinate."""
     import ctypes as C
     L = orc.lib()
     L.orc_check_even_size_phases.restype = C.c_long
-    assert L.orc_check_even_size_phases(8192) == 0
+    assert L.orc_check_even_size_phases(max_frame_dim()) == 0
 
 
 def test_wide_chroma_restatements_are_consistent():
