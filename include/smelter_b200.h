@@ -326,7 +326,7 @@ smr_status smr_debug_tile_plan(const int32_t *boxes, uint32_t n_layers, uint32_t
  * fit in cap (SMR_ERR_BUFFER_TOO_SMALL otherwise; out = NULL asks for the count). */
 typedef enum {
     SMR_FUSED_LDG = 0,             /* k_resample_fused_int<ratio, src_class> */
-    SMR_FUSED_TMA_INT = 1,         /* k_resample_tma3<ratio, src_class> */
+    SMR_FUSED_TMA_INT = 1,         /* k_resample_tma3<ratio, src_class, full_range> */
     SMR_FUSED_TMA_ANY = 2          /* k_resample_tma0<src_class, window, box> */
 } smr_fused_kernel;
 typedef struct {

@@ -994,21 +994,26 @@ static bool launch_tma0_src(int src, int box, const FusedJob *jobs_dev, const Fu
                     : launch_tma0<0, WINP, 0>(jobs_dev, pieces, piece_begin, nblocks, s);
 }
 
-template <int S, int SRC>
-static bool launch_tma3(const FusedJob *jobs_dev, const FusedPiece *pieces, const int *piece_begin, int nblocks, int full_range,
-                        cudaStream_t s) {
+template <int S, int SRC, bool FULL>
+static bool launch_tma3_range(const FusedJob *jobs_dev, const FusedPiece *pieces, const int *piece_begin, int nblocks, cudaStream_t s) {
     static std::atomic<unsigned long long> done{0};
     int dev = 0;
     cudaGetDevice(&dev);
     const unsigned long long bit = 1ull << (dev & 63);
     if (!(done.load(std::memory_order_acquire) & bit)) {
-        cudaFuncSetAttribute(tma_int::k_resample_tma3<S, SRC>, cudaFuncAttributeMaxDynamicSharedMemorySize, tma_int::Cfg<S>::SMEM);
+        cudaFuncSetAttribute(tma_int::k_resample_tma3<S, SRC, FULL>, cudaFuncAttributeMaxDynamicSharedMemorySize, tma_int::Cfg<S>::SMEM);
         done.fetch_or(bit, std::memory_order_release);
     }
     const int grid = (nblocks + tma_int::kGroups - 1) / tma_int::kGroups;   // the host cut the work for `nblocks` eight-warp groups
-    tma_int::k_resample_tma3<S, SRC><<<grid, dim3(32, tma::kWarps * tma_int::kGroups), tma_int::Cfg<S>::SMEM, s>>>(jobs_dev, pieces, piece_begin, nblocks,
-                                                                                                            full_range);
+    tma_int::k_resample_tma3<S, SRC, FULL><<<grid, dim3(32, tma::kWarps * tma_int::kGroups), tma_int::Cfg<S>::SMEM, s>>>(jobs_dev, pieces, piece_begin,
+                                                                                                                  nblocks);
     return check_launch("k_resample_tma3");
+}
+template <int S, int SRC>
+static bool launch_tma3(const FusedJob *jobs_dev, const FusedPiece *pieces, const int *piece_begin, int nblocks, int full_range,
+                        cudaStream_t s) {
+    return full_range ? launch_tma3_range<S, SRC, true>(jobs_dev, pieces, piece_begin, nblocks, s)
+                      : launch_tma3_range<S, SRC, false>(jobs_dev, pieces, piece_begin, nblocks, s);
 }
 
 // src: 0 planar 4:2:0, 1 NV12, 2 UYVY, 3 YUYV (fused_source_class)

@@ -43,6 +43,7 @@ constexpr uint32_t kMagicBits = 0x4B400000u;
 constexpr int kThrOff = 256 * kDecRep * 4;
 constexpr int kBarOff = kThrOff + 256 * 4;
 constexpr int kKaddrOff = kBarOff + 64;
+constexpr int kYbaseOff = kKaddrOff + 4;
 constexpr int kStashOff = kBarOff + 128;
 constexpr int kStashBytes = 1024;
 constexpr int kTailBytes = kStashOff + kStashBytes;
@@ -238,28 +239,25 @@ struct LaneWords {
     }
 };
 
-// Source row r of the stage sb whose tile starts at source row sr0 (chei chroma rows in the image): yw = the lane's 8 luma
-// bytes, v[k] = 3 * heavy + light chroma texel cx - 1 + k (u in bits 0..15, v in bits 16..31)
+// yw = the lane's 8 luma bytes of a source row, la: the shared address of the lane's words of it (stage + row + lw.l_off)
 template <bool NV12>
-__device__ __forceinline__ void fetch_row(uint32_t sb, const LaneWords<NV12> &lw, int r, int sr0, int chei, uint32_t (&yw)[2],
-                                          uint32_t (&v)[6]) {
+__device__ __forceinline__ void fetch_luma(uint32_t la, const LaneWords<NV12> &lw, uint32_t (&yw)[2]) {
     // raw bytes of this lane's 8 pixels: 12 bytes from a 4-byte aligned address; the half that is 8-byte aligned
     // (warp-uniform) goes as one LDS.64 (lanes 8 bytes apart: conflict-free, an LDS.32 is 2-way)
-    {
-        const uint32_t la = sb + (uint32_t)((r - sr0) * kLumaBox) + lw.l_off;
-        uint32_t w0, w1, w2;
-        if (lw.l_off & 4u) { w0 = lds32v(la); lds64v(la + 4, w1, w2); }
-        else { lds64v(la, w0, w1); w2 = lds32v(la + 8); }
-        yw[0] = __funnelshift_r(w0, w1, lw.l_sh);
-        yw[1] = __funnelshift_r(w1, w2, lw.l_sh);
-    }
-    const int cyb = (sr0 >> 1) - 1;                                     // chroma row of the tile's first row
-    const int ch = r >> 1;                                              // weight 3/4
-    const int cl = (r & 1) ? min(ch + 1, chei - 1) : max(ch - 1, 0);    // weight 1/4
+    uint32_t w0, w1, w2;
+    if (lw.l_off & 4u) { w0 = lds32v(la); lds64v(la + 4, w1, w2); }
+    else { lds64v(la, w0, w1); w2 = lds32v(la + 8); }
+    yw[0] = __funnelshift_r(w0, w1, lw.l_sh);
+    yw[1] = __funnelshift_r(w1, w2, lw.l_sh);
+}
+
+// v[k] = 3 * heavy + light chroma texel cx - 1 + k (u in bits 0..15, v in bits 16..31) of a source row; bh, bl: the shared
+// addresses of the lane's words (chroma tile + row + lw.c_off) of the chroma row that weighs 3/4 and of the one that weighs
+// 1/4; planar: in the u plane, the v plane lies kChromaBytesPlanar behind
+template <bool NV12>
+__device__ __forceinline__ void fetch_chroma(uint32_t bh, uint32_t bl, const LaneWords<NV12> &lw, uint32_t (&v)[6]) {
     const uint32_t c_off = lw.c_off, c_sh = lw.c_sh;
     if (NV12) {
-        const uint32_t bh = sb + kLumaBytes + (uint32_t)((ch - cyb) * kNv12Box) + c_off;
-        const uint32_t bl = sb + kLumaBytes + (uint32_t)((cl - cyb) * kNv12Box) + c_off;
         uint32_t h0, h1, h2, h3, l0, l1, l2, l3;
         if (c_off & 4u) {
             h0 = lds32v(bh); lds64v(bh + 4, h1, h2); h3 = lds32v(bh + 12);
@@ -278,8 +276,7 @@ __device__ __forceinline__ void fetch_row(uint32_t sb, const LaneWords<NV12> &lw
         v[4] = 3u * __byte_perm(ph2, 0, 0x4140) + __byte_perm(pl2, 0, 0x4140);
         v[5] = 3u * __byte_perm(ph2, 0, 0x4342) + __byte_perm(pl2, 0, 0x4342);
     } else {
-        const uint32_t uh = sb + kLumaBytes + (uint32_t)((ch - cyb) * kPlanarBox) + c_off;
-        const uint32_t ul = sb + kLumaBytes + (uint32_t)((cl - cyb) * kPlanarBox) + c_off;
+        const uint32_t uh = bh, ul = bl;
         const uint32_t vh = uh + kChromaBytesPlanar, vl = ul + kChromaBytesPlanar;
         // 8 bytes from the lane's first texel (cx - 1): texels cx-1 .. cx+4 are bytes 0 .. 5
         auto eight = [&](uint32_t a, uint32_t &q0, uint32_t &q1) {
@@ -297,6 +294,20 @@ __device__ __forceinline__ void fetch_row(uint32_t sb, const LaneWords<NV12> &lw
     }
 }
 
+// Source row r of the stage sb whose tile starts at source row sr0 (chei chroma rows in the image): fetch_luma and
+// fetch_chroma at the row's addresses
+template <bool NV12>
+__device__ __forceinline__ void fetch_row(uint32_t sb, const LaneWords<NV12> &lw, int r, int sr0, int chei, uint32_t (&yw)[2],
+                                          uint32_t (&v)[6]) {
+    constexpr int box = NV12 ? kNv12Box : kPlanarBox;
+    fetch_luma<NV12>(sb + (uint32_t)((r - sr0) * kLumaBox) + lw.l_off, lw, yw);
+    const int cyb = (sr0 >> 1) - 1;                                     // chroma row of the tile's first row
+    const int ch = r >> 1;                                              // weight 3/4
+    const int cl = (r & 1) ? min(ch + 1, chei - 1) : max(ch - 1, 0);    // weight 1/4
+    fetch_chroma<NV12>(sb + kLumaBytes + (uint32_t)((ch - cyb) * box) + lw.c_off,
+                       sb + kLumaBytes + (uint32_t)((cl - cyb) * box) + lw.c_off, lw, v);
+}
+
 // exact n / 255 of a byte n held as a float: fma(n, c, n * lo)
 constexpr uint32_t kDiv255C = 0x3b808081u, kDiv255Lo = 0xaf7efeffu;
 
@@ -309,14 +320,18 @@ __device__ __forceinline__ float luma_of(float ny, float nk16, float rcp_y) {
 
 // The luma table behind the tail (kLumaTabBytes, filled by the block before its first __syncthreads) and this lane's
 // lookup base: the entry of byte n is [(float bits of (n + 2^23)) << 6 + base]  (mod 2^32), so that the PRMT which puts
-// the byte under the exponent of 2^23 plus one LEA make the address.
+// the byte under the exponent of 2^23 plus one LEA make the address.  Like the decode table's base (setup_block) the base
+// takes a round trip through shared memory: known to the compiler it is a constant too wide for the load's address
+// field, and every lookup pays an extra add for its upper half.
 __device__ __forceinline__ void fill_luma_table(unsigned char *tail, float nk16, float rcp_y) {
     float *s_y = reinterpret_cast<float *>(tail + kTailBytes);
     const int btid = threadIdx.y * 32 + threadIdx.x, bn = blockDim.x * blockDim.y;
     for (int i = btid; i < 256 * kLumaRep; i += bn) s_y[i] = luma_of((float)(i / kLumaRep), nk16, rcp_y);
+    if (btid == 0) *reinterpret_cast<volatile uint32_t *>(tail + kYbaseOff) = smem_u32(s_y) - (0x4B000000u << 6);
 }
+// after the __syncthreads that follows fill_luma_table
 __device__ __forceinline__ uint32_t luma_base(unsigned char *tail) {
-    return smem_u32(tail + kTailBytes) - (0x4B000000u << 6) + 4u * (threadIdx.x % kLumaRep);
+    return *reinterpret_cast<volatile uint32_t *>(tail + kYbaseOff) + 4u * (threadIdx.x % kLumaRep);
 }
 
 // K1/K2 -> u8 of pixels 2p and 2p + 1 of an 8-pixel run (yw: its luma bytes, v: its combined chroma as fetch_row makes it),

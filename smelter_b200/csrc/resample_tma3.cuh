@@ -15,7 +15,8 @@
 //     consecutive output rows share TAPS - S of their ring rows, every row is loaded once for both.
 //
 // Template parameter S in {2, 4}: integer horizontal ratio with zero crop offset (first(o) = S * o + const).
-// SRC: 0 planar 4:2:0, 1 NV12.
+// SRC: 0 planar 4:2:0, 1 NV12.  FULL: the range of every source of the launch (the host keys the launches by it), so the
+// range constants of K1/K2 are immediates of the row loop and take no registers there.
 #pragma once
 
 namespace tma_int {
@@ -23,11 +24,36 @@ using namespace tma;
 
 constexpr int kGroups = 3;                            // independent 8-warp groups per block (one block per SM)
 
+// x as a value the compiler knows nothing about: it stays in ONE register across the row loop -- at the kernel's register
+// limit the compiler otherwise recomputes a loop-invariant value inside the loop, or folds a constant out of it and adds
+// that constant back at every use
+__device__ __forceinline__ uint32_t held(uint32_t x) {
+    asm("" : "+r"(x));
+    return x;
+}
+
 template <int S>
 struct Cfg {
     static constexpr int P = 8;                      // source pixels per lane and row
     static constexpr int OUT = P / S;                // output columns started per lane
     static constexpr int TAPS = 6 * S + 1;
+    // Taps in front of the trailing run of weights that are exactly zero: at an integer ratio with zero offset the Lanczos
+    // window covers 6 S pixels, and the last weight of int_weights.h is +0.  No fma is issued for it, in either pass,
+    // because there it is an identity:
+    //   * every multiplicand is finite (decoded sRGB values in [0, 1]; ring values are f16-rounded finite floats), so
+    //     the skipped product is +0 or -0;
+    //   * the accumulator is never -0: it starts at +0, and under round-to-nearest fma(x, w, acc) is -0 only if x * w is
+    //     -0 and acc is -0, or by underflow -- and x * w is a multiple of 2^-68 (pixels are multiples of 2^-35, ring
+    //     values of 2^-24, weights of 2^-33), so x * w + acc is a multiple of the smallest float and rounds to zero only
+    //     when it is zero, which gives +0;
+    //   * acc + (+-0) == acc bit for bit for every acc other than -0.
+    static __host__ __device__ constexpr int taps_nz() {
+        int n = TAPS;
+        while (n > 0 && int_weight<S>(n - 1) == 0.0f) n--;
+        return n;
+    }
+    static constexpr int TAPS_NZ = taps_nz();
+    static_assert(TAPS_NZ == 6 * S, "the integer-ratio weight rows end in exactly one zero");
     static constexpr int A = kLead<S>;               // X0 = first(O0) - A is even
     static constexpr int NST = (A + S * (OUT - 1) + TAPS + P - 1) / P;   // lanes an accumulator visits
     static __host__ __device__ constexpr int last_stage(int j) { return (A + S * j + TAPS - 1) / P; }
@@ -48,9 +74,9 @@ struct Cfg {
     static constexpr int SMEM = kGroups * GROUP_BYTES + kTailBytes + kLumaTabBytes;
 };
 
-template <int S, int SRC>
+template <int S, int SRC, bool FULL>
 __global__ void __launch_bounds__(32 * kWarps * kGroups, 1) k_resample_tma3(const FusedJob *jobs, const FusedPiece *pieces, const int *piece_begin,
-                                                                            int n_virtual_blocks, int full_range) {
+                                                                            int n_virtual_blocks) {
     using K = Cfg<S>;
     using It = ChunkIter<S, 1>;
     constexpr int P = K::P, OUT = K::OUT, TAPS = K::TAPS, A = K::A, NST = K::NST;
@@ -63,25 +89,24 @@ __global__ void __launch_bounds__(32 * kWarps * kGroups, 1) k_resample_tma3(cons
     const uint32_t stage0 = smem_u32(smem);
     float *ring = reinterpret_cast<float *>(smem + kStageBytes);
     const uint32_t bar0 = smem_u32(tail + kBarOff) + 16u * (uint32_t)grp;
-    // every source of the launch has the range full_range (the host keys the launches by it): the luma table is the block's
-    const float nk16 = full_range ? 0.0f : -K16, rcp_y = full_range ? 1.0f : RCP_Y, rcp_c = full_range ? 1.0f : RCP_C;
+    // every source of the launch has the range FULL: the luma table is the block's
+    constexpr float nk16 = FULL ? 0.0f : -K16, rcp_y = FULL ? 1.0f : RCP_Y, rcp_c = FULL ? 1.0f : RCP_C;
     const uint32_t kaddr = setup_block<kGroups>(tail, [&] { fill_luma_table(tail, nk16, rcp_y); });
     const uint32_t ybase = luma_base(tail);
     const int vb = blockIdx.x * kGroups + grp;         // the host cut the launch for SMs x 3 eight-warp blocks
     if (vb >= n_virtual_blocks) return;
 
     Stash<It> *stash = stash_slots<It, kGroups>(tail, grp);
-    uint32_t step = 0;
+    uint32_t phase = 0;         // bit 0: parity of the chunks that carried a TMA load so far (mbarrier parity); bit 1: of the steps
     It it;
     it.init(jobs, pieces, __ldg(piece_begin + vb), __ldg(piece_begin + vb + 1));
 
     Chunk cur = it.next();
     if (!cur.valid) return;
     if (tid == 0) issue<NV12, 1>(jobs, cur, stage0, bar0);
-    uint32_t nchunk = 0;        // chunks that carried a TMA load so far (mbarrier parity)
 
     while (cur.valid) {
-        Stash<It> *const parked = stash + (step & 1u);
+        Stash<It> *const parked = stash + (phase >> 1);
         {
             const Chunk nxt = it.next();
             if (tid == 0) { parked->it = it; parked->nxt = nxt; }
@@ -91,13 +116,29 @@ __global__ void __launch_bounds__(32 * kWarps * kGroups, 1) k_resample_tma3(cons
         const int W = J.src.width, H = J.src.height, chei = H >> 1;
         const uint32_t sb = stage0;
         if (cur_tma) {
-            mbar_wait(bar0, nchunk & 1u);
+            mbar_wait(bar0, phase & 1u);
             replicate_edges<NV12>(smem, cur.x0, cur.nrows, W, tid, grp);
-            const LaneWords<NV12> lw(cur.x0, lane);
+            LaneWords<NV12> lw(cur.x0, lane);
+            lw.c_off = held(lw.c_off);
             // ---- phase A: one source row per warp step ------------------------------------------------------------
-            for (int r = cur.r0 + warp; r < cur.r0 + cur.nrows; r += kWarps) {
+            // A warp's rows r are kWarps apart, so what the loop needs of a row is carried, not recomputed: the row's stage
+            // addresses (fetch_row) advance by a constant -- the parity of r, hence which neighbour is the light chroma
+            // row, stays -- and so does its ring slot, which wraps by a subtraction.  The row's luma address la counts the
+            // rows.  The light chroma row's clamp to the image can bite in one row only, the image's first (even r) or
+            // last (odd r), and makes it the heavy row there; la_clamp is that row's la (no row's, if it is not one of
+            // this warp's rows of the chunk: the rows' la are whole steps of kWarps * kLumaBox from the first).
+            constexpr int CBOX = NV12 ? kNv12Box : kPlanarBox;
+            const int r_first = cur.r0 + warp;
+            uint32_t la = sb + (uint32_t)(warp * kLumaBox) + lw.l_off;
+            const uint32_t la_end = sb + (uint32_t)(cur.nrows * kLumaBox) + lw.l_off;
+            const uint32_t la_clamp = la + (uint32_t)((((r_first & 1) ? 2 * chei - 1 : 0) - r_first) * kLumaBox);
+            uint32_t bh = sb + kLumaBytes + (uint32_t)(((r_first >> 1) - (cur.r0 >> 1) + 1) * CBOX) + lw.c_off;
+            const uint32_t dlight = held((r_first & 1) ? (uint32_t)CBOX : (uint32_t)-CBOX);
+            uint32_t slot_off = (uint32_t)(r_first % K::RROWS) * K::RROW_BYTES;
+            for (; la < la_end; la += kWarps * kLumaBox, bh += (kWarps / 2) * CBOX) {
                 uint32_t yw[2], v[6];
-                fetch_row<NV12>(sb, lw, r, cur.r0, chei, yw, v);
+                fetch_luma<NV12>(la, lw, yw);
+                fetch_chroma<NV12>(bh, la == la_clamp ? bh : bh + dlight, lw, v);
                 // A1: K1/K2 -> u8 -> sRGB decode, two pixels per instruction, luma from the luma table
                 float2 prg[P];   // (r, g) of pixel i
                 float pb[P];     // b of pixel i
@@ -115,7 +156,7 @@ __global__ void __launch_bounds__(32 * kWarps * kGroups, 1) k_resample_tma3(cons
 #pragma unroll
                         for (int j = 0; j < OUT; j++) {
                             const int t = P * s + i - A - S * j;   // compile-time after unrolling
-                            if (t >= 0 && t < TAPS) {
+                            if (t >= 0 && t < K::TAPS_NZ) {
                                 arg[j] = fma2(prg[i], splat(int_weight<S>(t)), arg[j]);
                                 ab[j] = __fmaf_rn(pb[i], int_weight<S>(t), ab[j]);
                             }
@@ -134,7 +175,9 @@ __global__ void __launch_bounds__(32 * kWarps * kGroups, 1) k_resample_tma3(cons
                 // normalise, quantise to f16 (NC-5) and park the row in the ring: [row][lane][channel][j]
                 {
                     constexpr float inv = int_inv<S>();
-                    float *dst = ring + (size_t)(r % K::RROWS) * (K::RROW_BYTES / 4) + lane * 3 * OUT;
+                    float *dst = reinterpret_cast<float *>(reinterpret_cast<unsigned char *>(ring) + slot_off) + lane * 3 * OUT;
+                    slot_off += kWarps * K::RROW_BYTES;
+                    slot_off = min(slot_off, slot_off - (uint32_t)K::RING_BYTES);   // unsigned: the difference is huge unless it wrapped
 #pragma unroll
                     for (int j = 0; j < OUT; j += 2) {
                         const float2 fr = __half22float2(__floats2half2_rn(arg[j].x * inv, arg[j + 1].x * inv));
@@ -146,7 +189,7 @@ __global__ void __launch_bounds__(32 * kWarps * kGroups, 1) k_resample_tma3(cons
                     }
                 }
             }
-            nchunk++;
+            phase ^= 1u;
         }
         // every warp has read its rows of the stage (and, for a last chunk, stored them in the ring): the next chunk's
         // loads refill the stage while the vertical pass runs
@@ -198,9 +241,10 @@ __global__ void __launch_bounds__(32 * kWarps * kGroups, 1) k_resample_tma3(cons
                 encode_store<OUT>(J, acc, oy, s_thr, cur.ox0, K::NOUT, col_of, px);
             };
             if (J.v_same) {
-                // same integer ratio vertically: rows o and o + 1 share TAPS - S of their TAPS ring rows.  Four warps (one
-                // per scheduler) take two output rows each: every ring row is loaded once for both, the weights are the
-                // compile-time row of int_weights.h, the loop unrolls; the ring wraps at most once inside the window.
+                // same integer ratio vertically: rows o and o + 1 share TAPS_NZ - S of their TAPS_NZ ring rows (the zero tap
+                // is skipped: Cfg::TAPS_NZ).  Four warps (one per scheduler) take two output rows each: every ring row is
+                // loaded once for both, the weights are the compile-time row of int_weights.h, the loop unrolls; the ring
+                // wraps at most once inside the window.
                 if (warp < kWarps / 2) {
                     const int oa = cur.o0 + 2 * warp, ob = oa + 1;
                     const int fa = __ldg(J.first_v) + S * oa;               // first_v(oa); first_v(ob) = fa + S
@@ -213,14 +257,14 @@ __global__ void __launch_bounds__(32 * kWarps * kGroups, 1) k_resample_tma3(cons
                         const int slot0 = fa % K::RROWS, nwrap = K::RROWS - slot0;
                         const float *p0 = lbase + slot0 * ROWF;
 #pragma unroll
-                        for (int u = 0; u < TAPS + S; u++) {
+                        for (int u = 0; u < K::TAPS_NZ + S; u++) {
                             const float *p = p0 + (u >= nwrap ? (u - K::RROWS) * ROWF : u * ROWF);
                             float2 v[3 * OUT / 2];
 #pragma unroll
                             for (int k = 0; k < 3 * OUT / 2; k++) v[k] = *reinterpret_cast<const float2 *>(p + 2 * k);
-                            if (u < TAPS) {
+                            if (u < K::TAPS_NZ) {
 #pragma unroll
-                                for (int k = 0; k < 3 * OUT / 2; k++) aa[k] = fma2(v[k], splat(int_weight<S>(u < TAPS ? u : 0)), aa[k]);
+                                for (int k = 0; k < 3 * OUT / 2; k++) aa[k] = fma2(v[k], splat(int_weight<S>(u < K::TAPS_NZ ? u : 0)), aa[k]);
                             }
                             if (u >= S) {
 #pragma unroll
@@ -244,7 +288,7 @@ __global__ void __launch_bounds__(32 * kWarps * kGroups, 1) k_resample_tma3(cons
             }
             group_sync(grp);   // the ring rows this pass read may be overwritten by the next step's horizontal pass
         }
-        cur = parked->nxt; it = parked->it; step++;   // written before this step's group_sync
+        cur = parked->nxt; it = parked->it; phase ^= 2u;   // written before this step's group_sync
     }
 }
 

@@ -1,9 +1,12 @@
 """Instruction budget of the integer-ratio TMA resample kernel, read from the compiler's output (no GPU needed).
 
 Compiles smelter_b200/csrc/kernels.cu alone with the library's nvcc flags into a temporary cubin and prints, for every
-k_resample_tma3<S, SRC>: registers, spill stores / loads (ptxas -v), the kernel's SASS instruction count, and the
+k_resample_tma3<S, SRC, FULL>: registers, spill stores / loads (ptxas -v), the kernel's SASS instruction count, and the
 instruction count of the phase-A row loop (one warp, one source row: fetch, K1/K2, decode, horizontal pass, ring
 store) by opcode.  The row loop is the backward-branch loop of the kernel that holds the SHFL.UP of the horizontal pass.
+Then the same-ratio vertical pass of one step (one warp, two output rows): it is unrolled, so it is the branch-free run
+of instructions outside the row loop with the most wide ring loads (LDS.64 / LDS.128); its FFMA and loads are printed, and
+the ring rows they cover (3 * 8 / S floats per lane and ring row).
 
     python tools/tma3_sass_budget.py                  # the tree's kernels.cu
     python tools/tma3_sass_budget.py --csrc DIR       # another copy of smelter_b200/csrc, e.g. a parent commit's
@@ -107,9 +110,34 @@ def row_loop(ins):
     return best or []
 
 
+def vertical_pass(ins, loop):
+    """the branch-free run outside the row loop with the most LDS.64 / LDS.128 (the unrolled same-ratio vertical pass)"""
+    inside = {x[0] for x in loop}
+    targets = set()
+    for _, op, args in ins:
+        if op.startswith(("BRA", "BSSY")):
+            m = re.search(r"0x([0-9a-f]+)\s*$", args)
+            if m:
+                targets.add(int(m.group(1), 16))
+    blocks, cur = [], []
+    for x in ins:
+        if x[0] in targets and cur:
+            blocks.append(cur)
+            cur = []
+        cur.append(x)
+        if x[1].startswith(("BRA", "EXIT", "RET", "BRX")):
+            blocks.append(cur)
+            cur = []
+    blocks.append(cur)
+
+    def wide(b):
+        return sum(1 for x in b if x[1].startswith(("LDS.64", "LDS.128")))
+    return max((b for b in blocks if b and b[0][0] not in inside), key=wide, default=[])
+
+
 def demangle_tma3(name):
-    m = re.search(r"k_resample_tma3ILi(\d)ELi(\d)E", name)
-    return (int(m.group(1)), int(m.group(2))) if m else None
+    m = re.search(r"k_resample_tma3ILi(\d)ELi(\d)ELb(\d)E", name)
+    return (int(m.group(1)), int(m.group(2)), int(m.group(3))) if m else None
 
 
 def short_names(names, cuobjdump_dir):
@@ -134,10 +162,10 @@ def main():
     regs = parse_ptxas(ptxas)
     funcs = parse_sass(sass)
     tma3 = sorted((demangle_tma3(n), n) for n in funcs if demangle_tma3(n))
-    for (S, SRC), name in tma3:
+    for (S, SRC, FULL), name in tma3:
         r, st, ld = regs.get(name, (0, 0, 0))
         loop = row_loop(funcs[name])
-        print(f"k_resample_tma3<{S},{SRC}>: {r} registers, spill {st}/{ld} B, {len(funcs[name])} SASS; "
+        print(f"k_resample_tma3<{S},{SRC},{FULL}>: {r} registers, spill {st}/{ld} B, {len(funcs[name])} SASS; "
               f"phase-A row loop {len(loop)} instructions")
         ops = collections.Counter(op for _, op, _ in loop)
         const = sum(n for op, n in ops.items() if op.startswith(("ULDC", "LDC")))
@@ -148,6 +176,12 @@ def main():
             line.append(f"{op} {n}")
         for i in range(0, len(line), 8):
             print("  " + ", ".join(line[i:i + 8]))
+        vp = collections.Counter(op.split(".reuse")[0] for _, op, _ in vertical_pass(funcs[name], loop))
+        l64 = sum(n for op, n in vp.items() if op.startswith("LDS.64"))
+        l128 = sum(n for op, n in vp.items() if op.startswith("LDS.128"))
+        ffma = sum(n for op, n in vp.items() if op.startswith("FFMA"))
+        print(f"  same-ratio vertical pass, one warp and step: FFMA {ffma}, LDS.64 {l64}, LDS.128 {l128}: "
+              f"{(2 * l64 + 4 * l128) * S // 24} ring rows")
     if a.all:
         print()
         nvcc_dir = os.path.dirname(os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc"))
