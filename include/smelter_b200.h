@@ -62,7 +62,7 @@ typedef enum {
     SMR_COMPONENT_SHADER = 4,
     SMR_COMPONENT_WEB_VIEW = 5,
     SMR_COMPONENT_IMAGE = 6,
-    SMR_COMPONENT_TEXT = 7
+    SMR_COMPONENT_TEXT = 7         /* payload in smr_component.text */
 } smr_component_type;
 
 typedef struct { uint8_t r, g, b, a; } smr_rgba;                                  /* RGBAColor */
@@ -94,6 +94,8 @@ typedef enum { SMR_RESCALE_FIT = 0, SMR_RESCALE_FILL = 1 } smr_rescale_mode;
 typedef enum { SMR_HALIGN_LEFT = 0, SMR_HALIGN_RIGHT = 1, SMR_HALIGN_JUSTIFIED = 2, SMR_HALIGN_CENTER = 3 } smr_horizontal_align;
 typedef enum { SMR_VALIGN_TOP = 0, SMR_VALIGN_CENTER = 1, SMR_VALIGN_BOTTOM = 2, SMR_VALIGN_JUSTIFIED = 3 } smr_vertical_align;
 
+struct smr_text;
+
 /* One node of the Component tree.  Fields that do not apply to `type` are ignored.
  * Use smr_component_default() to get the reference's `Default` values (components.rs:289-347). */
 typedef struct smr_component {
@@ -123,6 +125,8 @@ typedef struct smr_component {
     smr_opt_f32 tiles_width, tiles_height; /* Tiles */
     uint32_t tile_aspect_ratio_w, tile_aspect_ratio_h;
     float tiles_margin, tiles_padding;
+
+    const struct smr_text *text;           /* Text (smr_text below) */
 } smr_component;
 
 /* ------------------------------------ frames (types.rs:21-119) ------------------------------- */
@@ -234,7 +238,9 @@ void smr_destroy(smr_renderer *r);
 smr_status smr_register_input(smr_renderer *r, const char *input_id);
 smr_status smr_unregister_input(smr_renderer *r, const char *input_id);
 
-/* Renderer::update_scene(output_id, resolution, output_format, scene_root)   state.rs:177-188 */
+/* Renderer::update_scene(output_id, resolution, output_format, scene_root)   state.rs:177-188
+ * Components: InputStream, View, Tiles, Rescaler and Text (anywhere, the root included); Shader, WebView and Image answer
+ * SMR_ERR_UNSUPPORTED.  A Text root follows the rules of an InputStream root (an RGBA output has the text's size). */
 smr_status smr_update_scene(smr_renderer *r, const char *output_id, uint32_t width, uint32_t height,
                             int32_t output_format, const smr_component *scene_root);
 /* Renderer::unregister_output                                       state.rs:115-123 */
@@ -278,9 +284,8 @@ smr_status smr_premultiply_rgba8(smr_renderer *r, const smr_input_frame *frame, 
  * after its clipping to TextBounds (quad origin, size, atlas origin, colour, content type), the atlases are its mask
  * (R8) and colour (RGBA8) atlas pages.  Quads are alpha-blended in list order (wgpu::BlendState::ALPHA_BLENDING) through
  * the node texture's view.  color_mode: glyphon ColorMode, 0 = Accurate (TextAtlas::new, :95-100), 1 = Web.  The
- * result (width x height RGBA8, premultiplied by construction) is the text node's texture: hand it to smr_render as a
- * SMR_FRAME_RGBA8 input (device memory: zero copy) -- like the reference, render it once per scene update
- * (`was_rendered`, :73-75), not per frame.  glyphs and atlases are HOST memory; `rgba` per mem_kind.  Blocking. */
+ * result (width x height RGBA8, premultiplied by construction) is the text node's texture.  glyphs and atlases are HOST
+ * memory; `rgba` per mem_kind.  Blocking.  A scene draws text through SMR_COMPONENT_TEXT (smr_text below) instead. */
 typedef enum { SMR_GLYPH_COLOR = 0, SMR_GLYPH_MASK = 1 } smr_glyph_content;      /* glyphon ContentType */
 typedef struct {
     int32_t x, y;                  /* top-left pixel of the quad in the text texture */
@@ -293,6 +298,24 @@ typedef struct { const void *data; uint32_t width, height, pitch; } smr_atlas;  
 smr_status smr_render_text(smr_renderer *r, uint32_t width, uint32_t height, smr_rgba background, const smr_glyph *glyphs,
                            uint32_t n_glyphs, const smr_atlas *mask_atlas, const smr_atlas *color_atlas, int32_t color_mode,
                            void *rgba, uint32_t pitch, int32_t mem_kind);
+
+/* The payload of a Text component (smr_component.text): StatefulTextComponent's laid-out buffer (scene/text_component.rs).
+ * The caller shapes the text (cosmic-text) and prepares its glyphs (glyphon) as for smr_render_text; width x height is the
+ * resolution its layout produced, which is the component's size in the scene (scene.rs:101-127).  smr_update_scene checks
+ * it with smr_render_text's rules (SMR_ERR_INVALID_ARGUMENT: NULL payload, a glyph content other than COLOR / MASK, a
+ * missing atlas, a side above 16384, more than 2^22 glyphs), except that 0 x 0 is legal: like the reference
+ * (text_renderer.rs:77-85) its node texture is one transparent pixel.  Everything is copied before smr_update_scene
+ * returns; an atlas several components pass by the same pointer is uploaded once.  The node texture is drawn by the first
+ * smr_render of the output after each smr_update_scene of it (`was_rendered`, text_renderer.rs:73-75), then composited
+ * like any premultiplied RGBA8 child. */
+typedef struct smr_text {
+    uint32_t width, height;
+    smr_rgba background;
+    const smr_glyph *glyphs;
+    uint32_t n_glyphs;
+    const smr_atlas *mask_atlas, *color_atlas;
+    int32_t color_mode;
+} smr_text;
 
 /* inspection (no device needed): the balanced row partition the fused resample launch uses for jobs of
  * dst_w[i] x dst_h[i] output pixels on `max_blocks` resident blocks.  pieces: 4 ints each {job, strip, row_begin,
@@ -421,7 +444,8 @@ smr_status smr_debug_layouts(smr_renderer *r, const char *output_id, uint64_t pt
  * transitions, NestedLayout::flatten -- all Rust) hands over, per output and whenever they change, the RenderLayout[]
  * that transformations/layout/params.rs:169-333 would pack into uniform blocks: same fields, same units (pixels of
  * the root_width x root_height layout node texture), painter's order.  child_ids[k] is the input id of the node's
- * k-th child (scene/layout.rs:84-93), which `child_index` of a texture layout refers to.  Registers the output like
+ * k-th child (scene/layout.rs:84-93), which `child_index` of a texture layout refers to; children here are inputs only
+ * (a Text child needs smr_update_scene, or its texture from smr_render_text passed as an input).  Registers the output like
  * smr_update_scene does; stays in force until the next smr_set_layouts / smr_update_scene of that output.  The
  * resampler planning (layout.rs:238-278) and everything below it still happen here, per tick. */
 smr_status smr_set_layouts(smr_renderer *r, const char *output_id, uint32_t width, uint32_t height, int32_t format,

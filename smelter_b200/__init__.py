@@ -7,5 +7,5 @@ from .renderer import (  # noqa: F401
     BorderRadius, BoxShadow, Component, Frame, FrameData, FramePreProcessor, FrameSet, HorizontalAlign, InputStreamComponent,
     InterpolationKind, NvPlanes, OutputFrameFormat, Overflow, Padding, Position, Renderer, RendererError,
     RendererOptions, RenderingMode, RenderSceneError, RescaleMode, RescalerComponent, Resolution, RGBAColor,
-    TilesComponent, Transition, UpdateSceneError, VerticalAlign, ViewChildrenDirection, ViewComponent, YuvPlanes,
+    TextComponent, TilesComponent, Transition, UpdateSceneError, VerticalAlign, ViewChildrenDirection, ViewComponent, YuvPlanes,
 )

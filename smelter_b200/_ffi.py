@@ -59,6 +59,16 @@ class Position(C.Structure):
                 ("rotation_degrees", C.c_float)]
 
 
+class Atlas(C.Structure):       # smr_atlas
+    _fields_ = [("data", C.c_void_p), ("width", C.c_uint32), ("height", C.c_uint32), ("pitch", C.c_uint32)]
+
+
+class Text(C.Structure):        # smr_text: a Text component's laid-out payload (glyphs: smr_glyph records, GLYPH_DTYPE)
+    _fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("background", Rgba), ("glyphs", C.c_void_p),
+                ("n_glyphs", C.c_uint32), ("mask_atlas", C.POINTER(Atlas)), ("color_atlas", C.POINTER(Atlas)),
+                ("color_mode", C.c_int32)]
+
+
 class Component(C.Structure):
     pass
 
@@ -74,6 +84,7 @@ Component._fields_ = [
     ("tiles_width", OptF32), ("tiles_height", OptF32),
     ("tile_aspect_ratio_w", C.c_uint32), ("tile_aspect_ratio_h", C.c_uint32),
     ("tiles_margin", C.c_float), ("tiles_padding", C.c_float),
+    ("text", C.POINTER(Text)),
 ]
 
 
@@ -100,10 +111,6 @@ class RenderLayout(C.Structure):
                 ("child_index", C.c_int32), ("crop_top", C.c_float), ("crop_left", C.c_float),
                 ("crop_width", C.c_float), ("crop_height", C.c_float), ("masks_len", C.c_int32),
                 ("masks", Mask * MAX_MASKS)]
-
-
-class Atlas(C.Structure):       # smr_atlas
-    _fields_ = [("data", C.c_void_p), ("width", C.c_uint32), ("height", C.c_uint32), ("pitch", C.c_uint32)]
 
 
 GLYPH_COLOR, GLYPH_MASK = 0, 1

@@ -1898,14 +1898,30 @@ int launch_preprocess(const Tex &src, int mode, int rescale, uint8_t *out, int o
 // One thread per pixel of a 32 x 8 tile; the block walks the glyph list 256 entries at a time, keeps (in order) the
 // ones whose quad touches the tile, and every pixel blends those that cover it.  Quads sit on whole pixels and whole
 // atlas texels, so a covered pixel reads exactly one texel.  Rendered once per scene update, not per frame.
+// Every text node of a tick is one launch: block b belongs to the job whose tile range [tile_begin[i], tile_begin[i + 1])
+// holds it (a binary search by one thread), and the job is copied to shared memory.
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_text(const __grid_constant__ TextJob J) {
+__global__ void __launch_bounds__(256) k_text(const TextJob *__restrict__ jobs, const int32_t *__restrict__ tile_begin, int n_jobs) {
     __shared__ Tables T;
     __shared__ int s_list[256];
     __shared__ int s_wc[8];
-    load_tables(T);
+    __shared__ TextJob J;
     const int lane = threadIdx.x, warp = threadIdx.y, tid = warp * 32 + lane;
-    const int x0 = blockIdx.x * 32, y0 = blockIdx.y * 8, px = x0 + lane, py = y0 + warp;
+    if (tid == 0) {
+        const int b = (int)blockIdx.x;
+        int lo = 0, hi = n_jobs - 1;   // the last job i with tile_begin[i] <= b
+        while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if (tile_begin[mid] <= b) lo = mid; else hi = mid - 1;
+        }
+        J = jobs[lo];
+        const int t = b - tile_begin[lo], tiles_x = (J.width + 31) / 32;
+        s_wc[0] = (t % tiles_x) * 32;   // the tile's origin, handed over through s_wc before the glyph loop reuses it
+        s_wc[1] = (t / tiles_x) * 8;
+    }
+    load_tables(T);   // ends in __syncthreads
+    const int x0 = s_wc[0], y0 = s_wc[1], px = x0 + lane, py = y0 + warp;
+    __syncthreads();   // s_wc is rewritten by the glyph loop
     uchar4 d;
     if (J.mode == 0) d = make_uchar4((unsigned char)srgb_encode(T, J.bg[0]), (unsigned char)srgb_encode(T, J.bg[1]), (unsigned char)srgb_encode(T, J.bg[2]), (unsigned char)unorm8(J.bg[3]));
     else d = make_uchar4((unsigned char)unorm8(J.bg[0]), (unsigned char)unorm8(J.bg[1]), (unsigned char)unorm8(J.bg[2]), (unsigned char)unorm8(J.bg[3]));
@@ -1957,9 +1973,9 @@ __global__ void __launch_bounds__(256) k_text(const __grid_constant__ TextJob J)
     if (px < J.width && py < J.height) reinterpret_cast<uchar4 *>(J.out + (size_t)py * J.out_pitch)[px] = d;
 }
 
-int launch_text(const TextJob &job, Stream s) {
-    dim3 b(32, 8), g((job.width + 31) / 32, (job.height + 7) / 8);
-    k_text<<<g, b, 0, (cudaStream_t)s>>>(job);
+int launch_text(const TextJob *jobs_dev, const int32_t *tile_begin_dev, int n_jobs, int n_tiles, Stream s) {
+    if (n_jobs <= 0 || n_tiles <= 0) return 0;
+    k_text<<<n_tiles, dim3(32, 8), 0, (cudaStream_t)s>>>(jobs_dev, tile_begin_dev, n_jobs);
     return check_launch("k_text") ? 1 : -1;
 }
 

@@ -257,8 +257,11 @@ inline int fused_source_class(int tex_kind) {
 }
 // FramePreProcessor: node texture of `src` (rescale = 0) or its linear-filtered rescale to out_w x out_h
 int launch_preprocess(const Tex &src, int mode, int rescale, uint8_t *out, int out_pitch, int out_w, int out_h, Stream s);
-// text node texture: clear + glyph quads alpha-blended in list order
-int launch_text(const TextJob &job, Stream s);
+// text node textures: clear + glyph quads alpha-blended in list order, every job of jobs_dev in one launch.  Job i owns the
+// 32 x 8 tiles [tile_begin_dev[i], tile_begin_dev[i + 1]) of the grid (text_tiles of each job, prefix sums); n_tiles =
+// tile_begin[n_jobs]
+inline int text_tiles(int width, int height) { return ((width + 31) / 32) * ((height + 7) / 8); }
+int launch_text(const TextJob *jobs_dev, const int32_t *tile_begin_dev, int n_jobs, int n_tiles, Stream s);
 // full_range: fused_launch_range of every job of the launch
 int launch_resample_fused(const FusedKernel &k, int src, int full_range, const FusedJob *jobs_dev, const FusedPiece *pieces_dev,
                           const int *piece_begin_dev, int nblocks, Stream s);

@@ -303,8 +303,18 @@ class Renderer {
         int node_tex = -1;      // index in the tick's texture table of the materialised RGBA8 node texture
         int raw_tex = -1;       // index of the virtual (fused K1/K2) texture
     };
+    // A Text component of an output's scene (TextRendererNode, transformations/text_renderer.rs): its node texture and the
+    // job that draws it.  The texture, the glyphs and the atlases live in device memory allocated and freed in the order of
+    // stream_, so the ticks submitted before a scene update finish reading them before they are released.
+    struct TextNode {
+        Input in;               // the node texture as a layout child: TEX_RGBA8 of width x height (1 x 1 for 0 x 0), always live
+        dev::TextJob job = {};  // draws `in.tex`
+        std::shared_ptr<void> mem, atlas[2];   // texture + glyphs; the mask and colour atlases (shared within the scene)
+        bool rendered = false;  // drawn since the last smr_update_scene of the output (`was_rendered`)
+    };
     struct Output {
         OutputNode node;
+        std::vector<std::unique_ptr<TextNode>> texts;   // node.texts, in the same order
         int32_t format = 0;
         Resolution res;
         DevBuf planes[kTicksInFlight][3];       // device staging for host outputs, one set per tick in flight: the read-back of
@@ -435,14 +445,18 @@ class Renderer {
         std::vector<OutputRec> outputs;
         std::vector<Fill> fills;
         std::vector<PendingCopy> d2h;
+        std::vector<TextNode *> texts;        // text nodes drawn by this tick (one launch, before everything that reads them)
         std::map<std::tuple<int, uint32_t, uint32_t, uint32_t, uint32_t, int, int>, int> resample_cache;
         void clear() {   // keeps the vectors' capacity
             tex.clear();
             for (auto &s : stages) s.clear();
             fused.clear(); tmaps.clear(); weight_jobs.clear(); convert_jobs.clear();
-            composites.clear(); outputs.clear(); fills.clear(); d2h.clear(); resample_cache.clear();
+            composites.clear(); outputs.clear(); fills.clear(); d2h.clear(); texts.clear(); resample_cache.clear();
         }
     } plan_;
+    using AtlasUploads = std::map<const TextAtlas *, std::shared_ptr<void>>;
+    smr_status make_text_node(const std::shared_ptr<const TextPayload> &p, AtlasUploads &atlases, std::unique_ptr<TextNode> &out);
+    void plan_text_nodes(Output &o);
     void plan_tiles(Output &o, CompositeRec &pc, const std::vector<dev::LayerDev> &layers, int W, int H);
     std::vector<WeightKey> new_weight_keys_;   // cache entries whose k_weights launch is not enqueued yet
     void rollback_weights();                   // a tick that fails before that launch must not leave them behind
@@ -481,6 +495,7 @@ class Renderer {
     int slot_ = 0;
     bool uploaded_ = false;
     int sm_count_ = 132;
+    DevBuf text_job_;                  // smr_render_text: its one job and tile table
     void drain() {
         if (stream_) cudaStreamSynchronize(stream_);
         if (copy_stream_) cudaStreamSynchronize(copy_stream_);
@@ -539,6 +554,8 @@ Renderer::~Renderer() {
             cudaFree(kv.second.weights); cudaFree(kv.second.inv); cudaFree(kv.second.first);
         }
         for (auto &kv : lane_perms_) cudaFree(kv.second);
+        outputs_.clear();   // text nodes free their memory on stream_
+        cudaStreamSynchronize(stream_);
         for (void *p : peer_opened_) cudaIpcCloseMemHandle(p);
         for (void *p : peer_own_) cudaFree(p);
         if (barrier_word_) cudaFree(barrier_word_);
@@ -643,6 +660,20 @@ smr_status Renderer::update_scene(const char *output_id, uint32_t w, uint32_t h,
         set_error(err);
         return err.find("outside") != std::string::npos ? SMR_ERR_UNSUPPORTED : SMR_ERR_INVALID_ARGUMENT;
     }
+    // the text nodes are made (and uploaded) before the scene state changes, so that a failed upload leaves it as it was
+    std::vector<std::shared_ptr<const TextPayload>> payloads;
+    std::vector<const Component *> todo{&c};
+    while (!todo.empty()) {
+        const Component *k = todo.back();
+        todo.pop_back();
+        if (k->text) payloads.push_back(k->text);
+        for (const Component &ch : k->children) todo.push_back(&ch);
+    }
+    std::map<const TextPayload *, std::unique_ptr<TextNode>> made;
+    AtlasUploads atlases;
+    if (!host_only_) CUDA_OK(cudaSetDevice(opts_.cuda_device));   // text memory is allocated and released on stream_
+    for (const auto &p : payloads)
+        if (smr_status st = make_text_node(p, atlases, made[p.get()]); st != SMR_OK) return st;
     OutputNode node;
     if (!scene_.update_scene(output_id, c, {w, h}, node, err)) {
         set_error(err);
@@ -650,10 +681,78 @@ smr_status Renderer::update_scene(const char *output_id, uint32_t w, uint32_t h,
     }
     Output &o = outputs_[output_id];
     o.node = std::move(node);
+    o.texts.clear();   // the memory of the replaced nodes is released on stream_, after the ticks that read it
+    for (const auto &p : o.node.texts) o.texts.push_back(std::move(made[p.get()]));
     o.format = fmt;
     o.res = {w, h};
     o.flat = false; o.flat_layouts.clear(); o.flat_children.clear();
     return SMR_OK;
+}
+
+// A text node for `p`: the node texture (1 x 1 for 0 x 0), and on a device handle the texture, glyph and atlas memory and
+// the job that draws it.  Host memory is copied on stream_ (pageable sources: staged before the call returns).
+smr_status Renderer::make_text_node(const std::shared_ptr<const TextPayload> &p, AtlasUploads &atlases,
+                                    std::unique_ptr<TextNode> &out) {
+    auto t = std::make_unique<TextNode>();
+    const bool empty = p->width == 0 || p->height == 0;
+    const int w = empty ? 1 : (int)p->width, h = empty ? 1 : (int)p->height;
+    Input &in = t->in;
+    in.has_frame = true;
+    in.res = {(size_t)w, (size_t)h};
+    in.tex.kind = dev::TEX_RGBA8; in.tex.width = w; in.tex.height = h; in.tex.pitch0 = w * 4;
+    dev::TextJob &J = t->job;
+    J.width = w; J.height = h; J.mode = opts_.rendering_mode; J.color_mode = p->color_mode;
+    if (!empty) {   // 0 x 0: a transparent clear and no glyphs
+        J.n_glyphs = (int)p->glyphs.size();
+        shader_color(p->background, J.bg);
+    }
+    if (host_only_) { out = std::move(t); return SMR_OK; }
+    cudaStream_t s = stream_;
+    auto alloc = [&](size_t bytes, std::shared_ptr<void> &buf) -> smr_status {
+        void *d = nullptr;
+        CUDA_OK(cudaMallocAsync(&d, bytes, s));
+        buf = std::shared_ptr<void>(d, [s](void *q) { cudaFreeAsync(q, s); });
+        return SMR_OK;
+    };
+    const size_t tex_bytes = ((size_t)w * h * 4 + 255) & ~(size_t)255, glyph_bytes = sizeof(smr_glyph) * (size_t)J.n_glyphs;
+    if (smr_status st = alloc(tex_bytes + glyph_bytes, t->mem); st != SMR_OK) return st;
+    uint8_t *base = (uint8_t *)t->mem.get();
+    in.tex.p0 = base;
+    J.out = base; J.out_pitch = w * 4;
+    if (J.n_glyphs) {
+        CUDA_OK(cudaMemcpyAsync(base + tex_bytes, p->glyphs.data(), glyph_bytes, cudaMemcpyHostToDevice, s));
+        stats_.h2d_bytes += glyph_bytes;
+        J.glyphs = reinterpret_cast<const dev::GlyphDev *>(base + tex_bytes);
+    }
+    const TextAtlas *atl[2] = {p->mask.get(), p->color.get()};
+    for (int k = 0; k < 2; k++) {
+        if (!atl[k] || empty) continue;
+        std::shared_ptr<void> &buf = atlases[atl[k]];   // one upload per atlas of the scene
+        if (!buf) {
+            if (smr_status st = alloc(atl[k]->data.size(), buf); st != SMR_OK) return st;
+            CUDA_OK(cudaMemcpyAsync(buf.get(), atl[k]->data.data(), atl[k]->data.size(), cudaMemcpyHostToDevice, s));
+            stats_.h2d_bytes += atl[k]->data.size();
+        }
+        t->atlas[k] = buf;
+        const uint8_t *d = (const uint8_t *)buf.get();
+        if (k == 0) { J.mask = d; J.mask_w = (int)atl[k]->width; J.mask_h = (int)atl[k]->height; J.mask_pitch = (int)atl[k]->width; }
+        else { J.color = d; J.color_w = (int)atl[k]->width; J.color_h = (int)atl[k]->height; J.color_pitch = (int)atl[k]->width * 4; }
+    }
+    out = std::move(t);
+    return SMR_OK;
+}
+
+// A tick that renders output `o`: each of its text nodes enters the texture table, and those not drawn since the last
+// smr_update_scene join the tick's text launch
+void Renderer::plan_text_nodes(Output &o) {
+    if (o.flat) return;
+    for (auto &t : o.texts) {
+        t->in.node_tex = -1;
+        t->in.raw_tex = add_texture(t->in.tex, false);
+        if (t->rendered) continue;
+        t->rendered = true;   // undone if the tick fails before its launch
+        plan_.texts.push_back(t.get());
+    }
 }
 
 // One smr_render_layout (type and masks_len checked by the caller)
@@ -701,6 +800,8 @@ smr_status Renderer::set_layouts(const char *output_id, uint32_t w, uint32_t h, 
     o.format = fmt;
     o.res = {w, h};
     o.flat = true;
+    if (!o.texts.empty() && !host_only_) CUDA_OK(cudaSetDevice(opts_.cuda_device));
+    o.texts.clear();
     o.flat_root = {root_w, root_h};
     o.flat_children.clear();
     for (uint32_t i = 0; i < n_children; i++) o.flat_children.push_back(child_ids[i] ? child_ids[i] : "");
@@ -1312,9 +1413,17 @@ smr_status Renderer::render_text(uint32_t w, uint32_t h, smr_rgba bg, const smr_
         stats_.h2d_bytes += bytes;
         J.glyphs = reinterpret_cast<const dev::GlyphDev *>(pre_planes_[2].p);
     }
+    // the job and its tile table, as the tick's text launch reads them from the parameter arena
+    const size_t begin_off = (sizeof(dev::TextJob) + 15) & ~(size_t)15;
+    const int32_t begin[2] = {0, dev::text_tiles((int)w, (int)h)};
+    CUDA_OK(text_job_.ensure(begin_off + sizeof(begin)));
     return write_rgba(rgba, pitch, mem_kind, w, h, [&](uint8_t *dst, int dpitch) {
         J.out = dst; J.out_pitch = dpitch;
-        return dev::launch_text(J, stream_);
+        // pageable sources: staged before the copies return; write_rgba waits for the launch
+        if (cudaMemcpyAsync(text_job_.p, &J, sizeof(J), cudaMemcpyHostToDevice, stream_) != cudaSuccess ||
+            cudaMemcpyAsync(text_job_.p + begin_off, begin, sizeof(begin), cudaMemcpyHostToDevice, stream_) != cudaSuccess)
+            return -1;
+        return dev::launch_text((const dev::TextJob *)text_job_.p, (const int32_t *)(text_job_.p + begin_off), 1, begin[1], stream_);
     });
 }
 
@@ -1514,16 +1623,22 @@ void Renderer::plan_tiles(Output &o, CompositeRec &pc, const std::vector<dev::La
     }
 }
 
-// An output's children at `pts` (sources[i].resolution(), layout.rs:176-179): the input behind each (nullptr: no live frame)
-// and its resolution.  Returns the root resolution.
+// An output's children at `pts` (sources[i].resolution(), layout.rs:176-179): the input or text node behind each (nullptr:
+// an input without a live frame) and its resolution.  Returns the root resolution.
 Resolution Renderer::output_children(const Output &o, const OutputNode &node, uint64_t pts, std::vector<Input *> &child_in,
                                      std::vector<std::optional<Resolution>> &child_res) {
-    for (const std::string &id : (o.flat ? o.flat_children : node.child_input_ids)) {
-        auto it = inputs_.find(id);
-        Input *in = it != inputs_.end() && it->second.has_frame ? &it->second : nullptr;
+    auto add = [&](Input *in) {
         child_in.push_back(in);
         child_res.push_back(in ? std::optional<Resolution>(in->res) : std::nullopt);
-    }
+    };
+    auto input = [&](const std::string &id) {
+        auto it = inputs_.find(id);
+        return it != inputs_.end() && it->second.has_frame ? &it->second : nullptr;
+    };
+    if (o.flat)
+        for (const std::string &id : o.flat_children) add(input(id));
+    else
+        for (const NodeChild &ch : node.children) add(ch.text >= 0 ? &o.texts[ch.text]->in : input(ch.input_id));
     return o.flat ? o.flat_root : node.layout_resolution(pts);
 }
 
@@ -1664,10 +1779,17 @@ smr_status Renderer::plan_output(Output &o, smr_output_frame &of, uint64_t pts) 
         plan_.outputs.push_back({j, src_tex});
     };
 
-    if (!o.flat && o.node.root_is_input) {  // pass-through: the root texture IS the input's node texture
-        auto it = inputs_.find(o.node.root_input_id);
-        if (it == inputs_.end() || !it->second.has_frame) { push_fill(); return SMR_OK; }
-        Input &in = it->second;
+    plan_text_nodes(o);
+    if (!o.flat && (o.node.root_is_input || o.node.root_text >= 0)) {  // pass-through: the root texture IS the node texture
+        Input *root_in = nullptr;
+        if (o.node.root_text >= 0) {
+            root_in = &o.texts[o.node.root_text]->in;
+        } else {
+            auto it = inputs_.find(o.node.root_input_id);
+            if (it != inputs_.end() && it->second.has_frame) root_in = &it->second;
+        }
+        if (!root_in) { push_fill(); return SMR_OK; }
+        Input &in = *root_in;
         if (o.format == SMR_OUT_RGBA8 && (in.res.width != o.res.width || in.res.height != o.res.height)) {
             // the reference hands out a clone of the node texture at ITS resolution (render_loop.rs:81-103)
             set_error("RGBA output of a pass-through root must match the input resolution");
@@ -1784,6 +1906,10 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
         Renderer *r; bool armed = true;
         ~WeightGuard() { if (armed) r->rollback_weights(); }
     } weight_guard{this};
+    struct TextGuard {     // any return before the text launch is enqueued leaves this tick's text nodes to the next tick
+        std::vector<TextNode *> &nodes; bool armed = true;
+        ~TextGuard() { if (armed) for (TextNode *t : nodes) t->rendered = false; }
+    } text_guard{plan_.texts};
     smr_status st = select_inputs(pts, in, n_in, [&](Input &I, const smr_input_frame *f) {
         I.node_tex = I.raw_tex = -1;
         return f ? upload_input(I, *f) : SMR_OK;
@@ -1902,6 +2028,13 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
     }
     const size_t fj_off = param_put_all(plan_.fused, &FusedRec::job);
     const size_t cj_off = param_put_all(plan_.composites, &CompositeRec::job);   // read by k_composite_multi
+    // text jobs and the prefix table of their tile counts
+    std::vector<int32_t> text_begin(1, 0);
+    for (const TextNode *t : plan_.texts) text_begin.push_back(text_begin.back() + dev::text_tiles(t->job.width, t->job.height));
+    const size_t tj_off = param_alloc(sizeof(dev::TextJob) * plan_.texts.size());
+    for (size_t i = 0; i < plan_.texts.size(); i++)
+        memcpy(param_host_.data() + tj_off + i * sizeof(dev::TextJob), &plan_.texts[i]->job, sizeof(dev::TextJob));
+    const size_t tb_off = param_put(text_begin.data(), sizeof(int32_t) * text_begin.size());
     // the arena is sized: its offsets become device pointers in the packed jobs
     CUDA_OK(param_pinned_[slot_].ensure(param_used_));
     CUDA_OK(param_dev_[slot_].ensure(param_used_));
@@ -1931,6 +2064,12 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
     // ---- launches -----------------------------------------------------------------------------
     auto launched = [&](int n) -> bool { if (n < 0) return false; launches += (uint64_t)n; return true; };
     prof_mark(-1);
+    if (!plan_.texts.empty()) {   // every text node this tick draws: materialised node textures, like k_convert's
+        if (!launched(dev::launch_text((const dev::TextJob *)(pd + tj_off), (const int32_t *)(pd + tb_off), (int)plan_.texts.size(),
+                                       text_begin.back(), stream_))) goto fail;
+        prof_mark(SMR_KERNEL_CONVERT);
+    }
+    text_guard.armed = false;
     for (auto &cv : plan_.convert_jobs) {
         const dev::Tex &src = plan_.tex[cv.first].tex;
         if (!launched(dev::launch_convert_to_rgba(src, fb + cv.second, src.width * 4, stream_))) goto fail;
@@ -2388,7 +2527,7 @@ smr_status Renderer::debug_layouts(const char *output_id, uint64_t pts, smr_rend
     if (it == outputs_.end()) { set_error("output not registered"); return SMR_ERR_OUTPUT_NOT_REGISTERED; }
     Output &o = it->second;
     *n = 0;
-    if (!o.flat && o.node.root_is_input) { if (rw) *rw = 0; if (rh) *rh = 0; return SMR_OK; }
+    if (!o.flat && (o.node.root_is_input || o.node.root_text >= 0)) { if (rw) *rw = 0; if (rh) *rh = 0; return SMR_OK; }
     OutputNode copy = o.node;  // do not advance Tiles::last_layout
     std::vector<Input *> child_in;
     std::vector<std::optional<Resolution>> child_res;

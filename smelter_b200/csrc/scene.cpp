@@ -6,6 +6,7 @@
 #include <cmath>
 #include <cstring>
 #include <set>
+#include <tuple>
 
 namespace smr {
 
@@ -72,7 +73,56 @@ bool TilesParam::operator==(const TilesParam &o) const {
 static RGBA rgba_from_c(const smr_rgba &c) { return {c.r, c.g, c.b, c.a}; }
 static OptF optf_from_c(const smr_opt_f32 &o) { return o.has_value ? OptF(o.value) : OptF(); }
 
-bool component_from_c(const smr_component *c, Component &out, std::string &err, int depth) {
+// The atlases of one tree, by the caller's data pointer and geometry (pointer, width, height, pitch, row bytes): each is
+// copied once
+using AtlasKey = std::tuple<const void *, uint32_t, uint32_t, size_t, size_t>;
+using AtlasCopies = std::map<AtlasKey, std::shared_ptr<const TextAtlas>>;
+
+// smr_text -> TextPayload with smr_render_text's checks (0 x 0 allowed: the reference's 1 x 1 transparent node texture)
+static bool text_from_c(const smr_text *t, AtlasCopies &atlases, std::shared_ptr<const TextPayload> &out, std::string &err) {
+    if (!t) { err = "Text component without a payload"; return false; }
+    if (t->width > 16384 || t->height > 16384) { err = "text texture resolution out of range"; return false; }
+    if (t->n_glyphs > (1u << 22)) { err = "too many glyphs"; return false; }
+    if (t->n_glyphs && !t->glyphs) { err = "glyph pointer is null"; return false; }
+    if (t->color_mode != 0 && t->color_mode != 1) { err = "text color_mode must be 0 (Accurate) or 1 (Web)"; return false; }
+    auto p = std::make_shared<TextPayload>();
+    p->width = t->width; p->height = t->height;
+    p->background = rgba_from_c(t->background);
+    p->color_mode = t->color_mode;
+    p->glyphs.assign(t->glyphs, t->glyphs + t->n_glyphs);
+    bool need[2] = {false, false};   // mask, colour
+    for (const smr_glyph &g : p->glyphs) {
+        if (g.content == SMR_GLYPH_MASK) need[0] = true;
+        else if (g.content == SMR_GLYPH_COLOR) need[1] = true;
+        else { err = "glyph content type must be SMR_GLYPH_COLOR or SMR_GLYPH_MASK"; return false; }
+    }
+    const smr_atlas *atl[2] = {t->mask_atlas, t->color_atlas};
+    std::shared_ptr<const TextAtlas> *dst[2] = {&p->mask, &p->color};
+    for (int k = 0; k < 2; k++) {
+        if (!need[k]) continue;
+        const smr_atlas *a = atl[k];
+        if (!a || !a->data || a->width == 0 || a->height == 0 || a->width > 16384 || a->height > 16384) {
+            err = k == 0 ? "mask glyphs need a mask atlas" : "colour glyphs need a colour atlas";
+            return false;
+        }
+        const size_t row = (size_t)a->width * (k == 0 ? 1 : 4), sp = a->pitch ? a->pitch : row;
+        if (sp < row) { err = "atlas pitch smaller than a row"; return false; }
+        const AtlasKey key{a->data, a->width, a->height, sp, row};
+        auto hit = atlases.find(key);
+        if (hit != atlases.end()) { *dst[k] = hit->second; continue; }
+        auto copy = std::make_shared<TextAtlas>();
+        copy->width = a->width; copy->height = a->height;
+        copy->data.resize(row * a->height);
+        for (uint32_t y = 0; y < a->height; y++)
+            memcpy(copy->data.data() + row * y, (const uint8_t *)a->data + sp * y, row);
+        atlases[key] = copy;
+        *dst[k] = copy;
+    }
+    out = std::move(p);
+    return true;
+}
+
+static bool component_from_c(const smr_component *c, Component &out, std::string &err, int depth, AtlasCopies &atlases) {
     if (!c) { err = "null component"; return false; }
     if (depth > 256) { err = "component tree too deep"; return false; }
     out = Component();
@@ -83,12 +133,14 @@ bool component_from_c(const smr_component *c, Component &out, std::string &err, 
             if (!c->input_id) { err = "InputStream without input_id"; return false; }
             out.input_id = c->input_id;
             return true;
+        case SMR_COMPONENT_TEXT:
+            return text_from_c(c->text, atlases, out.text, err);
         case SMR_COMPONENT_VIEW:
         case SMR_COMPONENT_TILES:
         case SMR_COMPONENT_RESCALER:
             break;
         default:
-            err = "component type outside the compositor hot path (Shader/WebView/Image/Text)";
+            err = "component type outside the compositor hot path (Shader/WebView/Image)";
             return false;
     }
     if (c->type == SMR_COMPONENT_RESCALER && c->children_len != 1) {
@@ -98,7 +150,7 @@ bool component_from_c(const smr_component *c, Component &out, std::string &err, 
     if (c->children_len && !c->children) { err = "children pointer is null"; return false; }
     out.children.resize(c->children_len);
     for (uint32_t i = 0; i < c->children_len; i++)
-        if (!component_from_c(&c->children[i], out.children[i], err, depth + 1)) return false;
+        if (!component_from_c(&c->children[i], out.children[i], err, depth + 1, atlases)) return false;
 
     const smr_position &p = c->position;
     out.position.absolute = p.is_absolute != 0;
@@ -145,6 +197,11 @@ bool component_from_c(const smr_component *c, Component &out, std::string &err, 
         return false;
     }
     return true;
+}
+
+bool component_from_c(const smr_component *c, Component &out, std::string &err, int depth) {
+    AtlasCopies atlases;
+    return component_from_c(c, out, err, depth, atlases);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -386,7 +443,8 @@ static RescalerParam rescaler_at(const Stateful &c, uint64_t pts) {  // rescaler
 
 const std::optional<std::string> &Stateful::component_id() const {
     switch (kind) {
-        case InputStream: return input_component_id;
+        case InputStream:
+        case Text: return leaf_component_id;
         case View: return view_end.id;
         case Rescaler: return rescaler_end.id;
         default: return tiles.id;
@@ -419,11 +477,11 @@ Position Stateful::position(uint64_t pts) const {
 }
 
 OptF Stateful::width(uint64_t pts) const {
-    if (kind == InputStream) return OptF(size.width);
+    if (!is_layout()) return OptF(size.width);
     return position(pts).width;
 }
 OptF Stateful::height(uint64_t pts) const {
-    if (kind == InputStream) return OptF(size.height);
+    if (!is_layout()) return OptF(size.height);
     return position(pts).height;
 }
 
@@ -446,6 +504,8 @@ void Stateful::update_state(const std::optional<Resolution> *inputs, size_t n) {
             if (off < n && inputs[off]) c.size = {(float)inputs[off]->width, (float)inputs[off]->height};
             else c.size = {0.0f, 0.0f};
             off += 1;
+        } else if (c.kind == Text) {
+            off += 1;   // no state
         } else {
             size_t cnt = c.node_children_count();
             c.update_state(inputs + std::min(off, n), off < n ? std::min(cnt, n - off) : 0);
@@ -1033,9 +1093,16 @@ static Stateful build_stateful(const Component &c, const BuildCtx &ctx) {
         case SMR_COMPONENT_INPUT_STREAM: {  // input_stream_component.rs:24-44
             s.kind = Stateful::InputStream;
             s.input_id = c.input_id;
-            s.input_component_id = c.id;
+            s.leaf_component_id = c.id;
             auto it = ctx.input_resolutions->find(c.input_id);
             if (it != ctx.input_resolutions->end()) s.size = {(float)it->second.width, (float)it->second.height};
+            return s;
+        }
+        case SMR_COMPONENT_TEXT: {  // text_component.rs:36-53: the size is the caller's layout resolution
+            s.kind = Stateful::Text;
+            s.leaf_component_id = c.id;
+            s.text = c.text;
+            s.size = {(float)c.text->width, (float)c.text->height};
             return s;
         }
         case SMR_COMPONENT_VIEW: {  // view_component.rs:103-160
@@ -1139,7 +1206,10 @@ bool SceneState::update_scene(const std::string &output_id, const Component &roo
     // intermediate_node().build_tree(Some(resolution), last_pts), :154-196
     out = OutputNode();
     out.resolution = resolution;
-    if (!st.root.is_layout()) {
+    if (st.root.kind == Stateful::Text) {
+        out.root_text = 0;
+        out.texts.push_back(st.root.text);
+    } else if (!st.root.is_layout()) {
         out.root_is_input = true;
         out.root_input_id = st.root.input_id;
     } else {
@@ -1147,7 +1217,16 @@ bool SceneState::update_scene(const std::string &output_id, const Component &roo
         out.size = {(float)resolution.width, (float)resolution.height};
         std::vector<const Stateful *> leaves;
         st.root.node_children(leaves);
-        for (const Stateful *l : leaves) out.child_input_ids.push_back(l->input_id);
+        for (const Stateful *l : leaves) {
+            NodeChild ch;
+            if (l->kind == Stateful::Text) {
+                ch.text = (int)out.texts.size();
+                out.texts.push_back(l->text);
+            } else {
+                ch.input_id = l->input_id;
+            }
+            out.children.push_back(std::move(ch));
+        }
     }
     output_scenes_[output_id] = root;
     output_states_[output_id] = std::move(st);

@@ -8,6 +8,7 @@
 #include <cstddef>
 #include <cstdint>
 #include <map>
+#include <memory>
 #include <optional>
 #include <string>
 #include <utility>
@@ -90,6 +91,20 @@ struct Transition {
     bool should_interrupt = false;
 };
 
+// A Text component's laid-out payload (smr_text), copied out of the caller's memory.  Atlases are tightly packed and shared
+// by the components of one smr_update_scene that passed the same smr_atlas data pointer.
+struct TextAtlas {
+    std::vector<uint8_t> data;
+    uint32_t width = 0, height = 0;
+};
+struct TextPayload {
+    uint32_t width = 0, height = 0;   // the caller's layout resolution; 0 x 0 draws one transparent pixel
+    RGBA background;
+    std::vector<smr_glyph> glyphs;
+    std::shared_ptr<const TextAtlas> mask, color;   // null when no glyph reads it
+    int32_t color_mode = 0;
+};
+
 // scene::Component (scene.rs:50-60); only the variants on the compositor path
 struct Component {
     int type = SMR_COMPONENT_VIEW;
@@ -112,6 +127,7 @@ struct Component {
     OptF tiles_width, tiles_height;
     uint32_t tile_aspect_w = 16, tile_aspect_h = 9;
     float tiles_margin = 0, tiles_padding = 0;
+    std::shared_ptr<const TextPayload> text;
 };
 
 // Converts the C tree; returns false + message for variants outside the hot path.
@@ -238,11 +254,12 @@ struct TransitionState {
 };
 
 struct Stateful {
-    enum Kind { InputStream, View, Tiles, Rescaler } kind = View;
-    // InputStream (scene/input_stream_component.rs)
+    enum Kind { InputStream, View, Tiles, Rescaler, Text } kind = View;
+    // InputStream (scene/input_stream_component.rs), Text (scene/text_component.rs): the leaves
     std::string input_id;
-    std::optional<std::string> input_component_id;
-    Size size;
+    std::optional<std::string> leaf_component_id;
+    Size size;                                // InputStream: its last frame's resolution; Text: the layout resolution
+    std::shared_ptr<const TextPayload> text;
     // View
     std::optional<ViewParam> view_start;
     ViewParam view_end;
@@ -256,7 +273,7 @@ struct Stateful {
     std::optional<TransitionState> transition;
     std::vector<Stateful> children;  // Rescaler: exactly one
 
-    bool is_layout() const { return kind != InputStream; }
+    bool is_layout() const { return kind != InputStream && kind != Text; }
     const std::optional<std::string> &component_id() const;
     OptF width(uint64_t pts) const;   // scene.rs:105-117
     OptF height(uint64_t pts) const;  // scene.rs:119-131
@@ -267,13 +284,21 @@ struct Stateful {
     void update_state(const std::optional<Resolution> *inputs, size_t n);  // scene/layout.rs:105-137
 };
 
+// One child of the layout node (scene/layout.rs:95-103): an input, or text node `text` of the output
+struct NodeChild {
+    std::string input_id;
+    int text = -1;                            // index in OutputNode::texts, or -1: the input `input_id`
+};
+
 // scene/scene_state.rs
 struct OutputNode {
     bool root_is_input = false;
     std::string root_input_id;
+    int root_text = -1;                       // the root is text node texts[root_text] (-1: it is not a Text)
     Stateful layout_root;                     // LayoutNode.root.component (the render graph's clone)
     Size size;                                // SizedLayoutComponent.size
-    std::vector<std::string> child_input_ids; // node children, DFS order
+    std::vector<NodeChild> children;          // node children, DFS order
+    std::vector<std::shared_ptr<const TextPayload>> texts;   // the output's text nodes (the root, or children in DFS order)
     Resolution resolution;
 
     // scene::LayoutNode as LayoutProvider (scene/layout.rs:31-41, 240-261)

@@ -299,7 +299,22 @@ class TilesComponent:
     transition: Optional[Transition] = None
 
 
-Component = Union[InputStreamComponent, ViewComponent, RescalerComponent, TilesComponent]
+@dataclass
+class TextComponent:
+    """A Text component as the caller laid it out (smr_text): cosmic-text's resolution (width x height) and glyphon's
+    prepared glyph quads (records of _ffi.GLYPH_DTYPE, painter's order) over its mask atlas ((h, w) uint8) and colour
+    atlas ((h, w, 4) uint8).  color_mode: glyphon ColorMode, 0 Accurate, 1 Web."""
+    id: Optional[str] = None
+    width: int = 0
+    height: int = 0
+    background_color: RGBAColor = RGBAColor(0, 0, 0, 0)
+    glyphs: Optional[np.ndarray] = None
+    mask_atlas: Optional[np.ndarray] = None
+    color_atlas: Optional[np.ndarray] = None
+    color_mode: int = 0
+
+
+Component = Union[InputStreamComponent, ViewComponent, RescalerComponent, TilesComponent, TextComponent]
 
 
 def _opt(v):
@@ -373,6 +388,14 @@ def _to_c(comp, keep):
         c.horizontal_align, c.vertical_align = comp.horizontal_align, comp.vertical_align
         child = comp.child if comp.child is not None else ViewComponent()
         _children(c, [child], keep)
+    elif isinstance(comp, TextComponent):
+        F.lib().smr_component_default(F.COMPONENT_TEXT, C.byref(c))
+        g = _glyphs(comp.glyphs)
+        keep.append(g)
+        t = F.Text(comp.width, comp.height, _rgba(comp.background_color), g.ctypes.data if len(g) else None, len(g),
+                   _atlas(comp.mask_atlas, 1, keep), _atlas(comp.color_atlas, 4, keep), int(comp.color_mode))
+        keep.append(t)
+        c.text = C.pointer(t)
     elif isinstance(comp, TilesComponent):
         F.lib().smr_component_default(F.COMPONENT_TILES, C.byref(c))
         _fill_transition(c, comp.transition)
@@ -383,7 +406,7 @@ def _to_c(comp, keep):
         c.horizontal_align, c.vertical_align = comp.horizontal_align, comp.vertical_align
         _children(c, comp.children, keep)
     else:
-        # Shader / WebView / Image / Text are outside the compositor hot path: forward the tag so the
+        # Shader / WebView / Image are outside the compositor hot path: forward the tag so the
         # library answers SMR_ERR_UNSUPPORTED like any other caller would see
         c.type = getattr(comp, "component_type", F.COMPONENT_SHADER)
     if getattr(comp, "id", None) is not None:
@@ -391,6 +414,21 @@ def _to_c(comp, keep):
         keep.append(cid)
         c.id = cid
     return c
+
+
+def _glyphs(glyphs):
+    return np.ascontiguousarray(glyphs if glyphs is not None else np.zeros(0, F.GLYPH_DTYPE), dtype=np.dtype(F.GLYPH_DTYPE))
+
+
+def _atlas(a, channels, keep):
+    """an (h, w) R8 (channels 1) or (h, w, 4) RGBA8 atlas -> pointer to smr_atlas, or None"""
+    if a is None:
+        return None
+    a = np.ascontiguousarray(a, np.uint8)
+    assert a.ndim == (2 if channels == 1 else 3) and (channels == 1 or a.shape[2] == 4)
+    s = F.Atlas(a.ctypes.data, a.shape[1], a.shape[0], 0)
+    keep += [a, s]
+    return C.pointer(s)
 
 
 def _children(c, children, keep):
@@ -572,21 +610,11 @@ class Renderer:
         a valid FrameData.Rgba8 input.  A zero-sized text texture is one transparent pixel (text_renderer.rs:77-85)."""
         if width == 0 or height == 0:
             return np.zeros((1, 1, 4), np.uint8)
-        g = np.ascontiguousarray(glyphs, dtype=np.dtype(F.GLYPH_DTYPE))
-        keep, atl = [], []
-        for a, ch in ((mask_atlas, 1), (color_atlas, 4)):
-            if a is None:
-                atl.append(None)
-                continue
-            a = np.ascontiguousarray(a, np.uint8)
-            assert a.ndim == (2 if ch == 1 else 3) and (ch == 1 or a.shape[2] == 4)
-            keep.append(a)
-            atl.append(F.Atlas(a.ctypes.data, a.shape[1], a.shape[0], 0))
+        g = _glyphs(glyphs)
+        keep = []
         out = np.empty((height, width, 4), np.uint8)
-        bg = F.Rgba(background.r, background.g, background.b, background.a)
-        self._check(self._lib.smr_render_text(self._h, width, height, bg, g.ctypes.data if len(g) else None, len(g),
-                                              C.byref(atl[0]) if atl[0] is not None else None,
-                                              C.byref(atl[1]) if atl[1] is not None else None, int(color_mode),
+        self._check(self._lib.smr_render_text(self._h, width, height, _rgba(background), g.ctypes.data if len(g) else None, len(g),
+                                              _atlas(mask_atlas, 1, keep), _atlas(color_atlas, 4, keep), int(color_mode),
                                               out.ctypes.data, 0, F.MEM_HOST), RenderSceneError)
         return out
 
