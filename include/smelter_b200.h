@@ -61,7 +61,7 @@ typedef enum {
     /* declared so a shim can forward them; smr_update_scene answers SMR_ERR_UNSUPPORTED */
     SMR_COMPONENT_SHADER = 4,
     SMR_COMPONENT_WEB_VIEW = 5,
-    SMR_COMPONENT_IMAGE = 6,
+    SMR_COMPONENT_IMAGE = 6,       /* accepted when smr_component.image_id is set, see there */
     SMR_COMPONENT_TEXT = 7         /* payload in smr_component.text */
 } smr_component_type;
 
@@ -127,6 +127,14 @@ typedef struct smr_component {
     float tiles_margin, tiles_padding;
 
     const struct smr_text *text;           /* Text (smr_text below) */
+
+    /* Image (ImageComponent, scene/components.rs:63-80): an asset registered with smr_register_image, shown at
+     * image_width x image_height (a missing side follows from the asset's aspect ratio, both missing: the asset's size).
+     * NULL image_id: SMR_ERR_UNSUPPORTED, which is what a caller built before these fields existed sends (the tag and
+     * nothing else).  An id that is not registered, the empty string (the reference's Default) included, is
+     * SceneError::ImageNotFound: SMR_ERR_SCENE. */
+    const char *image_id;
+    smr_opt_f32 image_width, image_height;
 } smr_component;
 
 /* ------------------------------------ frames (types.rs:21-119) ------------------------------- */
@@ -222,7 +230,8 @@ typedef enum {
     SMR_KERNEL_OUTPUT = 6,         /* K10/K11 stand-alone */
     SMR_KERNEL_FILL = 7,           /* K6 */
     SMR_KERNEL_RESAMPLE_FUSED = 8, /* K1/K2 + both K8 passes in one kernel */
-    SMR_KERNEL_CLASSES = 9
+    SMR_KERNEL_IMAGE = 9,          /* image node textures (k_image) */
+    SMR_KERNEL_CLASSES = 10
 } smr_kernel_class;
 typedef struct {
     double total_ms[SMR_KERNEL_CLASSES];
@@ -238,9 +247,38 @@ void smr_destroy(smr_renderer *r);
 smr_status smr_register_input(smr_renderer *r, const char *input_id);
 smr_status smr_unregister_input(smr_renderer *r, const char *input_id);
 
+/* Renderer::register_renderer / unregister_renderer for RendererSpec::Image   state.rs:123-166, registry.rs:57-68
+ * An image asset arrives decoded, as straight-alpha RGBA8 frames of width x height in HOST memory (PNG / JPEG / GIF
+ * decoding stays with the caller, as text shaping does).  n_frames == 1 is a Bitmap asset (delay ignored), n_frames >= 2
+ * an Animated one (image.rs:69-79): frame k's pts is the sum of the delays before it, the animation's duration the sum
+ * of all delays, and a zero sum counts as 1 ns (animated_image.rs:52-112).  SMR_ERR_INVALID_ARGUMENT: a NULL id, spec
+ * or frame pointer, n_frames == 0 (NoFrames) or above 1000 (TooManyFrames), a side of 0 or above 16384, a pitch below
+ * 4 * width, delays whose sum does not fit 64 bits, an id already registered (RegisterError::KeyTaken), unregistering an
+ * unknown id; a failed call registers nothing.  The pixels are copied before the call returns (to the device, on the
+ * handle's stream); a host-only handle keeps sizes and timing only.  An asset is shared by the registry and every scene
+ * node that resolved it: unregistering removes the registry entry only, scenes already showing the asset keep drawing it,
+ * and its device memory is released on the handle's stream after the last tick that reads it.  Registering the same id
+ * again makes a new asset: a scene updated afterwards restarts its animation (Arc::ptr_eq, image_component.rs:100-111).
+ * Not supported: SVG assets (the reference rasterises them at the node's resolution, known only at scene update,
+ * svg_image.rs:262-292), URL / file sources (ImageSource). */
+typedef struct { const void *rgba; uint32_t pitch; uint64_t delay_ns; } smr_image_frame;   /* pitch 0 = packed */
+typedef struct { uint32_t width, height; const smr_image_frame *frames; uint32_t n_frames; } smr_image_spec;
+smr_status smr_register_image(smr_renderer *r, const char *image_id, const smr_image_spec *spec);
+smr_status smr_unregister_image(smr_renderer *r, const char *image_id);
+
 /* Renderer::update_scene(output_id, resolution, output_format, scene_root)   state.rs:177-188
- * Components: InputStream, View, Tiles, Rescaler and Text (anywhere, the root included); Shader, WebView and Image answer
- * SMR_ERR_UNSUPPORTED.  A Text root follows the rules of an InputStream root (an RGBA output has the text's size). */
+ * Components: InputStream, View, Tiles, Rescaler, Text and Image (anywhere, the root included); Shader and WebView answer
+ * SMR_ERR_UNSUPPORTED.  A Text or Image root follows the rules of an InputStream root (an RGBA output has the node's size).
+ * Image (scene/image_component.rs): the node's resolution is round(image_width) x round(image_height); with one side
+ * missing the other follows from the asset's aspect ratio, which the reference takes as the integer division
+ * width / height (640 x 360 gives 1, a portrait asset 0); with both missing it is the asset's size.  A resolved side of 0
+ * or above 16384 is SMR_ERR_SCENE and leaves the scene as it was.  A component with an id whose previous state is an Image
+ * with the same id, image_id, width and height and the same asset keeps its start pts; anything else starts at the pts
+ * of the last render.  The node texture is the asset frame sampled with the linear sampler at the node's resolution and
+ * premultiplied (add_premultiplied_alpha.wgsl).  A Bitmap node is drawn by the first smr_render of the output after each
+ * smr_update_scene of it.  An Animated node shows, at every tick, the frame whose pts is closest to
+ * (pts - start_pts) % duration (the first such frame on a tie); pts - start_pts saturates at 0 where the reference's
+ * subtraction would underflow.  A tick whose frame is the one the node texture already holds launches nothing for it. */
 smr_status smr_update_scene(smr_renderer *r, const char *output_id, uint32_t width, uint32_t height,
                             int32_t output_format, const smr_component *scene_root);
 /* Renderer::unregister_output                                       state.rs:115-123 */
@@ -439,6 +477,12 @@ void smr_component_default(int32_t type, smr_component *out);
 smr_status smr_debug_layouts(smr_renderer *r, const char *output_id, uint64_t pts_ns,
                              smr_render_layout *out, uint32_t capacity, uint32_t *n_out,
                              uint32_t *root_width, uint32_t *root_height);
+/* inspection (no device needed): the image nodes of an output's scene, the root or the node children in DFS order: the
+ * node's resolution, its start pts, and the asset frame a render at pts_ns shows.  SMR_ERR_BUFFER_TOO_SMALL when they do
+ * not fit in capacity (out = NULL asks for the count). */
+typedef struct { uint32_t width, height; uint64_t start_pts_ns; uint32_t frame; } smr_image_node_info;
+smr_status smr_debug_image_nodes(smr_renderer *r, const char *output_id, uint64_t pts_ns, smr_image_node_info *out,
+                                 uint32_t capacity, uint32_t *n_out);
 
 /* The FLATTENED form of the boundary (SURVEY 8b): a host that keeps the reference's scene/ tree (Component tree,
  * transitions, NestedLayout::flatten -- all Rust) hands over, per output and whenever they change, the RenderLayout[]

@@ -4,7 +4,7 @@
 The package is a thin ctypes mirror of the reference interface; all pixels come from
 libsmelter_b200.so (hand-written sm_90a CUDA).  There is no CPU fallback."""
 from .renderer import (  # noqa: F401
-    BorderRadius, BoxShadow, Component, Frame, FrameData, FramePreProcessor, FrameSet, HorizontalAlign, InputStreamComponent,
+    BorderRadius, BoxShadow, Component, Frame, FrameData, FramePreProcessor, FrameSet, HorizontalAlign, ImageComponent, InputStreamComponent,
     InterpolationKind, NvPlanes, OutputFrameFormat, Overflow, Padding, Position, Renderer, RendererError,
     RendererOptions, RenderingMode, RenderSceneError, RescaleMode, RescalerComponent, Resolution, RGBAColor,
     TextComponent, TilesComponent, Transition, UpdateSceneError, VerticalAlign, ViewChildrenDirection, ViewComponent, YuvPlanes,

@@ -69,6 +69,18 @@ class Text(C.Structure):        # smr_text: a Text component's laid-out payload 
                 ("color_mode", C.c_int32)]
 
 
+class ImageFrame(C.Structure):   # smr_image_frame
+    _fields_ = [("rgba", C.c_void_p), ("pitch", C.c_uint32), ("delay_ns", C.c_uint64)]
+
+
+class ImageSpec(C.Structure):    # smr_image_spec
+    _fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("frames", C.POINTER(ImageFrame)), ("n_frames", C.c_uint32)]
+
+
+class ImageNodeInfo(C.Structure):   # smr_image_node_info
+    _fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("start_pts_ns", C.c_uint64), ("frame", C.c_uint32)]
+
+
 class Component(C.Structure):
     pass
 
@@ -85,6 +97,7 @@ Component._fields_ = [
     ("tile_aspect_ratio_w", C.c_uint32), ("tile_aspect_ratio_h", C.c_uint32),
     ("tiles_margin", C.c_float), ("tiles_padding", C.c_float),
     ("text", C.POINTER(Text)),
+    ("image_id", C.c_char_p), ("image_width", OptF32), ("image_height", OptF32),
 ]
 
 
@@ -156,17 +169,17 @@ class CompositeLayerInfo(C.Structure):   # smr_composite_layer_info
 
 
 KERNEL_CLASSES = ["convert", "weights", "resample_box", "resample_first", "resample_last", "composite", "output",
-                  "fill", "resample_fused"]
+                  "fill", "resample_fused", "image"]
 
 
 class KernelTimes(C.Structure):
-    _fields_ = [("total_ms", C.c_double * 9), ("launches", C.c_uint64 * 9)]
+    _fields_ = [("total_ms", C.c_double * len(KERNEL_CLASSES)), ("launches", C.c_uint64 * len(KERNEL_CLASSES))]
 
 
 EXPORTS = [
-    "smr_create", "smr_destroy", "smr_register_input", "smr_unregister_input", "smr_update_scene",
+    "smr_create", "smr_destroy", "smr_register_input", "smr_unregister_input", "smr_register_image", "smr_unregister_image", "smr_update_scene",
     "smr_unregister_output", "smr_set_layouts", "smr_render", "smr_render_begin", "smr_render_end", "smr_preprocess_frame", "smr_premultiply_rgba8", "smr_render_text", "smr_debug_partition", "smr_debug_tile_plan", "smr_debug_weights", "smr_debug_sincos", "smr_debug_fused_jobs", "smr_debug_resample_stages", "smr_debug_composite_layers", "smr_debug_interior", "smr_output_plane_sizes",
-    "smr_component_default", "smr_debug_layouts", "smr_debug_set_inputs", "smr_get_stats", "smr_set_profiling", "smr_get_kernel_times",
+    "smr_component_default", "smr_debug_layouts", "smr_debug_image_nodes", "smr_debug_set_inputs", "smr_get_stats", "smr_set_profiling", "smr_get_kernel_times",
     "smr_comm_get_unique_id", "smr_comm_init", "smr_comm_broadcast_inputs", "smr_comm_exchange_inputs", "smr_comm_pull_inputs", "smr_peer_pool_alloc", "smr_peer_pool_open", "smr_peer_pool_close", "smr_peer_pool_free", "smr_comm_destroy", "smr_host_register", "smr_host_unregister", "smr_cuda_stream", "smr_last_error",
     "smr_version",
 ]
@@ -190,6 +203,8 @@ def lib():
     L.smr_destroy.restype = None
     L.smr_register_input.argtypes = [vp, C.c_char_p]
     L.smr_unregister_input.argtypes = [vp, C.c_char_p]
+    L.smr_register_image.argtypes = [vp, C.c_char_p, C.POINTER(ImageSpec)]
+    L.smr_unregister_image.argtypes = [vp, C.c_char_p]
     L.smr_update_scene.argtypes = [vp, C.c_char_p, C.c_uint32, C.c_uint32, C.c_int32, C.POINTER(Component)]
     L.smr_unregister_output.argtypes = [vp, C.c_char_p]
     for f in (L.smr_render, L.smr_render_begin):
@@ -227,6 +242,7 @@ def lib():
     L.smr_component_default.restype = None
     L.smr_debug_layouts.argtypes = [vp, C.c_char_p, C.c_uint64, C.POINTER(RenderLayout), C.c_uint32,
                                     C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]
+    L.smr_debug_image_nodes.argtypes = [vp, C.c_char_p, C.c_uint64, C.POINTER(ImageNodeInfo), C.c_uint32, C.POINTER(C.c_uint32)]
     L.smr_debug_set_inputs.argtypes = [vp, C.c_uint64, C.POINTER(InputFrame), C.c_uint32]
     L.smr_get_stats.argtypes = [vp, C.POINTER(Stats)]
     L.smr_comm_get_unique_id.argtypes = [C.POINTER(C.c_uint8 * 128)]

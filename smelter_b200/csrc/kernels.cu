@@ -1858,6 +1858,15 @@ int launch_output(const OutputJob &job, Stream s) {
 // ------------------------------------------------------------------------------------------------
 // FramePreProcessor (state/frame_pre_processor.rs): K1..K4 to RGBA8, optional rescale (rgba_rescale.wgsl, blend: None)
 // ------------------------------------------------------------------------------------------------
+// fs_main of add_premultiplied_alpha.wgsl:27-35 for one fragment: the sampled straight-alpha colour times max(alpha, 1e-5),
+// clamped, stored through the target view (sRGB in GpuOptimized, plain UNORM8 in CpuOptimized)
+__device__ __forceinline__ uchar4 premultiply_store(const Tables &T, int mode, float4 c) {
+    const float am = fmaxf(c.w, 0.00001f);
+    const float r = clamp01(c.x * am), g = clamp01(c.y * am), b = clamp01(c.z * am);
+    if (mode == 0) return make_uchar4(srgb_encode(T, r), srgb_encode(T, g), srgb_encode(T, b), unorm8(c.w));
+    return make_uchar4(unorm8(r), unorm8(g), unorm8(b), unorm8(c.w));
+}
+
 __global__ void __launch_bounds__(256) k_preprocess(Tex src, int mode, int rescale, uint8_t *out, int out_pitch, int ow, int oh) {
     __shared__ Tables T;
     load_tables(T);
@@ -1871,10 +1880,7 @@ __global__ void __launch_bounds__(256) k_preprocess(Tex src, int mode, int resca
         // samples at texel centres: weight exactly 1), colour times max(alpha, 1e-5), clamped, stored through the target view
         const uchar4 t = node_texel(T, src, x, y);
         const float *lut = mode == 0 ? T.dec : T.u8n;
-        const float a = T.u8n[t.w], am = fmaxf(a, 0.00001f);
-        const float r = clamp01(lut[t.x] * am), g = clamp01(lut[t.y] * am), b = clamp01(lut[t.z] * am);
-        if (mode == 0) o = make_uchar4(srgb_encode(T, r), srgb_encode(T, g), srgb_encode(T, b), unorm8(clamp01(a)));
-        else o = make_uchar4(unorm8(r), unorm8(g), unorm8(b), unorm8(clamp01(a)));
+        o = premultiply_store(T, mode, make_float4(lut[t.x], lut[t.y], lut[t.z], T.u8n[t.w]));
     } else {
         bool exact;
         uchar4 texel;
@@ -1901,6 +1907,16 @@ int launch_preprocess(const Tex &src, int mode, int rescale, uint8_t *out, int o
 // Every text node of a tick is one launch: block b belongs to the job whose tile range [tile_begin[i], tile_begin[i + 1])
 // holds it (a binary search by one thread), and the job is copied to shared memory.
 // ------------------------------------------------------------------------------------------------
+// The job of block b in a launch that draws several node textures: the last i with tile_begin[i] <= b
+__device__ __forceinline__ int tile_job(const int32_t *__restrict__ tile_begin, int n_jobs, int b) {
+    int lo = 0, hi = n_jobs - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (tile_begin[mid] <= b) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+}
+
 __global__ void __launch_bounds__(256) k_text(const TextJob *__restrict__ jobs, const int32_t *__restrict__ tile_begin, int n_jobs) {
     __shared__ Tables T;
     __shared__ int s_list[256];
@@ -1908,12 +1924,7 @@ __global__ void __launch_bounds__(256) k_text(const TextJob *__restrict__ jobs, 
     __shared__ TextJob J;
     const int lane = threadIdx.x, warp = threadIdx.y, tid = warp * 32 + lane;
     if (tid == 0) {
-        const int b = (int)blockIdx.x;
-        int lo = 0, hi = n_jobs - 1;   // the last job i with tile_begin[i] <= b
-        while (lo < hi) {
-            const int mid = (lo + hi + 1) >> 1;
-            if (tile_begin[mid] <= b) lo = mid; else hi = mid - 1;
-        }
+        const int b = (int)blockIdx.x, lo = tile_job(tile_begin, n_jobs, b);
         J = jobs[lo];
         const int t = b - tile_begin[lo], tiles_x = (J.width + 31) / 32;
         s_wc[0] = (t % tiles_x) * 32;   // the tile's origin, handed over through s_wc before the glyph loop reuses it
@@ -1977,6 +1988,38 @@ int launch_text(const TextJob *jobs_dev, const int32_t *tile_begin_dev, int n_jo
     if (n_jobs <= 0 || n_tiles <= 0) return 0;
     k_text<<<n_tiles, dim3(32, 8), 0, (cudaStream_t)s>>>(jobs_dev, tile_begin_dev, n_jobs);
     return check_launch("k_text") ? 1 : -1;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Image node texture (transformations/image.rs:178-187, add_premultiplied_alpha.wgsl): a full-target quad samples the
+// asset frame (straight alpha) with the linear / clamp-to-edge sampler through the mode's source view, premultiplies and
+// stores through the mode's target view.  When the node and the asset differ in size this pass is also the scaler.
+// Every image node a tick draws is one launch, block -> job as in k_text; one thread per pixel of a 32 x 8 tile.
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) k_image(const ImageJob *__restrict__ jobs, const int32_t *__restrict__ tile_begin, int n_jobs) {
+    __shared__ Tables T;
+    __shared__ ImageJob J;
+    __shared__ int s_origin[2];
+    if (threadIdx.x == 0 && threadIdx.y == 0) {
+        const int b = (int)blockIdx.x, lo = tile_job(tile_begin, n_jobs, b);
+        J = jobs[lo];
+        const int t = b - tile_begin[lo], tiles_x = (J.width + 31) / 32;
+        s_origin[0] = (t % tiles_x) * 32;
+        s_origin[1] = (t / tiles_x) * 8;
+    }
+    load_tables(T);   // ends in __syncthreads
+    const int x = s_origin[0] + (int)threadIdx.x, y = s_origin[1] + (int)threadIdx.y;
+    if (x >= J.width || y >= J.height) return;
+    bool exact;
+    uchar4 texel;
+    const float4 c = sample_node(T, &J.src, J.mode, ((float)x + 0.5f) / (float)J.width, ((float)y + 0.5f) / (float)J.height, exact, texel);
+    reinterpret_cast<uchar4 *>(J.out + (size_t)y * J.out_pitch)[x] = premultiply_store(T, J.mode, c);
+}
+
+int launch_image(const ImageJob *jobs_dev, const int32_t *tile_begin_dev, int n_jobs, int n_tiles, Stream s) {
+    if (n_jobs <= 0 || n_tiles <= 0) return 0;
+    k_image<<<n_tiles, dim3(32, 8), 0, (cudaStream_t)s>>>(jobs_dev, tile_begin_dev, n_jobs);
+    return check_launch("k_image") ? 1 : -1;
 }
 
 // ------------------------------------------------------------------------------------------------

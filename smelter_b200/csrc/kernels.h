@@ -237,6 +237,14 @@ struct TextJob {
     uint8_t *out; int32_t out_pitch;
 };
 
+// ImageNode::render (transformations/image.rs:178-187): one asset frame drawn into a node texture of the node's resolution
+struct ImageJob {
+    int32_t width, height;        // the node texture
+    int32_t mode;                 // 0 GpuOptimized (sRGB views), 1 CpuOptimized
+    Tex src;                      // the frame: TEX_RGBA8, straight alpha
+    uint8_t *out; int32_t out_pitch;
+};
+
 // host tables pushed once per device (numeric contract NC-1/3/4)
 void upload_tables(const float *u8n, const float *srgb_dec, const float *srgb_enc_thr);
 
@@ -258,10 +266,12 @@ inline int fused_source_class(int tex_kind) {
 // FramePreProcessor: node texture of `src` (rescale = 0) or its linear-filtered rescale to out_w x out_h
 int launch_preprocess(const Tex &src, int mode, int rescale, uint8_t *out, int out_pitch, int out_w, int out_h, Stream s);
 // text node textures: clear + glyph quads alpha-blended in list order, every job of jobs_dev in one launch.  Job i owns the
-// 32 x 8 tiles [tile_begin_dev[i], tile_begin_dev[i + 1]) of the grid (text_tiles of each job, prefix sums); n_tiles =
+// 32 x 8 tiles [tile_begin_dev[i], tile_begin_dev[i + 1]) of the grid (node_tiles of each job, prefix sums); n_tiles =
 // tile_begin[n_jobs]
-inline int text_tiles(int width, int height) { return ((width + 31) / 32) * ((height + 7) / 8); }
+inline int node_tiles(int width, int height) { return ((width + 31) / 32) * ((height + 7) / 8); }
 int launch_text(const TextJob *jobs_dev, const int32_t *tile_begin_dev, int n_jobs, int n_tiles, Stream s);
+// image node textures: the frame of each job sampled, premultiplied and stored; jobs and tiles as for launch_text
+int launch_image(const ImageJob *jobs_dev, const int32_t *tile_begin_dev, int n_jobs, int n_tiles, Stream s);
 // full_range: fused_launch_range of every job of the launch
 int launch_resample_fused(const FusedKernel &k, int src, int full_range, const FusedJob *jobs_dev, const FusedPiece *pieces_dev,
                           const int *piece_begin_dev, int nblocks, Stream s);

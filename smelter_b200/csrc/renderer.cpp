@@ -270,6 +270,8 @@ class Renderer {
 
     smr_status register_input(const char *id);
     smr_status unregister_input(const char *id);
+    smr_status register_image(const char *id, const smr_image_spec *spec);
+    smr_status unregister_image(const char *id);
     smr_status update_scene(const char *output_id, uint32_t w, uint32_t h, int32_t fmt, const smr_component *root);
     smr_status unregister_output(const char *id);
     smr_status set_layouts(const char *output_id, uint32_t w, uint32_t h, int32_t fmt, uint32_t root_w, uint32_t root_h,
@@ -284,6 +286,7 @@ class Renderer {
     smr_status debug_set_inputs(uint64_t pts, const smr_input_frame *in, uint32_t n_in);
     smr_status debug_layouts(const char *output_id, uint64_t pts, smr_render_layout *out, uint32_t cap, uint32_t *n,
                              uint32_t *rw, uint32_t *rh);
+    smr_status debug_image_nodes(const char *output_id, uint64_t pts, smr_image_node_info *out, uint32_t cap, uint32_t *n);
     smr_status debug_fused_jobs(smr_fused_job_info *out, uint32_t cap, uint32_t *n);
     smr_status debug_composite_layers(smr_composite_layer_info *out, uint32_t cap, uint32_t *n);
     smr_status debug_resample_stages(smr_resample_stage_info *out, uint32_t cap, uint32_t *n, int32_t *convert_kinds,
@@ -312,9 +315,20 @@ class Renderer {
         std::shared_ptr<void> mem, atlas[2];   // texture + glyphs; the mask and colour atlases (shared within the scene)
         bool rendered = false;  // drawn since the last smr_update_scene of the output (`was_rendered`)
     };
+    // An Image component of an output's scene (ImageNode, transformations/image.rs:137-187).  The node texture persists
+    // across ticks and is rewritten, in the order of stream_, by the ticks whose frame differs from the one it holds.
+    struct ImageNode {
+        Input in;               // the node texture as a layout child: premultiplied TEX_RGBA8 of the node's resolution, always live
+        ImageParams params;
+        dev::ImageJob job = {}; // draws `in.tex` from the frame job.src
+        std::shared_ptr<void> mem;
+        int held = -1;          // the frame `in.tex` holds (-1: not drawn since the last smr_update_scene of the output)
+        int held_before = -1;   // `held` when the current tick planned its draw
+    };
     struct Output {
         OutputNode node;
         std::vector<std::unique_ptr<TextNode>> texts;   // node.texts, in the same order
+        std::vector<std::unique_ptr<ImageNode>> images; // node.images, in the same order
         int32_t format = 0;
         Resolution res;
         DevBuf planes[kTicksInFlight][3];       // device staging for host outputs, one set per tick in flight: the read-back of
@@ -363,6 +377,18 @@ class Renderer {
         size_t off = param_alloc(sizeof(Dev) * recs.size());
         for (size_t i = 0; i < recs.size(); i++) memcpy(param_host_.data() + off + i * sizeof(Dev), &(recs[i].*dev), sizeof(Dev));
         return off;
+    }
+    // the jobs of the node textures one launch draws, and the prefix table of their 32 x 8 tile counts (launch_text, launch_image)
+    struct TileJobs { size_t jobs_off, begin_off; int n_tiles; };
+    template <class Node, class Job> TileJobs param_put_tile_jobs(const std::vector<Node *> &nodes, Job Node::*job) {
+        std::vector<int32_t> begin(1, 0);
+        const size_t jobs_off = param_alloc(sizeof(Job) * nodes.size());
+        for (size_t i = 0; i < nodes.size(); i++) {
+            const Job &j = nodes[i]->*job;
+            memcpy(param_host_.data() + jobs_off + i * sizeof(Job), &j, sizeof(Job));
+            begin.push_back(begin.back() + dev::node_tiles(j.width, j.height));
+        }
+        return {jobs_off, param_put(begin.data(), sizeof(int32_t) * begin.size()), begin.back()};
     }
     size_t frame_alloc(size_t bytes) {
         size_t off = (frame_used_ + 511) & ~(size_t)511;
@@ -446,17 +472,20 @@ class Renderer {
         std::vector<Fill> fills;
         std::vector<PendingCopy> d2h;
         std::vector<TextNode *> texts;        // text nodes drawn by this tick (one launch, before everything that reads them)
+        std::vector<ImageNode *> images;      // image nodes drawn by this tick (likewise)
         std::map<std::tuple<int, uint32_t, uint32_t, uint32_t, uint32_t, int, int>, int> resample_cache;
         void clear() {   // keeps the vectors' capacity
             tex.clear();
             for (auto &s : stages) s.clear();
             fused.clear(); tmaps.clear(); weight_jobs.clear(); convert_jobs.clear();
-            composites.clear(); outputs.clear(); fills.clear(); d2h.clear(); texts.clear(); resample_cache.clear();
+            composites.clear(); outputs.clear(); fills.clear(); d2h.clear(); texts.clear(); images.clear(); resample_cache.clear();
         }
     } plan_;
     using AtlasUploads = std::map<const TextAtlas *, std::shared_ptr<void>>;
     smr_status make_text_node(const std::shared_ptr<const TextPayload> &p, AtlasUploads &atlases, std::unique_ptr<TextNode> &out);
-    void plan_text_nodes(Output &o);
+    smr_status make_image_node(const ImageParams &p, std::unique_ptr<ImageNode> &out);
+    smr_status alloc_on_stream(size_t bytes, std::shared_ptr<void> &buf);
+    void plan_node_textures(Output &o, uint64_t pts);
     void plan_tiles(Output &o, CompositeRec &pc, const std::vector<dev::LayerDev> &layers, int W, int H);
     std::vector<WeightKey> new_weight_keys_;   // cache entries whose k_weights launch is not enqueued yet
     void rollback_weights();                   // a tick that fails before that launch must not leave them behind
@@ -554,7 +583,8 @@ Renderer::~Renderer() {
             cudaFree(kv.second.weights); cudaFree(kv.second.inv); cudaFree(kv.second.first);
         }
         for (auto &kv : lane_perms_) cudaFree(kv.second);
-        outputs_.clear();   // text nodes free their memory on stream_
+        outputs_.clear();   // text and image nodes and image assets free their memory on stream_
+        scene_ = SceneState();
         cudaStreamSynchronize(stream_);
         for (void *p : peer_opened_) cudaIpcCloseMemHandle(p);
         for (void *p : peer_own_) cudaFree(p);
@@ -635,6 +665,59 @@ smr_status Renderer::unregister_input(const char *id) {
     return SMR_OK;
 }
 
+// Memory allocated and released in the order of stream_: ticks submitted before the release finish reading it first
+smr_status Renderer::alloc_on_stream(size_t bytes, std::shared_ptr<void> &buf) {
+    cudaStream_t s = stream_;
+    void *d = nullptr;
+    CUDA_OK(cudaMallocAsync(&d, bytes, s));
+    buf = std::shared_ptr<void>(d, [s](void *q) { cudaFreeAsync(q, s); });
+    return SMR_OK;
+}
+
+smr_status Renderer::register_image(const char *id, const smr_image_spec *spec) {
+    if (!id || !spec || !spec->frames) return SMR_ERR_INVALID_ARGUMENT;
+    std::lock_guard<std::mutex> g(mu_);
+    auto bad = [&](const char *why) { set_error(why); return SMR_ERR_INVALID_ARGUMENT; };
+    if (spec->n_frames == 0) return bad("an image needs at least one frame");
+    if (spec->n_frames > 1000) return bad("an animated image has at most 1000 frames");
+    if (spec->width == 0 || spec->height == 0 || spec->width > 16384 || spec->height > 16384) return bad("image resolution out of range");
+    const size_t row = (size_t)spec->width * 4, frame_bytes = row * spec->height;
+    auto a = std::make_shared<ImageAsset>();
+    a->width = spec->width; a->height = spec->height;
+    uint64_t sum = 0;
+    for (uint32_t i = 0; i < spec->n_frames; i++) {
+        const smr_image_frame &f = spec->frames[i];
+        if (!f.rgba) return bad("image frame pointer is null");
+        if (f.pitch && f.pitch < row) return bad("image frame pitch smaller than a row");
+        a->frame_pts.push_back(sum);
+        if (spec->n_frames > 1 && __builtin_add_overflow(sum, f.delay_ns, &sum)) return bad("image frame delays overflow");
+    }
+    a->duration = sum ? sum : 1;
+    if (!host_only_) {
+        CUDA_OK(cudaSetDevice(opts_.cuda_device));
+        std::shared_ptr<void> px;
+        if (smr_status st = alloc_on_stream(frame_bytes * spec->n_frames, px); st != SMR_OK) return st;
+        for (uint32_t i = 0; i < spec->n_frames; i++) {
+            const smr_image_frame &f = spec->frames[i];
+            CUDA_OK(cudaMemcpy2DAsync((uint8_t *)px.get() + frame_bytes * i, row, f.rgba, f.pitch ? f.pitch : row, row, spec->height,
+                                      cudaMemcpyHostToDevice, stream_));
+        }
+        CUDA_OK(cudaStreamSynchronize(stream_));   // the caller's frames are free to change once this returns
+        stats_.h2d_bytes += frame_bytes * spec->n_frames;
+        a->pixels = std::move(px);
+    }
+    if (!scene_.register_image(id, std::move(a))) return bad("an image with this id is already registered");
+    return SMR_OK;
+}
+
+smr_status Renderer::unregister_image(const char *id) {
+    if (!id) return SMR_ERR_INVALID_ARGUMENT;
+    std::lock_guard<std::mutex> g(mu_);
+    if (!host_only_) CUDA_OK(cudaSetDevice(opts_.cuda_device));   // an asset no scene shows is released here, on stream_
+    if (!scene_.unregister_image(id)) { set_error("image not registered"); return SMR_ERR_INVALID_ARGUMENT; }
+    return SMR_OK;
+}
+
 smr_status Renderer::unregister_output(const char *id) {
     if (!id) return SMR_ERR_INVALID_ARGUMENT;
     std::lock_guard<std::mutex> g(mu_);
@@ -675,7 +758,18 @@ smr_status Renderer::update_scene(const char *output_id, uint32_t w, uint32_t h,
     for (const auto &p : payloads)
         if (smr_status st = make_text_node(p, atlases, made[p.get()]); st != SMR_OK) return st;
     OutputNode node;
-    if (!scene_.update_scene(output_id, c, {w, h}, node, err)) {
+    // image nodes have the resolution the scene state resolves; a node texture that cannot be allocated drops the update
+    std::vector<std::unique_ptr<ImageNode>> images;
+    smr_status image_st = SMR_OK;
+    auto make_images = [&](OutputNode &n) {
+        for (const ImageParams &p : n.images) {
+            images.emplace_back();
+            if ((image_st = make_image_node(p, images.back())) != SMR_OK) return false;
+        }
+        return true;
+    };
+    if (!scene_.update_scene(output_id, c, {w, h}, node, err, make_images)) {
+        if (image_st != SMR_OK) return image_st;
         set_error(err);
         return SMR_ERR_SCENE;
     }
@@ -683,6 +777,7 @@ smr_status Renderer::update_scene(const char *output_id, uint32_t w, uint32_t h,
     o.node = std::move(node);
     o.texts.clear();   // the memory of the replaced nodes is released on stream_, after the ticks that read it
     for (const auto &p : o.node.texts) o.texts.push_back(std::move(made[p.get()]));
+    o.images = std::move(images);
     o.format = fmt;
     o.res = {w, h};
     o.flat = false; o.flat_layouts.clear(); o.flat_children.clear();
@@ -708,12 +803,7 @@ smr_status Renderer::make_text_node(const std::shared_ptr<const TextPayload> &p,
     }
     if (host_only_) { out = std::move(t); return SMR_OK; }
     cudaStream_t s = stream_;
-    auto alloc = [&](size_t bytes, std::shared_ptr<void> &buf) -> smr_status {
-        void *d = nullptr;
-        CUDA_OK(cudaMallocAsync(&d, bytes, s));
-        buf = std::shared_ptr<void>(d, [s](void *q) { cudaFreeAsync(q, s); });
-        return SMR_OK;
-    };
+    auto alloc = [&](size_t bytes, std::shared_ptr<void> &buf) { return alloc_on_stream(bytes, buf); };
     const size_t tex_bytes = ((size_t)w * h * 4 + 255) & ~(size_t)255, glyph_bytes = sizeof(smr_glyph) * (size_t)J.n_glyphs;
     if (smr_status st = alloc(tex_bytes + glyph_bytes, t->mem); st != SMR_OK) return st;
     uint8_t *base = (uint8_t *)t->mem.get();
@@ -742,10 +832,43 @@ smr_status Renderer::make_text_node(const std::shared_ptr<const TextPayload> &p,
     return SMR_OK;
 }
 
-// A tick that renders output `o`: each of its text nodes enters the texture table, and those not drawn since the last
-// smr_update_scene join the tick's text launch
-void Renderer::plan_text_nodes(Output &o) {
+// An image node for `p`: its node texture, and the job that draws a frame of the asset into it
+smr_status Renderer::make_image_node(const ImageParams &p, std::unique_ptr<ImageNode> &out) {
+    auto n = std::make_unique<ImageNode>();
+    n->params = p;
+    const int w = (int)p.resolution.width, h = (int)p.resolution.height;
+    Input &in = n->in;
+    in.has_frame = true;
+    in.res = p.resolution;
+    in.tex.kind = dev::TEX_RGBA8; in.tex.width = w; in.tex.height = h; in.tex.pitch0 = w * 4;
+    dev::ImageJob &J = n->job;
+    J.width = w; J.height = h; J.mode = opts_.rendering_mode; J.out_pitch = w * 4;
+    J.src.kind = dev::TEX_RGBA8; J.src.width = (int)p.asset->width; J.src.height = (int)p.asset->height;
+    J.src.pitch0 = (int)p.asset->width * 4;
+    if (!host_only_) {
+        if (smr_status st = alloc_on_stream((size_t)w * h * 4, n->mem); st != SMR_OK) return st;
+        in.tex.p0 = J.out = (uint8_t *)n->mem.get();
+    }
+    out = std::move(n);
+    return SMR_OK;
+}
+
+// A tick that renders output `o` at `pts`: each of its text and image nodes enters the texture table.  The text nodes not
+// drawn since the last smr_update_scene join the tick's text launch; the image nodes whose frame at `pts` (a Bitmap's only
+// frame; AnimatedAsset::render's choice) is not the one their texture holds join its image launch.
+void Renderer::plan_node_textures(Output &o, uint64_t pts) {
     if (o.flat) return;
+    for (auto &n : o.images) {
+        n->in.node_tex = -1;
+        n->in.raw_tex = add_texture(n->in.tex, false);
+        const ImageAsset &a = *n->params.asset;
+        const int frame = a.animated() ? (int)a.frame_at(pts, n->params.start_pts) : 0;
+        if (frame == n->held) continue;
+        n->held_before = n->held;
+        n->held = frame;   // undone if the tick fails before its launch
+        n->job.src.p0 = (const uint8_t *)a.pixels.get() + (size_t)a.width * a.height * 4 * frame;
+        plan_.images.push_back(n.get());
+    }
     for (auto &t : o.texts) {
         t->in.node_tex = -1;
         t->in.raw_tex = add_texture(t->in.tex, false);
@@ -800,8 +923,9 @@ smr_status Renderer::set_layouts(const char *output_id, uint32_t w, uint32_t h, 
     o.format = fmt;
     o.res = {w, h};
     o.flat = true;
-    if (!o.texts.empty() && !host_only_) CUDA_OK(cudaSetDevice(opts_.cuda_device));
+    if ((!o.texts.empty() || !o.images.empty()) && !host_only_) CUDA_OK(cudaSetDevice(opts_.cuda_device));
     o.texts.clear();
+    o.images.clear();
     o.flat_root = {root_w, root_h};
     o.flat_children.clear();
     for (uint32_t i = 0; i < n_children; i++) o.flat_children.push_back(child_ids[i] ? child_ids[i] : "");
@@ -1415,7 +1539,7 @@ smr_status Renderer::render_text(uint32_t w, uint32_t h, smr_rgba bg, const smr_
     }
     // the job and its tile table, as the tick's text launch reads them from the parameter arena
     const size_t begin_off = (sizeof(dev::TextJob) + 15) & ~(size_t)15;
-    const int32_t begin[2] = {0, dev::text_tiles((int)w, (int)h)};
+    const int32_t begin[2] = {0, dev::node_tiles((int)w, (int)h)};
     CUDA_OK(text_job_.ensure(begin_off + sizeof(begin)));
     return write_rgba(rgba, pitch, mem_kind, w, h, [&](uint8_t *dst, int dpitch) {
         J.out = dst; J.out_pitch = dpitch;
@@ -1638,7 +1762,8 @@ Resolution Renderer::output_children(const Output &o, const OutputNode &node, ui
     if (o.flat)
         for (const std::string &id : o.flat_children) add(input(id));
     else
-        for (const NodeChild &ch : node.children) add(ch.text >= 0 ? &o.texts[ch.text]->in : input(ch.input_id));
+        for (const NodeChild &ch : node.children)
+            add(ch.text >= 0 ? &o.texts[ch.text]->in : ch.image >= 0 ? &o.images[ch.image]->in : input(ch.input_id));
     return o.flat ? o.flat_root : node.layout_resolution(pts);
 }
 
@@ -1779,11 +1904,13 @@ smr_status Renderer::plan_output(Output &o, smr_output_frame &of, uint64_t pts) 
         plan_.outputs.push_back({j, src_tex});
     };
 
-    plan_text_nodes(o);
-    if (!o.flat && (o.node.root_is_input || o.node.root_text >= 0)) {  // pass-through: the root texture IS the node texture
+    plan_node_textures(o, pts);
+    if (!o.flat && (o.node.root_is_input || o.node.root_text >= 0 || o.node.root_image >= 0)) {  // pass-through: the root texture IS the node texture
         Input *root_in = nullptr;
         if (o.node.root_text >= 0) {
             root_in = &o.texts[o.node.root_text]->in;
+        } else if (o.node.root_image >= 0) {
+            root_in = &o.images[o.node.root_image]->in;
         } else {
             auto it = inputs_.find(o.node.root_input_id);
             if (it != inputs_.end() && it->second.has_frame) root_in = &it->second;
@@ -1906,10 +2033,14 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
         Renderer *r; bool armed = true;
         ~WeightGuard() { if (armed) r->rollback_weights(); }
     } weight_guard{this};
-    struct TextGuard {     // any return before the text launch is enqueued leaves this tick's text nodes to the next tick
-        std::vector<TextNode *> &nodes; bool armed = true;
-        ~TextGuard() { if (armed) for (TextNode *t : nodes) t->rendered = false; }
-    } text_guard{plan_.texts};
+    struct NodeGuard {     // any return before the text and image launches are enqueued leaves this tick's nodes to the next tick
+        std::vector<TextNode *> &texts; std::vector<ImageNode *> &images; bool armed = true;
+        ~NodeGuard() {
+            if (!armed) return;
+            for (TextNode *t : texts) t->rendered = false;
+            for (ImageNode *n : images) n->held = n->held_before;
+        }
+    } node_guard{plan_.texts, plan_.images};
     smr_status st = select_inputs(pts, in, n_in, [&](Input &I, const smr_input_frame *f) {
         I.node_tex = I.raw_tex = -1;
         return f ? upload_input(I, *f) : SMR_OK;
@@ -2028,13 +2159,8 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
     }
     const size_t fj_off = param_put_all(plan_.fused, &FusedRec::job);
     const size_t cj_off = param_put_all(plan_.composites, &CompositeRec::job);   // read by k_composite_multi
-    // text jobs and the prefix table of their tile counts
-    std::vector<int32_t> text_begin(1, 0);
-    for (const TextNode *t : plan_.texts) text_begin.push_back(text_begin.back() + dev::text_tiles(t->job.width, t->job.height));
-    const size_t tj_off = param_alloc(sizeof(dev::TextJob) * plan_.texts.size());
-    for (size_t i = 0; i < plan_.texts.size(); i++)
-        memcpy(param_host_.data() + tj_off + i * sizeof(dev::TextJob), &plan_.texts[i]->job, sizeof(dev::TextJob));
-    const size_t tb_off = param_put(text_begin.data(), sizeof(int32_t) * text_begin.size());
+    const TileJobs text_jobs = param_put_tile_jobs(plan_.texts, &TextNode::job);
+    const TileJobs image_jobs = param_put_tile_jobs(plan_.images, &ImageNode::job);
     // the arena is sized: its offsets become device pointers in the packed jobs
     CUDA_OK(param_pinned_[slot_].ensure(param_used_));
     CUDA_OK(param_dev_[slot_].ensure(param_used_));
@@ -2065,11 +2191,16 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
     auto launched = [&](int n) -> bool { if (n < 0) return false; launches += (uint64_t)n; return true; };
     prof_mark(-1);
     if (!plan_.texts.empty()) {   // every text node this tick draws: materialised node textures, like k_convert's
-        if (!launched(dev::launch_text((const dev::TextJob *)(pd + tj_off), (const int32_t *)(pd + tb_off), (int)plan_.texts.size(),
-                                       text_begin.back(), stream_))) goto fail;
+        if (!launched(dev::launch_text((const dev::TextJob *)(pd + text_jobs.jobs_off), (const int32_t *)(pd + text_jobs.begin_off),
+                                       (int)plan_.texts.size(), text_jobs.n_tiles, stream_))) goto fail;
         prof_mark(SMR_KERNEL_CONVERT);
     }
-    text_guard.armed = false;
+    if (!plan_.images.empty()) {  // every image node this tick draws
+        if (!launched(dev::launch_image((const dev::ImageJob *)(pd + image_jobs.jobs_off), (const int32_t *)(pd + image_jobs.begin_off),
+                                        (int)plan_.images.size(), image_jobs.n_tiles, stream_))) goto fail;
+        prof_mark(SMR_KERNEL_IMAGE);
+    }
+    node_guard.armed = false;
     for (auto &cv : plan_.convert_jobs) {
         const dev::Tex &src = plan_.tex[cv.first].tex;
         if (!launched(dev::launch_convert_to_rgba(src, fb + cv.second, src.width * 4, stream_))) goto fail;
@@ -2519,6 +2650,23 @@ smr_status Renderer::set_profiling(int enabled) {
     return SMR_OK;
 }
 
+smr_status Renderer::debug_image_nodes(const char *output_id, uint64_t pts, smr_image_node_info *out, uint32_t cap, uint32_t *n) {
+    if (!output_id || !n) return SMR_ERR_INVALID_ARGUMENT;
+    std::lock_guard<std::mutex> g(mu_);
+    auto it = outputs_.find(output_id);
+    if (it == outputs_.end()) { set_error("output not registered"); return SMR_ERR_OUTPUT_NOT_REGISTERED; }
+    const std::vector<ImageParams> &images = it->second.node.images;
+    *n = it->second.flat ? 0 : (uint32_t)images.size();
+    if (!out) return SMR_OK;
+    if (cap < *n) return SMR_ERR_BUFFER_TOO_SMALL;
+    for (uint32_t i = 0; i < *n; i++) {
+        const ImageParams &p = images[i];
+        out[i] = {(uint32_t)p.resolution.width, (uint32_t)p.resolution.height, p.start_pts,
+                  p.asset->animated() ? (uint32_t)p.asset->frame_at(pts, p.start_pts) : 0u};
+    }
+    return SMR_OK;
+}
+
 smr_status Renderer::debug_layouts(const char *output_id, uint64_t pts, smr_render_layout *out, uint32_t cap,
                                    uint32_t *n, uint32_t *rw, uint32_t *rh) {
     if (!output_id || !n) return SMR_ERR_INVALID_ARGUMENT;
@@ -2527,7 +2675,7 @@ smr_status Renderer::debug_layouts(const char *output_id, uint64_t pts, smr_rend
     if (it == outputs_.end()) { set_error("output not registered"); return SMR_ERR_OUTPUT_NOT_REGISTERED; }
     Output &o = it->second;
     *n = 0;
-    if (!o.flat && (o.node.root_is_input || o.node.root_text >= 0)) { if (rw) *rw = 0; if (rh) *rh = 0; return SMR_OK; }
+    if (!o.flat && (o.node.root_is_input || o.node.root_text >= 0 || o.node.root_image >= 0)) { if (rw) *rw = 0; if (rh) *rh = 0; return SMR_OK; }
     OutputNode copy = o.node;  // do not advance Tiles::last_layout
     std::vector<Input *> child_in;
     std::vector<std::optional<Resolution>> child_res;
@@ -2603,6 +2751,8 @@ void smr_destroy(smr_renderer *r) { delete r; }
 
 smr_status smr_register_input(smr_renderer *r, const char *id) { SMR_GUARD(r->impl.register_input(id)) }
 smr_status smr_unregister_input(smr_renderer *r, const char *id) { SMR_GUARD(r->impl.unregister_input(id)) }
+smr_status smr_register_image(smr_renderer *r, const char *id, const smr_image_spec *spec) { SMR_GUARD(r->impl.register_image(id, spec)) }
+smr_status smr_unregister_image(smr_renderer *r, const char *id) { SMR_GUARD(r->impl.unregister_image(id)) }
 smr_status smr_update_scene(smr_renderer *r, const char *output_id, uint32_t w, uint32_t h, int32_t fmt,
                             const smr_component *root) { SMR_GUARD(r->impl.update_scene(output_id, w, h, fmt, root)) }
 smr_status smr_unregister_output(smr_renderer *r, const char *id) { SMR_GUARD(r->impl.unregister_output(id)) }
@@ -2666,6 +2816,8 @@ smr_status smr_render(smr_renderer *r, uint64_t pts, const smr_input_frame *in, 
 }
 smr_status smr_debug_layouts(smr_renderer *r, const char *output_id, uint64_t pts, smr_render_layout *out, uint32_t cap,
                              uint32_t *n, uint32_t *rw, uint32_t *rh) { SMR_GUARD(r->impl.debug_layouts(output_id, pts, out, cap, n, rw, rh)) }
+smr_status smr_debug_image_nodes(smr_renderer *r, const char *output_id, uint64_t pts, smr_image_node_info *out, uint32_t cap,
+                                 uint32_t *n) { SMR_GUARD(r->impl.debug_image_nodes(output_id, pts, out, cap, n)) }
 smr_status smr_debug_set_inputs(smr_renderer *r, uint64_t pts, const smr_input_frame *in, uint32_t n_in) { SMR_GUARD(r->impl.debug_set_inputs(pts, in, n_in)) }
 smr_status smr_debug_fused_jobs(smr_renderer *r, smr_fused_job_info *out, uint32_t cap, uint32_t *n) { SMR_GUARD(r->impl.debug_fused_jobs(out, cap, n)) }
 smr_status smr_debug_composite_layers(smr_renderer *r, smr_composite_layer_info *out, uint32_t cap, uint32_t *n) {

@@ -135,12 +135,18 @@ static bool component_from_c(const smr_component *c, Component &out, std::string
             return true;
         case SMR_COMPONENT_TEXT:
             return text_from_c(c->text, atlases, out.text, err);
+        case SMR_COMPONENT_IMAGE:
+            if (!c->image_id) { err = "component type outside the compositor hot path (Image without image_id)"; return false; }
+            out.image_id = c->image_id;
+            out.image_width = optf_from_c(c->image_width);
+            out.image_height = optf_from_c(c->image_height);
+            return true;
         case SMR_COMPONENT_VIEW:
         case SMR_COMPONENT_TILES:
         case SMR_COMPONENT_RESCALER:
             break;
         default:
-            err = "component type outside the compositor hot path (Shader/WebView/Image)";
+            err = "component type outside the compositor hot path (Shader/WebView)";
             return false;
     }
     if (c->type == SMR_COMPONENT_RESCALER && c->children_len != 1) {
@@ -444,7 +450,8 @@ static RescalerParam rescaler_at(const Stateful &c, uint64_t pts) {  // rescaler
 const std::optional<std::string> &Stateful::component_id() const {
     switch (kind) {
         case InputStream:
-        case Text: return leaf_component_id;
+        case Text:
+        case Image: return leaf_component_id;
         case View: return view_end.id;
         case Rescaler: return rescaler_end.id;
         default: return tiles.id;
@@ -504,7 +511,7 @@ void Stateful::update_state(const std::optional<Resolution> *inputs, size_t n) {
             if (off < n && inputs[off]) c.size = {(float)inputs[off]->width, (float)inputs[off]->height};
             else c.size = {0.0f, 0.0f};
             off += 1;
-        } else if (c.kind == Text) {
+        } else if (c.kind == Text || c.kind == Image) {
             off += 1;   // no state
         } else {
             size_t cnt = c.node_children_count();
@@ -1066,7 +1073,26 @@ struct BuildCtx {
     std::map<std::string, const Stateful *> prev_state;
     uint64_t last_render_pts;
     const std::map<std::string, Resolution> *input_resolutions;
+    const std::map<std::string, std::shared_ptr<const ImageAsset>> *images;
+    std::string *err;   // the first SceneError of the build
 };
+
+// `as usize` of an f32: saturating, NaN -> 0
+static size_t f32_as_usize(float v) {
+    if (!(v > 0.0f)) return 0;
+    if (v >= 1.8446744e19f) return (size_t)-1;
+    return (size_t)v;
+}
+
+// ImageComponent::stateful_component's resolution (image_component.rs:67-89), literally: the aspect ratio is a usize
+// division, so it is 1 for 640 x 360 and 0 for a portrait asset
+static Resolution image_resolution(const ImageAsset &a, const OptF &w, const OptF &h) {
+    const size_t aspect = (size_t)a.width / (size_t)a.height;
+    if (w && h) return {f32_as_usize(roundf(*w)), f32_as_usize(roundf(*h))};
+    if (w) return {f32_as_usize(roundf(*w)), f32_as_usize(roundf(*w / (float)aspect))};
+    if (h) return {f32_as_usize(roundf(*h * (float)aspect)), f32_as_usize(roundf(*h))};
+    return {a.width, a.height};
+}
 
 static void gather_components_with_id(const Stateful &c, std::map<std::string, const Stateful *> &out) {  // :259-311
     const std::optional<std::string> &id = c.component_id();
@@ -1103,6 +1129,29 @@ static Stateful build_stateful(const Component &c, const BuildCtx &ctx) {
             s.leaf_component_id = c.id;
             s.text = c.text;
             s.size = {(float)c.text->width, (float)c.text->height};
+            return s;
+        }
+        case SMR_COMPONENT_IMAGE: {  // image_component.rs:57-124
+            s.kind = Stateful::Image;
+            s.leaf_component_id = c.id;
+            s.image_id = c.image_id; s.image_width = c.image_width; s.image_height = c.image_height;
+            auto it = ctx.images->find(c.image_id);
+            if (it == ctx.images->end()) {
+                if (ctx.err->empty()) *ctx.err = "Image \"" + c.image_id + "\" is not registered";
+                return s;
+            }
+            const Stateful *prev = prev_of(Stateful::Image);
+            if (prev && prev->image_id == s.image_id && prev->image_width == s.image_width && prev->image_height == s.image_height &&
+                prev->image.asset == it->second) {
+                s.image = prev->image;
+            } else {
+                s.image = {it->second, ctx.last_render_pts, image_resolution(*it->second, c.image_width, c.image_height)};
+            }
+            const Resolution &r = s.image.resolution;
+            // the reference cannot create such a node texture
+            if ((r.width == 0 || r.width > 16384 || r.height == 0 || r.height > 16384) && ctx.err->empty())
+                *ctx.err = "Image \"" + c.image_id + "\" resolves to a node of " + std::to_string(r.width) + " x " + std::to_string(r.height);
+            s.size = {(float)r.width, (float)r.height};
             return s;
         }
         case SMR_COMPONENT_VIEW: {  // view_component.rs:103-160
@@ -1178,7 +1227,7 @@ void SceneState::unregister_output(const std::string &id) {
 }
 
 bool SceneState::update_scene(const std::string &output_id, const Component &root, Resolution resolution,
-                              OutputNode &out, std::string &err) {  // scene_state.rs:74-126
+                              OutputNode &out, std::string &err, const std::function<bool(OutputNode &)> &accept) {  // scene_state.rs:74-126
     {
         std::set<std::string> ids;
         std::string dup;
@@ -1198,9 +1247,13 @@ bool SceneState::update_scene(const std::string &output_id, const Component &roo
     if (prev != output_states_.end()) gather_components_with_id(prev->second.root, ctx.prev_state);
     ctx.last_render_pts = last_pts_ns_;
     ctx.input_resolutions = &input_resolutions_;
+    ctx.images = &images_;
+    std::string build_err;
+    ctx.err = &build_err;
 
     OutputSceneState st;
     st.root = build_stateful(root, ctx);
+    if (!build_err.empty()) { err = build_err; return false; }
     st.resolution = resolution;
 
     // intermediate_node().build_tree(Some(resolution), last_pts), :154-196
@@ -1209,6 +1262,9 @@ bool SceneState::update_scene(const std::string &output_id, const Component &roo
     if (st.root.kind == Stateful::Text) {
         out.root_text = 0;
         out.texts.push_back(st.root.text);
+    } else if (st.root.kind == Stateful::Image) {
+        out.root_image = 0;
+        out.images.push_back(st.root.image);
     } else if (!st.root.is_layout()) {
         out.root_is_input = true;
         out.root_input_id = st.root.input_id;
@@ -1222,27 +1278,43 @@ bool SceneState::update_scene(const std::string &output_id, const Component &roo
             if (l->kind == Stateful::Text) {
                 ch.text = (int)out.texts.size();
                 out.texts.push_back(l->text);
+            } else if (l->kind == Stateful::Image) {
+                ch.image = (int)out.images.size();
+                out.images.push_back(l->image);
             } else {
                 ch.input_id = l->input_id;
             }
             out.children.push_back(std::move(ch));
         }
     }
+    if (accept && !accept(out)) return false;
     output_scenes_[output_id] = root;
     output_states_[output_id] = std::move(st);
     return true;
+}
+
+bool SceneState::register_image(const std::string &image_id, std::shared_ptr<const ImageAsset> asset) {
+    return images_.emplace(image_id, std::move(asset)).second;
+}
+
+bool SceneState::unregister_image(const std::string &image_id) { return images_.erase(image_id) != 0; }
+
+size_t ImageAsset::frame_at(uint64_t pts, uint64_t start_pts) const {
+    const uint64_t animation_pts = (pts > start_pts ? pts - start_pts : 0) % duration;
+    size_t best = 0;
+    uint64_t best_d = UINT64_MAX;
+    for (size_t i = 0; i < frame_pts.size(); i++) {   // min_by_key: the first of equal keys
+        const uint64_t d = frame_pts[i] > animation_pts ? frame_pts[i] - animation_pts : animation_pts - frame_pts[i];
+        if (d < best_d) { best_d = d; best = i; }
+    }
+    return best;
 }
 
 Resolution OutputNode::layout_resolution(uint64_t pts) const {  // scene/layout.rs:245-257
     Position p = layout_root.position(pts);
     float w = p.width ? *p.width : size.width;
     float h = p.height ? *p.height : size.height;
-    auto trunc = [](float v) -> size_t {  // `as usize`: saturating, NaN -> 0
-        if (!(v > 0.0f)) return 0;
-        if (v >= 1.8446744e19f) return (size_t)-1;
-        return (size_t)v;
-    };
-    return {trunc(w), trunc(h)};
+    return {f32_as_usize(w), f32_as_usize(h)};
 }
 
 NestedLayout OutputNode::layouts(uint64_t pts, const std::vector<std::optional<Resolution>> &inputs) {

@@ -7,6 +7,7 @@
 
 #include <cstddef>
 #include <cstdint>
+#include <functional>
 #include <map>
 #include <memory>
 #include <optional>
@@ -105,6 +106,25 @@ struct TextPayload {
     int32_t color_mode = 0;
 };
 
+// A registered image (transformations/image.rs: Image::Bitmap for one frame, Image::Animated for more).  Scene nodes hold
+// it by shared_ptr, and the identity of the object is what state inheritance compares (Arc::ptr_eq).
+struct ImageAsset {
+    uint32_t width = 0, height = 0;
+    std::vector<uint64_t> frame_pts;   // AnimationFrame::pts, the sum of the delays before each frame; one entry for a Bitmap
+    uint64_t duration = 1;             // animation_duration (animated_image.rs:101-104)
+    std::shared_ptr<void> pixels;      // device memory: the frames, straight-alpha RGBA8, packed, one after the other (host-only: null)
+    bool animated() const { return frame_pts.size() > 1; }
+    // AnimatedAsset::render's frame choice (animated_image.rs:120-136); pts - start_pts saturates at 0
+    size_t frame_at(uint64_t pts, uint64_t start_pts) const;
+};
+
+// ImageRenderParams (scene/image_component.rs:10-15)
+struct ImageParams {
+    std::shared_ptr<const ImageAsset> asset;
+    uint64_t start_pts = 0;
+    Resolution resolution;
+};
+
 // scene::Component (scene.rs:50-60); only the variants on the compositor path
 struct Component {
     int type = SMR_COMPONENT_VIEW;
@@ -128,6 +148,8 @@ struct Component {
     uint32_t tile_aspect_w = 16, tile_aspect_h = 9;
     float tiles_margin = 0, tiles_padding = 0;
     std::shared_ptr<const TextPayload> text;
+    std::string image_id;                  // Image
+    OptF image_width, image_height;
 };
 
 // Converts the C tree; returns false + message for variants outside the hot path.
@@ -254,12 +276,15 @@ struct TransitionState {
 };
 
 struct Stateful {
-    enum Kind { InputStream, View, Tiles, Rescaler, Text } kind = View;
-    // InputStream (scene/input_stream_component.rs), Text (scene/text_component.rs): the leaves
+    enum Kind { InputStream, View, Tiles, Rescaler, Text, Image } kind = View;
+    // InputStream (scene/input_stream_component.rs), Text (scene/text_component.rs), Image (scene/image_component.rs): the leaves
     std::string input_id;
     std::optional<std::string> leaf_component_id;
-    Size size;                                // InputStream: its last frame's resolution; Text: the layout resolution
+    Size size;                                // InputStream: its last frame's resolution; Text: the layout resolution; Image: the node's
     std::shared_ptr<const TextPayload> text;
+    std::string image_id;                     // Image: the component (with leaf_component_id) ...
+    OptF image_width, image_height;
+    ImageParams image;                        // ... and what it resolved to
     // View
     std::optional<ViewParam> view_start;
     ViewParam view_end;
@@ -273,7 +298,7 @@ struct Stateful {
     std::optional<TransitionState> transition;
     std::vector<Stateful> children;  // Rescaler: exactly one
 
-    bool is_layout() const { return kind != InputStream && kind != Text; }
+    bool is_layout() const { return kind != InputStream && kind != Text && kind != Image; }
     const std::optional<std::string> &component_id() const;
     OptF width(uint64_t pts) const;   // scene.rs:105-117
     OptF height(uint64_t pts) const;  // scene.rs:119-131
@@ -284,10 +309,11 @@ struct Stateful {
     void update_state(const std::optional<Resolution> *inputs, size_t n);  // scene/layout.rs:105-137
 };
 
-// One child of the layout node (scene/layout.rs:95-103): an input, or text node `text` of the output
+// One child of the layout node (scene/layout.rs:95-103): an input, or text node `text` or image node `image` of the output
 struct NodeChild {
     std::string input_id;
-    int text = -1;                            // index in OutputNode::texts, or -1: the input `input_id`
+    int text = -1;                            // index in OutputNode::texts, or -1
+    int image = -1;                           // index in OutputNode::images, or -1; both -1: the input `input_id`
 };
 
 // scene/scene_state.rs
@@ -299,6 +325,8 @@ struct OutputNode {
     Size size;                                // SizedLayoutComponent.size
     std::vector<NodeChild> children;          // node children, DFS order
     std::vector<std::shared_ptr<const TextPayload>> texts;   // the output's text nodes (the root, or children in DFS order)
+    int root_image = -1;                      // the root is image node images[root_image] (-1: it is not an Image)
+    std::vector<ImageParams> images;          // the output's image nodes, likewise
     Resolution resolution;
 
     // scene::LayoutNode as LayoutProvider (scene/layout.rs:31-41, 240-261)
@@ -310,9 +338,13 @@ class SceneState {
   public:
     void register_render_event(uint64_t pts_ns, std::map<std::string, Resolution> input_resolutions);
     void unregister_output(const std::string &output_id);
-    // returns false and fills err on SceneError
+    // returns false and fills err on SceneError.  `accept` sees the new node before any state changes; when it returns
+    // false the update is dropped and the scene stays as it was.
     bool update_scene(const std::string &output_id, const Component &root, Resolution resolution,
-                      OutputNode &out, std::string &err);
+                      OutputNode &out, std::string &err, const std::function<bool(OutputNode &)> &accept = nullptr);
+    // the image registry (registry.rs:57-68): false when the id is taken / unknown
+    bool register_image(const std::string &image_id, std::shared_ptr<const ImageAsset> asset);
+    bool unregister_image(const std::string &image_id);
     uint64_t last_pts() const { return last_pts_ns_; }
 
   private:
@@ -324,6 +356,7 @@ class SceneState {
     std::map<std::string, OutputSceneState> output_states_;
     uint64_t last_pts_ns_ = 0;
     std::map<std::string, Resolution> input_resolutions_;
+    std::map<std::string, std::shared_ptr<const ImageAsset>> images_;
 };
 
 double cubic_bezier_easing(double progress, double x1, double y1, double x2, double y2);

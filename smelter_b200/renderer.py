@@ -314,7 +314,17 @@ class TextComponent:
     color_mode: int = 0
 
 
-Component = Union[InputStreamComponent, ViewComponent, RescalerComponent, TilesComponent, TextComponent]
+@dataclass
+class ImageComponent:
+    """An Image component (scene/components.rs:63-80): the asset registered as `image_id` (Renderer.register_image), shown at
+    width x height; a missing side follows from the asset's aspect ratio, both missing: the asset's size."""
+    id: Optional[str] = None
+    image_id: str = ""
+    width: Optional[float] = None
+    height: Optional[float] = None
+
+
+Component = Union[InputStreamComponent, ViewComponent, RescalerComponent, TilesComponent, TextComponent, ImageComponent]
 
 
 def _opt(v):
@@ -396,6 +406,10 @@ def _to_c(comp, keep):
                    _atlas(comp.mask_atlas, 1, keep), _atlas(comp.color_atlas, 4, keep), int(comp.color_mode))
         keep.append(t)
         c.text = C.pointer(t)
+    elif isinstance(comp, ImageComponent):
+        F.lib().smr_component_default(F.COMPONENT_IMAGE, C.byref(c))
+        c.image_id = comp.image_id.encode()
+        c.image_width, c.image_height = _opt(comp.width), _opt(comp.height)
     elif isinstance(comp, TilesComponent):
         F.lib().smr_component_default(F.COMPONENT_TILES, C.byref(c))
         _fill_transition(c, comp.transition)
@@ -406,7 +420,7 @@ def _to_c(comp, keep):
         c.horizontal_align, c.vertical_align = comp.horizontal_align, comp.vertical_align
         _children(c, comp.children, keep)
     else:
-        # Shader / WebView / Image are outside the compositor hot path: forward the tag so the
+        # Shader / WebView are outside the compositor hot path: forward the tag so the
         # library answers SMR_ERR_UNSUPPORTED like any other caller would see
         c.type = getattr(comp, "component_type", F.COMPONENT_SHADER)
     if getattr(comp, "id", None) is not None:
@@ -488,6 +502,23 @@ class Renderer:
 
     def unregister_input(self, input_id: str):
         self._check(self._lib.smr_unregister_input(self._h, input_id.encode()))
+
+    def register_image(self, image_id: str, frames, delays=None):
+        """Renderer::register_renderer for an image that arrives decoded: `frames` is one (h, w, 4) uint8 straight-alpha
+        array (a Bitmap asset) or a sequence of them, all of one size (two or more: an Animated asset, with `delays`, one
+        per frame, in nanoseconds)."""
+        if isinstance(frames, np.ndarray) and frames.ndim == 3:
+            frames = [frames]
+        frames = [np.ascontiguousarray(f, np.uint8) for f in frames]
+        delays = [0] * len(frames) if delays is None else [int(d) for d in delays]
+        assert len(delays) == len(frames) and all(f.ndim == 3 and f.shape == frames[0].shape and f.shape[2] == 4 for f in frames)
+        arr = (F.ImageFrame * max(1, len(frames)))(*[F.ImageFrame(f.ctypes.data, 0, d) for f, d in zip(frames, delays)])
+        h, w = frames[0].shape[:2] if frames else (0, 0)
+        spec = F.ImageSpec(w, h, arr, len(frames))
+        self._check(self._lib.smr_register_image(self._h, image_id.encode(), C.byref(spec)))
+
+    def unregister_image(self, image_id: str):
+        self._check(self._lib.smr_unregister_image(self._h, image_id.encode()))
 
     def unregister_output(self, output_id: str):
         self._check(self._lib.smr_unregister_output(self._h, output_id.encode()))
@@ -651,6 +682,15 @@ class Renderer:
         self._check(self._lib.smr_debug_layouts(self._h, output_id.encode(), pts_ns, arr, n.value, C.byref(n),
                                                 C.byref(rw), C.byref(rh)))
         return [arr[i] for i in range(n.value)], (rw.value, rh.value)
+
+    def debug_image_nodes(self, output_id: str, pts: float = 0.0):
+        """The image nodes of an output's scene (smr_debug_image_nodes): [((width, height), start pts in ns, the frame a
+        render at `pts` shows)], the root or the node children in DFS order."""
+        n = C.c_uint32()
+        self._check(self._lib.smr_debug_image_nodes(self._h, output_id.encode(), _secs_to_ns(pts), None, 0, C.byref(n)))
+        arr = (F.ImageNodeInfo * max(1, n.value))()
+        self._check(self._lib.smr_debug_image_nodes(self._h, output_id.encode(), _secs_to_ns(pts), arr, n.value, C.byref(n)))
+        return [((a.width, a.height), int(a.start_pts_ns), int(a.frame)) for a in arr[:n.value]]
 
     def debug_fused_jobs(self):
         """The fused resample jobs of the last planned tick (smr_debug_fused_jobs), one dict per job in plan order:
