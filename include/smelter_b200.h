@@ -60,7 +60,7 @@ typedef enum {
     SMR_COMPONENT_RESCALER = 3,
     /* declared so a shim can forward them; smr_update_scene answers SMR_ERR_UNSUPPORTED */
     SMR_COMPONENT_SHADER = 4,
-    SMR_COMPONENT_WEB_VIEW = 5,
+    SMR_COMPONENT_WEB_VIEW = 5,    /* accepted when smr_component.web_renderer_id is set, see there */
     SMR_COMPONENT_IMAGE = 6,       /* accepted when smr_component.image_id is set, see there */
     SMR_COMPONENT_TEXT = 7         /* payload in smr_component.text */
 } smr_component_type;
@@ -135,6 +135,13 @@ typedef struct smr_component {
      * SceneError::ImageNotFound: SMR_ERR_SCENE. */
     const char *image_id;
     smr_opt_f32 image_width, image_height;
+
+    /* WebView (WebViewComponent, scene/components.rs:55-61): the instance registered with smr_register_web_renderer, and
+     * in `children` the components embedded in the page, zipped in order with the instance's child rects
+     * (smr_web_set_child_rects).  A child is an InputStream, Image or Text component and has an id; a View, Tiles,
+     * Rescaler, WebView or Shader child is SMR_ERR_UNSUPPORTED (layout children inside a WebView are not supported yet).
+     * NULL web_renderer_id: SMR_ERR_UNSUPPORTED, which is what a caller built before this field existed sends. */
+    const char *web_renderer_id;
 } smr_component;
 
 /* ------------------------------------ frames (types.rs:21-119) ------------------------------- */
@@ -231,7 +238,8 @@ typedef enum {
     SMR_KERNEL_FILL = 7,           /* K6 */
     SMR_KERNEL_RESAMPLE_FUSED = 8, /* K1/K2 + both K8 passes in one kernel */
     SMR_KERNEL_IMAGE = 9,          /* image node textures (k_image) */
-    SMR_KERNEL_CLASSES = 10
+    SMR_KERNEL_WEB = 10,           /* web view node textures (k_web) */
+    SMR_KERNEL_CLASSES = 11
 } smr_kernel_class;
 typedef struct {
     double total_ms[SMR_KERNEL_CLASSES];
@@ -266,9 +274,45 @@ typedef struct { uint32_t width, height; const smr_image_frame *frames; uint32_t
 smr_status smr_register_image(smr_renderer *r, const char *image_id, const smr_image_spec *spec);
 smr_status smr_unregister_image(smr_renderer *r, const char *image_id);
 
+/* Renderer::register_renderer / unregister_renderer for RendererSpec::WebRenderer   state.rs:137-143
+ * The browser (CEF) stays with the caller, and so does the URL: the library receives what CEF's on_paint delivers (one
+ * BGRA plane of width x height, smr_web_set_frame) and the child rectangles of the GET_FRAME_POSITIONS reply
+ * (smr_web_set_child_rects), and draws the node texture on the GPU (web_renderer/renderer.rs:78-134).  Embedding:
+ * SMR_WEB_NATIVE_OVER_CONTENT draws the page, then each child over it; SMR_WEB_NATIVE_UNDER_CONTENT each child, then the
+ * page over them; SMR_WEB_CHROMIUM_EMBEDDING (the page draws the children itself, from textures read back every tick) is
+ * SMR_ERR_UNSUPPORTED.  SMR_ERR_INVALID_ARGUMENT: a NULL id or spec, a side of 0 or above 16384, an unknown embedding
+ * method, an id already registered, unregistering an unknown id.  An instance is shared by the registry and the scene that
+ * shows it: unregistering removes the registry entry only, and a scene still showing it keeps drawing its last frame. */
+typedef enum { SMR_WEB_CHROMIUM_EMBEDDING = 0, SMR_WEB_NATIVE_OVER_CONTENT = 1, SMR_WEB_NATIVE_UNDER_CONTENT = 2 } smr_web_embedding;
+typedef struct { uint32_t width, height; int32_t embedding_method; } smr_web_renderer_spec;
+smr_status smr_register_web_renderer(smr_renderer *r, const char *instance_id, const smr_web_renderer_spec *spec);
+smr_status smr_unregister_web_renderer(smr_renderer *r, const char *instance_id);
+/* The page as CEF's on_paint hands it over: BGRA8, premultiplied, exactly the instance's width x height, pitch bytes per
+ * row (0 = packed, at least 4 * width), in host or device memory (mem_kind).  The plane is copied before the call returns,
+ * on a copy stream: the call waits for that copy, not for the renders in flight, which keep drawing the frame they were
+ * submitted with.  The renders after it draw this frame until the next one arrives (renderer.rs:136-142).  Before the first frame the node
+ * texture is transparent.  SMR_ERR_INVALID_ARGUMENT: a NULL id, frame or pointer, a size other than the instance's, a pitch
+ * below 4 * width, an unknown instance. */
+typedef struct { const void *bgra; uint32_t width, height, pitch; int32_t mem_kind; } smr_web_frame;
+smr_status smr_web_set_frame(smr_renderer *r, const char *instance_id, const smr_web_frame *frame);
+/* The GET_FRAME_POSITIONS reply (browser_client.rs:28-93): child k is drawn at rects[k] (page pixels, narrowed to f32,
+ * rotation 0).  The latest list wins; children and rects are zipped, so extra children or extra rects are not drawn.
+ * n = 0 (rects may then be NULL) draws no child.  SMR_ERR_INVALID_ARGUMENT: a NULL id, NULL rects with n > 0, more than
+ * 65536 rects, an unknown instance. */
+typedef struct { double x, y, width, height; } smr_web_rect;
+smr_status smr_web_set_child_rects(smr_renderer *r, const char *instance_id, const smr_web_rect *rects, uint32_t n);
+
 /* Renderer::update_scene(output_id, resolution, output_format, scene_root)   state.rs:177-188
- * Components: InputStream, View, Tiles, Rescaler, Text and Image (anywhere, the root included); Shader and WebView answer
- * SMR_ERR_UNSUPPORTED.  A Text or Image root follows the rules of an InputStream root (an RGBA output has the node's size).
+ * Components: InputStream, View, Tiles, Rescaler, Text, Image and WebView (anywhere, the root included); Shader answers
+ * SMR_ERR_UNSUPPORTED.  A Text, Image or WebView root follows the rules of an InputStream root (an RGBA output has the
+ * node's size).
+ * WebView (scene/web_view_component.rs): its size is the instance's resolution.  SMR_ERR_SCENE, the scene staying as it
+ * was: an instance that is not registered (WebRendererNotFound), a child without an id (WebViewChildWithoutId), an
+ * instance shown by two WebViews of any outputs (WebRendererUsageNotExclusive).  The node texture is transparent when the
+ * scene is set; each render with a frame clears it and draws the planes in the embedding order, each child through its
+ * rect with the linear sampler and every plane blended with premultiplied alpha and stored as 8 bits (shader.rs:53-114).
+ * A child input without a live frame draws nothing.  Layout children (View, Tiles, Rescaler) and WebView children inside
+ * a WebView are not supported yet: each would need its own layout node texture.
  * Image (scene/image_component.rs): the node's resolution is round(image_width) x round(image_height); with one side
  * missing the other follows from the asset's aspect ratio, which the reference takes as the integer division
  * width / height (640 x 360 gives 1, a portrait asset 0); with both missing it is the asset's size.  A resolved side of 0

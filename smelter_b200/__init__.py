@@ -7,5 +7,6 @@ from .renderer import (  # noqa: F401
     BorderRadius, BoxShadow, Component, Frame, FrameData, FramePreProcessor, FrameSet, HorizontalAlign, ImageComponent, InputStreamComponent,
     InterpolationKind, NvPlanes, OutputFrameFormat, Overflow, Padding, Position, Renderer, RendererError,
     RendererOptions, RenderingMode, RenderSceneError, RescaleMode, RescalerComponent, Resolution, RGBAColor,
-    TextComponent, TilesComponent, Transition, UpdateSceneError, VerticalAlign, ViewChildrenDirection, ViewComponent, YuvPlanes,
+    TextComponent, TilesComponent, Transition, UpdateSceneError, VerticalAlign, ViewChildrenDirection, ViewComponent, WebViewComponent,
+    YuvPlanes,
 )

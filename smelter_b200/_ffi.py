@@ -17,6 +17,7 @@ COMPONENT_SHADER, COMPONENT_WEB_VIEW, COMPONENT_IMAGE, COMPONENT_TEXT = 4, 5, 6,
 FRAME_PLANAR_YUV420, FRAME_PLANAR_YUVJ420, FRAME_NV12, FRAME_BGRA, FRAME_ARGB, FRAME_RGBA8 = 0, 1, 2, 3, 4, 5
 FRAME_PLANAR_YUV422, FRAME_PLANAR_YUV444, FRAME_UYVY422, FRAME_YUYV422 = 6, 7, 8, 9
 MEM_HOST, MEM_DEVICE = 0, 1
+WEB_CHROMIUM_EMBEDDING, WEB_NATIVE_OVER_CONTENT, WEB_NATIVE_UNDER_CONTENT = 0, 1, 2
 OUT_PLANAR_YUV420, OUT_PLANAR_YUV422, OUT_PLANAR_YUV444, OUT_RGBA8, OUT_NV12 = 0, 1, 2, 3, 4
 MAX_MASKS = 20
 
@@ -77,6 +78,18 @@ class ImageSpec(C.Structure):    # smr_image_spec
     _fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("frames", C.POINTER(ImageFrame)), ("n_frames", C.c_uint32)]
 
 
+class WebRendererSpec(C.Structure):   # smr_web_renderer_spec
+    _fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("embedding_method", C.c_int32)]
+
+
+class WebFrame(C.Structure):     # smr_web_frame
+    _fields_ = [("bgra", C.c_void_p), ("width", C.c_uint32), ("height", C.c_uint32), ("pitch", C.c_uint32), ("mem_kind", C.c_int32)]
+
+
+class WebRect(C.Structure):      # smr_web_rect
+    _fields_ = [("x", C.c_double), ("y", C.c_double), ("width", C.c_double), ("height", C.c_double)]
+
+
 class ImageNodeInfo(C.Structure):   # smr_image_node_info
     _fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("start_pts_ns", C.c_uint64), ("frame", C.c_uint32)]
 
@@ -98,6 +111,7 @@ Component._fields_ = [
     ("tiles_margin", C.c_float), ("tiles_padding", C.c_float),
     ("text", C.POINTER(Text)),
     ("image_id", C.c_char_p), ("image_width", OptF32), ("image_height", OptF32),
+    ("web_renderer_id", C.c_char_p),
 ]
 
 
@@ -169,7 +183,7 @@ class CompositeLayerInfo(C.Structure):   # smr_composite_layer_info
 
 
 KERNEL_CLASSES = ["convert", "weights", "resample_box", "resample_first", "resample_last", "composite", "output",
-                  "fill", "resample_fused", "image"]
+                  "fill", "resample_fused", "image", "web"]
 
 
 class KernelTimes(C.Structure):
@@ -177,7 +191,8 @@ class KernelTimes(C.Structure):
 
 
 EXPORTS = [
-    "smr_create", "smr_destroy", "smr_register_input", "smr_unregister_input", "smr_register_image", "smr_unregister_image", "smr_update_scene",
+    "smr_create", "smr_destroy", "smr_register_input", "smr_unregister_input", "smr_register_image", "smr_unregister_image",
+    "smr_register_web_renderer", "smr_unregister_web_renderer", "smr_web_set_frame", "smr_web_set_child_rects", "smr_update_scene",
     "smr_unregister_output", "smr_set_layouts", "smr_render", "smr_render_begin", "smr_render_end", "smr_preprocess_frame", "smr_premultiply_rgba8", "smr_render_text", "smr_debug_partition", "smr_debug_tile_plan", "smr_debug_weights", "smr_debug_sincos", "smr_debug_fused_jobs", "smr_debug_resample_stages", "smr_debug_composite_layers", "smr_debug_interior", "smr_output_plane_sizes",
     "smr_component_default", "smr_debug_layouts", "smr_debug_image_nodes", "smr_debug_set_inputs", "smr_get_stats", "smr_set_profiling", "smr_get_kernel_times",
     "smr_comm_get_unique_id", "smr_comm_init", "smr_comm_broadcast_inputs", "smr_comm_exchange_inputs", "smr_comm_pull_inputs", "smr_peer_pool_alloc", "smr_peer_pool_open", "smr_peer_pool_close", "smr_peer_pool_free", "smr_comm_destroy", "smr_host_register", "smr_host_unregister", "smr_cuda_stream", "smr_last_error",
@@ -205,6 +220,10 @@ def lib():
     L.smr_unregister_input.argtypes = [vp, C.c_char_p]
     L.smr_register_image.argtypes = [vp, C.c_char_p, C.POINTER(ImageSpec)]
     L.smr_unregister_image.argtypes = [vp, C.c_char_p]
+    L.smr_register_web_renderer.argtypes = [vp, C.c_char_p, C.POINTER(WebRendererSpec)]
+    L.smr_unregister_web_renderer.argtypes = [vp, C.c_char_p]
+    L.smr_web_set_frame.argtypes = [vp, C.c_char_p, C.POINTER(WebFrame)]
+    L.smr_web_set_child_rects.argtypes = [vp, C.c_char_p, C.POINTER(WebRect), C.c_uint32]
     L.smr_update_scene.argtypes = [vp, C.c_char_p, C.c_uint32, C.c_uint32, C.c_int32, C.POINTER(Component)]
     L.smr_unregister_output.argtypes = [vp, C.c_char_p]
     for f in (L.smr_render, L.smr_render_begin):

@@ -2023,6 +2023,46 @@ int launch_image(const ImageJob *jobs_dev, const int32_t *tile_begin_dev, int n_
 }
 
 // ------------------------------------------------------------------------------------------------
+// Web view node texture (web_renderer/shader.rs:53-114, render_website.wgsl): one render pass per plane, the first one
+// clearing to transparent.  A pass leaves the pixels its quad does not cover as they are and blends the bare sample into
+// the others (PREMULTIPLIED_ALPHA_BLENDING through the target view), so each pixel walks the planes in order with its
+// value quantised to 8 bits after every plane, as the texture holds it between passes.  Every web node a tick draws is
+// one launch, block -> job as in k_text; one thread per pixel of a 32 x 8 tile.
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) k_web(const WebJob *__restrict__ jobs, const int32_t *__restrict__ tile_begin, int n_jobs) {
+    __shared__ Tables T;
+    __shared__ WebJob J;
+    __shared__ int s_origin[2];
+    if (threadIdx.x == 0 && threadIdx.y == 0) {
+        const int b = (int)blockIdx.x, lo = tile_job(tile_begin, n_jobs, b);
+        J = jobs[lo];
+        const int t = b - tile_begin[lo], tiles_x = (J.width + 31) / 32;
+        s_origin[0] = (t % tiles_x) * 32;
+        s_origin[1] = (t / tiles_x) * 8;
+    }
+    load_tables(T);   // ends in __syncthreads
+    const int x = s_origin[0] + (int)threadIdx.x, y = s_origin[1] + (int)threadIdx.y;
+    if (x >= J.width || y >= J.height) return;
+    const float pcx = (float)x + 0.5f, pcy = (float)y + 0.5f;
+    uchar4 o = make_uchar4(0, 0, 0, 0);
+    for (int i = 0; i < J.n_planes; i++) {
+        const WebPlane &P = J.planes[i];
+        if (x < P.px0 || x >= P.px1 || y < P.py0 || y >= P.py1) continue;
+        bool exact;
+        uchar4 texel;
+        const float4 s = sample_node(T, &P.tex, J.mode, (pcx - P.left) / P.width, (pcy - P.top) / P.height, exact, texel);
+        o = blend(T, J.mode, o, s);
+    }
+    reinterpret_cast<uchar4 *>(J.out + (size_t)y * J.out_pitch)[x] = o;
+}
+
+int launch_web(const WebJob *jobs_dev, const int32_t *tile_begin_dev, int n_jobs, int n_tiles, Stream s) {
+    if (n_jobs <= 0 || n_tiles <= 0) return 0;
+    k_web<<<n_tiles, dim3(32, 8), 0, (cudaStream_t)s>>>(jobs_dev, tile_begin_dev, n_jobs);
+    return check_launch("k_web") ? 1 : -1;
+}
+
+// ------------------------------------------------------------------------------------------------
 // K6: black frame (render_loop.rs:127-173)
 // ------------------------------------------------------------------------------------------------
 __global__ void k_fill(uint8_t *p0, uint8_t *p1, uint8_t *p2, int pitch0, int pitch1, int pitch2, int w, int h,

@@ -245,6 +245,24 @@ struct ImageJob {
     uint8_t *out; int32_t out_pitch;
 };
 
+// One plane of WebRendererShader::render (web_renderer/shader.rs:53-114): a quad of the plane mesh through its vertex
+// matrix, rasterised by NC-7 on the host (renderer.cpp: web_plane), and the bare linear sample of `tex` at the
+// interpolated texture coordinate (u, v) = ((x + .5 - left) / width, (y + .5 - top) / height)
+struct WebPlane {
+    Tex tex;                      // the page (TEX_BGRA: the fragment's b <-> r swap), a child's node texture, or TEX_NONE
+    int32_t px0, px1, py0, py1;   // exactly the covered pixels [px0, px1) x [py0, py1), inside the target
+    float left, top, width, height;   // the quad's corners in target pixels (width / height may be negative: mirrored)
+};
+// WebRenderer::render (web_renderer/renderer.rs:78-99) for a node with a frame: clear to transparent, then each plane in
+// order, blended with PREMULTIPLIED_ALPHA_BLENDING through the node texture's view and stored as 8 bits
+struct WebJob {
+    int32_t width, height;        // the node texture (the instance's resolution)
+    int32_t mode;                 // 0 GpuOptimized (sRGB views), 1 CpuOptimized
+    int32_t n_planes;
+    const WebPlane *planes;
+    uint8_t *out; int32_t out_pitch;
+};
+
 // host tables pushed once per device (numeric contract NC-1/3/4)
 void upload_tables(const float *u8n, const float *srgb_dec, const float *srgb_enc_thr);
 
@@ -272,6 +290,8 @@ inline int node_tiles(int width, int height) { return ((width + 31) / 32) * ((he
 int launch_text(const TextJob *jobs_dev, const int32_t *tile_begin_dev, int n_jobs, int n_tiles, Stream s);
 // image node textures: the frame of each job sampled, premultiplied and stored; jobs and tiles as for launch_text
 int launch_image(const ImageJob *jobs_dev, const int32_t *tile_begin_dev, int n_jobs, int n_tiles, Stream s);
+// web view node textures: each job's planes drawn over a transparent clear; jobs and tiles as for launch_text
+int launch_web(const WebJob *jobs_dev, const int32_t *tile_begin_dev, int n_jobs, int n_tiles, Stream s);
 // full_range: fused_launch_range of every job of the launch
 int launch_resample_fused(const FusedKernel &k, int src, int full_range, const FusedJob *jobs_dev, const FusedPiece *pieces_dev,
                           const int *piece_begin_dev, int nblocks, Stream s);

@@ -272,6 +272,10 @@ class Renderer {
     smr_status unregister_input(const char *id);
     smr_status register_image(const char *id, const smr_image_spec *spec);
     smr_status unregister_image(const char *id);
+    smr_status register_web_renderer(const char *id, const smr_web_renderer_spec *spec);
+    smr_status unregister_web_renderer(const char *id);
+    smr_status web_set_frame(const char *id, const smr_web_frame *f);
+    smr_status web_set_child_rects(const char *id, const smr_web_rect *rects, uint32_t n);
     smr_status update_scene(const char *output_id, uint32_t w, uint32_t h, int32_t fmt, const smr_component *root);
     smr_status unregister_output(const char *id);
     smr_status set_layouts(const char *output_id, uint32_t w, uint32_t h, int32_t fmt, uint32_t root_w, uint32_t root_h,
@@ -325,10 +329,21 @@ class Renderer {
         int held = -1;          // the frame `in.tex` holds (-1: not drawn since the last smr_update_scene of the output)
         int held_before = -1;   // `held` when the current tick planned its draw
     };
+    // A WebView component of an output's scene (WebRendererNode, transformations/web_renderer/node.rs).  The node texture is
+    // cleared when the node is made and redrawn, in the order of stream_, by every tick while the instance has a frame.
+    struct WebNode {
+        Input in;               // the node texture as a layout child: premultiplied TEX_RGBA8 of the instance's size, always live
+        WebParams params;
+        dev::WebJob job = {};   // draws `in.tex`; its planes are this tick's, packed into the parameter arena
+        std::vector<dev::WebPlane> planes;
+        size_t planes_off = 0;
+        std::shared_ptr<void> mem;
+    };
     struct Output {
         OutputNode node;
         std::vector<std::unique_ptr<TextNode>> texts;   // node.texts, in the same order
         std::vector<std::unique_ptr<ImageNode>> images; // node.images, in the same order
+        std::vector<std::unique_ptr<WebNode>> webs;     // node.webs, in the same order
         int32_t format = 0;
         Resolution res;
         DevBuf planes[kTicksInFlight][3];       // device staging for host outputs, one set per tick in flight: the read-back of
@@ -473,17 +488,25 @@ class Renderer {
         std::vector<PendingCopy> d2h;
         std::vector<TextNode *> texts;        // text nodes drawn by this tick (one launch, before everything that reads them)
         std::vector<ImageNode *> images;      // image nodes drawn by this tick (likewise)
+        std::vector<WebNode *> webs;          // web nodes drawn by this tick (after the text and image nodes they may read)
         std::map<std::tuple<int, uint32_t, uint32_t, uint32_t, uint32_t, int, int>, int> resample_cache;
         void clear() {   // keeps the vectors' capacity
             tex.clear();
             for (auto &s : stages) s.clear();
             fused.clear(); tmaps.clear(); weight_jobs.clear(); convert_jobs.clear();
-            composites.clear(); outputs.clear(); fills.clear(); d2h.clear(); texts.clear(); images.clear(); resample_cache.clear();
+            composites.clear(); outputs.clear(); fills.clear(); d2h.clear(); texts.clear(); images.clear(); webs.clear();
+            resample_cache.clear();
         }
     } plan_;
     using AtlasUploads = std::map<const TextAtlas *, std::shared_ptr<void>>;
     smr_status make_text_node(const std::shared_ptr<const TextPayload> &p, AtlasUploads &atlases, std::unique_ptr<TextNode> &out);
     smr_status make_image_node(const ImageParams &p, std::unique_ptr<ImageNode> &out);
+    smr_status make_web_node(const WebParams &p, std::unique_ptr<WebNode> &out);
+    void plan_web_node(Output &o, WebNode &n);
+    cudaEvent_t web_ev_ = nullptr;             // the end of a web frame's copy: later launches on stream_ wait for it
+    // Web frames: allocated on copy_stream_, released on stream_.  The pool never makes an allocation wait for a release
+    // that is still pending on stream_ (no internal dependencies), so a copy does not wait for the ticks in flight.
+    cudaMemPool_t web_pool_ = nullptr;
     smr_status alloc_on_stream(size_t bytes, std::shared_ptr<void> &buf);
     void plan_node_textures(Output &o, uint64_t pts);
     void plan_tiles(Output &o, CompositeRec &pc, const std::vector<dev::LayerDev> &layers, int W, int H);
@@ -577,15 +600,17 @@ Renderer::~Renderer() {
         if (comm_stream_) { cudaStreamSynchronize(comm_stream_); cudaStreamDestroy(comm_stream_); }
         if (comm_done_) cudaEventDestroy(comm_done_);
         if (tick_start_) cudaEventDestroy(tick_start_);
+        if (web_ev_) cudaEventDestroy(web_ev_);
         for (int i = 0; i < kTicksInFlight; i++) { if (h2d_done_[i]) cudaEventDestroy(h2d_done_[i]); if (tick_done_[i]) cudaEventDestroy(tick_done_[i]); }
         if (nccl_comm_) { g_nccl.CommDestroy(nccl_comm_); nccl_comm_ = nullptr; }
         for (auto &kv : weights_) {
             cudaFree(kv.second.weights); cudaFree(kv.second.inv); cudaFree(kv.second.first);
         }
         for (auto &kv : lane_perms_) cudaFree(kv.second);
-        outputs_.clear();   // text and image nodes and image assets free their memory on stream_
+        outputs_.clear();   // text, image and web nodes, image assets and web frames free their memory on stream_
         scene_ = SceneState();
         cudaStreamSynchronize(stream_);
+        if (web_pool_) cudaMemPoolDestroy(web_pool_);   // after the web frames it holds were released above
         for (void *p : peer_opened_) cudaIpcCloseMemHandle(p);
         for (void *p : peer_own_) cudaFree(p);
         if (barrier_word_) cudaFree(barrier_word_);
@@ -635,6 +660,18 @@ smr_status Renderer::init() {
     CUDA_OK(cudaStreamCreateWithFlags(&comm_stream_, cudaStreamNonBlocking));
     CUDA_OK(cudaEventCreateWithFlags(&comm_done_, cudaEventDisableTiming));
     CUDA_OK(cudaEventCreateWithFlags(&tick_start_, cudaEventDisableTiming));
+    CUDA_OK(cudaEventCreateWithFlags(&web_ev_, cudaEventDisableTiming));
+    {
+        cudaMemPoolProps props = {};
+        props.allocType = cudaMemAllocationTypePinned;
+        props.location.type = cudaMemLocationTypeDevice;
+        props.location.id = opts_.cuda_device;
+        CUDA_OK(cudaMemPoolCreate(&web_pool_, &props));
+        int no = 0;
+        CUDA_OK(cudaMemPoolSetAttribute(web_pool_, cudaMemPoolReuseAllowInternalDependencies, &no));
+        uint64_t keep = UINT64_MAX;   // released frames stay in the pool for the next ones
+        CUDA_OK(cudaMemPoolSetAttribute(web_pool_, cudaMemPoolAttrReleaseThreshold, &keep));
+    }
     CUDA_OK(cudaDeviceGetAttribute(&sm_count_, cudaDevAttrMultiProcessorCount, opts_.cuda_device));
     for (int i = 0; i < kTicksInFlight; i++) {
         CUDA_OK(cudaEventCreateWithFlags(&h2d_done_[i], cudaEventDisableTiming));
@@ -718,6 +755,81 @@ smr_status Renderer::unregister_image(const char *id) {
     return SMR_OK;
 }
 
+smr_status Renderer::register_web_renderer(const char *id, const smr_web_renderer_spec *spec) {
+    if (!id || !spec) return SMR_ERR_INVALID_ARGUMENT;
+    std::lock_guard<std::mutex> g(mu_);
+    auto bad = [&](const char *why) { set_error(why); return SMR_ERR_INVALID_ARGUMENT; };
+    if (spec->width == 0 || spec->height == 0 || spec->width > 16384 || spec->height > 16384) return bad("web renderer resolution out of range");
+    if (spec->embedding_method == SMR_WEB_CHROMIUM_EMBEDDING) {
+        set_error("ChromiumEmbedding reads every child back to host memory each tick; only the native embedding methods are supported");
+        return SMR_ERR_UNSUPPORTED;
+    }
+    if (spec->embedding_method != SMR_WEB_NATIVE_OVER_CONTENT && spec->embedding_method != SMR_WEB_NATIVE_UNDER_CONTENT)
+        return bad("unknown web embedding method");
+    auto w = std::make_shared<WebInstance>();
+    w->width = spec->width; w->height = spec->height; w->embedding = spec->embedding_method;
+    if (!scene_.register_web(id, std::move(w))) return bad("a web renderer with this id is already registered");
+    return SMR_OK;
+}
+
+smr_status Renderer::unregister_web_renderer(const char *id) {
+    if (!id) return SMR_ERR_INVALID_ARGUMENT;
+    std::lock_guard<std::mutex> g(mu_);
+    if (!host_only_) CUDA_OK(cudaSetDevice(opts_.cuda_device));   // a frame no scene shows is released here, on stream_
+    if (!scene_.unregister_web(id)) { set_error("web renderer not registered"); return SMR_ERR_INVALID_ARGUMENT; }
+    return SMR_OK;
+}
+
+// The page is copied once per call into a new buffer, on a copy stream: the call waits for that copy alone, not for the
+// ticks in flight, and every launch enqueued on stream_ after it waits for the copy too.  The frame it replaces is released
+// on stream_, so the ticks already submitted still read the frame they were planned with.
+smr_status Renderer::web_set_frame(const char *id, const smr_web_frame *f) {
+    if (!id || !f || !f->bgra) return SMR_ERR_INVALID_ARGUMENT;
+    std::lock_guard<std::mutex> g(mu_);
+    auto bad = [&](const char *why) { set_error(why); return SMR_ERR_INVALID_ARGUMENT; };
+    WebInstance *w = scene_.web_instance(id);
+    if (!w) return bad("web renderer not registered");
+    if (f->width != w->width || f->height != w->height) return bad("web frame size differs from the web renderer's resolution");
+    const size_t row = (size_t)w->width * 4, pitch = f->pitch ? f->pitch : row;
+    if (pitch < row) return bad("web frame pitch smaller than a row");
+    if (f->mem_kind != SMR_MEM_HOST && f->mem_kind != SMR_MEM_DEVICE) return bad("unknown mem_kind");
+    if (host_only_) return SMR_OK;
+    CUDA_OK(cudaSetDevice(opts_.cuda_device));
+    void *d = nullptr;
+    CUDA_OK(cudaMallocFromPoolAsync(&d, row * w->height, web_pool_, copy_stream_));
+    cudaError_t e = cudaMemcpy2DAsync(d, row, f->bgra, pitch, row, w->height,
+                                      f->mem_kind == SMR_MEM_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, copy_stream_);
+    if (e == cudaSuccess) e = cudaEventRecord(web_ev_, copy_stream_);
+    if (e == cudaSuccess) e = cudaStreamWaitEvent(stream_, web_ev_, 0);
+    if (e != cudaSuccess) {
+        cudaFreeAsync(d, copy_stream_);
+        set_error(std::string("web frame upload: ") + cudaGetErrorString(e));
+        return SMR_ERR_CUDA;
+    }
+    cudaStream_t rs = stream_;
+    // released on stream_, which has waited for the copy: every reader of the frame is a later launch on stream_
+    std::shared_ptr<void> buf(d, [rs](void *q) { cudaFreeAsync(q, rs); });
+    CUDA_OK(cudaEventSynchronize(web_ev_));   // the caller's plane is free to change once this returns
+    if (f->mem_kind == SMR_MEM_HOST) stats_.h2d_bytes += row * w->height;
+    w->frame = std::move(buf);
+    return SMR_OK;
+}
+
+smr_status Renderer::web_set_child_rects(const char *id, const smr_web_rect *rects, uint32_t n) {
+    if (!id || (n && !rects)) return SMR_ERR_INVALID_ARGUMENT;
+    std::lock_guard<std::mutex> g(mu_);
+    WebInstance *w = scene_.web_instance(id);
+    if (!w) { set_error("web renderer not registered"); return SMR_ERR_INVALID_ARGUMENT; }
+    if (n > 65536) { set_error("too many web child rects"); return SMR_ERR_INVALID_ARGUMENT; }
+    std::vector<float> r(4 * (size_t)n);
+    for (uint32_t i = 0; i < n; i++) {   // read_frame_position: `as f32`
+        r[4 * i] = (float)rects[i].x; r[4 * i + 1] = (float)rects[i].y;
+        r[4 * i + 2] = (float)rects[i].width; r[4 * i + 3] = (float)rects[i].height;
+    }
+    w->rects = std::move(r);
+    return SMR_OK;
+}
+
 smr_status Renderer::unregister_output(const char *id) {
     if (!id) return SMR_ERR_INVALID_ARGUMENT;
     std::lock_guard<std::mutex> g(mu_);
@@ -760,11 +872,16 @@ smr_status Renderer::update_scene(const char *output_id, uint32_t w, uint32_t h,
     OutputNode node;
     // image nodes have the resolution the scene state resolves; a node texture that cannot be allocated drops the update
     std::vector<std::unique_ptr<ImageNode>> images;
+    std::vector<std::unique_ptr<WebNode>> webs;
     smr_status image_st = SMR_OK;
     auto make_images = [&](OutputNode &n) {
         for (const ImageParams &p : n.images) {
             images.emplace_back();
             if ((image_st = make_image_node(p, images.back())) != SMR_OK) return false;
+        }
+        for (const WebParams &p : n.webs) {
+            webs.emplace_back();
+            if ((image_st = make_web_node(p, webs.back())) != SMR_OK) return false;
         }
         return true;
     };
@@ -778,6 +895,7 @@ smr_status Renderer::update_scene(const char *output_id, uint32_t w, uint32_t h,
     o.texts.clear();   // the memory of the replaced nodes is released on stream_, after the ticks that read it
     for (const auto &p : o.node.texts) o.texts.push_back(std::move(made[p.get()]));
     o.images = std::move(images);
+    o.webs = std::move(webs);
     o.format = fmt;
     o.res = {w, h};
     o.flat = false; o.flat_layouts.clear(); o.flat_children.clear();
@@ -853,11 +971,98 @@ smr_status Renderer::make_image_node(const ImageParams &p, std::unique_ptr<Image
     return SMR_OK;
 }
 
-// A tick that renders output `o` at `pts`: each of its text and image nodes enters the texture table.  The text nodes not
-// drawn since the last smr_update_scene join the tick's text launch; the image nodes whose frame at `pts` (a Bitmap's only
-// frame; AnimatedAsset::render's choice) is not the one their texture holds join its image launch.
+// A web node for `p`: its node texture, cleared to transparent (new_web_renderer_node's ensure_size), and the job that draws it
+smr_status Renderer::make_web_node(const WebParams &p, std::unique_ptr<WebNode> &out) {
+    auto n = std::make_unique<WebNode>();
+    n->params = p;
+    const int w = (int)p.instance->width, h = (int)p.instance->height;
+    Input &in = n->in;
+    in.has_frame = true;
+    in.res = {(size_t)w, (size_t)h};
+    in.tex.kind = dev::TEX_RGBA8; in.tex.width = w; in.tex.height = h; in.tex.pitch0 = w * 4;
+    dev::WebJob &J = n->job;
+    J.width = w; J.height = h; J.mode = opts_.rendering_mode; J.out_pitch = w * 4;
+    if (!host_only_) {
+        if (smr_status st = alloc_on_stream((size_t)w * h * 4, n->mem); st != SMR_OK) return st;
+        in.tex.p0 = J.out = (uint8_t *)n->mem.get();
+        CUDA_OK(cudaMemsetAsync(J.out, 0, (size_t)w * h * 4, stream_));
+    }
+    out = std::move(n);
+    return SMR_OK;
+}
+
+static inline long long snap256(float v);
+static inline long long ceil_div256(long long a);
+
+// One plane of WebRendererShader::render in a W x H target, from the entries of its vertex matrix that are not 0 or 1
+// (vertices_transformation_matrix, transformation_matrices.rs:14-68; the website's is the identity).  The plane mesh's
+// corners (+-1, +-1) map to clip x = m03 +- m00, y = m13 +- m11 (one rounding: the products by +-1 are exact) and to target
+// pixels by the viewport transform x * W/2 + W/2, y * -H/2 + H/2 (fmaf); the texture coordinate runs from 0 at the corner
+// (-1, +1) to 1 at (+1, -1).  NC-7 as in layer_geometry: corners snapped to 1/256 px, a pixel is covered when its centre
+// lies in [x0, x1) x [y0, y1).  A quad mirrored on one axis faces back and is culled (cull_mode Back, common_pipeline.rs).
+// False when the plane covers no pixel.
+static bool web_plane(float m00, float m03, float m11, float m13, int W, int H, dev::WebPlane &p) {
+    const float sx = (float)W / 2.0f, sy = (float)H / 2.0f;
+    const float X0 = std::fma(m03 - m00, sx, sx), X1 = std::fma(m03 + m00, sx, sx);
+    const float Y0 = std::fma(-(m13 + m11), sy, sy), Y1 = std::fma(-(m13 - m11), sy, sy);
+    if (!(std::isfinite(X0) && std::isfinite(X1) && std::isfinite(Y0) && std::isfinite(Y1))) return false;
+    if ((X1 < X0) != (Y1 < Y0)) return false;
+    auto snap = [](float v) { return snap256(std::fmin(std::fmax(v, -1e7f), 1e7f)); };
+    const long long x0 = snap(std::fmin(X0, X1)), x1 = snap(std::fmax(X0, X1));
+    const long long y0 = snap(std::fmin(Y0, Y1)), y1 = snap(std::fmax(Y0, Y1));
+    p.px0 = (int)std::max<long long>(ceil_div256(x0 - 128), 0); p.px1 = (int)std::min<long long>(ceil_div256(x1 - 128), W);
+    p.py0 = (int)std::max<long long>(ceil_div256(y0 - 128), 0); p.py1 = (int)std::min<long long>(ceil_div256(y1 - 128), H);
+    if (p.px0 >= p.px1 || p.py0 >= p.py1) return false;
+    p.left = X0; p.width = X1 - X0; p.top = Y0; p.height = Y1 - Y0;
+    return true;
+}
+
+// The planes a tick draws into web node `n` (WebRenderer::prepare_textures, renderer.rs:101-134), when its instance has a
+// frame: the page, and each child zipped with the latest rect list, in the instance's embedding order.  The frame pointer
+// and the rects are copied into this tick's parameters, so a later smr_web_set_frame / smr_web_set_child_rects does not
+// change what the tick reads.
+void Renderer::plan_web_node(Output &o, WebNode &n) {
+    const WebInstance &w = *n.params.instance;
+    if (!w.frame) return;   // no frame yet: the texture stays as it is (renderer.rs:89-96)
+    const int W = (int)w.width, H = (int)w.height;
+    dev::WebPlane site;
+    site.tex.kind = dev::TEX_BGRA; site.tex.width = W; site.tex.height = H; site.tex.pitch0 = W * 4;
+    site.tex.p0 = (const uint8_t *)w.frame.get();
+    const bool site_ok = web_plane(1.0f, 0.0f, 1.0f, 0.0f, W, H, site);
+    n.planes.clear();
+    if (site_ok && w.embedding == SMR_WEB_NATIVE_OVER_CONTENT) n.planes.push_back(site);
+    const size_t nc = std::min(n.params.children.size(), w.rects.size() / 4);
+    const float sx = (float)W / 2.0f, sy = (float)H / 2.0f, a = 1.0f / sx, b = 1.0f / sy;
+    for (size_t k = 0; k < nc; k++) {
+        const float *r = &w.rects[4 * k];   // left, top, width, height
+        const float tx = -((float)W / 2.0f) + (r[0] + r[2] / 2.0f), ty = (float)H / 2.0f - (r[1] + r[3] / 2.0f);
+        dev::WebPlane pl;
+        if (!web_plane(a * (sx * (r[2] / (float)W)), a * tx, b * (sy * (r[3] / (float)H)), b * ty, W, H, pl)) continue;
+        const NodeChild &ch = n.params.children[k];
+        if (ch.text >= 0) pl.tex = o.texts[ch.text]->in.tex;
+        else if (ch.image >= 0) pl.tex = o.images[ch.image]->in.tex;
+        else {   // an input without a live frame samples the empty view
+            auto it = inputs_.find(ch.input_id);
+            if (it != inputs_.end() && it->second.has_frame) pl.tex = it->second.tex;
+        }
+        n.planes.push_back(pl);
+    }
+    if (site_ok && w.embedding == SMR_WEB_NATIVE_UNDER_CONTENT) n.planes.push_back(site);
+    n.job.n_planes = (int)n.planes.size();
+    plan_.webs.push_back(&n);
+}
+
+// A tick that renders output `o` at `pts`: each of its text, image and web nodes enters the texture table.  The text nodes
+// not drawn since the last smr_update_scene join the tick's text launch; the image nodes whose frame at `pts` (a Bitmap's
+// only frame; AnimatedAsset::render's choice) is not the one their texture holds join its image launch; the web nodes whose
+// instance has a frame join its web launch.
 void Renderer::plan_node_textures(Output &o, uint64_t pts) {
     if (o.flat) return;
+    for (auto &n : o.webs) {
+        n->in.node_tex = -1;
+        n->in.raw_tex = add_texture(n->in.tex, false);
+        plan_web_node(o, *n);
+    }
     for (auto &n : o.images) {
         n->in.node_tex = -1;
         n->in.raw_tex = add_texture(n->in.tex, false);
@@ -923,9 +1128,10 @@ smr_status Renderer::set_layouts(const char *output_id, uint32_t w, uint32_t h, 
     o.format = fmt;
     o.res = {w, h};
     o.flat = true;
-    if ((!o.texts.empty() || !o.images.empty()) && !host_only_) CUDA_OK(cudaSetDevice(opts_.cuda_device));
+    if ((!o.texts.empty() || !o.images.empty() || !o.webs.empty()) && !host_only_) CUDA_OK(cudaSetDevice(opts_.cuda_device));
     o.texts.clear();
     o.images.clear();
+    o.webs.clear();
     o.flat_root = {root_w, root_h};
     o.flat_children.clear();
     for (uint32_t i = 0; i < n_children; i++) o.flat_children.push_back(child_ids[i] ? child_ids[i] : "");
@@ -1763,7 +1969,10 @@ Resolution Renderer::output_children(const Output &o, const OutputNode &node, ui
         for (const std::string &id : o.flat_children) add(input(id));
     else
         for (const NodeChild &ch : node.children)
-            add(ch.text >= 0 ? &o.texts[ch.text]->in : ch.image >= 0 ? &o.images[ch.image]->in : input(ch.input_id));
+            add(ch.text >= 0    ? &o.texts[ch.text]->in
+                : ch.image >= 0 ? &o.images[ch.image]->in
+                : ch.web >= 0   ? &o.webs[ch.web]->in
+                                : input(ch.input_id));
     return o.flat ? o.flat_root : node.layout_resolution(pts);
 }
 
@@ -1905,12 +2114,14 @@ smr_status Renderer::plan_output(Output &o, smr_output_frame &of, uint64_t pts) 
     };
 
     plan_node_textures(o, pts);
-    if (!o.flat && (o.node.root_is_input || o.node.root_text >= 0 || o.node.root_image >= 0)) {  // pass-through: the root texture IS the node texture
+    if (!o.flat && (o.node.root_is_input || o.node.root_text >= 0 || o.node.root_image >= 0 || o.node.root_web >= 0)) {  // pass-through: the root texture IS the node texture
         Input *root_in = nullptr;
         if (o.node.root_text >= 0) {
             root_in = &o.texts[o.node.root_text]->in;
         } else if (o.node.root_image >= 0) {
             root_in = &o.images[o.node.root_image]->in;
+        } else if (o.node.root_web >= 0) {
+            root_in = &o.webs[o.node.root_web]->in;
         } else {
             auto it = inputs_.find(o.node.root_input_id);
             if (it != inputs_.end() && it->second.has_frame) root_in = &it->second;
@@ -2161,11 +2372,15 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
     const size_t cj_off = param_put_all(plan_.composites, &CompositeRec::job);   // read by k_composite_multi
     const TileJobs text_jobs = param_put_tile_jobs(plan_.texts, &TextNode::job);
     const TileJobs image_jobs = param_put_tile_jobs(plan_.images, &ImageNode::job);
+    for (WebNode *n : plan_.webs) n->planes_off = param_put(n->planes.data(), sizeof(dev::WebPlane) * n->planes.size());
+    const TileJobs web_jobs = param_put_tile_jobs(plan_.webs, &WebNode::job);
     // the arena is sized: its offsets become device pointers in the packed jobs
     CUDA_OK(param_pinned_[slot_].ensure(param_used_));
     CUDA_OK(param_dev_[slot_].ensure(param_used_));
     uint8_t *pd = param_dev_[slot_].p;
     auto dev_ptr = [&](size_t off) -> uint8_t * { return off != SIZE_MAX ? pd + off : nullptr; };
+    dev::WebJob *wj = reinterpret_cast<dev::WebJob *>(param_host_.data() + web_jobs.jobs_off);
+    for (size_t i = 0; i < plan_.webs.size(); i++) wj[i].planes = (const dev::WebPlane *)(pd + plan_.webs[i]->planes_off);
     dev::FusedJob *fj = reinterpret_cast<dev::FusedJob *>(param_host_.data() + fj_off);
     for (size_t i = 0; i < plan_.fused.size(); i++) {
         const FusedRec &f = plan_.fused[i];
@@ -2199,6 +2414,11 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
         if (!launched(dev::launch_image((const dev::ImageJob *)(pd + image_jobs.jobs_off), (const int32_t *)(pd + image_jobs.begin_off),
                                         (int)plan_.images.size(), image_jobs.n_tiles, stream_))) goto fail;
         prof_mark(SMR_KERNEL_IMAGE);
+    }
+    if (!plan_.webs.empty()) {    // every web node this tick draws: after the text and image nodes its children may be
+        if (!launched(dev::launch_web((const dev::WebJob *)(pd + web_jobs.jobs_off), (const int32_t *)(pd + web_jobs.begin_off),
+                                      (int)plan_.webs.size(), web_jobs.n_tiles, stream_))) goto fail;
+        prof_mark(SMR_KERNEL_WEB);
     }
     node_guard.armed = false;
     for (auto &cv : plan_.convert_jobs) {
@@ -2675,7 +2895,11 @@ smr_status Renderer::debug_layouts(const char *output_id, uint64_t pts, smr_rend
     if (it == outputs_.end()) { set_error("output not registered"); return SMR_ERR_OUTPUT_NOT_REGISTERED; }
     Output &o = it->second;
     *n = 0;
-    if (!o.flat && (o.node.root_is_input || o.node.root_text >= 0 || o.node.root_image >= 0)) { if (rw) *rw = 0; if (rh) *rh = 0; return SMR_OK; }
+    if (!o.flat && (o.node.root_is_input || o.node.root_text >= 0 || o.node.root_image >= 0 || o.node.root_web >= 0)) {
+        if (rw) *rw = 0;
+        if (rh) *rh = 0;
+        return SMR_OK;
+    }
     OutputNode copy = o.node;  // do not advance Tiles::last_layout
     std::vector<Input *> child_in;
     std::vector<std::optional<Resolution>> child_res;
@@ -2753,6 +2977,14 @@ smr_status smr_register_input(smr_renderer *r, const char *id) { SMR_GUARD(r->im
 smr_status smr_unregister_input(smr_renderer *r, const char *id) { SMR_GUARD(r->impl.unregister_input(id)) }
 smr_status smr_register_image(smr_renderer *r, const char *id, const smr_image_spec *spec) { SMR_GUARD(r->impl.register_image(id, spec)) }
 smr_status smr_unregister_image(smr_renderer *r, const char *id) { SMR_GUARD(r->impl.unregister_image(id)) }
+smr_status smr_register_web_renderer(smr_renderer *r, const char *id, const smr_web_renderer_spec *spec) {
+    SMR_GUARD(r->impl.register_web_renderer(id, spec))
+}
+smr_status smr_unregister_web_renderer(smr_renderer *r, const char *id) { SMR_GUARD(r->impl.unregister_web_renderer(id)) }
+smr_status smr_web_set_frame(smr_renderer *r, const char *id, const smr_web_frame *frame) { SMR_GUARD(r->impl.web_set_frame(id, frame)) }
+smr_status smr_web_set_child_rects(smr_renderer *r, const char *id, const smr_web_rect *rects, uint32_t n) {
+    SMR_GUARD(r->impl.web_set_child_rects(id, rects, n))
+}
 smr_status smr_update_scene(smr_renderer *r, const char *output_id, uint32_t w, uint32_t h, int32_t fmt,
                             const smr_component *root) { SMR_GUARD(r->impl.update_scene(output_id, w, h, fmt, root)) }
 smr_status smr_unregister_output(smr_renderer *r, const char *id) { SMR_GUARD(r->impl.unregister_output(id)) }

@@ -141,12 +141,27 @@ static bool component_from_c(const smr_component *c, Component &out, std::string
             out.image_width = optf_from_c(c->image_width);
             out.image_height = optf_from_c(c->image_height);
             return true;
+        case SMR_COMPONENT_WEB_VIEW:
+            if (!c->web_renderer_id) { err = "component type outside the compositor hot path (WebView without web_renderer_id)"; return false; }
+            out.web_renderer_id = c->web_renderer_id;
+            if (c->children_len && !c->children) { err = "children pointer is null"; return false; }
+            out.children.resize(c->children_len);
+            for (uint32_t i = 0; i < c->children_len; i++) {
+                const int t = c->children[i].type;
+                if (t != SMR_COMPONENT_INPUT_STREAM && t != SMR_COMPONENT_IMAGE && t != SMR_COMPONENT_TEXT) {
+                    err = "a WebView child other than InputStream, Image or Text is outside the compositor hot path (layout and "
+                          "WebView children inside a WebView are not supported yet)";
+                    return false;
+                }
+                if (!component_from_c(&c->children[i], out.children[i], err, depth + 1, atlases)) return false;
+            }
+            return true;
         case SMR_COMPONENT_VIEW:
         case SMR_COMPONENT_TILES:
         case SMR_COMPONENT_RESCALER:
             break;
         default:
-            err = "component type outside the compositor hot path (Shader/WebView)";
+            err = "component type outside the compositor hot path (Shader)";
             return false;
     }
     if (c->type == SMR_COMPONENT_RESCALER && c->children_len != 1) {
@@ -451,7 +466,8 @@ const std::optional<std::string> &Stateful::component_id() const {
     switch (kind) {
         case InputStream:
         case Text:
-        case Image: return leaf_component_id;
+        case Image:
+        case WebView: return leaf_component_id;
         case View: return view_end.id;
         case Rescaler: return rescaler_end.id;
         default: return tiles.id;
@@ -511,8 +527,8 @@ void Stateful::update_state(const std::optional<Resolution> *inputs, size_t n) {
             if (off < n && inputs[off]) c.size = {(float)inputs[off]->width, (float)inputs[off]->height};
             else c.size = {0.0f, 0.0f};
             off += 1;
-        } else if (c.kind == Text || c.kind == Image) {
-            off += 1;   // no state
+        } else if (!c.is_layout()) {
+            off += 1;   // Text, Image, WebView: no state
         } else {
             size_t cnt = c.node_children_count();
             c.update_state(inputs + std::min(off, n), off < n ? std::min(cnt, n - off) : 0);
@@ -1074,6 +1090,7 @@ struct BuildCtx {
     uint64_t last_render_pts;
     const std::map<std::string, Resolution> *input_resolutions;
     const std::map<std::string, std::shared_ptr<const ImageAsset>> *images;
+    const std::map<std::string, std::shared_ptr<WebInstance>> *webs;
     std::string *err;   // the first SceneError of the build
 };
 
@@ -1154,6 +1171,22 @@ static Stateful build_stateful(const Component &c, const BuildCtx &ctx) {
             s.size = {(float)r.width, (float)r.height};
             return s;
         }
+        case SMR_COMPONENT_WEB_VIEW: {  // web_view_component.rs:41-71: the instance, then the children, then their ids
+            s.kind = Stateful::WebView;
+            s.leaf_component_id = c.id;
+            auto it = ctx.webs->find(c.web_renderer_id);
+            if (it == ctx.webs->end()) {
+                if (ctx.err->empty()) *ctx.err = "Web renderer \"" + c.web_renderer_id + "\" does not exist";
+                return s;
+            }
+            s.web = it->second;
+            s.size = {(float)s.web->width, (float)s.web->height};
+            for (const Component &ch : c.children) s.children.push_back(build_stateful(ch, ctx));
+            for (const Stateful &ch : s.children)
+                if (!ch.component_id() && ctx.err->empty())
+                    *ctx.err = "Web view \"" + c.web_renderer_id + "\" has a child without an id";
+            return s;
+        }
         case SMR_COMPONENT_VIEW: {  // view_component.rs:103-160
             s.kind = Stateful::View;
             const Stateful *prev = prev_of(Stateful::View);
@@ -1214,6 +1247,38 @@ static bool visit_ids(const Component &c, std::set<std::string> &ids, std::strin
         if (!visit_ids(ch, ids, dup)) return false;
     return true;
 }
+
+static bool visit_web_ids(const Component &c, std::set<std::string> &ids, std::string &dup) {  // validation.rs:74-100
+    if (c.type == SMR_COMPONENT_WEB_VIEW) {
+        if (ids.count(c.web_renderer_id)) { dup = c.web_renderer_id; return false; }
+        ids.insert(c.web_renderer_id);
+    }
+    for (const Component &ch : c.children)
+        if (!visit_web_ids(ch, ids, dup)) return false;
+    return true;
+}
+
+// A node child of the render graph (build_tree, scene_state.rs:154-196): an input, or a text, image or web node appended to
+// `out`, whose own children come first in DFS order for a web node
+static NodeChild node_child(const Stateful &l, OutputNode &out) {
+    NodeChild ch;
+    if (l.kind == Stateful::Text) {
+        ch.text = (int)out.texts.size();
+        out.texts.push_back(l.text);
+    } else if (l.kind == Stateful::Image) {
+        ch.image = (int)out.images.size();
+        out.images.push_back(l.image);
+    } else if (l.kind == Stateful::WebView) {
+        WebParams w;
+        w.instance = l.web;
+        for (const Stateful &c : l.children) w.children.push_back(node_child(c, out));
+        ch.web = (int)out.webs.size();
+        out.webs.push_back(std::move(w));
+    } else {
+        ch.input_id = l.input_id;
+    }
+    return ch;
+}
 }  // namespace
 
 void SceneState::register_render_event(uint64_t pts, std::map<std::string, Resolution> res) {
@@ -1235,6 +1300,14 @@ bool SceneState::update_scene(const std::string &output_id, const Component &roo
             err = "More than one component has an id \"" + dup + "\". Component IDs in scene definition need to be unique.";
             return false;
         }
+        ids.clear();   // one web renderer instance per WebView, across the outputs as they would be after the update
+        for (const auto &kv : output_scenes_)
+            if (kv.first != output_id && !visit_web_ids(kv.second, ids, dup)) break;
+        if (dup.empty()) visit_web_ids(root, ids, dup);
+        if (!dup.empty()) {
+            err = "Instance of web renderer \"" + dup + "\" is used more than once; one WebView per instance is allowed.";
+            return false;
+        }
     }
     // recalculate_layout on every output at last_pts (refreshes Tiles::last_layout), :87-94,198-230
     for (auto &kv : output_states_) {
@@ -1248,6 +1321,7 @@ bool SceneState::update_scene(const std::string &output_id, const Component &roo
     ctx.last_render_pts = last_pts_ns_;
     ctx.input_resolutions = &input_resolutions_;
     ctx.images = &images_;
+    ctx.webs = &webs_;
     std::string build_err;
     ctx.err = &build_err;
 
@@ -1265,6 +1339,8 @@ bool SceneState::update_scene(const std::string &output_id, const Component &roo
     } else if (st.root.kind == Stateful::Image) {
         out.root_image = 0;
         out.images.push_back(st.root.image);
+    } else if (st.root.kind == Stateful::WebView) {
+        out.root_web = node_child(st.root, out).web;
     } else if (!st.root.is_layout()) {
         out.root_is_input = true;
         out.root_input_id = st.root.input_id;
@@ -1273,19 +1349,7 @@ bool SceneState::update_scene(const std::string &output_id, const Component &roo
         out.size = {(float)resolution.width, (float)resolution.height};
         std::vector<const Stateful *> leaves;
         st.root.node_children(leaves);
-        for (const Stateful *l : leaves) {
-            NodeChild ch;
-            if (l->kind == Stateful::Text) {
-                ch.text = (int)out.texts.size();
-                out.texts.push_back(l->text);
-            } else if (l->kind == Stateful::Image) {
-                ch.image = (int)out.images.size();
-                out.images.push_back(l->image);
-            } else {
-                ch.input_id = l->input_id;
-            }
-            out.children.push_back(std::move(ch));
-        }
+        for (const Stateful *l : leaves) out.children.push_back(node_child(*l, out));
     }
     if (accept && !accept(out)) return false;
     output_scenes_[output_id] = root;
@@ -1298,6 +1362,17 @@ bool SceneState::register_image(const std::string &image_id, std::shared_ptr<con
 }
 
 bool SceneState::unregister_image(const std::string &image_id) { return images_.erase(image_id) != 0; }
+
+bool SceneState::register_web(const std::string &instance_id, std::shared_ptr<WebInstance> instance) {
+    return webs_.emplace(instance_id, std::move(instance)).second;
+}
+
+bool SceneState::unregister_web(const std::string &instance_id) { return webs_.erase(instance_id) != 0; }
+
+WebInstance *SceneState::web_instance(const std::string &instance_id) const {
+    auto it = webs_.find(instance_id);
+    return it == webs_.end() ? nullptr : it->second.get();
+}
 
 size_t ImageAsset::frame_at(uint64_t pts, uint64_t start_pts) const {
     const uint64_t animation_pts = (pts > start_pts ? pts - start_pts : 0) % duration;

@@ -125,6 +125,15 @@ struct ImageParams {
     Resolution resolution;
 };
 
+// A registered web renderer instance (transformations/web_renderer/renderer.rs: WebRenderer).  The registry and the scene
+// nodes that show it hold it by shared_ptr.  The renderer owns the latest frame and child rects; a scene only reads the size.
+struct WebInstance {
+    uint32_t width = 0, height = 0;
+    int32_t embedding = 1;                // smr_web_embedding (never SMR_WEB_CHROMIUM_EMBEDDING)
+    std::shared_ptr<void> frame;          // device memory: the latest page, BGRA8 packed (null: no frame yet)
+    std::vector<float> rects;             // the latest child rects: x, y, width, height per child, narrowed to f32
+};
+
 // scene::Component (scene.rs:50-60); only the variants on the compositor path
 struct Component {
     int type = SMR_COMPONENT_VIEW;
@@ -150,6 +159,7 @@ struct Component {
     std::shared_ptr<const TextPayload> text;
     std::string image_id;                  // Image
     OptF image_width, image_height;
+    std::string web_renderer_id;           // WebView (children: the embedded components)
 };
 
 // Converts the C tree; returns false + message for variants outside the hot path.
@@ -276,15 +286,19 @@ struct TransitionState {
 };
 
 struct Stateful {
-    enum Kind { InputStream, View, Tiles, Rescaler, Text, Image } kind = View;
-    // InputStream (scene/input_stream_component.rs), Text (scene/text_component.rs), Image (scene/image_component.rs): the leaves
+    enum Kind { InputStream, View, Tiles, Rescaler, Text, Image, WebView } kind = View;
+    // InputStream (scene/input_stream_component.rs), Text (scene/text_component.rs), Image (scene/image_component.rs),
+    // WebView (scene/web_view_component.rs): the node children of a layout
     std::string input_id;
     std::optional<std::string> leaf_component_id;
-    Size size;                                // InputStream: its last frame's resolution; Text: the layout resolution; Image: the node's
+    Size size;                                // InputStream: its last frame's resolution; Text: the layout resolution; Image: the
+                                              // node's; WebView: the instance's
     std::shared_ptr<const TextPayload> text;
     std::string image_id;                     // Image: the component (with leaf_component_id) ...
     OptF image_width, image_height;
     ImageParams image;                        // ... and what it resolved to
+    std::shared_ptr<WebInstance> web;         // WebView: the instance; `children` are its embedded components (render
+                                              // nodes of their own, never laid out)
     // View
     std::optional<ViewParam> view_start;
     ViewParam view_end;
@@ -298,7 +312,7 @@ struct Stateful {
     std::optional<TransitionState> transition;
     std::vector<Stateful> children;  // Rescaler: exactly one
 
-    bool is_layout() const { return kind != InputStream && kind != Text && kind != Image; }
+    bool is_layout() const { return kind == View || kind == Tiles || kind == Rescaler; }
     const std::optional<std::string> &component_id() const;
     OptF width(uint64_t pts) const;   // scene.rs:105-117
     OptF height(uint64_t pts) const;  // scene.rs:119-131
@@ -313,7 +327,14 @@ struct Stateful {
 struct NodeChild {
     std::string input_id;
     int text = -1;                            // index in OutputNode::texts, or -1
-    int image = -1;                           // index in OutputNode::images, or -1; both -1: the input `input_id`
+    int image = -1;                           // index in OutputNode::images, or -1
+    int web = -1;                             // index in OutputNode::webs, or -1; all -1: the input `input_id`
+};
+
+// A WebView render node (state/node.rs:127-141, NodeParams::Web): the instance and its children, each its own node
+struct WebParams {
+    std::shared_ptr<WebInstance> instance;
+    std::vector<NodeChild> children;          // input, text or image nodes (never `web`)
 };
 
 // scene/scene_state.rs
@@ -326,7 +347,9 @@ struct OutputNode {
     std::vector<NodeChild> children;          // node children, DFS order
     std::vector<std::shared_ptr<const TextPayload>> texts;   // the output's text nodes (the root, or children in DFS order)
     int root_image = -1;                      // the root is image node images[root_image] (-1: it is not an Image)
-    std::vector<ImageParams> images;          // the output's image nodes, likewise
+    std::vector<ImageParams> images;          // the output's image nodes, likewise (web view children included)
+    int root_web = -1;                        // the root is web node webs[root_web] (-1: it is not a WebView)
+    std::vector<WebParams> webs;              // the output's web nodes, likewise
     Resolution resolution;
 
     // scene::LayoutNode as LayoutProvider (scene/layout.rs:31-41, 240-261)
@@ -345,6 +368,10 @@ class SceneState {
     // the image registry (registry.rs:57-68): false when the id is taken / unknown
     bool register_image(const std::string &image_id, std::shared_ptr<const ImageAsset> asset);
     bool unregister_image(const std::string &image_id);
+    // the web renderer registry (registry.rs:57-68), likewise; web_instance: nullptr when the id is unknown
+    bool register_web(const std::string &instance_id, std::shared_ptr<WebInstance> instance);
+    bool unregister_web(const std::string &instance_id);
+    WebInstance *web_instance(const std::string &instance_id) const;
     uint64_t last_pts() const { return last_pts_ns_; }
 
   private:
@@ -357,6 +384,7 @@ class SceneState {
     uint64_t last_pts_ns_ = 0;
     std::map<std::string, Resolution> input_resolutions_;
     std::map<std::string, std::shared_ptr<const ImageAsset>> images_;
+    std::map<std::string, std::shared_ptr<WebInstance>> webs_;
 };
 
 double cubic_bezier_easing(double progress, double x1, double y1, double x2, double y2);

@@ -324,7 +324,18 @@ class ImageComponent:
     height: Optional[float] = None
 
 
-Component = Union[InputStreamComponent, ViewComponent, RescalerComponent, TilesComponent, TextComponent, ImageComponent]
+@dataclass
+class WebViewComponent:
+    """A WebView component (scene/components.rs:55-61): the web renderer instance registered as `instance_id`
+    (Renderer.register_web_renderer) at its resolution, with `children` (InputStream, Image or Text components, each with
+    an id) drawn at the instance's child rects (Renderer.set_web_child_rects)."""
+    id: Optional[str] = None
+    instance_id: str = ""
+    children: List["Component"] = field(default_factory=list)
+
+
+Component = Union[InputStreamComponent, ViewComponent, RescalerComponent, TilesComponent, TextComponent, ImageComponent,
+                  WebViewComponent]
 
 
 def _opt(v):
@@ -410,6 +421,10 @@ def _to_c(comp, keep):
         F.lib().smr_component_default(F.COMPONENT_IMAGE, C.byref(c))
         c.image_id = comp.image_id.encode()
         c.image_width, c.image_height = _opt(comp.width), _opt(comp.height)
+    elif isinstance(comp, WebViewComponent):
+        F.lib().smr_component_default(F.COMPONENT_WEB_VIEW, C.byref(c))
+        c.web_renderer_id = comp.instance_id.encode()
+        _children(c, comp.children, keep)
     elif isinstance(comp, TilesComponent):
         F.lib().smr_component_default(F.COMPONENT_TILES, C.byref(c))
         _fill_transition(c, comp.transition)
@@ -420,7 +435,7 @@ def _to_c(comp, keep):
         c.horizontal_align, c.vertical_align = comp.horizontal_align, comp.vertical_align
         _children(c, comp.children, keep)
     else:
-        # Shader / WebView are outside the compositor hot path: forward the tag so the
+        # Shader is outside the compositor hot path: forward the tag so the
         # library answers SMR_ERR_UNSUPPORTED like any other caller would see
         c.type = getattr(comp, "component_type", F.COMPONENT_SHADER)
     if getattr(comp, "id", None) is not None:
@@ -519,6 +534,32 @@ class Renderer:
 
     def unregister_image(self, image_id: str):
         self._check(self._lib.smr_unregister_image(self._h, image_id.encode()))
+
+    def register_web_renderer(self, instance_id: str, width: int, height: int, embedding_method=F.WEB_NATIVE_OVER_CONTENT):
+        """Renderer::register_renderer for RendererSpec::WebRenderer: the browser and its URL stay with the caller, which
+        hands over the painted frames (set_web_frame) and the child rects (set_web_child_rects)"""
+        spec = F.WebRendererSpec(int(width), int(height), int(embedding_method))
+        self._check(self._lib.smr_register_web_renderer(self._h, instance_id.encode(), C.byref(spec)))
+
+    def unregister_web_renderer(self, instance_id: str):
+        self._check(self._lib.smr_unregister_web_renderer(self._h, instance_id.encode()))
+
+    def set_web_frame(self, instance_id: str, bgra, mem_kind=F.MEM_HOST):
+        """the page as CEF's on_paint delivers it: an (h, w, 4) uint8 premultiplied BGRA array of the instance's size, or with
+        mem_kind MEM_DEVICE a CUDA tensor of that shape; copied before this returns"""
+        h, w = bgra.shape[:2]
+        if mem_kind == F.MEM_HOST:
+            bgra = np.ascontiguousarray(bgra, np.uint8)
+            ptr, pitch = bgra.ctypes.data, w * 4
+        else:
+            ptr, pitch = bgra.data_ptr(), bgra.stride(0)
+        frame = F.WebFrame(ptr, w, h, pitch, mem_kind)
+        self._check(self._lib.smr_web_set_frame(self._h, instance_id.encode(), C.byref(frame)))
+
+    def set_web_child_rects(self, instance_id: str, rects):
+        """the GET_FRAME_POSITIONS reply: one (x, y, width, height) per child, in page pixels"""
+        arr = (F.WebRect * max(1, len(rects)))(*[F.WebRect(*map(float, r)) for r in rects])
+        self._check(self._lib.smr_web_set_child_rects(self._h, instance_id.encode(), arr if rects else None, len(rects)))
 
     def unregister_output(self, output_id: str):
         self._check(self._lib.smr_unregister_output(self._h, output_id.encode()))
