@@ -58,8 +58,7 @@ typedef enum {
     SMR_COMPONENT_VIEW = 1,
     SMR_COMPONENT_TILES = 2,
     SMR_COMPONENT_RESCALER = 3,
-    /* declared so a shim can forward them; smr_update_scene answers SMR_ERR_UNSUPPORTED */
-    SMR_COMPONENT_SHADER = 4,
+    SMR_COMPONENT_SHADER = 4,      /* accepted when smr_component.shader_id is set, see there */
     SMR_COMPONENT_WEB_VIEW = 5,    /* accepted when smr_component.web_renderer_id is set, see there */
     SMR_COMPONENT_IMAGE = 6,       /* accepted when smr_component.image_id is set, see there */
     SMR_COMPONENT_TEXT = 7         /* payload in smr_component.text */
@@ -95,6 +94,19 @@ typedef enum { SMR_HALIGN_LEFT = 0, SMR_HALIGN_RIGHT = 1, SMR_HALIGN_JUSTIFIED =
 typedef enum { SMR_VALIGN_TOP = 0, SMR_VALIGN_CENTER = 1, SMR_VALIGN_BOTTOM = 2, SMR_VALIGN_JUSTIFIED = 3 } smr_vertical_align;
 
 struct smr_text;
+
+/* ShaderParam (scene/components.rs:40-55) and the type a shader declares for it (smr_shader_spec.param_type) */
+typedef enum {
+    SMR_SHADER_PARAM_F32 = 0, SMR_SHADER_PARAM_U32 = 1, SMR_SHADER_PARAM_I32 = 2,
+    SMR_SHADER_PARAM_LIST = 3, SMR_SHADER_PARAM_STRUCT = 4
+} smr_shader_param_kind;
+typedef struct smr_shader_param {
+    int32_t kind;                          /* smr_shader_param_kind */
+    const char *field_name;                /* a Struct's field: its name (ShaderParamStructField::field_name) */
+    float f32; uint32_t u32; int32_t i32;  /* the scalar of its kind */
+    const struct smr_shader_param *items;  /* List: the elements; Struct: the fields */
+    uint32_t items_len;
+} smr_shader_param;
 
 /* One node of the Component tree.  Fields that do not apply to `type` are ignored.
  * Use smr_component_default() to get the reference's `Default` values (components.rs:289-347). */
@@ -142,6 +154,14 @@ typedef struct smr_component {
      * Rescaler, WebView or Shader child is SMR_ERR_UNSUPPORTED (layout children inside a WebView are not supported yet).
      * NULL web_renderer_id: SMR_ERR_UNSUPPORTED, which is what a caller built before this field existed sends. */
     const char *web_renderer_id;
+
+    /* Shader (ShaderComponent, scene/components.rs:29-38): the shader registered with smr_register_shader, its parameter
+     * (NULL: None), the node's size (Size; the node texture is (size_t)shader_width x (size_t)shader_height), and in
+     * `children` its textures, in order.  NULL shader_id: SMR_ERR_UNSUPPORTED, which is what a caller built before these
+     * fields existed sends.  See smr_update_scene for the rules. */
+    const char *shader_id;
+    const smr_shader_param *shader_param;
+    float shader_width, shader_height;
 } smr_component;
 
 /* ------------------------------------ frames (types.rs:21-119) ------------------------------- */
@@ -239,7 +259,8 @@ typedef enum {
     SMR_KERNEL_RESAMPLE_FUSED = 8, /* K1/K2 + both K8 passes in one kernel */
     SMR_KERNEL_IMAGE = 9,          /* image node textures (k_image) */
     SMR_KERNEL_WEB = 10,           /* web view node textures (k_web) */
-    SMR_KERNEL_CLASSES = 11
+    SMR_KERNEL_SHADER = 11,        /* shader node textures (each shader module's smr_shader_main) */
+    SMR_KERNEL_CLASSES = 12
 } smr_kernel_class;
 typedef struct {
     double total_ms[SMR_KERNEL_CLASSES];
@@ -302,17 +323,69 @@ smr_status smr_web_set_frame(smr_renderer *r, const char *instance_id, const smr
 typedef struct { double x, y, width, height; } smr_web_rect;
 smr_status smr_web_set_child_rects(smr_renderer *r, const char *instance_id, const smr_web_rect *rects, uint32_t n);
 
+/* Renderer::register_renderer / unregister_renderer for RendererSpec::Shader   state.rs:123-166, registry.rs:57-68
+ * The reference compiles WGSL through naga and wgpu; here a shader is CUDA C++, compiled for sm_90a by NVRTC when it is
+ * registered.  `source` (NUL-terminated) defines one device function, smr_fragment, of the signature
+ *   float4 (smr_fragment_in in, const smr_base_params &base, const void *params, const smr_textures &tex)
+ * in.tex_coords runs from (0, 0) at the node texture's top-left corner to (1, 1); in.position is the pixel centre in
+ * texture pixels (x + .5, y + .5, 0, 1).  base has BaseShaderParameters' fields and values (base_params.rs): plane_id,
+ * time (the pts in seconds, Duration::as_secs_f32), output_resolution (the node's size) and texture_count.  params points
+ * at the parameter's bytes (ShaderParam::to_bytes: the scalars, little-endian, tightly concatenated; NULL without a
+ * parameter).  tex.sample(i, uv) samples child i with the reference's sampler (linear, clamp to edge) through the node
+ * texture's view: sRGB-decoded in GpuOptimized mode, raw in CpuOptimized mode, premultiplied; an index at or above
+ * texture_count samples the empty view.  The returned colour is premultiplied.  The library prepends the header that
+ * declares these types (smelter_b200/csrc/shader_rt.cuh).  Deliberate deviation: there is no user vertex stage; every
+ * plane is the full-target quad under the identity transform, as in the reference's example shaders.
+ * The source is compiled with --fmad=false and without fast math, so its arithmetic is reproducible.  NVRTC is loaded at
+ * run time (libnvrtc.so.12); when it cannot be, registration answers SMR_ERR_UNSUPPORTED with the reason in
+ * smr_last_error.  A compile error is SMR_ERR_INVALID_ARGUMENT (CreateShaderError) with NVRTC's log in smr_last_error.
+ * A host-only handle compiles too (the source is validated) but loads nothing.
+ * param_type: the parameter's type (the WGSL uniform of the reference), a tree of F32 / U32 / I32 scalars, LISTs (one
+ * item: the element type, `length` elements) and STRUCTs (items: the fields, each with its `name`); NULL: no parameter.
+ * SMR_ERR_INVALID_ARGUMENT also for a NULL id, spec or source, a malformed type, an id already registered (KeyTaken),
+ * unregistering an unknown id.  A shader is shared by the registry and the scenes that show it: unregistering removes the
+ * registry entry only, a scene still showing it keeps drawing it, and its module is unloaded after the last tick that
+ * launched it. */
+typedef struct smr_shader_param_type {
+    int32_t kind;                                  /* smr_shader_param_kind */
+    const char *name;                              /* a struct field's name (ignored elsewhere) */
+    const struct smr_shader_param_type *items;     /* LIST: exactly one, the element type; STRUCT: the fields */
+    uint32_t items_len;
+    uint32_t length;                               /* LIST: the element count (at least 1) */
+} smr_shader_param_type;
+typedef struct { const char *source; const smr_shader_param_type *param_type; } smr_shader_spec;
+smr_status smr_register_shader(smr_renderer *r, const char *shader_id, const smr_shader_spec *spec);
+smr_status smr_unregister_shader(smr_renderer *r, const char *shader_id);
+
 /* Renderer::update_scene(output_id, resolution, output_format, scene_root)   state.rs:177-188
- * Components: InputStream, View, Tiles, Rescaler, Text, Image and WebView (anywhere, the root included); Shader answers
- * SMR_ERR_UNSUPPORTED.  A Text, Image or WebView root follows the rules of an InputStream root (an RGBA output has the
- * node's size).
+ * Components: InputStream, View, Tiles, Rescaler, Text, Image, WebView and Shader (anywhere, the root included).  A
+ * Text, Image, WebView or Shader root follows the rules of an InputStream root (an RGBA output has the node's size).
+ * Shader (scene/shader_component.rs, transformations/shader/node.rs): SMR_ERR_SCENE, the scene staying as it was: a shader
+ * that is not registered (ShaderNotFound), a parameter that does not match the shader's type
+ * (ShaderNodeParametersValidationError, validation.rs:314-520: the same kind; a list no longer than the type's length,
+ * each element matching; a struct with the same number of fields, the same names in order, each value matching; a
+ * parameter for a shader without a parameter type is NoBindingInShader), a node size that resolves to 0 or above 16384,
+ * a View, Tiles or Rescaler child without width and height (UnknownDimensionsForLayoutNodeRoot, scene_state.rs:198-228).
+ * Its children are render nodes of their own: InputStream, Image, Text, WebView, Shader, View, Tiles or Rescaler
+ * components.  A View, Tiles or Rescaler child is a layout node of its own (scene_state.rs:154-196): its size is its width
+ * and height at the last render's pts, its resolution at each render SizedLayoutComponent::resolution, and its layout
+ * state (transitions, Tiles' last layout) carries over scene updates as the root's does; every render evaluates its
+ * layouts and composites them into a texture of that resolution, which the shader samples (a resolution of 0 or above
+ * 16384 samples the empty view).  More than 16 children is SMR_ERR_UNSUPPORTED (the reference fails in wgpu validation,
+ * SHADER_INPUT_TEXTURES_AMOUNT).  Every render
+ * clears the node texture and draws max(1, texture_count) planes (plane_id -1 without children), each pixel's
+ * smr_fragment blended with premultiplied alpha and stored as 8 bits (pipeline.rs:81-140).  A child input without a live
+ * frame samples the empty view.  A tick draws the nodes below the roots in order of depth (1 + the deepest child's; an
+ * input, text or image 0, a web node 1): per depth the resample passes and one composite launch for its layout nodes, then
+ * one launch per shader for its shader nodes; the roots' composite comes last.
  * WebView (scene/web_view_component.rs): its size is the instance's resolution.  SMR_ERR_SCENE, the scene staying as it
  * was: an instance that is not registered (WebRendererNotFound), a child without an id (WebViewChildWithoutId), an
  * instance shown by two WebViews of any outputs (WebRendererUsageNotExclusive).  The node texture is transparent when the
  * scene is set; each render with a frame clears it and draws the planes in the embedding order, each child through its
  * rect with the linear sampler and every plane blended with premultiplied alpha and stored as 8 bits (shader.rs:53-114).
  * A child input without a live frame draws nothing.  Layout children (View, Tiles, Rescaler) and WebView children inside
- * a WebView are not supported yet: each would need its own layout node texture.
+ * a WebView are not supported yet: each would need its own layout node texture.  A Shader inside a WebView is
+ * SMR_ERR_UNSUPPORTED too.
  * Image (scene/image_component.rs): the node's resolution is round(image_width) x round(image_height); with one side
  * missing the other follows from the asset's aspect ratio, which the reference takes as the integer division
  * width / height (640 x 360 gives 1, a portrait asset 0); with both missing it is the asset's size.  A resolved side of 0
@@ -521,6 +594,12 @@ void smr_component_default(int32_t type, smr_component *out);
 smr_status smr_debug_layouts(smr_renderer *r, const char *output_id, uint64_t pts_ns,
                              smr_render_layout *out, uint32_t capacity, uint32_t *n_out,
                              uint32_t *root_width, uint32_t *root_height);
+/* inspection (no device needed): the same for any layout node of an output's render graph.  node 0 is the root when the
+ * root is a layout; the layout nodes below it (a View, Tiles or Rescaler child of a Shader) follow in DFS order, children
+ * before parents.  root_width x root_height is the node's resolution at pts.  SMR_ERR_INVALID_ARGUMENT: no such node. */
+smr_status smr_debug_node_layouts(smr_renderer *r, const char *output_id, uint32_t node, uint64_t pts_ns,
+                                  smr_render_layout *out, uint32_t capacity, uint32_t *n_out,
+                                  uint32_t *root_width, uint32_t *root_height);
 /* inspection (no device needed): the image nodes of an output's scene, the root or the node children in DFS order: the
  * node's resolution, its start pts, and the asset frame a render at pts_ns shows.  SMR_ERR_BUFFER_TOO_SMALL when they do
  * not fit in capacity (out = NULL asks for the count). */

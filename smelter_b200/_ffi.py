@@ -94,6 +94,29 @@ class ImageNodeInfo(C.Structure):   # smr_image_node_info
     _fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("start_pts_ns", C.c_uint64), ("frame", C.c_uint32)]
 
 
+SHADER_PARAM_F32, SHADER_PARAM_U32, SHADER_PARAM_I32, SHADER_PARAM_LIST, SHADER_PARAM_STRUCT = 0, 1, 2, 3, 4
+
+
+class ShaderParam(C.Structure):   # smr_shader_param
+    pass
+
+
+ShaderParam._fields_ = [("kind", C.c_int32), ("field_name", C.c_char_p), ("f32", C.c_float), ("u32", C.c_uint32),
+                        ("i32", C.c_int32), ("items", C.POINTER(ShaderParam)), ("items_len", C.c_uint32)]
+
+
+class ShaderParamType(C.Structure):   # smr_shader_param_type
+    pass
+
+
+ShaderParamType._fields_ = [("kind", C.c_int32), ("name", C.c_char_p), ("items", C.POINTER(ShaderParamType)),
+                            ("items_len", C.c_uint32), ("length", C.c_uint32)]
+
+
+class ShaderSpec(C.Structure):    # smr_shader_spec
+    _fields_ = [("source", C.c_char_p), ("param_type", C.POINTER(ShaderParamType))]
+
+
 class Component(C.Structure):
     pass
 
@@ -112,6 +135,7 @@ Component._fields_ = [
     ("text", C.POINTER(Text)),
     ("image_id", C.c_char_p), ("image_width", OptF32), ("image_height", OptF32),
     ("web_renderer_id", C.c_char_p),
+    ("shader_id", C.c_char_p), ("shader_param", C.POINTER(ShaderParam)), ("shader_width", C.c_float), ("shader_height", C.c_float),
 ]
 
 
@@ -183,7 +207,7 @@ class CompositeLayerInfo(C.Structure):   # smr_composite_layer_info
 
 
 KERNEL_CLASSES = ["convert", "weights", "resample_box", "resample_first", "resample_last", "composite", "output",
-                  "fill", "resample_fused", "image", "web"]
+                  "fill", "resample_fused", "image", "web", "shader"]
 
 
 class KernelTimes(C.Structure):
@@ -192,9 +216,9 @@ class KernelTimes(C.Structure):
 
 EXPORTS = [
     "smr_create", "smr_destroy", "smr_register_input", "smr_unregister_input", "smr_register_image", "smr_unregister_image",
-    "smr_register_web_renderer", "smr_unregister_web_renderer", "smr_web_set_frame", "smr_web_set_child_rects", "smr_update_scene",
+    "smr_register_web_renderer", "smr_unregister_web_renderer", "smr_web_set_frame", "smr_web_set_child_rects", "smr_register_shader", "smr_unregister_shader", "smr_update_scene",
     "smr_unregister_output", "smr_set_layouts", "smr_render", "smr_render_begin", "smr_render_end", "smr_preprocess_frame", "smr_premultiply_rgba8", "smr_render_text", "smr_debug_partition", "smr_debug_tile_plan", "smr_debug_weights", "smr_debug_sincos", "smr_debug_fused_jobs", "smr_debug_resample_stages", "smr_debug_composite_layers", "smr_debug_interior", "smr_output_plane_sizes",
-    "smr_component_default", "smr_debug_layouts", "smr_debug_image_nodes", "smr_debug_set_inputs", "smr_get_stats", "smr_set_profiling", "smr_get_kernel_times",
+    "smr_component_default", "smr_debug_layouts", "smr_debug_node_layouts", "smr_debug_image_nodes", "smr_debug_set_inputs", "smr_get_stats", "smr_set_profiling", "smr_get_kernel_times",
     "smr_comm_get_unique_id", "smr_comm_init", "smr_comm_broadcast_inputs", "smr_comm_exchange_inputs", "smr_comm_pull_inputs", "smr_peer_pool_alloc", "smr_peer_pool_open", "smr_peer_pool_close", "smr_peer_pool_free", "smr_comm_destroy", "smr_host_register", "smr_host_unregister", "smr_cuda_stream", "smr_last_error",
     "smr_version",
 ]
@@ -224,6 +248,8 @@ def lib():
     L.smr_unregister_web_renderer.argtypes = [vp, C.c_char_p]
     L.smr_web_set_frame.argtypes = [vp, C.c_char_p, C.POINTER(WebFrame)]
     L.smr_web_set_child_rects.argtypes = [vp, C.c_char_p, C.POINTER(WebRect), C.c_uint32]
+    L.smr_register_shader.argtypes = [vp, C.c_char_p, C.POINTER(ShaderSpec)]
+    L.smr_unregister_shader.argtypes = [vp, C.c_char_p]
     L.smr_update_scene.argtypes = [vp, C.c_char_p, C.c_uint32, C.c_uint32, C.c_int32, C.POINTER(Component)]
     L.smr_unregister_output.argtypes = [vp, C.c_char_p]
     for f in (L.smr_render, L.smr_render_begin):
@@ -261,6 +287,8 @@ def lib():
     L.smr_component_default.restype = None
     L.smr_debug_layouts.argtypes = [vp, C.c_char_p, C.c_uint64, C.POINTER(RenderLayout), C.c_uint32,
                                     C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]
+    L.smr_debug_node_layouts.argtypes = [vp, C.c_char_p, C.c_uint32, C.c_uint64, C.POINTER(RenderLayout), C.c_uint32,
+                                         C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]
     L.smr_debug_image_nodes.argtypes = [vp, C.c_char_p, C.c_uint64, C.POINTER(ImageNodeInfo), C.c_uint32, C.POINTER(C.c_uint32)]
     L.smr_debug_set_inputs.argtypes = [vp, C.c_uint64, C.POINTER(InputFrame), C.c_uint32]
     L.smr_get_stats.argtypes = [vp, C.POINTER(Stats)]

@@ -10,7 +10,10 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libsmelter_b200.so")
 SOURCES = ["kernels.cu", "renderer.cpp", "scene.cpp"]
-HEADERS = ["kernels.h", "interior.h", "int_weights.h", "scene.h", "ptx_helpers.cuh", "resample_tma.cuh", "resample_tma3.cuh", "resample_tma0.cuh", os.path.join("..", "..", "include", "smelter_b200.h")]
+# the sources a shader module is compiled from at registration (renderer.cpp, NVRTC), embedded as string literals
+EMBEDDED = ["kernels.h", "node_sample.cuh", "shader_rt.cuh"]
+EMBEDDED_INC = os.path.join(CSRC, "shader_sources.inc")   # generated, kept out of git
+HEADERS = ["node_sample.cuh", "shader_rt.cuh", "kernels.h", "interior.h", "int_weights.h", "scene.h", "ptx_helpers.cuh", "resample_tma.cuh", "resample_tma3.cuh", "resample_tma0.cuh", os.path.join("..", "..", "include", "smelter_b200.h")]
 
 NVCC_FLAGS = [
     "-std=c++17", "-O3",
@@ -32,9 +35,24 @@ def needs_build():
     return any(os.path.getmtime(d) > t for d in deps)
 
 
+def write_embedded():
+    """shader_sources.inc: one raw string literal per EMBEDDED file, named kSrc_<file stem>"""
+    out = []
+    for name in EMBEDDED:
+        with open(os.path.join(CSRC, name)) as f:
+            text = f.read()
+        assert ')SMRSRC"' not in text
+        out.append(f'static const char kSrc_{name.split(".")[0]}[] = R"SMRSRC({text})SMRSRC";\n')
+    text = "".join(out)
+    if not os.path.exists(EMBEDDED_INC) or open(EMBEDDED_INC).read() != text:
+        with open(EMBEDDED_INC, "w") as f:
+            f.write(text)
+
+
 def build(force=False, verbose=False, extra=()):
     if not force and not needs_build():
         return LIB
+    write_embedded()
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
     cmd = [nvcc] + NVCC_FLAGS + list(extra) + ["-o", LIB] + [os.path.join(CSRC, s) for s in SOURCES]
     if verbose:

@@ -263,8 +263,24 @@ struct WebJob {
     uint8_t *out; int32_t out_pitch;
 };
 
+// ShaderNode::render (transformations/shader/node.rs, pipeline.rs:81-140) for one node: clear to transparent, then
+// max(1, n_tex) full-target planes, each pixel's smr_fragment at its centre blended with PREMULTIPLIED_ALPHA_BLENDING
+// through the node texture's view and stored as 8 bits.  The kernel is the shader module's own (shader_rt.cuh).
+struct ShaderJob {
+    int32_t width, height;        // the node texture
+    int32_t mode;                 // 0 GpuOptimized (sRGB views), 1 CpuOptimized
+    int32_t n_tex;                // texture_count: the children, in order
+    float time;                   // BaseShaderParameters::time, pts as Duration::as_secs_f32
+    const Tex *tex;               // n_tex child textures (TEX_NONE: the empty view), in the parameter arena
+    const uint8_t *params;        // ShaderParam::to_bytes, in the parameter arena (null: no parameter)
+    uint8_t *out; int32_t out_pitch;
+};
+
 // host tables pushed once per device (numeric contract NC-1/3/4)
 void upload_tables(const float *u8n, const float *srgb_dec, const float *srgb_enc_thr);
+// the device tables of node_sample.cuh in this module (c_u8n, c_dec, c_thr, c_yl, c_enc1): addresses and bytes, for the
+// copies a shader module receives when it is loaded.  false on a CUDA error
+bool table_symbols(const void *ptr[5], size_t bytes[5]);
 
 typedef void *Stream;  // cudaStream_t
 
@@ -292,6 +308,9 @@ int launch_text(const TextJob *jobs_dev, const int32_t *tile_begin_dev, int n_jo
 int launch_image(const ImageJob *jobs_dev, const int32_t *tile_begin_dev, int n_jobs, int n_tiles, Stream s);
 // web view node textures: each job's planes drawn over a transparent clear; jobs and tiles as for launch_text
 int launch_web(const WebJob *jobs_dev, const int32_t *tile_begin_dev, int n_jobs, int n_tiles, Stream s);
+// shader node textures of one shader module: `kernel` is its smr_shader_main (a cudaKernel_t); jobs and tiles as for
+// launch_text
+int launch_shader(const void *kernel, const ShaderJob *jobs_dev, const int32_t *tile_begin_dev, int n_jobs, int n_tiles, Stream s);
 // full_range: fused_launch_range of every job of the launch
 int launch_resample_fused(const FusedKernel &k, int src, int full_range, const FusedJob *jobs_dev, const FusedPiece *pieces_dev,
                           const int *piece_begin_dev, int nblocks, Stream s);

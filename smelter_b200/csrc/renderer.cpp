@@ -194,6 +194,120 @@ static struct {
     const char *(*GetErrorString)(int) = nullptr;
 } g_nccl;
 
+// NVRTC (shader registration), also dlopen'ed on first use: the library does not link against it
+static struct {
+    void *lib = nullptr;
+    int (*CreateProgram)(void **, const char *, const char *, int, const char *const *, const char *const *) = nullptr;
+    int (*CompileProgram)(void *, int, const char *const *) = nullptr;
+    int (*GetProgramLogSize)(void *, size_t *) = nullptr;
+    int (*GetProgramLog)(void *, char *) = nullptr;
+    int (*GetCUBINSize)(void *, size_t *) = nullptr;
+    int (*GetCUBIN)(void *, char *) = nullptr;
+    int (*AddNameExpression)(void *, const char *) = nullptr;
+    int (*GetLoweredName)(void *, const char *, const char **) = nullptr;
+    int (*DestroyProgram)(void **) = nullptr;
+    const char *(*GetErrorString)(int) = nullptr;
+} g_nvrtc;
+
+static bool nvrtc_load(std::string &err) {
+    if (g_nvrtc.lib) return true;
+    void *h = dlopen("libnvrtc.so.12", RTLD_NOW | RTLD_NOLOAD);   // the one already in the process (e.g. torch's)
+    if (!h) h = dlopen("libnvrtc.so.12", RTLD_NOW);
+    if (!h) h = dlopen("libnvrtc.so", RTLD_NOW);
+    if (!h) {
+        const char *home = getenv("CUDA_HOME");
+        h = dlopen((std::string(home ? home : "/usr/local/cuda") + "/lib64/libnvrtc.so.12").c_str(), RTLD_NOW);
+    }
+    if (!h) { err = std::string("cannot load NVRTC (libnvrtc.so.12), which compiles shaders: ") + dlerror(); return false; }
+    g_nvrtc.CreateProgram = (decltype(g_nvrtc.CreateProgram))dlsym(h, "nvrtcCreateProgram");
+    g_nvrtc.CompileProgram = (decltype(g_nvrtc.CompileProgram))dlsym(h, "nvrtcCompileProgram");
+    g_nvrtc.GetProgramLogSize = (decltype(g_nvrtc.GetProgramLogSize))dlsym(h, "nvrtcGetProgramLogSize");
+    g_nvrtc.GetProgramLog = (decltype(g_nvrtc.GetProgramLog))dlsym(h, "nvrtcGetProgramLog");
+    g_nvrtc.GetCUBINSize = (decltype(g_nvrtc.GetCUBINSize))dlsym(h, "nvrtcGetCUBINSize");
+    g_nvrtc.GetCUBIN = (decltype(g_nvrtc.GetCUBIN))dlsym(h, "nvrtcGetCUBIN");
+    g_nvrtc.AddNameExpression = (decltype(g_nvrtc.AddNameExpression))dlsym(h, "nvrtcAddNameExpression");
+    g_nvrtc.GetLoweredName = (decltype(g_nvrtc.GetLoweredName))dlsym(h, "nvrtcGetLoweredName");
+    g_nvrtc.DestroyProgram = (decltype(g_nvrtc.DestroyProgram))dlsym(h, "nvrtcDestroyProgram");
+    g_nvrtc.GetErrorString = (decltype(g_nvrtc.GetErrorString))dlsym(h, "nvrtcGetErrorString");
+    if (!g_nvrtc.CreateProgram || !g_nvrtc.CompileProgram || !g_nvrtc.GetProgramLogSize || !g_nvrtc.GetProgramLog ||
+        !g_nvrtc.GetCUBINSize || !g_nvrtc.GetCUBIN || !g_nvrtc.AddNameExpression || !g_nvrtc.GetLoweredName ||
+        !g_nvrtc.DestroyProgram || !g_nvrtc.GetErrorString) { err = "libnvrtc lacks required symbols"; return false; }
+    g_nvrtc.lib = h;
+    return true;
+}
+
+// the sources a shader module is compiled against (generated from kernels.h, node_sample.cuh, shader_rt.cuh by build.py)
+#include "shader_sources.inc"
+// the node_sample.cuh tables of a shader module, in table_symbols' order
+static const char *const kShaderTables[5] = {"&smr::dev::c_u8n", "&smr::dev::c_dec", "&smr::dev::c_thr", "&smr::dev::c_yl",
+                                             "&smr::dev::c_enc1"};
+
+// CreateShaderError analogue: false with NVRTC's log in `err`; `names` receives the lowered names of kShaderTables
+static bool compile_shader(const std::string &source, std::vector<char> &cubin, std::vector<std::string> &names, std::string &err) {
+    static const char kCstddef[] = "typedef decltype(sizeof(0)) size_t;\nnamespace std { using ::size_t; }\n";
+    static const char kCstdint[] =
+        "typedef signed char int8_t; typedef short int16_t; typedef int int32_t; typedef long int64_t;\n"
+        "typedef unsigned char uint8_t; typedef unsigned short uint16_t; typedef unsigned int uint32_t;\n"
+        "typedef unsigned long uint64_t; typedef unsigned long uintptr_t;\n"
+        "namespace std { using ::int8_t; using ::int16_t; using ::int32_t; using ::int64_t; using ::uint8_t; using ::uint16_t;\n"
+        "using ::uint32_t; using ::uint64_t; using ::uintptr_t; }\n";
+    const char *hdr[3] = {kSrc_kernels, kCstddef, kCstdint}, *hdr_names[3] = {"kernels.h", "cstddef", "cstdint"};
+    const std::string src = std::string("#include \"kernels.h\"\nnamespace smr {\nnamespace dev {\n") + kSrc_node_sample +
+                            "}  // namespace dev\n}  // namespace smr\n#define SMR_SHADER_API\n" + kSrc_shader_rt +
+                            "#undef SMR_SHADER_API\n#line 1 \"shader\"\n" + source + "\n#define SMR_SHADER_MAIN\n" + kSrc_shader_rt;
+    void *prog = nullptr;
+    int rc = g_nvrtc.CreateProgram(&prog, src.c_str(), "shader.cu", 3, hdr, hdr_names);
+    if (rc != 0) { err = std::string("nvrtcCreateProgram: ") + g_nvrtc.GetErrorString(rc); return false; }
+    for (const char *t : kShaderTables) g_nvrtc.AddNameExpression(prog, t);
+    // the numeric contract of kernels.cu: only explicit fmaf() is fused, IEEE division and square root, no flush to zero.
+    // -default-device: kernels.h's host declarations, and unannotated helpers of the shader, are device code here
+    const char *opts[] = {"--gpu-architecture=sm_90a", "-std=c++17", "--fmad=false", "--prec-div=true", "--prec-sqrt=true",
+                          "--ftz=false", "-default-device"};
+    rc = g_nvrtc.CompileProgram(prog, 7, opts);
+    if (rc != 0) {
+        size_t n = 0;
+        g_nvrtc.GetProgramLogSize(prog, &n);
+        std::string log(n, '\0');
+        if (n) g_nvrtc.GetProgramLog(prog, &log[0]);
+        err = std::string("shader does not compile (") + g_nvrtc.GetErrorString(rc) + "):\n" + log.c_str();
+        g_nvrtc.DestroyProgram(&prog);
+        return false;
+    }
+    size_t n = 0;
+    g_nvrtc.GetCUBINSize(prog, &n);
+    cubin.resize(n);
+    if (n) g_nvrtc.GetCUBIN(prog, cubin.data());
+    names.clear();
+    for (const char *t : kShaderTables) {
+        const char *lowered = nullptr;
+        g_nvrtc.GetLoweredName(prog, t, &lowered);
+        names.push_back(lowered ? lowered : "");
+    }
+    g_nvrtc.DestroyProgram(&prog);
+    return true;
+}
+
+// smr_shader_param_type -> ShaderParamType; false with the reason on a malformed type
+static bool param_type_from_c(const smr_shader_param_type *t, ShaderParamType &out, std::string &err, int depth) {
+    if (depth > 64) { err = "shader parameter type too deep"; return false; }
+    out.kind = t->kind;
+    if (t->name) out.name = t->name;
+    if (t->kind >= SMR_SHADER_PARAM_F32 && t->kind <= SMR_SHADER_PARAM_I32) return true;
+    if (t->kind != SMR_SHADER_PARAM_LIST && t->kind != SMR_SHADER_PARAM_STRUCT) { err = "unknown shader parameter kind"; return false; }
+    if (!t->items || t->items_len == 0) { err = "a list or struct parameter type needs items"; return false; }
+    if (t->kind == SMR_SHADER_PARAM_LIST && (t->items_len != 1 || t->length == 0)) {
+        err = "a list parameter type has one item type and a length of at least 1";
+        return false;
+    }
+    out.length = t->length;
+    out.items.resize(t->items_len);
+    for (uint32_t i = 0; i < t->items_len; i++) {
+        if (t->kind == SMR_SHADER_PARAM_STRUCT && !t->items[i].name) { err = "a struct parameter type's field has no name"; return false; }
+        if (!param_type_from_c(&t->items[i], out.items[i], err, depth + 1)) return false;
+    }
+    return true;
+}
+
 static bool nccl_load(std::string &err) {
     if (g_nccl.lib) return true;
     // RTLD_NOLOAD first: reuse the NCCL already in the process (e.g. the one torch.distributed loaded)
@@ -276,6 +390,8 @@ class Renderer {
     smr_status unregister_web_renderer(const char *id);
     smr_status web_set_frame(const char *id, const smr_web_frame *f);
     smr_status web_set_child_rects(const char *id, const smr_web_rect *rects, uint32_t n);
+    smr_status register_shader(const char *id, const smr_shader_spec *spec);
+    smr_status unregister_shader(const char *id);
     smr_status update_scene(const char *output_id, uint32_t w, uint32_t h, int32_t fmt, const smr_component *root);
     smr_status unregister_output(const char *id);
     smr_status set_layouts(const char *output_id, uint32_t w, uint32_t h, int32_t fmt, uint32_t root_w, uint32_t root_h,
@@ -290,6 +406,9 @@ class Renderer {
     smr_status debug_set_inputs(uint64_t pts, const smr_input_frame *in, uint32_t n_in);
     smr_status debug_layouts(const char *output_id, uint64_t pts, smr_render_layout *out, uint32_t cap, uint32_t *n,
                              uint32_t *rw, uint32_t *rh);
+    smr_status debug_node_layouts(const char *output_id, uint32_t node, uint64_t pts, smr_render_layout *out, uint32_t cap,
+                                  uint32_t *n, uint32_t *rw, uint32_t *rh);
+    smr_status layouts_to_c(const std::vector<RenderLayout> &layouts, smr_render_layout *out, uint32_t cap, uint32_t *n);
     smr_status debug_image_nodes(const char *output_id, uint64_t pts, smr_image_node_info *out, uint32_t cap, uint32_t *n);
     smr_status debug_fused_jobs(smr_fused_job_info *out, uint32_t cap, uint32_t *n);
     smr_status debug_composite_layers(smr_composite_layer_info *out, uint32_t cap, uint32_t *n);
@@ -339,11 +458,28 @@ class Renderer {
         size_t planes_off = 0;
         std::shared_ptr<void> mem;
     };
+    // A Shader component of an output's scene (ShaderNode, transformations/shader/node.rs).  The node texture persists and
+    // is redrawn, in the order of stream_, by every tick.
+    struct Output;
+    struct ShaderNode {
+        Input in;               // the node texture as a layout child: premultiplied TEX_RGBA8 of the node's resolution, always live
+        ShaderParams params;
+        Output *owner = nullptr;   // the output whose nodes its children are (set when a tick plans it)
+        dev::ShaderJob job = {};   // draws `in.tex`; its textures and parameter bytes are this tick's, in the parameter arena
+        std::vector<dev::Tex> tex;
+        size_t tex_off = 0, params_off = SIZE_MAX;
+        std::shared_ptr<void> mem;
+    };
     struct Output {
         OutputNode node;
         std::vector<std::unique_ptr<TextNode>> texts;   // node.texts, in the same order
         std::vector<std::unique_ptr<ImageNode>> images; // node.images, in the same order
         std::vector<std::unique_ptr<WebNode>> webs;     // node.webs, in the same order
+        std::vector<std::unique_ptr<ShaderNode>> shaders;   // node.shaders, in the same order
+        // node.nested: each layout node's texture of the current tick, RGBA8 in the frame arena (has_frame false: it has no
+        // pixels this tick, readers see the empty view)
+        std::deque<Input> nested;
+        uint64_t nodes_planned = 0;             // the tick whose texture table holds this output's node textures
         int32_t format = 0;
         Resolution res;
         DevBuf planes[kTicksInFlight][3];       // device staging for host outputs, one set per tick in flight: the read-back of
@@ -420,6 +556,10 @@ class Renderer {
     std::vector<RenderLayout> output_layouts(const Output &o, OutputNode &node, uint64_t pts,
                                              const std::vector<std::optional<Resolution>> &child_res, Resolution root);
     smr_status plan_output(Output &o, smr_output_frame &of, uint64_t pts);
+    Input *child_input(Output &o, const NodeChild &ch);
+    smr_status plan_layers(std::vector<RenderLayout> &layouts, const std::vector<Input *> &child_in, int W, int H,
+                           std::vector<dev::LayerDev> &layers, std::vector<dev::MaskDev> &masks);
+    smr_status plan_layout_node(Output &o, size_t k, uint64_t pts);
     smr_status child_texture(Input &in, RenderLayout &l, int &tex_index, int &tex_w, int &tex_h);
     template <class Launch> smr_status write_rgba(void *rgba, uint32_t pitch, int32_t mem_kind, uint32_t w, uint32_t h, Launch launch);
     smr_status get_weights(const KernelPass &p, WeightEntry &out);
@@ -489,12 +629,17 @@ class Renderer {
         std::vector<TextNode *> texts;        // text nodes drawn by this tick (one launch, before everything that reads them)
         std::vector<ImageNode *> images;      // image nodes drawn by this tick (likewise)
         std::vector<WebNode *> webs;          // web nodes drawn by this tick (after the text and image nodes they may read)
+        std::vector<ShaderNode *> shaders;    // shader nodes drawn by this tick (after the web nodes they may read)
+        // the tick's phases: one per depth of its layout and shader nodes below the roots, then the roots'.  A phase's
+        // generic resample passes and composite jobs are those from its mark up to the next one (planned in phase order)
+        struct Phase { size_t stages[3], composites; };
+        std::vector<Phase> phases;
         std::map<std::tuple<int, uint32_t, uint32_t, uint32_t, uint32_t, int, int>, int> resample_cache;
         void clear() {   // keeps the vectors' capacity
             tex.clear();
             for (auto &s : stages) s.clear();
             fused.clear(); tmaps.clear(); weight_jobs.clear(); convert_jobs.clear();
-            composites.clear(); outputs.clear(); fills.clear(); d2h.clear(); texts.clear(); images.clear(); webs.clear();
+            composites.clear(); outputs.clear(); fills.clear(); d2h.clear(); texts.clear(); images.clear(); webs.clear(); shaders.clear(); phases.clear();
             resample_cache.clear();
         }
     } plan_;
@@ -503,6 +648,11 @@ class Renderer {
     smr_status make_image_node(const ImageParams &p, std::unique_ptr<ImageNode> &out);
     smr_status make_web_node(const WebParams &p, std::unique_ptr<WebNode> &out);
     void plan_web_node(Output &o, WebNode &n);
+    smr_status make_shader_node(const ShaderParams &p, std::unique_ptr<ShaderNode> &out);
+    void plan_shader_node(Output &o, ShaderNode &n, uint64_t pts);
+    // Shader modules whose last user is gone: each is unloaded once the event recorded on stream_ at that time completes
+    std::vector<std::pair<void *, cudaEvent_t>> retired_shaders_;
+    void reap_shaders(bool all);
     cudaEvent_t web_ev_ = nullptr;             // the end of a web frame's copy: later launches on stream_ wait for it
     // Web frames: allocated on copy_stream_, released on stream_.  The pool never makes an allocation wait for a release
     // that is still pending on stream_ (no internal dependencies), so a copy does not wait for the ticks in flight.
@@ -610,6 +760,7 @@ Renderer::~Renderer() {
         outputs_.clear();   // text, image and web nodes, image assets and web frames free their memory on stream_
         scene_ = SceneState();
         cudaStreamSynchronize(stream_);
+        reap_shaders(true);
         if (web_pool_) cudaMemPoolDestroy(web_pool_);   // after the web frames it holds were released above
         for (void *p : peer_opened_) cudaIpcCloseMemHandle(p);
         for (void *p : peer_own_) cudaFree(p);
@@ -839,6 +990,84 @@ smr_status Renderer::unregister_output(const char *id) {
     return SMR_OK;
 }
 
+void Renderer::reap_shaders(bool all) {
+    for (size_t i = 0; i < retired_shaders_.size();) {
+        auto &r = retired_shaders_[i];
+        if (all || cudaEventQuery(r.second) == cudaSuccess) {
+            cudaLibraryUnload((cudaLibrary_t)r.first);
+            cudaEventDestroy(r.second);
+            retired_shaders_.erase(retired_shaders_.begin() + (long)i);
+        } else {
+            i++;
+        }
+    }
+}
+
+smr_status Renderer::register_shader(const char *id, const smr_shader_spec *spec) {
+    if (!id || !spec || !spec->source) return SMR_ERR_INVALID_ARGUMENT;
+    std::lock_guard<std::mutex> g(mu_);
+    if (scene_.has_shader(id)) { set_error("a shader with this id is already registered"); return SMR_ERR_INVALID_ARGUMENT; }
+    std::string err;
+    auto program = std::make_unique<ShaderProgram>();
+    if (spec->param_type) {
+        program->param_type.emplace();
+        if (!param_type_from_c(spec->param_type, *program->param_type, err, 0)) { set_error(err); return SMR_ERR_INVALID_ARGUMENT; }
+    }
+    if (!nvrtc_load(err)) { set_error(err); return SMR_ERR_UNSUPPORTED; }
+    std::vector<std::string> tables;
+    if (!compile_shader(spec->source, program->cubin, tables, err)) { set_error(err); return SMR_ERR_INVALID_ARGUMENT; }
+    if (!host_only_) {
+        CUDA_OK(cudaSetDevice(opts_.cuda_device));
+        reap_shaders(false);
+        cudaLibrary_t lib = nullptr;
+        CUDA_OK(cudaLibraryLoadData(&lib, program->cubin.data(), nullptr, nullptr, 0, nullptr, nullptr, 0));
+        program->library = lib;
+        cudaKernel_t k = nullptr;
+        const void *src[5];
+        size_t bytes[5];
+        cudaError_t e = cudaLibraryGetKernel(&k, lib, "smr_shader_main");
+        if (e == cudaSuccess && !dev::table_symbols(src, bytes)) e = cudaErrorInvalidSymbol;
+        for (int i = 0; i < 5 && e == cudaSuccess; i++) {   // the module's copies of the sampler and encode tables
+            void *dst = nullptr;
+            size_t n = 0;
+            e = cudaLibraryGetGlobal(&dst, &n, lib, tables[i].c_str());
+            if (e == cudaSuccess && n != bytes[i]) e = cudaErrorInvalidSymbol;
+            if (e == cudaSuccess) e = cudaMemcpyAsync(dst, src[i], n, cudaMemcpyDeviceToDevice, stream_);
+        }
+        if (e == cudaSuccess) e = cudaStreamSynchronize(stream_);
+        if (e != cudaSuccess) {
+            cudaLibraryUnload(lib);
+            set_error(std::string("loading the shader module: ") + cudaGetErrorString(e));
+            return SMR_ERR_CUDA;
+        }
+        program->kernel = (const void *)k;
+    }
+    // the module is unloaded after the ticks submitted before its last user let go of it
+    std::shared_ptr<ShaderProgram> shared(program.release(), [this](ShaderProgram *p) {
+        cudaEvent_t ev = nullptr;
+        if (p->library) {
+            cudaSetDevice(opts_.cuda_device);
+            if (cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) == cudaSuccess && cudaEventRecord(ev, stream_) == cudaSuccess) {
+                retired_shaders_.push_back({p->library, ev});
+            } else {   // no event: wait for the stream instead
+                if (ev) cudaEventDestroy(ev);
+                cudaStreamSynchronize(stream_);
+                cudaLibraryUnload((cudaLibrary_t)p->library);
+            }
+        }
+        delete p;
+    });
+    if (!scene_.register_shader(id, std::move(shared))) { set_error("a shader with this id is already registered"); return SMR_ERR_INVALID_ARGUMENT; }
+    return SMR_OK;
+}
+
+smr_status Renderer::unregister_shader(const char *id) {
+    if (!id) return SMR_ERR_INVALID_ARGUMENT;
+    std::lock_guard<std::mutex> g(mu_);
+    if (!scene_.unregister_shader(id)) { set_error("shader not registered"); return SMR_ERR_INVALID_ARGUMENT; }
+    return SMR_OK;
+}
+
 smr_status Renderer::check_output(uint32_t w, uint32_t h, int32_t fmt) {
     if (fmt < SMR_OUT_PLANAR_YUV420 || fmt > SMR_OUT_NV12) { set_error("unsupported output format"); return SMR_ERR_UNSUPPORTED; }
     if (w == 0 || h == 0 || w > 16384 || h > 16384) { set_error("output resolution out of range"); return SMR_ERR_INVALID_ARGUMENT; }
@@ -873,6 +1102,7 @@ smr_status Renderer::update_scene(const char *output_id, uint32_t w, uint32_t h,
     // image nodes have the resolution the scene state resolves; a node texture that cannot be allocated drops the update
     std::vector<std::unique_ptr<ImageNode>> images;
     std::vector<std::unique_ptr<WebNode>> webs;
+    std::vector<std::unique_ptr<ShaderNode>> shaders;
     smr_status image_st = SMR_OK;
     auto make_images = [&](OutputNode &n) {
         for (const ImageParams &p : n.images) {
@@ -882,6 +1112,10 @@ smr_status Renderer::update_scene(const char *output_id, uint32_t w, uint32_t h,
         for (const WebParams &p : n.webs) {
             webs.emplace_back();
             if ((image_st = make_web_node(p, webs.back())) != SMR_OK) return false;
+        }
+        for (const ShaderParams &p : n.shaders) {
+            shaders.emplace_back();
+            if ((image_st = make_shader_node(p, shaders.back())) != SMR_OK) return false;
         }
         return true;
     };
@@ -896,6 +1130,9 @@ smr_status Renderer::update_scene(const char *output_id, uint32_t w, uint32_t h,
     for (const auto &p : o.node.texts) o.texts.push_back(std::move(made[p.get()]));
     o.images = std::move(images);
     o.webs = std::move(webs);
+    o.shaders = std::move(shaders);
+    o.nested.clear();
+    o.nested.resize(o.node.nested.size());
     o.format = fmt;
     o.res = {w, h};
     o.flat = false; o.flat_layouts.clear(); o.flat_children.clear();
@@ -991,6 +1228,27 @@ smr_status Renderer::make_web_node(const WebParams &p, std::unique_ptr<WebNode> 
     return SMR_OK;
 }
 
+// A shader node for `p`: its node texture (transparent until its first tick) and the job that draws it
+smr_status Renderer::make_shader_node(const ShaderParams &p, std::unique_ptr<ShaderNode> &out) {
+    auto n = std::make_unique<ShaderNode>();
+    n->params = p;
+    const int w = (int)p.resolution.width, h = (int)p.resolution.height;
+    Input &in = n->in;
+    in.has_frame = true;
+    in.res = p.resolution;
+    in.tex.kind = dev::TEX_RGBA8; in.tex.width = w; in.tex.height = h; in.tex.pitch0 = w * 4;
+    dev::ShaderJob &J = n->job;
+    J.width = w; J.height = h; J.mode = opts_.rendering_mode; J.out_pitch = w * 4;
+    J.n_tex = (int)p.children.size();
+    if (!host_only_) {
+        if (smr_status st = alloc_on_stream((size_t)w * h * 4, n->mem); st != SMR_OK) return st;
+        in.tex.p0 = J.out = (uint8_t *)n->mem.get();
+        CUDA_OK(cudaMemsetAsync(J.out, 0, (size_t)w * h * 4, stream_));
+    }
+    out = std::move(n);
+    return SMR_OK;
+}
+
 static inline long long snap256(float v);
 static inline long long ceil_div256(long long a);
 
@@ -1052,16 +1310,31 @@ void Renderer::plan_web_node(Output &o, WebNode &n) {
     plan_.webs.push_back(&n);
 }
 
-// A tick that renders output `o` at `pts`: each of its text, image and web nodes enters the texture table.  The text nodes
+// The textures a tick's draw of shader node `n` reads (its children, each its own node; an input without a live frame is the
+// empty view) and BaseShaderParameters::time at `pts` (Duration::as_secs_f32: whole seconds plus nanoseconds / 1e9, in f32)
+// The textures themselves are read when the tick is packed, once the layout nodes' frame-arena textures have addresses.
+void Renderer::plan_shader_node(Output &o, ShaderNode &n, uint64_t pts) {
+    n.owner = &o;
+    n.job.time = (float)(pts / 1000000000ull) + (float)(uint32_t)(pts % 1000000000ull) / 1e9f;
+    plan_.shaders.push_back(&n);
+}
+
+// A tick that renders output `o` at `pts`: each of its text, image, web and shader nodes enters the texture table.  The text nodes
 // not drawn since the last smr_update_scene join the tick's text launch; the image nodes whose frame at `pts` (a Bitmap's
 // only frame; AnimatedAsset::render's choice) is not the one their texture holds join its image launch; the web nodes whose
 // instance has a frame join its web launch.
 void Renderer::plan_node_textures(Output &o, uint64_t pts) {
-    if (o.flat) return;
+    if (o.flat || o.nodes_planned == tick_) return;
+    o.nodes_planned = tick_;
     for (auto &n : o.webs) {
         n->in.node_tex = -1;
         n->in.raw_tex = add_texture(n->in.tex, false);
         plan_web_node(o, *n);
+    }
+    for (auto &n : o.shaders) {   // every tick draws every shader node (ShaderNode::render has no cache)
+        n->in.node_tex = -1;
+        n->in.raw_tex = add_texture(n->in.tex, false);
+        plan_shader_node(o, *n, pts);
     }
     for (auto &n : o.images) {
         n->in.node_tex = -1;
@@ -1128,10 +1401,13 @@ smr_status Renderer::set_layouts(const char *output_id, uint32_t w, uint32_t h, 
     o.format = fmt;
     o.res = {w, h};
     o.flat = true;
-    if ((!o.texts.empty() || !o.images.empty() || !o.webs.empty()) && !host_only_) CUDA_OK(cudaSetDevice(opts_.cuda_device));
+    if ((!o.texts.empty() || !o.images.empty() || !o.webs.empty() || !o.shaders.empty()) && !host_only_)
+        CUDA_OK(cudaSetDevice(opts_.cuda_device));
     o.texts.clear();
     o.images.clear();
     o.webs.clear();
+    o.shaders.clear();
+    o.nested.clear();
     o.flat_root = {root_w, root_h};
     o.flat_children.clear();
     for (uint32_t i = 0; i < n_children; i++) o.flat_children.push_back(child_ids[i] ? child_ids[i] : "");
@@ -1968,12 +2244,20 @@ Resolution Renderer::output_children(const Output &o, const OutputNode &node, ui
     if (o.flat)
         for (const std::string &id : o.flat_children) add(input(id));
     else
-        for (const NodeChild &ch : node.children)
-            add(ch.text >= 0    ? &o.texts[ch.text]->in
-                : ch.image >= 0 ? &o.images[ch.image]->in
-                : ch.web >= 0   ? &o.webs[ch.web]->in
-                                : input(ch.input_id));
+        for (const NodeChild &ch : node.children) add(child_input(const_cast<Output &>(o), ch));
     return o.flat ? o.flat_root : node.layout_resolution(pts);
+}
+
+// The Input behind a node child: a text, image, web, shader or layout node's texture, or a caller's input; nullptr when it
+// has no pixels this tick (an input without a live frame, a layout node of no size), which reads as the empty view
+Renderer::Input *Renderer::child_input(Output &o, const NodeChild &ch) {
+    if (ch.text >= 0) return &o.texts[ch.text]->in;
+    if (ch.image >= 0) return &o.images[ch.image]->in;
+    if (ch.web >= 0) return &o.webs[ch.web]->in;
+    if (ch.shader >= 0) return &o.shaders[ch.shader]->in;
+    if (ch.layout >= 0) return (size_t)ch.layout < o.nested.size() && o.nested[ch.layout].has_frame ? &o.nested[ch.layout] : nullptr;
+    auto it = inputs_.find(ch.input_id);
+    return it != inputs_.end() && it->second.has_frame ? &it->second : nullptr;
 }
 
 // Its flattened layouts (layout.rs:180-181), untruncated.  Evaluating them advances Tiles::last_layout of `node`: o.node
@@ -2065,6 +2349,68 @@ smr_status Renderer::child_texture(Input &in, RenderLayout &l, int &tex_index, i
     return SMR_OK;
 }
 
+// The composite layers of a W x H layout node: each child's texture (resampled where the layout scales it) and its masks
+smr_status Renderer::plan_layers(std::vector<RenderLayout> &layouts, const std::vector<Input *> &child_in, int W, int H,
+                                 std::vector<dev::LayerDev> &layers, std::vector<dev::MaskDev> &masks) {
+    for (RenderLayout &l : layouts) {
+        int tex_index = -1, tex_w = 1, tex_h = 1;
+        Input *in = l.kind == RenderLayout::ChildNode && l.index < child_in.size() ? child_in[l.index] : nullptr;
+        if (in) {
+            smr_status st = child_texture(*in, l, tex_index, tex_w, tex_h);
+            if (st != SMR_OK) return st;
+        }
+        dev::LayerDev d;
+        bool skip;
+        prepare_layer(l, W, H, tex_index, tex_w, tex_h, d, skip);
+        if (skip) continue;
+        d.mask_begin = (int)masks.size();
+        d.mask_count = layer_masks(l, masks);
+        layers.push_back(d);
+    }
+    return SMR_OK;
+}
+
+// Layout node k of output `o` below its root (LayoutNode::render): its layouts are evaluated every tick (update_state and
+// Tiles::last_layout advance as in the reference whether or not anything shows the node), then composited into an RGBA8
+// frame-arena texture of the tick's resolution (no tile plan, no direct tiles), which its readers take as a child texture
+smr_status Renderer::plan_layout_node(Output &o, size_t k, uint64_t pts) {
+    LayoutParams &lp = o.node.nested[k];
+    Input &nn = o.nested[k];
+    nn.has_frame = false;
+    nn.node_tex = nn.raw_tex = -1;
+    std::vector<Input *> child_in;
+    std::vector<std::optional<Resolution>> child_res;
+    for (const NodeChild &ch : lp.children) {
+        Input *in = child_input(o, ch);
+        child_in.push_back(in);
+        child_res.push_back(in ? std::optional<Resolution>(in->res) : std::nullopt);
+    }
+    const Resolution root = lp.resolution(pts);
+    std::vector<RenderLayout> layouts = lp.layouts(pts, child_res).flatten(child_res, root);
+    if (root.width == 0 || root.height == 0 || root.width > 16384 || root.height > 16384) return SMR_OK;
+    if (layouts.size() > opts_.max_layouts_count) layouts.resize(opts_.max_layouts_count);
+    const int W = (int)root.width, H = (int)root.height;
+    std::vector<dev::LayerDev> layers;
+    std::vector<dev::MaskDev> masks;
+    if (smr_status st = plan_layers(layouts, child_in, W, H, layers, masks); st != SMR_OK) return st;
+    CompositeRec pc;
+    memset(&pc.job, 0, sizeof(pc.job));
+    pc.job.width = W; pc.job.height = H; pc.job.mode = opts_.rendering_mode;
+    pc.job.n_layers = (int)layers.size();
+    pc.layers_off = param_put(layers.data(), sizeof(dev::LayerDev) * layers.size());
+    pc.masks_off = param_put(masks.data(), sizeof(dev::MaskDev) * masks.size());
+    pc.out_frame_off = frame_alloc((size_t)W * H * 4);
+    pc.job.out_format = -1;
+    pc.job.out_pitch0 = W * 4;
+    plan_.composites.push_back(pc);
+    nn.tex = dev::Tex();
+    nn.tex.kind = dev::TEX_RGBA8; nn.tex.width = W; nn.tex.height = H; nn.tex.pitch0 = W * 4;
+    nn.res = root;
+    nn.has_frame = true;
+    nn.raw_tex = add_texture(nn.tex, false, pc.out_frame_off);
+    return SMR_OK;
+}
+
 smr_status Renderer::plan_output(Output &o, smr_output_frame &of, uint64_t pts) {
     const int mode = opts_.rendering_mode;
     of.width = (uint32_t)o.res.width; of.height = (uint32_t)o.res.height;
@@ -2114,7 +2460,8 @@ smr_status Renderer::plan_output(Output &o, smr_output_frame &of, uint64_t pts) 
     };
 
     plan_node_textures(o, pts);
-    if (!o.flat && (o.node.root_is_input || o.node.root_text >= 0 || o.node.root_image >= 0 || o.node.root_web >= 0)) {  // pass-through: the root texture IS the node texture
+    if (!o.flat && (o.node.root_is_input || o.node.root_text >= 0 || o.node.root_image >= 0 || o.node.root_web >= 0 ||
+                    o.node.root_shader >= 0)) {  // pass-through: the root texture IS the node texture
         Input *root_in = nullptr;
         if (o.node.root_text >= 0) {
             root_in = &o.texts[o.node.root_text]->in;
@@ -2122,6 +2469,8 @@ smr_status Renderer::plan_output(Output &o, smr_output_frame &of, uint64_t pts) 
             root_in = &o.images[o.node.root_image]->in;
         } else if (o.node.root_web >= 0) {
             root_in = &o.webs[o.node.root_web]->in;
+        } else if (o.node.root_shader >= 0) {
+            root_in = &o.shaders[o.node.root_shader]->in;
         } else {
             auto it = inputs_.find(o.node.root_input_id);
             if (it != inputs_.end() && it->second.has_frame) root_in = &it->second;
@@ -2172,21 +2521,7 @@ smr_status Renderer::plan_output(Output &o, smr_output_frame &of, uint64_t pts) 
     const int W = (int)root.width, H = (int)root.height;
     std::vector<dev::LayerDev> layers;
     std::vector<dev::MaskDev> masks;
-    for (RenderLayout &l : layouts) {
-        int tex_index = -1, tex_w = 1, tex_h = 1;
-        Input *in = l.kind == RenderLayout::ChildNode && l.index < child_in.size() ? child_in[l.index] : nullptr;
-        if (in) {
-            smr_status st = child_texture(*in, l, tex_index, tex_w, tex_h);
-            if (st != SMR_OK) return st;
-        }
-        dev::LayerDev d;
-        bool skip;
-        prepare_layer(l, W, H, tex_index, tex_w, tex_h, d, skip);
-        if (skip) continue;
-        d.mask_begin = (int)masks.size();
-        d.mask_count = layer_masks(l, masks);
-        layers.push_back(d);
-    }
+    if (smr_status st = plan_layers(layouts, child_in, W, H, layers, masks); st != SMR_OK) return st;
 
     CompositeRec pc;
     memset(&pc.job, 0, sizeof(pc.job));
@@ -2257,14 +2592,41 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
         return f ? upload_input(I, *f) : SMR_OK;
     });
     if (st != SMR_OK) return st;
+    // the outputs up to the first that is not registered: those before it are planned, as they always were, before the
+    // tick fails on it
+    std::vector<Output *> outs;
+    int max_depth = 0;   // of the layout and shader nodes below the roots
     for (uint32_t i = 0; i < n_out; i++) {
-        if (!out[i].output_id) return SMR_ERR_INVALID_ARGUMENT;
-        auto it = outputs_.find(out[i].output_id);
-        if (it == outputs_.end()) {
+        auto it = out[i].output_id ? outputs_.find(out[i].output_id) : outputs_.end();
+        if (it == outputs_.end()) break;
+        Output &o = it->second;
+        outs.push_back(&o);
+        if (o.flat) continue;
+        for (const LayoutParams &lp : o.node.nested) max_depth = std::max(max_depth, lp.depth);
+        for (const ShaderParams &sp : o.node.shaders) max_depth = std::max(max_depth, sp.depth);
+    }
+    auto mark = [&]() {
+        plan_.phases.push_back({{plan_.stages[0].size(), plan_.stages[1].size(), plan_.stages[2].size()}, plan_.composites.size()});
+    };
+    for (int d = 1; d <= max_depth; d++) {   // the layout nodes below the roots, shallow first (a tick without any: no phase)
+        mark();
+        for (Output *o : outs) {
+            if (o->flat) continue;
+            for (size_t k = 0; k < o->node.nested.size(); k++) {
+                if (o->node.nested[k].depth != d) continue;
+                plan_node_textures(*o, pts);
+                if ((st = plan_layout_node(*o, k, pts)) != SMR_OK) return st;
+            }
+        }
+    }
+    mark();   // the roots
+    for (uint32_t i = 0; i < n_out; i++) {
+        if (i == outs.size()) {
+            if (!out[i].output_id) return SMR_ERR_INVALID_ARGUMENT;
             set_error(std::string("Output \"") + out[i].output_id + "\" does not exist, register it first");
             return SMR_ERR_OUTPUT_NOT_REGISTERED;
         }
-        st = plan_output(it->second, out[i], pts);
+        st = plan_output(*outs[i], out[i], pts);
         if (st != SMR_OK) return st;
     }
 
@@ -2374,6 +2736,31 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
     const TileJobs image_jobs = param_put_tile_jobs(plan_.images, &ImageNode::job);
     for (WebNode *n : plan_.webs) n->planes_off = param_put(n->planes.data(), sizeof(dev::WebPlane) * n->planes.size());
     const TileJobs web_jobs = param_put_tile_jobs(plan_.webs, &WebNode::job);
+    // shader nodes: one launch per (depth, shader), shallow first, so that every child is drawn before its reader
+    std::vector<std::vector<ShaderNode *>> shader_launches;
+    std::vector<TileJobs> shader_jobs;
+    {
+        std::vector<ShaderNode *> order = plan_.shaders;
+        std::stable_sort(order.begin(), order.end(), [](const ShaderNode *a, const ShaderNode *b) { return a->params.depth < b->params.depth; });
+        for (ShaderNode *n : order) {
+            auto same = [&](const std::vector<ShaderNode *> &l) { return l[0]->params.depth == n->params.depth && l[0]->params.shader == n->params.shader; };
+            auto it = std::find_if(shader_launches.begin(), shader_launches.end(), same);
+            if (it == shader_launches.end()) shader_launches.push_back({n});
+            else it->push_back(n);
+        }
+        for (ShaderNode *n : plan_.shaders) {   // the children's textures, frame-arena addresses resolved
+            n->tex.assign(n->params.children.size(), dev::Tex());
+            for (size_t k = 0; k < n->params.children.size(); k++) {
+                const NodeChild &ch = n->params.children[k];
+                Input *in = child_input(*n->owner, ch);
+                if (in) n->tex[k] = ch.layout >= 0 ? plan_.tex[in->raw_tex].tex : in->tex;
+            }
+            n->tex_off = param_put(n->tex.data(), sizeof(dev::Tex) * n->tex.size());
+            const std::vector<uint8_t> &b = n->params.param_bytes;
+            n->params_off = b.empty() ? SIZE_MAX : param_put(b.data(), b.size());
+        }
+        for (const auto &l : shader_launches) shader_jobs.push_back(param_put_tile_jobs(l, &ShaderNode::job));
+    }
     // the arena is sized: its offsets become device pointers in the packed jobs
     CUDA_OK(param_pinned_[slot_].ensure(param_used_));
     CUDA_OK(param_dev_[slot_].ensure(param_used_));
@@ -2381,6 +2768,13 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
     auto dev_ptr = [&](size_t off) -> uint8_t * { return off != SIZE_MAX ? pd + off : nullptr; };
     dev::WebJob *wj = reinterpret_cast<dev::WebJob *>(param_host_.data() + web_jobs.jobs_off);
     for (size_t i = 0; i < plan_.webs.size(); i++) wj[i].planes = (const dev::WebPlane *)(pd + plan_.webs[i]->planes_off);
+    for (size_t l = 0; l < shader_launches.size(); l++) {
+        dev::ShaderJob *sj = reinterpret_cast<dev::ShaderJob *>(param_host_.data() + shader_jobs[l].jobs_off);
+        for (size_t i = 0; i < shader_launches[l].size(); i++) {
+            sj[i].tex = (const dev::Tex *)(pd + shader_launches[l][i]->tex_off);
+            sj[i].params = dev_ptr(shader_launches[l][i]->params_off);
+        }
+    }
     dev::FusedJob *fj = reinterpret_cast<dev::FusedJob *>(param_host_.data() + fj_off);
     for (size_t i = 0; i < plan_.fused.size(); i++) {
         const FusedRec &f = plan_.fused[i];
@@ -2437,17 +2831,36 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
                                                  fl.nblocks, stream_))) goto fail;
         prof_mark(SMR_KERNEL_RESAMPLE_FUSED);
     }
-    for (int s = 0; s < 3; s++) {
-        if (!launched(dev::launch_resample((const dev::ResampleJob *)(pd + stage_off[s]),
-                                           (const dev::ResampleJob *)(param_host_.data() + stage_off[s]), (int)plan_.stages[s].size(),
-                                           stream_))) goto fail;
-        if (!plan_.stages[s].empty()) prof_mark(SMR_KERNEL_RESAMPLE_BOX + s);
-    }
-    if (!plan_.composites.empty()) {   // ONE launch for every output of the tick
-        if (!launched(dev::launch_composite((const dev::CompositeJob *)(pd + cj_off), cj,
-                                            (const dev::LayerDev *)(param_host_.data() + plan_.composites[0].layers_off),
-                                            (int)plan_.composites.size(), stream_))) goto fail;
-        prof_mark(SMR_KERNEL_COMPOSITE);
+    // phase by phase: the generic resample passes feeding its layout nodes, one composite launch for them, then the shader
+    // nodes of that depth; the last phase is the roots' (ONE composite launch for every output of the tick)
+    for (size_t p = 0; p < plan_.phases.size(); p++) {
+        const TickPlan::Phase &b = plan_.phases[p];
+        const bool last_phase = p + 1 == plan_.phases.size();
+        const TickPlan::Phase e = last_phase ? TickPlan::Phase{{plan_.stages[0].size(), plan_.stages[1].size(), plan_.stages[2].size()},
+                                                               plan_.composites.size()}
+                                             : plan_.phases[p + 1];
+        for (int s = 0; s < 3; s++) {
+            const size_t off = stage_off[s] + sizeof(dev::ResampleJob) * b.stages[s];
+            const int count = (int)(e.stages[s] - b.stages[s]);
+            if (!launched(dev::launch_resample((const dev::ResampleJob *)(pd + off), (const dev::ResampleJob *)(param_host_.data() + off),
+                                               count, stream_))) goto fail;
+            if (count) prof_mark(SMR_KERNEL_RESAMPLE_BOX + s);
+        }
+        if (e.composites > b.composites) {
+            if (!launched(dev::launch_composite((const dev::CompositeJob *)(pd + cj_off) + b.composites, cj + b.composites,
+                                                (const dev::LayerDev *)(param_host_.data() + plan_.composites[b.composites].layers_off),
+                                                (int)(e.composites - b.composites), stream_))) goto fail;
+            prof_mark(SMR_KERNEL_COMPOSITE);
+        }
+        if (last_phase) break;
+        for (size_t l = 0; l < shader_launches.size(); l++) {   // the shader nodes of depth p + 1
+            if (shader_launches[l][0]->params.depth != (int)p + 1) continue;
+            const TileJobs &t = shader_jobs[l];
+            if (!launched(dev::launch_shader(shader_launches[l][0]->params.shader->kernel, (const dev::ShaderJob *)(pd + t.jobs_off),
+                                             (const int32_t *)(pd + t.begin_off), (int)shader_launches[l].size(), t.n_tiles, stream_)))
+                goto fail;
+            prof_mark(SMR_KERNEL_SHADER);
+        }
     }
     for (OutputRec &o : plan_.outputs) {
         if (!launched(dev::launch_output(o.job, stream_))) goto fail;
@@ -2612,6 +3025,7 @@ smr_status Renderer::render_end() {   // retires the OLDEST tick in flight
     inflight_.pop_front();
     CUDA_OK(cudaEventSynchronize(tick_done_[s]));
     if (inflight_.empty()) fold_profile();
+    reap_shaders(false);
     return SMR_OK;
 }
 
@@ -2895,7 +3309,8 @@ smr_status Renderer::debug_layouts(const char *output_id, uint64_t pts, smr_rend
     if (it == outputs_.end()) { set_error("output not registered"); return SMR_ERR_OUTPUT_NOT_REGISTERED; }
     Output &o = it->second;
     *n = 0;
-    if (!o.flat && (o.node.root_is_input || o.node.root_text >= 0 || o.node.root_image >= 0 || o.node.root_web >= 0)) {
+    if (!o.flat && (o.node.root_is_input || o.node.root_text >= 0 || o.node.root_image >= 0 || o.node.root_web >= 0 ||
+                    o.node.root_shader >= 0)) {
         if (rw) *rw = 0;
         if (rh) *rh = 0;
         return SMR_OK;
@@ -2906,7 +3321,45 @@ smr_status Renderer::debug_layouts(const char *output_id, uint64_t pts, smr_rend
     const Resolution root = output_children(o, copy, pts, child_in, child_res);
     if (rw) *rw = (uint32_t)root.width;
     if (rh) *rh = (uint32_t)root.height;
-    std::vector<RenderLayout> layouts = output_layouts(o, copy, pts, child_res, root);
+    return layouts_to_c(output_layouts(o, copy, pts, child_res, root), out, cap, n);
+}
+
+// Layout node `node` of an output: 0 is the root when the root is a layout, the nodes below it follow in DFS order
+smr_status Renderer::debug_node_layouts(const char *output_id, uint32_t node, uint64_t pts, smr_render_layout *out, uint32_t cap,
+                                        uint32_t *n, uint32_t *rw, uint32_t *rh) {
+    if (!output_id || !n) return SMR_ERR_INVALID_ARGUMENT;
+    {
+        std::lock_guard<std::mutex> g(mu_);
+        auto it = outputs_.find(output_id);
+        if (it == outputs_.end()) { set_error("output not registered"); return SMR_ERR_OUTPUT_NOT_REGISTERED; }
+        Output &o = it->second;
+        const bool root_layout = !o.flat && !o.node.root_is_input && o.node.root_text < 0 && o.node.root_image < 0 &&
+                                 o.node.root_web < 0 && o.node.root_shader < 0;
+        if (!(root_layout && node == 0)) {
+            const size_t k = node - (root_layout ? 1 : 0);
+            if (o.flat || k >= o.node.nested.size()) { set_error("no such layout node"); return SMR_ERR_INVALID_ARGUMENT; }
+            LayoutParams copy = o.node.nested[k];   // do not advance Tiles::last_layout
+            std::vector<std::optional<Resolution>> child_res;
+            for (const NodeChild &ch : copy.children) {
+                if (ch.layout >= 0) {   // a layout node's texture has its resolution at pts
+                    const Resolution r = o.node.nested[ch.layout].resolution(pts);
+                    const bool ok = r.width && r.height && r.width <= 16384 && r.height <= 16384;
+                    child_res.push_back(ok ? std::optional<Resolution>(r) : std::nullopt);
+                } else {
+                    Input *in = child_input(o, ch);
+                    child_res.push_back(in ? std::optional<Resolution>(in->res) : std::nullopt);
+                }
+            }
+            const Resolution root = copy.resolution(pts);
+            if (rw) *rw = (uint32_t)root.width;
+            if (rh) *rh = (uint32_t)root.height;
+            return layouts_to_c(copy.layouts(pts, child_res).flatten(child_res, root), out, cap, n);
+        }
+    }
+    return debug_layouts(output_id, pts, out, cap, n, rw, rh);
+}
+
+smr_status Renderer::layouts_to_c(const std::vector<RenderLayout> &layouts, smr_render_layout *out, uint32_t cap, uint32_t *n) {
     *n = (uint32_t)layouts.size();
     if (!out) return SMR_OK;
     if (cap < layouts.size()) return SMR_ERR_BUFFER_TOO_SMALL;
@@ -2985,6 +3438,8 @@ smr_status smr_web_set_frame(smr_renderer *r, const char *id, const smr_web_fram
 smr_status smr_web_set_child_rects(smr_renderer *r, const char *id, const smr_web_rect *rects, uint32_t n) {
     SMR_GUARD(r->impl.web_set_child_rects(id, rects, n))
 }
+smr_status smr_register_shader(smr_renderer *r, const char *id, const smr_shader_spec *spec) { SMR_GUARD(r->impl.register_shader(id, spec)) }
+smr_status smr_unregister_shader(smr_renderer *r, const char *id) { SMR_GUARD(r->impl.unregister_shader(id)) }
 smr_status smr_update_scene(smr_renderer *r, const char *output_id, uint32_t w, uint32_t h, int32_t fmt,
                             const smr_component *root) { SMR_GUARD(r->impl.update_scene(output_id, w, h, fmt, root)) }
 smr_status smr_unregister_output(smr_renderer *r, const char *id) { SMR_GUARD(r->impl.unregister_output(id)) }
@@ -3055,6 +3510,11 @@ smr_status smr_debug_fused_jobs(smr_renderer *r, smr_fused_job_info *out, uint32
 smr_status smr_debug_composite_layers(smr_renderer *r, smr_composite_layer_info *out, uint32_t cap, uint32_t *n) {
     SMR_GUARD(r->impl.debug_composite_layers(out, cap, n))
 }
+smr_status smr_debug_node_layouts(smr_renderer *r, const char *output_id, uint32_t node, uint64_t pts_ns, smr_render_layout *out,
+                                  uint32_t capacity, uint32_t *n_out, uint32_t *root_width, uint32_t *root_height) {
+    SMR_GUARD(r->impl.debug_node_layouts(output_id, node, pts_ns, out, capacity, n_out, root_width, root_height))
+}
+
 smr_status smr_debug_interior(const smr_render_layout *layout, uint32_t width, uint32_t height, int32_t box[12], uint8_t *shortcut) {
     if (!layout || !box || width == 0 || height == 0 || width > 16384 || height > 16384) return SMR_ERR_INVALID_ARGUMENT;
     if (layout->type < 0 || layout->type > 2 || layout->masks_len < 0 || layout->masks_len > SMR_MAX_MASKS) return SMR_ERR_INVALID_ARGUMENT;

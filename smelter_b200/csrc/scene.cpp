@@ -122,6 +122,34 @@ static bool text_from_c(const smr_text *t, AtlasCopies &atlases, std::shared_ptr
     return true;
 }
 
+static bool shader_param_from_c(const smr_shader_param *p, ShaderParamValue &out, std::string &err, int depth) {
+    if (depth > 64) { err = "shader parameter too deep"; return false; }
+    out.kind = p->kind;
+    if (p->field_name) out.field_name = p->field_name;
+    switch (p->kind) {
+        case SMR_SHADER_PARAM_F32: out.f32 = p->f32; return true;
+        case SMR_SHADER_PARAM_U32: out.u32 = p->u32; return true;
+        case SMR_SHADER_PARAM_I32: out.i32 = p->i32; return true;
+        case SMR_SHADER_PARAM_LIST:
+        case SMR_SHADER_PARAM_STRUCT:
+            if (p->items_len && !p->items) { err = "shader parameter items pointer is null"; return false; }
+            if (p->items_len > (1u << 20)) { err = "shader parameter has too many items"; return false; }
+            out.items.resize(p->items_len);
+            for (uint32_t i = 0; i < p->items_len; i++) {
+                if (p->kind == SMR_SHADER_PARAM_STRUCT && !p->items[i].field_name) { err = "shader parameter field without a name"; return false; }
+                if (!shader_param_from_c(&p->items[i], out.items[i], err, depth + 1)) return false;
+            }
+            return true;
+        default: err = "unknown shader parameter kind"; return false;
+    }
+}
+
+void ShaderParamValue::to_bytes(std::vector<uint8_t> &out) const {   // little-endian, like the host
+    const void *v = kind == SMR_SHADER_PARAM_F32 ? (const void *)&f32 : kind == SMR_SHADER_PARAM_U32 ? (const void *)&u32 : (const void *)&i32;
+    if (kind <= SMR_SHADER_PARAM_I32) { out.insert(out.end(), (const uint8_t *)v, (const uint8_t *)v + 4); return; }
+    for (const ShaderParamValue &i : items) i.to_bytes(out);
+}
+
 static bool component_from_c(const smr_component *c, Component &out, std::string &err, int depth, AtlasCopies &atlases) {
     if (!c) { err = "null component"; return false; }
     if (depth > 256) { err = "component tree too deep"; return false; }
@@ -156,12 +184,27 @@ static bool component_from_c(const smr_component *c, Component &out, std::string
                 if (!component_from_c(&c->children[i], out.children[i], err, depth + 1, atlases)) return false;
             }
             return true;
+        case SMR_COMPONENT_SHADER:
+            if (!c->shader_id) { err = "component type outside the compositor hot path (Shader without shader_id)"; return false; }
+            out.shader_id = c->shader_id;
+            out.shader_width = c->shader_width;
+            out.shader_height = c->shader_height;
+            if (c->shader_param) {
+                out.shader_param.emplace();
+                if (!shader_param_from_c(c->shader_param, *out.shader_param, err, 0)) return false;
+            }
+            if (c->children_len && !c->children) { err = "children pointer is null"; return false; }
+            if (c->children_len > 16) { err = "a Shader with more than 16 children is outside the compositor hot path (16 textures)"; return false; }
+            out.children.resize(c->children_len);
+            for (uint32_t i = 0; i < c->children_len; i++)
+                if (!component_from_c(&c->children[i], out.children[i], err, depth + 1, atlases)) return false;
+            return true;
         case SMR_COMPONENT_VIEW:
         case SMR_COMPONENT_TILES:
         case SMR_COMPONENT_RESCALER:
             break;
         default:
-            err = "component type outside the compositor hot path (Shader)";
+            err = "component type outside the compositor hot path";
             return false;
     }
     if (c->type == SMR_COMPONENT_RESCALER && c->children_len != 1) {
@@ -467,7 +510,8 @@ const std::optional<std::string> &Stateful::component_id() const {
         case InputStream:
         case Text:
         case Image:
-        case WebView: return leaf_component_id;
+        case WebView:
+        case Shader: return leaf_component_id;
         case View: return view_end.id;
         case Rescaler: return rescaler_end.id;
         default: return tiles.id;
@@ -528,7 +572,7 @@ void Stateful::update_state(const std::optional<Resolution> *inputs, size_t n) {
             else c.size = {0.0f, 0.0f};
             off += 1;
         } else if (!c.is_layout()) {
-            off += 1;   // Text, Image, WebView: no state
+            off += 1;   // Text, Image, WebView, Shader: no state
         } else {
             size_t cnt = c.node_children_count();
             c.update_state(inputs + std::min(off, n), off < n ? std::min(cnt, n - off) : 0);
@@ -1091,6 +1135,7 @@ struct BuildCtx {
     const std::map<std::string, Resolution> *input_resolutions;
     const std::map<std::string, std::shared_ptr<const ImageAsset>> *images;
     const std::map<std::string, std::shared_ptr<WebInstance>> *webs;
+    const std::map<std::string, std::shared_ptr<const ShaderProgram>> *shaders;
     std::string *err;   // the first SceneError of the build
 };
 
@@ -1122,6 +1167,35 @@ static bool did_child_order_change(const std::vector<Stateful> &prev, const std:
     for (size_t i = 0; i < cur.size(); i++)
         if (prev[i].component_id() != cur[i].component_id()) return true;
     return false;
+}
+
+// validate_params (transformations/shader/validation.rs:314-520) over the types a smr_shader_param_type can describe;
+// `why` names the first mismatch
+static void validate_shader_param(const ShaderParamValue &v, const ShaderParamType &t, std::string &why) {
+    static const char *names[] = {"F32", "U32", "I32", "List", "Struct"};
+    if (v.kind != t.kind) {
+        why = std::string("expected ") + names[t.kind] + ", got " + names[v.kind];
+        return;
+    }
+    if (t.kind == SMR_SHADER_PARAM_LIST) {
+        if (v.items.size() > t.length) {
+            why = "list too long: expected at most " + std::to_string(t.length) + ", got " + std::to_string(v.items.size());
+            return;
+        }
+        for (size_t i = 0; i < v.items.size() && why.empty(); i++) validate_shader_param(v.items[i], t.items[0], why);
+    } else if (t.kind == SMR_SHADER_PARAM_STRUCT) {
+        if (v.items.size() != t.items.size()) {
+            why = "expected " + std::to_string(t.items.size()) + " fields, got " + std::to_string(v.items.size());
+            return;
+        }
+        for (size_t i = 0; i < v.items.size() && why.empty(); i++) {
+            if (v.items[i].field_name != t.items[i].name) {
+                why = "field " + std::to_string(i) + " is \"" + t.items[i].name + "\", got \"" + v.items[i].field_name + "\"";
+                return;
+            }
+            validate_shader_param(v.items[i], t.items[i], why);
+        }
+    }
 }
 
 static Stateful build_stateful(const Component &c, const BuildCtx &ctx) {
@@ -1185,6 +1259,29 @@ static Stateful build_stateful(const Component &c, const BuildCtx &ctx) {
             for (const Stateful &ch : s.children)
                 if (!ch.component_id() && ctx.err->empty())
                     *ctx.err = "Web view \"" + c.web_renderer_id + "\" has a child without an id";
+            return s;
+        }
+        case SMR_COMPONENT_SHADER: {  // shader_component.rs:43-72: the shader, the parameter, then the children
+            s.kind = Stateful::Shader;
+            s.leaf_component_id = c.id;
+            auto it = ctx.shaders->find(c.shader_id);
+            if (it == ctx.shaders->end()) {
+                if (ctx.err->empty()) *ctx.err = "Shader \"" + c.shader_id + "\" not found";
+                return s;
+            }
+            s.shader = it->second;
+            s.shader_param = c.shader_param;
+            if (c.shader_param && ctx.err->empty()) {
+                std::string why;
+                if (!s.shader->param_type) why = "the shader declares no parameter (NoBindingInShader)";
+                else validate_shader_param(*c.shader_param, *s.shader->param_type, why);
+                if (!why.empty()) *ctx.err = "Shader \"" + c.shader_id + "\": parameters do not match: " + why;
+            }
+            for (const Component &ch : c.children) s.children.push_back(build_stateful(ch, ctx));
+            s.size = {c.shader_width, c.shader_height};
+            const Resolution r{f32_as_usize(c.shader_width), f32_as_usize(c.shader_height)};
+            if ((r.width == 0 || r.width > 16384 || r.height == 0 || r.height > 16384) && ctx.err->empty())
+                *ctx.err = "Shader \"" + c.shader_id + "\" node of " + std::to_string(r.width) + " x " + std::to_string(r.height);
             return s;
         }
         case SMR_COMPONENT_VIEW: {  // view_component.rs:103-160
@@ -1258,10 +1355,14 @@ static bool visit_web_ids(const Component &c, std::set<std::string> &ids, std::s
     return true;
 }
 
-// A node child of the render graph (build_tree, scene_state.rs:154-196): an input, or a text, image or web node appended to
-// `out`, whose own children come first in DFS order for a web node
-static NodeChild node_child(const Stateful &l, OutputNode &out) {
+// A node child of the render graph (build_tree, scene_state.rs:154-196): an input, or a text, image, web, shader or layout
+// node appended to `out`, whose own children come first in DFS order.  A layout node's size is node_size at `pts`; a layout
+// root without width and height is UnknownDimensionsForLayoutNodeRoot (scene_state.rs:206-228), reported in `err`.
+static NodeChild node_child(const Stateful &l, OutputNode &out, uint64_t pts, std::string &err) {
     NodeChild ch;
+    auto depth_of = [&](const NodeChild &k) {
+        return k.shader >= 0 ? out.shaders[k.shader].depth : k.layout >= 0 ? out.nested[k.layout].depth : k.web >= 0 ? 1 : 0;
+    };
     if (l.kind == Stateful::Text) {
         ch.text = (int)out.texts.size();
         out.texts.push_back(l.text);
@@ -1271,13 +1372,62 @@ static NodeChild node_child(const Stateful &l, OutputNode &out) {
     } else if (l.kind == Stateful::WebView) {
         WebParams w;
         w.instance = l.web;
-        for (const Stateful &c : l.children) w.children.push_back(node_child(c, out));
+        for (const Stateful &c : l.children) w.children.push_back(node_child(c, out, pts, err));
         ch.web = (int)out.webs.size();
         out.webs.push_back(std::move(w));
+    } else if (l.kind == Stateful::Shader) {
+        ShaderParams p;
+        p.shader = l.shader;
+        if (l.shader_param) l.shader_param->to_bytes(p.param_bytes);
+        p.resolution = {f32_as_usize(l.size.width), f32_as_usize(l.size.height)};
+        for (const Stateful &c : l.children) {
+            const NodeChild k = node_child(c, out, pts, err);
+            p.depth = std::max(p.depth, depth_of(k) + 1);
+            p.children.push_back(k);
+        }
+        ch.shader = (int)out.shaders.size();
+        out.shaders.push_back(std::move(p));
+    } else if (l.is_layout()) {
+        LayoutParams p;
+        const Position pos = l.position(pts);
+        if (!pos.width || !pos.height) {
+            if (err.empty()) {
+                const std::optional<std::string> &id = l.component_id();
+                err = "Unknown dimensions for layout node root: " +
+                      (id ? "Please provide width and height values for component with id \"" + *id + "\"" : std::string("Please provide width and height values."));
+            }
+            return ch;
+        }
+        p.size = {*pos.width, *pos.height};
+        p.root = l;   // the render graph's clone
+        std::vector<const Stateful *> leaves;
+        l.node_children(leaves);
+        for (const Stateful *c : leaves) {
+            const NodeChild k = node_child(*c, out, pts, err);
+            p.depth = std::max(p.depth, depth_of(k) + 1);
+            p.children.push_back(k);
+        }
+        ch.layout = (int)out.nested.size();
+        out.nested.push_back(std::move(p));
     } else {
         ch.input_id = l.input_id;
     }
     return ch;
+}
+
+// recalculate_layout (scene_state.rs:233-262): every layout component whose parent is not a layout is laid out at its size
+// (the output's resolution for the root, its own width and height otherwise), which refreshes Tiles::last_layout
+static void recalculate_layout(Stateful &c, std::optional<Size> size, uint64_t pts, bool parent_is_layout) {
+    const OptF w = c.width(pts), h = c.height(pts);
+    if (c.is_layout()) {
+        if (!parent_is_layout) {
+            if (!size && w && h) size = Size{*w, *h};
+            if (size) c.layout(*size, pts);
+        }
+        for (Stateful &k : c.children) recalculate_layout(k, std::nullopt, pts, true);
+    } else {
+        for (Stateful &k : c.children) recalculate_layout(k, std::nullopt, pts, false);
+    }
 }
 }  // namespace
 
@@ -1312,8 +1462,7 @@ bool SceneState::update_scene(const std::string &output_id, const Component &roo
     // recalculate_layout on every output at last_pts (refreshes Tiles::last_layout), :87-94,198-230
     for (auto &kv : output_states_) {
         OutputSceneState &st = kv.second;
-        if (st.root.is_layout())
-            st.root.layout({(float)st.resolution.width, (float)st.resolution.height}, last_pts_ns_);
+        recalculate_layout(st.root, Size{(float)st.resolution.width, (float)st.resolution.height}, last_pts_ns_, false);
     }
     BuildCtx ctx;
     auto prev = output_states_.find(output_id);
@@ -1322,6 +1471,7 @@ bool SceneState::update_scene(const std::string &output_id, const Component &roo
     ctx.input_resolutions = &input_resolutions_;
     ctx.images = &images_;
     ctx.webs = &webs_;
+    ctx.shaders = &shaders_;
     std::string build_err;
     ctx.err = &build_err;
 
@@ -1331,6 +1481,7 @@ bool SceneState::update_scene(const std::string &output_id, const Component &roo
     st.resolution = resolution;
 
     // intermediate_node().build_tree(Some(resolution), last_pts), :154-196
+    err.clear();
     out = OutputNode();
     out.resolution = resolution;
     if (st.root.kind == Stateful::Text) {
@@ -1340,7 +1491,9 @@ bool SceneState::update_scene(const std::string &output_id, const Component &roo
         out.root_image = 0;
         out.images.push_back(st.root.image);
     } else if (st.root.kind == Stateful::WebView) {
-        out.root_web = node_child(st.root, out).web;
+        out.root_web = node_child(st.root, out, last_pts_ns_, err).web;
+    } else if (st.root.kind == Stateful::Shader) {
+        out.root_shader = node_child(st.root, out, last_pts_ns_, err).shader;
     } else if (!st.root.is_layout()) {
         out.root_is_input = true;
         out.root_input_id = st.root.input_id;
@@ -1349,8 +1502,9 @@ bool SceneState::update_scene(const std::string &output_id, const Component &roo
         out.size = {(float)resolution.width, (float)resolution.height};
         std::vector<const Stateful *> leaves;
         st.root.node_children(leaves);
-        for (const Stateful *l : leaves) out.children.push_back(node_child(*l, out));
+        for (const Stateful *l : leaves) out.children.push_back(node_child(*l, out, last_pts_ns_, err));
     }
+    if (!err.empty()) return false;
     if (accept && !accept(out)) return false;
     output_scenes_[output_id] = root;
     output_states_[output_id] = std::move(st);
@@ -1368,6 +1522,12 @@ bool SceneState::register_web(const std::string &instance_id, std::shared_ptr<We
 }
 
 bool SceneState::unregister_web(const std::string &instance_id) { return webs_.erase(instance_id) != 0; }
+
+bool SceneState::register_shader(const std::string &shader_id, std::shared_ptr<const ShaderProgram> shader) {
+    return shaders_.emplace(shader_id, std::move(shader)).second;
+}
+
+bool SceneState::unregister_shader(const std::string &shader_id) { return shaders_.erase(shader_id) != 0; }
 
 WebInstance *SceneState::web_instance(const std::string &instance_id) const {
     auto it = webs_.find(instance_id);
@@ -1390,6 +1550,18 @@ Resolution OutputNode::layout_resolution(uint64_t pts) const {  // scene/layout.
     float w = p.width ? *p.width : size.width;
     float h = p.height ? *p.height : size.height;
     return {f32_as_usize(w), f32_as_usize(h)};
+}
+
+Resolution LayoutParams::resolution(uint64_t pts) const {
+    Position p = root.position(pts);
+    float w = p.width ? *p.width : size.width;
+    float h = p.height ? *p.height : size.height;
+    return {f32_as_usize(w), f32_as_usize(h)};
+}
+
+NestedLayout LayoutParams::layouts(uint64_t pts, const std::vector<std::optional<Resolution>> &inputs) {
+    root.update_state(inputs.data(), inputs.size());
+    return root.layout(size, pts);
 }
 
 NestedLayout OutputNode::layouts(uint64_t pts, const std::vector<std::optional<Resolution>> &inputs) {

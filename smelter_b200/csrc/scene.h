@@ -134,6 +134,33 @@ struct WebInstance {
     std::vector<float> rects;             // the latest child rects: x, y, width, height per child, narrowed to f32
 };
 
+// The type of a shader's parameter (smr_shader_param_type): the tree of scalars, fixed-length lists and structs that stands
+// in for the WGSL uniform type the reference reads out of the shader module (pipeline.rs:143-160)
+struct ShaderParamType {
+    int32_t kind = SMR_SHADER_PARAM_F32;  // smr_shader_param_kind
+    std::string name;                     // a struct field's name
+    std::vector<ShaderParamType> items;   // List: the element type (one); Struct: the fields, in order
+    uint32_t length = 0;                  // List: the element count
+};
+// A ShaderParam value (scene/components.rs:40-55)
+struct ShaderParamValue {
+    int32_t kind = SMR_SHADER_PARAM_F32;
+    std::string field_name;               // a Struct's field
+    float f32 = 0;
+    uint32_t u32 = 0;
+    int32_t i32 = 0;
+    std::vector<ShaderParamValue> items;  // List: the elements; Struct: the fields
+    void to_bytes(std::vector<uint8_t> &out) const;   // ShaderParamExt::to_bytes (node.rs:92-115)
+};
+// A registered shader (transformations/shader.rs: Shader): its parameter type and its compiled module.  The registry and
+// the scene nodes hold it by shared_ptr; the renderer unloads the module after the last tick that launched it.
+struct ShaderProgram {
+    std::optional<ShaderParamType> param_type;
+    std::vector<char> cubin;              // NVRTC's image for sm_90a
+    void *library = nullptr;              // cudaLibrary_t (device handles only)
+    const void *kernel = nullptr;         // its smr_shader_main, a cudaKernel_t
+};
+
 // scene::Component (scene.rs:50-60); only the variants on the compositor path
 struct Component {
     int type = SMR_COMPONENT_VIEW;
@@ -160,6 +187,9 @@ struct Component {
     std::string image_id;                  // Image
     OptF image_width, image_height;
     std::string web_renderer_id;           // WebView (children: the embedded components)
+    std::string shader_id;                 // Shader (children: its textures)
+    std::optional<ShaderParamValue> shader_param;
+    float shader_width = 0, shader_height = 0;
 };
 
 // Converts the C tree; returns false + message for variants outside the hot path.
@@ -286,7 +316,7 @@ struct TransitionState {
 };
 
 struct Stateful {
-    enum Kind { InputStream, View, Tiles, Rescaler, Text, Image, WebView } kind = View;
+    enum Kind { InputStream, View, Tiles, Rescaler, Text, Image, WebView, Shader } kind = View;
     // InputStream (scene/input_stream_component.rs), Text (scene/text_component.rs), Image (scene/image_component.rs),
     // WebView (scene/web_view_component.rs): the node children of a layout
     std::string input_id;
@@ -299,6 +329,8 @@ struct Stateful {
     ImageParams image;                        // ... and what it resolved to
     std::shared_ptr<WebInstance> web;         // WebView: the instance; `children` are its embedded components (render
                                               // nodes of their own, never laid out)
+    std::shared_ptr<const ShaderProgram> shader;   // Shader: the program; `children` are its textures (render nodes)
+    std::optional<ShaderParamValue> shader_param;
     // View
     std::optional<ViewParam> view_start;
     ViewParam view_end;
@@ -328,13 +360,39 @@ struct NodeChild {
     std::string input_id;
     int text = -1;                            // index in OutputNode::texts, or -1
     int image = -1;                           // index in OutputNode::images, or -1
-    int web = -1;                             // index in OutputNode::webs, or -1; all -1: the input `input_id`
+    int web = -1;                             // index in OutputNode::webs, or -1
+    int shader = -1;                          // index in OutputNode::shaders, or -1
+    int layout = -1;                          // index in OutputNode::nested, or -1; all -1: the input `input_id`
+};
+
+// A layout node other than the output's root (scene_state.rs:154-228, NodeParams::Layout): a View, Tiles or Rescaler whose
+// parent is a Shader.  Its own clone of the stateful component, its size (node_size at the last render's pts: the root's
+// width and height), its node children in DFS order, and its depth (1 + its deepest child's).  It is composited into its
+// own texture every tick.
+struct LayoutParams {
+    Stateful root;
+    Size size;
+    std::vector<NodeChild> children;
+    int depth = 1;
+    Resolution resolution(uint64_t pts) const;   // SizedLayoutComponent::resolution (scene/layout.rs:245-257)
+    NestedLayout layouts(uint64_t pts, const std::vector<std::optional<Resolution>> &inputs);
 };
 
 // A WebView render node (state/node.rs:127-141, NodeParams::Web): the instance and its children, each its own node
 struct WebParams {
     std::shared_ptr<WebInstance> instance;
     std::vector<NodeChild> children;          // input, text or image nodes (never `web`)
+};
+
+// A Shader render node (state/node.rs, NodeParams::Shader): the program, the parameter bytes, the node's resolution
+// (Size as Resolution: `as usize`) and its children, each its own node.  depth: 1 + the deepest child's (an input, text or
+// image 0, a web node 1), so that a tick draws every child before the shader that reads it.
+struct ShaderParams {
+    std::shared_ptr<const ShaderProgram> shader;
+    std::vector<uint8_t> param_bytes;
+    Resolution resolution;
+    std::vector<NodeChild> children;
+    int depth = 1;
 };
 
 // scene/scene_state.rs
@@ -350,6 +408,9 @@ struct OutputNode {
     std::vector<ImageParams> images;          // the output's image nodes, likewise (web view children included)
     int root_web = -1;                        // the root is web node webs[root_web] (-1: it is not a WebView)
     std::vector<WebParams> webs;              // the output's web nodes, likewise
+    int root_shader = -1;                     // the root is shader node shaders[root_shader] (-1: it is not a Shader)
+    std::vector<ShaderParams> shaders;        // the output's shader nodes, children before parents
+    std::vector<LayoutParams> nested;         // the output's layout nodes below the root, DFS order, children before parents
     Resolution resolution;
 
     // scene::LayoutNode as LayoutProvider (scene/layout.rs:31-41, 240-261)
@@ -372,6 +433,10 @@ class SceneState {
     bool register_web(const std::string &instance_id, std::shared_ptr<WebInstance> instance);
     bool unregister_web(const std::string &instance_id);
     WebInstance *web_instance(const std::string &instance_id) const;
+    // the shader registry (registry.rs:57-68), likewise
+    bool register_shader(const std::string &shader_id, std::shared_ptr<const ShaderProgram> shader);
+    bool unregister_shader(const std::string &shader_id);
+    bool has_shader(const std::string &shader_id) const { return shaders_.count(shader_id) != 0; }
     uint64_t last_pts() const { return last_pts_ns_; }
 
   private:
@@ -385,6 +450,7 @@ class SceneState {
     std::map<std::string, Resolution> input_resolutions_;
     std::map<std::string, std::shared_ptr<const ImageAsset>> images_;
     std::map<std::string, std::shared_ptr<WebInstance>> webs_;
+    std::map<std::string, std::shared_ptr<const ShaderProgram>> shaders_;
 };
 
 double cubic_bezier_easing(double progress, double x1, double y1, double x2, double y2);

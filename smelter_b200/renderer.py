@@ -334,8 +334,102 @@ class WebViewComponent:
     children: List["Component"] = field(default_factory=list)
 
 
+@dataclass
+class ShaderParam:
+    """A ShaderParam value (scene/components.rs:40-55): kind one of "f32", "u32", "i32" (value: the scalar), "list" (value:
+    a list of ShaderParam) or "struct" (value: a list of (field name, ShaderParam) pairs)."""
+    kind: str
+    value: object
+
+    @staticmethod
+    def f32(v):
+        return ShaderParam("f32", float(v))
+
+    @staticmethod
+    def u32(v):
+        return ShaderParam("u32", int(v))
+
+    @staticmethod
+    def i32(v):
+        return ShaderParam("i32", int(v))
+
+    @staticmethod
+    def list(items):
+        return ShaderParam("list", list(items))
+
+    @staticmethod
+    def struct(fields):
+        return ShaderParam("struct", [(str(n), v) for n, v in fields])
+
+
+@dataclass
+class ShaderParamType:
+    """The type of a shader's parameter (smr_shader_param_type): kind "f32", "u32", "i32", "list" (item: the element type,
+    length: the element count) or "struct" (fields: (name, ShaderParamType) pairs)."""
+    kind: str
+    item: Optional["ShaderParamType"] = None
+    length: int = 0
+    fields: List[Tuple[str, "ShaderParamType"]] = field(default_factory=list)
+
+
+@dataclass
+class ShaderComponent:
+    """A Shader component (scene/components.rs:29-38): the shader registered as `shader_id` (Renderer.register_shader) drawn
+    into a node of width x height, with `children` as its textures and `shader_param` as its parameter (None: none)."""
+    id: Optional[str] = None
+    shader_id: str = ""
+    shader_param: Optional[ShaderParam] = None
+    width: float = 0.0
+    height: float = 0.0
+    children: List["Component"] = field(default_factory=list)
+
+
 Component = Union[InputStreamComponent, ViewComponent, RescalerComponent, TilesComponent, TextComponent, ImageComponent,
-                  WebViewComponent]
+                  WebViewComponent, ShaderComponent]
+
+_PARAM_KINDS = {"f32": F.SHADER_PARAM_F32, "u32": F.SHADER_PARAM_U32, "i32": F.SHADER_PARAM_I32, "list": F.SHADER_PARAM_LIST,
+                "struct": F.SHADER_PARAM_STRUCT}
+
+
+def _param_to_c(p, keep, name=None):
+    """ShaderParam -> smr_shader_param (buffers kept alive in `keep`)"""
+    c = F.ShaderParam()
+    c.kind = _PARAM_KINDS[p.kind]
+    if name is not None:
+        nb = name.encode()
+        keep.append(nb)
+        c.field_name = nb
+    if p.kind == "f32":
+        c.f32 = float(p.value)
+    elif p.kind == "u32":
+        c.u32 = int(p.value)
+    elif p.kind == "i32":
+        c.i32 = int(p.value)
+    else:
+        items = [_param_to_c(v, keep) for v in p.value] if p.kind == "list" else [_param_to_c(v, keep, n) for n, v in p.value]
+        if items:
+            arr = (F.ShaderParam * len(items))(*items)
+            keep.append(arr)
+            c.items, c.items_len = arr, len(items)
+    return c
+
+
+def _param_type_to_c(t, keep, name=None):
+    """ShaderParamType -> smr_shader_param_type"""
+    c = F.ShaderParamType()
+    c.kind = _PARAM_KINDS[t.kind]
+    if name is not None:
+        nb = name.encode()
+        keep.append(nb)
+        c.name = nb
+    items = ([_param_type_to_c(t.item, keep)] if t.kind == "list" and t.item is not None else
+             [_param_type_to_c(v, keep, n) for n, v in t.fields] if t.kind == "struct" else [])
+    if items:
+        arr = (F.ShaderParamType * len(items))(*items)
+        keep.append(arr)
+        c.items, c.items_len = arr, len(items)
+    c.length = int(t.length)
+    return c
 
 
 def _opt(v):
@@ -434,9 +528,20 @@ def _to_c(comp, keep):
         c.tiles_margin, c.tiles_padding = float(comp.margin), float(comp.padding)
         c.horizontal_align, c.vertical_align = comp.horizontal_align, comp.vertical_align
         _children(c, comp.children, keep)
+    elif isinstance(comp, ShaderComponent):
+        F.lib().smr_component_default(F.COMPONENT_SHADER, C.byref(c))
+        sid = comp.shader_id.encode()
+        keep.append(sid)
+        c.shader_id = sid
+        if comp.shader_param is not None:
+            pc = _param_to_c(comp.shader_param, keep)
+            keep.append(pc)
+            c.shader_param = C.pointer(pc)
+        c.shader_width, c.shader_height = float(comp.width), float(comp.height)
+        _children(c, comp.children, keep)
     else:
-        # Shader is outside the compositor hot path: forward the tag so the
-        # library answers SMR_ERR_UNSUPPORTED like any other caller would see
+        # any other object: forward its tag with shader_id left NULL, which is what a caller built before the Shader
+        # fields existed sends, so the library answers SMR_ERR_UNSUPPORTED
         c.type = getattr(comp, "component_type", F.COMPONENT_SHADER)
     if getattr(comp, "id", None) is not None:
         cid = comp.id.encode()
@@ -540,6 +645,18 @@ class Renderer:
         hands over the painted frames (set_web_frame) and the child rects (set_web_child_rects)"""
         spec = F.WebRendererSpec(int(width), int(height), int(embedding_method))
         self._check(self._lib.smr_register_web_renderer(self._h, instance_id.encode(), C.byref(spec)))
+
+    def register_shader(self, shader_id: str, source: str, param_type: Optional[ShaderParamType] = None):
+        """Renderer::register_renderer for RendererSpec::Shader: `source` is CUDA C++ defining smr_fragment (see
+        include/smelter_b200.h), compiled here for sm_90a; `param_type` the type of its parameter (None: none)"""
+        keep = []
+        src = source.encode()
+        pt = _param_type_to_c(param_type, keep) if param_type is not None else None
+        spec = F.ShaderSpec(src, C.pointer(pt) if pt is not None else None)
+        self._check(self._lib.smr_register_shader(self._h, shader_id.encode(), C.byref(spec)))
+
+    def unregister_shader(self, shader_id: str):
+        self._check(self._lib.smr_unregister_shader(self._h, shader_id.encode()))
 
     def unregister_web_renderer(self, instance_id: str):
         self._check(self._lib.smr_unregister_web_renderer(self._h, instance_id.encode()))
@@ -722,6 +839,19 @@ class Renderer:
         arr = (F.RenderLayout * max(1, n.value))()
         self._check(self._lib.smr_debug_layouts(self._h, output_id.encode(), pts_ns, arr, n.value, C.byref(n),
                                                 C.byref(rw), C.byref(rh)))
+        return [arr[i] for i in range(n.value)], (rw.value, rh.value)
+
+    def debug_node_layouts(self, output_id: str, node: int, pts: float = 0.0):
+        """smr_debug_node_layouts: the flattened layouts of layout node `node` of an output's render graph (0: the root when
+        it is a layout; the layout nodes below it follow in DFS order) and its resolution at `pts`"""
+        n = C.c_uint32()
+        rw, rh = C.c_uint32(), C.c_uint32()
+        pts_ns = _secs_to_ns(pts)
+        self._check(self._lib.smr_debug_node_layouts(self._h, output_id.encode(), int(node), pts_ns, None, 0, C.byref(n),
+                                                     C.byref(rw), C.byref(rh)))
+        arr = (F.RenderLayout * max(1, n.value))()
+        self._check(self._lib.smr_debug_node_layouts(self._h, output_id.encode(), int(node), pts_ns, arr, n.value, C.byref(n),
+                                                     C.byref(rw), C.byref(rh)))
         return [arr[i] for i in range(n.value)], (rw.value, rh.value)
 
     def debug_image_nodes(self, output_id: str, pts: float = 0.0):
