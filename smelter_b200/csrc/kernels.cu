@@ -1585,21 +1585,16 @@ __global__ void __launch_bounds__(256) k_text(const TextJob *__restrict__ jobs, 
     __shared__ int s_wc[8];
     __shared__ TextJob J;
     const int lane = threadIdx.x, warp = threadIdx.y, tid = warp * 32 + lane;
-    if (tid == 0) {
-        const int b = (int)blockIdx.x, lo = tile_job(tile_begin, n_jobs, b);
-        J = jobs[lo];
-        const int t = b - tile_begin[lo], tiles_x = (J.width + 31) / 32;
-        s_wc[0] = (t % tiles_x) * 32;   // the tile's origin, handed over through s_wc before the glyph loop reuses it
-        s_wc[1] = (t / tiles_x) * 8;
-    }
+    // the tile's origin is handed over through s_wc before the glyph loop reuses it
+    if (tid == 0) load_block_job(jobs, tile_begin, n_jobs, J, s_wc);
     load_tables(T);   // ends in __syncthreads
     const int x0 = s_wc[0], y0 = s_wc[1], px = x0 + lane, py = y0 + warp;
     __syncthreads();   // s_wc is rewritten by the glyph loop
     uchar4 d;
-    if (J.mode == 0) d = make_uchar4((unsigned char)srgb_encode(T, J.bg[0]), (unsigned char)srgb_encode(T, J.bg[1]), (unsigned char)srgb_encode(T, J.bg[2]), (unsigned char)unorm8(J.bg[3]));
+    if (J.dst.mode == 0) d = make_uchar4((unsigned char)srgb_encode(T, J.bg[0]), (unsigned char)srgb_encode(T, J.bg[1]), (unsigned char)srgb_encode(T, J.bg[2]), (unsigned char)unorm8(J.bg[3]));
     else d = make_uchar4((unsigned char)unorm8(J.bg[0]), (unsigned char)unorm8(J.bg[1]), (unsigned char)unorm8(J.bg[2]), (unsigned char)unorm8(J.bg[3]));
     const float *clut = J.color_mode == 0 ? T.dec : T.u8n;   // ColorMode::Accurate: glyph colours and colour-atlas texels -> linear
-    const float *dlut = J.mode == 0 ? T.dec : T.u8n;         // the node texture's view
+    const float *dlut = J.dst.mode == 0 ? T.dec : T.u8n;     // the node texture's view
     for (int base = 0; base < J.n_glyphs; base += 256) {
         const int gi = base + tid;
         bool hit = false;
@@ -1637,13 +1632,13 @@ __global__ void __launch_bounds__(256) k_text(const TextJob *__restrict__ jobs, 
             if (a == 0.0f) continue;   // dst * 1 + src * 0: encode(decode(b)) == b, unorm8(b / 255) == b
             const float ia = 1.0f - a;
             const float r0 = fmaf(dlut[d.x], ia, s0 * a), r1 = fmaf(dlut[d.y], ia, s1 * a), r2 = fmaf(dlut[d.z], ia, s2 * a);
-            if (J.mode == 0) { d.x = (unsigned char)srgb_encode(T, r0); d.y = (unsigned char)srgb_encode(T, r1); d.z = (unsigned char)srgb_encode(T, r2); }
+            if (J.dst.mode == 0) { d.x = (unsigned char)srgb_encode(T, r0); d.y = (unsigned char)srgb_encode(T, r1); d.z = (unsigned char)srgb_encode(T, r2); }
             else { d.x = (unsigned char)unorm8(r0); d.y = (unsigned char)unorm8(r1); d.z = (unsigned char)unorm8(r2); }
             d.w = (unsigned char)unorm8(fmaf(T.u8n[d.w], ia, a));
         }
         __syncthreads();   // s_list / s_wc are rewritten by the next batch
     }
-    if (px < J.width && py < J.height) reinterpret_cast<uchar4 *>(J.out + (size_t)py * J.out_pitch)[px] = d;
+    if (px < J.dst.width && py < J.dst.height) reinterpret_cast<uchar4 *>(J.dst.out + (size_t)py * J.dst.out_pitch)[px] = d;
 }
 
 int launch_text(const TextJob *jobs_dev, const int32_t *tile_begin_dev, int n_jobs, int n_tiles, Stream s) {
@@ -1662,20 +1657,14 @@ __global__ void __launch_bounds__(256) k_image(const ImageJob *__restrict__ jobs
     __shared__ Tables T;
     __shared__ ImageJob J;
     __shared__ int s_origin[2];
-    if (threadIdx.x == 0 && threadIdx.y == 0) {
-        const int b = (int)blockIdx.x, lo = tile_job(tile_begin, n_jobs, b);
-        J = jobs[lo];
-        const int t = b - tile_begin[lo], tiles_x = (J.width + 31) / 32;
-        s_origin[0] = (t % tiles_x) * 32;
-        s_origin[1] = (t / tiles_x) * 8;
-    }
+    if (threadIdx.x == 0 && threadIdx.y == 0) load_block_job(jobs, tile_begin, n_jobs, J, s_origin);
     load_tables(T);   // ends in __syncthreads
     const int x = s_origin[0] + (int)threadIdx.x, y = s_origin[1] + (int)threadIdx.y;
-    if (x >= J.width || y >= J.height) return;
+    if (x >= J.dst.width || y >= J.dst.height) return;
     bool exact;
     uchar4 texel;
-    const float4 c = sample_node(T, &J.src, J.mode, ((float)x + 0.5f) / (float)J.width, ((float)y + 0.5f) / (float)J.height, exact, texel);
-    reinterpret_cast<uchar4 *>(J.out + (size_t)y * J.out_pitch)[x] = premultiply_store(T, J.mode, c);
+    const float4 c = sample_node(T, &J.src, J.dst.mode, ((float)x + 0.5f) / (float)J.dst.width, ((float)y + 0.5f) / (float)J.dst.height, exact, texel);
+    reinterpret_cast<uchar4 *>(J.dst.out + (size_t)y * J.dst.out_pitch)[x] = premultiply_store(T, J.dst.mode, c);
 }
 
 int launch_image(const ImageJob *jobs_dev, const int32_t *tile_begin_dev, int n_jobs, int n_tiles, Stream s) {
@@ -1695,16 +1684,10 @@ __global__ void __launch_bounds__(256) k_web(const WebJob *__restrict__ jobs, co
     __shared__ Tables T;
     __shared__ WebJob J;
     __shared__ int s_origin[2];
-    if (threadIdx.x == 0 && threadIdx.y == 0) {
-        const int b = (int)blockIdx.x, lo = tile_job(tile_begin, n_jobs, b);
-        J = jobs[lo];
-        const int t = b - tile_begin[lo], tiles_x = (J.width + 31) / 32;
-        s_origin[0] = (t % tiles_x) * 32;
-        s_origin[1] = (t / tiles_x) * 8;
-    }
+    if (threadIdx.x == 0 && threadIdx.y == 0) load_block_job(jobs, tile_begin, n_jobs, J, s_origin);
     load_tables(T);   // ends in __syncthreads
     const int x = s_origin[0] + (int)threadIdx.x, y = s_origin[1] + (int)threadIdx.y;
-    if (x >= J.width || y >= J.height) return;
+    if (x >= J.dst.width || y >= J.dst.height) return;
     const float pcx = (float)x + 0.5f, pcy = (float)y + 0.5f;
     uchar4 o = make_uchar4(0, 0, 0, 0);
     for (int i = 0; i < J.n_planes; i++) {
@@ -1712,10 +1695,10 @@ __global__ void __launch_bounds__(256) k_web(const WebJob *__restrict__ jobs, co
         if (x < P.px0 || x >= P.px1 || y < P.py0 || y >= P.py1) continue;
         bool exact;
         uchar4 texel;
-        const float4 s = sample_node(T, &P.tex, J.mode, (pcx - P.left) / P.width, (pcy - P.top) / P.height, exact, texel);
-        o = blend(T, J.mode, o, s);
+        const float4 s = sample_node(T, &P.tex, J.dst.mode, (pcx - P.left) / P.width, (pcy - P.top) / P.height, exact, texel);
+        o = blend(T, J.dst.mode, o, s);
     }
-    reinterpret_cast<uchar4 *>(J.out + (size_t)y * J.out_pitch)[x] = o;
+    reinterpret_cast<uchar4 *>(J.dst.out + (size_t)y * J.dst.out_pitch)[x] = o;
 }
 
 int launch_web(const WebJob *jobs_dev, const int32_t *tile_begin_dev, int n_jobs, int n_tiles, Stream s) {

@@ -225,24 +225,26 @@ struct GlyphDev {
     uint8_t color[4];             // straight-alpha sRGB colour
     int32_t content;              // 0 colour atlas (RGBA8), 1 mask atlas (R8)
 };
-struct TextJob {
+// The node texture a node job draws: width x height RGBA8 at `out`, written through the mode's view
+struct NodeTarget {
     int32_t width, height;
-    int32_t mode;                 // 0 GpuOptimized (sRGB node texture), 1 CpuOptimized
+    int32_t mode;                 // 0 GpuOptimized (sRGB views), 1 CpuOptimized
+    uint8_t *out; int32_t out_pitch;
+};
+struct TextJob {
+    NodeTarget dst;
     int32_t color_mode;           // glyphon ColorMode: 0 Accurate (colours -> linear, colour atlas sRGB), 1 Web
     int32_t n_glyphs;
     float bg[4];                  // premultiplied shader colour of the clear (wgpu/utils.rs:51-71)
     const GlyphDev *glyphs;
     const uint8_t *mask; int32_t mask_w, mask_h, mask_pitch;
     const uint8_t *color; int32_t color_w, color_h, color_pitch;
-    uint8_t *out; int32_t out_pitch;
 };
 
 // ImageNode::render (transformations/image.rs:178-187): one asset frame drawn into a node texture of the node's resolution
 struct ImageJob {
-    int32_t width, height;        // the node texture
-    int32_t mode;                 // 0 GpuOptimized (sRGB views), 1 CpuOptimized
+    NodeTarget dst;               // the node's resolution
     Tex src;                      // the frame: TEX_RGBA8, straight alpha
-    uint8_t *out; int32_t out_pitch;
 };
 
 // One plane of WebRendererShader::render (web_renderer/shader.rs:53-114): a quad of the plane mesh through its vertex
@@ -256,24 +258,20 @@ struct WebPlane {
 // WebRenderer::render (web_renderer/renderer.rs:78-99) for a node with a frame: clear to transparent, then each plane in
 // order, blended with PREMULTIPLIED_ALPHA_BLENDING through the node texture's view and stored as 8 bits
 struct WebJob {
-    int32_t width, height;        // the node texture (the instance's resolution)
-    int32_t mode;                 // 0 GpuOptimized (sRGB views), 1 CpuOptimized
+    NodeTarget dst;               // the instance's resolution
     int32_t n_planes;
     const WebPlane *planes;
-    uint8_t *out; int32_t out_pitch;
 };
 
 // ShaderNode::render (transformations/shader/node.rs, pipeline.rs:81-140) for one node: clear to transparent, then
 // max(1, n_tex) full-target planes, each pixel's smr_fragment at its centre blended with PREMULTIPLIED_ALPHA_BLENDING
 // through the node texture's view and stored as 8 bits.  The kernel is the shader module's own (shader_rt.cuh).
 struct ShaderJob {
-    int32_t width, height;        // the node texture
-    int32_t mode;                 // 0 GpuOptimized (sRGB views), 1 CpuOptimized
+    NodeTarget dst;               // the node's resolution
     int32_t n_tex;                // texture_count: the children, in order
     float time;                   // BaseShaderParameters::time, pts as Duration::as_secs_f32
     const Tex *tex;               // n_tex child textures (TEX_NONE: the empty view), in the parameter arena
     const uint8_t *params;        // ShaderParam::to_bytes, in the parameter arena (null: no parameter)
-    uint8_t *out; int32_t out_pitch;
 };
 
 // host tables pushed once per device (numeric contract NC-1/3/4)

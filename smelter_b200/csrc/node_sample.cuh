@@ -344,3 +344,14 @@ __device__ __forceinline__ int tile_job(const int32_t *__restrict__ tile_begin, 
     }
     return lo;
 }
+
+// Thread (0, 0) of such a launch: the block's job copied to the caller's shared `J`, and its 32 x 8 tile's origin
+template <class Job>
+__device__ __forceinline__ void load_block_job(const Job *__restrict__ jobs, const int32_t *__restrict__ tile_begin, int n_jobs,
+                                               Job &J, int *origin) {
+    const int b = (int)blockIdx.x, lo = tile_job(tile_begin, n_jobs, b);
+    J = jobs[lo];
+    const int t = b - tile_begin[lo], tiles_x = (J.dst.width + 31) / 32;
+    origin[0] = (t % tiles_x) * 32;
+    origin[1] = (t / tiles_x) * 8;
+}

@@ -429,46 +429,46 @@ class Renderer {
         int node_tex = -1;      // index in the tick's texture table of the materialised RGBA8 node texture
         int raw_tex = -1;       // index of the virtual (fused K1/K2) texture
     };
-    // A Text component of an output's scene (TextRendererNode, transformations/text_renderer.rs): its node texture and the
-    // job that draws it.  The texture, the glyphs and the atlases live in device memory allocated and freed in the order of
-    // stream_, so the ticks submitted before a scene update finish reading them before they are released.
-    struct TextNode {
-        Input in;               // the node texture as a layout child: TEX_RGBA8 of width x height (1 x 1 for 0 x 0), always live
+    // A component node of an output's scene: its node texture as a layout child (premultiplied TEX_RGBA8, always live) and
+    // the device memory behind it, allocated and freed in the order of stream_, so the ticks submitted before a scene update
+    // finish reading it before it is released
+    struct NodeTexture {
+        Input in;
+        std::shared_ptr<void> mem;
+    };
+    // A Text component (TextRendererNode, transformations/text_renderer.rs): width x height (1 x 1 for 0 x 0), its glyphs
+    // after the texture in `mem`
+    struct TextNode : NodeTexture {
         dev::TextJob job = {};  // draws `in.tex`
-        std::shared_ptr<void> mem, atlas[2];   // texture + glyphs; the mask and colour atlases (shared within the scene)
+        std::shared_ptr<void> atlas[2];   // the mask and colour atlases (shared within the scene)
         bool rendered = false;  // drawn since the last smr_update_scene of the output (`was_rendered`)
     };
-    // An Image component of an output's scene (ImageNode, transformations/image.rs:137-187).  The node texture persists
-    // across ticks and is rewritten, in the order of stream_, by the ticks whose frame differs from the one it holds.
-    struct ImageNode {
-        Input in;               // the node texture as a layout child: premultiplied TEX_RGBA8 of the node's resolution, always live
+    // An Image component (ImageNode, transformations/image.rs:137-187).  The node texture persists across ticks and is
+    // rewritten, in the order of stream_, by the ticks whose frame differs from the one it holds.
+    struct ImageNode : NodeTexture {
         ImageParams params;
         dev::ImageJob job = {}; // draws `in.tex` from the frame job.src
-        std::shared_ptr<void> mem;
         int held = -1;          // the frame `in.tex` holds (-1: not drawn since the last smr_update_scene of the output)
         int held_before = -1;   // `held` when the current tick planned its draw
     };
-    // A WebView component of an output's scene (WebRendererNode, transformations/web_renderer/node.rs).  The node texture is
-    // cleared when the node is made and redrawn, in the order of stream_, by every tick while the instance has a frame.
-    struct WebNode {
-        Input in;               // the node texture as a layout child: premultiplied TEX_RGBA8 of the instance's size, always live
+    // A WebView component (WebRendererNode, transformations/web_renderer/node.rs), of the instance's size.  The node
+    // texture is cleared when the node is made and redrawn, in the order of stream_, by every tick while the instance has a
+    // frame.
+    struct WebNode : NodeTexture {
         WebParams params;
         dev::WebJob job = {};   // draws `in.tex`; its planes are this tick's, packed into the parameter arena
         std::vector<dev::WebPlane> planes;
         size_t planes_off = 0;
-        std::shared_ptr<void> mem;
     };
-    // A Shader component of an output's scene (ShaderNode, transformations/shader/node.rs).  The node texture persists and
-    // is redrawn, in the order of stream_, by every tick.
+    // A Shader component (ShaderNode, transformations/shader/node.rs).  The node texture persists and is redrawn, in the
+    // order of stream_, by every tick.
     struct Output;
-    struct ShaderNode {
-        Input in;               // the node texture as a layout child: premultiplied TEX_RGBA8 of the node's resolution, always live
+    struct ShaderNode : NodeTexture {
         ShaderParams params;
         Output *owner = nullptr;   // the output whose nodes its children are (set when a tick plans it)
         dev::ShaderJob job = {};   // draws `in.tex`; its textures and parameter bytes are this tick's, in the parameter arena
         std::vector<dev::Tex> tex;
         size_t tex_off = 0, params_off = SIZE_MAX;
-        std::shared_ptr<void> mem;
     };
     struct Output {
         OutputNode node;
@@ -494,7 +494,7 @@ class Renderer {
         std::vector<uint32_t> tile_list;         // tiles that are left for the composite, most expensive first
         bool flat = false;
         Resolution flat_root;
-        std::vector<std::string> flat_children;
+        std::vector<NodeRef> flat_children;      // Input refs
         std::vector<RenderLayout> flat_layouts;
     };
     struct WeightKey {
@@ -529,7 +529,8 @@ class Renderer {
         for (size_t i = 0; i < recs.size(); i++) memcpy(param_host_.data() + off + i * sizeof(Dev), &(recs[i].*dev), sizeof(Dev));
         return off;
     }
-    // the jobs of the node textures one launch draws, and the prefix table of their 32 x 8 tile counts (launch_text, launch_image)
+    // the jobs of the node textures one launch draws, and the prefix table of their 32 x 8 tile counts (launch_text,
+    // launch_image, launch_web, launch_shader)
     struct TileJobs { size_t jobs_off, begin_off; int n_tiles; };
     template <class Node, class Job> TileJobs param_put_tile_jobs(const std::vector<Node *> &nodes, Job Node::*job) {
         std::vector<int32_t> begin(1, 0);
@@ -537,7 +538,7 @@ class Renderer {
         for (size_t i = 0; i < nodes.size(); i++) {
             const Job &j = nodes[i]->*job;
             memcpy(param_host_.data() + jobs_off + i * sizeof(Job), &j, sizeof(Job));
-            begin.push_back(begin.back() + dev::node_tiles(j.width, j.height));
+            begin.push_back(begin.back() + dev::node_tiles(j.dst.width, j.dst.height));
         }
         return {jobs_off, param_put(begin.data(), sizeof(int32_t) * begin.size()), begin.back()};
     }
@@ -556,7 +557,7 @@ class Renderer {
     std::vector<RenderLayout> output_layouts(const Output &o, OutputNode &node, uint64_t pts,
                                              const std::vector<std::optional<Resolution>> &child_res, Resolution root);
     smr_status plan_output(Output &o, smr_output_frame &of, uint64_t pts);
-    Input *child_input(Output &o, const NodeChild &ch);
+    Input *node_input(Output &o, const NodeRef &r);
     smr_status plan_layers(std::vector<RenderLayout> &layouts, const std::vector<Input *> &child_in, int W, int H,
                            std::vector<dev::LayerDev> &layers, std::vector<dev::MaskDev> &masks);
     smr_status plan_layout_node(Output &o, size_t k, uint64_t pts);
@@ -643,6 +644,7 @@ class Renderer {
             resample_cache.clear();
         }
     } plan_;
+    smr_status make_node_texture(int w, int h, bool clear, size_t extra_bytes, NodeTexture &n, dev::NodeTarget &t);
     using AtlasUploads = std::map<const TextAtlas *, std::shared_ptr<void>>;
     smr_status make_text_node(const std::shared_ptr<const TextPayload> &p, AtlasUploads &atlases, std::unique_ptr<TextNode> &out);
     smr_status make_image_node(const ImageParams &p, std::unique_ptr<ImageNode> &out);
@@ -1104,20 +1106,16 @@ smr_status Renderer::update_scene(const char *output_id, uint32_t w, uint32_t h,
     std::vector<std::unique_ptr<WebNode>> webs;
     std::vector<std::unique_ptr<ShaderNode>> shaders;
     smr_status image_st = SMR_OK;
-    auto make_images = [&](OutputNode &n) {
-        for (const ImageParams &p : n.images) {
-            images.emplace_back();
-            if ((image_st = make_image_node(p, images.back())) != SMR_OK) return false;
-        }
-        for (const WebParams &p : n.webs) {
-            webs.emplace_back();
-            if ((image_st = make_web_node(p, webs.back())) != SMR_OK) return false;
-        }
-        for (const ShaderParams &p : n.shaders) {
-            shaders.emplace_back();
-            if ((image_st = make_shader_node(p, shaders.back())) != SMR_OK) return false;
+    auto make_all = [&](const auto &params, auto &nodes, auto make) {
+        for (const auto &p : params) {
+            nodes.emplace_back();
+            if ((image_st = (this->*make)(p, nodes.back())) != SMR_OK) return false;
         }
         return true;
+    };
+    auto make_images = [&](OutputNode &n) {
+        return make_all(n.images, images, &Renderer::make_image_node) && make_all(n.webs, webs, &Renderer::make_web_node) &&
+               make_all(n.shaders, shaders, &Renderer::make_shader_node);
     };
     if (!scene_.update_scene(output_id, c, {w, h}, node, err, make_images)) {
         if (image_st != SMR_OK) return image_st;
@@ -1139,42 +1137,54 @@ smr_status Renderer::update_scene(const char *output_id, uint32_t w, uint32_t h,
     return SMR_OK;
 }
 
-// A text node for `p`: the node texture (1 x 1 for 0 x 0), and on a device handle the texture, glyph and atlas memory and
-// the job that draws it.  Host memory is copied on stream_ (pageable sources: staged before the call returns).
+// The bytes of a w x h node texture in its allocation, rounded up so that what follows it stays aligned
+static size_t node_texture_bytes(int w, int h) { return ((size_t)w * h * 4 + 255) & ~(size_t)255; }
+
+// A w x h node texture: `n.in` as a layout child and `t`, the target of the job that draws it.  On a device handle its
+// memory, with `extra_bytes` more after the texture (at node_texture_bytes), is allocated on stream_, and with `clear` the
+// texture is cleared to transparent there.
+smr_status Renderer::make_node_texture(int w, int h, bool clear, size_t extra_bytes, NodeTexture &n, dev::NodeTarget &t) {
+    Input &in = n.in;
+    in.has_frame = true;
+    in.res = {(size_t)w, (size_t)h};
+    in.tex.kind = dev::TEX_RGBA8; in.tex.width = w; in.tex.height = h; in.tex.pitch0 = w * 4;
+    t.width = w; t.height = h; t.mode = opts_.rendering_mode; t.out_pitch = w * 4;
+    if (host_only_) return SMR_OK;
+    if (smr_status st = alloc_on_stream(node_texture_bytes(w, h) + extra_bytes, n.mem); st != SMR_OK) return st;
+    in.tex.p0 = t.out = (uint8_t *)n.mem.get();
+    if (clear) CUDA_OK(cudaMemsetAsync(t.out, 0, (size_t)w * h * 4, stream_));
+    return SMR_OK;
+}
+
+// A text node for `p`: the node texture (1 x 1 for 0 x 0), and on a device handle the glyph and atlas memory and the job
+// that draws it.  Host memory is copied on stream_ (pageable sources: staged before the call returns).
 smr_status Renderer::make_text_node(const std::shared_ptr<const TextPayload> &p, AtlasUploads &atlases,
                                     std::unique_ptr<TextNode> &out) {
     auto t = std::make_unique<TextNode>();
     const bool empty = p->width == 0 || p->height == 0;
     const int w = empty ? 1 : (int)p->width, h = empty ? 1 : (int)p->height;
-    Input &in = t->in;
-    in.has_frame = true;
-    in.res = {(size_t)w, (size_t)h};
-    in.tex.kind = dev::TEX_RGBA8; in.tex.width = w; in.tex.height = h; in.tex.pitch0 = w * 4;
     dev::TextJob &J = t->job;
-    J.width = w; J.height = h; J.mode = opts_.rendering_mode; J.color_mode = p->color_mode;
+    J.color_mode = p->color_mode;
     if (!empty) {   // 0 x 0: a transparent clear and no glyphs
         J.n_glyphs = (int)p->glyphs.size();
         shader_color(p->background, J.bg);
     }
+    const size_t glyph_bytes = sizeof(smr_glyph) * (size_t)J.n_glyphs;
+    if (smr_status st = make_node_texture(w, h, false, glyph_bytes, *t, J.dst); st != SMR_OK) return st;
     if (host_only_) { out = std::move(t); return SMR_OK; }
     cudaStream_t s = stream_;
-    auto alloc = [&](size_t bytes, std::shared_ptr<void> &buf) { return alloc_on_stream(bytes, buf); };
-    const size_t tex_bytes = ((size_t)w * h * 4 + 255) & ~(size_t)255, glyph_bytes = sizeof(smr_glyph) * (size_t)J.n_glyphs;
-    if (smr_status st = alloc(tex_bytes + glyph_bytes, t->mem); st != SMR_OK) return st;
-    uint8_t *base = (uint8_t *)t->mem.get();
-    in.tex.p0 = base;
-    J.out = base; J.out_pitch = w * 4;
     if (J.n_glyphs) {
-        CUDA_OK(cudaMemcpyAsync(base + tex_bytes, p->glyphs.data(), glyph_bytes, cudaMemcpyHostToDevice, s));
+        uint8_t *glyphs = J.dst.out + node_texture_bytes(w, h);
+        CUDA_OK(cudaMemcpyAsync(glyphs, p->glyphs.data(), glyph_bytes, cudaMemcpyHostToDevice, s));
         stats_.h2d_bytes += glyph_bytes;
-        J.glyphs = reinterpret_cast<const dev::GlyphDev *>(base + tex_bytes);
+        J.glyphs = reinterpret_cast<const dev::GlyphDev *>(glyphs);
     }
     const TextAtlas *atl[2] = {p->mask.get(), p->color.get()};
     for (int k = 0; k < 2; k++) {
         if (!atl[k] || empty) continue;
         std::shared_ptr<void> &buf = atlases[atl[k]];   // one upload per atlas of the scene
         if (!buf) {
-            if (smr_status st = alloc(atl[k]->data.size(), buf); st != SMR_OK) return st;
+            if (smr_status st = alloc_on_stream(atl[k]->data.size(), buf); st != SMR_OK) return st;
             CUDA_OK(cudaMemcpyAsync(buf.get(), atl[k]->data.data(), atl[k]->data.size(), cudaMemcpyHostToDevice, s));
             stats_.h2d_bytes += atl[k]->data.size();
         }
@@ -1191,19 +1201,11 @@ smr_status Renderer::make_text_node(const std::shared_ptr<const TextPayload> &p,
 smr_status Renderer::make_image_node(const ImageParams &p, std::unique_ptr<ImageNode> &out) {
     auto n = std::make_unique<ImageNode>();
     n->params = p;
-    const int w = (int)p.resolution.width, h = (int)p.resolution.height;
-    Input &in = n->in;
-    in.has_frame = true;
-    in.res = p.resolution;
-    in.tex.kind = dev::TEX_RGBA8; in.tex.width = w; in.tex.height = h; in.tex.pitch0 = w * 4;
     dev::ImageJob &J = n->job;
-    J.width = w; J.height = h; J.mode = opts_.rendering_mode; J.out_pitch = w * 4;
     J.src.kind = dev::TEX_RGBA8; J.src.width = (int)p.asset->width; J.src.height = (int)p.asset->height;
     J.src.pitch0 = (int)p.asset->width * 4;
-    if (!host_only_) {
-        if (smr_status st = alloc_on_stream((size_t)w * h * 4, n->mem); st != SMR_OK) return st;
-        in.tex.p0 = J.out = (uint8_t *)n->mem.get();
-    }
+    if (smr_status st = make_node_texture((int)p.resolution.width, (int)p.resolution.height, false, 0, *n, J.dst); st != SMR_OK)
+        return st;
     out = std::move(n);
     return SMR_OK;
 }
@@ -1212,18 +1214,8 @@ smr_status Renderer::make_image_node(const ImageParams &p, std::unique_ptr<Image
 smr_status Renderer::make_web_node(const WebParams &p, std::unique_ptr<WebNode> &out) {
     auto n = std::make_unique<WebNode>();
     n->params = p;
-    const int w = (int)p.instance->width, h = (int)p.instance->height;
-    Input &in = n->in;
-    in.has_frame = true;
-    in.res = {(size_t)w, (size_t)h};
-    in.tex.kind = dev::TEX_RGBA8; in.tex.width = w; in.tex.height = h; in.tex.pitch0 = w * 4;
-    dev::WebJob &J = n->job;
-    J.width = w; J.height = h; J.mode = opts_.rendering_mode; J.out_pitch = w * 4;
-    if (!host_only_) {
-        if (smr_status st = alloc_on_stream((size_t)w * h * 4, n->mem); st != SMR_OK) return st;
-        in.tex.p0 = J.out = (uint8_t *)n->mem.get();
-        CUDA_OK(cudaMemsetAsync(J.out, 0, (size_t)w * h * 4, stream_));
-    }
+    if (smr_status st = make_node_texture((int)p.instance->width, (int)p.instance->height, true, 0, *n, n->job.dst); st != SMR_OK)
+        return st;
     out = std::move(n);
     return SMR_OK;
 }
@@ -1232,19 +1224,9 @@ smr_status Renderer::make_web_node(const WebParams &p, std::unique_ptr<WebNode> 
 smr_status Renderer::make_shader_node(const ShaderParams &p, std::unique_ptr<ShaderNode> &out) {
     auto n = std::make_unique<ShaderNode>();
     n->params = p;
-    const int w = (int)p.resolution.width, h = (int)p.resolution.height;
-    Input &in = n->in;
-    in.has_frame = true;
-    in.res = p.resolution;
-    in.tex.kind = dev::TEX_RGBA8; in.tex.width = w; in.tex.height = h; in.tex.pitch0 = w * 4;
-    dev::ShaderJob &J = n->job;
-    J.width = w; J.height = h; J.mode = opts_.rendering_mode; J.out_pitch = w * 4;
-    J.n_tex = (int)p.children.size();
-    if (!host_only_) {
-        if (smr_status st = alloc_on_stream((size_t)w * h * 4, n->mem); st != SMR_OK) return st;
-        in.tex.p0 = J.out = (uint8_t *)n->mem.get();
-        CUDA_OK(cudaMemsetAsync(J.out, 0, (size_t)w * h * 4, stream_));
-    }
+    n->job.n_tex = (int)p.children.size();
+    if (smr_status st = make_node_texture((int)p.resolution.width, (int)p.resolution.height, true, 0, *n, n->job.dst); st != SMR_OK)
+        return st;
     out = std::move(n);
     return SMR_OK;
 }
@@ -1296,13 +1278,7 @@ void Renderer::plan_web_node(Output &o, WebNode &n) {
         const float tx = -((float)W / 2.0f) + (r[0] + r[2] / 2.0f), ty = (float)H / 2.0f - (r[1] + r[3] / 2.0f);
         dev::WebPlane pl;
         if (!web_plane(a * (sx * (r[2] / (float)W)), a * tx, b * (sy * (r[3] / (float)H)), b * ty, W, H, pl)) continue;
-        const NodeChild &ch = n.params.children[k];
-        if (ch.text >= 0) pl.tex = o.texts[ch.text]->in.tex;
-        else if (ch.image >= 0) pl.tex = o.images[ch.image]->in.tex;
-        else {   // an input without a live frame samples the empty view
-            auto it = inputs_.find(ch.input_id);
-            if (it != inputs_.end() && it->second.has_frame) pl.tex = it->second.tex;
-        }
+        if (const Input *in = node_input(o, n.params.children[k])) pl.tex = in->tex;   // else the empty view
         n.planes.push_back(pl);
     }
     if (site_ok && w.embedding == SMR_WEB_NATIVE_UNDER_CONTENT) n.planes.push_back(site);
@@ -1326,19 +1302,20 @@ void Renderer::plan_shader_node(Output &o, ShaderNode &n, uint64_t pts) {
 void Renderer::plan_node_textures(Output &o, uint64_t pts) {
     if (o.flat || o.nodes_planned == tick_) return;
     o.nodes_planned = tick_;
+    auto enter = [&](NodeTexture &n) {
+        n.in.node_tex = -1;
+        n.in.raw_tex = add_texture(n.in.tex, false);
+    };
     for (auto &n : o.webs) {
-        n->in.node_tex = -1;
-        n->in.raw_tex = add_texture(n->in.tex, false);
+        enter(*n);
         plan_web_node(o, *n);
     }
     for (auto &n : o.shaders) {   // every tick draws every shader node (ShaderNode::render has no cache)
-        n->in.node_tex = -1;
-        n->in.raw_tex = add_texture(n->in.tex, false);
+        enter(*n);
         plan_shader_node(o, *n, pts);
     }
     for (auto &n : o.images) {
-        n->in.node_tex = -1;
-        n->in.raw_tex = add_texture(n->in.tex, false);
+        enter(*n);
         const ImageAsset &a = *n->params.asset;
         const int frame = a.animated() ? (int)a.frame_at(pts, n->params.start_pts) : 0;
         if (frame == n->held) continue;
@@ -1348,8 +1325,7 @@ void Renderer::plan_node_textures(Output &o, uint64_t pts) {
         plan_.images.push_back(n.get());
     }
     for (auto &t : o.texts) {
-        t->in.node_tex = -1;
-        t->in.raw_tex = add_texture(t->in.tex, false);
+        enter(*t);
         if (t->rendered) continue;
         t->rendered = true;   // undone if the tick fails before its launch
         plan_.texts.push_back(t.get());
@@ -1401,16 +1377,12 @@ smr_status Renderer::set_layouts(const char *output_id, uint32_t w, uint32_t h, 
     o.format = fmt;
     o.res = {w, h};
     o.flat = true;
-    if ((!o.texts.empty() || !o.images.empty() || !o.webs.empty() || !o.shaders.empty()) && !host_only_)
-        CUDA_OK(cudaSetDevice(opts_.cuda_device));
-    o.texts.clear();
-    o.images.clear();
-    o.webs.clear();
-    o.shaders.clear();
+    if (!host_only_) CUDA_OK(cudaSetDevice(opts_.cuda_device));   // the memory of the replaced nodes is released on stream_
+    o.texts.clear(); o.images.clear(); o.webs.clear(); o.shaders.clear();
     o.nested.clear();
     o.flat_root = {root_w, root_h};
     o.flat_children.clear();
-    for (uint32_t i = 0; i < n_children; i++) o.flat_children.push_back(child_ids[i] ? child_ids[i] : "");
+    for (uint32_t i = 0; i < n_children; i++) o.flat_children.push_back({NodeRef::Input, -1, child_ids[i] ? child_ids[i] : ""});
     o.flat_layouts = std::move(ls);
     return SMR_OK;
 }
@@ -1990,7 +1962,7 @@ smr_status Renderer::render_text(uint32_t w, uint32_t h, smr_rgba bg, const smr_
         else { set_error("glyph content type must be SMR_GLYPH_COLOR or SMR_GLYPH_MASK"); return SMR_ERR_INVALID_ARGUMENT; }
     }
     dev::TextJob J = {};
-    J.width = (int)w; J.height = (int)h; J.mode = opts_.rendering_mode; J.color_mode = color_mode; J.n_glyphs = (int)n;
+    J.dst.width = (int)w; J.dst.height = (int)h; J.dst.mode = opts_.rendering_mode; J.color_mode = color_mode; J.n_glyphs = (int)n;
     shader_color(RGBA{bg.r, bg.g, bg.b, bg.a}, J.bg);
     const smr_atlas *atl[2] = {mask, color};
     const bool need[2] = {need_mask, need_color};
@@ -2024,7 +1996,7 @@ smr_status Renderer::render_text(uint32_t w, uint32_t h, smr_rgba bg, const smr_
     const int32_t begin[2] = {0, dev::node_tiles((int)w, (int)h)};
     CUDA_OK(text_job_.ensure(begin_off + sizeof(begin)));
     return write_rgba(rgba, pitch, mem_kind, w, h, [&](uint8_t *dst, int dpitch) {
-        J.out = dst; J.out_pitch = dpitch;
+        J.dst.out = dst; J.dst.out_pitch = dpitch;
         // pageable sources: staged before the copies return; write_rgba waits for the launch
         if (cudaMemcpyAsync(text_job_.p, &J, sizeof(J), cudaMemcpyHostToDevice, stream_) != cudaSuccess ||
             cudaMemcpyAsync(text_job_.p + begin_off, begin, sizeof(begin), cudaMemcpyHostToDevice, stream_) != cudaSuccess)
@@ -2229,34 +2201,30 @@ void Renderer::plan_tiles(Output &o, CompositeRec &pc, const std::vector<dev::La
     }
 }
 
-// An output's children at `pts` (sources[i].resolution(), layout.rs:176-179): the input or text node behind each (nullptr:
-// an input without a live frame) and its resolution.  Returns the root resolution.
+// An output's children at `pts` (sources[i].resolution(), layout.rs:176-179): the Input behind each (node_input) and its
+// resolution.  Returns the root resolution.
 Resolution Renderer::output_children(const Output &o, const OutputNode &node, uint64_t pts, std::vector<Input *> &child_in,
                                      std::vector<std::optional<Resolution>> &child_res) {
-    auto add = [&](Input *in) {
+    for (const NodeRef &r : o.flat ? o.flat_children : node.children) {
+        Input *in = node_input(const_cast<Output &>(o), r);
         child_in.push_back(in);
         child_res.push_back(in ? std::optional<Resolution>(in->res) : std::nullopt);
-    };
-    auto input = [&](const std::string &id) {
-        auto it = inputs_.find(id);
-        return it != inputs_.end() && it->second.has_frame ? &it->second : nullptr;
-    };
-    if (o.flat)
-        for (const std::string &id : o.flat_children) add(input(id));
-    else
-        for (const NodeChild &ch : node.children) add(child_input(const_cast<Output &>(o), ch));
+    }
     return o.flat ? o.flat_root : node.layout_resolution(pts);
 }
 
-// The Input behind a node child: a text, image, web, shader or layout node's texture, or a caller's input; nullptr when it
+// The Input behind a render node: a text, image, web, shader or layout node's texture, or a caller's input; nullptr when it
 // has no pixels this tick (an input without a live frame, a layout node of no size), which reads as the empty view
-Renderer::Input *Renderer::child_input(Output &o, const NodeChild &ch) {
-    if (ch.text >= 0) return &o.texts[ch.text]->in;
-    if (ch.image >= 0) return &o.images[ch.image]->in;
-    if (ch.web >= 0) return &o.webs[ch.web]->in;
-    if (ch.shader >= 0) return &o.shaders[ch.shader]->in;
-    if (ch.layout >= 0) return (size_t)ch.layout < o.nested.size() && o.nested[ch.layout].has_frame ? &o.nested[ch.layout] : nullptr;
-    auto it = inputs_.find(ch.input_id);
+Renderer::Input *Renderer::node_input(Output &o, const NodeRef &r) {
+    switch (r.kind) {
+        case NodeRef::Text: return &o.texts[r.index]->in;
+        case NodeRef::Image: return &o.images[r.index]->in;
+        case NodeRef::Web: return &o.webs[r.index]->in;
+        case NodeRef::Shader: return &o.shaders[r.index]->in;
+        case NodeRef::Layout: return (size_t)r.index < o.nested.size() && o.nested[r.index].has_frame ? &o.nested[r.index] : nullptr;
+        case NodeRef::Input: break;
+    }
+    auto it = inputs_.find(r.input_id);
     return it != inputs_.end() && it->second.has_frame ? &it->second : nullptr;
 }
 
@@ -2380,8 +2348,8 @@ smr_status Renderer::plan_layout_node(Output &o, size_t k, uint64_t pts) {
     nn.node_tex = nn.raw_tex = -1;
     std::vector<Input *> child_in;
     std::vector<std::optional<Resolution>> child_res;
-    for (const NodeChild &ch : lp.children) {
-        Input *in = child_input(o, ch);
+    for (const NodeRef &ch : lp.children) {
+        Input *in = node_input(o, ch);
         child_in.push_back(in);
         child_res.push_back(in ? std::optional<Resolution>(in->res) : std::nullopt);
     }
@@ -2460,21 +2428,8 @@ smr_status Renderer::plan_output(Output &o, smr_output_frame &of, uint64_t pts) 
     };
 
     plan_node_textures(o, pts);
-    if (!o.flat && (o.node.root_is_input || o.node.root_text >= 0 || o.node.root_image >= 0 || o.node.root_web >= 0 ||
-                    o.node.root_shader >= 0)) {  // pass-through: the root texture IS the node texture
-        Input *root_in = nullptr;
-        if (o.node.root_text >= 0) {
-            root_in = &o.texts[o.node.root_text]->in;
-        } else if (o.node.root_image >= 0) {
-            root_in = &o.images[o.node.root_image]->in;
-        } else if (o.node.root_web >= 0) {
-            root_in = &o.webs[o.node.root_web]->in;
-        } else if (o.node.root_shader >= 0) {
-            root_in = &o.shaders[o.node.root_shader]->in;
-        } else {
-            auto it = inputs_.find(o.node.root_input_id);
-            if (it != inputs_.end() && it->second.has_frame) root_in = &it->second;
-        }
+    if (!o.flat && o.node.root) {  // pass-through: the root texture IS the node texture
+        Input *root_in = node_input(o, *o.node.root);
         if (!root_in) { push_fill(); return SMR_OK; }
         Input &in = *root_in;
         if (o.format == SMR_OUT_RGBA8 && (in.res.width != o.res.width || in.res.height != o.res.height)) {
@@ -2751,9 +2706,9 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
         for (ShaderNode *n : plan_.shaders) {   // the children's textures, frame-arena addresses resolved
             n->tex.assign(n->params.children.size(), dev::Tex());
             for (size_t k = 0; k < n->params.children.size(); k++) {
-                const NodeChild &ch = n->params.children[k];
-                Input *in = child_input(*n->owner, ch);
-                if (in) n->tex[k] = ch.layout >= 0 ? plan_.tex[in->raw_tex].tex : in->tex;
+                const NodeRef &ch = n->params.children[k];
+                Input *in = node_input(*n->owner, ch);
+                if (in) n->tex[k] = ch.kind == NodeRef::Layout ? plan_.tex[in->raw_tex].tex : in->tex;
             }
             n->tex_off = param_put(n->tex.data(), sizeof(dev::Tex) * n->tex.size());
             const std::vector<uint8_t> &b = n->params.param_bytes;
@@ -3309,8 +3264,7 @@ smr_status Renderer::debug_layouts(const char *output_id, uint64_t pts, smr_rend
     if (it == outputs_.end()) { set_error("output not registered"); return SMR_ERR_OUTPUT_NOT_REGISTERED; }
     Output &o = it->second;
     *n = 0;
-    if (!o.flat && (o.node.root_is_input || o.node.root_text >= 0 || o.node.root_image >= 0 || o.node.root_web >= 0 ||
-                    o.node.root_shader >= 0)) {
+    if (!o.flat && o.node.root) {
         if (rw) *rw = 0;
         if (rh) *rh = 0;
         return SMR_OK;
@@ -3333,20 +3287,19 @@ smr_status Renderer::debug_node_layouts(const char *output_id, uint32_t node, ui
         auto it = outputs_.find(output_id);
         if (it == outputs_.end()) { set_error("output not registered"); return SMR_ERR_OUTPUT_NOT_REGISTERED; }
         Output &o = it->second;
-        const bool root_layout = !o.flat && !o.node.root_is_input && o.node.root_text < 0 && o.node.root_image < 0 &&
-                                 o.node.root_web < 0 && o.node.root_shader < 0;
+        const bool root_layout = !o.flat && !o.node.root;
         if (!(root_layout && node == 0)) {
             const size_t k = node - (root_layout ? 1 : 0);
             if (o.flat || k >= o.node.nested.size()) { set_error("no such layout node"); return SMR_ERR_INVALID_ARGUMENT; }
             LayoutParams copy = o.node.nested[k];   // do not advance Tiles::last_layout
             std::vector<std::optional<Resolution>> child_res;
-            for (const NodeChild &ch : copy.children) {
-                if (ch.layout >= 0) {   // a layout node's texture has its resolution at pts
-                    const Resolution r = o.node.nested[ch.layout].resolution(pts);
+            for (const NodeRef &ch : copy.children) {
+                if (ch.kind == NodeRef::Layout) {   // a layout node's texture has its resolution at pts
+                    const Resolution r = o.node.nested[ch.index].resolution(pts);
                     const bool ok = r.width && r.height && r.width <= 16384 && r.height <= 16384;
                     child_res.push_back(ok ? std::optional<Resolution>(r) : std::nullopt);
                 } else {
-                    Input *in = child_input(o, ch);
+                    Input *in = node_input(o, ch);
                     child_res.push_back(in ? std::optional<Resolution>(in->res) : std::nullopt);
                 }
             }

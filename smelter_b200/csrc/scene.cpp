@@ -1358,22 +1358,27 @@ static bool visit_web_ids(const Component &c, std::set<std::string> &ids, std::s
 // A node child of the render graph (build_tree, scene_state.rs:154-196): an input, or a text, image, web, shader or layout
 // node appended to `out`, whose own children come first in DFS order.  A layout node's size is node_size at `pts`; a layout
 // root without width and height is UnknownDimensionsForLayoutNodeRoot (scene_state.rs:206-228), reported in `err`.
-static NodeChild node_child(const Stateful &l, OutputNode &out, uint64_t pts, std::string &err) {
-    NodeChild ch;
-    auto depth_of = [&](const NodeChild &k) {
-        return k.shader >= 0 ? out.shaders[k.shader].depth : k.layout >= 0 ? out.nested[k.layout].depth : k.web >= 0 ? 1 : 0;
+static NodeRef node_child(const Stateful &l, OutputNode &out, uint64_t pts, std::string &err) {
+    NodeRef ch;
+    auto depth_of = [&](const NodeRef &k) {
+        switch (k.kind) {
+            case NodeRef::Shader: return out.shaders[k.index].depth;
+            case NodeRef::Layout: return out.nested[k.index].depth;
+            case NodeRef::Web: return 1;
+            default: return 0;
+        }
     };
     if (l.kind == Stateful::Text) {
-        ch.text = (int)out.texts.size();
+        ch = {NodeRef::Text, (int)out.texts.size()};
         out.texts.push_back(l.text);
     } else if (l.kind == Stateful::Image) {
-        ch.image = (int)out.images.size();
+        ch = {NodeRef::Image, (int)out.images.size()};
         out.images.push_back(l.image);
     } else if (l.kind == Stateful::WebView) {
         WebParams w;
         w.instance = l.web;
         for (const Stateful &c : l.children) w.children.push_back(node_child(c, out, pts, err));
-        ch.web = (int)out.webs.size();
+        ch = {NodeRef::Web, (int)out.webs.size()};
         out.webs.push_back(std::move(w));
     } else if (l.kind == Stateful::Shader) {
         ShaderParams p;
@@ -1381,11 +1386,11 @@ static NodeChild node_child(const Stateful &l, OutputNode &out, uint64_t pts, st
         if (l.shader_param) l.shader_param->to_bytes(p.param_bytes);
         p.resolution = {f32_as_usize(l.size.width), f32_as_usize(l.size.height)};
         for (const Stateful &c : l.children) {
-            const NodeChild k = node_child(c, out, pts, err);
+            const NodeRef k = node_child(c, out, pts, err);
             p.depth = std::max(p.depth, depth_of(k) + 1);
             p.children.push_back(k);
         }
-        ch.shader = (int)out.shaders.size();
+        ch = {NodeRef::Shader, (int)out.shaders.size()};
         out.shaders.push_back(std::move(p));
     } else if (l.is_layout()) {
         LayoutParams p;
@@ -1403,11 +1408,11 @@ static NodeChild node_child(const Stateful &l, OutputNode &out, uint64_t pts, st
         std::vector<const Stateful *> leaves;
         l.node_children(leaves);
         for (const Stateful *c : leaves) {
-            const NodeChild k = node_child(*c, out, pts, err);
+            const NodeRef k = node_child(*c, out, pts, err);
             p.depth = std::max(p.depth, depth_of(k) + 1);
             p.children.push_back(k);
         }
-        ch.layout = (int)out.nested.size();
+        ch = {NodeRef::Layout, (int)out.nested.size()};
         out.nested.push_back(std::move(p));
     } else {
         ch.input_id = l.input_id;
@@ -1484,19 +1489,8 @@ bool SceneState::update_scene(const std::string &output_id, const Component &roo
     err.clear();
     out = OutputNode();
     out.resolution = resolution;
-    if (st.root.kind == Stateful::Text) {
-        out.root_text = 0;
-        out.texts.push_back(st.root.text);
-    } else if (st.root.kind == Stateful::Image) {
-        out.root_image = 0;
-        out.images.push_back(st.root.image);
-    } else if (st.root.kind == Stateful::WebView) {
-        out.root_web = node_child(st.root, out, last_pts_ns_, err).web;
-    } else if (st.root.kind == Stateful::Shader) {
-        out.root_shader = node_child(st.root, out, last_pts_ns_, err).shader;
-    } else if (!st.root.is_layout()) {
-        out.root_is_input = true;
-        out.root_input_id = st.root.input_id;
+    if (!st.root.is_layout()) {
+        out.root = node_child(st.root, out, last_pts_ns_, err);
     } else {
         out.layout_root = st.root;  // the render graph owns a clone
         out.size = {(float)resolution.width, (float)resolution.height};

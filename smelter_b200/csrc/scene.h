@@ -355,14 +355,12 @@ struct Stateful {
     void update_state(const std::optional<Resolution> *inputs, size_t n);  // scene/layout.rs:105-137
 };
 
-// One child of the layout node (scene/layout.rs:95-103): an input, or text node `text` or image node `image` of the output
-struct NodeChild {
+// A render node of an output (scene/layout.rs:95-103): the caller's input `input_id`, or entry `index` of the output's
+// list of that kind (OutputNode::texts, images, webs, shaders or nested)
+struct NodeRef {
+    enum Kind { Input, Text, Image, Web, Shader, Layout } kind = Input;
+    int index = -1;
     std::string input_id;
-    int text = -1;                            // index in OutputNode::texts, or -1
-    int image = -1;                           // index in OutputNode::images, or -1
-    int web = -1;                             // index in OutputNode::webs, or -1
-    int shader = -1;                          // index in OutputNode::shaders, or -1
-    int layout = -1;                          // index in OutputNode::nested, or -1; all -1: the input `input_id`
 };
 
 // A layout node other than the output's root (scene_state.rs:154-228, NodeParams::Layout): a View, Tiles or Rescaler whose
@@ -372,7 +370,7 @@ struct NodeChild {
 struct LayoutParams {
     Stateful root;
     Size size;
-    std::vector<NodeChild> children;
+    std::vector<NodeRef> children;
     int depth = 1;
     Resolution resolution(uint64_t pts) const;   // SizedLayoutComponent::resolution (scene/layout.rs:245-257)
     NestedLayout layouts(uint64_t pts, const std::vector<std::optional<Resolution>> &inputs);
@@ -381,7 +379,7 @@ struct LayoutParams {
 // A WebView render node (state/node.rs:127-141, NodeParams::Web): the instance and its children, each its own node
 struct WebParams {
     std::shared_ptr<WebInstance> instance;
-    std::vector<NodeChild> children;          // input, text or image nodes (never `web`)
+    std::vector<NodeRef> children;            // Input, Text or Image nodes
 };
 
 // A Shader render node (state/node.rs, NodeParams::Shader): the program, the parameter bytes, the node's resolution
@@ -391,24 +389,19 @@ struct ShaderParams {
     std::shared_ptr<const ShaderProgram> shader;
     std::vector<uint8_t> param_bytes;
     Resolution resolution;
-    std::vector<NodeChild> children;
+    std::vector<NodeRef> children;
     int depth = 1;
 };
 
 // scene/scene_state.rs
 struct OutputNode {
-    bool root_is_input = false;
-    std::string root_input_id;
-    int root_text = -1;                       // the root is text node texts[root_text] (-1: it is not a Text)
+    std::optional<NodeRef> root;              // the root render node; empty: the root is a layout, `layout_root`
     Stateful layout_root;                     // LayoutNode.root.component (the render graph's clone)
     Size size;                                // SizedLayoutComponent.size
-    std::vector<NodeChild> children;          // node children, DFS order
+    std::vector<NodeRef> children;            // node children, DFS order
     std::vector<std::shared_ptr<const TextPayload>> texts;   // the output's text nodes (the root, or children in DFS order)
-    int root_image = -1;                      // the root is image node images[root_image] (-1: it is not an Image)
     std::vector<ImageParams> images;          // the output's image nodes, likewise (web view children included)
-    int root_web = -1;                        // the root is web node webs[root_web] (-1: it is not a WebView)
     std::vector<WebParams> webs;              // the output's web nodes, likewise
-    int root_shader = -1;                     // the root is shader node shaders[root_shader] (-1: it is not a Shader)
     std::vector<ShaderParams> shaders;        // the output's shader nodes, children before parents
     std::vector<LayoutParams> nested;         // the output's layout nodes below the root, DFS order, children before parents
     Resolution resolution;

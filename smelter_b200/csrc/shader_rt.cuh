@@ -44,32 +44,26 @@ extern "C" __global__ void __launch_bounds__(256) smr_shader_main(const smr::dev
     __shared__ smr::dev::Tables T;
     __shared__ smr::dev::ShaderJob J;
     __shared__ int s_origin[2];
-    if (threadIdx.x == 0 && threadIdx.y == 0) {
-        const int b = (int)blockIdx.x, lo = smr::dev::tile_job(tile_begin, n_jobs, b);
-        J = jobs[lo];
-        const int t = b - tile_begin[lo], tiles_x = (J.width + 31) / 32;
-        s_origin[0] = (t % tiles_x) * 32;
-        s_origin[1] = (t / tiles_x) * 8;
-    }
+    if (threadIdx.x == 0 && threadIdx.y == 0) smr::dev::load_block_job(jobs, tile_begin, n_jobs, J, s_origin);
     smr::dev::load_tables(T);   // ends in __syncthreads
     const int x = s_origin[0] + (int)threadIdx.x, y = s_origin[1] + (int)threadIdx.y;
-    if (x >= J.width || y >= J.height) return;
+    if (x >= J.dst.width || y >= J.dst.height) return;
     smr_fragment_in in;
     in.position = make_float4((float)x + 0.5f, (float)y + 0.5f, 0.0f, 1.0f);
-    in.tex_coords = make_float2(in.position.x / (float)J.width, in.position.y / (float)J.height);
+    in.tex_coords = make_float2(in.position.x / (float)J.dst.width, in.position.y / (float)J.dst.height);
     smr_base_params base;
     base.time = J.time;
-    base.output_resolution[0] = (unsigned)J.width;
-    base.output_resolution[1] = (unsigned)J.height;
+    base.output_resolution[0] = (unsigned)J.dst.width;
+    base.output_resolution[1] = (unsigned)J.dst.height;
     base.texture_count = (unsigned)J.n_tex;
     smr_textures tex;
-    tex.T = &T; tex.tex = J.tex; tex.count = (unsigned)J.n_tex; tex.mode = J.mode;
+    tex.T = &T; tex.tex = J.tex; tex.count = (unsigned)J.n_tex; tex.mode = J.dst.mode;
     uchar4 o = make_uchar4(0, 0, 0, 0);
     const int planes = J.n_tex > 0 ? J.n_tex : 1;
     for (int p = 0; p < planes; p++) {
         base.plane_id = J.n_tex > 0 ? p : -1;
-        o = smr::dev::blend(T, J.mode, o, smr_fragment(in, base, J.params, tex));
+        o = smr::dev::blend(T, J.dst.mode, o, smr_fragment(in, base, J.params, tex));
     }
-    reinterpret_cast<uchar4 *>(J.out + (size_t)y * J.out_pitch)[x] = o;
+    reinterpret_cast<uchar4 *>(J.dst.out + (size_t)y * J.dst.out_pitch)[x] = o;
 }
 #endif
