@@ -334,8 +334,9 @@ smr_status smr_web_set_child_rects(smr_renderer *r, const char *instance_id, con
  * parameter).  tex.sample(i, uv) samples child i with the reference's sampler (linear, clamp to edge) through the node
  * texture's view: sRGB-decoded in GpuOptimized mode, raw in CpuOptimized mode, premultiplied; an index at or above
  * texture_count samples the empty view.  The returned colour is premultiplied.  The library prepends the header that
- * declares these types (smelter_b200/csrc/shader_rt.cuh).  Deliberate deviation: there is no user vertex stage; every
- * plane is the full-target quad under the identity transform, as in the reference's example shaders.
+ * declares these types (smelter_b200/csrc/shader_rt.cuh).  A CUDA shader has no user vertex stage: every plane is the
+ * full-target quad under the identity transform.  smr_register_wgsl_shader below takes the reference's WGSL instead,
+ * vertex stage included; both share this registry.
  * The source is compiled with --fmad=false and without fast math, so its arithmetic is reproducible.  NVRTC is loaded at
  * run time (libnvrtc.so.12); when it cannot be, registration answers SMR_ERR_UNSUPPORTED with the reason in
  * smr_last_error.  A compile error is SMR_ERR_INVALID_ARGUMENT (CreateShaderError) with NVRTC's log in smr_last_error.
@@ -356,6 +357,35 @@ typedef struct smr_shader_param_type {
 typedef struct { const char *source; const smr_shader_param_type *param_type; } smr_shader_spec;
 smr_status smr_register_shader(smr_renderer *r, const char *shader_id, const smr_shader_spec *spec);
 smr_status smr_unregister_shader(smr_renderer *r, const char *shader_id);
+
+/* RendererSpec::Shader(ShaderSpec { source }) as the reference takes it: `wgsl_source` is WGSL that contains the shader
+ * header (shader_header.wgsl: textures, sampler_ and base_params: BaseShaderParameters as var<immediate>) and defines
+ * @vertex vs_main(VertexInput) and @fragment fs_main returning @location(0) vec4<f32>.  It is translated to CUDA C++
+ * (smelter_b200/csrc/wgsl.cpp, against wgsl_rt.cuh) and compiled as smr_register_shader compiles, host-only handles
+ * included; it shares that registry (KeyTaken, unregistering, scenes keeping an unregistered shader).
+ * Statuses: SMR_ERR_INVALID_ARGUMENT (CreateShaderError) for WGSL that does not parse or type-check, or that fails the
+ * reference's header validation (a missing header global or one of another type, var<push_constant> for base_params,
+ * vs_main without exactly one VertexInput, a group(1) binding(0) that is not var<uniform>); smr_last_error names the
+ * line and column.  SMR_ERR_UNSUPPORTED for valid WGSL outside the subset, named in smr_last_error: derivatives
+ * (dpdx, fwidth, ...), storage buffers, atomics, override, pointers, textures and bindings other than the header's and
+ * the uniform, f16, and builtins not listed in the WGSL section of DESIGN.md.
+ * The parameter type is the uniform's WGSL type: scalars, vectors (a LIST of exactly N scalars), matrices (a LIST of
+ * exactly R rows of C scalars), arrays (a LIST of at most N) and structs, validated as validation.rs does.  The bytes
+ * stay ShaderParam::to_bytes (tight); the shader reads them at WGSL uniform-address-space offsets (AlignOf, SizeOf,
+ * array stride), as the reference's GPU reads that buffer, and bytes beyond those supplied (a short list, or no
+ * parameter) read as zero.
+ * Drawing (ShaderPipeline::render): the node texture is cleared to transparent, then max(1, texture_count) planes are
+ * drawn, plane_id -1 without children; each is the plane mesh (4 vertices, indices 0,1,2 and 2,3,0) through vs_main, a
+ * triangle list with front face counter-clockwise and back faces culled (the plane as the mesh gives it is front-facing).
+ * The rasteriser's arithmetic is the contract, stated in full at the WGSL section of smelter_b200/csrc/shader_rt.cuh:
+ * window coordinates snapped to 1/256 px; integer edge functions and the top-left rule (a pixel on an edge two triangles
+ * share is drawn once); f32 barycentrics E_i / A; perspective-correct varyings by default, @interpolate(linear) and
+ * @interpolate(flat) (the provoking vertex is the triangle's first) honoured; @builtin(position) is (x + .5, y + .5,
+ * depth, 1/w).  A fragment whose depth z/w is outside [0, 1] is not drawn.  A plane with a vertex whose clip w is not
+ * above 0, or whose window coordinate is beyond 2^20 px, is not drawn at all (there is no homogeneous clipping).
+ * `discard` leaves the pixel as it was; every other fragment is blended with PREMULTIPLIED_ALPHA_BLENDING and stored as
+ * 8 bits, through the sRGB view in GpuOptimized mode, with the same sampler and blend as a CUDA shader. */
+smr_status smr_register_wgsl_shader(smr_renderer *r, const char *shader_id, const char *wgsl_source);
 
 /* Renderer::update_scene(output_id, resolution, output_format, scene_root)   state.rs:177-188
  * Components: InputStream, View, Tiles, Rescaler, Text, Image, WebView and Shader (anywhere, the root included).  A

@@ -31,6 +31,7 @@
 #include "interior.h"
 #include "kernels.h"
 #include "scene.h"
+#include "wgsl.h"
 
 namespace smr {
 
@@ -391,6 +392,8 @@ class Renderer {
     smr_status web_set_frame(const char *id, const smr_web_frame *f);
     smr_status web_set_child_rects(const char *id, const smr_web_rect *rects, uint32_t n);
     smr_status register_shader(const char *id, const smr_shader_spec *spec);
+    smr_status register_wgsl_shader(const char *id, const char *source);
+    smr_status add_shader(const char *id, std::unique_ptr<ShaderProgram> program, const std::string &source);
     smr_status unregister_shader(const char *id);
     smr_status update_scene(const char *output_id, uint32_t w, uint32_t h, int32_t fmt, const smr_component *root);
     smr_status unregister_output(const char *id);
@@ -1015,9 +1018,29 @@ smr_status Renderer::register_shader(const char *id, const smr_shader_spec *spec
         program->param_type.emplace();
         if (!param_type_from_c(spec->param_type, *program->param_type, err, 0)) { set_error(err); return SMR_ERR_INVALID_ARGUMENT; }
     }
+    return add_shader(id, std::move(program), spec->source);
+}
+
+// WGSL: translated (wgsl.cpp), then compiled after wgsl_rt.cuh as a CUDA source is; the parameter type is the uniform's
+smr_status Renderer::register_wgsl_shader(const char *id, const char *source) {
+    if (!id || !source) return SMR_ERR_INVALID_ARGUMENT;
+    std::lock_guard<std::mutex> g(mu_);
+    if (scene_.has_shader(id)) { set_error("a shader with this id is already registered"); return SMR_ERR_INVALID_ARGUMENT; }
+    wgsl::Translation t = wgsl::translate(source);
+    if (t.status != SMR_OK) { set_error(t.error); return (smr_status)t.status; }
+    auto program = std::make_unique<ShaderProgram>();
+    program->param_type = std::move(t.param_type);
+    program->wgsl = true;
+    program->uniform_size = t.uniform_size;
+    return add_shader(id, std::move(program), std::string(kSrc_wgsl_rt) + t.cuda);
+}
+
+// Compiles `source` into `program`, loads it on a device handle and registers it as `id` (the caller holds mu_)
+smr_status Renderer::add_shader(const char *id, std::unique_ptr<ShaderProgram> program, const std::string &source) {
+    std::string err;
     if (!nvrtc_load(err)) { set_error(err); return SMR_ERR_UNSUPPORTED; }
     std::vector<std::string> tables;
-    if (!compile_shader(spec->source, program->cubin, tables, err)) { set_error(err); return SMR_ERR_INVALID_ARGUMENT; }
+    if (!compile_shader(source, program->cubin, tables, err)) { set_error(err); return SMR_ERR_INVALID_ARGUMENT; }
     if (!host_only_) {
         CUDA_OK(cudaSetDevice(opts_.cuda_device));
         reap_shaders(false);
@@ -3392,6 +3415,9 @@ smr_status smr_web_set_child_rects(smr_renderer *r, const char *id, const smr_we
     SMR_GUARD(r->impl.web_set_child_rects(id, rects, n))
 }
 smr_status smr_register_shader(smr_renderer *r, const char *id, const smr_shader_spec *spec) { SMR_GUARD(r->impl.register_shader(id, spec)) }
+smr_status smr_register_wgsl_shader(smr_renderer *r, const char *id, const char *wgsl_source) {
+    SMR_GUARD(r->impl.register_wgsl_shader(id, wgsl_source))
+}
 smr_status smr_unregister_shader(smr_renderer *r, const char *id) { SMR_GUARD(r->impl.unregister_shader(id)) }
 smr_status smr_update_scene(smr_renderer *r, const char *output_id, uint32_t w, uint32_t h, int32_t fmt,
                             const smr_component *root) { SMR_GUARD(r->impl.update_scene(output_id, w, h, fmt, root)) }

@@ -1172,7 +1172,21 @@ static bool did_child_order_change(const std::vector<Stateful> &prev, const std:
 // validate_params (transformations/shader/validation.rs:314-520) over the types a smr_shader_param_type can describe;
 // `why` names the first mismatch
 static void validate_shader_param(const ShaderParamValue &v, const ShaderParamType &t, std::string &why) {
-    static const char *names[] = {"F32", "U32", "I32", "List", "Struct"};
+    static const char *names[] = {"F32", "U32", "I32", "List", "Struct", "Vector", "Matrix"};
+    if (t.kind == kShaderParamVector || t.kind == kShaderParamMatrix) {   // validate_vector / validate_matrix (:450-520)
+        const char *what = t.kind == kShaderParamVector ? "a vector" : "a matrix";
+        if (v.kind != SMR_SHADER_PARAM_LIST) {
+            why = std::string("expected ") + what + " (a List), got " + names[v.kind];
+            return;
+        }
+        if (v.items.size() != t.length) {
+            why = std::string(what) + " needs exactly " + std::to_string(t.length) + (t.kind == kShaderParamVector ? " items" : " rows") +
+                  ", got " + std::to_string(v.items.size());
+            return;
+        }
+        for (size_t i = 0; i < v.items.size() && why.empty(); i++) validate_shader_param(v.items[i], t.items[0], why);
+        return;
+    }
     if (v.kind != t.kind) {
         why = std::string("expected ") + names[t.kind] + ", got " + names[v.kind];
         return;
@@ -1384,6 +1398,8 @@ static NodeRef node_child(const Stateful &l, OutputNode &out, uint64_t pts, std:
         ShaderParams p;
         p.shader = l.shader;
         if (l.shader_param) l.shader_param->to_bytes(p.param_bytes);
+        // a WGSL shader reads its whole uniform: bytes a short list (or no parameter) leaves out read as zero
+        if (p.shader->wgsl && p.param_bytes.size() < p.shader->uniform_size) p.param_bytes.resize(p.shader->uniform_size, 0);
         p.resolution = {f32_as_usize(l.size.width), f32_as_usize(l.size.height)};
         for (const Stateful &c : l.children) {
             const NodeRef k = node_child(c, out, pts, err);

@@ -136,11 +136,14 @@ struct WebInstance {
 
 // The type of a shader's parameter (smr_shader_param_type): the tree of scalars, fixed-length lists and structs that stands
 // in for the WGSL uniform type the reference reads out of the shader module (pipeline.rs:143-160)
+// A WGSL shader's uniform type (smr_register_wgsl_shader) adds vectors and matrices, which only the module can declare.
+constexpr int32_t kShaderParamVector = 5;   // vecN: length N, items[0] the scalar
+constexpr int32_t kShaderParamMatrix = 6;   // matCxR: length R (rows), items[0] the row, a vector of C scalars
 struct ShaderParamType {
-    int32_t kind = SMR_SHADER_PARAM_F32;  // smr_shader_param_kind
+    int32_t kind = SMR_SHADER_PARAM_F32;  // smr_shader_param_kind, kShaderParamVector or kShaderParamMatrix
     std::string name;                     // a struct field's name
-    std::vector<ShaderParamType> items;   // List: the element type (one); Struct: the fields, in order
-    uint32_t length = 0;                  // List: the element count
+    std::vector<ShaderParamType> items;   // List / Vector / Matrix: the element type (one); Struct: the fields, in order
+    uint32_t length = 0;                  // List: the element count; Vector: N; Matrix: rows
 };
 // A ShaderParam value (scene/components.rs:40-55)
 struct ShaderParamValue {
@@ -156,6 +159,8 @@ struct ShaderParamValue {
 // the scene nodes hold it by shared_ptr; the renderer unloads the module after the last tick that launched it.
 struct ShaderProgram {
     std::optional<ShaderParamType> param_type;
+    bool wgsl = false;                    // built by smr_register_wgsl_shader: drawn through its vertex stage
+    uint32_t uniform_size = 0;            // WGSL: SizeOf of the uniform; the parameter bytes are zero-padded to it
     std::vector<char> cubin;              // NVRTC's image for sm_90a
     void *library = nullptr;              // cudaLibrary_t (device handles only)
     const void *kernel = nullptr;         // its smr_shader_main, a cudaKernel_t

@@ -655,6 +655,11 @@ class Renderer:
         spec = F.ShaderSpec(src, C.pointer(pt) if pt is not None else None)
         self._check(self._lib.smr_register_shader(self._h, shader_id.encode(), C.byref(spec)))
 
+    def register_wgsl_shader(self, shader_id: str, source: str):
+        """Renderer::register_renderer for RendererSpec::Shader(ShaderSpec { source }) as the reference takes it: WGSL with
+        the shader header, vs_main and fs_main (see smr_register_wgsl_shader); its parameter type is its uniform's"""
+        self._check(self._lib.smr_register_wgsl_shader(self._h, shader_id.encode(), source.encode()))
+
     def unregister_shader(self, shader_id: str):
         self._check(self._lib.smr_unregister_shader(self._h, shader_id.encode()))
 
