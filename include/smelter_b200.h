@@ -625,8 +625,8 @@ smr_status smr_debug_layouts(smr_renderer *r, const char *output_id, uint64_t pt
                              smr_render_layout *out, uint32_t capacity, uint32_t *n_out,
                              uint32_t *root_width, uint32_t *root_height);
 /* inspection (no device needed): the same for any layout node of an output's render graph.  node 0 is the root when the
- * root is a layout; the layout nodes below it (a View, Tiles or Rescaler child of a Shader) follow in DFS order, children
- * before parents.  root_width x root_height is the node's resolution at pts.  SMR_ERR_INVALID_ARGUMENT: no such node. */
+ * root is a layout (for an output of smr_set_layouts, the root layout it was given); the layout nodes below it (a View,
+ * Tiles or Rescaler child of a Shader) follow in DFS order, children before parents.  root_width x root_height is the node's resolution at pts.  SMR_ERR_INVALID_ARGUMENT: no such node. */
 smr_status smr_debug_node_layouts(smr_renderer *r, const char *output_id, uint32_t node, uint64_t pts_ns,
                                   smr_render_layout *out, uint32_t capacity, uint32_t *n_out,
                                   uint32_t *root_width, uint32_t *root_height);

@@ -407,10 +407,8 @@ class Renderer {
     smr_status render_text(uint32_t w, uint32_t h, smr_rgba bg, const smr_glyph *glyphs, uint32_t n, const smr_atlas *mask,
                            const smr_atlas *color, int32_t color_mode, void *rgba, uint32_t pitch, int32_t mem_kind);
     smr_status debug_set_inputs(uint64_t pts, const smr_input_frame *in, uint32_t n_in);
-    smr_status debug_layouts(const char *output_id, uint64_t pts, smr_render_layout *out, uint32_t cap, uint32_t *n,
-                             uint32_t *rw, uint32_t *rh);
-    smr_status debug_node_layouts(const char *output_id, uint32_t node, uint64_t pts, smr_render_layout *out, uint32_t cap,
-                                  uint32_t *n, uint32_t *rw, uint32_t *rh);
+    smr_status debug_node_layouts(const char *output_id, std::optional<uint32_t> node, uint64_t pts, smr_render_layout *out,
+                                  uint32_t cap, uint32_t *n, uint32_t *rw, uint32_t *rh);
     smr_status layouts_to_c(const std::vector<RenderLayout> &layouts, smr_render_layout *out, uint32_t cap, uint32_t *n);
     smr_status debug_image_nodes(const char *output_id, uint64_t pts, smr_image_node_info *out, uint32_t cap, uint32_t *n);
     smr_status debug_fused_jobs(smr_fused_job_info *out, uint32_t cap, uint32_t *n);
@@ -487,18 +485,12 @@ class Renderer {
         Resolution res;
         DevBuf planes[kTicksInFlight][3];       // device staging for host outputs, one set per tick in flight: the read-back of
                                                 // tick k runs on its own stream while tick k + 1 composes into the next set
-        // smr_set_layouts: the caller flattened the scene itself (the reference's scene/** stays in Rust); used instead
-        // of `node` until the next smr_update_scene of this output
         // tile plan of the composite (direct-tile owners + cost-sorted list of the tiles that are left), kept while the
         // flattened layers and the resamples feeding them stay the same (a static scene plans once)
         uint64_t tile_key = 0;
         bool tile_key_valid = false;
         std::vector<int> tile_owner_layer;       // per tile: index of the layer whose child is shown there 1:1 and alone, or -1
         std::vector<uint32_t> tile_list;         // tiles that are left for the composite, most expensive first
-        bool flat = false;
-        Resolution flat_root;
-        std::vector<NodeRef> flat_children;      // Input refs
-        std::vector<RenderLayout> flat_layouts;
     };
     struct WeightKey {
         uint32_t scale_bits, offset_bits;
@@ -555,10 +547,13 @@ class Renderer {
     smr_status read_frame(const smr_input_frame &f, FrameView &v);
     template <class Use> smr_status select_inputs(uint64_t pts, const smr_input_frame *in, uint32_t n_in, Use use);
     smr_status upload_input(Input &I, const smr_input_frame &f);
-    Resolution output_children(const Output &o, const OutputNode &node, uint64_t pts, std::vector<Input *> &child_in,
-                               std::vector<std::optional<Resolution>> &child_res);
-    std::vector<RenderLayout> output_layouts(const Output &o, OutputNode &node, uint64_t pts,
-                                             const std::vector<std::optional<Resolution>> &child_res, Resolution root);
+    struct LayoutEval {
+        std::vector<Input *> child_in;                      // the Input behind each child; nullptr: the empty view
+        std::vector<std::optional<Resolution>> child_res;
+        Resolution res;                                     // the node's
+        std::vector<RenderLayout> layouts;                  // flattened, untruncated
+    };
+    LayoutEval eval_layout(Output &o, LayoutParams &lp, uint64_t pts);
     smr_status plan_output(Output &o, smr_output_frame &of, uint64_t pts);
     Input *node_input(Output &o, const NodeRef &r);
     smr_status plan_layers(std::vector<RenderLayout> &layouts, const std::vector<Input *> &child_in, int W, int H,
@@ -663,7 +658,10 @@ class Renderer {
     // that is still pending on stream_ (no internal dependencies), so a copy does not wait for the ticks in flight.
     cudaMemPool_t web_pool_ = nullptr;
     smr_status alloc_on_stream(size_t bytes, std::shared_ptr<void> &buf);
+    Output &install_output(const char *output_id, OutputNode &&node, int32_t fmt, uint32_t w, uint32_t h);
     void plan_node_textures(Output &o, uint64_t pts);
+    CompositeRec composite_rec(int W, int H, const std::vector<dev::LayerDev> &layers, const std::vector<dev::MaskDev> &masks);
+    int composite_texture(CompositeRec pc);
     void plan_tiles(Output &o, CompositeRec &pc, const std::vector<dev::LayerDev> &layers, int W, int H);
     std::vector<WeightKey> new_weight_keys_;   // cache entries whose k_weights launch is not enqueued yet
     void rollback_weights();                   // a tick that fails before that launch must not leave them behind
@@ -1145,19 +1143,26 @@ smr_status Renderer::update_scene(const char *output_id, uint32_t w, uint32_t h,
         set_error(err);
         return SMR_ERR_SCENE;
     }
-    Output &o = outputs_[output_id];
-    o.node = std::move(node);
-    o.texts.clear();   // the memory of the replaced nodes is released on stream_, after the ticks that read it
+    Output &o = install_output(output_id, std::move(node), fmt, w, h);
     for (const auto &p : o.node.texts) o.texts.push_back(std::move(made[p.get()]));
     o.images = std::move(images);
     o.webs = std::move(webs);
     o.shaders = std::move(shaders);
+    return SMR_OK;
+}
+
+// Output `output_id` (registered here if it is new) renders `node` from now on, in `fmt` at w x h, with no node textures
+// until the caller moves in those it made for `node`.  The memory of the replaced ones is released on stream_, after the
+// ticks that read it.
+Renderer::Output &Renderer::install_output(const char *output_id, OutputNode &&node, int32_t fmt, uint32_t w, uint32_t h) {
+    Output &o = outputs_[output_id];
+    o.node = std::move(node);
+    o.texts.clear(); o.images.clear(); o.webs.clear(); o.shaders.clear();
     o.nested.clear();
     o.nested.resize(o.node.nested.size());
     o.format = fmt;
     o.res = {w, h};
-    o.flat = false; o.flat_layouts.clear(); o.flat_children.clear();
-    return SMR_OK;
+    return o;
 }
 
 // The bytes of a w x h node texture in its allocation, rounded up so that what follows it stays aligned
@@ -1323,7 +1328,7 @@ void Renderer::plan_shader_node(Output &o, ShaderNode &n, uint64_t pts) {
 // only frame; AnimatedAsset::render's choice) is not the one their texture holds join its image launch; the web nodes whose
 // instance has a frame join its web launch.
 void Renderer::plan_node_textures(Output &o, uint64_t pts) {
-    if (o.flat || o.nodes_planned == tick_) return;
+    if (o.nodes_planned == tick_) return;
     o.nodes_planned = tick_;
     auto enter = [&](NodeTexture &n) {
         n.in.node_tex = -1;
@@ -1396,17 +1401,14 @@ smr_status Renderer::set_layouts(const char *output_id, uint32_t w, uint32_t h, 
         }
         l = layout_from_c(d);
     }
-    Output &o = outputs_[output_id];
-    o.format = fmt;
-    o.res = {w, h};
-    o.flat = true;
+    OutputNode node;   // the root is a layout: the given one
+    node.resolution = {w, h};
+    node.root_layout.given_layouts = std::move(ls);
+    node.root_layout.given_resolution = {root_w, root_h};
+    for (uint32_t i = 0; i < n_children; i++)
+        node.root_layout.children.push_back({NodeRef::Input, -1, child_ids[i] ? child_ids[i] : ""});
     if (!host_only_) CUDA_OK(cudaSetDevice(opts_.cuda_device));   // the memory of the replaced nodes is released on stream_
-    o.texts.clear(); o.images.clear(); o.webs.clear(); o.shaders.clear();
-    o.nested.clear();
-    o.flat_root = {root_w, root_h};
-    o.flat_children.clear();
-    for (uint32_t i = 0; i < n_children; i++) o.flat_children.push_back({NodeRef::Input, -1, child_ids[i] ? child_ids[i] : ""});
-    o.flat_layouts = std::move(ls);
+    install_output(output_id, std::move(node), fmt, w, h);
     return SMR_OK;
 }
 
@@ -2224,16 +2226,19 @@ void Renderer::plan_tiles(Output &o, CompositeRec &pc, const std::vector<dev::La
     }
 }
 
-// An output's children at `pts` (sources[i].resolution(), layout.rs:176-179): the Input behind each (node_input) and its
-// resolution.  Returns the root resolution.
-Resolution Renderer::output_children(const Output &o, const OutputNode &node, uint64_t pts, std::vector<Input *> &child_in,
-                                     std::vector<std::optional<Resolution>> &child_res) {
-    for (const NodeRef &r : o.flat ? o.flat_children : node.children) {
-        Input *in = node_input(const_cast<Output &>(o), r);
-        child_in.push_back(in);
-        child_res.push_back(in ? std::optional<Resolution>(in->res) : std::nullopt);
+// Layout node `lp` of output `o` at `pts` (LayoutNode::render, layout.rs:170-181): its children (sources[i].resolution(),
+// layout.rs:176-179), its resolution and its flattened layouts.  Evaluating them advances the state of `lp`: o.node's when
+// rendering, a copy's for inspection.
+Renderer::LayoutEval Renderer::eval_layout(Output &o, LayoutParams &lp, uint64_t pts) {
+    LayoutEval e;
+    for (const NodeRef &r : lp.children) {
+        Input *in = node_input(o, r);
+        e.child_in.push_back(in);
+        e.child_res.push_back(in ? std::optional<Resolution>(in->res) : std::nullopt);
     }
-    return o.flat ? o.flat_root : node.layout_resolution(pts);
+    e.res = lp.resolution(pts);
+    e.layouts = lp.layouts(pts, e.child_res);
+    return e;
 }
 
 // The Input behind a render node: a text, image, web, shader or layout node's texture, or a caller's input; nullptr when it
@@ -2249,13 +2254,6 @@ Renderer::Input *Renderer::node_input(Output &o, const NodeRef &r) {
     }
     auto it = inputs_.find(r.input_id);
     return it != inputs_.end() && it->second.has_frame ? &it->second : nullptr;
-}
-
-// Its flattened layouts (layout.rs:180-181), untruncated.  Evaluating them advances Tiles::last_layout of `node`: o.node
-// when rendering, a copy for inspection.
-std::vector<RenderLayout> Renderer::output_layouts(const Output &o, OutputNode &node, uint64_t pts,
-                                                   const std::vector<std::optional<Resolution>> &child_res, Resolution root) {
-    return o.flat ? o.flat_layouts : node.layouts(pts, child_res).flatten(child_res, root);
 }
 
 // The texture a child layer samples: the input's own, or in GpuOptimized mode its copy resampled to the layer's size, whose
@@ -2365,45 +2363,48 @@ smr_status Renderer::plan_layers(std::vector<RenderLayout> &layouts, const std::
 // Tiles::last_layout advance as in the reference whether or not anything shows the node), then composited into an RGBA8
 // frame-arena texture of the tick's resolution (no tile plan, no direct tiles), which its readers take as a child texture
 smr_status Renderer::plan_layout_node(Output &o, size_t k, uint64_t pts) {
-    LayoutParams &lp = o.node.nested[k];
     Input &nn = o.nested[k];
     nn.has_frame = false;
     nn.node_tex = nn.raw_tex = -1;
-    std::vector<Input *> child_in;
-    std::vector<std::optional<Resolution>> child_res;
-    for (const NodeRef &ch : lp.children) {
-        Input *in = node_input(o, ch);
-        child_in.push_back(in);
-        child_res.push_back(in ? std::optional<Resolution>(in->res) : std::nullopt);
-    }
-    const Resolution root = lp.resolution(pts);
-    std::vector<RenderLayout> layouts = lp.layouts(pts, child_res).flatten(child_res, root);
-    if (root.width == 0 || root.height == 0 || root.width > 16384 || root.height > 16384) return SMR_OK;
-    if (layouts.size() > opts_.max_layouts_count) layouts.resize(opts_.max_layouts_count);
-    const int W = (int)root.width, H = (int)root.height;
+    LayoutEval e = eval_layout(o, o.node.nested[k], pts);
+    if (e.res.width == 0 || e.res.height == 0 || e.res.width > 16384 || e.res.height > 16384) return SMR_OK;
+    if (e.layouts.size() > opts_.max_layouts_count) e.layouts.resize(opts_.max_layouts_count);
+    const int W = (int)e.res.width, H = (int)e.res.height;
     std::vector<dev::LayerDev> layers;
     std::vector<dev::MaskDev> masks;
-    if (smr_status st = plan_layers(layouts, child_in, W, H, layers, masks); st != SMR_OK) return st;
+    if (smr_status st = plan_layers(e.layouts, e.child_in, W, H, layers, masks); st != SMR_OK) return st;
+    nn.raw_tex = composite_texture(composite_rec(W, H, layers, masks));
+    nn.tex = plan_.tex[nn.raw_tex].tex;
+    nn.res = e.res;
+    nn.has_frame = true;
+    return SMR_OK;
+}
+
+// A composite of `layers` (and their `masks`) into a W x H target, which the caller sets
+Renderer::CompositeRec Renderer::composite_rec(int W, int H, const std::vector<dev::LayerDev> &layers,
+                                               const std::vector<dev::MaskDev> &masks) {
     CompositeRec pc;
     memset(&pc.job, 0, sizeof(pc.job));
     pc.job.width = W; pc.job.height = H; pc.job.mode = opts_.rendering_mode;
     pc.job.n_layers = (int)layers.size();
     pc.layers_off = param_put(layers.data(), sizeof(dev::LayerDev) * layers.size());
     pc.masks_off = param_put(masks.data(), sizeof(dev::MaskDev) * masks.size());
+    return pc;
+}
+
+// Plans composite `pc` into an RGBA8 frame-arena texture of its size; returns that texture's index in the table
+int Renderer::composite_texture(CompositeRec pc) {
+    const int W = pc.job.width, H = pc.job.height;
     pc.out_frame_off = frame_alloc((size_t)W * H * 4);
     pc.job.out_format = -1;
     pc.job.out_pitch0 = W * 4;
     plan_.composites.push_back(pc);
-    nn.tex = dev::Tex();
-    nn.tex.kind = dev::TEX_RGBA8; nn.tex.width = W; nn.tex.height = H; nn.tex.pitch0 = W * 4;
-    nn.res = root;
-    nn.has_frame = true;
-    nn.raw_tex = add_texture(nn.tex, false, pc.out_frame_off);
-    return SMR_OK;
+    dev::Tex t;
+    t.kind = dev::TEX_RGBA8; t.width = W; t.height = H; t.pitch0 = W * 4;
+    return add_texture(t, false, pc.out_frame_off);
 }
 
 smr_status Renderer::plan_output(Output &o, smr_output_frame &of, uint64_t pts) {
-    const int mode = opts_.rendering_mode;
     of.width = (uint32_t)o.res.width; of.height = (uint32_t)o.res.height;
     of.format = o.format; of.pts_ns = pts;
 
@@ -2449,9 +2450,14 @@ smr_status Renderer::plan_output(Output &o, smr_output_frame &of, uint64_t pts) 
         j.out_pitch0 = pitch[0]; j.out_pitch1 = pitch[1]; j.out_pitch2 = pitch[2];
         plan_.outputs.push_back({j, src_tex});
     };
+    auto to_planes = [&](CompositeRec &pc) {   // the composite writes the output's planes (K10/K11 fused)
+        pc.job.out_format = o.format;
+        pc.job.out0 = dst[0]; pc.job.out1 = dst[1]; pc.job.out2 = dst[2];
+        pc.job.out_pitch0 = pitch[0]; pc.job.out_pitch1 = pitch[1]; pc.job.out_pitch2 = pitch[2];
+    };
 
     plan_node_textures(o, pts);
-    if (!o.flat && o.node.root) {  // pass-through: the root texture IS the node texture
+    if (o.node.root) {  // pass-through: the root texture IS the node texture
         Input *root_in = node_input(o, *o.node.root);
         if (!root_in) { push_fill(); return SMR_OK; }
         Input &in = *root_in;
@@ -2470,18 +2476,12 @@ smr_status Renderer::plan_output(Output &o, smr_output_frame &of, uint64_t pts) 
             l.kind = RenderLayout::ChildNode;
             l.width = (float)of.width; l.height = (float)of.height;
             l.crop = {0.0f, 0.0f, (float)of.width, (float)of.height};
-            dev::LayerDev d;
+            std::vector<dev::LayerDev> layers(1);
             bool skip;
-            prepare_layer(l, (int)of.width, (int)of.height, in.raw_tex, (int)of.width, (int)of.height, d, skip);
-            CompositeRec pc;
-            memset(&pc.job, 0, sizeof(pc.job));
-            pc.job.width = (int)of.width; pc.job.height = (int)of.height; pc.job.mode = mode;
-            pc.job.n_layers = skip ? 0 : 1;
-            pc.layers_off = param_put(&d, sizeof(d));
-            pc.masks_off = param_alloc(sizeof(dev::MaskDev));
-            pc.job.out_format = o.format;
-            pc.job.out0 = dst[0]; pc.job.out1 = dst[1]; pc.job.out2 = dst[2];
-            pc.job.out_pitch0 = pitch[0]; pc.job.out_pitch1 = pitch[1]; pc.job.out_pitch2 = pitch[2];
+            prepare_layer(l, (int)of.width, (int)of.height, in.raw_tex, (int)of.width, (int)of.height, layers[0], skip);
+            if (skip) layers.clear();
+            CompositeRec pc = composite_rec((int)of.width, (int)of.height, layers, {});
+            to_planes(pc);
             plan_.composites.push_back(pc);
             return SMR_OK;
         }
@@ -2489,43 +2489,26 @@ smr_status Renderer::plan_output(Output &o, smr_output_frame &of, uint64_t pts) 
         return SMR_OK;
     }
 
-    std::vector<Input *> child_in;
-    std::vector<std::optional<Resolution>> child_res;
-    const Resolution root = output_children(o, o.node, pts, child_in, child_res);
-    if (root.width == 0 || root.height == 0 || root.width > 16384 || root.height > 16384) { push_fill(); return SMR_OK; }
-    std::vector<RenderLayout> layouts = output_layouts(o, o.node, pts, child_res, root);
-    if (layouts.size() > opts_.max_layouts_count) layouts.resize(opts_.max_layouts_count);  // params.rs:176-182
+    LayoutEval e = eval_layout(o, o.node.root_layout, pts);
+    if (e.res.width == 0 || e.res.height == 0 || e.res.width > 16384 || e.res.height > 16384) { push_fill(); return SMR_OK; }
+    if (e.layouts.size() > opts_.max_layouts_count) e.layouts.resize(opts_.max_layouts_count);  // params.rs:176-182
 
-    const int W = (int)root.width, H = (int)root.height;
+    const int W = (int)e.res.width, H = (int)e.res.height;
     std::vector<dev::LayerDev> layers;
     std::vector<dev::MaskDev> masks;
-    if (smr_status st = plan_layers(layouts, child_in, W, H, layers, masks); st != SMR_OK) return st;
-
-    CompositeRec pc;
-    memset(&pc.job, 0, sizeof(pc.job));
-    pc.job.width = W; pc.job.height = H; pc.job.mode = mode;
-    pc.job.n_layers = (int)layers.size();
-    pc.layers_off = param_put(layers.data(), sizeof(dev::LayerDev) * layers.size());
-    pc.masks_off = param_put(masks.data(), sizeof(dev::MaskDev) * masks.size());
+    if (smr_status st = plan_layers(e.layouts, e.child_in, W, H, layers, masks); st != SMR_OK) return st;
+    CompositeRec pc = composite_rec(W, H, layers, masks);
 
     bool same_size = (size_t)W == o.res.width && (size_t)H == o.res.height;
     bool fused_fmt = o.format == SMR_OUT_PLANAR_YUV420 || o.format == SMR_OUT_NV12;
     bool fusable = same_size && (o.format == SMR_OUT_RGBA8 || (fused_fmt && (W % 2 == 0) && (H % 2 == 0)));
     if (fusable) {
-        pc.job.out_format = o.format;
-        pc.job.out0 = dst[0]; pc.job.out1 = dst[1]; pc.job.out2 = dst[2];
-        pc.job.out_pitch0 = pitch[0]; pc.job.out_pitch1 = pitch[1]; pc.job.out_pitch2 = pitch[2];
+        to_planes(pc);
         if (fused_fmt) plan_tiles(o, pc, layers, W, H);
         plan_.composites.push_back(pc);
     } else {
         if (o.format == SMR_OUT_RGBA8) { set_error("RGBA output must match the root layout resolution"); return SMR_ERR_UNSUPPORTED; }
-        pc.out_frame_off = frame_alloc((size_t)W * H * 4);
-        pc.job.out_format = -1;
-        pc.job.out_pitch0 = W * 4;
-        plan_.composites.push_back(pc);
-        dev::Tex t;
-        t.kind = dev::TEX_RGBA8; t.width = W; t.height = H; t.pitch0 = W * 4;
-        push_output_job(add_texture(t, false, pc.out_frame_off));
+        push_output_job(composite_texture(pc));
     }
     return SMR_OK;
 }
@@ -2579,7 +2562,6 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
         if (it == outputs_.end()) break;
         Output &o = it->second;
         outs.push_back(&o);
-        if (o.flat) continue;
         for (const LayoutParams &lp : o.node.nested) max_depth = std::max(max_depth, lp.depth);
         for (const ShaderParams &sp : o.node.shaders) max_depth = std::max(max_depth, sp.depth);
     }
@@ -2589,7 +2571,6 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
     for (int d = 1; d <= max_depth; d++) {   // the layout nodes below the roots, shallow first (a tick without any: no phase)
         mark();
         for (Output *o : outs) {
-            if (o->flat) continue;
             for (size_t k = 0; k < o->node.nested.size(); k++) {
                 if (o->node.nested[k].depth != d) continue;
                 plan_node_textures(*o, pts);
@@ -3268,7 +3249,7 @@ smr_status Renderer::debug_image_nodes(const char *output_id, uint64_t pts, smr_
     auto it = outputs_.find(output_id);
     if (it == outputs_.end()) { set_error("output not registered"); return SMR_ERR_OUTPUT_NOT_REGISTERED; }
     const std::vector<ImageParams> &images = it->second.node.images;
-    *n = it->second.flat ? 0 : (uint32_t)images.size();
+    *n = (uint32_t)images.size();
     if (!out) return SMR_OK;
     if (cap < *n) return SMR_ERR_BUFFER_TOO_SMALL;
     for (uint32_t i = 0; i < *n; i++) {
@@ -3279,60 +3260,35 @@ smr_status Renderer::debug_image_nodes(const char *output_id, uint64_t pts, smr_
     return SMR_OK;
 }
 
-smr_status Renderer::debug_layouts(const char *output_id, uint64_t pts, smr_render_layout *out, uint32_t cap,
-                                   uint32_t *n, uint32_t *rw, uint32_t *rh) {
+// Layout node `node` of an output: 0 is the root when the root is a layout, the nodes below it follow in DFS order.  No
+// `node` (smr_debug_layouts): the root, which has no layouts at 0 x 0 when it is not a layout.
+smr_status Renderer::debug_node_layouts(const char *output_id, std::optional<uint32_t> node, uint64_t pts, smr_render_layout *out,
+                                        uint32_t cap, uint32_t *n, uint32_t *rw, uint32_t *rh) {
     if (!output_id || !n) return SMR_ERR_INVALID_ARGUMENT;
     std::lock_guard<std::mutex> g(mu_);
     auto it = outputs_.find(output_id);
     if (it == outputs_.end()) { set_error("output not registered"); return SMR_ERR_OUTPUT_NOT_REGISTERED; }
     Output &o = it->second;
-    *n = 0;
-    if (!o.flat && o.node.root) {
+    const bool root_layout = !o.node.root;
+    const LayoutParams *lp = nullptr;
+    if (root_layout && node.value_or(0) == 0) {
+        lp = &o.node.root_layout;
+    } else if (node) {
+        const size_t k = *node - (root_layout ? 1 : 0);
+        if (k >= o.node.nested.size()) { set_error("no such layout node"); return SMR_ERR_INVALID_ARGUMENT; }
+        lp = &o.node.nested[k];
+    }
+    if (!lp) {
+        *n = 0;
         if (rw) *rw = 0;
         if (rh) *rh = 0;
         return SMR_OK;
     }
-    OutputNode copy = o.node;  // do not advance Tiles::last_layout
-    std::vector<Input *> child_in;
-    std::vector<std::optional<Resolution>> child_res;
-    const Resolution root = output_children(o, copy, pts, child_in, child_res);
-    if (rw) *rw = (uint32_t)root.width;
-    if (rh) *rh = (uint32_t)root.height;
-    return layouts_to_c(output_layouts(o, copy, pts, child_res, root), out, cap, n);
-}
-
-// Layout node `node` of an output: 0 is the root when the root is a layout, the nodes below it follow in DFS order
-smr_status Renderer::debug_node_layouts(const char *output_id, uint32_t node, uint64_t pts, smr_render_layout *out, uint32_t cap,
-                                        uint32_t *n, uint32_t *rw, uint32_t *rh) {
-    if (!output_id || !n) return SMR_ERR_INVALID_ARGUMENT;
-    {
-        std::lock_guard<std::mutex> g(mu_);
-        auto it = outputs_.find(output_id);
-        if (it == outputs_.end()) { set_error("output not registered"); return SMR_ERR_OUTPUT_NOT_REGISTERED; }
-        Output &o = it->second;
-        const bool root_layout = !o.flat && !o.node.root;
-        if (!(root_layout && node == 0)) {
-            const size_t k = node - (root_layout ? 1 : 0);
-            if (o.flat || k >= o.node.nested.size()) { set_error("no such layout node"); return SMR_ERR_INVALID_ARGUMENT; }
-            LayoutParams copy = o.node.nested[k];   // do not advance Tiles::last_layout
-            std::vector<std::optional<Resolution>> child_res;
-            for (const NodeRef &ch : copy.children) {
-                if (ch.kind == NodeRef::Layout) {   // a layout node's texture has its resolution at pts
-                    const Resolution r = o.node.nested[ch.index].resolution(pts);
-                    const bool ok = r.width && r.height && r.width <= 16384 && r.height <= 16384;
-                    child_res.push_back(ok ? std::optional<Resolution>(r) : std::nullopt);
-                } else {
-                    Input *in = node_input(o, ch);
-                    child_res.push_back(in ? std::optional<Resolution>(in->res) : std::nullopt);
-                }
-            }
-            const Resolution root = copy.resolution(pts);
-            if (rw) *rw = (uint32_t)root.width;
-            if (rh) *rh = (uint32_t)root.height;
-            return layouts_to_c(copy.layouts(pts, child_res).flatten(child_res, root), out, cap, n);
-        }
-    }
-    return debug_layouts(output_id, pts, out, cap, n, rw, rh);
+    LayoutParams copy = *lp;   // inspection does not advance the node's state
+    const LayoutEval e = eval_layout(o, copy, pts);
+    if (rw) *rw = (uint32_t)e.res.width;
+    if (rh) *rh = (uint32_t)e.res.height;
+    return layouts_to_c(e.layouts, out, cap, n);
 }
 
 smr_status Renderer::layouts_to_c(const std::vector<RenderLayout> &layouts, smr_render_layout *out, uint32_t cap, uint32_t *n) {
@@ -3481,7 +3437,7 @@ smr_status smr_render(smr_renderer *r, uint64_t pts, const smr_input_frame *in, 
     SMR_GUARD(r->impl.render_end_all())   // every tick in flight, the one just submitted included
 }
 smr_status smr_debug_layouts(smr_renderer *r, const char *output_id, uint64_t pts, smr_render_layout *out, uint32_t cap,
-                             uint32_t *n, uint32_t *rw, uint32_t *rh) { SMR_GUARD(r->impl.debug_layouts(output_id, pts, out, cap, n, rw, rh)) }
+                             uint32_t *n, uint32_t *rw, uint32_t *rh) { SMR_GUARD(r->impl.debug_node_layouts(output_id, std::nullopt, pts, out, cap, n, rw, rh)) }
 smr_status smr_debug_image_nodes(smr_renderer *r, const char *output_id, uint64_t pts, smr_image_node_info *out, uint32_t cap,
                                  uint32_t *n) { SMR_GUARD(r->impl.debug_image_nodes(output_id, pts, out, cap, n)) }
 smr_status smr_debug_set_inputs(smr_renderer *r, uint64_t pts, const smr_input_frame *in, uint32_t n_in) { SMR_GUARD(r->impl.debug_set_inputs(pts, in, n_in)) }

@@ -1369,19 +1369,38 @@ static bool visit_web_ids(const Component &c, std::set<std::string> &ids, std::s
     return true;
 }
 
+static int depth_of(const OutputNode &out, const NodeRef &k) {
+    switch (k.kind) {
+        case NodeRef::Shader: return out.shaders[k.index].depth;
+        case NodeRef::Layout: return out.nested[k.index].depth;
+        case NodeRef::Web: return 1;
+        default: return 0;
+    }
+}
+
+static NodeRef node_child(const Stateful &l, OutputNode &out, uint64_t pts, std::string &err);
+
+// The layout node of layout component `l` at `size` (scene_state.rs:206-228): the render graph's clone of `l`, and its node
+// children appended to `out` in DFS order
+static LayoutParams layout_node(const Stateful &l, Size size, OutputNode &out, uint64_t pts, std::string &err) {
+    LayoutParams p;
+    p.size = size;
+    p.root = l;
+    std::vector<const Stateful *> leaves;
+    l.node_children(leaves);
+    for (const Stateful *c : leaves) {
+        const NodeRef k = node_child(*c, out, pts, err);
+        p.depth = std::max(p.depth, depth_of(out, k) + 1);
+        p.children.push_back(k);
+    }
+    return p;
+}
+
 // A node child of the render graph (build_tree, scene_state.rs:154-196): an input, or a text, image, web, shader or layout
 // node appended to `out`, whose own children come first in DFS order.  A layout node's size is node_size at `pts`; a layout
 // root without width and height is UnknownDimensionsForLayoutNodeRoot (scene_state.rs:206-228), reported in `err`.
 static NodeRef node_child(const Stateful &l, OutputNode &out, uint64_t pts, std::string &err) {
     NodeRef ch;
-    auto depth_of = [&](const NodeRef &k) {
-        switch (k.kind) {
-            case NodeRef::Shader: return out.shaders[k.index].depth;
-            case NodeRef::Layout: return out.nested[k.index].depth;
-            case NodeRef::Web: return 1;
-            default: return 0;
-        }
-    };
     if (l.kind == Stateful::Text) {
         ch = {NodeRef::Text, (int)out.texts.size()};
         out.texts.push_back(l.text);
@@ -1403,13 +1422,12 @@ static NodeRef node_child(const Stateful &l, OutputNode &out, uint64_t pts, std:
         p.resolution = {f32_as_usize(l.size.width), f32_as_usize(l.size.height)};
         for (const Stateful &c : l.children) {
             const NodeRef k = node_child(c, out, pts, err);
-            p.depth = std::max(p.depth, depth_of(k) + 1);
+            p.depth = std::max(p.depth, depth_of(out, k) + 1);
             p.children.push_back(k);
         }
         ch = {NodeRef::Shader, (int)out.shaders.size()};
         out.shaders.push_back(std::move(p));
     } else if (l.is_layout()) {
-        LayoutParams p;
         const Position pos = l.position(pts);
         if (!pos.width || !pos.height) {
             if (err.empty()) {
@@ -1419,15 +1437,7 @@ static NodeRef node_child(const Stateful &l, OutputNode &out, uint64_t pts, std:
             }
             return ch;
         }
-        p.size = {*pos.width, *pos.height};
-        p.root = l;   // the render graph's clone
-        std::vector<const Stateful *> leaves;
-        l.node_children(leaves);
-        for (const Stateful *c : leaves) {
-            const NodeRef k = node_child(*c, out, pts, err);
-            p.depth = std::max(p.depth, depth_of(k) + 1);
-            p.children.push_back(k);
-        }
+        LayoutParams p = layout_node(l, {*pos.width, *pos.height}, out, pts, err);
         ch = {NodeRef::Layout, (int)out.nested.size()};
         out.nested.push_back(std::move(p));
     } else {
@@ -1505,15 +1515,10 @@ bool SceneState::update_scene(const std::string &output_id, const Component &roo
     err.clear();
     out = OutputNode();
     out.resolution = resolution;
-    if (!st.root.is_layout()) {
+    if (!st.root.is_layout())
         out.root = node_child(st.root, out, last_pts_ns_, err);
-    } else {
-        out.layout_root = st.root;  // the render graph owns a clone
-        out.size = {(float)resolution.width, (float)resolution.height};
-        std::vector<const Stateful *> leaves;
-        st.root.node_children(leaves);
-        for (const Stateful *l : leaves) out.children.push_back(node_child(*l, out, last_pts_ns_, err));
-    }
+    else
+        out.root_layout = layout_node(st.root, {(float)resolution.width, (float)resolution.height}, out, last_pts_ns_, err);
     if (!err.empty()) return false;
     if (accept && !accept(out)) return false;
     output_scenes_[output_id] = root;
@@ -1555,28 +1560,19 @@ size_t ImageAsset::frame_at(uint64_t pts, uint64_t start_pts) const {
     return best;
 }
 
-Resolution OutputNode::layout_resolution(uint64_t pts) const {  // scene/layout.rs:245-257
-    Position p = layout_root.position(pts);
-    float w = p.width ? *p.width : size.width;
-    float h = p.height ? *p.height : size.height;
-    return {f32_as_usize(w), f32_as_usize(h)};
-}
-
 Resolution LayoutParams::resolution(uint64_t pts) const {
+    if (given_layouts) return given_resolution;
     Position p = root.position(pts);
     float w = p.width ? *p.width : size.width;
     float h = p.height ? *p.height : size.height;
     return {f32_as_usize(w), f32_as_usize(h)};
 }
 
-NestedLayout LayoutParams::layouts(uint64_t pts, const std::vector<std::optional<Resolution>> &inputs) {
+std::vector<RenderLayout> LayoutParams::layouts(uint64_t pts, const std::vector<std::optional<Resolution>> &inputs) {
+    if (given_layouts) return *given_layouts;
+    const Resolution res = resolution(pts);
     root.update_state(inputs.data(), inputs.size());
-    return root.layout(size, pts);
-}
-
-NestedLayout OutputNode::layouts(uint64_t pts, const std::vector<std::optional<Resolution>> &inputs) {
-    layout_root.update_state(inputs.data(), inputs.size());
-    return layout_root.layout(size, pts);
+    return root.layout(size, pts).flatten(inputs, res);
 }
 
 }  // namespace smr

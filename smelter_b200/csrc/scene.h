@@ -368,17 +368,21 @@ struct NodeRef {
     std::string input_id;
 };
 
-// A layout node other than the output's root (scene_state.rs:154-228, NodeParams::Layout): a View, Tiles or Rescaler whose
-// parent is a Shader.  Its own clone of the stateful component, its size (node_size at the last render's pts: the root's
-// width and height), its node children in DFS order, and its depth (1 + its deepest child's).  It is composited into its
-// own texture every tick.
+// A layout node (scene_state.rs:154-228, NodeParams::Layout): an output's root that is a layout, or a View, Tiles or
+// Rescaler whose parent is a Shader.  Its own clone of the stateful component, its size (the output's resolution for the
+// root; node_size at the last render's pts, the component's width and height, otherwise), its node children in DFS order,
+// and its depth (1 + its deepest child's; unused for the root).  A node below the root is composited into its own texture
+// every tick.  smr_set_layouts gives the root's flattened layouts and resolution instead, used as they are.
 struct LayoutParams {
     Stateful root;
     Size size;
     std::vector<NodeRef> children;
     int depth = 1;
+    std::optional<std::vector<RenderLayout>> given_layouts;   // smr_set_layouts: `root` and `size` are unused
+    Resolution given_resolution;
     Resolution resolution(uint64_t pts) const;   // SizedLayoutComponent::resolution (scene/layout.rs:245-257)
-    NestedLayout layouts(uint64_t pts, const std::vector<std::optional<Resolution>> &inputs);
+    // The flattened layouts at `pts` (layout.rs:176-181), untruncated; laying them out advances the state of `root`
+    std::vector<RenderLayout> layouts(uint64_t pts, const std::vector<std::optional<Resolution>> &inputs);
 };
 
 // A WebView render node (state/node.rs:127-141, NodeParams::Web): the instance and its children, each its own node
@@ -400,20 +404,14 @@ struct ShaderParams {
 
 // scene/scene_state.rs
 struct OutputNode {
-    std::optional<NodeRef> root;              // the root render node; empty: the root is a layout, `layout_root`
-    Stateful layout_root;                     // LayoutNode.root.component (the render graph's clone)
-    Size size;                                // SizedLayoutComponent.size
-    std::vector<NodeRef> children;            // node children, DFS order
+    std::optional<NodeRef> root;              // the root render node; empty: the root is a layout, `root_layout`
+    LayoutParams root_layout;
     std::vector<std::shared_ptr<const TextPayload>> texts;   // the output's text nodes (the root, or children in DFS order)
     std::vector<ImageParams> images;          // the output's image nodes, likewise (web view children included)
     std::vector<WebParams> webs;              // the output's web nodes, likewise
     std::vector<ShaderParams> shaders;        // the output's shader nodes, children before parents
     std::vector<LayoutParams> nested;         // the output's layout nodes below the root, DFS order, children before parents
     Resolution resolution;
-
-    // scene::LayoutNode as LayoutProvider (scene/layout.rs:31-41, 240-261)
-    Resolution layout_resolution(uint64_t pts) const;
-    NestedLayout layouts(uint64_t pts, const std::vector<std::optional<Resolution>> &inputs);
 };
 
 class SceneState {

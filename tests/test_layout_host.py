@@ -420,7 +420,9 @@ def test_frame_pre_processor_without_gpu_fails_loudly():
 
 def test_set_layouts_flattened_boundary_round_trip():
     """smr_set_layouts (SURVEY 8b, flattened form): the layouts one handle flattened from a scene, handed to another
-    handle as RenderLayout[], come back field for field from debug_layouts -- what smr_render then consumes"""
+    handle as RenderLayout[], come back field for field from debug_layouts -- what smr_render then consumes.  They are
+    the output's root layout node (debug_node_layouts node 0, the only one), and they replace its scene's image nodes."""
+    import numpy as np
     V = s.ViewComponent
     kids = [s.RescalerComponent(child=c, border_radius=s.BorderRadius.new_with_radius(12.0),
                                 box_shadow=[s.BoxShadow(3.0, 4.0, 10.0, s.RGBAColor(0, 0, 0, 128))]) for c in inputs(3)]
@@ -433,12 +435,21 @@ def test_set_layouts_flattened_boundary_round_trip():
     b = host_renderer()
     for i in range(1, 4):
         b.register_input(f"input_{i}")
+    b.register_image("image", np.zeros((4, 8, 4), np.uint8))
+    b.update_scene("output_1", RES, s.OutputFrameFormat.PlanarYuv420Bytes, V(children=[s.ImageComponent(image_id="image")]))
+    assert len(b.debug_image_nodes("output_1")) == 1
     b.set_layouts("output_1", RES, s.OutputFrameFormat.PlanarYuv420Bytes, root, [f"input_{i}" for i in range(1, 4)], ls)
+    assert b.debug_image_nodes("output_1") == []
     b.debug_set_inputs(0.0, {f"input_{i}": RES for i in range(1, 4)})
     ls2, root2 = b.debug_layouts("output_1")
     assert root2 == root and len(ls2) == len(ls)
     for x, y in zip(ls, ls2):
         assert bytes(x) == bytes(y)
+    ls_node, root_node = b.debug_node_layouts("output_1", 0)
+    assert root_node == root2 and [bytes(x) for x in ls_node] == [bytes(y) for y in ls2]
+    with pytest.raises(s.RendererError) as e:
+        b.debug_node_layouts("output_1", 1)
+    assert e.value.status == 1   # SMR_ERR_INVALID_ARGUMENT: no such layout node
     # a later update_scene of the same output replaces the flattened layouts
     b.update_scene("output_1", RES, s.OutputFrameFormat.PlanarYuv420Bytes, V(background_color=BG))
     ls3, _ = b.debug_layouts("output_1")
