@@ -150,9 +150,11 @@ typedef struct smr_component {
 
     /* WebView (WebViewComponent, scene/components.rs:55-61): the instance registered with smr_register_web_renderer, and
      * in `children` the components embedded in the page, zipped in order with the instance's child rects
-     * (smr_web_set_child_rects).  A child is an InputStream, Image or Text component and has an id; a View, Tiles,
-     * Rescaler, WebView or Shader child is SMR_ERR_UNSUPPORTED (layout children inside a WebView are not supported yet).
-     * NULL web_renderer_id: SMR_ERR_UNSUPPORTED, which is what a caller built before this field existed sends. */
+     * (smr_web_set_child_rects).  A child has an id and is an InputStream, Image or Text component, or a View, Tiles or
+     * Rescaler that declares both width and height (a layout node of its own, holding any component).  A WebView or
+     * Shader child, and a View, Tiles or Rescaler child without both sides, are SMR_ERR_UNSUPPORTED (see
+     * smr_update_scene).  NULL web_renderer_id: SMR_ERR_UNSUPPORTED, which is what a caller built before this field
+     * existed sends. */
     const char *web_renderer_id;
 
     /* Shader (ShaderComponent, scene/components.rs:29-38): the shader registered with smr_register_shader, its parameter
@@ -406,16 +408,23 @@ smr_status smr_register_wgsl_shader(smr_renderer *r, const char *shader_id, cons
  * clears the node texture and draws max(1, texture_count) planes (plane_id -1 without children), each pixel's
  * smr_fragment blended with premultiplied alpha and stored as 8 bits (pipeline.rs:81-140).  A child input without a live
  * frame samples the empty view.  A tick draws the nodes below the roots in order of depth (1 + the deepest child's; an
- * input, text or image 0, a web node 1): per depth the resample passes and one composite launch for its layout nodes, then
- * one launch per shader for its shader nodes; the roots' composite comes last.
+ * input, text or image 0): the web nodes of depth 1 first, then per depth the resample passes and one composite launch
+ * for its layout nodes, one launch per shader for its shader nodes and one launch for its web nodes; the roots'
+ * composite comes last.
  * WebView (scene/web_view_component.rs): its size is the instance's resolution.  SMR_ERR_SCENE, the scene staying as it
  * was: an instance that is not registered (WebRendererNotFound), a child without an id (WebViewChildWithoutId), an
- * instance shown by two WebViews of any outputs (WebRendererUsageNotExclusive).  The node texture is transparent when the
- * scene is set; each render with a frame clears it and draws the planes in the embedding order, each child through its
- * rect with the linear sampler and every plane blended with premultiplied alpha and stored as 8 bits (shader.rs:53-114).
- * A child input without a live frame draws nothing.  Layout children (View, Tiles, Rescaler) and WebView children inside
- * a WebView are not supported yet: each would need its own layout node texture.  A Shader inside a WebView is
- * SMR_ERR_UNSUPPORTED too.
+ * instance shown by two WebViews of any outputs, at any depth of nesting (WebRendererUsageNotExclusive).  The node texture
+ * is transparent when the scene is set; each render with a frame clears it and draws the planes in the embedding order,
+ * each child through its rect with the linear sampler and every plane blended with premultiplied alpha and stored as 8
+ * bits (shader.rs:53-114).  A child input without a live frame draws nothing.  A View, Tiles or Rescaler child is a layout
+ * node of its own, as under a Shader: its size is its width and height at the last render's pts, its layout state carries
+ * over scene updates, every render evaluates and composites it whether or not the instance has a frame, and a
+ * resolution of 0 or above 16384 draws nothing.  Below it any component may appear, Shaders and WebViews included (a
+ * sizeless layout root there is UnknownDimensionsForLayoutNodeRoot).  SMR_ERR_UNSUPPORTED: a WebView or Shader child of a
+ * WebView, and a View, Tiles or Rescaler child of a WebView without both width and height (Tiles: tiles_width and
+ * tiles_height; View and Rescaler: the position's).  The reference answers UnknownDimensionsForLayoutNodeRoot for the
+ * sizeless layout child and accepts the WebView and Shader children; these shapes keep the status they had before
+ * layout children were accepted, so that callers that relied on it see no change.
  * Image (scene/image_component.rs): the node's resolution is round(image_width) x round(image_height); with one side
  * missing the other follows from the asset's aspect ratio, which the reference takes as the integer division
  * width / height (640 x 360 gives 1, a portrait asset 0); with both missing it is the asset's size.  A resolved side of 0

@@ -1677,8 +1677,8 @@ int launch_image(const ImageJob *jobs_dev, const int32_t *tile_begin_dev, int n_
 // Web view node texture (web_renderer/shader.rs:53-114, render_website.wgsl): one render pass per plane, the first one
 // clearing to transparent.  A pass leaves the pixels its quad does not cover as they are and blends the bare sample into
 // the others (PREMULTIPLIED_ALPHA_BLENDING through the target view), so each pixel walks the planes in order with its
-// value quantised to 8 bits after every plane, as the texture holds it between passes.  Every web node a tick draws is
-// one launch, block -> job as in k_text; one thread per pixel of a 32 x 8 tile.
+// value quantised to 8 bits after every plane, as the texture holds it between passes.  The web nodes of one depth a tick
+// draws are one launch, block -> job as in k_text; one thread per pixel of a 32 x 8 tile.
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) k_web(const WebJob *__restrict__ jobs, const int32_t *__restrict__ tile_begin, int n_jobs) {
     __shared__ Tables T;

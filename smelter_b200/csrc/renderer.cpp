@@ -455,15 +455,17 @@ class Renderer {
     // A WebView component (WebRendererNode, transformations/web_renderer/node.rs), of the instance's size.  The node
     // texture is cleared when the node is made and redrawn, in the order of stream_, by every tick while the instance has a
     // frame.
+    struct Output;
     struct WebNode : NodeTexture {
         WebParams params;
+        Output *owner = nullptr;      // the output whose nodes its children are (set when a tick plans it)
         dev::WebJob job = {};   // draws `in.tex`; its planes are this tick's, packed into the parameter arena
         std::vector<dev::WebPlane> planes;
+        std::vector<int> plane_child; // per plane: the child it shows (its texture is read when the tick is packed), -1 the page
         size_t planes_off = 0;
     };
     // A Shader component (ShaderNode, transformations/shader/node.rs).  The node texture persists and is redrawn, in the
     // order of stream_, by every tick.
-    struct Output;
     struct ShaderNode : NodeTexture {
         ShaderParams params;
         Output *owner = nullptr;   // the output whose nodes its children are (set when a tick plans it)
@@ -556,6 +558,7 @@ class Renderer {
     LayoutEval eval_layout(Output &o, LayoutParams &lp, uint64_t pts);
     smr_status plan_output(Output &o, smr_output_frame &of, uint64_t pts);
     Input *node_input(Output &o, const NodeRef &r);
+    dev::Tex packed_node_tex(Output &o, const NodeRef &r);
     smr_status plan_layers(std::vector<RenderLayout> &layouts, const std::vector<Input *> &child_in, int W, int H,
                            std::vector<dev::LayerDev> &layers, std::vector<dev::MaskDev> &masks);
     smr_status plan_layout_node(Output &o, size_t k, uint64_t pts);
@@ -627,9 +630,9 @@ class Renderer {
         std::vector<PendingCopy> d2h;
         std::vector<TextNode *> texts;        // text nodes drawn by this tick (one launch, before everything that reads them)
         std::vector<ImageNode *> images;      // image nodes drawn by this tick (likewise)
-        std::vector<WebNode *> webs;          // web nodes drawn by this tick (after the text and image nodes they may read)
-        std::vector<ShaderNode *> shaders;    // shader nodes drawn by this tick (after the web nodes they may read)
-        // the tick's phases: one per depth of its layout and shader nodes below the roots, then the roots'.  A phase's
+        std::vector<WebNode *> webs;          // web nodes drawn by this tick (after every node they may read, by depth)
+        std::vector<ShaderNode *> shaders;    // shader nodes drawn by this tick (likewise)
+        // the tick's phases: one per depth of its layout, shader and web nodes below the roots, then the roots'.  A phase's
         // generic resample passes and composite jobs are those from its mark up to the next one (planned in phase order)
         struct Phase { size_t stages[3], composites; };
         std::vector<Phase> phases;
@@ -1288,17 +1291,21 @@ static bool web_plane(float m00, float m03, float m11, float m13, int W, int H, 
 // The planes a tick draws into web node `n` (WebRenderer::prepare_textures, renderer.rs:101-134), when its instance has a
 // frame: the page, and each child zipped with the latest rect list, in the instance's embedding order.  The frame pointer
 // and the rects are copied into this tick's parameters, so a later smr_web_set_frame / smr_web_set_child_rects does not
-// change what the tick reads.
+// change what the tick reads.  The children's textures are read when the tick is packed, once the layout nodes'
+// frame-arena textures have addresses.
 void Renderer::plan_web_node(Output &o, WebNode &n) {
     const WebInstance &w = *n.params.instance;
     if (!w.frame) return;   // no frame yet: the texture stays as it is (renderer.rs:89-96)
+    n.owner = &o;
     const int W = (int)w.width, H = (int)w.height;
     dev::WebPlane site;
     site.tex.kind = dev::TEX_BGRA; site.tex.width = W; site.tex.height = H; site.tex.pitch0 = W * 4;
     site.tex.p0 = (const uint8_t *)w.frame.get();
     const bool site_ok = web_plane(1.0f, 0.0f, 1.0f, 0.0f, W, H, site);
     n.planes.clear();
-    if (site_ok && w.embedding == SMR_WEB_NATIVE_OVER_CONTENT) n.planes.push_back(site);
+    n.plane_child.clear();
+    auto push = [&](const dev::WebPlane &pl, int child) { n.planes.push_back(pl); n.plane_child.push_back(child); };
+    if (site_ok && w.embedding == SMR_WEB_NATIVE_OVER_CONTENT) push(site, -1);
     const size_t nc = std::min(n.params.children.size(), w.rects.size() / 4);
     const float sx = (float)W / 2.0f, sy = (float)H / 2.0f, a = 1.0f / sx, b = 1.0f / sy;
     for (size_t k = 0; k < nc; k++) {
@@ -1306,10 +1313,9 @@ void Renderer::plan_web_node(Output &o, WebNode &n) {
         const float tx = -((float)W / 2.0f) + (r[0] + r[2] / 2.0f), ty = (float)H / 2.0f - (r[1] + r[3] / 2.0f);
         dev::WebPlane pl;
         if (!web_plane(a * (sx * (r[2] / (float)W)), a * tx, b * (sy * (r[3] / (float)H)), b * ty, W, H, pl)) continue;
-        if (const Input *in = node_input(o, n.params.children[k])) pl.tex = in->tex;   // else the empty view
-        n.planes.push_back(pl);
+        push(pl, (int)k);
     }
-    if (site_ok && w.embedding == SMR_WEB_NATIVE_UNDER_CONTENT) n.planes.push_back(site);
+    if (site_ok && w.embedding == SMR_WEB_NATIVE_UNDER_CONTENT) push(site, -1);
     n.job.n_planes = (int)n.planes.size();
     plan_.webs.push_back(&n);
 }
@@ -1326,7 +1332,7 @@ void Renderer::plan_shader_node(Output &o, ShaderNode &n, uint64_t pts) {
 // A tick that renders output `o` at `pts`: each of its text, image, web and shader nodes enters the texture table.  The text nodes
 // not drawn since the last smr_update_scene join the tick's text launch; the image nodes whose frame at `pts` (a Bitmap's
 // only frame; AnimatedAsset::render's choice) is not the one their texture holds join its image launch; the web nodes whose
-// instance has a frame join its web launch.
+// instance has a frame join its web launch of their depth.
 void Renderer::plan_node_textures(Output &o, uint64_t pts) {
     if (o.nodes_planned == tick_) return;
     o.nodes_planned = tick_;
@@ -2256,6 +2262,14 @@ Renderer::Input *Renderer::node_input(Output &o, const NodeRef &r) {
     return it != inputs_.end() && it->second.has_frame ? &it->second : nullptr;
 }
 
+// The texture a shader or web node's draw reads for child `r` once the tick's frame-arena addresses are resolved: a layout
+// node's composite from the texture table, any other node's own texture; the empty view when it has no pixels this tick
+dev::Tex Renderer::packed_node_tex(Output &o, const NodeRef &r) {
+    Input *in = node_input(o, r);
+    if (!in) return dev::Tex();
+    return r.kind == NodeRef::Layout ? plan_.tex[in->raw_tex].tex : in->tex;
+}
+
 // The texture a child layer samples: the input's own, or in GpuOptimized mode its copy resampled to the layer's size, whose
 // crop then replaces the layer's (resample_scaled_children, layout.rs:238-278)
 smr_status Renderer::child_texture(Input &in, RenderLayout &l, int &tex_index, int &tex_w, int &tex_h) {
@@ -2556,7 +2570,7 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
     // the outputs up to the first that is not registered: those before it are planned, as they always were, before the
     // tick fails on it
     std::vector<Output *> outs;
-    int max_depth = 0;   // of the layout and shader nodes below the roots
+    int max_depth = 0;   // of the layout, shader and web nodes below the roots
     for (uint32_t i = 0; i < n_out; i++) {
         auto it = out[i].output_id ? outputs_.find(out[i].output_id) : outputs_.end();
         if (it == outputs_.end()) break;
@@ -2564,6 +2578,7 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
         outs.push_back(&o);
         for (const LayoutParams &lp : o.node.nested) max_depth = std::max(max_depth, lp.depth);
         for (const ShaderParams &sp : o.node.shaders) max_depth = std::max(max_depth, sp.depth);
+        for (const WebParams &wp : o.node.webs) max_depth = std::max(max_depth, wp.depth);
     }
     auto mark = [&]() {
         plan_.phases.push_back({{plan_.stages[0].size(), plan_.stages[1].size(), plan_.stages[2].size()}, plan_.composites.size()});
@@ -2693,8 +2708,23 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
     const size_t cj_off = param_put_all(plan_.composites, &CompositeRec::job);   // read by k_composite_multi
     const TileJobs text_jobs = param_put_tile_jobs(plan_.texts, &TextNode::job);
     const TileJobs image_jobs = param_put_tile_jobs(plan_.images, &ImageNode::job);
-    for (WebNode *n : plan_.webs) n->planes_off = param_put(n->planes.data(), sizeof(dev::WebPlane) * n->planes.size());
-    const TileJobs web_jobs = param_put_tile_jobs(plan_.webs, &WebNode::job);
+    // web nodes: one launch per depth, shallow first (depth 1 before the conversions, depth d after phase d - 1's shaders)
+    std::vector<std::vector<WebNode *>> web_launches;
+    std::vector<TileJobs> web_jobs;
+    {
+        for (WebNode *n : plan_.webs) {   // the children's textures, frame-arena addresses resolved
+            for (size_t i = 0; i < n->planes.size(); i++)
+                if (n->plane_child[i] >= 0) n->planes[i].tex = packed_node_tex(*n->owner, n->params.children[n->plane_child[i]]);
+            n->planes_off = param_put(n->planes.data(), sizeof(dev::WebPlane) * n->planes.size());
+        }
+        std::vector<WebNode *> order = plan_.webs;
+        std::stable_sort(order.begin(), order.end(), [](const WebNode *a, const WebNode *b) { return a->params.depth < b->params.depth; });
+        for (WebNode *n : order) {
+            if (web_launches.empty() || web_launches.back()[0]->params.depth != n->params.depth) web_launches.emplace_back();
+            web_launches.back().push_back(n);
+        }
+        for (const auto &l : web_launches) web_jobs.push_back(param_put_tile_jobs(l, &WebNode::job));
+    }
     // shader nodes: one launch per (depth, shader), shallow first, so that every child is drawn before its reader
     std::vector<std::vector<ShaderNode *>> shader_launches;
     std::vector<TileJobs> shader_jobs;
@@ -2708,12 +2738,8 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
             else it->push_back(n);
         }
         for (ShaderNode *n : plan_.shaders) {   // the children's textures, frame-arena addresses resolved
-            n->tex.assign(n->params.children.size(), dev::Tex());
-            for (size_t k = 0; k < n->params.children.size(); k++) {
-                const NodeRef &ch = n->params.children[k];
-                Input *in = node_input(*n->owner, ch);
-                if (in) n->tex[k] = ch.kind == NodeRef::Layout ? plan_.tex[in->raw_tex].tex : in->tex;
-            }
+            n->tex.resize(n->params.children.size());
+            for (size_t k = 0; k < n->params.children.size(); k++) n->tex[k] = packed_node_tex(*n->owner, n->params.children[k]);
             n->tex_off = param_put(n->tex.data(), sizeof(dev::Tex) * n->tex.size());
             const std::vector<uint8_t> &b = n->params.param_bytes;
             n->params_off = b.empty() ? SIZE_MAX : param_put(b.data(), b.size());
@@ -2725,8 +2751,10 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
     CUDA_OK(param_dev_[slot_].ensure(param_used_));
     uint8_t *pd = param_dev_[slot_].p;
     auto dev_ptr = [&](size_t off) -> uint8_t * { return off != SIZE_MAX ? pd + off : nullptr; };
-    dev::WebJob *wj = reinterpret_cast<dev::WebJob *>(param_host_.data() + web_jobs.jobs_off);
-    for (size_t i = 0; i < plan_.webs.size(); i++) wj[i].planes = (const dev::WebPlane *)(pd + plan_.webs[i]->planes_off);
+    for (size_t l = 0; l < web_launches.size(); l++) {
+        dev::WebJob *wj = reinterpret_cast<dev::WebJob *>(param_host_.data() + web_jobs[l].jobs_off);
+        for (size_t i = 0; i < web_launches[l].size(); i++) wj[i].planes = (const dev::WebPlane *)(pd + web_launches[l][i]->planes_off);
+    }
     for (size_t l = 0; l < shader_launches.size(); l++) {
         dev::ShaderJob *sj = reinterpret_cast<dev::ShaderJob *>(param_host_.data() + shader_jobs[l].jobs_off);
         for (size_t i = 0; i < shader_launches[l].size(); i++) {
@@ -2757,6 +2785,16 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
 
     // ---- launches -----------------------------------------------------------------------------
     auto launched = [&](int n) -> bool { if (n < 0) return false; launches += (uint64_t)n; return true; };
+    auto launch_webs = [&](int depth) -> bool {   // the web nodes of `depth` this tick draws, if any
+        for (size_t l = 0; l < web_launches.size(); l++) {
+            if (web_launches[l][0]->params.depth != depth) continue;
+            const TileJobs &t = web_jobs[l];
+            if (!launched(dev::launch_web((const dev::WebJob *)(pd + t.jobs_off), (const int32_t *)(pd + t.begin_off),
+                                          (int)web_launches[l].size(), t.n_tiles, stream_))) return false;
+            prof_mark(SMR_KERNEL_WEB);
+        }
+        return true;
+    };
     prof_mark(-1);
     if (!plan_.texts.empty()) {   // every text node this tick draws: materialised node textures, like k_convert's
         if (!launched(dev::launch_text((const dev::TextJob *)(pd + text_jobs.jobs_off), (const int32_t *)(pd + text_jobs.begin_off),
@@ -2768,11 +2806,7 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
                                         (int)plan_.images.size(), image_jobs.n_tiles, stream_))) goto fail;
         prof_mark(SMR_KERNEL_IMAGE);
     }
-    if (!plan_.webs.empty()) {    // every web node this tick draws: after the text and image nodes its children may be
-        if (!launched(dev::launch_web((const dev::WebJob *)(pd + web_jobs.jobs_off), (const int32_t *)(pd + web_jobs.begin_off),
-                                      (int)plan_.webs.size(), web_jobs.n_tiles, stream_))) goto fail;
-        prof_mark(SMR_KERNEL_WEB);
-    }
+    if (!launch_webs(1)) goto fail;   // the web nodes of depth 1: after the text and image nodes their children may be
     node_guard.armed = false;
     for (auto &cv : plan_.convert_jobs) {
         const dev::Tex &src = plan_.tex[cv.first].tex;
@@ -2791,7 +2825,8 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
         prof_mark(SMR_KERNEL_RESAMPLE_FUSED);
     }
     // phase by phase: the generic resample passes feeding its layout nodes, one composite launch for them, then the shader
-    // nodes of that depth; the last phase is the roots' (ONE composite launch for every output of the tick)
+    // nodes of that depth and its web nodes (from depth 2); the last phase is the roots' (ONE composite launch for every
+    // output of the tick)
     for (size_t p = 0; p < plan_.phases.size(); p++) {
         const TickPlan::Phase &b = plan_.phases[p];
         const bool last_phase = p + 1 == plan_.phases.size();
@@ -2820,6 +2855,7 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
                 goto fail;
             prof_mark(SMR_KERNEL_SHADER);
         }
+        if (p > 0 && !launch_webs((int)p + 1)) goto fail;   // the web nodes of depth p + 1 (depth 1: launched above)
     }
     for (OutputRec &o : plan_.outputs) {
         if (!launched(dev::launch_output(o.job, stream_))) goto fail;

@@ -175,13 +175,19 @@ static bool component_from_c(const smr_component *c, Component &out, std::string
             if (c->children_len && !c->children) { err = "children pointer is null"; return false; }
             out.children.resize(c->children_len);
             for (uint32_t i = 0; i < c->children_len; i++) {
-                const int t = c->children[i].type;
-                if (t != SMR_COMPONENT_INPUT_STREAM && t != SMR_COMPONENT_IMAGE && t != SMR_COMPONENT_TEXT) {
-                    err = "a WebView child other than InputStream, Image or Text is outside the compositor hot path (layout and "
-                          "WebView children inside a WebView are not supported yet)";
+                // a direct WebView or Shader child, and a layout child without both sides, stay refused with the status
+                // they had before layout children were accepted (the reference would answer
+                // UnknownDimensionsForLayoutNodeRoot for the sizeless layout child)
+                const smr_component &k = c->children[i];
+                const bool sized = k.type == SMR_COMPONENT_TILES ? k.tiles_width.has_value && k.tiles_height.has_value
+                                                                 : k.position.width.has_value && k.position.height.has_value;
+                if (k.type == SMR_COMPONENT_WEB_VIEW || k.type == SMR_COMPONENT_SHADER ||
+                    ((k.type == SMR_COMPONENT_VIEW || k.type == SMR_COMPONENT_TILES || k.type == SMR_COMPONENT_RESCALER) && !sized)) {
+                    err = "a WebView or Shader child of a WebView, or a View, Tiles or Rescaler child without width and height, "
+                          "is outside the compositor hot path";
                     return false;
                 }
-                if (!component_from_c(&c->children[i], out.children[i], err, depth + 1, atlases)) return false;
+                if (!component_from_c(&k, out.children[i], err, depth + 1, atlases)) return false;
             }
             return true;
         case SMR_COMPONENT_SHADER:
@@ -1373,7 +1379,7 @@ static int depth_of(const OutputNode &out, const NodeRef &k) {
     switch (k.kind) {
         case NodeRef::Shader: return out.shaders[k.index].depth;
         case NodeRef::Layout: return out.nested[k.index].depth;
-        case NodeRef::Web: return 1;
+        case NodeRef::Web: return out.webs[k.index].depth;
         default: return 0;
     }
 }
@@ -1410,7 +1416,11 @@ static NodeRef node_child(const Stateful &l, OutputNode &out, uint64_t pts, std:
     } else if (l.kind == Stateful::WebView) {
         WebParams w;
         w.instance = l.web;
-        for (const Stateful &c : l.children) w.children.push_back(node_child(c, out, pts, err));
+        for (const Stateful &c : l.children) {
+            const NodeRef k = node_child(c, out, pts, err);
+            w.depth = std::max(w.depth, depth_of(out, k) + 1);
+            w.children.push_back(k);
+        }
         ch = {NodeRef::Web, (int)out.webs.size()};
         out.webs.push_back(std::move(w));
     } else if (l.kind == Stateful::Shader) {

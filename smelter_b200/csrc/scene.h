@@ -333,7 +333,7 @@ struct Stateful {
     OptF image_width, image_height;
     ImageParams image;                        // ... and what it resolved to
     std::shared_ptr<WebInstance> web;         // WebView: the instance; `children` are its embedded components (render
-                                              // nodes of their own, never laid out)
+                                              // nodes of their own, not laid out by the WebView's parent)
     std::shared_ptr<const ShaderProgram> shader;   // Shader: the program; `children` are its textures (render nodes)
     std::optional<ShaderParamValue> shader_param;
     // View
@@ -369,7 +369,7 @@ struct NodeRef {
 };
 
 // A layout node (scene_state.rs:154-228, NodeParams::Layout): an output's root that is a layout, or a View, Tiles or
-// Rescaler whose parent is a Shader.  Its own clone of the stateful component, its size (the output's resolution for the
+// Rescaler whose parent is a Shader or a WebView.  Its own clone of the stateful component, its size (the output's resolution for the
 // root; node_size at the last render's pts, the component's width and height, otherwise), its node children in DFS order,
 // and its depth (1 + its deepest child's; unused for the root).  A node below the root is composited into its own texture
 // every tick.  smr_set_layouts gives the root's flattened layouts and resolution instead, used as they are.
@@ -385,15 +385,17 @@ struct LayoutParams {
     std::vector<RenderLayout> layouts(uint64_t pts, const std::vector<std::optional<Resolution>> &inputs);
 };
 
-// A WebView render node (state/node.rs:127-141, NodeParams::Web): the instance and its children, each its own node
+// A WebView render node (state/node.rs:127-141, NodeParams::Web): the instance and its children, each its own node.
+// depth: 1 + the deepest child's, as for ShaderParams.
 struct WebParams {
     std::shared_ptr<WebInstance> instance;
-    std::vector<NodeRef> children;            // Input, Text or Image nodes
+    std::vector<NodeRef> children;            // Input, Text, Image or Layout nodes
+    int depth = 1;
 };
 
 // A Shader render node (state/node.rs, NodeParams::Shader): the program, the parameter bytes, the node's resolution
 // (Size as Resolution: `as usize`) and its children, each its own node.  depth: 1 + the deepest child's (an input, text or
-// image 0, a web node 1), so that a tick draws every child before the shader that reads it.
+// image 0; a web, shader or layout node its own), so that a tick draws every child before the node that reads it.
 struct ShaderParams {
     std::shared_ptr<const ShaderProgram> shader;
     std::vector<uint8_t> param_bytes;

@@ -327,8 +327,11 @@ class ImageComponent:
 @dataclass
 class WebViewComponent:
     """A WebView component (scene/components.rs:55-61): the web renderer instance registered as `instance_id`
-    (Renderer.register_web_renderer) at its resolution, with `children` (InputStream, Image or Text components, each with
-    an id) drawn at the instance's child rects (Renderer.set_web_child_rects)."""
+    (Renderer.register_web_renderer) at its resolution, with `children` (each with an id) drawn at the instance's child
+    rects (Renderer.set_web_child_rects).  A child is an InputStream, Image or Text component, or a View, Tiles or Rescaler
+    with both width and height (Tiles: width and height; View and Rescaler: the position's), which is a layout node of its
+    own and may hold any component, Shaders and WebViews included.  A WebView or Shader child, and a View, Tiles or
+    Rescaler child without both sides, raise RendererError with status SMR_ERR_UNSUPPORTED."""
     id: Optional[str] = None
     instance_id: str = ""
     children: List["Component"] = field(default_factory=list)
