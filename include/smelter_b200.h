@@ -290,12 +290,32 @@ smr_status smr_unregister_input(smr_renderer *r, const char *input_id);
  * node that resolved it: unregistering removes the registry entry only, scenes already showing the asset keep drawing it,
  * and its device memory is released on the handle's stream after the last tick that reads it.  Registering the same id
  * again makes a new asset: a scene updated afterwards restarts its animation (Arc::ptr_eq, image_component.rs:100-111).
- * Not supported: SVG assets (the reference rasterises them at the node's resolution, known only at scene update,
- * svg_image.rs:262-292), URL / file sources (ImageSource). */
+ * SVG assets register through smr_register_svg_image below, into the same registry; smr_unregister_image removes
+ * either kind.  Not supported: URL / file sources (ImageSource). */
 typedef struct { const void *rgba; uint32_t pitch; uint64_t delay_ns; } smr_image_frame;   /* pitch 0 = packed */
 typedef struct { uint32_t width, height; const smr_image_frame *frames; uint32_t n_frames; } smr_image_spec;
 smr_status smr_register_image(smr_renderer *r, const char *image_id, const smr_image_spec *spec);
 smr_status smr_unregister_image(smr_renderer *r, const char *image_id);
+
+/* Renderer::register_renderer for RendererSpec::Image with ImageType::Svg (transformations/image/svg_image.rs).  SVG
+ * parsing and rasterisation stay with the caller, as text shaping and image decoding do: the library asks for a raster
+ * when the reference would draw one, at the resolution the reference would use.
+ * width x height is the asset's intrinsic size, the parsed tree's size truncated to integers (SvgAsset::resolution); the
+ * node resolution follows from it exactly as for a bitmap asset (see smr_update_scene).
+ * rasterize fills `rgba` (height rows of `pitch` bytes, pitch == 4 * width, zeroed on entry, valid only during the call)
+ * with the asset drawn at width x height, premultiplied RGBA8 as tiny-skia's Pixmap holds it (svg_image.rs:262-292: the
+ * tree scaled by resolution / tree.size in f32), and returns 0; anything else refuses the scene update.  It is called
+ * during smr_update_scene, once per SVG image node of the updated output (the root, layout children, and children of
+ * Shaders, WebViews and layout nodes), with that node's resolution, after the scene has passed every other check: a
+ * refused scene never calls it.  It runs on the calling thread under the handle's lock, so it must not call into the
+ * same handle.  `user` must stay valid until smr_unregister_image of the id, or smr_destroy, returns; after an unregister
+ * the rasteriser is never called again.  A host-only handle calls it too and drops the pixels.
+ * SMR_ERR_INVALID_ARGUMENT: a NULL id, spec or rasterize, a side of 0 or above 16384, an id already registered as any
+ * kind of image (KeyTaken); a failed call registers nothing.  Registering the same id again after an unregister makes a
+ * new asset. */
+typedef int32_t (*smr_svg_rasterize_fn)(void *user, uint32_t width, uint32_t height, uint8_t *rgba, uint32_t pitch);
+typedef struct { uint32_t width, height; smr_svg_rasterize_fn rasterize; void *user; } smr_svg_spec;
+smr_status smr_register_svg_image(smr_renderer *r, const char *image_id, const smr_svg_spec *spec);
 
 /* Renderer::register_renderer / unregister_renderer for RendererSpec::WebRenderer   state.rs:137-143
  * The browser (CEF) stays with the caller, and so does the URL: the library receives what CEF's on_paint delivers (one
@@ -434,7 +454,12 @@ smr_status smr_register_wgsl_shader(smr_renderer *r, const char *shader_id, cons
  * premultiplied (add_premultiplied_alpha.wgsl).  A Bitmap node is drawn by the first smr_render of the output after each
  * smr_update_scene of it.  An Animated node shows, at every tick, the frame whose pts is closest to
  * (pts - start_pts) % duration (the first such frame on a tie); pts - start_pts saturates at 0 where the reference's
- * subtraction would underflow.  A tick whose frame is the one the node texture already holds launches nothing for it. */
+ * subtraction would underflow.  A tick whose frame is the one the node texture already holds launches nothing for it.
+ * An SVG node (smr_register_svg_image) is rasterised by the caller during smr_update_scene at the node's resolution and
+ * drawn once, by the first smr_render of the output after the update, with its start pts and frame 0.  GpuOptimized
+ * converts the raster as the reference's two passes do (remove_premultiplied_alpha.wgsl through UNORM views, then
+ * add_premultiplied_alpha.wgsl through sRGB views); CpuOptimized stores its bytes unchanged.  A rasteriser that returns
+ * non-zero is SMR_ERR_SCENE, smr_last_error naming the image id and the resolution, and leaves the scene as it was. */
 smr_status smr_update_scene(smr_renderer *r, const char *output_id, uint32_t width, uint32_t height,
                             int32_t output_format, const smr_component *scene_root);
 /* Renderer::unregister_output                                       state.rs:115-123 */

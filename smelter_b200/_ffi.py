@@ -78,6 +78,14 @@ class ImageSpec(C.Structure):    # smr_image_spec
     _fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("frames", C.POINTER(ImageFrame)), ("n_frames", C.c_uint32)]
 
 
+# smr_svg_rasterize_fn: (user, width, height, rgba, pitch) -> 0, or anything else to refuse the scene update
+SVG_RASTERIZE_FN = C.CFUNCTYPE(C.c_int32, C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(C.c_uint8), C.c_uint32)
+
+
+class SvgSpec(C.Structure):      # smr_svg_spec
+    _fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("rasterize", SVG_RASTERIZE_FN), ("user", C.c_void_p)]
+
+
 class WebRendererSpec(C.Structure):   # smr_web_renderer_spec
     _fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("embedding_method", C.c_int32)]
 
@@ -216,6 +224,7 @@ class KernelTimes(C.Structure):
 
 EXPORTS = [
     "smr_create", "smr_destroy", "smr_register_input", "smr_unregister_input", "smr_register_image", "smr_unregister_image",
+    "smr_register_svg_image",
     "smr_register_web_renderer", "smr_unregister_web_renderer", "smr_web_set_frame", "smr_web_set_child_rects", "smr_register_shader", "smr_unregister_shader", "smr_register_wgsl_shader", "smr_update_scene",
     "smr_unregister_output", "smr_set_layouts", "smr_render", "smr_render_begin", "smr_render_end", "smr_preprocess_frame", "smr_premultiply_rgba8", "smr_render_text", "smr_debug_partition", "smr_debug_tile_plan", "smr_debug_weights", "smr_debug_sincos", "smr_debug_fused_jobs", "smr_debug_resample_stages", "smr_debug_composite_layers", "smr_debug_interior", "smr_output_plane_sizes",
     "smr_component_default", "smr_debug_layouts", "smr_debug_node_layouts", "smr_debug_image_nodes", "smr_debug_set_inputs", "smr_get_stats", "smr_set_profiling", "smr_get_kernel_times",
@@ -244,6 +253,7 @@ def lib():
     L.smr_unregister_input.argtypes = [vp, C.c_char_p]
     L.smr_register_image.argtypes = [vp, C.c_char_p, C.POINTER(ImageSpec)]
     L.smr_unregister_image.argtypes = [vp, C.c_char_p]
+    L.smr_register_svg_image.argtypes = [vp, C.c_char_p, C.POINTER(SvgSpec)]
     L.smr_register_web_renderer.argtypes = [vp, C.c_char_p, C.POINTER(WebRendererSpec)]
     L.smr_unregister_web_renderer.argtypes = [vp, C.c_char_p]
     L.smr_web_set_frame.argtypes = [vp, C.c_char_p, C.POINTER(WebFrame)]

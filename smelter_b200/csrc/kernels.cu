@@ -1651,6 +1651,14 @@ int launch_text(const TextJob *jobs_dev, const int32_t *tile_begin_dev, int n_jo
 // Image node texture (transformations/image.rs:178-187, add_premultiplied_alpha.wgsl): a full-target quad samples the
 // asset frame (straight alpha) with the linear / clamp-to-edge sampler through the mode's source view, premultiplies and
 // stores through the mode's target view.  When the node and the asset differ in size this pass is also the scaler.
+// An SVG raster (svg_image.rs:144-180, 262-292: premultiplied, at the node's size) is stored unchanged in CpuOptimized;
+// GpuOptimized runs the reference's two full-target passes per pixel:
+//   1. remove_premultiplied_alpha.wgsl through UNORM views: the NC-6u sample, a = max(c.a, 1e-5), clamp(c.rgb / a) and
+//      clamp(c.a), stored as UNORM8 (NC-2);
+//   2. add_premultiplied_alpha.wgsl through sRGB views: pass 1's four bytes decoded as a straight-alpha texel (NC-3) and
+//      premultiply_store.  Pass 2 samples a texture of the target's size at the pixel centre, as pass 1 does: the tap is
+//      texel (x, y) with weight 1 at every size up to 16384 (tests/svg_oracle.c: orc_check_same_size_taps), so the
+//      texel is the byte pass 1 stored for this pixel.
 // Every image node a tick draws is one launch, block -> job as in k_text; one thread per pixel of a 32 x 8 tile.
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) k_image(const ImageJob *__restrict__ jobs, const int32_t *__restrict__ tile_begin, int n_jobs) {
@@ -1662,9 +1670,19 @@ __global__ void __launch_bounds__(256) k_image(const ImageJob *__restrict__ jobs
     const int x = s_origin[0] + (int)threadIdx.x, y = s_origin[1] + (int)threadIdx.y;
     if (x >= J.dst.width || y >= J.dst.height) return;
     bool exact;
-    uchar4 texel;
-    const float4 c = sample_node(T, &J.src, J.dst.mode, ((float)x + 0.5f) / (float)J.dst.width, ((float)y + 0.5f) / (float)J.dst.height, exact, texel);
-    reinterpret_cast<uchar4 *>(J.dst.out + (size_t)y * J.dst.out_pitch)[x] = premultiply_store(T, J.dst.mode, c);
+    uchar4 texel, o;
+    const float tx = ((float)x + 0.5f) / (float)J.dst.width, ty = ((float)y + 0.5f) / (float)J.dst.height;
+    if (!J.raster) {
+        o = premultiply_store(T, J.dst.mode, sample_node(T, &J.src, J.dst.mode, tx, ty, exact, texel));
+    } else if (J.dst.mode != 0) {
+        o = node_texel(T, J.src, x, y);
+    } else {
+        const float4 c = sample_node(T, &J.src, 1, tx, ty, exact, texel);
+        const float a = fmaxf(c.w, 0.00001f);
+        const uchar4 s = make_uchar4(unorm8(c.x / a), unorm8(c.y / a), unorm8(c.z / a), unorm8(c.w));   // unorm8 clamps
+        o = premultiply_store(T, 0, make_float4(T.dec[s.x], T.dec[s.y], T.dec[s.z], T.u8n[s.w]));
+    }
+    reinterpret_cast<uchar4 *>(J.dst.out + (size_t)y * J.dst.out_pitch)[x] = o;
 }
 
 int launch_image(const ImageJob *jobs_dev, const int32_t *tile_begin_dev, int n_jobs, int n_tiles, Stream s) {

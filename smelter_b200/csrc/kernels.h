@@ -244,7 +244,8 @@ struct TextJob {
 // ImageNode::render (transformations/image.rs:178-187): one asset frame drawn into a node texture of the node's resolution
 struct ImageJob {
     NodeTarget dst;               // the node's resolution
-    Tex src;                      // the frame: TEX_RGBA8, straight alpha
+    Tex src;                      // the frame: TEX_RGBA8, straight alpha; with `raster`, premultiplied and of dst's size
+    int32_t raster;               // 1: src is an SVG raster (svg_image.rs:144-167), 0: an asset frame
 };
 
 // One plane of WebRendererShader::render (web_renderer/shader.rs:53-114): a quad of the plane mesh through its vertex

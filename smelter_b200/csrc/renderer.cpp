@@ -386,6 +386,7 @@ class Renderer {
     smr_status register_input(const char *id);
     smr_status unregister_input(const char *id);
     smr_status register_image(const char *id, const smr_image_spec *spec);
+    smr_status register_svg_image(const char *id, const smr_svg_spec *spec);
     smr_status unregister_image(const char *id);
     smr_status register_web_renderer(const char *id, const smr_web_renderer_spec *spec);
     smr_status unregister_web_renderer(const char *id);
@@ -904,6 +905,24 @@ smr_status Renderer::register_image(const char *id, const smr_image_spec *spec) 
     return SMR_OK;
 }
 
+// An SVG asset: its intrinsic size and the caller's rasteriser, in the registry bitmap assets use; nothing is drawn until
+// a scene update resolves a node of it (make_image_node)
+smr_status Renderer::register_svg_image(const char *id, const smr_svg_spec *spec) {
+    if (!id || !spec || !spec->rasterize) return SMR_ERR_INVALID_ARGUMENT;
+    std::lock_guard<std::mutex> g(mu_);
+    if (spec->width == 0 || spec->height == 0 || spec->width > 16384 || spec->height > 16384) {
+        set_error("SVG image resolution out of range");
+        return SMR_ERR_INVALID_ARGUMENT;
+    }
+    auto a = std::make_shared<ImageAsset>();
+    a->width = spec->width; a->height = spec->height;
+    a->frame_pts.push_back(0);
+    a->rasterize = spec->rasterize; a->user = spec->user;
+    a->svg_id = id;
+    if (!scene_.register_image(id, std::move(a))) { set_error("an image with this id is already registered"); return SMR_ERR_INVALID_ARGUMENT; }
+    return SMR_OK;
+}
+
 smr_status Renderer::unregister_image(const char *id) {
     if (!id) return SMR_ERR_INVALID_ARGUMENT;
     std::lock_guard<std::mutex> g(mu_);
@@ -1125,7 +1144,9 @@ smr_status Renderer::update_scene(const char *output_id, uint32_t w, uint32_t h,
     for (const auto &p : payloads)
         if (smr_status st = make_text_node(p, atlases, made[p.get()]); st != SMR_OK) return st;
     OutputNode node;
-    // image nodes have the resolution the scene state resolves; a node texture that cannot be allocated drops the update
+    // image nodes have the resolution the scene state resolves; a node texture that cannot be allocated, or an SVG raster
+    // the caller refuses, drops the update.  The image nodes come last, so that a rasteriser sees only scenes that passed
+    // every other check.
     std::vector<std::unique_ptr<ImageNode>> images;
     std::vector<std::unique_ptr<WebNode>> webs;
     std::vector<std::unique_ptr<ShaderNode>> shaders;
@@ -1138,8 +1159,8 @@ smr_status Renderer::update_scene(const char *output_id, uint32_t w, uint32_t h,
         return true;
     };
     auto make_images = [&](OutputNode &n) {
-        return make_all(n.images, images, &Renderer::make_image_node) && make_all(n.webs, webs, &Renderer::make_web_node) &&
-               make_all(n.shaders, shaders, &Renderer::make_shader_node);
+        return make_all(n.webs, webs, &Renderer::make_web_node) && make_all(n.shaders, shaders, &Renderer::make_shader_node) &&
+               make_all(n.images, images, &Renderer::make_image_node);
     };
     if (!scene_.update_scene(output_id, c, {w, h}, node, err, make_images)) {
         if (image_st != SMR_OK) return image_st;
@@ -1228,15 +1249,37 @@ smr_status Renderer::make_text_node(const std::shared_ptr<const TextPayload> &p,
     return SMR_OK;
 }
 
-// An image node for `p`: its node texture, and the job that draws a frame of the asset into it
+// An image node for `p`: its node texture, and the job that draws a frame of the asset into it.  An SVG asset is
+// rasterised here by the caller at the node's resolution (SvgNodeState: one render per scene update) and the raster is
+// copied after the node texture, in its memory (pageable source: staged before the call returns); a host-only handle
+// drops it.  A rasteriser that refuses drops the update.
 smr_status Renderer::make_image_node(const ImageParams &p, std::unique_ptr<ImageNode> &out) {
     auto n = std::make_unique<ImageNode>();
     n->params = p;
     dev::ImageJob &J = n->job;
-    J.src.kind = dev::TEX_RGBA8; J.src.width = (int)p.asset->width; J.src.height = (int)p.asset->height;
-    J.src.pitch0 = (int)p.asset->width * 4;
-    if (smr_status st = make_node_texture((int)p.resolution.width, (int)p.resolution.height, false, 0, *n, J.dst); st != SMR_OK)
-        return st;
+    const ImageAsset &a = *p.asset;
+    const int w = (int)p.resolution.width, h = (int)p.resolution.height;
+    if (!a.svg()) {
+        J.src.kind = dev::TEX_RGBA8; J.src.width = (int)a.width; J.src.height = (int)a.height; J.src.pitch0 = (int)a.width * 4;
+        if (smr_status st = make_node_texture(w, h, false, 0, *n, J.dst); st != SMR_OK) return st;
+        out = std::move(n);
+        return SMR_OK;
+    }
+    const size_t bytes = (size_t)w * h * 4;
+    std::vector<uint8_t> raster(bytes, 0);
+    if (a.rasterize(a.user, (uint32_t)w, (uint32_t)h, raster.data(), (uint32_t)w * 4) != 0) {
+        set_error("SVG image \"" + a.svg_id + "\": the rasteriser refused a raster of " + std::to_string(w) + " x " + std::to_string(h));
+        return SMR_ERR_SCENE;
+    }
+    J.raster = 1;
+    J.src.kind = dev::TEX_RGBA8; J.src.width = w; J.src.height = h; J.src.pitch0 = w * 4;
+    if (smr_status st = make_node_texture(w, h, false, bytes, *n, J.dst); st != SMR_OK) return st;
+    if (!host_only_) {
+        uint8_t *dst = J.dst.out + node_texture_bytes(w, h);
+        CUDA_OK(cudaMemcpyAsync(dst, raster.data(), bytes, cudaMemcpyHostToDevice, stream_));
+        stats_.h2d_bytes += bytes;
+        J.src.p0 = dst;
+    }
     out = std::move(n);
     return SMR_OK;
 }
@@ -1331,8 +1374,8 @@ void Renderer::plan_shader_node(Output &o, ShaderNode &n, uint64_t pts) {
 
 // A tick that renders output `o` at `pts`: each of its text, image, web and shader nodes enters the texture table.  The text nodes
 // not drawn since the last smr_update_scene join the tick's text launch; the image nodes whose frame at `pts` (a Bitmap's
-// only frame; AnimatedAsset::render's choice) is not the one their texture holds join its image launch; the web nodes whose
-// instance has a frame join its web launch of their depth.
+// or an SVG raster's only frame; AnimatedAsset::render's choice) is not the one their texture holds join its image
+// launch; the web nodes whose instance has a frame join its web launch of their depth.
 void Renderer::plan_node_textures(Output &o, uint64_t pts) {
     if (o.nodes_planned == tick_) return;
     o.nodes_planned = tick_;
@@ -1355,7 +1398,7 @@ void Renderer::plan_node_textures(Output &o, uint64_t pts) {
         if (frame == n->held) continue;
         n->held_before = n->held;
         n->held = frame;   // undone if the tick fails before its launch
-        n->job.src.p0 = (const uint8_t *)a.pixels.get() + (size_t)a.width * a.height * 4 * frame;
+        if (!a.svg()) n->job.src.p0 = (const uint8_t *)a.pixels.get() + (size_t)a.width * a.height * 4 * frame;
         plan_.images.push_back(n.get());
     }
     for (auto &t : o.texts) {
@@ -3397,6 +3440,7 @@ void smr_destroy(smr_renderer *r) { delete r; }
 smr_status smr_register_input(smr_renderer *r, const char *id) { SMR_GUARD(r->impl.register_input(id)) }
 smr_status smr_unregister_input(smr_renderer *r, const char *id) { SMR_GUARD(r->impl.unregister_input(id)) }
 smr_status smr_register_image(smr_renderer *r, const char *id, const smr_image_spec *spec) { SMR_GUARD(r->impl.register_image(id, spec)) }
+smr_status smr_register_svg_image(smr_renderer *r, const char *id, const smr_svg_spec *spec) { SMR_GUARD(r->impl.register_svg_image(id, spec)) }
 smr_status smr_unregister_image(smr_renderer *r, const char *id) { SMR_GUARD(r->impl.unregister_image(id)) }
 smr_status smr_register_web_renderer(smr_renderer *r, const char *id, const smr_web_renderer_spec *spec) {
     SMR_GUARD(r->impl.register_web_renderer(id, spec))

@@ -106,13 +106,20 @@ struct TextPayload {
     int32_t color_mode = 0;
 };
 
-// A registered image (transformations/image.rs: Image::Bitmap for one frame, Image::Animated for more).  Scene nodes hold
-// it by shared_ptr, and the identity of the object is what state inheritance compares (Arc::ptr_eq).
+// A registered image (transformations/image.rs: Image::Bitmap for one frame, Image::Animated for more, Image::Svg with a
+// rasteriser).  Scene nodes hold it by shared_ptr, and the identity of the object is what state inheritance compares
+// (Arc::ptr_eq).
 struct ImageAsset {
-    uint32_t width = 0, height = 0;
+    uint32_t width = 0, height = 0;    // Svg: the intrinsic size
     std::vector<uint64_t> frame_pts;   // AnimationFrame::pts, the sum of the delays before each frame; one entry for a Bitmap
+                                       // or an Svg
     uint64_t duration = 1;             // animation_duration (animated_image.rs:101-104)
-    std::shared_ptr<void> pixels;      // device memory: the frames, straight-alpha RGBA8, packed, one after the other (host-only: null)
+    std::shared_ptr<void> pixels;      // device memory: the frames, straight-alpha RGBA8, packed, one after the other (host-only
+                                       // or Svg: null)
+    smr_svg_rasterize_fn rasterize = nullptr;   // Svg: the caller's rasteriser and its `user`, called per node at scene update
+    void *user = nullptr;
+    std::string svg_id;                // Svg: the id it was registered under, named when its rasteriser refuses
+    bool svg() const { return rasterize != nullptr; }
     bool animated() const { return frame_pts.size() > 1; }
     // AnimatedAsset::render's frame choice (animated_image.rs:120-136); pts - start_pts saturates at 0
     size_t frame_at(uint64_t pts, uint64_t start_pts) const;

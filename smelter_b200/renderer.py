@@ -600,6 +600,7 @@ class Renderer:
         if st != F.SMR_OK:
             raise RendererError(st, (self._lib.smr_last_error(None) or b"").decode())
         self._outputs: Dict[str, Tuple[Resolution, int]] = {}
+        self._svg_rasterizers = {}
         self.opts = opts
 
     def close(self):
@@ -640,8 +641,29 @@ class Renderer:
         spec = F.ImageSpec(w, h, arr, len(frames))
         self._check(self._lib.smr_register_image(self._h, image_id.encode(), C.byref(spec)))
 
+    def register_svg_image(self, image_id: str, width: int, height: int, rasterize):
+        """Renderer::register_renderer for ImageType::Svg: the caller parses the SVG.  (width, height) is its intrinsic
+        size (the tree's size truncated); `rasterize(w, h)` returns the asset drawn at w x h as an (h, w, 4) uint8
+        premultiplied array.  It is called during update_scene, once per SVG node, with the node's resolution; an exception
+        or an array of another shape or dtype refuses the update (RendererError, SMR_ERR_SCENE)."""
+        def trampoline(user, w, h, rgba, pitch):
+            try:
+                px = np.asarray(rasterize(int(w), int(h)))
+                if px.dtype != np.uint8 or px.shape != (h, w, 4):
+                    return 1
+                dst = np.ctypeslib.as_array(rgba, shape=(h, pitch))
+                dst[:, :w * 4] = px.reshape(h, w * 4)
+                return 0
+            except Exception:
+                return 1
+        fn = F.SVG_RASTERIZE_FN(trampoline)
+        spec = F.SvgSpec(int(width), int(height), fn, None)
+        self._check(self._lib.smr_register_svg_image(self._h, image_id.encode(), C.byref(spec)))
+        self._svg_rasterizers[image_id] = fn     # called back until the id is unregistered
+
     def unregister_image(self, image_id: str):
         self._check(self._lib.smr_unregister_image(self._h, image_id.encode()))
+        self._svg_rasterizers.pop(image_id, None)
 
     def register_web_renderer(self, instance_id: str, width: int, height: int, embedding_method=F.WEB_NATIVE_OVER_CONTENT):
         """Renderer::register_renderer for RendererSpec::WebRenderer: the browser and its URL stay with the caller, which
