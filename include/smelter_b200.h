@@ -390,7 +390,10 @@ smr_status smr_unregister_shader(smr_renderer *r, const char *shader_id);
  * vs_main without exactly one VertexInput, a group(1) binding(0) that is not var<uniform>); smr_last_error names the
  * line and column.  SMR_ERR_UNSUPPORTED for valid WGSL outside the subset, named in smr_last_error: derivatives
  * (dpdx, fwidth, ...), storage buffers, atomics, override, pointers, textures and bindings other than the header's and
- * the uniform, f16, and builtins not listed in the WGSL section of DESIGN.md.
+ * the uniform, f16, and builtins not in the list of accepted builtins in DESIGN.md ("WGSL builtins"), which states each
+ * one's exact rule.  textureSampleBias is fragment-only: vs_main, or a function it calls, using it is
+ * SMR_ERR_INVALID_ARGUMENT; textureSample, textureSampleLevel, textureSampleGrad and textureSampleBaseClampToEdge may
+ * also be used in vs_main.  textureGather's component must be a const-expression in 0..3 (SMR_ERR_INVALID_ARGUMENT).
  * The parameter type is the uniform's WGSL type: scalars, vectors (a LIST of exactly N scalars), matrices (a LIST of
  * exactly R rows of C scalars), arrays (a LIST of at most N) and structs, validated as validation.rs does.  The bytes
  * stay ShaderParam::to_bytes (tight); the shader reads them at WGSL uniform-address-space offsets (AlignOf, SizeOf,

@@ -303,6 +303,23 @@ __device__ __forceinline__ float4 sample_node(const Tables &T, const Tex *tex, i
     return r;
 }
 
+// textureGather(c, ...) of a child through the same view: component c of the four texels of sample_node's bilinear
+// footprint (NC-6's taps, clamped to the edge), in the order (i0, i1), (i1, i1), (i1, i0), (i0, i0) of (x, y).  Each texel
+// is decoded as a sample's taps are (NC-3 colour in GpuOptimized, NC-1 otherwise and for alpha); a YUV texture goes
+// through node_texel, the per-texel fetch of sample_node's bilinear path.
+__device__ __forceinline__ float4 gather_node(const Tables &T, const Tex *tex, int mode, float tx, float ty, int c) {
+    if (tex == nullptr || tex->kind == TEX_NONE) return make_float4(0.f, 0.f, 0.f, 0.f);  // default_empty_view
+    const LinTap ax = linear_tap(tx, tex->width), ay = linear_tap(ty, tex->height);
+    const float *lut = mode == 0 && c < 3 ? T.dec : T.u8n;
+    float r[4];
+#pragma unroll 1
+    for (int k = 0; k < 4; k++) {   // one node_texel in the code: a YUV fetch is long
+        const uchar4 p = node_texel(T, *tex, k == 1 || k == 2 ? ax.i1 : ax.i0, k < 2 ? ay.i1 : ay.i0);
+        r[k] = lut[c == 0 ? p.x : c == 1 ? p.y : c == 2 ? p.z : p.w];
+    }
+    return make_float4(r[0], r[1], r[2], r[3]);
+}
+
 // PREMULTIPLIED_ALPHA_BLENDING through the target's view: decode dst -> blend -> encode (per layer)
 __device__ __forceinline__ uchar4 blend(const Tables &T, int mode, uchar4 dst, float4 s) {
     s.x = clamp01(s.x); s.y = clamp01(s.y); s.z = clamp01(s.z); s.w = clamp01(s.w);

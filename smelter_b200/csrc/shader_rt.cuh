@@ -54,6 +54,8 @@ __device__ float4 smr_fragment(smr_fragment_in in, const smr_base_params &base, 
 //    vertex's.  @builtin(position) is (x + 1/2, y + 1/2, depth, s).
 //  - Each covered fragment runs fs_main; unless it discards, its value is blended (PREMULTIPLIED_ALPHA_BLENDING) and
 //    stored as 8 bits, in plane order and, within a plane, triangle order.
+// Two blocks per SM are enough to hide the prologue's barriers; asking for no more lets ptxas keep a vertex stage that
+// samples textures (textureSampleLevel / Grad) and a gather-heavy fragment stage in registers, without spills.
 struct wg_tri {
     long long x[3], y[3];   // snapped window coordinates, 1/256 px
     long long area;         // doubled, of the front-facing (sign-normalised) triangle: > 0
@@ -76,8 +78,8 @@ __device__ inline long long wg_edge(const wg_tri &t, int a, int b, long long px,
     return sgn * ((t.x[b] - t.x[a]) * (py - t.y[a]) - (t.y[b] - t.y[a]) * (px - t.x[a]));
 }
 
-extern "C" __global__ void __launch_bounds__(256) smr_shader_main(const smr::dev::ShaderJob *__restrict__ jobs,
-                                                                  const int *__restrict__ tile_begin, int n_jobs) {
+extern "C" __global__ void __launch_bounds__(256, 2) smr_shader_main(const smr::dev::ShaderJob *__restrict__ jobs,
+                                                                     const int *__restrict__ tile_begin, int n_jobs) {
     constexpr int NV = WG_NVARY > 0 ? WG_NVARY : 1;
     __shared__ smr::dev::Tables T;
     __shared__ smr::dev::ShaderJob J;

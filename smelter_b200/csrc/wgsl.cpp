@@ -219,6 +219,8 @@ struct Expr {
     Ty target;
     std::string code;             // what emit() returns when not an abstract value
     bool uref = false;            // the uniform, or a member / element of it: `code` is its byte offset
+    bool cint = false;            // a concrete integer constant (suffixed literal or const), whose value is civ
+    long long civ = 0;
 };
 
 struct Stmt;
@@ -764,6 +766,7 @@ struct StructInfo {
     std::vector<FieldInfo> fields;
     int line = 0, col = 0;
     bool resolved = false;
+    std::string cname;   // a predeclared result struct (frexp, modf): its wgsl_rt.cuh type
 };
 
 struct Sym {
@@ -773,6 +776,8 @@ struct Sym {
     bool has_cv = false;
     CV cv;
     std::string code;
+    bool cint = false;   // a constant of concrete integer type, whose value is civ
+    long long civ = 0;
 };
 
 struct FnInfo {
@@ -780,23 +785,21 @@ struct FnInfo {
     std::vector<Ty> params;
     Ty ret;
     std::string cname;
+    std::vector<std::string> calls;   // the user functions it calls
+    int frag_line = 0, frag_col = 0;  // its first fragment-only builtin, if any
 };
 
 const char *kUnsupportedFns[] = {"dpdx", "dpdy", "fwidth", "dpdxCoarse", "dpdyCoarse", "dpdxFine", "dpdyFine", "fwidthCoarse",
                                  "fwidthFine", "atomicLoad", "atomicStore", "atomicAdd", "atomicSub", "atomicMax", "atomicMin",
                                  "atomicAnd", "atomicOr", "atomicXor", "atomicExchange", "atomicCompareExchangeWeak",
-                                 "textureLoad", "textureSampleLevel", "textureSampleBias", "textureSampleGrad",
-                                 "textureSampleCompare", "textureSampleCompareLevel", "textureSampleBaseClampToEdge",
-                                 "textureGather", "textureGatherCompare", "textureStore", "textureNumLayers",
-                                 "textureNumLevels", "textureNumSamples", "arrayLength", "workgroupBarrier",
-                                 "storageBarrier", "textureBarrier", "workgroupUniformLoad", "ldexp", "frexp", "modf",
-                                 "fma", "determinant", "faceForward", "reflect", "refract", "quantizeToF16", "pack4x8snorm",
-                                 "pack4x8unorm", "pack2x16snorm", "pack2x16unorm", "pack2x16float", "unpack4x8snorm",
-                                 "unpack4x8unorm", "unpack2x16snorm", "unpack2x16unorm", "unpack2x16float", "countLeadingZeros",
-                                 "countOneBits", "countTrailingZeros", "extractBits", "insertBits", "firstLeadingBit",
-                                 "firstTrailingBit", "reverseBits", "dot4U8Packed", "dot4I8Packed", "saturate", "sinh",
-                                 "cosh", "tanh", "asinh", "acosh", "atanh", "degrees", "radians", "subgroupAdd",
+                                 "textureLoad", "textureSampleCompare", "textureSampleCompareLevel", "textureGatherCompare",
+                                 "textureStore", "textureNumLayers", "textureNumSamples", "arrayLength", "workgroupBarrier",
+                                 "storageBarrier", "textureBarrier", "workgroupUniformLoad", "subgroupAdd",
                                  "subgroupBroadcast", "f16", "ptr", "atomic"};
+// the texture builtins: their texture and sampler arguments are checked where they are translated
+const std::set<std::string> kTextureFns = {"textureSample", "textureSampleLevel", "textureSampleBias", "textureSampleGrad",
+                                           "textureSampleBaseClampToEdge", "textureGather", "textureDimensions",
+                                           "textureNumLevels"};
 
 struct Checker {
     Module &m;
@@ -805,7 +808,7 @@ struct Checker {
     std::vector<std::map<std::string, Sym>> scopes;
     std::map<std::string, FnInfo> fns;
     std::string out_structs, out_consts, out_loaders, out_protos, out_bodies;
-    const FnInfo *cur_fn = nullptr;
+    FnInfo *cur_fn = nullptr;
     std::string cur_stage;            // "vertex", "fragment" or "" (a helper)
     std::vector<int> loops;           // label numbers of the enclosing loops (-1: a switch)
     int label = 0;
@@ -853,7 +856,7 @@ struct Checker {
             case Ty::Vec: return "wv<" + cscalar(t.s) + ", " + std::to_string(t.n) + ">";
             case Ty::Mat: return "wm<" + std::to_string(t.n) + ", " + std::to_string(t.m) + ">";
             case Ty::Arr: return "wa<" + cty(*t.el) + ", " + std::to_string(t.n) + ">";
-            case Ty::Struct: return "S_" + structs[t.sid].name;
+            case Ty::Struct: return structs[t.sid].cname.empty() ? "S_" + structs[t.sid].name : structs[t.sid].cname;
             default: return "void";
         }
     }
@@ -1131,6 +1134,13 @@ struct Checker {
         invalid(at->line, at->col, "mismatched operand types " + sname(a) + " and " + sname(b));
     }
 
+    // a const of concrete integer type keeps its value, for the builtins that need a const-expression (textureGather)
+    void const_int(Sym &sym, const ExprP &init) {
+        if (sym.ty.k != Ty::Scalar || !integral(sym.ty.s)) return;
+        if (init->has_cv && !init->cv.f && !init->cv.n) { sym.cint = true; sym.civ = init->cv.iv[0]; }
+        else if (init->cint) { sym.cint = true; sym.civ = init->civ; }
+    }
+
     // ---- expressions ----
     Ty set(const ExprP &e, const Ty &t) { e->ty = t; return t; }
     Ty set_cv(const ExprP &e, const CV &cv) {
@@ -1158,6 +1168,8 @@ struct Checker {
                 if (e->suf.empty()) return set_cv(e, cv);
                 SK s = e->suf == "f" ? S_F32 : e->suf == "i" ? S_I32 : S_U32;   // a suffixed literal is concrete
                 e->code = lit(cv, 0, s, e->line, e->col);
+                e->cint = s != S_F32;
+                e->civ = e->iv;
                 return set(e, scalar(s));
             }
             case Expr::Id: {
@@ -1169,6 +1181,8 @@ struct Checker {
                 if (s->has_cv) { e->has_cv = true; e->cv = s->cv; return set(e, s->ty); }
                 e->code = s->code;
                 e->uref = s->k == Sym::Uniform;
+                e->cint = s->cint;
+                e->civ = s->civ;
                 return set(e, s->ty);
             }
             case Expr::Un: return check_unary(e);
@@ -1411,7 +1425,7 @@ struct Checker {
         const std::string &n = c->name;
         for (const char *u : kUnsupportedFns) if (n == u) unsupported(e->line, e->col, n);
         std::vector<Ty> A;
-        if (n != "textureSample" && n != "textureDimensions")
+        if (!kTextureFns.count(n))
             for (auto &x : e->a) A.push_back(check(x));
         auto args = [&](const std::vector<Ty> &to) {
             std::string s;
@@ -1430,6 +1444,7 @@ struct Checker {
             if (uf->second.d->attrs.size() && (find_attr(uf->second.d->attrs, "vertex") || find_attr(uf->second.d->attrs, "fragment")))
                 invalid(e->line, e->col, "an entry point cannot be called");
             nargs(uf->second.params.size());
+            if (cur_fn) cur_fn->calls.push_back(n);
             std::string s = args(uf->second.params);
             e->code = uf->second.cname + "(ctx" + (s.empty() ? "" : ", " + s) + ")";
             return set(e, uf->second.ret);
@@ -1583,26 +1598,79 @@ struct Checker {
             e->code = cty(t) + "{{" + args(to) + "}}";
             return set(e, t);
         }
-        // texture builtins
+        // texture builtins: textures[i] and the sampler, as the header declares them
+        auto tex_arg = [&](size_t i) {
+            Ty tt = check(e->a[i]);
+            if (tt.k != Ty::Tex || e->a[i]->k != Expr::Idx) invalid(e->line, e->col, n + " takes textures[i]");
+            return "(unsigned)(" + e->a[i]->code + ")";
+        };
+        auto samp_arg = [&](size_t i) {
+            if (check(e->a[i]).k != Ty::Samp) invalid(e->line, e->col, n + " takes the sampler");
+        };
+        auto val_arg = [&](size_t i, const Ty &t) {
+            check(e->a[i]);
+            conv(e->a[i], t);
+            return code(e->a[i]);
+        };
         if (n == "textureSample") {
             nargs(3);
-            Ty tt = check(e->a[0]), ts = check(e->a[1]), tu = check(e->a[2]);
-            if (tt.k != Ty::Tex || e->a[0]->k != Expr::Idx) invalid(e->line, e->col, "textureSample takes textures[i]");
-            if (ts.k != Ty::Samp) invalid(e->line, e->col, "textureSample takes the sampler");
-            conv(e->a[2], vec(S_F32, 2));
-            e->code = "ctx.tex.sample((unsigned)(" + e->a[0]->code + "), " + code(e->a[2]) + ")";
+            std::string t = tex_arg(0);
+            samp_arg(1);
+            e->code = "ctx.tex.sample(" + t + ", " + val_arg(2, vec(S_F32, 2)) + ")";
             return set(e, vec(S_F32, 4));
         }
-        if (n == "textureDimensions") {
-            if (e->a.size() != 1) unsupported(e->line, e->col, "textureDimensions with a level");
-            Ty tt = check(e->a[0]);
-            if (tt.k != Ty::Tex || e->a[0]->k != Expr::Idx) invalid(e->line, e->col, "textureDimensions takes textures[i]");
-            e->code = "ctx.tex.dims((unsigned)(" + e->a[0]->code + "))";
+        if (n == "textureSampleLevel" || n == "textureSampleBias" || n == "textureSampleGrad" || n == "textureSampleBaseClampToEdge" ||
+            n == "textureGather") {
+            const bool gather = n == "textureGather";
+            const size_t k = n == "textureSampleGrad" ? 5 : n == "textureSampleBaseClampToEdge" ? 3 : 4;
+            if (e->a.size() == k + 1 && n != "textureSampleBaseClampToEdge") unsupported(e->line, e->col, n + " with an offset");
+            nargs(k);
+            std::string comp;
+            if (gather) {   // textureGather(component, t, s, coords): the component is a const-expression in 0..3
+                const ExprP &c = e->a[0];
+                Ty ct = check(c);
+                if (ct.k != Ty::Scalar || !integral(ct.s)) invalid(c->line, c->col, "textureGather's component must be i32 or u32, found " + tname(ct));
+                long long v;
+                if (c->has_cv && !c->cv.f && !c->cv.n) v = c->cv.iv[0];
+                else if (c->cint) v = c->civ;
+                else invalid(c->line, c->col, "textureGather's component must be a const-expression");
+                if (v < 0 || v > 3) invalid(c->line, c->col, "textureGather's component must be 0, 1, 2 or 3, found " + std::to_string(v));
+                comp = std::to_string(v) + ", ";
+            }
+            const size_t o = gather ? 1 : 0;
+            std::string t = tex_arg(o);
+            samp_arg(o + 1);
+            std::string a = t + ", " + val_arg(o + 2, vec(S_F32, 2));
+            if (n == "textureSampleBias" && cur_fn && !cur_fn->frag_line) { cur_fn->frag_line = e->line; cur_fn->frag_col = e->col; }
+            if (n == "textureSampleLevel" || n == "textureSampleBias") a += ", " + val_arg(3, scalar(S_F32));
+            if (n == "textureSampleGrad") a += ", " + val_arg(3, vec(S_F32, 2)) + ", " + val_arg(4, vec(S_F32, 2));
+            const char *m = n == "textureSampleLevel" ? "sample_level" : n == "textureSampleBias" ? "sample_bias" :
+                            n == "textureSampleGrad" ? "sample_grad" : gather ? "gather" : "sample_clamped";
+            e->code = std::string("ctx.tex.") + m + "(" + comp + a + ")";
+            return set(e, vec(S_F32, 4));
+        }
+        if (n == "textureDimensions" || n == "textureNumLevels") {
+            const bool dims = n == "textureDimensions";
+            if (e->a.size() != 1 && !(dims && e->a.size() == 2)) nargs(1);
+            std::string t = tex_arg(0);
+            if (!dims) {
+                e->code = "ctx.tex.levels(" + t + ")";
+                return set(e, scalar(S_U32));
+            }
+            if (e->a.size() == 2) {   // any level: a node texture's size (levels are clamped to its one level)
+                Ty l = check(e->a[1]);
+                if (l.k != Ty::Scalar || !integral(l.s)) invalid(e->a[1]->line, e->a[1]->col, "textureDimensions' level must be i32 or u32, found " + tname(l));
+                conv_default(e->a[1]);
+                t += ", " + code(e->a[1]);
+            }
+            e->code = "ctx.tex.dims(" + t + ")";
             return set(e, vec(S_U32, 2));
         }
         // math builtins
         static const std::set<std::string> f1 = {"floor", "ceil", "fract", "round", "trunc", "sqrt", "inverseSqrt", "exp", "exp2",
-                                                 "log", "log2", "sin", "cos", "tan", "asin", "acos", "atan"};
+                                                 "log", "log2", "sin", "cos", "tan", "asin", "acos", "atan", "saturate",
+                                                 "degrees", "radians", "sinh", "cosh", "tanh", "asinh", "acosh", "atanh",
+                                                 "quantizeToF16"};
         auto fv = [&](const Ty &t) { return (t.k == Ty::Scalar || t.k == Ty::Vec) && (t.s == S_F32 || t.s == S_AF || t.s == S_AI); };
         auto common = [&](bool floats) {   // every argument to one type (scalars and vectors as they are)
             SK s = A[0].s;
@@ -1629,8 +1697,9 @@ struct Checker {
             conv_default(e->a[0]);
             return fin(concrete(A[0]));
         }
-        if (n == "min" || n == "max" || n == "clamp" || n == "atan2" || n == "pow" || n == "step" || n == "mix" || n == "smoothstep") {
-            size_t k = n == "clamp" || n == "mix" || n == "smoothstep" ? 3 : 2;
+        if (n == "min" || n == "max" || n == "clamp" || n == "atan2" || n == "pow" || n == "step" || n == "mix" || n == "smoothstep" ||
+            n == "fma") {
+            size_t k = n == "clamp" || n == "mix" || n == "smoothstep" || n == "fma" ? 3 : 2;
             nargs(k);
             bool floats = !(n == "min" || n == "max" || n == "clamp");
             for (const Ty &t : A)
@@ -1692,7 +1761,105 @@ struct Checker {
             std::swap(r.n, r.m);
             return fin(r);
         }
+        if (n == "ldexp") {
+            nargs(2);
+            if (!fv(A[0])) invalid(e->line, e->col, "ldexp needs f32 or vecN<f32>, found " + tname(A[0]));
+            if (A[1].k != A[0].k || A[1].n != A[0].n || !(A[1].s == S_I32 || A[1].s == S_AI))
+                invalid(e->a[1]->line, e->a[1]->col, "ldexp's exponent must be " + tname(with_elem(A[0], S_I32)) + ", found " + tname(A[1]));
+            conv(e->a[0], with_elem(A[0], S_F32));
+            conv(e->a[1], with_elem(A[1], S_I32));
+            return fin(with_elem(A[0], S_F32));
+        }
+        if (n == "frexp" || n == "modf") {
+            nargs(1);
+            if (!fv(A[0])) invalid(e->line, e->col, n + " needs f32 or vecN<f32>, found " + tname(A[0]));
+            Ty f = with_elem(A[0], S_F32);
+            conv(e->a[0], f);
+            return fin(result_struct(n, f));
+        }
+        if (n == "determinant") {
+            nargs(1);
+            if (A[0].k != Ty::Mat || A[0].n != A[0].m) invalid(e->line, e->col, "determinant needs a square matrix, found " + tname(A[0]));
+            return fin(scalar(S_F32));
+        }
+        if (n == "faceForward" || n == "reflect" || n == "refract") {
+            const size_t k = n == "reflect" ? 2 : 3, nv = n == "refract" ? 2 : k;
+            nargs(k);
+            if (A[0].k != Ty::Vec || !fv(A[0])) invalid(e->line, e->col, n + " needs vecN<f32>, found " + tname(A[0]));
+            const Ty v = with_elem(A[0], S_F32);
+            for (size_t i = 0; i < k; i++) {
+                const Ty want = i < nv ? v : scalar(S_F32);
+                if (A[i].k != want.k || A[i].n != want.n || !fv(A[i])) invalid(e->a[i]->line, e->a[i]->col, n + ": expected " + tname(want) + ", found " + tname(A[i]));
+                conv(e->a[i], want);
+            }
+            return fin(v);
+        }
+        // bit builtins: i32, u32 and vectors of them
+        auto iv = [&](const Ty &t) { return (t.k == Ty::Scalar || t.k == Ty::Vec) && (t.s == S_I32 || t.s == S_U32 || t.s == S_AI); };
+        static const std::set<std::string> b1 = {"countOneBits", "countLeadingZeros", "countTrailingZeros", "reverseBits",
+                                                 "firstTrailingBit", "firstLeadingBit"};
+        if (b1.count(n) || n == "extractBits" || n == "insertBits") {
+            const size_t k = b1.count(n) ? 1 : n == "extractBits" ? 3 : 4, nv = n == "insertBits" ? 2 : 1;
+            nargs(k);
+            if (!iv(A[0])) invalid(e->line, e->col, n + " needs i32, u32 or a vector of them, found " + tname(A[0]));
+            Ty t = concrete(A[0]);
+            if (nv == 2) {
+                if (!iv(A[1]) || A[1].k != A[0].k || A[1].n != A[0].n) invalid(e->a[1]->line, e->a[1]->col, n + ": mismatched argument " + tname(A[1]));
+                t = concrete(with_elem(A[0], unify(A[0].s, A[1].s, e)));
+            }
+            for (size_t i = 0; i < k; i++) {
+                if (i < nv) { conv(e->a[i], t); continue; }
+                if (A[i].k != Ty::Scalar || !(A[i].s == S_U32 || A[i].s == S_AI))
+                    invalid(e->a[i]->line, e->a[i]->col, n + "'s offset and count must be u32, found " + tname(A[i]));
+                conv(e->a[i], scalar(S_U32));
+            }
+            return fin(t);
+        }
+        if (n == "dot4U8Packed" || n == "dot4I8Packed") {
+            nargs(2);
+            for (size_t i = 0; i < 2; i++) {
+                if (A[i].k != Ty::Scalar || !(A[i].s == S_U32 || A[i].s == S_AI)) invalid(e->a[i]->line, e->a[i]->col, n + " needs u32, found " + tname(A[i]));
+                conv(e->a[i], scalar(S_U32));
+            }
+            return fin(scalar(n == "dot4U8Packed" ? S_U32 : S_I32));
+        }
+        // packing: pack4x8* / pack2x16* take vec4 / vec2<f32>, unpack* give them
+        if (n.compare(0, 4, "pack") == 0 && (n == "pack4x8snorm" || n == "pack4x8unorm" || n == "pack2x16snorm" ||
+                                             n == "pack2x16unorm" || n == "pack2x16float")) {
+            nargs(1);
+            const int N = n[4] == '4' ? 4 : 2;
+            if (A[0].k != Ty::Vec || A[0].n != N || !fv(A[0])) invalid(e->line, e->col, n + " needs " + tname(vec(S_F32, N)) + ", found " + tname(A[0]));
+            conv(e->a[0], vec(S_F32, N));
+            return fin(scalar(S_U32));
+        }
+        if (n == "unpack4x8snorm" || n == "unpack4x8unorm" || n == "unpack2x16snorm" || n == "unpack2x16unorm" || n == "unpack2x16float") {
+            nargs(1);
+            if (A[0].k != Ty::Scalar || !(A[0].s == S_U32 || A[0].s == S_AI)) invalid(e->line, e->col, n + " needs u32, found " + tname(A[0]));
+            conv(e->a[0], scalar(S_U32));
+            return fin(vec(S_F32, n[6] == '4' ? 4 : 2));
+        }
         invalid(e->line, e->col, "unknown function '" + n + "'");
+    }
+
+    // the predeclared result struct of frexp / modf for f32 or vecN<f32>: __frexp_result_f32 { fract, exp },
+    // __modf_result_vec2_f32 { fract, whole }, ...
+    std::map<std::string, int> result_structs;
+    Ty result_struct(const std::string &fn, const Ty &f) {
+        const std::string name = "__" + fn + "_result_" + (f.k == Ty::Vec ? "vec" + std::to_string(f.n) + "_" : "") + "f32";
+        auto it = result_structs.find(name);
+        Ty t;
+        t.k = Ty::Struct;
+        if (it != result_structs.end()) { t.sid = it->second; return t; }
+        StructInfo si;
+        si.name = name;
+        si.resolved = true;
+        const Ty second = fn == "frexp" ? with_elem(f, S_I32) : f;
+        si.fields = {FieldInfo{"fract", f, {}, 0}, FieldInfo{fn == "frexp" ? "exp" : "whole", second, {}, 0}};
+        si.cname = fn == "frexp" ? "wfrexp<" + cty(f) + ", " + cty(second) + ">" : "wmodf<" + cty(f) + ">";
+        t.sid = (int)structs.size();
+        structs.push_back(si);
+        result_structs[name] = t.sid;
+        return t;
     }
 
     // ---- statements ----
@@ -1769,6 +1936,7 @@ struct Checker {
                     sym.has_cv = true; sym.cv = s->e->cv;
                 } else {
                     sym.code = "u_" + s->name;
+                    if (s->k == Stmt::Const) const_int(sym, s->e);
                     o += ind(d) + "const " + cty(t) + " u_" + s->name + " = " + value(s->e) + ";\n";
                 }
                 declare(s->name, sym, s->line, s->col);
@@ -1993,6 +2161,7 @@ Translation run(const std::string &src) {
             sym.has_cv = true; sym.cv = c.init->cv;
         } else {
             sym.code = "u_" + c.name + "()";
+            ck.const_int(sym, c.init);
             if (c.init->code.find("ctx") != std::string::npos) invalid(c.line, c.col, "a module constant must be a constant expression");
             ck.out_consts += "__device__ inline " + ck.cty(t) + " u_" + c.name + "() { return " + ck.value(c.init) + "; }\n";
         }
@@ -2127,6 +2296,17 @@ Translation run(const std::string &src) {
         body += "}\n";
         ck.pop();
         ck.out_bodies += body;
+    }
+    // textureSampleBias is a fragment-stage builtin: refused in vs_main and in every function vs_main reaches
+    {
+        std::set<std::string> seen;
+        std::function<void(const std::string &)> vertex_ok = [&](const std::string &fn) {
+            if (!seen.insert(fn).second) return;
+            const FnInfo &fi = ck.fns[fn];
+            if (fi.frag_line) invalid(fi.frag_line, fi.frag_col, "textureSampleBias is only allowed in the fragment stage, and vs_main reaches it");
+            for (const std::string &c : fi.calls) vertex_ok(c);
+        };
+        vertex_ok("vs_main");
     }
     // the stage interface: vs_main's output and fs_main's input
     const FnInfo &vsi = ck.fns["vs_main"], &fsi = ck.fns["fs_main"];

@@ -247,6 +247,176 @@ template <int N> __device__ inline bool wb_all(const wv<bool, N> &a) { bool r = 
 __device__ inline bool wb_any(bool a) { return a; }
 __device__ inline bool wb_all(bool a) { return a; }
 
+// numeric builtins (DESIGN.md, "WGSL builtins"): each rule is written out there and restated in numpy by
+// tests/test_wgsl_builtins.py
+__device__ inline float wb_saturate(float x) { return wb_clamp(x, 0.0f, 1.0f); }
+__device__ inline float wb_degrees(float x) { return x * __uint_as_float(0x42652ee1u); }   // f32(180 / pi)
+__device__ inline float wb_radians(float x) { return x * __uint_as_float(0x3c8efa35u); }   // f32(pi / 180)
+__device__ inline float wb_fma(float a, float b, float c) { return fmaf(a, b, c); }
+__device__ inline float wb_sinh(float x) { return sinhf(x); }
+__device__ inline float wb_cosh(float x) { return coshf(x); }
+__device__ inline float wb_tanh(float x) { return tanhf(x); }
+__device__ inline float wb_asinh(float x) { return asinhf(x); }
+__device__ inline float wb_acosh(float x) { return acoshf(x); }
+__device__ inline float wb_atanh(float x) { return atanhf(x); }
+// f32 -> f16 (round to nearest even, no flush) and back, in PTX: NVRTC compiles this without cuda_fp16.h
+__device__ inline unsigned short wg_f16(float x) { unsigned short h; asm("cvt.rn.f16.f32 %0, %1;" : "=h"(h) : "f"(x)); return h; }
+__device__ inline float wg_f32(unsigned short h) { float x; asm("cvt.f32.f16 %0, %1;" : "=f"(x) : "h"(h)); return x; }
+__device__ inline float wb_quantizeToF16(float x) { return wg_f32(wg_f16(x)); }
+WG_VUN(wb_saturate) WG_VUN(wb_degrees) WG_VUN(wb_radians) WG_VTRI(wb_fma) WG_VUN(wb_sinh) WG_VUN(wb_cosh) WG_VUN(wb_tanh)
+WG_VUN(wb_asinh) WG_VUN(wb_acosh) WG_VUN(wb_atanh) WG_VUN(wb_quantizeToF16)
+__device__ inline float wb_ldexp(float x, int e) { return ldexpf(x, e); }
+template <int N> __device__ inline wv<float, N> wb_ldexp(const wv<float, N> &x, const wv<int, N> &e) {
+    wv<float, N> r;
+    for (int i = 0; i < N; i++) r.v[i] = ldexpf(x.v[i], e.v[i]);
+    return r;
+}
+// the predeclared result structs: __frexp_result_f32 / _vecN_f32 { fract, exp } and __modf_result* { fract, whole }
+template <class F, class E> struct wfrexp { F m_fract; E m_exp; };
+template <class F> struct wmodf { F m_fract; F m_whole; };
+__device__ inline wfrexp<float, int> wb_frexp(float x) {   // the fraction's magnitude in [0.5, 1); 0 gives (0, 0)
+    wfrexp<float, int> r;
+    r.m_fract = frexpf(x, &r.m_exp);
+    return r;
+}
+template <int N> __device__ inline wfrexp<wv<float, N>, wv<int, N>> wb_frexp(const wv<float, N> &x) {
+    wfrexp<wv<float, N>, wv<int, N>> r;
+    for (int i = 0; i < N; i++) r.m_fract.v[i] = frexpf(x.v[i], &r.m_exp.v[i]);
+    return r;
+}
+__device__ inline wmodf<float> wb_modf(float x) { const float w = truncf(x); return {x - w, w}; }
+template <int N> __device__ inline wmodf<wv<float, N>> wb_modf(const wv<float, N> &x) {
+    wmodf<wv<float, N>> r;
+    for (int i = 0; i < N; i++) { r.m_whole.v[i] = truncf(x.v[i]); r.m_fract.v[i] = x.v[i] - r.m_whole.v[i]; }
+    return r;
+}
+// cofactor expansion along the first column, terms added left to right; a[r][c] is row r, column c
+template <int N> __device__ inline float wg_det(const float (&a)[N][N]) {
+    float s = 0.0f;
+    for (int i = 0; i < N; i++) {
+        float m[N - 1][N - 1];
+        for (int r = 0, k = 0; r < N; r++) {
+            if (r == i) continue;
+            for (int c = 1; c < N; c++) m[k][c - 1] = a[r][c];
+            k++;
+        }
+        const float t = a[i][0] * wg_det<N - 1>(m);
+        s = i == 0 ? t : (i & 1) ? s - t : s + t;
+    }
+    return s;
+}
+template <> __device__ inline float wg_det<1>(const float (&a)[1][1]) { return a[0][0]; }
+template <int N> __device__ inline float wb_determinant(const wm<N, N> &m) {
+    float a[N][N];
+    for (int r = 0; r < N; r++)
+        for (int c = 0; c < N; c++) a[r][c] = m.c[c].v[r];
+    return wg_det<N>(a);
+}
+template <int N> __device__ inline wv<float, N> wb_faceForward(const wv<float, N> &e1, const wv<float, N> &e2, const wv<float, N> &e3) {
+    return wb_dot(e2, e3) < 0.0f ? e1 : w_neg(e1);
+}
+template <int N> __device__ inline wv<float, N> wb_reflect(const wv<float, N> &e1, const wv<float, N> &e2) {
+    const float k = 2.0f * wb_dot(e2, e1);
+    wv<float, N> r;
+    for (int i = 0; i < N; i++) r.v[i] = e1.v[i] - k * e2.v[i];
+    return r;
+}
+template <int N> __device__ inline wv<float, N> wb_refract(const wv<float, N> &e1, const wv<float, N> &e2, float e3) {
+    const float d = wb_dot(e2, e1), k = 1.0f - e3 * e3 * (1.0f - d * d);
+    wv<float, N> r;
+    if (k < 0.0f) return wsplat<N>(0.0f);
+    const float s = e3 * d + sqrtf(k);
+    for (int i = 0; i < N; i++) r.v[i] = e3 * e1.v[i] - s * e2.v[i];
+    return r;
+}
+
+// bit builtins, i32 and u32
+__device__ inline unsigned wb_countOneBits(unsigned x) { return (unsigned)__popc(x); }
+__device__ inline int wb_countOneBits(int x) { return __popc((unsigned)x); }
+__device__ inline unsigned wb_countLeadingZeros(unsigned x) { return (unsigned)__clz((int)x); }   // 32 for 0
+__device__ inline int wb_countLeadingZeros(int x) { return __clz(x); }
+__device__ inline unsigned wb_countTrailingZeros(unsigned x) { return x ? (unsigned)(__ffs((int)x) - 1) : 32u; }
+__device__ inline int wb_countTrailingZeros(int x) { return (int)wb_countTrailingZeros((unsigned)x); }
+__device__ inline unsigned wb_reverseBits(unsigned x) { return __brev(x); }
+__device__ inline int wb_reverseBits(int x) { return (int)__brev((unsigned)x); }
+__device__ inline unsigned wb_firstTrailingBit(unsigned x) { return x ? (unsigned)(__ffs((int)x) - 1) : 0xffffffffu; }
+__device__ inline int wb_firstTrailingBit(int x) { return (int)wb_firstTrailingBit((unsigned)x); }
+__device__ inline unsigned wb_firstLeadingBit(unsigned x) { return x ? 31u - (unsigned)__clz((int)x) : 0xffffffffu; }
+__device__ inline int wb_firstLeadingBit(int x) {   // the highest bit that differs from the sign bit; -1 for 0 and -1
+    const unsigned u = x < 0 ? ~(unsigned)x : (unsigned)x;
+    return u ? 31 - __clz((int)u) : -1;
+}
+__device__ inline unsigned wg_bitmask(unsigned c) { return c >= 32u ? 0xffffffffu : (1u << c) - 1u; }   // bits [0, c)
+__device__ inline unsigned wb_extractBits(unsigned e, unsigned offset, unsigned count) {
+    const unsigned o = min(offset, 32u), c = min(count, 32u - o);
+    return c == 0u ? 0u : (e >> o) & wg_bitmask(c);
+}
+__device__ inline int wb_extractBits(int e, unsigned offset, unsigned count) {   // sign-extended from bit c - 1
+    const unsigned o = min(offset, 32u), c = min(count, 32u - o);
+    return c == 0u ? 0 : (int)(wb_extractBits((unsigned)e, o, c) << (32u - c)) >> (32u - c);
+}
+__device__ inline unsigned wb_insertBits(unsigned e, unsigned newbits, unsigned offset, unsigned count) {
+    const unsigned o = min(offset, 32u), c = min(count, 32u - o);
+    if (c == 0u) return e;
+    const unsigned mask = wg_bitmask(c) << o;
+    return (e & ~mask) | ((newbits << o) & mask);
+}
+__device__ inline int wb_insertBits(int e, int newbits, unsigned offset, unsigned count) {
+    return (int)wb_insertBits((unsigned)e, (unsigned)newbits, offset, count);
+}
+WG_VUN(wb_countOneBits) WG_VUN(wb_countLeadingZeros) WG_VUN(wb_countTrailingZeros) WG_VUN(wb_reverseBits)
+WG_VUN(wb_firstTrailingBit) WG_VUN(wb_firstLeadingBit)
+template <class T, int N> __device__ inline wv<T, N> wb_extractBits(const wv<T, N> &e, unsigned offset, unsigned count) {
+    wv<T, N> r;
+    for (int i = 0; i < N; i++) r.v[i] = wb_extractBits(e.v[i], offset, count);
+    return r;
+}
+template <class T, int N> __device__ inline wv<T, N> wb_insertBits(const wv<T, N> &e, const wv<T, N> &b, unsigned offset, unsigned count) {
+    wv<T, N> r;
+    for (int i = 0; i < N; i++) r.v[i] = wb_insertBits(e.v[i], b.v[i], offset, count);
+    return r;
+}
+__device__ inline unsigned wb_dot4U8Packed(unsigned a, unsigned b) {
+    unsigned s = 0u;
+    for (int i = 0; i < 32; i += 8) s += ((a >> i) & 255u) * ((b >> i) & 255u);
+    return s;
+}
+__device__ inline int wb_dot4I8Packed(unsigned a, unsigned b) {
+    int s = 0;
+    for (int i = 0; i < 32; i += 8) s += (int)(signed char)(a >> i) * (int)(signed char)(b >> i);
+    return s;
+}
+
+// packing: component i goes to byte / half-word i, from the least significant
+template <int N> __device__ inline unsigned wg_pack(const wv<float, N> &e, float lo, float scale) {
+    unsigned r = 0u;
+    for (int i = 0; i < N; i++) {
+        const int q = (int)floorf(0.5f + scale * wb_min(1.0f, wb_max(lo, e.v[i])));
+        r |= ((unsigned)q & (N == 4 ? 0xffu : 0xffffu)) << (i * (32 / N));
+    }
+    return r;
+}
+__device__ inline unsigned wb_pack4x8snorm(const wv<float, 4> &e) { return wg_pack(e, -1.0f, 127.0f); }
+__device__ inline unsigned wb_pack4x8unorm(const wv<float, 4> &e) { return wg_pack(e, 0.0f, 255.0f); }
+__device__ inline unsigned wb_pack2x16snorm(const wv<float, 2> &e) { return wg_pack(e, -1.0f, 32767.0f); }
+__device__ inline unsigned wb_pack2x16unorm(const wv<float, 2> &e) { return wg_pack(e, 0.0f, 65535.0f); }
+__device__ inline unsigned wb_pack2x16float(const wv<float, 2> &e) { return (unsigned)wg_f16(e.v[0]) | ((unsigned)wg_f16(e.v[1]) << 16); }
+__device__ inline wv<float, 4> wb_unpack4x8snorm(unsigned x) {
+    wv<float, 4> r;
+    for (int i = 0; i < 4; i++) r.v[i] = wb_max((float)(signed char)(x >> (8 * i)) / 127.0f, -1.0f);
+    return r;
+}
+__device__ inline wv<float, 4> wb_unpack4x8unorm(unsigned x) {
+    wv<float, 4> r;
+    for (int i = 0; i < 4; i++) r.v[i] = (float)((x >> (8 * i)) & 255u) / 255.0f;
+    return r;
+}
+__device__ inline wv<float, 2> wb_unpack2x16snorm(unsigned x) {
+    return {{wb_max((float)(short)x / 32767.0f, -1.0f), wb_max((float)(short)(x >> 16) / 32767.0f, -1.0f)}};
+}
+__device__ inline wv<float, 2> wb_unpack2x16unorm(unsigned x) { return {{(float)(x & 0xffffu) / 65535.0f, (float)(x >> 16) / 65535.0f}}; }
+__device__ inline wv<float, 2> wb_unpack2x16float(unsigned x) { return {{wg_f32((unsigned short)x), wg_f32((unsigned short)(x >> 16))}}; }
+
 // the uniform: read at WGSL uniform-address-space offsets from the node's parameter bytes (zero-padded to its size)
 template <class T> __device__ inline T wld(const unsigned char *p) { return *(const T *)p; }
 template <class T, int N> __device__ inline wv<T, N> wldv(const unsigned char *p) {
@@ -271,5 +441,28 @@ struct wg_textures {
     __device__ wv<unsigned, 2> dims(unsigned i) const {
         if (i >= count || tex[i].kind == smr::dev::TEX_NONE) return {{1u, 1u}};
         return {{(unsigned)tex[i].width, (unsigned)tex[i].height}};
+    }
+    // A node texture has one mip level and naga's Restrict policy clamps levels: a level, bias or gradient selects
+    // level 0, so these are textureSample itself (the arguments are still evaluated, as WGSL evaluates them).
+    __device__ wv<float, 4> sample_level(unsigned i, const wv<float, 2> &uv, float) const { return sample(i, uv); }
+    __device__ wv<float, 4> sample_bias(unsigned i, const wv<float, 2> &uv, float) const { return sample(i, uv); }
+    __device__ wv<float, 4> sample_grad(unsigned i, const wv<float, 2> &uv, const wv<float, 2> &, const wv<float, 2> &) const {
+        return sample(i, uv);
+    }
+    template <class L> __device__ wv<unsigned, 2> dims(unsigned i, L) const { return dims(i); }
+    __device__ unsigned levels(unsigned) const { return 1u; }
+    // textureSampleBaseClampToEdge: each coordinate clamped to [0.5 / dim, 1 - 0.5 / dim], then the level-0 sample
+    __device__ wv<float, 4> sample_clamped(unsigned i, const wv<float, 2> &uv) const {
+        const wv<unsigned, 2> d = dims(i);
+        wv<float, 2> c;
+        for (int k = 0; k < 2; k++) {
+            const float lo = 0.5f / (float)d.v[k];
+            c.v[k] = wb_min(wb_max(uv.v[k], lo), 1.0f - lo);
+        }
+        return sample(i, c);
+    }
+    __device__ wv<float, 4> gather(int c, unsigned i, const wv<float, 2> &uv) const {
+        float4 r = smr::dev::gather_node(*T, i < count ? tex + i : nullptr, mode, uv.v[0], uv.v[1], c);
+        return {{r.x, r.y, r.z, r.w}};
     }
 };
