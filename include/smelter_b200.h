@@ -262,7 +262,8 @@ typedef enum {
     SMR_KERNEL_IMAGE = 9,          /* image node textures (k_image) */
     SMR_KERNEL_WEB = 10,           /* web view node textures (k_web) */
     SMR_KERNEL_SHADER = 11,        /* shader node textures (each shader module's smr_shader_main) */
-    SMR_KERNEL_CLASSES = 12
+    SMR_KERNEL_TRANSCODE = 12,     /* transcoder renditions (k_transcode, smr_transcode_resize) */
+    SMR_KERNEL_CLASSES = 13
 } smr_kernel_class;
 typedef struct {
     double total_ms[SMR_KERNEL_CLASSES];
@@ -499,6 +500,28 @@ smr_status smr_preprocess_frame(smr_renderer *r, const smr_input_frame *frame, u
  * smr_render are expected to hold.  Blocking; `rgba` has height rows of `pitch` bytes (0 = tightly packed). */
 smr_status smr_premultiply_rgba8(smr_renderer *r, const smr_input_frame *frame, void *rgba, uint32_t pitch, int32_t mem_kind);
 
+/* gpu-video's transcoder resize (VideoTranscoder, vulkan_transcoder/shader.wgsl + pipeline.rs): one NV12 frame -> n NV12
+ * renditions, each at its own size with its own ScalingAlgorithm, in ONE kernel launch ("decode once, encode a ladder").
+ * `src` is an SMR_FRAME_NV12 frame, host or device; its width x height is the decoder's cropped extent with origin (0, 0),
+ * so a 1920 x 1088 surface with a 1080-row crop is passed as height 1080 with the surface's pointers and pitch.  Nothing
+ * outside the crop is read.  Each rendition's y plane has height rows of `width` bytes, its uv plane height / 2 rows of
+ * width / 2 {u, v} pairs, each at its pitch (0 = tightly packed) in host or device memory per mem_kind; bytes past a
+ * row's width are not written.  Arithmetic: DESIGN.md NC-10.  Blocking, like smr_preprocess_frame.
+ * SMR_ERR_INVALID_ARGUMENT (checked before anything needs a device, so a host-only handle answers it too): n = 0 or
+ * n > 8 (WrongOutputNumber), a rendition side that is 0, odd or above 16384, an unknown scaling, a null plane, a pitch
+ * shorter than a row, an unknown mem_kind, an odd source side, and smr_render's checks of the source frame (size,
+ * planes, pitch, device-plane alignment).  SMR_ERR_UNSUPPORTED: a source format other than NV12. */
+typedef enum { SMR_SCALE_NEAREST = 0, SMR_SCALE_BILINEAR = 1, SMR_SCALE_LANCZOS3 = 2 } smr_scaling_algorithm;  /* ScalingAlgorithm as u32 */
+typedef struct {
+    uint32_t width, height;        /* TranscoderOutputParameters::output_width / output_height */
+    int32_t scaling;               /* smr_scaling_algorithm */
+    void *planes[2];               /* NV12: y, uv */
+    uint32_t pitch[2];             /* 0 = tightly packed */
+    int32_t mem_kind;              /* smr_mem_kind */
+} smr_rendition;
+#define SMR_MAX_RENDITIONS 8
+smr_status smr_transcode_resize(smr_renderer *r, const smr_input_frame *src, const smr_rendition *out, uint32_t n);
+
 /* Text nodes (SURVEY 8f-2): TextRendererNode::render (transformations/text_renderer.rs:72-167).  Shaping and glyph
  * rasterisation (cosmic-text / swash inside glyphon, CPU code in the reference too) stay on the caller's side; what the
  * reference does on the GPU -- clear the node texture to the component's background colour (:141-150) and draw glyphon's
@@ -561,6 +584,12 @@ smr_status smr_debug_weights(float scale, float offset, uint32_t n_out, float *w
 /* inspection (needs a device): the weight kernel's sin and cos (f32 argument, evaluated in fp64, rounded to f32) of n
  * host values x into host arrays s and c. */
 smr_status smr_debug_sincos(const float *x, uint32_t n, float *s, float *c);
+/* inspection (no device needed): the host tables smr_transcode_resize's kernel reads for one axis of in_len source
+ * texels and out_len output texels (each 1 .. 16384; a luma axis is (in, out), a chroma axis (in / 2, out / 2)).  Per
+ * output coordinate k: nearest[k]; bilinear[2 k], bilinear[2 k + 1] = x0, x1 and frac[k]; center[k] and
+ * lanczos[6 k .. 6 k + 5], the Lanczos3 weights of taps center - 2 .. center + 3 (DESIGN.md NC-10). */
+smr_status smr_debug_transcode_taps(uint32_t in_len, uint32_t out_len, int32_t *nearest, int32_t *bilinear, float *frac,
+                                    int32_t *center, float *lanczos);
 
 smr_status smr_debug_tile_plan(const int32_t *boxes, uint32_t n_layers, uint32_t width, uint32_t height, int32_t sorted,
                                int32_t *owner_layer, uint32_t owner_cap, uint32_t *tiles, uint32_t tiles_cap, uint32_t *n_tiles);

@@ -6,7 +6,7 @@ libsmelter_b200.so (hand-written sm_90a CUDA).  There is no CPU fallback."""
 from .renderer import (  # noqa: F401
     BorderRadius, BoxShadow, Component, Frame, FrameData, FramePreProcessor, FrameSet, HorizontalAlign, ImageComponent, InputStreamComponent,
     InterpolationKind, NvPlanes, OutputFrameFormat, Overflow, Padding, Position, Renderer, RendererError,
-    RendererOptions, RenderingMode, RenderSceneError, RescaleMode, RescalerComponent, Resolution, RGBAColor, ShaderComponent,
+    RendererOptions, RenderingMode, RenderSceneError, RescaleMode, RescalerComponent, Resolution, RGBAColor, ScalingAlgorithm, ShaderComponent,
     ShaderParam, ShaderParamType,
     TextComponent, TilesComponent, Transition, UpdateSceneError, VerticalAlign, ViewChildrenDirection, ViewComponent, WebViewComponent,
     YuvPlanes,

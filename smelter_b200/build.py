@@ -13,7 +13,7 @@ SOURCES = ["kernels.cu", "renderer.cpp", "scene.cpp", "wgsl.cpp"]
 # the sources a shader module is compiled from at registration (renderer.cpp, NVRTC), embedded as string literals
 EMBEDDED = ["kernels.h", "node_sample.cuh", "shader_rt.cuh", "wgsl_rt.cuh"]
 EMBEDDED_INC = os.path.join(CSRC, "shader_sources.inc")   # generated, kept out of git
-HEADERS = ["node_sample.cuh", "shader_rt.cuh", "wgsl_rt.cuh", "wgsl.h", "kernels.h", "interior.h", "int_weights.h", "scene.h", "ptx_helpers.cuh", "resample_tma.cuh", "resample_tma3.cuh", "resample_tma0.cuh", os.path.join("..", "..", "include", "smelter_b200.h")]
+HEADERS = ["node_sample.cuh", "shader_rt.cuh", "wgsl_rt.cuh", "wgsl.h", "kernels.h", "interior.h", "int_weights.h", "scene.h", "ptx_helpers.cuh", "resample_tma.cuh", "resample_tma3.cuh", "resample_tma0.cuh", "transcode.cuh", os.path.join("..", "..", "include", "smelter_b200.h")]
 
 NVCC_FLAGS = [
     "-std=c++17", "-O3",

@@ -10,6 +10,7 @@
 //                 rgba_to_yuv.wgsl / rgba_to_nv12.wgsl on the way out                   (K9,K10,K11)
 //   k_output      rgba_to_yuv / rgba_to_nv12 stand-alone (root size != output size, odd sizes)
 //   k_fill        r8/rg8_fill_value.wgsl (black frame)                                  (K6)
+//   k_transcode   gpu-video's vulkan_transcoder/shader.wgsl: NV12 -> up to eight NV12 renditions (transcode.cuh)
 //
 // Numeric contract: identical to oracle/smelter_oracle.c (DESIGN.md section 3).  Compiled with
 // -fmad=false: only explicit fmaf() is fused, every other operation rounds separately, division and
@@ -1526,6 +1527,9 @@ int launch_output(const OutputJob &job, Stream s) {
     k_output<<<g, b, 0, (cudaStream_t)s>>>(job);
     return check_launch("k_output") ? 1 : -1;
 }
+
+// gpu-video's transcoder resize (smr_transcode_resize, NC-10)
+#include "transcode.cuh"
 
 // ------------------------------------------------------------------------------------------------
 // FramePreProcessor (state/frame_pre_processor.rs): K1..K4 to RGBA8, optional rescale (rgba_rescale.wgsl, blend: None)

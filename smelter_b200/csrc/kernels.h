@@ -275,6 +275,35 @@ struct ShaderJob {
     const uint8_t *params;        // ShaderParam::to_bytes, in the parameter arena (null: no parameter)
 };
 
+// gpu-video's transcoder resize (vulkan_transcoder/shader.wgsl, NC-10): one output coordinate of one axis, computed on the
+// host (renderer.cpp: transcode_axis) so that the kernel evaluates no transcendental
+struct TranscodeTap {
+    int32_t nearest;              // u32(in * float_coords)
+    int32_t lo, hi;               // bilinear: u32(max(floor(fc), 0)), min(lo + 1, in - 1)
+    float frac;                   // bilinear: fc - floor(fc), from the unclamped fc
+    int32_t center;               // Lanczos3: floor(fc)
+    float w[6];                   // Lanczos3: lanczos3_weight(fc - (center + d)), d = -2 .. 3
+};
+constexpr int kTranscodeMaxOutputs = 8;                  // the reference's binding arrays hold eight renditions
+constexpr int kTranscodeTileX = 32, kTranscodeTileY = 8; // chroma samples per block (a thread: one sample, its 2 x 2 luma quad)
+struct TranscodeOut {             // one NV12 rendition
+    uint8_t *y, *uv;
+    int32_t pitch_y, pitch_uv;
+    int32_t width, height;        // even
+    int32_t scaling;              // 0 nearest, 1 bilinear, 2 Lanczos3 (ScalingAlgorithm)
+    const TranscodeTap *tx, *ty;  // luma: in -> out per axis
+    const TranscodeTap *cx, *cy;  // chroma: in / 2 -> out / 2 per axis
+    int32_t tiles_x;              // blocks per row of tiles
+    int32_t tile_begin;           // first block of this rendition
+};
+struct TranscodeLaunch {          // every rendition of one call: one launch
+    const uint8_t *src_y, *src_uv;   // NV12 crop, origin (0, 0); uv 2-byte aligned
+    int32_t pitch_y, pitch_uv;
+    int32_t width, height;        // even
+    int32_t n;
+    TranscodeOut out[kTranscodeMaxOutputs];
+};
+
 // host tables pushed once per device (numeric contract NC-1/3/4)
 void upload_tables(const float *u8n, const float *srgb_dec, const float *srgb_enc_thr);
 // the device tables of node_sample.cuh in this module (c_u8n, c_dec, c_thr, c_yl, c_enc1): addresses and bytes, for the
@@ -317,6 +346,8 @@ int launch_resample_fused(const FusedKernel &k, int src, int full_range, const F
 // with a short layer list (layers0_host: host copy of jobs_host[0].layers) passes job and layers in the parameter block
 int launch_composite(const CompositeJob *jobs_dev, const CompositeJob *jobs_host, const LayerDev *layers0_host, int n, Stream s);
 int launch_output(const OutputJob &job, Stream s);
+// every rendition of L in one launch of n_blocks blocks (the last rendition's tile_begin + its tiles)
+int launch_transcode(const TranscodeLaunch &L, int n_blocks, Stream s);
 int launch_fill_yuv(uint8_t *p0, uint8_t *p1, uint8_t *p2, int pitch0, int pitch1, int pitch2, int w, int h,
                     int out_format, uint8_t y, uint8_t u, uint8_t v, Stream s);
 const char *last_launch_error();

@@ -405,6 +405,7 @@ class Renderer {
     smr_status render_end_all();
     smr_status preprocess_frame(const smr_input_frame *f, uint32_t ow, uint32_t oh, void *rgba, uint32_t pitch, int32_t mem_kind,
                                 bool premultiply = false);
+    smr_status transcode_resize(const smr_input_frame *src, const smr_rendition *out, uint32_t n);
     smr_status render_text(uint32_t w, uint32_t h, smr_rgba bg, const smr_glyph *glyphs, uint32_t n, const smr_atlas *mask,
                            const smr_atlas *color, int32_t color_mode, void *rgba, uint32_t pitch, int32_t mem_kind);
     smr_status debug_set_inputs(uint64_t pts, const smr_input_frame *in, uint32_t n_in);
@@ -717,6 +718,15 @@ class Renderer {
     void fold_profile();
     bool host_only_ = false;
     DevBuf pre_planes_[3], pre_out_;   // FramePreProcessor scratch (input_texture / rescale_texture / download_buffer)
+    smr_status upload_pre_planes(const smr_input_frame &f, FrameView &v);
+    // smr_transcode_resize's per-axis tables, per (source length, output length); at most kTranscodeTapTables are kept, the
+    // least recently used beyond that are released when a call needs room (no call uses more than 32)
+    struct TapTable { DevBuf buf; uint64_t used = 0; };
+    static constexpr size_t kTranscodeTapTables = 64;
+    std::map<std::pair<uint32_t, uint32_t>, TapTable> transcode_taps_;
+    uint64_t transcode_calls_ = 0;
+    const dev::TranscodeTap *transcode_table(uint32_t in_len, uint32_t out_len);
+    cudaEvent_t transcode_ev_[2] = {};   // profiling: around the k_transcode launch
     // optional per-kernel-class device timing (cudaEvents on the launching stream)
     void prof_mark(int kernel_class);
     bool profiling_ = false;
@@ -758,6 +768,7 @@ Renderer::~Renderer() {
         if (comm_done_) cudaEventDestroy(comm_done_);
         if (tick_start_) cudaEventDestroy(tick_start_);
         if (web_ev_) cudaEventDestroy(web_ev_);
+        for (cudaEvent_t e : transcode_ev_) if (e) cudaEventDestroy(e);
         for (int i = 0; i < kTicksInFlight; i++) { if (h2d_done_[i]) cudaEventDestroy(h2d_done_[i]); if (tick_done_[i]) cudaEventDestroy(tick_done_[i]); }
         if (nccl_comm_) { g_nccl.CommDestroy(nccl_comm_); nccl_comm_ = nullptr; }
         for (auto &kv : weights_) {
@@ -1983,6 +1994,175 @@ smr_status Renderer::write_rgba(void *rgba, uint32_t pitch, int32_t mem_kind, ui
     return SMR_OK;
 }
 
+// A frame read_frame has checked, for a blocking call: host planes are copied, packed, into pre_planes_ on stream_ and `v`
+// is pointed at them; device planes stay where they are
+smr_status Renderer::upload_pre_planes(const smr_input_frame &f, FrameView &v) {
+    for (int p = 0; p < 3 && f.mem_kind != SMR_MEM_DEVICE; p++) {
+        const FrameView::Plane &P = v.plane[p];
+        if (!P.p) continue;
+        if (P.row_bytes * P.rows > pre_planes_[p].cap) CUDA_OK(cudaStreamSynchronize(stream_));
+        CUDA_OK(pre_planes_[p].ensure(P.row_bytes * P.rows));
+        CUDA_OK(cudaMemcpy2DAsync(pre_planes_[p].p, P.row_bytes, P.p, P.pitch, P.row_bytes, P.rows, cudaMemcpyHostToDevice, stream_));
+        stats_.h2d_bytes += P.row_bytes * P.rows;
+        set_tex_plane(v.tex, p, pre_planes_[p].p, P.row_bytes);
+    }
+    return SMR_OK;
+}
+
+// One axis of gpu-video's transcoder resize (vulkan_transcoder/shader.wgsl, NC-10) for every output coordinate: what
+// main and its samplers compute from (coordinate + 0.5) / size before they load a texel.  f32 throughout, each operation
+// rounded on its own (-ffp-contract=off), sin in fp64 rounded to f32 (NC-8).
+static float transcode_sinc(float x) {
+    if (std::fabs(x) < 1e-6f) return 1.0f;
+    const float px = 3.14159265358979323846f * x;
+    return (float)std::sin((double)px) / px;
+}
+static float transcode_lanczos3(float x) { return std::fabs(x) >= 3.0f ? 0.0f : transcode_sinc(x) * transcode_sinc(x / 3.0f); }
+static void transcode_axis(uint32_t in_len, uint32_t out_len, std::vector<dev::TranscodeTap> &taps) {
+    taps.resize(out_len);
+    const float fin = (float)in_len, fout = (float)out_len;
+    for (uint32_t k = 0; k < out_len; k++) {
+        dev::TranscodeTap &t = taps[k];
+        const float coord = ((float)k + 0.5f) / fout;   // float_coords
+        const float scaled = fin * coord;
+        t.nearest = (int32_t)(uint32_t)scaled;            // u32(): truncation; scaled < in_len for in_len, out_len <= 16384
+        const float fc = scaled - 0.5f;
+        const float fl = std::floor(fc);
+        t.lo = (int32_t)(uint32_t)std::fmax(fl, 0.0f);
+        t.hi = std::min(t.lo + 1, (int32_t)in_len - 1);
+        t.frac = fc - fl;
+        t.center = (int32_t)fl;
+        for (int d = 0; d < 6; d++) t.w[d] = transcode_lanczos3(fc - (fl + (float)(d - 2)));
+    }
+}
+
+const dev::TranscodeTap *Renderer::transcode_table(uint32_t in_len, uint32_t out_len) {
+    auto it = transcode_taps_.find({in_len, out_len});
+    if (it == transcode_taps_.end()) {
+        while (transcode_taps_.size() >= kTranscodeTapTables) {   // release the least recently used (not this call's)
+            auto lru = transcode_taps_.begin();
+            for (auto j = transcode_taps_.begin(); j != transcode_taps_.end(); ++j)
+                if (j->second.used < lru->second.used) lru = j;
+            if (lru->second.used == transcode_calls_) break;
+            transcode_taps_.erase(lru);
+        }
+        std::vector<dev::TranscodeTap> host;
+        transcode_axis(in_len, out_len, host);
+        TapTable &t = transcode_taps_[{in_len, out_len}];
+        const size_t bytes = sizeof(dev::TranscodeTap) * host.size();
+        // pageable source: staged before cudaMemcpyAsync returns, and ordered before the launch on stream_
+        if (t.buf.ensure(bytes) != cudaSuccess ||
+            cudaMemcpyAsync(t.buf.p, host.data(), bytes, cudaMemcpyHostToDevice, stream_) != cudaSuccess) {
+            transcode_taps_.erase({in_len, out_len});
+            return nullptr;
+        }
+        it = transcode_taps_.find({in_len, out_len});
+    }
+    it->second.used = transcode_calls_;
+    return reinterpret_cast<const dev::TranscodeTap *>(it->second.buf.p);
+}
+
+// VideoTranscoder's resize step (gpu-video vulkan_transcoder/pipeline.rs + shader.wgsl): every rendition in one launch
+smr_status Renderer::transcode_resize(const smr_input_frame *src, const smr_rendition *out, uint32_t n) {
+    if (!src || (n && !out)) return SMR_ERR_INVALID_ARGUMENT;
+    std::lock_guard<std::mutex> g(mu_);
+    if (n == 0 || n > (uint32_t)dev::kTranscodeMaxOutputs) {
+        set_error("wrong output number: expected 1 to 8 renditions");
+        return SMR_ERR_INVALID_ARGUMENT;
+    }
+    for (uint32_t i = 0; i < n; i++) {
+        const smr_rendition &o = out[i];
+        if (o.width == 0 || o.height == 0 || o.width > kMaxFrameDim || o.height > kMaxFrameDim || ((o.width | o.height) & 1)) {
+            set_error("rendition " + std::to_string(i) + ": width and height must be even and in 2 .. 16384");
+            return SMR_ERR_INVALID_ARGUMENT;
+        }
+        if (o.scaling != SMR_SCALE_NEAREST && o.scaling != SMR_SCALE_BILINEAR && o.scaling != SMR_SCALE_LANCZOS3) {
+            set_error("rendition " + std::to_string(i) + ": unknown scaling algorithm");
+            return SMR_ERR_INVALID_ARGUMENT;
+        }
+        if (o.mem_kind != SMR_MEM_HOST && o.mem_kind != SMR_MEM_DEVICE) {
+            set_error("rendition " + std::to_string(i) + ": unknown mem_kind");
+            return SMR_ERR_INVALID_ARGUMENT;
+        }
+        for (int p = 0; p < 2; p++) {   // an NV12 row is `width` bytes in both planes
+            if (!o.planes[p]) { set_error("rendition " + std::to_string(i) + ": plane pointer is null"); return SMR_ERR_INVALID_ARGUMENT; }
+            if (o.pitch[p] && o.pitch[p] < o.width) {
+                set_error("rendition " + std::to_string(i) + ": pitch is smaller than a row");
+                return SMR_ERR_INVALID_ARGUMENT;
+            }
+        }
+    }
+    FrameView v;
+    if (smr_status st = read_frame(*src, v); st != SMR_OK) return st;
+    if (src->format != SMR_FRAME_NV12) { set_error("the transcoder resize takes NV12 frames"); return SMR_ERR_UNSUPPORTED; }
+    if ((src->width | src->height) & 1) { set_error("NV12 source width and height must be even"); return SMR_ERR_INVALID_ARGUMENT; }
+    if (host_only_) { set_error("host-only handle (cuda_device = -1) has no device: no CPU fallback"); return SMR_ERR_CUDA; }
+    CUDA_OK(cudaSetDevice(opts_.cuda_device));
+    if (smr_status st = upload_pre_planes(*src, v); st != SMR_OK) return st;
+
+    dev::TranscodeLaunch L = {};
+    L.src_y = v.tex.p0; L.src_uv = v.tex.p1;
+    L.pitch_y = v.tex.pitch0; L.pitch_uv = v.tex.pitch1;
+    L.width = (int)src->width; L.height = (int)src->height;
+    L.n = (int)n;
+    // host destinations are written into pre_out_, packed, and copied back after the launch
+    size_t staged = 0;
+    for (uint32_t i = 0; i < n; i++)
+        if (out[i].mem_kind != SMR_MEM_DEVICE) staged += (size_t)out[i].width * out[i].height * 3 / 2;
+    if (staged > pre_out_.cap) CUDA_OK(cudaStreamSynchronize(stream_));
+    if (staged) CUDA_OK(pre_out_.ensure(staged));
+    transcode_calls_++;
+    int blocks = 0;
+    size_t off = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        const smr_rendition &o = out[i];
+        dev::TranscodeOut &J = L.out[i];
+        J.width = (int)o.width; J.height = (int)o.height; J.scaling = o.scaling;
+        if (o.mem_kind == SMR_MEM_DEVICE) {
+            J.y = (uint8_t *)o.planes[0]; J.uv = (uint8_t *)o.planes[1];
+            J.pitch_y = (int)(o.pitch[0] ? o.pitch[0] : o.width); J.pitch_uv = (int)(o.pitch[1] ? o.pitch[1] : o.width);
+        } else {
+            J.y = pre_out_.p + off; J.uv = J.y + (size_t)o.width * o.height;
+            J.pitch_y = J.pitch_uv = (int)o.width;
+            off += (size_t)o.width * o.height * 3 / 2;
+        }
+        J.tx = transcode_table(src->width, o.width);
+        J.ty = transcode_table(src->height, o.height);
+        J.cx = transcode_table(src->width / 2, o.width / 2);
+        J.cy = transcode_table(src->height / 2, o.height / 2);
+        if (!J.tx || !J.ty || !J.cx || !J.cy) { set_error("out of device memory for the transcoder tables"); return SMR_ERR_OUT_OF_MEMORY; }
+        J.tiles_x = (int)((o.width / 2 + dev::kTranscodeTileX - 1) / dev::kTranscodeTileX);
+        J.tile_begin = blocks;
+        blocks += J.tiles_x * (int)((o.height / 2 + dev::kTranscodeTileY - 1) / dev::kTranscodeTileY);
+    }
+    if (profiling_ && !transcode_ev_[0]) {
+        CUDA_OK(cudaEventCreate(&transcode_ev_[0]));
+        CUDA_OK(cudaEventCreate(&transcode_ev_[1]));
+    }
+    if (profiling_) CUDA_OK(cudaEventRecord(transcode_ev_[0], stream_));
+    if (dev::launch_transcode(L, blocks, stream_) < 0) { set_error(dev::last_launch_error()); return SMR_ERR_CUDA; }
+    stats_.kernel_launches++;
+    if (profiling_) CUDA_OK(cudaEventRecord(transcode_ev_[1], stream_));
+    for (uint32_t i = 0; i < n; i++) {
+        const smr_rendition &o = out[i];
+        if (o.mem_kind == SMR_MEM_DEVICE) continue;
+        const dev::TranscodeOut &J = L.out[i];
+        CUDA_OK(cudaMemcpy2DAsync(o.planes[0], o.pitch[0] ? o.pitch[0] : o.width, J.y, J.pitch_y, o.width, o.height,
+                                  cudaMemcpyDeviceToHost, stream_));
+        CUDA_OK(cudaMemcpy2DAsync(o.planes[1], o.pitch[1] ? o.pitch[1] : o.width, J.uv, J.pitch_uv, o.width, o.height / 2,
+                                  cudaMemcpyDeviceToHost, stream_));
+        stats_.d2h_bytes += (size_t)o.width * o.height * 3 / 2;
+    }
+    CUDA_OK(cudaStreamSynchronize(stream_));
+    if (profiling_) {
+        float ms = 0.0f;
+        CUDA_OK(cudaEventElapsedTime(&ms, transcode_ev_[0], transcode_ev_[1]));
+        prof_.total_ms[SMR_KERNEL_TRANSCODE] += ms;
+        prof_.launches[SMR_KERNEL_TRANSCODE] += 1;
+    }
+    return SMR_OK;
+}
+
 // FramePreProcessor::process_to_bytes / process_to_texture (state/frame_pre_processor.rs:60-100)
 smr_status Renderer::preprocess_frame(const smr_input_frame *f, uint32_t ow, uint32_t oh, void *rgba, uint32_t pitch,
                                       int32_t mem_kind, bool premultiply) {
@@ -2003,15 +2183,7 @@ smr_status Renderer::preprocess_frame(const smr_input_frame *f, uint32_t ow, uin
     FrameView v;
     if (smr_status st = read_frame(*f, v); st != SMR_OK) return st;
     if (!rescale) { ow = f->width; oh = f->height; }
-    for (int p = 0; p < 3 && f->mem_kind != SMR_MEM_DEVICE; p++) {
-        const FrameView::Plane &P = v.plane[p];
-        if (!P.p) continue;
-        if (P.row_bytes * P.rows > pre_planes_[p].cap) CUDA_OK(cudaStreamSynchronize(stream_));
-        CUDA_OK(pre_planes_[p].ensure(P.row_bytes * P.rows));
-        CUDA_OK(cudaMemcpy2DAsync(pre_planes_[p].p, P.row_bytes, P.p, P.pitch, P.row_bytes, P.rows, cudaMemcpyHostToDevice, stream_));
-        stats_.h2d_bytes += P.row_bytes * P.rows;
-        set_tex_plane(v.tex, p, pre_planes_[p].p, P.row_bytes);
-    }
+    if (smr_status st = upload_pre_planes(*f, v); st != SMR_OK) return st;
     const int kind = premultiply ? 2 : (rescale ? 1 : 0);
     return write_rgba(rgba, pitch, mem_kind, ow, oh, [&](uint8_t *dst, int dpitch) {
         return dev::launch_preprocess(v.tex, opts_.rendering_mode, kind, dst, dpitch, (int)ow, (int)oh, stream_);
@@ -3496,6 +3668,22 @@ smr_status smr_debug_sincos(const float *x, uint32_t n, float *s, float *c) {
     if (n == 0) return SMR_OK;
     return smr::dev::debug_sincos(x, (int)n, s, c) > 0 ? SMR_OK : SMR_ERR_CUDA;
 }
+smr_status smr_debug_transcode_taps(uint32_t in_len, uint32_t out_len, int32_t *nearest, int32_t *bilinear, float *frac,
+                                    int32_t *center, float *lanczos) {
+    if (!nearest || !bilinear || !frac || !center || !lanczos || in_len == 0 || out_len == 0 || in_len > 16384 || out_len > 16384)
+        return SMR_ERR_INVALID_ARGUMENT;
+    std::vector<smr::dev::TranscodeTap> taps;
+    smr::transcode_axis(in_len, out_len, taps);
+    for (uint32_t k = 0; k < out_len; k++) {
+        const smr::dev::TranscodeTap &t = taps[k];
+        nearest[k] = t.nearest;
+        bilinear[2 * k] = t.lo; bilinear[2 * k + 1] = t.hi;
+        frac[k] = t.frac;
+        center[k] = t.center;
+        for (int d = 0; d < 6; d++) lanczos[6 * k + d] = t.w[d];
+    }
+    return SMR_OK;
+}
 smr_status smr_debug_resample_stages(smr_renderer *r, smr_resample_stage_info *out, uint32_t cap, uint32_t *n,
                                      int32_t *convert_kinds, uint32_t convert_cap, uint32_t *n_convert) {
     SMR_GUARD(r->impl.debug_resample_stages(out, cap, n, convert_kinds, convert_cap, n_convert))
@@ -3504,6 +3692,9 @@ smr_status smr_preprocess_frame(smr_renderer *r, const smr_input_frame *f, uint3
                                 int32_t mem_kind) { SMR_GUARD(r->impl.preprocess_frame(f, ow, oh, rgba, pitch, mem_kind)) }
 smr_status smr_premultiply_rgba8(smr_renderer *r, const smr_input_frame *f, void *rgba, uint32_t pitch, int32_t mem_kind) {
     SMR_GUARD(r->impl.preprocess_frame(f, 0, 0, rgba, pitch, mem_kind, true))
+}
+smr_status smr_transcode_resize(smr_renderer *r, const smr_input_frame *src, const smr_rendition *out, uint32_t n) {
+    SMR_GUARD(r->impl.transcode_resize(src, out, n))
 }
 smr_status smr_render_text(smr_renderer *r, uint32_t w, uint32_t h, smr_rgba bg, const smr_glyph *glyphs, uint32_t n,
                            const smr_atlas *mask, const smr_atlas *color, int32_t color_mode, void *rgba, uint32_t pitch, int32_t mem_kind) {

@@ -133,6 +133,13 @@ class FrameSet:
     pts: float = 0.0
 
 
+class ScalingAlgorithm:
+    """gpu-video's ScalingAlgorithm (parameters.rs), the filter of one transcoder rendition"""
+    NearestNeighbor = F.SCALE_NEAREST
+    Bilinear = F.SCALE_BILINEAR
+    Lanczos3 = F.SCALE_LANCZOS3
+
+
 class FramePreProcessor:
     """smelter_render::FramePreProcessor (state/frame_pre_processor.rs:33-116) over a Renderer handle."""
 
@@ -798,6 +805,22 @@ class Renderer:
         out = np.empty((h, w, 4), np.uint8)
         self._check(self._lib.smr_preprocess_frame(self._h, arr, ow, oh, out.ctypes.data, 0, F.MEM_HOST), RenderSceneError)
         return out
+
+    def transcode_resize(self, frame: Frame, renditions) -> List[Tuple[np.ndarray, np.ndarray]]:
+        """VideoTranscoder's resize step (gpu-video vulkan_transcoder): one NV12 frame -> up to eight NV12 renditions in one
+        launch.  `renditions` is a sequence of (width, height, ScalingAlgorithm); returns, per rendition, its (h, w) Y plane
+        and its (h / 2, w / 2, 2) UV plane as host arrays."""
+        keep = []
+        arr = self._input_frames(FrameSet(frames={"_": frame}), keep)
+        outs = (F.Rendition * max(1, len(renditions)))()
+        planes = []
+        for i, (w, h, scaling) in enumerate(renditions):
+            y, uv = np.empty((h, w), np.uint8), np.empty((h // 2, w // 2, 2), np.uint8)
+            planes.append((y, uv))
+            outs[i].width, outs[i].height, outs[i].scaling, outs[i].mem_kind = w, h, scaling, F.MEM_HOST
+            outs[i].planes[0], outs[i].planes[1] = y.ctypes.data, uv.ctypes.data
+        self._check(self._lib.smr_transcode_resize(self._h, arr, outs, len(renditions)), RenderSceneError)
+        return planes
 
     def set_layouts(self, output_id: str, resolution: Resolution, output_format: int, root: Tuple[int, int],
                     child_input_ids: List[str], layouts):
