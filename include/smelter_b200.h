@@ -395,6 +395,19 @@ smr_status smr_unregister_shader(smr_renderer *r, const char *shader_id);
  * one's exact rule.  textureSampleBias is fragment-only: vs_main, or a function it calls, using it is
  * SMR_ERR_INVALID_ARGUMENT; textureSample, textureSampleLevel, textureSampleGrad and textureSampleBaseClampToEdge may
  * also be used in vs_main.  textureGather's component must be a const-expression in 0..3 (SMR_ERR_INVALID_ARGUMENT).
+ * The module language DESIGN.md states ("WGSL module language") is accepted: var<private> (per-invocation state: every
+ * vs_main vertex and every fs_main fragment, each plane's and each triangle's included, starts from the initial value;
+ * an initializer must be a const-expression), texture_2d<f32> and sampler values in helper parameters and lets, alias,
+ * const_assert, hexadecimal float literals (exactly representable), @size / @align on struct members (they move the
+ * uniform's fields), an fs_main result struct whose only member is @location(0) vec4<f32>, and diagnostic directives and
+ * attributes (checked, then ignored).  Their misuse is SMR_ERR_INVALID_ARGUMENT with line and column: a var<private>
+ * initializer that is not a const-expression or a var<private> of a texture or sampler type; a var or const of a texture
+ * or sampler, a function returning one or an entry point taking one; an alias cycle, redeclaration or unknown target; a
+ * const_assert that is false or not a const-expression; a hexadecimal float that is not exactly representable; an
+ * @align that is not a positive power of two or is below the member type's alignment, or an @size below its SizeOf;
+ * two diagnostic filters giving one rule two severities, a diagnostic directive after a declaration, or @diagnostic
+ * anywhere but on a function or a control-flow statement.  requires directives stay SMR_ERR_UNSUPPORTED.
+ * In a module with var<private>, operands are evaluated left to right, as WGSL orders them.
  * The parameter type is the uniform's WGSL type: scalars, vectors (a LIST of exactly N scalars), matrices (a LIST of
  * exactly R rows of C scalars), arrays (a LIST of at most N) and structs, validated as validation.rs does.  The bytes
  * stay ShaderParam::to_bytes (tight); the shader reads them at WGSL uniform-address-space offsets (AlignOf, SizeOf,

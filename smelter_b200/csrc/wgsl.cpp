@@ -41,6 +41,42 @@ struct Tok {
     int line = 1, col = 1;
 };
 
+// A hexadecimal float literal ("0x" digits ["." digits] ["p" exponent]) must be exactly representable: in f32 with the f
+// suffix, in f64 (abstract-float) without it.  Anything else is refused, as hexf-style parsers without rounding do.
+double hex_float(const std::string &num, bool f32, int line, int col) {
+    unsigned long long m = 0;
+    long long e2 = 0;
+    int sig = 0;   // significant hex digits in m
+    bool frac = false, inexact = false;
+    size_t i = 2;
+    for (; i < num.size() && num[i] != 'p' && num[i] != 'P'; i++) {
+        if (num[i] == '.') { frac = true; continue; }
+        const int d = isdigit((unsigned char)num[i]) ? num[i] - '0' : (tolower((unsigned char)num[i]) - 'a' + 10);
+        if (sig < 16) {
+            if (m || d) { m = m * 16 + d; sig++; }
+            if (frac) e2 -= 4;
+        } else {
+            inexact = inexact || d;   // past 61 significant bits: more than any f64 holds
+            if (!frac) e2 += 4;
+        }
+    }
+    if (i < num.size()) {
+        const long long e = strtoll(num.c_str() + i + 1, nullptr, 10);   // saturates; a huge exponent is out of range below
+        e2 += std::max(-100000LL, std::min(100000LL, e));
+    }
+    const char *what = f32 ? "f32" : "abstract-float (f64)";
+    if (inexact) invalid(line, col, std::string("hexadecimal float literal is not exactly representable in ") + what);
+    if (!m) return 0.0;
+    while (!(m & 1)) { m >>= 1; e2++; }
+    int bits = 0;
+    for (unsigned long long v = m; v; v >>= 1) bits++;
+    const int p = f32 ? 24 : 53, emin = f32 ? -126 : -1022, emax = f32 ? 127 : 1023;
+    const long long top = e2 + bits - 1;
+    if (top > emax) invalid(line, col, std::string("hexadecimal float literal out of the range of ") + what);
+    if (bits > p || e2 < emin - (p - 1)) invalid(line, col, std::string("hexadecimal float literal is not exactly representable in ") + what);
+    return std::ldexp((double)m, (int)e2);
+}
+
 std::vector<Tok> lex(const std::string &src) {
     std::vector<Tok> out;
     size_t i = 0;
@@ -84,10 +120,22 @@ std::vector<Tok> lex(const std::string &src) {
             size_t j = i;
             bool hex = c == '0' && i + 1 < src.size() && (src[i + 1] == 'x' || src[i + 1] == 'X');
             bool isf = false;
-            if (hex) {
+            if (hex) {   // 0x1f is an integer; 0x1.8, 0x.8p0 and 0X1P-2f are floats (without an exponent, f is a digit)
                 j += 2;
-                while (j < src.size() && isxdigit((unsigned char)src[j])) j++;
-                if (j < src.size() && (src[j] == '.' || src[j] == 'p' || src[j] == 'P')) unsupported(line, col, "hexadecimal float literals");
+                size_t digits = 0;
+                for (; j < src.size() && isxdigit((unsigned char)src[j]); j++) digits++;
+                if (j < src.size() && src[j] == '.') {
+                    isf = true;
+                    for (j++; j < src.size() && isxdigit((unsigned char)src[j]); j++) digits++;
+                }
+                if (j < src.size() && (src[j] == 'p' || src[j] == 'P')) {
+                    isf = true;
+                    j++;
+                    if (j < src.size() && (src[j] == '+' || src[j] == '-')) j++;
+                    if (j >= src.size() || !isdigit((unsigned char)src[j])) invalid(line, col, "malformed number");
+                    while (j < src.size() && isdigit((unsigned char)src[j])) j++;
+                }
+                if (!digits) invalid(line, col, "malformed number");
             } else {
                 while (j < src.size() && isdigit((unsigned char)src[j])) j++;
                 if (j < src.size() && src[j] == '.') { isf = true; j++; while (j < src.size() && isdigit((unsigned char)src[j])) j++; }
@@ -107,9 +155,9 @@ std::vector<Tok> lex(const std::string &src) {
             if (j < src.size() && (isalnum((unsigned char)src[j]) || src[j] == '_')) invalid(line, col, "malformed number");
             if (suf == "h") unsupported(line, col, "f16 literals");
             if (isf || suf == "f") {
-                if (hex) invalid(line, col, "malformed number");
                 t.k = Tok::Float;
-                t.fv = strtod(num.c_str(), nullptr);
+                if (hex && suf != "" && suf != "f") invalid(line, col, "malformed number");
+                t.fv = hex ? hex_float(num, suf == "f", line, col) : strtod(num.c_str(), nullptr);
             } else {
                 t.k = Tok::Int;
                 errno = 0;
@@ -232,7 +280,7 @@ struct Clause {
 };
 struct Stmt {
     enum K { Block, Var, Let, Const, Assign, Incr, Decr, If, Switch, Loop, For, While, Break, BreakIf, Continue, Return,
-             Discard, CallS, Phony } k = Block;
+             Discard, CallS, Phony, ConstAssert } k = Block;
     int line = 0, col = 0;
     std::string name, op;
     TypeP ty;
@@ -270,6 +318,7 @@ struct Param {
     std::string name;
     TypeP ty;
     Attrs attrs;
+    int line = 0, col = 0;
 };
 struct FnDecl {
     std::string name;
@@ -279,11 +328,18 @@ struct FnDecl {
     std::vector<StmtP> body;
     int line = 0, col = 0;
 };
+struct AliasDecl {
+    std::string name;
+    TypeP ty;
+    int line = 0, col = 0;
+};
 struct Module {
     std::vector<StructDecl> structs;
     std::vector<Global> globals;
     std::vector<ConstDecl> consts;
     std::vector<FnDecl> fns;
+    std::vector<AliasDecl> aliases;
+    std::vector<StmtP> asserts;   // module-scope const_assert
 };
 
 // ---------------------------------------------------------------------------------------------------------------- parser
@@ -315,14 +371,45 @@ struct Parser {
         return t[p++].s;
     }
 
+    // diagnostic(severity, rule) of a directive or an attribute: {severity, rule}; the rule may be namespaced (a.b)
+    std::vector<std::string> diagnostic_args() {
+        expect("(");
+        int line = cur().line, col = cur().col;
+        std::string sev = ident();
+        if (sev != "error" && sev != "warning" && sev != "info" && sev != "off")
+            invalid(line, col, "unknown diagnostic severity '" + sev + "'");
+        expect(",");
+        std::string rule = ident();
+        if (accept(".")) rule += "." + ident();
+        accept(",");
+        expect(")");
+        return {sev, rule};
+    }
+    // diagnostic filters on one range conflict when they give one rule two severities
+    std::map<std::string, std::string> module_diagnostics;
+    static void diagnostic_filter(std::map<std::string, std::string> &seen, const std::vector<std::string> &d, int line, int col) {
+        auto it = seen.find(d[1]);
+        if (it != seen.end() && it->second != d[0]) invalid(line, col, "conflicting diagnostic filters for '" + d[1] + "'");
+        seen[d[1]] = d[0];
+    }
+
+    // WGSL allows @diagnostic on functions and control-flow statements only
+    static void no_diagnostic(const Attrs &a) {
+        if (const Attr *d = find_attr(a, "diagnostic")) invalid(d->line, d->col, "@diagnostic is allowed only on a function or a control-flow statement");
+    }
+
     Attrs attrs() {
         Attrs out;
+        std::map<std::string, std::string> diags;
         while (is("@")) {
             p++;
             Attr a;
             a.line = cur().line; a.col = cur().col;
             a.name = ident();
-            if (accept("(")) {
+            if (a.name == "diagnostic") {   // checked, then ignored: there is no uniformity analysis to filter
+                a.args = diagnostic_args();
+                diagnostic_filter(diags, a.args, a.line, a.col);
+            } else if (accept("(")) {
                 while (!is(")")) {
                     if (cur().k == Tok::Id) a.args.push_back(t[p++].s);
                     else if (cur().k == Tok::Int) { a.args.push_back(std::to_string(t[p].iv)); p++; }
@@ -562,7 +649,7 @@ struct Parser {
 
     StmtP stmt() {
         Attrs a = attrs();
-        (void)a;
+        if (!(is("{") || is_id("if") || is_id("switch") || is_id("loop") || is_id("for") || is_id("while"))) no_diagnostic(a);
         if (accept(";")) return mks(Stmt::Block);
         if (is("{")) {
             StmtP s = mks(Stmt::Block);
@@ -652,7 +739,7 @@ struct Parser {
             p++;
             if (!is(";")) s->e = expr();
         } else if (is_id("const_assert")) {
-            unsupported(cur().line, cur().col, "const_assert");
+            s = const_assert();
         } else {
             s = simple();
         }
@@ -660,9 +747,31 @@ struct Parser {
         return s;
     }
 
+    StmtP const_assert() {
+        StmtP s = mks(Stmt::ConstAssert);
+        p++;
+        s->e = expr();
+        return s;
+    }
+
     void module() {
+        bool declared = false;   // directives come before every declaration
         while (cur().k != Tok::End) {
             if (accept(";")) continue;
+            if (is_id("diagnostic")) {
+                int line = cur().line, col = cur().col;
+                if (declared) invalid(line, col, "a diagnostic directive must come before every declaration");
+                p++;
+                diagnostic_filter(module_diagnostics, diagnostic_args(), line, col);
+                expect(";");
+                continue;
+            }
+            declared = declared || !is_id("enable");
+            if (is_id("const_assert")) {
+                m.asserts.push_back(const_assert());
+                expect(";");
+                continue;
+            }
             if (is_id("enable")) {
                 p++;
                 for (;;) {
@@ -673,9 +782,10 @@ struct Parser {
                 expect(";");
                 continue;
             }
-            if (is_id("requires") || is_id("diagnostic")) unsupported(cur().line, cur().col, cur().s + " directives");
+            if (is_id("requires")) unsupported(cur().line, cur().col, "requires directives");
             Attrs a = attrs();
             int line = cur().line, col = cur().col;
+            if (!is_id("fn")) no_diagnostic(a);
             if (is_id("struct")) {
                 p++;
                 StructDecl s;
@@ -685,6 +795,7 @@ struct Parser {
                 while (!is("}")) {
                     Member mb;
                     mb.attrs = attrs();
+                    no_diagnostic(mb.attrs);
                     mb.line = cur().line; mb.col = cur().col;
                     mb.name = ident();
                     expect(":");
@@ -723,7 +834,14 @@ struct Parser {
             } else if (is_id("override")) {
                 unsupported(line, col, "override declarations");
             } else if (is_id("alias")) {
-                unsupported(line, col, "type aliases");
+                p++;
+                AliasDecl a;
+                a.line = line; a.col = col;
+                a.name = ident();
+                expect("=");
+                a.ty = type();
+                expect(";");
+                m.aliases.push_back(a);
             } else if (is_id("fn")) {
                 p++;
                 FnDecl f;
@@ -734,6 +852,8 @@ struct Parser {
                 while (!is(")")) {
                     Param pr;
                     pr.attrs = attrs();
+                    no_diagnostic(pr.attrs);
+                    pr.line = cur().line; pr.col = cur().col;
                     pr.name = ident();
                     expect(":");
                     pr.ty = type();
@@ -743,6 +863,7 @@ struct Parser {
                 expect(")");
                 if (accept("->")) {
                     f.ret_attrs = attrs();
+                    no_diagnostic(f.ret_attrs);
                     f.ret = type();
                 }
                 f.body = block();
@@ -760,6 +881,7 @@ struct FieldInfo {
     Ty ty;
     Attrs attrs;
     uint32_t offset = 0;
+    uint32_t size = 0, align = 0;   // @size / @align, 0 when absent
 };
 struct StructInfo {
     std::string name;
@@ -769,8 +891,17 @@ struct StructInfo {
     std::string cname;   // a predeclared result struct (frexp, modf): its wgsl_rt.cuh type
 };
 
+// a const-expression's value, as const_assert evaluates it: s the scalar kind, n 0 (a scalar) or the vector size; floats
+// in f, integers and bools in i
+struct KV {
+    SK s = S_BOOL;
+    int n = 0;
+    double f[4] = {0, 0, 0, 0};
+    long long i[4] = {0, 0, 0, 0};
+};
+
 struct Sym {
-    enum K { Local, Param, Const, ModConst, Uniform, Base, Textures, Sampler } k = Local;
+    enum K { Local, Param, Const, ModConst, Uniform, Base, Textures, Sampler, Private } k = Local;
     Ty ty;
     bool mut = false;
     bool has_cv = false;
@@ -778,6 +909,9 @@ struct Sym {
     std::string code;
     bool cint = false;   // a constant of concrete integer type, whose value is civ
     long long civ = 0;
+    bool is_const = false;       // a const declaration: kv is its value when kv_status is 0
+    int kv_status = 0;           // otherwise why it has none (SMR_ERR_INVALID_ARGUMENT: not a const-expression)
+    KV kv;
 };
 
 struct FnInfo {
@@ -815,6 +949,9 @@ struct Checker {
     const Global *uniform = nullptr;
     Ty uniform_ty;
     std::map<std::string, std::string> loader_names;
+    std::map<std::string, const AliasDecl *> aliases;
+    std::string out_private, out_private_init;   // var<private>: the members of wg_private and their initialisers
+    std::vector<std::string> alias_stack;   // the aliases being resolved, to find a cycle
 
     explicit Checker(Module &mod) : m(mod) {}
 
@@ -857,6 +994,8 @@ struct Checker {
             case Ty::Mat: return "wm<" + std::to_string(t.n) + ", " + std::to_string(t.m) + ">";
             case Ty::Arr: return "wa<" + cty(*t.el) + ", " + std::to_string(t.n) + ">";
             case Ty::Struct: return structs[t.sid].cname.empty() ? "S_" + structs[t.sid].name : structs[t.sid].cname;
+            case Ty::Tex: return "unsigned";      // a texture value is its binding-array index
+            case Ty::Samp: return "wg_sampler";
             default: return "void";
         }
     }
@@ -879,6 +1018,15 @@ struct Checker {
 
     Ty resolve(const TypeP &tp) {
         const std::string &n = tp->name;
+        auto al = aliases.find(n);
+        if (al != aliases.end()) {   // a type alias is its target, wherever it is written
+            if (!tp->targs.empty()) invalid(tp->line, tp->col, "the alias " + n + " takes no template arguments");
+            for (const std::string &a : alias_stack) if (a == n) invalid(al->second->line, al->second->col, "alias " + n + " refers to itself");
+            alias_stack.push_back(n);
+            Ty t = resolve(al->second->ty);
+            alias_stack.pop_back();
+            return t;
+        }
         auto need = [&](size_t k) {
             if (tp->targs.size() != k) invalid(tp->line, tp->col, n + " expects " + std::to_string(k) + " template argument(s)");
         };
@@ -979,7 +1127,6 @@ struct Checker {
         for (const Member &mb : d->members) {
             if (!seen.insert(mb.name).second) invalid(mb.line, mb.col, "duplicate member " + mb.name);
             for (const Attr &a : mb.attrs) {
-                if (a.name == "size" || a.name == "align") unsupported(a.line, a.col, "@" + a.name + " on struct members");
                 if (a.name == "builtin" && !a.args.empty() && a.args[0] != "position" && a.args[0] != "front_facing")
                     unsupported(a.line, a.col, "@builtin(" + a.args[0] + ")");
             }
@@ -988,6 +1135,21 @@ struct Checker {
             f.ty = resolve(mb.ty);
             if (f.ty.k == Ty::Tex || f.ty.k == Ty::Samp || f.ty.k == Ty::TexArr) invalid(mb.line, mb.col, "a struct member cannot be a texture or sampler");
             f.attrs = mb.attrs;
+            for (const Attr &a : mb.attrs) {   // @size / @align: the member's place in memory (the uniform's layout)
+                if (a.name != "size" && a.name != "align") continue;
+                uint32_t ta, ts;
+                layout(f.ty, ta, ts, a.line, a.col, false);
+                const long long v = attr_int(a);
+                if (a.name == "align") {
+                    if (v <= 0 || (v & (v - 1)) || v > (1LL << 30)) invalid(a.line, a.col, "@align must be a positive power of two, found " + std::to_string(v));
+                    // a member sits at a multiple of its type's alignment in every address space (RequiredAlignOf)
+                    if (v < (long long)ta) invalid(a.line, a.col, "@align(" + std::to_string(v) + ") is below the AlignOf " + std::to_string(ta) + " of " + tname(f.ty));
+                    f.align = (uint32_t)v;
+                } else {
+                    if (v < (long long)ts || v > (1LL << 30)) invalid(a.line, a.col, "@size(" + std::to_string(v) + ") is below the SizeOf " + std::to_string(ts) + " of " + tname(f.ty));
+                    f.size = (uint32_t)v;
+                }
+            }
             si.fields.push_back(f);
             body += "    " + cty(f.ty) + " m_" + mb.name + ";\n";
         }
@@ -997,15 +1159,27 @@ struct Checker {
         resolving.pop_back();
     }
 
-    // the uniform address space layout (WGSL: AlignOf, SizeOf, array stride), with its constraints checked
-    void layout(const Ty &t, uint32_t &align, uint32_t &size, int line, int col) {
+    // an attribute's one integer argument: a literal or a module constant
+    long long attr_int(const Attr &a) {
+        if (a.args.size() != 1) invalid(a.line, a.col, "@" + a.name + " takes one argument");
+        const std::string &v = a.args[0];
+        if (isdigit((unsigned char)v[0])) return atoll(v.c_str());
+        Sym *s = lookup(v);
+        if (s && s->k == Sym::ModConst && s->has_cv && !s->cv.f && !s->cv.n) return s->cv.iv[0];
+        if (s && s->k == Sym::ModConst && s->cint) return s->civ;
+        invalid(a.line, a.col, "@" + a.name + " needs a constant integer");
+    }
+
+    // WGSL's memory layout (AlignOf, SizeOf, array stride; a member's @align / @size replace its type's); `uniform`: with
+    // the uniform address space's constraints checked
+    void layout(const Ty &t, uint32_t &align, uint32_t &size, int line, int col, bool uniform = true) {
         switch (t.k) {
             case Ty::Scalar:
-                if (t.s == S_BOOL) invalid(line, col, "bool is not host-shareable and cannot be in a uniform");
+                if (uniform && t.s == S_BOOL) invalid(line, col, "bool is not host-shareable and cannot be in a uniform");
                 align = size = 4;
                 return;
             case Ty::Vec:
-                if (t.s == S_BOOL) invalid(line, col, "bool is not host-shareable and cannot be in a uniform");
+                if (uniform && t.s == S_BOOL) invalid(line, col, "bool is not host-shareable and cannot be in a uniform");
                 align = t.n == 2 ? 8 : 16;
                 size = 4 * t.n;
                 return;
@@ -1017,9 +1191,9 @@ struct Checker {
             }
             case Ty::Arr: {
                 uint32_t ea, es;
-                layout(*t.el, ea, es, line, col);
+                layout(*t.el, ea, es, line, col, uniform);
                 uint32_t stride = (es + ea - 1) / ea * ea;
-                if (stride % 16) invalid(line, col, "the uniform address space needs an array stride that is a multiple of 16; " +
+                if (uniform && stride % 16) invalid(line, col, "the uniform address space needs an array stride that is a multiple of 16; " +
                                                     tname(t) + " has " + std::to_string(stride));
                 align = ea;
                 size = stride * t.n;
@@ -1031,16 +1205,17 @@ struct Checker {
                 bool after_struct = false;
                 uint32_t min_next = 0;
                 for (FieldInfo &f : si.fields) {
-                    uint32_t fa, fs;
-                    layout(f.ty, fa, fs, line, col);
+                    uint32_t ta, ts;
+                    layout(f.ty, ta, ts, line, col, uniform);
+                    const uint32_t fa = f.align ? f.align : ta, fs = f.size ? f.size : ts;
                     off = (off + fa - 1) / fa * fa;
-                    if ((f.ty.k == Ty::Struct || f.ty.k == Ty::Arr) && off % 16)
+                    if (uniform && (f.ty.k == Ty::Struct || f.ty.k == Ty::Arr) && off % 16)
                         invalid(line, col, "the uniform address space needs member " + si.name + "." + f.name + " at a multiple of 16");
-                    if (after_struct && off < min_next)
+                    if (uniform && after_struct && off < min_next)
                         invalid(line, col, "the uniform address space needs 16 bytes of padding after a struct member of " + si.name);
                     f.offset = off;
                     after_struct = f.ty.k == Ty::Struct;
-                    min_next = off + (fs + 15) / 16 * 16;
+                    min_next = off + (ts + 15) / 16 * 16;
                     off += fs;
                     al = std::max(al, fa);
                 }
@@ -1294,7 +1469,7 @@ struct Checker {
             else if (op == "*" && R.k == Ty::Mat && L.k == Ty::Vec && L.n == R.m) r = vec(S_F32, R.n);
             else if (op == "*" && L.k == Ty::Mat && R.k == Ty::Mat && L.n == R.m) { r = L; r.n = R.n; }
             else invalid(e->line, e->col, "no '" + op + "' for " + tname(L) + " and " + tname(R));
-            e->code = f + "(" + code(a) + ", " + code(b) + ")";
+            e->code = ordered(f, {code(a), code(b)});
             return set(e, r);
         }
         if (!(L.k == Ty::Scalar || L.k == Ty::Vec) || !(R.k == Ty::Scalar || R.k == Ty::Vec))
@@ -1303,7 +1478,7 @@ struct Checker {
             if (!integral(L.s) || !integral(R.s) || L.k != R.k || L.n != R.n) invalid(e->line, e->col, "no '" + op + "' for " + tname(L) + " and " + tname(R));
             conv_default(a);
             conv(b, with_elem(R, S_U32));
-            e->code = f + "(" + code(a) + ", " + code(b) + ")";
+            e->code = ordered(f, {code(a), code(b)});
             return set(e, concrete(L));
         }
         if (op == "&" || op == "|" || op == "^") {
@@ -1312,7 +1487,7 @@ struct Checker {
             if (!(integral(s) || (s == S_BOOL && op != "^"))) invalid(e->line, e->col, "no '" + op + "' for " + tname(L));
             Ty t = concrete(with_elem(L, s));
             conv(a, t); conv(b, t);
-            e->code = f + "(" + code(a) + ", " + code(b) + ")";
+            e->code = ordered(f, {code(a), code(b)});
             return set(e, t);
         }
         bool cmp = !arith;
@@ -1331,7 +1506,7 @@ struct Checker {
         int n = std::max(L.k == Ty::Vec ? L.n : 0, R.k == Ty::Vec ? R.n : 0);
         if (L.k == Ty::Scalar && n) ca = "wsplat<" + std::to_string(n) + ">(" + ca + ")";
         if (R.k == Ty::Scalar && n) cb = "wsplat<" + std::to_string(n) + ">(" + cb + ")";
-        e->code = f + "(" + ca + ", " + cb + ")";
+        e->code = ordered(f, {ca, cb});
         SK rs = cmp ? S_BOOL : s;
         return set(e, n ? vec(rs, n) : scalar(rs));
     }
@@ -1420,8 +1595,44 @@ struct Checker {
 
     std::string value(const ExprP &e) { return code(e); }
 
+    // f(operands).  WGSL evaluates operands left to right and C++ leaves a call's argument order unspecified; that is
+    // only visible once a call can write var<private> state, so in a module with var<private>, operands of which two
+    // or more call a user function or read private state are evaluated in order into temporaries first.
+    bool has_private = false;
+    std::string ordered(const std::string &f, const std::vector<std::string> &ops) {
+        int touching = 0;
+        bool call = false;
+        for (const std::string &o : ops) {
+            const bool c = o.find("fn_") != std::string::npos;
+            call = call || c;
+            touching += c || o.find("ctx.pv.") != std::string::npos;
+        }
+        std::string s;
+        if (!has_private || !call || touching < 2) {
+            for (size_t i = 0; i < ops.size(); i++) s += (i ? ", " : "") + ops[i];
+            return f + "(" + s + ")";
+        }
+        std::string args;
+        for (size_t i = 0; i < ops.size(); i++) {   // values, copied: a later operand may write what an earlier one read
+            const std::string t = ops[i] == "ctx" ? ops[i] : "wg_o" + std::to_string(i);
+            if (t != ops[i]) s += "const auto " + t + " = " + ops[i] + "; ";
+            args += (i ? ", " : "") + t;
+        }
+        return "[&]() { " + s + "return " + f + "(" + args + "); }()";
+    }
+
+    // the type expression an alias names, followed to a type that is not an alias
+    TypeP dealias(TypeP tp) {
+        std::set<std::string> seen;
+        for (auto it = aliases.find(tp->name); it != aliases.end() && tp->targs.empty(); it = aliases.find(tp->name)) {
+            if (!seen.insert(tp->name).second) invalid(it->second->line, it->second->col, "alias " + tp->name + " refers to itself");
+            tp = it->second->ty;
+        }
+        return tp;
+    }
+
     Ty check_call(const ExprP &e) {
-        const TypeP &c = e->callee;
+        const TypeP c = dealias(e->callee);
         const std::string &n = c->name;
         for (const char *u : kUnsupportedFns) if (n == u) unsupported(e->line, e->col, n);
         std::vector<Ty> A;
@@ -1445,8 +1656,12 @@ struct Checker {
                 invalid(e->line, e->col, "an entry point cannot be called");
             nargs(uf->second.params.size());
             if (cur_fn) cur_fn->calls.push_back(n);
-            std::string s = args(uf->second.params);
-            e->code = uf->second.cname + "(ctx" + (s.empty() ? "" : ", " + s) + ")";
+            std::vector<std::string> ops = {"ctx"};
+            for (size_t i = 0; i < e->a.size(); i++) {
+                conv(e->a[i], uf->second.params[i]);
+                ops.push_back(code(e->a[i]));
+            }
+            e->code = ordered(uf->second.cname, ops);
             return set(e, uf->second.ret);
         }
         // structs
@@ -1552,12 +1767,12 @@ struct Checker {
                 return set_cv(e, cv);
             }
             s = concrete_of(s);
-            std::string parts;
+            std::vector<std::string> parts;
             for (size_t i = 0; i < A.size(); i++) {
                 conv(e->a[i], with_elem(A[i], s));
-                parts += (i ? ", " : "") + code(e->a[i]);
+                parts.push_back(code(e->a[i]));
             }
-            e->code = "wvec<" + cscalar(s) + ", " + std::to_string(N) + ">(" + parts + ")";
+            e->code = ordered("wvec<" + cscalar(s) + ", " + std::to_string(N) + ">", parts);
             return set(e, vec(s, N));
         }
         if (n.compare(0, 3, "mat") == 0 && (n.size() == 6 || n.size() == 7) && n[4] == 'x') {
@@ -1568,16 +1783,16 @@ struct Checker {
             if (e->a.empty()) { e->code = cty(t) + "{}"; return set(e, t); }
             if (e->a.size() == 1 && A[0] == t) { e->code = code(e->a[0]); return set(e, t); }
             int total = 0;
-            std::string parts;
+            std::vector<std::string> parts;
             for (size_t i = 0; i < A.size(); i++) {
                 if (A[i].k == Ty::Scalar) total += 1;
                 else if (A[i].k == Ty::Vec && A[i].n == t.m) total += t.m;
                 else invalid(e->a[i]->line, e->a[i]->col, "a matrix constructor takes scalars or column vectors");
                 conv(e->a[i], with_elem(A[i], S_F32));
-                parts += (i ? ", " : "") + code(e->a[i]);
+                parts.push_back(code(e->a[i]));
             }
             if (total != t.n * t.m) invalid(e->line, e->col, n + " needs " + std::to_string(t.n * t.m) + " components");
-            e->code = "wmat<" + std::to_string(t.n) + ", " + std::to_string(t.m) + ">(" + parts + ")";
+            e->code = ordered("wmat<" + std::to_string(t.n) + ", " + std::to_string(t.m) + ">", parts);
             return set(e, t);
         }
         if (n == "array") {
@@ -1598,10 +1813,10 @@ struct Checker {
             e->code = cty(t) + "{{" + args(to) + "}}";
             return set(e, t);
         }
-        // texture builtins: textures[i] and the sampler, as the header declares them
+        // texture builtins: a texture value (textures[i], or a let or parameter holding one) and the sampler
         auto tex_arg = [&](size_t i) {
             Ty tt = check(e->a[i]);
-            if (tt.k != Ty::Tex || e->a[i]->k != Expr::Idx) invalid(e->line, e->col, n + " takes textures[i]");
+            if (tt.k != Ty::Tex) invalid(e->line, e->col, n + " takes a texture_2d<f32>, such as textures[i]");
             return "(unsigned)(" + e->a[i]->code + ")";
         };
         auto samp_arg = [&](size_t i) {
@@ -1616,7 +1831,7 @@ struct Checker {
             nargs(3);
             std::string t = tex_arg(0);
             samp_arg(1);
-            e->code = "ctx.tex.sample(" + t + ", " + val_arg(2, vec(S_F32, 2)) + ")";
+            e->code = ordered("ctx.tex.sample", {t, val_arg(2, vec(S_F32, 2))});
             return set(e, vec(S_F32, 4));
         }
         if (n == "textureSampleLevel" || n == "textureSampleBias" || n == "textureSampleGrad" || n == "textureSampleBaseClampToEdge" ||
@@ -1625,7 +1840,7 @@ struct Checker {
             const size_t k = n == "textureSampleGrad" ? 5 : n == "textureSampleBaseClampToEdge" ? 3 : 4;
             if (e->a.size() == k + 1 && n != "textureSampleBaseClampToEdge") unsupported(e->line, e->col, n + " with an offset");
             nargs(k);
-            std::string comp;
+            std::vector<std::string> ops;
             if (gather) {   // textureGather(component, t, s, coords): the component is a const-expression in 0..3
                 const ExprP &c = e->a[0];
                 Ty ct = check(c);
@@ -1635,18 +1850,18 @@ struct Checker {
                 else if (c->cint) v = c->civ;
                 else invalid(c->line, c->col, "textureGather's component must be a const-expression");
                 if (v < 0 || v > 3) invalid(c->line, c->col, "textureGather's component must be 0, 1, 2 or 3, found " + std::to_string(v));
-                comp = std::to_string(v) + ", ";
+                ops.push_back(std::to_string(v));
             }
             const size_t o = gather ? 1 : 0;
-            std::string t = tex_arg(o);
+            ops.push_back(tex_arg(o));
             samp_arg(o + 1);
-            std::string a = t + ", " + val_arg(o + 2, vec(S_F32, 2));
+            ops.push_back(val_arg(o + 2, vec(S_F32, 2)));
             if (n == "textureSampleBias" && cur_fn && !cur_fn->frag_line) { cur_fn->frag_line = e->line; cur_fn->frag_col = e->col; }
-            if (n == "textureSampleLevel" || n == "textureSampleBias") a += ", " + val_arg(3, scalar(S_F32));
-            if (n == "textureSampleGrad") a += ", " + val_arg(3, vec(S_F32, 2)) + ", " + val_arg(4, vec(S_F32, 2));
+            if (n == "textureSampleLevel" || n == "textureSampleBias") ops.push_back(val_arg(3, scalar(S_F32)));
+            if (n == "textureSampleGrad") { ops.push_back(val_arg(3, vec(S_F32, 2))); ops.push_back(val_arg(4, vec(S_F32, 2))); }
             const char *m = n == "textureSampleLevel" ? "sample_level" : n == "textureSampleBias" ? "sample_bias" :
                             n == "textureSampleGrad" ? "sample_grad" : gather ? "gather" : "sample_clamped";
-            e->code = std::string("ctx.tex.") + m + "(" + comp + a + ")";
+            e->code = ordered(std::string("ctx.tex.") + m, ops);
             return set(e, vec(S_F32, 4));
         }
         if (n == "textureDimensions" || n == "textureNumLevels") {
@@ -1661,7 +1876,8 @@ struct Checker {
                 Ty l = check(e->a[1]);
                 if (l.k != Ty::Scalar || !integral(l.s)) invalid(e->a[1]->line, e->a[1]->col, "textureDimensions' level must be i32 or u32, found " + tname(l));
                 conv_default(e->a[1]);
-                t += ", " + code(e->a[1]);
+                e->code = ordered("ctx.tex.dims", {t, code(e->a[1])});
+                return set(e, vec(S_U32, 2));
             }
             e->code = "ctx.tex.dims(" + t + ")";
             return set(e, vec(S_U32, 2));
@@ -1679,9 +1895,9 @@ struct Checker {
             return s;
         };
         auto fin = [&](const Ty &r) {
-            std::string s;
-            for (size_t i = 0; i < e->a.size(); i++) s += (i ? ", " : "") + code(e->a[i]);
-            e->code = "wb_" + n + "(" + s + ")";
+            std::vector<std::string> ops;
+            for (size_t i = 0; i < e->a.size(); i++) ops.push_back(code(e->a[i]));
+            e->code = ordered("wb_" + n, ops);
             return set(e, r);
         };
         if (f1.count(n)) {
@@ -1708,19 +1924,19 @@ struct Checker {
             Ty shape = A[0].k == Ty::Vec ? A[0] : A.back();
             for (const Ty &t : A) if (t.k == Ty::Vec) shape = t;
             Ty r = with_elem(shape, s);
-            std::string parts;
+            std::vector<std::string> parts;
             for (size_t i = 0; i < k; i++) {
                 bool scalar_ok = n == "mix" && i == 2;   // mix(vec, vec, f32)
                 if (A[i].k != r.k || A[i].n != r.n) {
                     if (!(scalar_ok && A[i].k == Ty::Scalar)) invalid(e->a[i]->line, e->a[i]->col, n + ": mismatched argument " + tname(A[i]));
                     conv(e->a[i], scalar(s));
-                    parts += (i ? ", " : "") + std::string("wsplat<") + std::to_string(r.n) + ">(" + code(e->a[i]) + ")";
+                    parts.push_back("wsplat<" + std::to_string(r.n) + ">(" + code(e->a[i]) + ")");
                 } else {
                     conv(e->a[i], r);
-                    parts += (i ? ", " : "") + code(e->a[i]);
+                    parts.push_back(code(e->a[i]));
                 }
             }
-            e->code = "wb_" + n + "(" + parts + ")";
+            e->code = ordered("wb_" + n, parts);
             return set(e, r);
         }
         if (n == "length" || n == "normalize" || n == "dot" || n == "distance" || n == "cross") {
@@ -1862,6 +2078,225 @@ struct Checker {
         return t;
     }
 
+    // ---- const-expressions: const_assert evaluates them here, with WGSL's rules for const-expressions ----
+    // Concrete f32 results are rounded to f32 after each operation; abstract ones stay f64 / int64, and a comparison of two
+    // abstract operands compares them unconverted.  Overflow, a non-finite float, division by zero and a shift by the bit
+    // width or more are errors, as WGSL makes them for const-expressions.
+    [[noreturn]] void not_const(const ExprP &e) { invalid(e->line, e->col, "not a const-expression"); }
+    static bool is_float(SK s) { return s == S_F32 || s == S_AF; }
+
+    double kv_float(const KV &v, int k, int line, int col, SK to) {
+        double d = is_float(v.s) ? v.f[k] : (double)v.i[k];
+        if (to == S_F32) d = (float)d;
+        if (!std::isfinite(d)) invalid(line, col, "constant expression overflows");
+        return d;
+    }
+    long long kv_int(long double x, SK to, int line, int col) {
+        const long double lo = to == S_I32 ? -2147483648.0L : to == S_U32 ? 0.0L : -9223372036854775808.0L;
+        const long double hi = to == S_I32 ? 2147483647.0L : to == S_U32 ? 4294967295.0L : 9223372036854775807.0L;
+        if (!(x >= lo && x <= hi)) invalid(line, col, "constant expression overflows " + sname(to));
+        return (long long)x;
+    }
+    // a component converted to `to` as a value constructor converts it (f32 -> integer truncates and saturates)
+    KV kv_convert(const KV &v, SK to, int line, int col) {
+        KV r = v;
+        r.s = to;
+        for (int k = 0; k < std::max(1, v.n); k++) {
+            if (is_float(to)) { r.f[k] = kv_float(v, k, line, col, to); continue; }
+            if (to == S_BOOL) { r.i[k] = is_float(v.s) ? v.f[k] != 0.0 : v.i[k] != 0; continue; }
+            if (!is_float(v.s)) {   // i32 <-> u32 keep the bits
+                r.i[k] = to == S_U32 ? (long long)(uint32_t)v.i[k] : to == S_I32 ? (long long)(int32_t)(uint32_t)v.i[k] : v.i[k];
+                continue;
+            }
+            const double x = std::trunc(v.f[k]);
+            r.i[k] = x != x ? 0 : to == S_U32 ? (x < 0 ? 0 : x > 4294967295.0 ? 4294967295LL : (long long)x)
+                                              : (x < -2147483648.0 ? -2147483648LL : x > 2147483647.0 ? 2147483647LL : (long long)x);
+        }
+        return r;
+    }
+
+    KV ceval(const ExprP &e, bool keep_abstract = false) {
+        if (e->has_cv) {
+            KV r;
+            r.s = e->cv.f ? S_AF : S_AI;
+            r.n = e->cv.n;
+            for (int k = 0; k < 4; k++) { r.f[k] = e->cv.fv[k]; r.i[k] = e->cv.iv[k]; }
+            if (keep_abstract) return r;
+            const SK to = e->has_target ? e->target.s : concrete_of(r.s);
+            if (!is_float(to)) for (int k = 0; k < std::max(1, r.n); k++) lit(e->cv, k, to, e->line, e->col);   // range
+            return kv_convert(r, to, e->line, e->col);
+        }
+        const Ty &t = e->ty;
+        KV r;
+        r.s = t.s;
+        r.n = t.k == Ty::Vec ? t.n : 0;
+        const bool value_type = t.k == Ty::Scalar || t.k == Ty::Vec;
+        switch (e->k) {
+            case Expr::Lit:
+                if (e->lk == 'b') r.i[0] = e->bv;
+                else if (r.s == S_F32) r.f[0] = (float)e->fv;
+                else r.i[0] = e->iv;
+                return r;
+            case Expr::Id: {
+                Sym *s = lookup(e->s);
+                if (!s || !s->is_const) not_const(e);
+                if (s->kv_status == SMR_ERR_UNSUPPORTED) unsupported(e->line, e->col, "const_assert over '" + e->s + "', which is not evaluated at translation");
+                if (s->kv_status) invalid(e->line, e->col, "'" + e->s + "' is not a const-expression");
+                return s->kv;
+            }
+            case Expr::Un: {
+                const KV a = ceval(e->a[0]);
+                for (int k = 0; k < std::max(1, r.n); k++) {
+                    if (e->s == "!") r.i[k] = !a.i[k];
+                    else if (e->s == "~") r.i[k] = r.s == S_U32 ? (long long)(uint32_t)~a.i[k] : ~a.i[k];
+                    else if (is_float(r.s)) r.f[k] = -a.f[k];
+                    else r.i[k] = kv_int(-(long double)a.i[k], r.s, e->line, e->col);
+                }
+                return r;
+            }
+            case Expr::Bin: return ceval_binary(e, r);
+            case Expr::Idx: {
+                const KV b = ceval(e->a[0]), i = ceval(e->a[1]);
+                if (!value_type || !b.n) unsupported(e->line, e->col, "const_assert over elements of " + tname(e->a[0]->ty));
+                if (i.i[0] < 0 || i.i[0] >= b.n) invalid(e->a[1]->line, e->a[1]->col, "index out of bounds");
+                r = b;
+                r.n = 0;
+                r.f[0] = b.f[i.i[0]]; r.i[0] = b.i[i.i[0]];
+                return r;
+            }
+            case Expr::Mem: {
+                const KV b = ceval(e->a[0]);
+                if (e->a[0]->ty.k != Ty::Vec) unsupported(e->line, e->col, "const_assert over struct members");
+                for (size_t k = 0; k < e->s.size(); k++) {
+                    const char *c = strchr("xyzw", e->s[k]);
+                    const int j = c ? (int)(c - "xyzw") : (int)(strchr("rgba", e->s[k]) - "rgba");
+                    r.f[k] = b.f[j]; r.i[k] = b.i[j];
+                }
+                return r;
+            }
+            case Expr::Call: {
+                const TypeP c = dealias(e->callee);
+                const std::string &n = c->name;
+                if (fns.count(n) || kTextureFns.count(n)) not_const(e);
+                std::vector<KV> A;
+                for (const ExprP &x : e->a) A.push_back(ceval(x));
+                if (!value_type) unsupported(e->line, e->col, "const_assert over " + tname(t) + " values");
+                if (A.empty()) return r;   // the zero value
+                if (n == "f32" || n == "i32" || n == "u32" || n == "bool" || (t.k == Ty::Vec && A.size() == 1 && A[0].n == r.n))
+                    return kv_convert(A[0], r.s, e->line, e->col);
+                if (t.k == Ty::Vec && n.compare(0, 3, "vec") == 0) {   // components in order, or one scalar splatted
+                    int k = 0;
+                    for (const KV &a : A) {
+                        const KV v = kv_convert(a, r.s, e->line, e->col);
+                        for (int j = 0; j < std::max(1, a.n); j++, k++) { r.f[k] = v.f[j]; r.i[k] = v.i[j]; }
+                    }
+                    for (; k < r.n; k++) { r.f[k] = r.f[0]; r.i[k] = r.i[0]; }
+                    return r;
+                }
+                if ((n == "all" || n == "any") && A.size() == 1) {
+                    bool all = true, any = false;
+                    for (int k = 0; k < std::max(1, A[0].n); k++) { all = all && A[0].i[k]; any = any || A[0].i[k]; }
+                    r.i[0] = n == "all" ? all : any;
+                    return r;
+                }
+                if (n == "select" && A.size() == 3) {
+                    const KV f = kv_convert(A[0], r.s, e->line, e->col), tr = kv_convert(A[1], r.s, e->line, e->col);
+                    for (int k = 0; k < std::max(1, r.n); k++) {
+                        const bool c2 = A[2].i[A[2].n ? k : 0] != 0;
+                        r.f[k] = c2 ? tr.f[k] : f.f[k]; r.i[k] = c2 ? tr.i[k] : f.i[k];
+                    }
+                    return r;
+                }
+                if ((n == "abs" || n == "min" || n == "max") && A.size() == (n == "abs" ? 1u : 2u)) {
+                    for (int k = 0; k < std::max(1, r.n); k++) {
+                        const KV x = kv_convert(A[0], r.s, e->line, e->col), y = kv_convert(A.back(), r.s, e->line, e->col);
+                        const int ka = A[0].n ? k : 0, kb = A.back().n ? k : 0;
+                        if (is_float(r.s)) r.f[k] = n == "abs" ? std::fabs(x.f[ka]) : n == "min" ? std::fmin(x.f[ka], y.f[kb]) : std::fmax(x.f[ka], y.f[kb]);
+                        else r.i[k] = n == "abs" ? (r.s == S_I32 ? (long long)(int32_t)(uint32_t)std::llabs(x.i[ka]) : std::llabs(x.i[ka]))
+                                                 : n == "min" ? std::min(x.i[ka], y.i[kb]) : std::max(x.i[ka], y.i[kb]);
+                    }
+                    return r;
+                }
+                unsupported(e->line, e->col, n + " in a const_assert");
+            }
+        }
+        return r;
+    }
+
+    KV ceval_binary(const ExprP &e, KV r) {
+        const std::string &op = e->s;
+        const bool cmp = op == "==" || op == "!=" || op == "<" || op == "<=" || op == ">" || op == ">=";
+        const bool abs_cmp = cmp && e->a[0]->has_cv && e->a[1]->has_cv;   // two abstract operands compare as they are
+        const KV a = ceval(e->a[0], abs_cmp), b = ceval(e->a[1], abs_cmp);
+        const int line = e->line, col = e->col;
+        if (op == "&&" || op == "||") { r.i[0] = op == "&&" ? (a.i[0] && b.i[0]) : (a.i[0] || b.i[0]); return r; }
+        const SK s = a.s;   // the operands' common kind (a shift's count is u32)
+        for (int k = 0; k < std::max(1, std::max(a.n, b.n)); k++) {
+            const int ka = a.n ? k : 0, kb = b.n ? k : 0;
+            if (cmp) {
+                int c;
+                if (is_float(s) || is_float(b.s)) {
+                    const double x = kv_float(a, ka, line, col, S_AF), y = kv_float(b, kb, line, col, S_AF);
+                    c = x < y ? -1 : x > y ? 1 : 0;
+                } else {
+                    c = a.i[ka] < b.i[kb] ? -1 : a.i[ka] > b.i[kb] ? 1 : 0;
+                }
+                r.i[k] = op == "==" ? c == 0 : op == "!=" ? c != 0 : op == "<" ? c < 0 : op == "<=" ? c <= 0 : op == ">" ? c > 0 : c >= 0;
+                continue;
+            }
+            if (is_float(s)) {
+                const double x = a.f[ka], y = b.f[kb];
+                auto rd = [&](double v) { return s == S_F32 ? (double)(float)v : v; };
+                double v;
+                if (op == "+") v = rd(x + y);
+                else if (op == "-") v = rd(x - y);
+                else if (op == "*") v = rd(x * y);
+                else if (op == "/") v = rd(x / y);
+                else if (op == "%") v = rd(x - rd(y * std::trunc(rd(x / y))));
+                else unsupported(line, col, "'" + op + "' in a const_assert");
+                if (!std::isfinite(v)) invalid(line, col, "constant expression overflows");
+                r.f[k] = v;
+                continue;
+            }
+            const long long x = a.i[ka], y = b.i[kb];
+            if (s == S_BOOL) { r.i[k] = op == "&" ? (x && y) : (x || y); continue; }
+            if (op == "&" || op == "|" || op == "^") { r.i[k] = op == "&" ? x & y : op == "|" ? x | y : x ^ y; continue; }
+            if (op == "<<" || op == ">>") {
+                const int bits = s == S_AI ? 64 : 32;
+                if (y < 0 || y >= bits) invalid(line, col, "shift by " + std::to_string(y) + " in a const-expression");
+                if (op == ">>") { r.i[k] = s == S_U32 ? (long long)((uint64_t)x >> y) : x >> y; continue; }
+                r.i[k] = kv_int((long double)x * std::ldexp(1.0L, (int)y), s, line, col);
+                continue;
+            }
+            if ((op == "/" || op == "%") && y == 0) invalid(line, col, "integer division by zero in a constant expression");
+            long double v;   // in long double, where no int64 operation here overflows; kv_int checks the range
+            if (op == "+") v = (long double)x + y;
+            else if (op == "-") v = (long double)x - y;
+            else if (op == "*") v = (long double)x * y;
+            else if (op == "/") v = y == -1 ? -(long double)x : (long double)(x / y);
+            else v = y == -1 ? 0 : (long double)(x % y);
+            r.i[k] = kv_int(v, s, line, col);
+        }
+        return r;
+    }
+
+    // a const declaration's value, for const_assert: evaluated now, or the reason it cannot be
+    void const_value(Sym &sym, const ExprP &init) {
+        sym.is_const = true;
+        if (sym.has_cv) return;   // an abstract constant: its uses carry the value
+        try {
+            sym.kv = ceval(init);
+        } catch (const Fail &f) {
+            sym.kv_status = f.status;
+        }
+    }
+
+    void const_assert(const StmtP &s) {
+        const Ty t = check(s->e);
+        if (t != scalar(S_BOOL)) invalid(s->e->line, s->e->col, "const_assert needs a bool, found " + tname(t));
+        if (!ceval(s->e).i[0]) invalid(s->line, s->col, "const_assert failed");
+    }
+
     // ---- statements ----
     std::string ind(int d) { return std::string(4 * d, ' '); }
 
@@ -1896,12 +2331,20 @@ struct Checker {
         return o + ind(d) + "}";
     }
 
+    // a texture or sampler is a value a let or a parameter may hold, never a var's or a const's
+    void handle_decl(const StmtP &s, const Ty &t) {
+        if (t.k == Ty::TexArr) unsupported(s->line, s->col, "binding arrays in local values");
+        if ((t.k == Ty::Tex || t.k == Ty::Samp) && s->k != Stmt::Let)
+            invalid(s->line, s->col, std::string("a ") + (s->k == Stmt::Var ? "var" : "const") + " cannot hold " + tname(t));
+    }
+
     Ty decl_type(const StmtP &s) {
         Ty t = check(s->e);
         if (t.k == Ty::Void) invalid(s->e->line, s->e->col, "a function without a return value has no value");
-        if (t.k == Ty::Tex || t.k == Ty::Samp || t.k == Ty::TexArr) unsupported(s->line, s->col, "textures and samplers in local values");
+        handle_decl(s, t);
         if (s->ty) {
             Ty d = resolve(s->ty);
+            handle_decl(s, d);
             conv(s->e, d);
             return d;
         }
@@ -1919,7 +2362,7 @@ struct Checker {
                 Ty t;
                 std::string init;
                 if (s->e) { t = decl_type(s); init = value(s->e); }
-                else if (s->ty) t = resolve(s->ty);
+                else if (s->ty) { t = resolve(s->ty); handle_decl(s, t); }
                 else invalid(s->line, s->col, "a var needs a type or an initializer");
                 Sym sym;
                 sym.k = Sym::Local; sym.ty = t; sym.mut = true; sym.code = "u_" + s->name;
@@ -1939,9 +2382,13 @@ struct Checker {
                     if (s->k == Stmt::Const) const_int(sym, s->e);
                     o += ind(d) + "const " + cty(t) + " u_" + s->name + " = " + value(s->e) + ";\n";
                 }
+                if (s->k == Stmt::Const) const_value(sym, s->e);
                 declare(s->name, sym, s->line, s->col);
                 return;
             }
+            case Stmt::ConstAssert:
+                const_assert(s);
+                return;
             case Stmt::Phony:
                 check(s->e);
                 conv_default(s->e);
@@ -1953,26 +2400,32 @@ struct Checker {
                 check(s->e);
                 if (s->op == "=") {
                     conv(s->e, L);
-                    o += ind(d) + code(s->lhs) + " = " + value(s->e) + ";\n";
+                    if (has_private)   // WGSL evaluates the left side first; C++17 evaluates the right operand of = first
+                        o += ind(d) + "{ auto &wg_ref_ = " + code(s->lhs) + "; wg_ref_ = " + value(s->e) + "; }\n";
+                    else
+                        o += ind(d) + code(s->lhs) + " = " + value(s->e) + ";\n";
                     return;
                 }
-                // e1 op= e2 is e1 = e1 op e2, with e1 evaluated once
+                // e1 op= e2 is e1 = e1 op e2, with e1 evaluated once.  With private state, e1's value is read into wg_val_
+                // before e2 is evaluated, as WGSL's `let p = &e1; *p = *p op e2;` does (e2 may call a function writing e1)
+                const std::string cur = has_private ? "wg_val_" : "wg_ref_";
                 auto bin = std::make_shared<Expr>();
                 bin->k = Expr::Bin; bin->line = s->line; bin->col = s->col;
                 bin->s = s->op.substr(0, s->op.size() - 1);
                 auto ref = std::make_shared<Expr>();
-                ref->k = Expr::Id; ref->s = "wg_ref_"; ref->line = s->line; ref->col = s->col;
+                ref->k = Expr::Id; ref->s = cur; ref->line = s->line; ref->col = s->col;
                 push();
                 Sym rs;
-                rs.ty = L; rs.mut = true; rs.code = "wg_ref_";
-                scopes.back()["wg_ref_"] = rs;
+                rs.ty = L; rs.mut = true; rs.code = cur;
+                scopes.back()[cur] = rs;
                 bin->a = {ref, s->e};
                 s->e->has_target = false;
                 Ty r = check(bin);
                 pop();
                 conv(bin, L);
                 if (r != L) invalid(s->line, s->col, "'" + s->op + "' changes the type of the left side");
-                o += ind(d) + "{ auto &wg_ref_ = " + code(s->lhs) + "; wg_ref_ = " + code(bin) + "; }\n";
+                o += ind(d) + "{ auto &wg_ref_ = " + code(s->lhs) + "; " + (has_private ? "const auto wg_val_ = wg_ref_; " : "") +
+                     "wg_ref_ = " + code(bin) + "; }\n";
                 return;
             }
             case Stmt::Incr:
@@ -2145,6 +2598,10 @@ Translation run(const std::string &src) {
         si.name = s.name; si.line = s.line; si.col = s.col;
         ck.structs.push_back(si);
     }
+    for (const AliasDecl &a : m.aliases) {
+        if (ck.struct_ids.count(a.name) || ck.aliases.count(a.name)) invalid(a.line, a.col, "redeclaration of '" + a.name + "'");
+        ck.aliases[a.name] = &a;
+    }
     ck.push();   // module scope
     // module constants, in order (a constant may use only those before it)
     for (const ConstDecl &c : m.consts) {
@@ -2165,27 +2622,44 @@ Translation run(const std::string &src) {
             if (c.init->code.find("ctx") != std::string::npos) invalid(c.line, c.col, "a module constant must be a constant expression");
             ck.out_consts += "__device__ inline " + ck.cty(t) + " u_" + c.name + "() { return " + ck.value(c.init) + "; }\n";
         }
+        if (ck.aliases.count(c.name)) invalid(c.line, c.col, "redeclaration of '" + c.name + "'");
+        ck.const_value(sym, c.init);
         ck.declare(c.name, sym, c.line, c.col);
     }
     for (size_t i = 0; i < ck.structs.size(); i++) ck.resolve_struct((int)i);
+    for (const AliasDecl &a : m.aliases) ck.resolve(a.ty);   // an unknown target or a cycle, even when unused
     // globals: the header's and the user's uniform
     const Global *g_tex = nullptr, *g_samp = nullptr, *g_base = nullptr;
     for (const Global &g : m.globals) {
         const Attr *ga = find_attr(g.attrs, "group"), *ba = find_attr(g.attrs, "binding");
         int group = ga && !ga->args.empty() ? atoi(ga->args[0].c_str()) : -1, binding = ba && !ba->args.empty() ? atoi(ba->args[0].c_str()) : -1;
-        if (!g.ty) invalid(g.line, g.col, "a module variable needs a type");
+        if (!g.ty && !(g.space == "private" && g.init)) invalid(g.line, g.col, "a module variable needs a type");
         if (group == 1 && binding == 0 && g.space != "uniform")
             invalid(g.line, g.col, "the user binding at group(1) binding(0) must be var<uniform> (UserBindingNotUniform)");
         if (g.space == "storage") unsupported(g.line, g.col, "storage buffers (var<storage>)");
         if (g.space == "workgroup") unsupported(g.line, g.col, "var<workgroup>");
-        if (g.space == "private") unsupported(g.line, g.col, "var<private>");
         if (g.space == "push_constant")
             invalid(g.line, g.col, "var<push_constant> is not accepted: base_params is var<immediate>, as the shader header declares it");
-        if (g.init) unsupported(g.line, g.col, "initialised module variables");
-        Ty t = ck.resolve(g.ty);
+        if (g.init && g.space != "private") unsupported(g.line, g.col, "initialised module variables");
+        Ty t = g.ty ? ck.resolve(g.ty) : Ty();
         Sym sym;
         sym.ty = t;
-        if (g.space == "immediate") {
+        if (g.space == "private") {   // per-invocation state in wg_ctx, reset as each vs_main / fs_main invocation begins
+            if (ga || ba) invalid(g.line, g.col, "var<private> takes no binding");
+            std::string init;
+            if (g.init) {
+                Ty it = ck.check(g.init);
+                if (g.ty) ck.conv(g.init, t);
+                else { ck.conv_default(g.init); t = concrete(it); }
+                init = ck.value(g.init);
+                if (init.find("ctx") != std::string::npos) invalid(g.init->line, g.init->col, "a var<private> initializer must be a const-expression");
+            }
+            if (t.k == Ty::Tex || t.k == Ty::Samp || t.k == Ty::TexArr || t.k == Ty::Void) invalid(g.line, g.col, "a var<private> cannot hold " + ck.tname(t));
+            sym.k = Sym::Private; sym.ty = t; sym.mut = true; sym.code = "ctx.pv.u_" + g.name;
+            ck.has_private = true;
+            ck.out_private += "    " + ck.cty(t) + " u_" + g.name + ";\n";
+            if (g.init) ck.out_private_init += "    ctx.pv.u_" + g.name + " = " + init + ";\n";
+        } else if (g.space == "immediate") {
             if (group >= 0 || binding >= 0) invalid(g.line, g.col, "var<immediate> takes no binding");
             if (g_base) invalid(g.line, g.col, "a second var<immediate>");
             g_base = &g;
@@ -2202,7 +2676,7 @@ Translation run(const std::string &src) {
             sym.k = Sym::Textures;
         } else if (group == 2 && binding == 0 && g.space.empty()) {
             g_samp = &g;
-            sym.k = Sym::Sampler;
+            sym.k = Sym::Sampler; sym.code = "wg_sampler{}";
         } else if (g.space == "uniform") {
             unsupported(g.line, g.col, "uniform bindings other than group(1) binding(0)");
         } else if (g.space.empty() && group >= 0) {
@@ -2211,7 +2685,7 @@ Translation run(const std::string &src) {
         } else {
             invalid(g.line, g.col, "unknown address space '" + g.space + "'");
         }
-        if (ck.lookup(g.name)) invalid(g.line, g.col, "redeclaration of '" + g.name + "'");
+        if (ck.lookup(g.name) || ck.aliases.count(g.name)) invalid(g.line, g.col, "redeclaration of '" + g.name + "'");
         ck.declare(g.name, sym, g.line, g.col);
     }
     // validate_contains_header: the header's globals, at their spaces and bindings, with equivalent types (matched by
@@ -2240,16 +2714,20 @@ Translation run(const std::string &src) {
     // functions: signatures first (a function may call one declared after it)
     const FnDecl *vs = nullptr, *fs = nullptr;
     for (const FnDecl &f : m.fns) {
-        if (ck.fns.count(f.name) || ck.struct_ids.count(f.name) || ck.lookup(f.name)) invalid(f.line, f.col, "redeclaration of '" + f.name + "'");
+        if (ck.fns.count(f.name) || ck.struct_ids.count(f.name) || ck.aliases.count(f.name) || ck.lookup(f.name))
+            invalid(f.line, f.col, "redeclaration of '" + f.name + "'");
         if (find_attr(f.attrs, "compute")) unsupported(f.line, f.col, "compute shaders");
+        const bool entry = find_attr(f.attrs, "vertex") || find_attr(f.attrs, "fragment");
         FnInfo fi;
         fi.d = &f;
-        for (const Param &p : f.params) {
+        for (const Param &p : f.params) {   // a helper may take a texture or the sampler; an entry point may not
             Ty t = ck.resolve(p.ty);
-            if (t.k == Ty::Tex || t.k == Ty::Samp || t.k == Ty::TexArr) unsupported(f.line, f.col, "texture and sampler parameters");
+            if (t.k == Ty::TexArr) unsupported(f.line, f.col, "binding array parameters");
+            if ((t.k == Ty::Tex || t.k == Ty::Samp) && entry) invalid(p.line, p.col, "an entry point cannot take " + ck.tname(t));
             fi.params.push_back(t);
         }
         fi.ret = f.ret ? ck.resolve(f.ret) : Ty();
+        if (fi.ret.k == Ty::Tex || fi.ret.k == Ty::Samp || fi.ret.k == Ty::TexArr) invalid(f.ret->line, f.ret->col, "a function cannot return " + ck.tname(fi.ret));
         fi.cname = "fn_" + f.name;
         if (find_attr(f.attrs, "vertex")) {
             if (f.name == "vs_main") vs = &f;
@@ -2275,6 +2753,7 @@ Translation run(const std::string &src) {
         if (!ok) invalid(vs->line, vs->col, "VertexInput must be { @location(0) position: vec3<f32>, @location(1) tex_coords: vec2<f32> } (VertexShaderBadInput)");
     }
     if (!fs) invalid(1, 1, "no @fragment fn fs_main");
+    for (const StmtP &a : m.asserts) ck.const_assert(a);
     // function bodies
     for (const FnDecl &f : m.fns) {
         FnInfo &fi = ck.fns[f.name];
@@ -2399,16 +2878,28 @@ Translation run(const std::string &src) {
         }
         fs_args += ", " + nm;
     }
+    // fs_main's result: @location(0) vec4<f32>, or a struct whose only member is one
+    std::string fs_result;
     {
-        const Attr *l = find_attr(fs->ret_attrs, "location");
-        if (fsi.ret != vec(S_F32, 4) || !l || l->args.size() != 1 || l->args[0] != "0")
-            unsupported(fs->line, fs->col, "fs_main results other than @location(0) vec4<f32>");
+        auto location0 = [](const Attrs &a) {
+            const Attr *l = find_attr(a, "location");
+            return l && l->args.size() == 1 && l->args[0] == "0";
+        };
+        bool ok = fsi.ret == vec(S_F32, 4) && location0(fs->ret_attrs);
+        if (fsi.ret.k == Ty::Struct && fs->ret_attrs.empty()) {
+            const auto &f = ck.structs[fsi.ret.sid].fields;
+            ok = f.size() == 1 && f[0].ty == vec(S_F32, 4) && f[0].attrs.size() == 1 && location0(f[0].attrs);
+            if (ok) fs_result = ".m_" + f[0].name;
+        }
+        if (!ok) unsupported(fs->line, fs->col, "fs_main results other than @location(0) vec4<f32>");
     }
     // the translation
     Translation tr;
     std::string out = "// translated from WGSL\n" + ck.out_structs;
     const Ty base = ck.lookup(g_base->name)->ty;
-    out += "struct wg_ctx {\n    " + ck.cty(base) + " base;\n    const unsigned char *params;\n    wg_textures tex;\n    bool discarded;\n};\n";
+    if (!ck.out_private.empty()) out += "struct wg_private {\n" + ck.out_private + "};\n";
+    out += "struct wg_ctx {\n    " + ck.cty(base) + " base;\n    const unsigned char *params;\n    wg_textures tex;\n    bool discarded;\n" +
+           (ck.out_private.empty() ? "" : "    wg_private pv;\n") + "};\n";
     if (ck.uniform) {
         ck.load(ck.uniform_ty, "p");   // the loaders of the uniform's composite types
         uint32_t al, sz;
@@ -2416,6 +2907,12 @@ Translation run(const std::string &src) {
         tr.uniform_size = sz;
     }
     out += ck.out_loaders + ck.out_consts + ck.out_protos;
+    // the var<private> state starts at its initial value (or zero) in every invocation
+    std::string reset;
+    if (!ck.out_private.empty()) {
+        out += "__device__ inline void wg_private_reset(wg_ctx &ctx) {\n    ctx.pv = wg_private{};\n" + ck.out_private_init + "}\n";
+        reset = "    wg_private_reset(ctx);\n";
+    }
     out += ck.out_bodies;
     const Ty &vin = vsi.params[0];
     out += "#define WG_NVARY " + std::to_string(nvary) + "\n";
@@ -2431,11 +2928,11 @@ Translation run(const std::string &src) {
            "                           {-1.0f, 1.0f, 0.0f, 0.0f, 0.0f}, {-1.0f, -1.0f, 0.0f, 0.0f, 1.0f}};\n"
            "    " + ck.cty(vin) + " in;\n"
            "    in.m_position = wv<float, 3>{{P[vid][0], P[vid][1], P[vid][2]}};\n"
-           "    in.m_tex_coords = wv<float, 2>{{P[vid][3], P[vid][4]}};\n"
+           "    in.m_tex_coords = wv<float, 2>{{P[vid][3], P[vid][4]}};\n" + reset +
            "    const " + ck.cty(vsi.ret) + " o = fn_vs_main(ctx, in);\n" + vs_store +
            "    (void)vary;\n}\n";
-    out += "__device__ inline bool wg_fragment(wg_ctx &ctx, const float *pos, const float *vary, float4 &out) {\n" + fs_pre +
-           "    (void)vary;\n    ctx.discarded = false;\n    const wv<float, 4> r = fn_fs_main(ctx" + fs_args + ");\n"
+    out += "__device__ inline bool wg_fragment(wg_ctx &ctx, const float *pos, const float *vary, float4 &out) {\n" + fs_pre + reset +
+           "    (void)vary;\n    ctx.discarded = false;\n    const wv<float, 4> r = fn_fs_main(ctx" + fs_args + ")" + fs_result + ";\n"
            "    out = make_float4(r.v[0], r.v[1], r.v[2], r.v[3]);\n    return !ctx.discarded;\n}\n";
     tr.cuda = out;
     // the parameter type: validate_params' view of the uniform's WGSL type

@@ -425,6 +425,10 @@ template <class T, int N> __device__ inline wv<T, N> wldv(const unsigned char *p
     return r;
 }
 
+// A texture value is its index into the header's textures (an unsigned); the header has one sampler, so a sampler value
+// carries nothing
+struct wg_sampler {};
+
 // the header's bindings: textures (group 0) through sampler_ (group 2), as smr_textures samples them
 struct wg_textures {
     const smr::dev::Tables *T;
