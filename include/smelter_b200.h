@@ -263,7 +263,9 @@ typedef enum {
     SMR_KERNEL_WEB = 10,           /* web view node textures (k_web) */
     SMR_KERNEL_SHADER = 11,        /* shader node textures (each shader module's smr_shader_main) */
     SMR_KERNEL_TRANSCODE = 12,     /* transcoder renditions (k_transcode, smr_transcode_resize) */
-    SMR_KERNEL_CLASSES = 13
+    SMR_KERNEL_VIDEO_CONVERT = 13, /* NV12 -> RGBA frame converter (k_video_nv12_to_rgba, smr_video_nv12_to_rgba); the
+                                      reverse converter is k_output and counts as SMR_KERNEL_OUTPUT */
+    SMR_KERNEL_CLASSES = 14
 } smr_kernel_class;
 typedef struct {
     double total_ms[SMR_KERNEL_CLASSES];
@@ -534,6 +536,37 @@ typedef struct {
 } smr_rendition;
 #define SMR_MAX_RENDITIONS 8
 smr_status smr_transcode_resize(smr_renderer *r, const smr_input_frame *src, const smr_rendition *out, uint32_t n);
+
+/* gpu-video's frame converters (wgpu_helpers/: WgpuNv12ToRgbaConverter, WgpuRgbaToNv12Converter): one conversion per
+ * call, on the renderer's stream, blocking like smr_preprocess_frame.  Both are full-target draws sampled with a linear,
+ * clamp-to-edge sampler at the target's pixel centres, so a target of another size than the source is a bilinear
+ * rescale.  The result does not depend on the renderer's rendering mode.
+ * `converter` is the converter's WgpuConverterParameters; only (BT709, Limited) exists (OnlyLimitedBT709Supported:
+ * SMR_ERR_UNSUPPORTED for every other pair).
+ *
+ * smr_video_nv12_to_rgba: `src` is an SMR_FRAME_NV12 frame, host or device, whose width x height is the decoder's crop
+ * with origin (0, 0), as smr_transcode_resize takes it; nothing outside the crop is read.  `frame` is the decoded frame's
+ * metadata: its color_space must be Unspecified or the converter's and its color_range the converter's
+ * (IncompatibleFrame: SMR_ERR_INVALID_ARGUMENT).  `rgba` has out_height rows of `pitch` bytes (0 = tightly packed) in
+ * host or device memory per mem_kind; bytes past a row's out_width x 4 are not written.  0 x 0 is the source size.
+ * Arithmetic: DESIGN.md NC-11.
+ * smr_video_rgba_to_nv12: `src` is an SMR_FRAME_RGBA8 frame of any size, read as raw bytes (an Rgba8Unorm view); alpha is
+ * not used.  The target's y plane has out_height rows of out_width bytes, its uv plane out_height / 2 rows of
+ * out_width / 2 {u, v} pairs, each at its pitch (0, or a NULL `pitch`: tightly packed); bytes past a row are not written.  The arithmetic is
+ * K11's (rgba_to_nv12.wgsl), the kernel k_output's.
+ * Checked before anything needs a device, so a host-only handle answers them too: SMR_ERR_UNSUPPORTED for the converter
+ * pair and for a source format other than NV12 (nv12_to_rgba) or RGBA8 (rgba_to_nv12); SMR_ERR_INVALID_ARGUMENT for
+ * an unknown enum value, an odd NV12 side, a target side of 0 (except 0 x 0 for nv12_to_rgba) or above 16384, an odd
+ * NV12 target side, a null plane, a pitch shorter than a row, an unknown mem_kind, a device RGBA target whose pointer or
+ * pitch is not 4-byte aligned, and smr_render's checks of the source frame (size, planes, pitch, device-plane alignment). */
+typedef enum { SMR_COLOR_SPACE_UNSPECIFIED = 0, SMR_COLOR_SPACE_BT709 = 1, SMR_COLOR_SPACE_BT601_NTSC = 2,
+               SMR_COLOR_SPACE_BT601_PAL = 3 } smr_color_space;                     /* gpu-video device.rs ColorSpace */
+typedef enum { SMR_COLOR_RANGE_FULL = 0, SMR_COLOR_RANGE_LIMITED = 1 } smr_color_range;   /* device.rs ColorRange */
+typedef struct { int32_t color_space, color_range; } smr_video_color;   /* WgpuConverterParameters / a frame's metadata */
+smr_status smr_video_nv12_to_rgba(smr_renderer *r, smr_video_color converter, const smr_input_frame *src, smr_video_color frame,
+                                  uint32_t out_width, uint32_t out_height, void *rgba, uint32_t pitch, int32_t mem_kind);
+smr_status smr_video_rgba_to_nv12(smr_renderer *r, smr_video_color converter, const smr_input_frame *src, uint32_t out_width,
+                                  uint32_t out_height, void *const planes[2], const uint32_t pitch[2], int32_t mem_kind);
 
 /* Text nodes (SURVEY 8f-2): TextRendererNode::render (transformations/text_renderer.rs:72-167).  Shaping and glyph
  * rasterisation (cosmic-text / swash inside glyphon, CPU code in the reference too) stay on the caller's side; what the

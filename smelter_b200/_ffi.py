@@ -223,8 +223,16 @@ class Rendition(C.Structure):   # smr_rendition
                 ("pitch", C.c_uint32 * 2), ("mem_kind", C.c_int32)]
 
 
+COLOR_SPACE_UNSPECIFIED, COLOR_SPACE_BT709, COLOR_SPACE_BT601_NTSC, COLOR_SPACE_BT601_PAL = 0, 1, 2, 3
+COLOR_RANGE_FULL, COLOR_RANGE_LIMITED = 0, 1
+
+
+class VideoColor(C.Structure):   # smr_video_color
+    _fields_ = [("color_space", C.c_int32), ("color_range", C.c_int32)]
+
+
 KERNEL_CLASSES = ["convert", "weights", "resample_box", "resample_first", "resample_last", "composite", "output",
-                  "fill", "resample_fused", "image", "web", "shader", "transcode"]
+                  "fill", "resample_fused", "image", "web", "shader", "transcode", "video_convert"]
 
 
 class KernelTimes(C.Structure):
@@ -235,7 +243,7 @@ EXPORTS = [
     "smr_create", "smr_destroy", "smr_register_input", "smr_unregister_input", "smr_register_image", "smr_unregister_image",
     "smr_register_svg_image",
     "smr_register_web_renderer", "smr_unregister_web_renderer", "smr_web_set_frame", "smr_web_set_child_rects", "smr_register_shader", "smr_unregister_shader", "smr_register_wgsl_shader", "smr_update_scene",
-    "smr_unregister_output", "smr_set_layouts", "smr_render", "smr_render_begin", "smr_render_end", "smr_preprocess_frame", "smr_premultiply_rgba8", "smr_transcode_resize", "smr_render_text", "smr_debug_partition", "smr_debug_tile_plan", "smr_debug_weights", "smr_debug_sincos", "smr_debug_transcode_taps", "smr_debug_fused_jobs", "smr_debug_resample_stages", "smr_debug_composite_layers", "smr_debug_interior", "smr_output_plane_sizes",
+    "smr_unregister_output", "smr_set_layouts", "smr_render", "smr_render_begin", "smr_render_end", "smr_preprocess_frame", "smr_premultiply_rgba8", "smr_transcode_resize", "smr_video_nv12_to_rgba", "smr_video_rgba_to_nv12", "smr_render_text", "smr_debug_partition", "smr_debug_tile_plan", "smr_debug_weights", "smr_debug_sincos", "smr_debug_transcode_taps", "smr_debug_fused_jobs", "smr_debug_resample_stages", "smr_debug_composite_layers", "smr_debug_interior", "smr_output_plane_sizes",
     "smr_component_default", "smr_debug_layouts", "smr_debug_node_layouts", "smr_debug_image_nodes", "smr_debug_set_inputs", "smr_get_stats", "smr_set_profiling", "smr_get_kernel_times",
     "smr_comm_get_unique_id", "smr_comm_init", "smr_comm_broadcast_inputs", "smr_comm_exchange_inputs", "smr_comm_pull_inputs", "smr_peer_pool_alloc", "smr_peer_pool_open", "smr_peer_pool_close", "smr_peer_pool_free", "smr_comm_destroy", "smr_host_register", "smr_host_unregister", "smr_cuda_stream", "smr_last_error",
     "smr_version",
@@ -281,6 +289,12 @@ def lib():
     L.smr_premultiply_rgba8.restype = C.c_int32
     L.smr_transcode_resize.argtypes = [vp, C.POINTER(InputFrame), C.POINTER(Rendition), C.c_uint32]
     L.smr_transcode_resize.restype = C.c_int32
+    L.smr_video_nv12_to_rgba.argtypes = [vp, VideoColor, C.POINTER(InputFrame), VideoColor, C.c_uint32, C.c_uint32, C.c_void_p,
+                                         C.c_uint32, C.c_int32]
+    L.smr_video_nv12_to_rgba.restype = C.c_int32
+    L.smr_video_rgba_to_nv12.argtypes = [vp, VideoColor, C.POINTER(InputFrame), C.c_uint32, C.c_uint32, C.c_void_p,
+                                         C.c_void_p, C.c_int32]
+    L.smr_video_rgba_to_nv12.restype = C.c_int32
     L.smr_render_text.argtypes = [vp, C.c_uint32, C.c_uint32, Rgba, C.c_void_p, C.c_uint32, C.POINTER(Atlas), C.POINTER(Atlas),
                                   C.c_int32, C.c_void_p, C.c_uint32, C.c_int32]
     L.smr_render_text.restype = C.c_int32

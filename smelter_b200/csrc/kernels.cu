@@ -11,6 +11,7 @@
 //   k_output      rgba_to_yuv / rgba_to_nv12 stand-alone (root size != output size, odd sizes)
 //   k_fill        r8/rg8_fill_value.wgsl (black frame)                                  (K6)
 //   k_transcode   gpu-video's vulkan_transcoder/shader.wgsl: NV12 -> up to eight NV12 renditions (transcode.cuh)
+//   k_video_nv12_to_rgba  gpu-video's nv12_to_rgba.wgsl: NV12 -> RGBA8 at any size (video_convert.cuh)
 //
 // Numeric contract: identical to oracle/smelter_oracle.c (DESIGN.md section 3).  Compiled with
 // -fmad=false: only explicit fmaf() is fused, every other operation rounds separately, division and
@@ -1530,6 +1531,9 @@ int launch_output(const OutputJob &job, Stream s) {
 
 // gpu-video's transcoder resize (smr_transcode_resize, NC-10)
 #include "transcode.cuh"
+
+// gpu-video's NV12 -> RGBA converter (smr_video_nv12_to_rgba, NC-11)
+#include "video_convert.cuh"
 
 // ------------------------------------------------------------------------------------------------
 // FramePreProcessor (state/frame_pre_processor.rs): K1..K4 to RGBA8, optional rescale (rgba_rescale.wgsl, blend: None)

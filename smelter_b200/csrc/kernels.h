@@ -304,6 +304,15 @@ struct TranscodeLaunch {          // every rendition of one call: one launch
     TranscodeOut out[kTranscodeMaxOutputs];
 };
 
+// gpu-video's NV12 -> RGBA converter (WgpuNv12ToRgbaConverter, NC-11): one NV12 crop to one RGBA8 target of any size
+struct VideoConvertJob {
+    Tex src;                      // TEX_NV12, even sides, origin (0, 0); luma and uv planes 2-byte aligned
+    uint8_t *out;                 // out_h rows of out_pitch bytes, 4-byte aligned
+    int32_t out_pitch;
+    int32_t out_w, out_h;
+};
+constexpr int kVideoConvertTileX = 32, kVideoConvertTileY = 8;   // threads per block
+
 // host tables pushed once per device (numeric contract NC-1/3/4)
 void upload_tables(const float *u8n, const float *srgb_dec, const float *srgb_enc_thr);
 // the device tables of node_sample.cuh in this module (c_u8n, c_dec, c_thr, c_yl, c_enc1): addresses and bytes, for the
@@ -348,6 +357,8 @@ int launch_composite(const CompositeJob *jobs_dev, const CompositeJob *jobs_host
 int launch_output(const OutputJob &job, Stream s);
 // every rendition of L in one launch of n_blocks blocks (the last rendition's tile_begin + its tiles)
 int launch_transcode(const TranscodeLaunch &L, int n_blocks, Stream s);
+// k_video_nv12_to_rgba: a thread per 2 x 2 pixel quad when the target has the source's size, a thread per pixel otherwise
+int launch_video_nv12_to_rgba(const VideoConvertJob &J, Stream s);
 int launch_fill_yuv(uint8_t *p0, uint8_t *p1, uint8_t *p2, int pitch0, int pitch1, int pitch2, int w, int h,
                     int out_format, uint8_t y, uint8_t u, uint8_t v, Stream s);
 const char *last_launch_error();

@@ -87,12 +87,16 @@ __device__ __forceinline__ float filter_u8(int t00, int t10, int t01, int t11, f
     return div255((float)n, 1.0f / 65536.0f);
 }
 
-__device__ __forceinline__ float sample_plane(const Tables &T, const uint8_t *p, int pitch, int stride, int ch,
-                                              const LinTap &ax, const LinTap &ay) {
+// channel ch of a UNORM8 plane of `stride`-byte texels, NC-6u at the taps (ax, ay)
+__device__ __forceinline__ float sample_u8(const uint8_t *p, int pitch, int stride, int ch, const LinTap &ax, const LinTap &ay) {
     const uint8_t *r0 = p + (size_t)ay.i0 * pitch, *r1 = p + (size_t)ay.i1 * pitch;
     const int t00 = __ldg(r0 + ax.i0 * stride + ch), t10 = __ldg(r0 + ax.i1 * stride + ch);
     const int t01 = __ldg(r1 + ax.i0 * stride + ch), t11 = __ldg(r1 + ax.i1 * stride + ch);
     return filter_u8(t00, t10, t01, t11, ax.f, ay.f);
+}
+__device__ __forceinline__ float sample_plane(const Tables &T, const uint8_t *p, int pitch, int stride, int ch,
+                                              const LinTap &ax, const LinTap &ay) {
+    return sample_u8(p, pitch, stride, ch, ax, ay);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -234,10 +238,23 @@ __device__ __forceinline__ bool yuv_quad_ok(const Tex &s, int x, int y) {
     return (s.kind == TEX_NV12 || s.kind == TEX_YUV420) && (((s.width | s.height | x | y) & 1) == 0) && x >= 2 &&
            x + 3 <= s.width - 1 && y >= 2 && y + 3 <= s.height - 1;
 }
+// The chroma of the aligned 2x2 pixel quad over chroma texel (cx, cy) of an even-sized 4:2:0 texture at the pixel centres:
+// NC-6's .25 / .75 taps, in exact integers, with texels packed u in bits 0..15 and v in bits 16..31 so that both channels
+// share every integer multiply-add (max 4080 < 65536).  quad_chroma_row: texels a, b, d of columns cx - 1, cx, cx + 1 of
+// one chroma row -> its horizontal terms for the quad's even and odd pixel; quad_chroma16: the terms of rows cy - 1 .. cy + 1
+// -> 16 x the interpolated chroma of pixels (0,0), (1,0), (0,1), (1,1).
+__device__ __forceinline__ void quad_chroma_row(unsigned a, unsigned b, unsigned d, unsigned &he, unsigned &ho) {
+    he = a + 3u * b;   // even pixel: taps (cx-1, cx), weights (1/4, 3/4)
+    ho = 3u * b + d;   // odd pixel:  taps (cx, cx+1), weights (3/4, 1/4)
+}
+__device__ __forceinline__ void quad_chroma16(const unsigned he[3], const unsigned ho[3], unsigned &n00, unsigned &n10,
+                                              unsigned &n01, unsigned &n11) {
+    // even row: chroma rows (cy-1, cy) weights (1/4, 3/4) ; odd row: (cy, cy+1) weights (3/4, 1/4)
+    n00 = he[0] + 3u * he[1]; n10 = ho[0] + 3u * ho[1]; n01 = 3u * he[1] + he[2]; n11 = 3u * ho[1] + ho[2];
+}
 __device__ __forceinline__ void yuv_quad(const Tables &T, const Tex &s, int x, int y, uchar4 &p00, uchar4 &p10,
                                          uchar4 &p01, uchar4 &p11) {
     const int cx = x >> 1, cy = y >> 1;
-    // u in bits 0..15, v in bits 16..31: both channels share every integer multiply-add (max 4080 < 65536)
     unsigned he[3], ho[3];
 #pragma unroll
     for (int i = 0; i < 3; i++) {
@@ -250,13 +267,12 @@ __device__ __forceinline__ void yuv_quad(const Tables &T, const Tex &s, int x, i
             const uint8_t *ru = s.p1 + (size_t)(cy - 1 + i) * s.pitch1 + cx, *rv = s.p2 + (size_t)(cy - 1 + i) * s.pitch2 + cx;
             a = __ldg(ru - 1) | (__ldg(rv - 1) << 16); b = __ldg(ru) | (__ldg(rv) << 16); d = __ldg(ru + 1) | (__ldg(rv + 1) << 16);
         }
-        he[i] = a + 3u * b;   // even pixel: taps (cx-1, cx), weights (1/4, 3/4)
-        ho[i] = 3u * b + d;   // odd pixel:  taps (cx, cx+1), weights (3/4, 1/4)
+        quad_chroma_row(a, b, d, he[i], ho[i]);
     }
     const uchar2 y0 = __ldg(reinterpret_cast<const uchar2 *>(s.p0 + (size_t)y * s.pitch0 + x));
     const uchar2 y1 = __ldg(reinterpret_cast<const uchar2 *>(s.p0 + (size_t)(y + 1) * s.pitch0 + x));
-    // even row: chroma rows (cy-1, cy) weights (1/4, 3/4) ; odd row: (cy, cy+1) weights (3/4, 1/4)
-    const unsigned n00 = he[0] + 3u * he[1], n10 = ho[0] + 3u * ho[1], n01 = 3u * he[1] + he[2], n11 = 3u * ho[1] + ho[2];
+    unsigned n00, n10, n01, n11;
+    quad_chroma16(he, ho, n00, n10, n01, n11);
     p00 = yuv_to_rgba8(T.u8n[y0.x], div255((float)(n00 & 0xffffu), 0.0625f), div255((float)(n00 >> 16), 0.0625f), s.full_range);
     p10 = yuv_to_rgba8(T.u8n[y0.y], div255((float)(n10 & 0xffffu), 0.0625f), div255((float)(n10 >> 16), 0.0625f), s.full_range);
     p01 = yuv_to_rgba8(T.u8n[y1.x], div255((float)(n01 & 0xffffu), 0.0625f), div255((float)(n01 >> 16), 0.0625f), s.full_range);

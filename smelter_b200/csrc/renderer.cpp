@@ -406,6 +406,10 @@ class Renderer {
     smr_status preprocess_frame(const smr_input_frame *f, uint32_t ow, uint32_t oh, void *rgba, uint32_t pitch, int32_t mem_kind,
                                 bool premultiply = false);
     smr_status transcode_resize(const smr_input_frame *src, const smr_rendition *out, uint32_t n);
+    smr_status video_nv12_to_rgba(const smr_video_color &converter, const smr_input_frame *src, const smr_video_color &frame,
+                                  uint32_t ow, uint32_t oh, void *rgba, uint32_t pitch, int32_t mem_kind);
+    smr_status video_rgba_to_nv12(const smr_video_color &converter, const smr_input_frame *src, uint32_t ow, uint32_t oh,
+                                  void *const planes[2], const uint32_t pitch[2], int32_t mem_kind);
     smr_status render_text(uint32_t w, uint32_t h, smr_rgba bg, const smr_glyph *glyphs, uint32_t n, const smr_atlas *mask,
                            const smr_atlas *color, int32_t color_mode, void *rgba, uint32_t pitch, int32_t mem_kind);
     smr_status debug_set_inputs(uint64_t pts, const smr_input_frame *in, uint32_t n_in);
@@ -726,7 +730,12 @@ class Renderer {
     std::map<std::pair<uint32_t, uint32_t>, TapTable> transcode_taps_;
     uint64_t transcode_calls_ = 0;
     const dev::TranscodeTap *transcode_table(uint32_t in_len, uint32_t out_len);
-    cudaEvent_t transcode_ev_[2] = {};   // profiling: around the k_transcode launch
+    smr_status video_converter_ok(const smr_video_color &c);
+    // profiling of the one kernel of a blocking call (smr_transcode_resize, the video converters): call_prof(0) before the
+    // launch and call_prof(1) after it record events on stream_; call_prof_fold adds the time once the stream has drained
+    cudaEvent_t call_ev_[2] = {};
+    smr_status call_prof(int i);
+    smr_status call_prof_fold(int kernel_class);
     // optional per-kernel-class device timing (cudaEvents on the launching stream)
     void prof_mark(int kernel_class);
     bool profiling_ = false;
@@ -768,7 +777,7 @@ Renderer::~Renderer() {
         if (comm_done_) cudaEventDestroy(comm_done_);
         if (tick_start_) cudaEventDestroy(tick_start_);
         if (web_ev_) cudaEventDestroy(web_ev_);
-        for (cudaEvent_t e : transcode_ev_) if (e) cudaEventDestroy(e);
+        for (cudaEvent_t e : call_ev_) if (e) cudaEventDestroy(e);
         for (int i = 0; i < kTicksInFlight; i++) { if (h2d_done_[i]) cudaEventDestroy(h2d_done_[i]); if (tick_done_[i]) cudaEventDestroy(tick_done_[i]); }
         if (nccl_comm_) { g_nccl.CommDestroy(nccl_comm_); nccl_comm_ = nullptr; }
         for (auto &kv : weights_) {
@@ -2135,14 +2144,10 @@ smr_status Renderer::transcode_resize(const smr_input_frame *src, const smr_rend
         J.tile_begin = blocks;
         blocks += J.tiles_x * (int)((o.height / 2 + dev::kTranscodeTileY - 1) / dev::kTranscodeTileY);
     }
-    if (profiling_ && !transcode_ev_[0]) {
-        CUDA_OK(cudaEventCreate(&transcode_ev_[0]));
-        CUDA_OK(cudaEventCreate(&transcode_ev_[1]));
-    }
-    if (profiling_) CUDA_OK(cudaEventRecord(transcode_ev_[0], stream_));
+    if (smr_status st = call_prof(0); st != SMR_OK) return st;
     if (dev::launch_transcode(L, blocks, stream_) < 0) { set_error(dev::last_launch_error()); return SMR_ERR_CUDA; }
     stats_.kernel_launches++;
-    if (profiling_) CUDA_OK(cudaEventRecord(transcode_ev_[1], stream_));
+    if (smr_status st = call_prof(1); st != SMR_OK) return st;
     for (uint32_t i = 0; i < n; i++) {
         const smr_rendition &o = out[i];
         if (o.mem_kind == SMR_MEM_DEVICE) continue;
@@ -2154,13 +2159,134 @@ smr_status Renderer::transcode_resize(const smr_input_frame *src, const smr_rend
         stats_.d2h_bytes += (size_t)o.width * o.height * 3 / 2;
     }
     CUDA_OK(cudaStreamSynchronize(stream_));
-    if (profiling_) {
-        float ms = 0.0f;
-        CUDA_OK(cudaEventElapsedTime(&ms, transcode_ev_[0], transcode_ev_[1]));
-        prof_.total_ms[SMR_KERNEL_TRANSCODE] += ms;
-        prof_.launches[SMR_KERNEL_TRANSCODE] += 1;
+    return call_prof_fold(SMR_KERNEL_TRANSCODE);
+}
+
+smr_status Renderer::call_prof(int i) {
+    if (!profiling_) return SMR_OK;
+    if (!call_ev_[0]) {
+        CUDA_OK(cudaEventCreate(&call_ev_[0]));
+        CUDA_OK(cudaEventCreate(&call_ev_[1]));
+    }
+    CUDA_OK(cudaEventRecord(call_ev_[i], stream_));
+    return SMR_OK;
+}
+
+smr_status Renderer::call_prof_fold(int kernel_class) {
+    if (!profiling_) return SMR_OK;
+    float ms = 0.0f;
+    CUDA_OK(cudaEventElapsedTime(&ms, call_ev_[0], call_ev_[1]));
+    prof_.total_ms[kernel_class] += ms;
+    prof_.launches[kernel_class] += 1;
+    return SMR_OK;
+}
+
+// gpu-video's converters (wgpu_helpers/): WgpuConverterParameters as `new` checks them (OnlyLimitedBT709Supported)
+static bool video_color_known(const smr_video_color &c) {
+    return c.color_space >= SMR_COLOR_SPACE_UNSPECIFIED && c.color_space <= SMR_COLOR_SPACE_BT601_PAL &&
+           (c.color_range == SMR_COLOR_RANGE_FULL || c.color_range == SMR_COLOR_RANGE_LIMITED);
+}
+smr_status Renderer::video_converter_ok(const smr_video_color &c) {
+    if (!video_color_known(c)) { set_error("unknown color space or color range"); return SMR_ERR_INVALID_ARGUMENT; }
+    if (c.color_space != SMR_COLOR_SPACE_BT709 || c.color_range != SMR_COLOR_RANGE_LIMITED) {
+        set_error("only limited-range BT.709 converters are supported");
+        return SMR_ERR_UNSUPPORTED;
     }
     return SMR_OK;
+}
+
+// WgpuNv12ToRgbaConverter: create_input_bind_group + convert (gpu-video wgpu_helpers/nv12_to_rgba.rs)
+smr_status Renderer::video_nv12_to_rgba(const smr_video_color &converter, const smr_input_frame *src, const smr_video_color &frame,
+                                        uint32_t ow, uint32_t oh, void *rgba, uint32_t pitch, int32_t mem_kind) {
+    if (!src || !rgba) return SMR_ERR_INVALID_ARGUMENT;
+    std::lock_guard<std::mutex> g(mu_);
+    if (smr_status st = video_converter_ok(converter); st != SMR_OK) return st;
+    if (!video_color_known(frame)) { set_error("unknown frame color space or color range"); return SMR_ERR_INVALID_ARGUMENT; }
+    if ((frame.color_space != SMR_COLOR_SPACE_UNSPECIFIED && frame.color_space != converter.color_space) ||
+        frame.color_range != converter.color_range) {
+        set_error("incompatible frame: its color space and range do not match the converter's");
+        return SMR_ERR_INVALID_ARGUMENT;
+    }
+    if ((ow == 0) != (oh == 0) || ow > kMaxFrameDim || oh > kMaxFrameDim) {
+        set_error("output resolution out of range");
+        return SMR_ERR_INVALID_ARGUMENT;
+    }
+    if (mem_kind != SMR_MEM_HOST && mem_kind != SMR_MEM_DEVICE) { set_error("unknown mem_kind"); return SMR_ERR_INVALID_ARGUMENT; }
+    FrameView v;
+    if (smr_status st = read_frame(*src, v); st != SMR_OK) return st;
+    if (src->format != SMR_FRAME_NV12) { set_error("the NV12 to RGBA converter takes NV12 frames"); return SMR_ERR_UNSUPPORTED; }
+    if ((src->width | src->height) & 1) { set_error("NV12 source width and height must be even"); return SMR_ERR_INVALID_ARGUMENT; }
+    if (ow == 0) { ow = src->width; oh = src->height; }
+    const size_t row = (size_t)ow * 4;
+    if (pitch && pitch < row) { set_error("output pitch smaller than a row"); return SMR_ERR_INVALID_ARGUMENT; }
+    if (mem_kind == SMR_MEM_DEVICE && (((uintptr_t)rgba | (pitch ? pitch : row)) & 3)) {
+        set_error("device RGBA8 planes are 4-byte aligned");
+        return SMR_ERR_INVALID_ARGUMENT;
+    }
+    if (host_only_) { set_error("host-only handle (cuda_device = -1) has no device: no CPU fallback"); return SMR_ERR_CUDA; }
+    CUDA_OK(cudaSetDevice(opts_.cuda_device));
+    if (smr_status st = upload_pre_planes(*src, v); st != SMR_OK) return st;
+    dev::VideoConvertJob J = {};
+    J.src = v.tex;
+    J.out_w = (int)ow; J.out_h = (int)oh;
+    smr_status st = write_rgba(rgba, pitch, mem_kind, ow, oh, [&](uint8_t *dst, int dpitch) {
+        J.out = dst; J.out_pitch = dpitch;
+        if (call_prof(0) != SMR_OK) return -1;
+        const int n = dev::launch_video_nv12_to_rgba(J, stream_);
+        return n < 0 || call_prof(1) != SMR_OK ? -1 : n;
+    });
+    return st != SMR_OK ? st : call_prof_fold(SMR_KERNEL_VIDEO_CONVERT);
+}
+
+// WgpuRgbaToNv12Converter::convert (gpu-video wgpu_helpers/rgba_to_nv12.rs): rgba_to_nv12.wgsl is K11, so the kernel is
+// k_output's NV12 target
+smr_status Renderer::video_rgba_to_nv12(const smr_video_color &converter, const smr_input_frame *src, uint32_t ow, uint32_t oh,
+                                        void *const planes[2], const uint32_t pitch[2], int32_t mem_kind) {
+    if (!src || !planes) return SMR_ERR_INVALID_ARGUMENT;
+    std::lock_guard<std::mutex> g(mu_);
+    if (smr_status st = video_converter_ok(converter); st != SMR_OK) return st;
+    if (ow == 0 || oh == 0 || ow > kMaxFrameDim || oh > kMaxFrameDim || ((ow | oh) & 1)) {
+        set_error("NV12 target width and height must be even and in 2 .. 16384");
+        return SMR_ERR_INVALID_ARGUMENT;
+    }
+    if (mem_kind != SMR_MEM_HOST && mem_kind != SMR_MEM_DEVICE) { set_error("unknown mem_kind"); return SMR_ERR_INVALID_ARGUMENT; }
+    uint32_t tp[2];
+    for (int p = 0; p < 2; p++) {   // an NV12 row is `ow` bytes in both planes
+        tp[p] = pitch && pitch[p] ? pitch[p] : ow;
+        if (!planes[p]) { set_error("target plane pointer is null"); return SMR_ERR_INVALID_ARGUMENT; }
+        if (tp[p] < ow) { set_error("target pitch is smaller than a row"); return SMR_ERR_INVALID_ARGUMENT; }
+    }
+    FrameView v;
+    if (smr_status st = read_frame(*src, v); st != SMR_OK) return st;
+    if (src->format != SMR_FRAME_RGBA8) { set_error("the RGBA to NV12 converter takes RGBA8 frames"); return SMR_ERR_UNSUPPORTED; }
+    if (host_only_) { set_error("host-only handle (cuda_device = -1) has no device: no CPU fallback"); return SMR_ERR_CUDA; }
+    CUDA_OK(cudaSetDevice(opts_.cuda_device));
+    if (smr_status st = upload_pre_planes(*src, v); st != SMR_OK) return st;
+    dev::OutputJob J = {};
+    J.src = v.tex;
+    J.out_w = (int)ow; J.out_h = (int)oh;
+    J.out_format = SMR_OUT_NV12;
+    const size_t luma = (size_t)ow * oh;
+    if (mem_kind == SMR_MEM_DEVICE) {
+        J.out0 = (uint8_t *)planes[0]; J.out1 = (uint8_t *)planes[1];
+        J.out_pitch0 = (int)tp[0]; J.out_pitch1 = (int)tp[1];
+    } else {   // written into pre_out_, packed, and copied back after the launch
+        if (luma * 3 / 2 > pre_out_.cap) CUDA_OK(cudaStreamSynchronize(stream_));
+        CUDA_OK(pre_out_.ensure(luma * 3 / 2));
+        J.out0 = pre_out_.p; J.out1 = pre_out_.p + luma;
+        J.out_pitch0 = J.out_pitch1 = (int)ow;
+    }
+    if (smr_status st = call_prof(0); st != SMR_OK) return st;
+    if (dev::launch_output(J, stream_) < 0) { set_error(dev::last_launch_error()); return SMR_ERR_CUDA; }
+    stats_.kernel_launches++;
+    if (smr_status st = call_prof(1); st != SMR_OK) return st;
+    if (mem_kind != SMR_MEM_DEVICE) {
+        CUDA_OK(cudaMemcpy2DAsync(planes[0], tp[0], J.out0, J.out_pitch0, ow, oh, cudaMemcpyDeviceToHost, stream_));
+        CUDA_OK(cudaMemcpy2DAsync(planes[1], tp[1], J.out1, J.out_pitch1, ow, oh / 2, cudaMemcpyDeviceToHost, stream_));
+        stats_.d2h_bytes += luma * 3 / 2;
+    }
+    CUDA_OK(cudaStreamSynchronize(stream_));
+    return call_prof_fold(SMR_KERNEL_OUTPUT);
 }
 
 // FramePreProcessor::process_to_bytes / process_to_texture (state/frame_pre_processor.rs:60-100)
@@ -3695,6 +3821,14 @@ smr_status smr_premultiply_rgba8(smr_renderer *r, const smr_input_frame *f, void
 }
 smr_status smr_transcode_resize(smr_renderer *r, const smr_input_frame *src, const smr_rendition *out, uint32_t n) {
     SMR_GUARD(r->impl.transcode_resize(src, out, n))
+}
+smr_status smr_video_nv12_to_rgba(smr_renderer *r, smr_video_color converter, const smr_input_frame *src, smr_video_color frame,
+                                  uint32_t out_width, uint32_t out_height, void *rgba, uint32_t pitch, int32_t mem_kind) {
+    SMR_GUARD(r->impl.video_nv12_to_rgba(converter, src, frame, out_width, out_height, rgba, pitch, mem_kind))
+}
+smr_status smr_video_rgba_to_nv12(smr_renderer *r, smr_video_color converter, const smr_input_frame *src, uint32_t out_width,
+                                  uint32_t out_height, void *const planes[2], const uint32_t pitch[2], int32_t mem_kind) {
+    SMR_GUARD(r->impl.video_rgba_to_nv12(converter, src, out_width, out_height, planes, pitch, mem_kind))
 }
 smr_status smr_render_text(smr_renderer *r, uint32_t w, uint32_t h, smr_rgba bg, const smr_glyph *glyphs, uint32_t n,
                            const smr_atlas *mask, const smr_atlas *color, int32_t color_mode, void *rgba, uint32_t pitch, int32_t mem_kind) {

@@ -140,6 +140,20 @@ class ScalingAlgorithm:
     Lanczos3 = F.SCALE_LANCZOS3
 
 
+class ColorSpace:
+    """gpu-video's ColorSpace (device.rs), a decoded frame's or a converter's colour space"""
+    Unspecified = F.COLOR_SPACE_UNSPECIFIED
+    BT709 = F.COLOR_SPACE_BT709
+    BT601Ntsc = F.COLOR_SPACE_BT601_NTSC
+    BT601Pal = F.COLOR_SPACE_BT601_PAL
+
+
+class ColorRange:
+    """gpu-video's ColorRange (device.rs)"""
+    Full = F.COLOR_RANGE_FULL
+    Limited = F.COLOR_RANGE_LIMITED
+
+
 class FramePreProcessor:
     """smelter_render::FramePreProcessor (state/frame_pre_processor.rs:33-116) over a Renderer handle."""
 
@@ -821,6 +835,35 @@ class Renderer:
             outs[i].planes[0], outs[i].planes[1] = y.ctypes.data, uv.ctypes.data
         self._check(self._lib.smr_transcode_resize(self._h, arr, outs, len(renditions)), RenderSceneError)
         return planes
+
+    def video_nv12_to_rgba(self, frame: Frame, resolution: Optional[Resolution] = None,
+                           converter=(ColorSpace.BT709, ColorRange.Limited),
+                           frame_color=(ColorSpace.Unspecified, ColorRange.Limited)) -> np.ndarray:
+        """gpu-video's WgpuNv12ToRgbaConverter: one NV12 frame (its crop, origin (0, 0)) -> Rgba8Unorm bytes, bilinearly
+        rescaled to `resolution` when it is given.  `converter` is the converter's (ColorSpace, ColorRange), `frame_color`
+        the decoded frame's metadata.  Returns an (h, w, 4) uint8 array."""
+        keep = []
+        arr = self._input_frames(FrameSet(frames={"_": frame}), keep)
+        ow, oh = (resolution.width, resolution.height) if resolution else (0, 0)
+        w, h = (ow, oh) if resolution else (frame.resolution.width, frame.resolution.height)
+        out = np.empty((h, w, 4), np.uint8)
+        self._check(self._lib.smr_video_nv12_to_rgba(self._h, F.VideoColor(*converter), arr, F.VideoColor(*frame_color), ow, oh,
+                                                     out.ctypes.data, 0, F.MEM_HOST), RenderSceneError)
+        return out
+
+    def video_rgba_to_nv12(self, frame: Frame, resolution: Optional[Resolution] = None,
+                           converter=(ColorSpace.BT709, ColorRange.Limited)) -> Tuple[np.ndarray, np.ndarray]:
+        """gpu-video's WgpuRgbaToNv12Converter: one RGBA8 frame (raw bytes, alpha unused) -> NV12 planes, bilinearly
+        rescaled to `resolution` (even sides; default: the frame's size).  Returns the (h, w) Y plane and the
+        (h / 2, w / 2, 2) UV plane."""
+        keep = []
+        arr = self._input_frames(FrameSet(frames={"_": frame}), keep)
+        w, h = (resolution.width, resolution.height) if resolution else (frame.resolution.width, frame.resolution.height)
+        y, uv = np.empty((h, w), np.uint8), np.empty((h // 2, w // 2, 2), np.uint8)
+        planes = (C.c_void_p * 2)(y.ctypes.data, uv.ctypes.data)
+        self._check(self._lib.smr_video_rgba_to_nv12(self._h, F.VideoColor(*converter), arr, w, h, planes, None, F.MEM_HOST),
+                    RenderSceneError)
+        return y, uv
 
     def set_layouts(self, output_id: str, resolution: Resolution, output_format: int, root: Tuple[int, int],
                     child_input_ids: List[str], layouts):
