@@ -1649,12 +1649,6 @@ __global__ void __launch_bounds__(256) k_text(const TextJob *__restrict__ jobs, 
     if (px < J.dst.width && py < J.dst.height) reinterpret_cast<uchar4 *>(J.dst.out + (size_t)py * J.dst.out_pitch)[px] = d;
 }
 
-int launch_text(const TextJob *jobs_dev, const int32_t *tile_begin_dev, int n_jobs, int n_tiles, Stream s) {
-    if (n_jobs <= 0 || n_tiles <= 0) return 0;
-    k_text<<<n_tiles, dim3(32, 8), 0, (cudaStream_t)s>>>(jobs_dev, tile_begin_dev, n_jobs);
-    return check_launch("k_text") ? 1 : -1;
-}
-
 // ------------------------------------------------------------------------------------------------
 // Image node texture (transformations/image.rs:178-187, add_premultiplied_alpha.wgsl): a full-target quad samples the
 // asset frame (straight alpha) with the linear / clamp-to-edge sampler through the mode's source view, premultiplies and
@@ -1693,12 +1687,6 @@ __global__ void __launch_bounds__(256) k_image(const ImageJob *__restrict__ jobs
     reinterpret_cast<uchar4 *>(J.dst.out + (size_t)y * J.dst.out_pitch)[x] = o;
 }
 
-int launch_image(const ImageJob *jobs_dev, const int32_t *tile_begin_dev, int n_jobs, int n_tiles, Stream s) {
-    if (n_jobs <= 0 || n_tiles <= 0) return 0;
-    k_image<<<n_tiles, dim3(32, 8), 0, (cudaStream_t)s>>>(jobs_dev, tile_begin_dev, n_jobs);
-    return check_launch("k_image") ? 1 : -1;
-}
-
 // ------------------------------------------------------------------------------------------------
 // Web view node texture (web_renderer/shader.rs:53-114, render_website.wgsl): one render pass per plane, the first one
 // clearing to transparent.  A pass leaves the pixels its quad does not cover as they are and blends the bare sample into
@@ -1727,17 +1715,17 @@ __global__ void __launch_bounds__(256) k_web(const WebJob *__restrict__ jobs, co
     reinterpret_cast<uchar4 *>(J.dst.out + (size_t)y * J.dst.out_pitch)[x] = o;
 }
 
-int launch_web(const WebJob *jobs_dev, const int32_t *tile_begin_dev, int n_jobs, int n_tiles, Stream s) {
-    if (n_jobs <= 0 || n_tiles <= 0) return 0;
-    k_web<<<n_tiles, dim3(32, 8), 0, (cudaStream_t)s>>>(jobs_dev, tile_begin_dev, n_jobs);
-    return check_launch("k_web") ? 1 : -1;
+const void *node_kernel(NodeKernel k) {
+    const void *const kernels[] = {(const void *)k_text, (const void *)k_image, (const void *)k_web};
+    return kernels[k];
 }
 
-int launch_shader(const void *kernel, const ShaderJob *jobs_dev, const int32_t *tile_begin_dev, int n_jobs, int n_tiles, Stream s) {
+int launch_tile_jobs(const void *kernel, const void *jobs_dev, const int32_t *tile_begin_dev, int n_jobs, int n_tiles,
+                     const char *name, Stream s) {
     if (n_jobs <= 0 || n_tiles <= 0) return 0;
     void *args[] = {(void *)&jobs_dev, (void *)&tile_begin_dev, (void *)&n_jobs};
     cudaLaunchKernel(kernel, dim3(n_tiles), dim3(32, 8), args, 0, (cudaStream_t)s);
-    return check_launch("smr_shader_main") ? 1 : -1;
+    return check_launch(name) ? 1 : -1;
 }
 
 bool table_symbols(const void *ptr[5], size_t bytes[5]) {

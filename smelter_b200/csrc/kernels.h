@@ -336,18 +336,14 @@ inline int fused_source_class(int tex_kind) {
 }
 // FramePreProcessor: node texture of `src` (rescale = 0) or its linear-filtered rescale to out_w x out_h
 int launch_preprocess(const Tex &src, int mode, int rescale, uint8_t *out, int out_pitch, int out_w, int out_h, Stream s);
-// text node textures: clear + glyph quads alpha-blended in list order, every job of jobs_dev in one launch.  Job i owns the
-// 32 x 8 tiles [tile_begin_dev[i], tile_begin_dev[i + 1]) of the grid (node_tiles of each job, prefix sums); n_tiles =
-// tile_begin[n_jobs]
+// node textures: every job of jobs_dev in one launch of a 32 x 8 tile-job kernel, node_kernel's or a shader module's
+// smr_shader_main (a cudaKernel_t, ShaderJob).  Job i owns the 32 x 8 tiles [tile_begin_dev[i], tile_begin_dev[i + 1]) of the
+// grid (node_tiles of each job, prefix sums); n_tiles = tile_begin[n_jobs].  `name` names the kernel in a launch error
 inline int node_tiles(int width, int height) { return ((width + 31) / 32) * ((height + 7) / 8); }
-int launch_text(const TextJob *jobs_dev, const int32_t *tile_begin_dev, int n_jobs, int n_tiles, Stream s);
-// image node textures: the frame of each job sampled, premultiplied and stored; jobs and tiles as for launch_text
-int launch_image(const ImageJob *jobs_dev, const int32_t *tile_begin_dev, int n_jobs, int n_tiles, Stream s);
-// web view node textures: each job's planes drawn over a transparent clear; jobs and tiles as for launch_text
-int launch_web(const WebJob *jobs_dev, const int32_t *tile_begin_dev, int n_jobs, int n_tiles, Stream s);
-// shader node textures of one shader module: `kernel` is its smr_shader_main (a cudaKernel_t); jobs and tiles as for
-// launch_text
-int launch_shader(const void *kernel, const ShaderJob *jobs_dev, const int32_t *tile_begin_dev, int n_jobs, int n_tiles, Stream s);
+int launch_tile_jobs(const void *kernel, const void *jobs_dev, const int32_t *tile_begin_dev, int n_jobs, int n_tiles,
+                     const char *name, Stream s);
+enum NodeKernel { NODE_TEXT, NODE_IMAGE, NODE_WEB };   // k_text (TextJob), k_image (ImageJob), k_web (WebJob)
+const void *node_kernel(NodeKernel k);
 // full_range: fused_launch_range of every job of the launch
 int launch_resample_fused(const FusedKernel &k, int src, int full_range, const FusedJob *jobs_dev, const FusedPiece *pieces_dev,
                           const int *piece_begin_dev, int nblocks, Stream s);

@@ -442,6 +442,7 @@ class Renderer {
     struct NodeTexture {
         Input in;
         std::shared_ptr<void> mem;
+        size_t job_off = 0;     // its job in the parameter arena, when a tick draws it
     };
     // A Text component (TextRendererNode, transformations/text_renderer.rs): width x height (1 x 1 for 0 x 0), its glyphs
     // after the texture in `mem`
@@ -476,7 +477,6 @@ class Renderer {
         ShaderParams params;
         Output *owner = nullptr;   // the output whose nodes its children are (set when a tick plans it)
         dev::ShaderJob job = {};   // draws `in.tex`; its textures and parameter bytes are this tick's, in the parameter arena
-        std::vector<dev::Tex> tex;
         size_t tex_off = 0, params_off = SIZE_MAX;
     };
     struct Output {
@@ -532,18 +532,27 @@ class Renderer {
         for (size_t i = 0; i < recs.size(); i++) memcpy(param_host_.data() + off + i * sizeof(Dev), &(recs[i].*dev), sizeof(Dev));
         return off;
     }
-    // the jobs of the node textures one launch draws, and the prefix table of their 32 x 8 tile counts (launch_text,
-    // launch_image, launch_web, launch_shader)
-    struct TileJobs { size_t jobs_off, begin_off; int n_tiles; };
-    template <class Node, class Job> TileJobs param_put_tile_jobs(const std::vector<Node *> &nodes, Job Node::*job) {
-        std::vector<int32_t> begin(1, 0);
-        const size_t jobs_off = param_alloc(sizeof(Job) * nodes.size());
-        for (size_t i = 0; i < nodes.size(); i++) {
-            const Job &j = nodes[i]->*job;
-            memcpy(param_host_.data() + jobs_off + i * sizeof(Job), &j, sizeof(Job));
-            begin.push_back(begin.back() + dev::node_tiles(j.dst.width, j.dst.height));
+    // One launch of `kernel` after phase `phase` (-1: before the conversions) that draws the nodes of `nodes` that `in`
+    // selects, in their order: their jobs and the prefix table of their 32 x 8 tile counts go to the parameter arena
+    template <class Node, class Job, class In>
+    void add_node_launch(const void *kernel, const char *name, int prof_class, int phase, const std::vector<Node *> &nodes,
+                         Job Node::*job, In in) {
+        NodeLaunch l{kernel, name, prof_class, phase, (int)std::count_if(nodes.begin(), nodes.end(), in)};
+        if (l.n_jobs == 0) return;
+        l.jobs_off = param_alloc(sizeof(Job) * l.n_jobs);
+        l.begin_off = param_alloc(sizeof(int32_t) * (l.n_jobs + 1));
+        int32_t *begin = reinterpret_cast<int32_t *>(param_host_.data() + l.begin_off);
+        int k = 0;
+        for (Node *n : nodes) {
+            if (!in(n)) continue;
+            const Job &j = n->*job;
+            n->job_off = l.jobs_off + sizeof(Job) * k;
+            memcpy(param_host_.data() + n->job_off, &j, sizeof(Job));
+            begin[k++] = l.n_tiles;
+            l.n_tiles += dev::node_tiles(j.dst.width, j.dst.height);
         }
-        return {jobs_off, param_put(begin.data(), sizeof(int32_t) * begin.size()), begin.back()};
+        begin[k] = l.n_tiles;
+        plan_.node_launches.push_back(l);
     }
     size_t frame_alloc(size_t bytes) {
         size_t off = (frame_used_ + 511) & ~(size_t)511;
@@ -621,6 +630,21 @@ class Renderer {
         std::vector<uint32_t> list;
         size_t list_off = SIZE_MAX;       // param-arena offset of `list`
     };
+    struct FusedKey {           // the fused jobs one launch runs: same kernel, source class and launch range
+        dev::FusedKernel kernel; int src, range;
+        bool operator==(const FusedKey &o) const { return kernel == o.kernel && src == o.src && range == o.range; }
+    };
+    struct FusedLaunch { FusedKey key; size_t pieces_off, begin_off; int nblocks; };
+    // One launch of a node-texture kernel (launch_tile_jobs): launch_tick enqueues it after phase `phase`'s composite (-1:
+    // before the conversions)
+    struct NodeLaunch {
+        const void *kernel;
+        const char *name;                 // in a launch error
+        int prof_class, phase;
+        int n_jobs;                       // the nodes it draws, one job each
+        size_t jobs_off, begin_off;       // in the parameter arena: their jobs, the prefix table of their tiles
+        int n_tiles;
+    };
     struct PendingCopy { void *dst; size_t dpitch; const void *src; size_t spitch; size_t width, height; };
     struct Fill { uint8_t *p[3]; int pitch[3]; int w, h, fmt; uint8_t yuv[3]; };
     struct TickPlan {
@@ -638,17 +662,25 @@ class Renderer {
         std::vector<ImageNode *> images;      // image nodes drawn by this tick (likewise)
         std::vector<WebNode *> webs;          // web nodes drawn by this tick (after every node they may read, by depth)
         std::vector<ShaderNode *> shaders;    // shader nodes drawn by this tick (likewise)
-        // the tick's phases: one per depth of its layout, shader and web nodes below the roots, then the roots'.  A phase's
-        // generic resample passes and composite jobs are those from its mark up to the next one (planned in phase order)
+        // the tick's phases: one per depth of its layout, shader and web nodes below the roots, then the roots'.  Phase p's
+        // generic resample passes and composite jobs are those from phases[p] up to phases[p + 1] (the last entry: the end)
         struct Phase { size_t stages[3], composites; };
         std::vector<Phase> phases;
         std::map<std::tuple<int, uint32_t, uint32_t, uint32_t, uint32_t, int, int>, int> resample_cache;
+        std::vector<FusedLaunch> fused_launches;
+        std::vector<NodeLaunch> node_launches;   // the text, image, web and shader launches (pack_params)
+        size_t stage_off[3], weights_off, fused_off, composites_off;   // the packed job arrays in the parameter arena
+        uint64_t launches, direct_tiles;
+        bool nodes_enqueued;                  // the node launches before the conversions
         void clear() {   // keeps the vectors' capacity
             tex.clear();
             for (auto &s : stages) s.clear();
             fused.clear(); tmaps.clear(); weight_jobs.clear(); convert_jobs.clear();
             composites.clear(); outputs.clear(); fills.clear(); d2h.clear(); texts.clear(); images.clear(); webs.clear(); shaders.clear(); phases.clear();
             resample_cache.clear();
+            fused_launches.clear(); node_launches.clear();
+            launches = direct_tiles = 0;
+            nodes_enqueued = false;
         }
     } plan_;
     smr_status make_node_texture(int w, int h, bool clear, size_t extra_bytes, NodeTexture &n, dev::NodeTarget &t);
@@ -672,6 +704,14 @@ class Renderer {
     CompositeRec composite_rec(int W, int H, const std::vector<dev::LayerDev> &layers, const std::vector<dev::MaskDev> &masks);
     int composite_texture(CompositeRec pc);
     void plan_tiles(Output &o, CompositeRec &pc, const std::vector<dev::LayerDev> &layers, int W, int H);
+    // the steps of render_begin, in order
+    smr_status begin_tick();
+    smr_status plan_tick(uint64_t pts, const smr_input_frame *in, uint32_t n_in, smr_output_frame *out, uint32_t n_out);
+    smr_status resolve_frame_arena();
+    void plan_fused_launches();
+    smr_status pack_params();
+    smr_status launch_tick();
+    smr_status enqueue_readback(uint32_t n_out);
     std::vector<WeightKey> new_weight_keys_;   // cache entries whose k_weights launch is not enqueued yet
     void rollback_weights();                   // a tick that fails before that launch must not leave them behind
     // TMA kernels of the fused resample: descriptors of the source planes, cached per (pointer, pitch, size, kind)
@@ -2373,7 +2413,8 @@ smr_status Renderer::render_text(uint32_t w, uint32_t h, smr_rgba bg, const smr_
         if (cudaMemcpyAsync(text_job_.p, &J, sizeof(J), cudaMemcpyHostToDevice, stream_) != cudaSuccess ||
             cudaMemcpyAsync(text_job_.p + begin_off, begin, sizeof(begin), cudaMemcpyHostToDevice, stream_) != cudaSuccess)
             return -1;
-        return dev::launch_text((const dev::TextJob *)text_job_.p, (const int32_t *)(text_job_.p + begin_off), 1, begin[1], stream_);
+        return dev::launch_tile_jobs(dev::node_kernel(dev::NODE_TEXT), text_job_.p, (const int32_t *)(text_job_.p + begin_off), 1,
+                                     begin[1], "k_text", stream_);
     });
 }
 
@@ -2874,6 +2915,29 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
     std::lock_guard<std::mutex> g(mu_);
     if (host_only_) { set_error("host-only handle (cuda_device = -1) cannot render: no CPU fallback"); return SMR_ERR_CUDA; }
     CUDA_OK(cudaSetDevice(opts_.cuda_device));
+    if (smr_status st = begin_tick(); st != SMR_OK) return st;
+    // any return from here (a status or an exception) before a launch is enqueued undoes what the tick planned for it: the
+    // new weight-cache entries are dropped, the text and image nodes are left to the next tick
+    struct TickGuard {
+        Renderer &r;
+        ~TickGuard() {
+            if (!r.new_weight_keys_.empty()) r.rollback_weights();   // emptied once the k_weights launch is enqueued
+            if (r.plan_.nodes_enqueued) return;
+            for (TextNode *t : r.plan_.texts) t->rendered = false;
+            for (ImageNode *n : r.plan_.images) n->held = n->held_before;
+        }
+    } guard{*this};
+    smr_status st = plan_tick(pts, in, n_in, out, n_out);
+    if (st == SMR_OK) st = resolve_frame_arena();
+    if (st == SMR_OK) plan_fused_launches();
+    if (st == SMR_OK) st = pack_params();
+    if (st == SMR_OK) st = launch_tick();
+    if (st == SMR_OK) st = enqueue_readback(n_out);
+    return st;
+}
+
+// A new tick: its slot, free for it, an empty plan and empty arenas
+smr_status Renderer::begin_tick() {
     if (profiling_ && !inflight_.empty()) drain();   // per-kernel timing: one tick at a time
     tick_++;
     slot_ = (int)(tick_ % kTicksInFlight);
@@ -2888,21 +2952,11 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
     rollback_weights();   // leftovers of a tick that failed before its weight launch (normally empty)
     plan_.clear();
     param_used_ = 0; frame_used_ = 0;
-    uint64_t launches = 0;
-    cudaStream_t done_on = stream_;   // the stream the tick's last operation goes to
+    return SMR_OK;
+}
 
-    struct WeightGuard {   // any return before the k_weights launch is enqueued drops this tick's new cache entries
-        Renderer *r; bool armed = true;
-        ~WeightGuard() { if (armed) r->rollback_weights(); }
-    } weight_guard{this};
-    struct NodeGuard {     // any return before the text and image launches are enqueued leaves this tick's nodes to the next tick
-        std::vector<TextNode *> &texts; std::vector<ImageNode *> &images; bool armed = true;
-        ~NodeGuard() {
-            if (!armed) return;
-            for (TextNode *t : texts) t->rendered = false;
-            for (ImageNode *n : images) n->held = n->held_before;
-        }
-    } node_guard{plan_.texts, plan_.images};
+// The tick's inputs and its plan, phase by phase; plan_.phases gets each phase's start and the end of the last
+smr_status Renderer::plan_tick(uint64_t pts, const smr_input_frame *in, uint32_t n_in, smr_output_frame *out, uint32_t n_out) {
     smr_status st = select_inputs(pts, in, n_in, [&](Input &I, const smr_input_frame *f) {
         I.node_tex = I.raw_tex = -1;
         return f ? upload_input(I, *f) : SMR_OK;
@@ -2944,7 +2998,12 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
         st = plan_output(*outs[i], out[i], pts);
         if (st != SMR_OK) return st;
     }
+    mark();   // the end of the roots' phase
+    return SMR_OK;
+}
 
+// Orders the tick's kernels after its inputs, sizes the frame arena and resolves the plan's frame-arena addresses
+smr_status Renderer::resolve_frame_arena() {
     // everything already on the stream belongs to earlier ticks: a broadcast issued after this call may overwrite any
     // buffer those ticks read once this event has fired
     CUDA_OK(cudaEventRecord(tick_start_, stream_));
@@ -2953,7 +3012,6 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
         CUDA_OK(cudaStreamWaitEvent(stream_, comm_done_, 0));
         comm_pending_ = false;
     }
-    // ---- resolve frame-arena addresses --------------------------------------------------------
     if (uploaded_) {   // kernels of this tick start after its uploads; earlier ticks keep running meanwhile
         CUDA_OK(cudaEventRecord(h2d_done_[slot_], copy_stream_));
         CUDA_OK(cudaStreamWaitEvent(stream_, h2d_done_[slot_], 0));
@@ -2978,65 +3036,61 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
     }
     for (CompositeRec &c : plan_.composites)
         if (c.out_frame_off != SIZE_MAX) c.job.out0 = fb + c.out_frame_off;
+    return SMR_OK;
+}
 
-    // ---- pack the parameter arena and ship it in one copy -------------------------------------
-    // partition the fused resamples of the tick over a persistent grid, one launch per kernel, source class and launch range
-    struct FusedKey {
-        dev::FusedKernel kernel; int src, range;
-        bool operator==(const FusedKey &o) const { return kernel == o.kernel && src == o.src && range == o.range; }
-    };
+// The tick's fused resamples over a persistent grid, one launch per kernel, source class and launch range; runs before the
+// composites' tile lists are packed, as a job cut at an odd row gives its direct tiles back to its composite
+void Renderer::plan_fused_launches() {
     auto key_of = [](const FusedRec &f) {
         return FusedKey{f.kernel, dev::fused_source_class(f.job.src.kind), dev::fused_launch_range(f.kernel, f.job)};
     };
-    struct FusedLaunch { FusedKey key; size_t pieces_off, begin_off; int nblocks; };
-    std::vector<FusedLaunch> fused_launches;
-    {
-        std::vector<FusedKey> keys;
-        for (const FusedRec &f : plan_.fused)
-            if (std::find(keys.begin(), keys.end(), key_of(f)) == keys.end()) keys.push_back(key_of(f));
-        for (const FusedKey &v : keys) {
-            std::vector<int> idx, widths, heights, cols;
-            dev::FusedShape shape{};
-            for (size_t ji = 0; ji < plan_.fused.size(); ji++) {
-                const FusedRec &f = plan_.fused[ji];
-                if (!(key_of(f) == v)) continue;
-                shape = dev::fused_shape(f.kernel, f.job);
-                idx.push_back((int)ji); widths.push_back(f.job.dst_w); heights.push_back(f.job.dst_h); cols.push_back(shape.strip_cols);
-            }
-            std::vector<dev::FusedPiece> pieces;
-            std::vector<int> begin;
-            partition_fused_rows(idx.data(), widths.data(), heights.data(), (int)idx.size(), sm_count_ * shape.groups_per_sm, pieces,
-                                 begin, dev::kFusedStripCols, cols.data(), shape.row_gran);
-            if (pieces.empty()) continue;
-            // direct tiles: the vertical pass emits K10 / K11 per PAIR of output rows, so a job's pieces must hold whole pairs
-            // (they do whenever every job of the launch has an even height); a job cut at an odd row writes nothing directly
-            for (const dev::FusedPiece &pp : pieces)
-                if (plan_.fused[pp.job].direct_off != SIZE_MAX && ((pp.oy_begin | pp.oy_end) & 1)) {
-                    plan_.fused[pp.job].direct_off = SIZE_MAX;
-                    for (CompositeRec &pc : plan_.composites)
-                        for (size_t t = 0; t < pc.direct_owner.size(); t++)
-                            if (pc.direct_owner[t] == pp.job) {   // back to the composite (cheap interior tiles: at the end of the list)
-                                pc.direct_owner[t] = -1;
-                                pc.list.push_back((uint32_t)(t % (size_t)pc.job.map_w) | ((uint32_t)(t / (size_t)pc.job.map_w) << 16));
-                            }
-                }
-            fused_launches.push_back({v, param_put(pieces.data(), sizeof(dev::FusedPiece) * pieces.size()),
-                                      param_put(begin.data(), sizeof(int) * begin.size()), (int)begin.size() - 1});
+    for (size_t i = 0; i < plan_.fused.size(); i++) {
+        const FusedKey v = key_of(plan_.fused[i]);
+        if (std::any_of(plan_.fused.begin(), plan_.fused.begin() + i, [&](const FusedRec &f) { return key_of(f) == v; })) continue;
+        std::vector<int> idx, widths, heights, cols;
+        dev::FusedShape shape{};
+        for (size_t ji = i; ji < plan_.fused.size(); ji++) {
+            const FusedRec &f = plan_.fused[ji];
+            if (!(key_of(f) == v)) continue;
+            shape = dev::fused_shape(f.kernel, f.job);
+            idx.push_back((int)ji); widths.push_back(f.job.dst_w); heights.push_back(f.job.dst_h); cols.push_back(shape.strip_cols);
         }
+        std::vector<dev::FusedPiece> pieces;
+        std::vector<int> begin;
+        partition_fused_rows(idx.data(), widths.data(), heights.data(), (int)idx.size(), sm_count_ * shape.groups_per_sm, pieces,
+                             begin, dev::kFusedStripCols, cols.data(), shape.row_gran);
+        if (pieces.empty()) continue;
+        // direct tiles: the vertical pass emits K10 / K11 per PAIR of output rows, so a job's pieces must hold whole pairs
+        // (they do whenever every job of the launch has an even height); a job cut at an odd row writes nothing directly
+        for (const dev::FusedPiece &pp : pieces)
+            if (plan_.fused[pp.job].direct_off != SIZE_MAX && ((pp.oy_begin | pp.oy_end) & 1)) {
+                plan_.fused[pp.job].direct_off = SIZE_MAX;
+                for (CompositeRec &pc : plan_.composites)
+                    for (size_t t = 0; t < pc.direct_owner.size(); t++)
+                        if (pc.direct_owner[t] == pp.job) {   // back to the composite (cheap interior tiles: at the end of the list)
+                            pc.direct_owner[t] = -1;
+                            pc.list.push_back((uint32_t)(t % (size_t)pc.job.map_w) | ((uint32_t)(t / (size_t)pc.job.map_w) << 16));
+                        }
+            }
+        plan_.fused_launches.push_back({v, param_put(pieces.data(), sizeof(dev::FusedPiece) * pieces.size()),
+                                        param_put(begin.data(), sizeof(int) * begin.size()), (int)begin.size() - 1});
     }
+}
+
+// Packs the parameter arena, turns its offsets into device pointers in the packed jobs and ships it in one copy
+smr_status Renderer::pack_params() {
     const size_t tex_off = param_put_all(plan_.tex, &TexRec::tex);
-    size_t stage_off[3];
-    for (int s = 0; s < 3; s++) stage_off[s] = param_put_all(plan_.stages[s], &StageRec::job);
-    const size_t wj_off = param_put(plan_.weight_jobs.data(), sizeof(dev::WeightJob) * plan_.weight_jobs.size());
+    for (int s = 0; s < 3; s++) plan_.stage_off[s] = param_put_all(plan_.stages[s], &StageRec::job);
+    plan_.weights_off = param_put(plan_.weight_jobs.data(), sizeof(dev::WeightJob) * plan_.weight_jobs.size());
     const size_t tm_off = param_put(plan_.tmaps.data(), sizeof(CUtensorMap) * plan_.tmaps.size());
-    uint64_t direct_tiles = 0;
     for (CompositeRec &pc : plan_.composites) {   // direct-tile maps (one byte per tile: the owner's id) and tile lists
         if (pc.direct_off != SIZE_MAX) {
             bool any = false;
             for (size_t t = 0; t < pc.direct_owner.size(); t++) {
                 param_host_[pc.direct_off + t] = pc.direct_owner[t] >= 0 ? (uint8_t)(pc.direct_owner[t] + 1) : 0;
                 any = any || pc.direct_owner[t] >= 0;
-                direct_tiles += pc.direct_owner[t] >= 0 ? 1 : 0;
+                plan_.direct_tiles += pc.direct_owner[t] >= 0 ? 1 : 0;
             }
             if (!any) pc.direct_off = SIZE_MAX;
         }
@@ -3045,65 +3099,47 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
             pc.job.n_tiles = (int)pc.list.size();
         }
     }
-    const size_t fj_off = param_put_all(plan_.fused, &FusedRec::job);
-    const size_t cj_off = param_put_all(plan_.composites, &CompositeRec::job);   // read by k_composite_multi
-    const TileJobs text_jobs = param_put_tile_jobs(plan_.texts, &TextNode::job);
-    const TileJobs image_jobs = param_put_tile_jobs(plan_.images, &ImageNode::job);
-    // web nodes: one launch per depth, shallow first (depth 1 before the conversions, depth d after phase d - 1's shaders)
-    std::vector<std::vector<WebNode *>> web_launches;
-    std::vector<TileJobs> web_jobs;
-    {
-        for (WebNode *n : plan_.webs) {   // the children's textures, frame-arena addresses resolved
-            for (size_t i = 0; i < n->planes.size(); i++)
-                if (n->plane_child[i] >= 0) n->planes[i].tex = packed_node_tex(*n->owner, n->params.children[n->plane_child[i]]);
-            n->planes_off = param_put(n->planes.data(), sizeof(dev::WebPlane) * n->planes.size());
-        }
-        std::vector<WebNode *> order = plan_.webs;
-        std::stable_sort(order.begin(), order.end(), [](const WebNode *a, const WebNode *b) { return a->params.depth < b->params.depth; });
-        for (WebNode *n : order) {
-            if (web_launches.empty() || web_launches.back()[0]->params.depth != n->params.depth) web_launches.emplace_back();
-            web_launches.back().push_back(n);
-        }
-        for (const auto &l : web_launches) web_jobs.push_back(param_put_tile_jobs(l, &WebNode::job));
+    plan_.fused_off = param_put_all(plan_.fused, &FusedRec::job);
+    plan_.composites_off = param_put_all(plan_.composites, &CompositeRec::job);   // read by k_composite_multi
+    for (WebNode *n : plan_.webs) {   // the children's textures, frame-arena addresses resolved
+        for (size_t i = 0; i < n->planes.size(); i++)
+            if (n->plane_child[i] >= 0) n->planes[i].tex = packed_node_tex(*n->owner, n->params.children[n->plane_child[i]]);
+        n->planes_off = param_put(n->planes.data(), sizeof(dev::WebPlane) * n->planes.size());
     }
-    // shader nodes: one launch per (depth, shader), shallow first, so that every child is drawn before its reader
-    std::vector<std::vector<ShaderNode *>> shader_launches;
-    std::vector<TileJobs> shader_jobs;
-    {
-        std::vector<ShaderNode *> order = plan_.shaders;
-        std::stable_sort(order.begin(), order.end(), [](const ShaderNode *a, const ShaderNode *b) { return a->params.depth < b->params.depth; });
-        for (ShaderNode *n : order) {
-            auto same = [&](const std::vector<ShaderNode *> &l) { return l[0]->params.depth == n->params.depth && l[0]->params.shader == n->params.shader; };
-            auto it = std::find_if(shader_launches.begin(), shader_launches.end(), same);
-            if (it == shader_launches.end()) shader_launches.push_back({n});
-            else it->push_back(n);
+    for (ShaderNode *n : plan_.shaders) {   // likewise
+        n->tex_off = param_alloc(sizeof(dev::Tex) * n->params.children.size());
+        for (size_t k = 0; k < n->params.children.size(); k++)
+            reinterpret_cast<dev::Tex *>(param_host_.data() + n->tex_off)[k] = packed_node_tex(*n->owner, n->params.children[k]);
+        const std::vector<uint8_t> &b = n->params.param_bytes;
+        n->params_off = b.empty() ? SIZE_MAX : param_put(b.data(), b.size());
+    }
+    // the node-texture launches, in the order launch_tick enqueues those of one phase
+    auto all = [](const NodeTexture *) { return true; };
+    add_node_launch(dev::node_kernel(dev::NODE_TEXT), "k_text", SMR_KERNEL_CONVERT, -1, plan_.texts, &TextNode::job, all);
+    add_node_launch(dev::node_kernel(dev::NODE_IMAGE), "k_image", SMR_KERNEL_IMAGE, -1, plan_.images, &ImageNode::job, all);
+    for (int d = 1; d + 1 < (int)plan_.phases.size(); d++) {   // each depth below the roots
+        for (size_t i = 0; i < plan_.shaders.size(); i++) {   // one launch per shader, in the order of its first node
+            auto same = [&](const ShaderNode *n) { return n->params.depth == d && n->params.shader == plan_.shaders[i]->params.shader; };
+            if (same(plan_.shaders[i]) && std::none_of(plan_.shaders.begin(), plan_.shaders.begin() + i, same))
+                add_node_launch(plan_.shaders[i]->params.shader->kernel, "smr_shader_main", SMR_KERNEL_SHADER, d - 1, plan_.shaders,
+                                &ShaderNode::job, same);
         }
-        for (ShaderNode *n : plan_.shaders) {   // the children's textures, frame-arena addresses resolved
-            n->tex.resize(n->params.children.size());
-            for (size_t k = 0; k < n->params.children.size(); k++) n->tex[k] = packed_node_tex(*n->owner, n->params.children[k]);
-            n->tex_off = param_put(n->tex.data(), sizeof(dev::Tex) * n->tex.size());
-            const std::vector<uint8_t> &b = n->params.param_bytes;
-            n->params_off = b.empty() ? SIZE_MAX : param_put(b.data(), b.size());
-        }
-        for (const auto &l : shader_launches) shader_jobs.push_back(param_put_tile_jobs(l, &ShaderNode::job));
+        add_node_launch(dev::node_kernel(dev::NODE_WEB), "k_web", SMR_KERNEL_WEB, d == 1 ? -1 : d - 1, plan_.webs, &WebNode::job,
+                        [&](const WebNode *n) { return n->params.depth == d; });
     }
     // the arena is sized: its offsets become device pointers in the packed jobs
     CUDA_OK(param_pinned_[slot_].ensure(param_used_));
     CUDA_OK(param_dev_[slot_].ensure(param_used_));
     uint8_t *pd = param_dev_[slot_].p;
     auto dev_ptr = [&](size_t off) -> uint8_t * { return off != SIZE_MAX ? pd + off : nullptr; };
-    for (size_t l = 0; l < web_launches.size(); l++) {
-        dev::WebJob *wj = reinterpret_cast<dev::WebJob *>(param_host_.data() + web_jobs[l].jobs_off);
-        for (size_t i = 0; i < web_launches[l].size(); i++) wj[i].planes = (const dev::WebPlane *)(pd + web_launches[l][i]->planes_off);
+    for (WebNode *n : plan_.webs)   // the nodes' own arena data in their packed jobs
+        reinterpret_cast<dev::WebJob *>(param_host_.data() + n->job_off)->planes = (const dev::WebPlane *)(pd + n->planes_off);
+    for (ShaderNode *n : plan_.shaders) {
+        dev::ShaderJob *j = reinterpret_cast<dev::ShaderJob *>(param_host_.data() + n->job_off);
+        j->tex = (const dev::Tex *)(pd + n->tex_off);
+        j->params = dev_ptr(n->params_off);
     }
-    for (size_t l = 0; l < shader_launches.size(); l++) {
-        dev::ShaderJob *sj = reinterpret_cast<dev::ShaderJob *>(param_host_.data() + shader_jobs[l].jobs_off);
-        for (size_t i = 0; i < shader_launches[l].size(); i++) {
-            sj[i].tex = (const dev::Tex *)(pd + shader_launches[l][i]->tex_off);
-            sj[i].params = dev_ptr(shader_launches[l][i]->params_off);
-        }
-    }
-    dev::FusedJob *fj = reinterpret_cast<dev::FusedJob *>(param_host_.data() + fj_off);
+    dev::FusedJob *fj = reinterpret_cast<dev::FusedJob *>(param_host_.data() + plan_.fused_off);
     for (size_t i = 0; i < plan_.fused.size(); i++) {
         const FusedRec &f = plan_.fused[i];
         if (f.tmap_idx >= 0) {
@@ -3112,7 +3148,7 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
         }
         fj[i].direct_map = dev_ptr(f.direct_off);
     }
-    dev::CompositeJob *cj = reinterpret_cast<dev::CompositeJob *>(param_host_.data() + cj_off);
+    dev::CompositeJob *cj = reinterpret_cast<dev::CompositeJob *>(param_host_.data() + plan_.composites_off);
     for (size_t i = 0; i < plan_.composites.size(); i++) {
         const CompositeRec &c = plan_.composites[i];
         cj[i].layers = (const dev::LayerDev *)(pd + c.layers_off);
@@ -3123,91 +3159,74 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
     }
     memcpy(param_pinned_[slot_].p, param_host_.data(), param_used_);
     CUDA_OK(cudaMemcpyAsync(pd, param_pinned_[slot_].p, param_used_, cudaMemcpyHostToDevice, stream_));
+    return SMR_OK;
+}
 
-    // ---- launches -----------------------------------------------------------------------------
-    auto launched = [&](int n) -> bool { if (n < 0) return false; launches += (uint64_t)n; return true; };
-    auto launch_webs = [&](int depth) -> bool {   // the web nodes of `depth` this tick draws, if any
-        for (size_t l = 0; l < web_launches.size(); l++) {
-            if (web_launches[l][0]->params.depth != depth) continue;
-            const TileJobs &t = web_jobs[l];
-            if (!launched(dev::launch_web((const dev::WebJob *)(pd + t.jobs_off), (const int32_t *)(pd + t.begin_off),
-                                          (int)web_launches[l].size(), t.n_tiles, stream_))) return false;
-            prof_mark(SMR_KERNEL_WEB);
+// Enqueues the tick's kernels on stream_, in this order: the text nodes, the image nodes and the web nodes of depth 1 (they
+// read inputs, text and image nodes only); k_convert, k_weights, the fused resamples; per phase p, its generic resample
+// passes, its composite (the last phase's: ONE launch for every output) and then, after its layout nodes of depth p + 1, the
+// shader nodes of that depth (one launch per shader) and its web nodes; the output jobs; the fills.
+smr_status Renderer::launch_tick() {
+    const uint8_t *pd = param_dev_[slot_].p, *ph = param_host_.data();
+    auto launched = [&](int n, int kernel_class) {   // n: the kernels a launcher enqueued, -1: it failed and the tick ends
+        if (n < 0) {
+            set_error(dev::last_launch_error());
+            cudaStreamSynchronize(stream_);
+            return false;
         }
+        plan_.launches += (uint64_t)n;
+        prof_mark(kernel_class);
+        return true;
+    };
+    auto launch_nodes = [&](int phase) {   // the node launches after `phase`, in list order
+        for (const NodeLaunch &l : plan_.node_launches)
+            if (l.phase == phase && !launched(dev::launch_tile_jobs(l.kernel, pd + l.jobs_off, (const int32_t *)(pd + l.begin_off),
+                                                                    l.n_jobs, l.n_tiles, l.name, stream_), l.prof_class)) return false;
         return true;
     };
     prof_mark(-1);
-    if (!plan_.texts.empty()) {   // every text node this tick draws: materialised node textures, like k_convert's
-        if (!launched(dev::launch_text((const dev::TextJob *)(pd + text_jobs.jobs_off), (const int32_t *)(pd + text_jobs.begin_off),
-                                       (int)plan_.texts.size(), text_jobs.n_tiles, stream_))) goto fail;
-        prof_mark(SMR_KERNEL_CONVERT);
-    }
-    if (!plan_.images.empty()) {  // every image node this tick draws
-        if (!launched(dev::launch_image((const dev::ImageJob *)(pd + image_jobs.jobs_off), (const int32_t *)(pd + image_jobs.begin_off),
-                                        (int)plan_.images.size(), image_jobs.n_tiles, stream_))) goto fail;
-        prof_mark(SMR_KERNEL_IMAGE);
-    }
-    if (!launch_webs(1)) goto fail;   // the web nodes of depth 1: after the text and image nodes their children may be
-    node_guard.armed = false;
+    if (!launch_nodes(-1)) return SMR_ERR_CUDA;
+    plan_.nodes_enqueued = true;
     for (auto &cv : plan_.convert_jobs) {
         const dev::Tex &src = plan_.tex[cv.first].tex;
-        if (!launched(dev::launch_convert_to_rgba(src, fb + cv.second, src.width * 4, stream_))) goto fail;
-        prof_mark(SMR_KERNEL_CONVERT);
+        if (!launched(dev::launch_convert_to_rgba(src, frame_dev_.p + cv.second, src.width * 4, stream_), SMR_KERNEL_CONVERT))
+            return SMR_ERR_CUDA;
     }
-    if (!launched(dev::launch_weights((const dev::WeightJob *)(pd + wj_off), plan_.weight_jobs.data(), (int)plan_.weight_jobs.size(),
-                                      stream_))) goto fail;
-    if (!plan_.weight_jobs.empty()) prof_mark(SMR_KERNEL_WEIGHTS);
-    new_weight_keys_.clear();
-    weight_guard.armed = false;   // the tables are being computed on the stream: the cache entries are good
-    for (const FusedLaunch &fl : fused_launches) {
-        if (!launched(dev::launch_resample_fused(fl.key.kernel, fl.key.src, fl.key.range, (const dev::FusedJob *)(pd + fj_off),
+    if (!plan_.weight_jobs.empty() &&
+        !launched(dev::launch_weights((const dev::WeightJob *)(pd + plan_.weights_off), plan_.weight_jobs.data(),
+                                      (int)plan_.weight_jobs.size(), stream_), SMR_KERNEL_WEIGHTS)) return SMR_ERR_CUDA;
+    new_weight_keys_.clear();   // the tables are being computed on the stream: the cache entries are good
+    for (const FusedLaunch &fl : plan_.fused_launches)
+        if (!launched(dev::launch_resample_fused(fl.key.kernel, fl.key.src, fl.key.range, (const dev::FusedJob *)(pd + plan_.fused_off),
                                                  (const dev::FusedPiece *)(pd + fl.pieces_off), (const int *)(pd + fl.begin_off),
-                                                 fl.nblocks, stream_))) goto fail;
-        prof_mark(SMR_KERNEL_RESAMPLE_FUSED);
-    }
-    // phase by phase: the generic resample passes feeding its layout nodes, one composite launch for them, then the shader
-    // nodes of that depth and its web nodes (from depth 2); the last phase is the roots' (ONE composite launch for every
-    // output of the tick)
-    for (size_t p = 0; p < plan_.phases.size(); p++) {
-        const TickPlan::Phase &b = plan_.phases[p];
-        const bool last_phase = p + 1 == plan_.phases.size();
-        const TickPlan::Phase e = last_phase ? TickPlan::Phase{{plan_.stages[0].size(), plan_.stages[1].size(), plan_.stages[2].size()},
-                                                               plan_.composites.size()}
-                                             : plan_.phases[p + 1];
+                                                 fl.nblocks, stream_), SMR_KERNEL_RESAMPLE_FUSED)) return SMR_ERR_CUDA;
+    for (size_t p = 0; p + 1 < plan_.phases.size(); p++) {
+        const TickPlan::Phase &b = plan_.phases[p], &e = plan_.phases[p + 1];
         for (int s = 0; s < 3; s++) {
-            const size_t off = stage_off[s] + sizeof(dev::ResampleJob) * b.stages[s];
+            const size_t off = plan_.stage_off[s] + sizeof(dev::ResampleJob) * b.stages[s];
             const int count = (int)(e.stages[s] - b.stages[s]);
-            if (!launched(dev::launch_resample((const dev::ResampleJob *)(pd + off), (const dev::ResampleJob *)(param_host_.data() + off),
-                                               count, stream_))) goto fail;
-            if (count) prof_mark(SMR_KERNEL_RESAMPLE_BOX + s);
+            if (count && !launched(dev::launch_resample((const dev::ResampleJob *)(pd + off), (const dev::ResampleJob *)(ph + off), count,
+                                                        stream_), SMR_KERNEL_RESAMPLE_BOX + s)) return SMR_ERR_CUDA;
         }
-        if (e.composites > b.composites) {
-            if (!launched(dev::launch_composite((const dev::CompositeJob *)(pd + cj_off) + b.composites, cj + b.composites,
-                                                (const dev::LayerDev *)(param_host_.data() + plan_.composites[b.composites].layers_off),
-                                                (int)(e.composites - b.composites), stream_))) goto fail;
-            prof_mark(SMR_KERNEL_COMPOSITE);
-        }
-        if (last_phase) break;
-        for (size_t l = 0; l < shader_launches.size(); l++) {   // the shader nodes of depth p + 1
-            if (shader_launches[l][0]->params.depth != (int)p + 1) continue;
-            const TileJobs &t = shader_jobs[l];
-            if (!launched(dev::launch_shader(shader_launches[l][0]->params.shader->kernel, (const dev::ShaderJob *)(pd + t.jobs_off),
-                                             (const int32_t *)(pd + t.begin_off), (int)shader_launches[l].size(), t.n_tiles, stream_)))
-                goto fail;
-            prof_mark(SMR_KERNEL_SHADER);
-        }
-        if (p > 0 && !launch_webs((int)p + 1)) goto fail;   // the web nodes of depth p + 1 (depth 1: launched above)
+        if (e.composites > b.composites &&
+            !launched(dev::launch_composite((const dev::CompositeJob *)(pd + plan_.composites_off) + b.composites,
+                                            (const dev::CompositeJob *)(ph + plan_.composites_off) + b.composites,
+                                            (const dev::LayerDev *)(ph + plan_.composites[b.composites].layers_off),
+                                            (int)(e.composites - b.composites), stream_), SMR_KERNEL_COMPOSITE)) return SMR_ERR_CUDA;
+        if (!launch_nodes((int)p)) return SMR_ERR_CUDA;
     }
-    for (OutputRec &o : plan_.outputs) {
-        if (!launched(dev::launch_output(o.job, stream_))) goto fail;
-        prof_mark(SMR_KERNEL_OUTPUT);
-    }
-    for (Fill &f : plan_.fills) {
+    for (OutputRec &o : plan_.outputs)
+        if (!launched(dev::launch_output(o.job, stream_), SMR_KERNEL_OUTPUT)) return SMR_ERR_CUDA;
+    for (Fill &f : plan_.fills)
         if (!launched(dev::launch_fill_yuv(f.p[0], f.p[1], f.p[2], f.pitch[0], f.pitch[1], f.pitch[2], f.w, f.h, f.fmt,
-                                           f.yuv[0], f.yuv[1], f.yuv[2], stream_))) goto fail;
-        prof_mark(SMR_KERNEL_FILL);
-    }
-    // read-back on its own stream: the staging planes are per slot, so the next tick's kernels need not wait for it
+                                           f.yuv[0], f.yuv[1], f.yuv[2], stream_), SMR_KERNEL_FILL)) return SMR_ERR_CUDA;
+    return SMR_OK;
+}
+
+// The read-back of the host outputs, on its own stream: the staging planes are per slot, so the next tick's kernels need
+// not wait for it
+smr_status Renderer::enqueue_readback(uint32_t n_out) {
+    cudaStream_t done_on = stream_;   // the stream the tick's last operation goes to
     if (!plan_.d2h.empty() && !profiling_) {
         CUDA_OK(cudaEventRecord(kernels_done_[slot_], stream_));
         CUDA_OK(cudaStreamWaitEvent(d2h_stream_, kernels_done_[slot_], 0));
@@ -3218,17 +3237,13 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
             CUDA_OK(cudaMemcpyAsync(c.dst, c.src, c.width * c.height, cudaMemcpyDeviceToHost, done_on));
         else
             CUDA_OK(cudaMemcpy2DAsync(c.dst, c.dpitch, c.src, c.spitch, c.width, c.height, cudaMemcpyDeviceToHost, done_on));
-    stats_.kernel_launches += launches;
-    stats_.last_render_kernel_launches = launches;
-    stats_.last_render_direct_tiles = direct_tiles;
+    stats_.kernel_launches += plan_.launches;
+    stats_.last_render_kernel_launches = plan_.launches;
+    stats_.last_render_direct_tiles = plan_.direct_tiles;
     stats_.frames_rendered += n_out;
     CUDA_OK(cudaEventRecord(tick_done_[slot_], done_on));
     inflight_.push_back(slot_);
     return SMR_OK;
-fail:
-    set_error(dev::last_launch_error());
-    cudaStreamSynchronize(stream_);
-    return SMR_ERR_CUDA;
 }
 
 // inspection: what smr_render records for this FrameSet (select_inputs), without reading or copying the frames
