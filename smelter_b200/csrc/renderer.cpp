@@ -578,7 +578,6 @@ class Renderer {
                            std::vector<dev::LayerDev> &layers, std::vector<dev::MaskDev> &masks);
     smr_status plan_layout_node(Output &o, size_t k, uint64_t pts);
     smr_status child_texture(Input &in, RenderLayout &l, int &tex_index, int &tex_w, int &tex_h);
-    template <class Launch> smr_status write_rgba(void *rgba, uint32_t pitch, int32_t mem_kind, uint32_t w, uint32_t h, Launch launch);
     smr_status get_weights(const KernelPass &p, WeightEntry &out);
     int materialised_input(Input &in);
     int try_fused_resample(Input &in, const struct AxisMapping &hm, const struct AxisMapping &vm, int dw, int dh);
@@ -761,8 +760,19 @@ class Renderer {
     }
     void fold_profile();
     bool host_only_ = false;
+    // the steps of the blocking calls (smr_preprocess_frame, smr_premultiply_rgba8, smr_render_text, smr_transcode_resize,
+    // the video converters)
     DevBuf pre_planes_[3], pre_out_;   // FramePreProcessor scratch (input_texture / rescale_texture / download_buffer)
+    smr_status need_device();
+    smr_status stage_in(DevBuf &scratch, const void *src, size_t src_pitch, size_t row_bytes, size_t rows);
     smr_status upload_pre_planes(const smr_input_frame &f, FrameView &v);
+    struct TargetPlane {               // one plane a blocking call writes
+        void *p; size_t pitch, row_bytes, rows; bool device;   // the caller's
+        uint8_t *out; int out_pitch;                            // where its kernel writes it (place_targets)
+    };
+    smr_status place_targets(TargetPlane *t, size_t n);
+    template <class Launch> smr_status launch_and_finish(const TargetPlane *t, size_t n, int kernel_class, Launch launch);
+    cudaEvent_t call_ev_[2] = {};      // launch_and_finish's profiling events
     // smr_transcode_resize's per-axis tables, per (source length, output length); at most kTranscodeTapTables are kept, the
     // least recently used beyond that are released when a call needs room (no call uses more than 32)
     struct TapTable { DevBuf buf; uint64_t used = 0; };
@@ -771,11 +781,6 @@ class Renderer {
     uint64_t transcode_calls_ = 0;
     const dev::TranscodeTap *transcode_table(uint32_t in_len, uint32_t out_len);
     smr_status video_converter_ok(const smr_video_color &c);
-    // profiling of the one kernel of a blocking call (smr_transcode_resize, the video converters): call_prof(0) before the
-    // launch and call_prof(1) after it record events on stream_; call_prof_fold adds the time once the stream has drained
-    cudaEvent_t call_ev_[2] = {};
-    smr_status call_prof(int i);
-    smr_status call_prof_fold(int kernel_class);
     // optional per-kernel-class device timing (cudaEvents on the launching stream)
     void prof_mark(int kernel_class);
     bool profiling_ = false;
@@ -2019,41 +2024,78 @@ void Renderer::prepare_layer(const RenderLayout &l, int W, int H, int tex_index,
     }
 }
 
-// An RGBA8 result of w x h for the caller: `launch` writes it into `rgba` itself (device memory) or into pre_out_, which is
-// copied back (host memory).  Returns once the result is complete, like the reference's device.poll
-// (frame_pre_processor.rs:171-176); the caller's host buffers are borrowed for the call only.
-template <class Launch>
-smr_status Renderer::write_rgba(void *rgba, uint32_t pitch, int32_t mem_kind, uint32_t w, uint32_t h, Launch launch) {
-    const size_t row = (size_t)w * 4, user_pitch = pitch ? pitch : row;
-    if (user_pitch < row) { set_error("output pitch smaller than a row"); return SMR_ERR_BUFFER_TOO_SMALL; }
-    uint8_t *dst = (uint8_t *)rgba;
-    size_t dpitch = user_pitch;
-    if (mem_kind != SMR_MEM_DEVICE) {
-        if (row * h > pre_out_.cap) CUDA_OK(cudaStreamSynchronize(stream_));
-        CUDA_OK(pre_out_.ensure(row * h));
-        dst = pre_out_.p; dpitch = row;
-    } else if ((dpitch & 3) || ((uintptr_t)dst & 3)) { set_error("device RGBA8 planes are 4-byte aligned"); return SMR_ERR_INVALID_ARGUMENT; }
-    if (launch(dst, (int)dpitch) < 0) { set_error(dev::last_launch_error()); return SMR_ERR_CUDA; }
-    stats_.kernel_launches++;
-    if (mem_kind != SMR_MEM_DEVICE) {
-        CUDA_OK(cudaMemcpy2DAsync(rgba, user_pitch, dst, dpitch, row, h, cudaMemcpyDeviceToHost, stream_));
-        stats_.d2h_bytes += row * h;
-    }
-    CUDA_OK(cudaStreamSynchronize(stream_));
+// The blocking calls run one kernel each on stream_ and return once its result is complete, like the reference's
+// device.poll (frame_pre_processor.rs:171-176); the caller's host buffers are borrowed for the call only.  Each checks its
+// arguments, passes need_device, stages its host sources, places its targets, fills its job and calls launch_and_finish.
+smr_status Renderer::need_device() {
+    if (host_only_) { set_error("host-only handle (cuda_device = -1) has no device: no CPU fallback"); return SMR_ERR_CUDA; }
+    CUDA_OK(cudaSetDevice(opts_.cuda_device));
     return SMR_OK;
 }
 
-// A frame read_frame has checked, for a blocking call: host planes are copied, packed, into pre_planes_ on stream_ and `v`
-// is pointed at them; device planes stay where they are
+// rows x row_bytes host bytes at src_pitch, copied packed into `scratch` on stream_ (pageable sources are staged before
+// the copy returns).  Work still on stream_ may read `scratch`, so the stream drains before it is reallocated.
+smr_status Renderer::stage_in(DevBuf &scratch, const void *src, size_t src_pitch, size_t row_bytes, size_t rows) {
+    if (row_bytes * rows > scratch.cap) CUDA_OK(cudaStreamSynchronize(stream_));
+    CUDA_OK(scratch.ensure(row_bytes * rows));
+    CUDA_OK(cudaMemcpy2DAsync(scratch.p, row_bytes, src, src_pitch, row_bytes, rows, cudaMemcpyHostToDevice, stream_));
+    stats_.h2d_bytes += row_bytes * rows;
+    return SMR_OK;
+}
+
+// A frame read_frame has checked: host planes are staged into pre_planes_ and `v` is pointed at them; device planes stay
+// where they are
 smr_status Renderer::upload_pre_planes(const smr_input_frame &f, FrameView &v) {
     for (int p = 0; p < 3 && f.mem_kind != SMR_MEM_DEVICE; p++) {
         const FrameView::Plane &P = v.plane[p];
         if (!P.p) continue;
-        if (P.row_bytes * P.rows > pre_planes_[p].cap) CUDA_OK(cudaStreamSynchronize(stream_));
-        CUDA_OK(pre_planes_[p].ensure(P.row_bytes * P.rows));
-        CUDA_OK(cudaMemcpy2DAsync(pre_planes_[p].p, P.row_bytes, P.p, P.pitch, P.row_bytes, P.rows, cudaMemcpyHostToDevice, stream_));
-        stats_.h2d_bytes += P.row_bytes * P.rows;
+        if (smr_status st = stage_in(pre_planes_[p], P.p, P.pitch, P.row_bytes, P.rows); st != SMR_OK) return st;
         set_tex_plane(v.tex, p, pre_planes_[p].p, P.row_bytes);
+    }
+    return SMR_OK;
+}
+
+// Where the kernel writes each target plane: a device plane itself; host planes packed, in order, into pre_out_, which
+// launch_and_finish copies back.  pre_out_ is sized for them all before a pointer into it is taken (ensure reallocates).
+smr_status Renderer::place_targets(TargetPlane *t, size_t n) {
+    size_t staged = 0;
+    for (size_t i = 0; i < n; i++)
+        if (!t[i].device) staged += t[i].row_bytes * t[i].rows;
+    if (staged > pre_out_.cap) CUDA_OK(cudaStreamSynchronize(stream_));
+    if (staged) CUDA_OK(pre_out_.ensure(staged));
+    for (size_t i = 0, off = 0; i < n; i++) {
+        if (t[i].device) { t[i].out = (uint8_t *)t[i].p; t[i].out_pitch = (int)t[i].pitch; continue; }
+        t[i].out = pre_out_.p + off; t[i].out_pitch = (int)t[i].row_bytes;
+        off += t[i].row_bytes * t[i].rows;
+    }
+    return SMR_OK;
+}
+
+// Enqueues the call's kernel (`launch` returns what a dev::launch_* does) and the copy-backs of its host targets, and waits
+// for them.  The profiling events of `kernel_class` (-1: none) enclose the launch alone.
+template <class Launch>
+smr_status Renderer::launch_and_finish(const TargetPlane *t, size_t n, int kernel_class, Launch launch) {
+    const bool prof = profiling_ && kernel_class >= 0;
+    if (prof && !call_ev_[0]) {
+        CUDA_OK(cudaEventCreate(&call_ev_[0]));
+        CUDA_OK(cudaEventCreate(&call_ev_[1]));
+    }
+    if (prof) CUDA_OK(cudaEventRecord(call_ev_[0], stream_));
+    if (launch() < 0) { set_error(dev::last_launch_error()); return SMR_ERR_CUDA; }
+    stats_.kernel_launches++;
+    if (prof) CUDA_OK(cudaEventRecord(call_ev_[1], stream_));
+    for (size_t i = 0; i < n; i++) {
+        if (t[i].device) continue;
+        CUDA_OK(cudaMemcpy2DAsync(t[i].p, t[i].pitch, t[i].out, t[i].out_pitch, t[i].row_bytes, t[i].rows, cudaMemcpyDeviceToHost,
+                                  stream_));
+        stats_.d2h_bytes += t[i].row_bytes * t[i].rows;
+    }
+    CUDA_OK(cudaStreamSynchronize(stream_));
+    if (prof) {
+        float ms = 0.0f;
+        CUDA_OK(cudaEventElapsedTime(&ms, call_ev_[0], call_ev_[1]));
+        prof_.total_ms[kernel_class] += ms;
+        prof_.launches[kernel_class] += 1;
     }
     return SMR_OK;
 }
@@ -2145,36 +2187,30 @@ smr_status Renderer::transcode_resize(const smr_input_frame *src, const smr_rend
     if (smr_status st = read_frame(*src, v); st != SMR_OK) return st;
     if (src->format != SMR_FRAME_NV12) { set_error("the transcoder resize takes NV12 frames"); return SMR_ERR_UNSUPPORTED; }
     if ((src->width | src->height) & 1) { set_error("NV12 source width and height must be even"); return SMR_ERR_INVALID_ARGUMENT; }
-    if (host_only_) { set_error("host-only handle (cuda_device = -1) has no device: no CPU fallback"); return SMR_ERR_CUDA; }
-    CUDA_OK(cudaSetDevice(opts_.cuda_device));
+    if (smr_status st = need_device(); st != SMR_OK) return st;
     if (smr_status st = upload_pre_planes(*src, v); st != SMR_OK) return st;
+    TargetPlane t[2 * dev::kTranscodeMaxOutputs];   // Y and UV of each rendition
+    for (uint32_t i = 0; i < n; i++) {   // an NV12 row is `width` bytes in both planes
+        const smr_rendition &o = out[i];
+        for (int p = 0; p < 2; p++)
+            t[2 * i + p] = {o.planes[p], o.pitch[p] ? o.pitch[p] : o.width, o.width, p ? o.height / 2 : o.height,
+                            o.mem_kind == SMR_MEM_DEVICE};
+    }
+    if (smr_status st = place_targets(t, 2 * n); st != SMR_OK) return st;
 
     dev::TranscodeLaunch L = {};
     L.src_y = v.tex.p0; L.src_uv = v.tex.p1;
     L.pitch_y = v.tex.pitch0; L.pitch_uv = v.tex.pitch1;
     L.width = (int)src->width; L.height = (int)src->height;
     L.n = (int)n;
-    // host destinations are written into pre_out_, packed, and copied back after the launch
-    size_t staged = 0;
-    for (uint32_t i = 0; i < n; i++)
-        if (out[i].mem_kind != SMR_MEM_DEVICE) staged += (size_t)out[i].width * out[i].height * 3 / 2;
-    if (staged > pre_out_.cap) CUDA_OK(cudaStreamSynchronize(stream_));
-    if (staged) CUDA_OK(pre_out_.ensure(staged));
     transcode_calls_++;
     int blocks = 0;
-    size_t off = 0;
     for (uint32_t i = 0; i < n; i++) {
         const smr_rendition &o = out[i];
         dev::TranscodeOut &J = L.out[i];
         J.width = (int)o.width; J.height = (int)o.height; J.scaling = o.scaling;
-        if (o.mem_kind == SMR_MEM_DEVICE) {
-            J.y = (uint8_t *)o.planes[0]; J.uv = (uint8_t *)o.planes[1];
-            J.pitch_y = (int)(o.pitch[0] ? o.pitch[0] : o.width); J.pitch_uv = (int)(o.pitch[1] ? o.pitch[1] : o.width);
-        } else {
-            J.y = pre_out_.p + off; J.uv = J.y + (size_t)o.width * o.height;
-            J.pitch_y = J.pitch_uv = (int)o.width;
-            off += (size_t)o.width * o.height * 3 / 2;
-        }
+        J.y = t[2 * i].out; J.pitch_y = t[2 * i].out_pitch;
+        J.uv = t[2 * i + 1].out; J.pitch_uv = t[2 * i + 1].out_pitch;
         J.tx = transcode_table(src->width, o.width);
         J.ty = transcode_table(src->height, o.height);
         J.cx = transcode_table(src->width / 2, o.width / 2);
@@ -2184,41 +2220,7 @@ smr_status Renderer::transcode_resize(const smr_input_frame *src, const smr_rend
         J.tile_begin = blocks;
         blocks += J.tiles_x * (int)((o.height / 2 + dev::kTranscodeTileY - 1) / dev::kTranscodeTileY);
     }
-    if (smr_status st = call_prof(0); st != SMR_OK) return st;
-    if (dev::launch_transcode(L, blocks, stream_) < 0) { set_error(dev::last_launch_error()); return SMR_ERR_CUDA; }
-    stats_.kernel_launches++;
-    if (smr_status st = call_prof(1); st != SMR_OK) return st;
-    for (uint32_t i = 0; i < n; i++) {
-        const smr_rendition &o = out[i];
-        if (o.mem_kind == SMR_MEM_DEVICE) continue;
-        const dev::TranscodeOut &J = L.out[i];
-        CUDA_OK(cudaMemcpy2DAsync(o.planes[0], o.pitch[0] ? o.pitch[0] : o.width, J.y, J.pitch_y, o.width, o.height,
-                                  cudaMemcpyDeviceToHost, stream_));
-        CUDA_OK(cudaMemcpy2DAsync(o.planes[1], o.pitch[1] ? o.pitch[1] : o.width, J.uv, J.pitch_uv, o.width, o.height / 2,
-                                  cudaMemcpyDeviceToHost, stream_));
-        stats_.d2h_bytes += (size_t)o.width * o.height * 3 / 2;
-    }
-    CUDA_OK(cudaStreamSynchronize(stream_));
-    return call_prof_fold(SMR_KERNEL_TRANSCODE);
-}
-
-smr_status Renderer::call_prof(int i) {
-    if (!profiling_) return SMR_OK;
-    if (!call_ev_[0]) {
-        CUDA_OK(cudaEventCreate(&call_ev_[0]));
-        CUDA_OK(cudaEventCreate(&call_ev_[1]));
-    }
-    CUDA_OK(cudaEventRecord(call_ev_[i], stream_));
-    return SMR_OK;
-}
-
-smr_status Renderer::call_prof_fold(int kernel_class) {
-    if (!profiling_) return SMR_OK;
-    float ms = 0.0f;
-    CUDA_OK(cudaEventElapsedTime(&ms, call_ev_[0], call_ev_[1]));
-    prof_.total_ms[kernel_class] += ms;
-    prof_.launches[kernel_class] += 1;
-    return SMR_OK;
+    return launch_and_finish(t, 2 * n, SMR_KERNEL_TRANSCODE, [&] { return dev::launch_transcode(L, blocks, stream_); });
 }
 
 // gpu-video's converters (wgpu_helpers/): WgpuConverterParameters as `new` checks them (OnlyLimitedBT709Supported)
@@ -2263,19 +2265,15 @@ smr_status Renderer::video_nv12_to_rgba(const smr_video_color &converter, const 
         set_error("device RGBA8 planes are 4-byte aligned");
         return SMR_ERR_INVALID_ARGUMENT;
     }
-    if (host_only_) { set_error("host-only handle (cuda_device = -1) has no device: no CPU fallback"); return SMR_ERR_CUDA; }
-    CUDA_OK(cudaSetDevice(opts_.cuda_device));
+    if (smr_status st = need_device(); st != SMR_OK) return st;
     if (smr_status st = upload_pre_planes(*src, v); st != SMR_OK) return st;
+    TargetPlane t = {rgba, pitch ? pitch : row, row, oh, mem_kind == SMR_MEM_DEVICE};
+    if (smr_status st = place_targets(&t, 1); st != SMR_OK) return st;
     dev::VideoConvertJob J = {};
     J.src = v.tex;
     J.out_w = (int)ow; J.out_h = (int)oh;
-    smr_status st = write_rgba(rgba, pitch, mem_kind, ow, oh, [&](uint8_t *dst, int dpitch) {
-        J.out = dst; J.out_pitch = dpitch;
-        if (call_prof(0) != SMR_OK) return -1;
-        const int n = dev::launch_video_nv12_to_rgba(J, stream_);
-        return n < 0 || call_prof(1) != SMR_OK ? -1 : n;
-    });
-    return st != SMR_OK ? st : call_prof_fold(SMR_KERNEL_VIDEO_CONVERT);
+    J.out = t.out; J.out_pitch = t.out_pitch;
+    return launch_and_finish(&t, 1, SMR_KERNEL_VIDEO_CONVERT, [&] { return dev::launch_video_nv12_to_rgba(J, stream_); });
 }
 
 // WgpuRgbaToNv12Converter::convert (gpu-video wgpu_helpers/rgba_to_nv12.rs): rgba_to_nv12.wgsl is K11, so the kernel is
@@ -2299,34 +2297,18 @@ smr_status Renderer::video_rgba_to_nv12(const smr_video_color &converter, const 
     FrameView v;
     if (smr_status st = read_frame(*src, v); st != SMR_OK) return st;
     if (src->format != SMR_FRAME_RGBA8) { set_error("the RGBA to NV12 converter takes RGBA8 frames"); return SMR_ERR_UNSUPPORTED; }
-    if (host_only_) { set_error("host-only handle (cuda_device = -1) has no device: no CPU fallback"); return SMR_ERR_CUDA; }
-    CUDA_OK(cudaSetDevice(opts_.cuda_device));
+    if (smr_status st = need_device(); st != SMR_OK) return st;
     if (smr_status st = upload_pre_planes(*src, v); st != SMR_OK) return st;
+    const bool device = mem_kind == SMR_MEM_DEVICE;
+    TargetPlane t[2] = {{planes[0], tp[0], ow, oh, device}, {planes[1], tp[1], ow, oh / 2, device}};
+    if (smr_status st = place_targets(t, 2); st != SMR_OK) return st;
     dev::OutputJob J = {};
     J.src = v.tex;
     J.out_w = (int)ow; J.out_h = (int)oh;
     J.out_format = SMR_OUT_NV12;
-    const size_t luma = (size_t)ow * oh;
-    if (mem_kind == SMR_MEM_DEVICE) {
-        J.out0 = (uint8_t *)planes[0]; J.out1 = (uint8_t *)planes[1];
-        J.out_pitch0 = (int)tp[0]; J.out_pitch1 = (int)tp[1];
-    } else {   // written into pre_out_, packed, and copied back after the launch
-        if (luma * 3 / 2 > pre_out_.cap) CUDA_OK(cudaStreamSynchronize(stream_));
-        CUDA_OK(pre_out_.ensure(luma * 3 / 2));
-        J.out0 = pre_out_.p; J.out1 = pre_out_.p + luma;
-        J.out_pitch0 = J.out_pitch1 = (int)ow;
-    }
-    if (smr_status st = call_prof(0); st != SMR_OK) return st;
-    if (dev::launch_output(J, stream_) < 0) { set_error(dev::last_launch_error()); return SMR_ERR_CUDA; }
-    stats_.kernel_launches++;
-    if (smr_status st = call_prof(1); st != SMR_OK) return st;
-    if (mem_kind != SMR_MEM_DEVICE) {
-        CUDA_OK(cudaMemcpy2DAsync(planes[0], tp[0], J.out0, J.out_pitch0, ow, oh, cudaMemcpyDeviceToHost, stream_));
-        CUDA_OK(cudaMemcpy2DAsync(planes[1], tp[1], J.out1, J.out_pitch1, ow, oh / 2, cudaMemcpyDeviceToHost, stream_));
-        stats_.d2h_bytes += luma * 3 / 2;
-    }
-    CUDA_OK(cudaStreamSynchronize(stream_));
-    return call_prof_fold(SMR_KERNEL_OUTPUT);
+    J.out0 = t[0].out; J.out1 = t[1].out;
+    J.out_pitch0 = t[0].out_pitch; J.out_pitch1 = t[1].out_pitch;
+    return launch_and_finish(t, 2, SMR_KERNEL_OUTPUT, [&] { return dev::launch_output(J, stream_); });
 }
 
 // FramePreProcessor::process_to_bytes / process_to_texture (state/frame_pre_processor.rs:60-100)
@@ -2338,8 +2320,7 @@ smr_status Renderer::preprocess_frame(const smr_input_frame *f, uint32_t ow, uin
         return SMR_ERR_INVALID_ARGUMENT;
     }
     std::lock_guard<std::mutex> g(mu_);
-    if (host_only_) { set_error("host-only handle (cuda_device = -1) has no device: no CPU fallback"); return SMR_ERR_CUDA; }
-    CUDA_OK(cudaSetDevice(opts_.cuda_device));
+    if (smr_status st = need_device(); st != SMR_OK) return st;
     const bool rescale = ow != 0 || oh != 0;
     // the output size is checked after the input size and before the rest of the frame
     if (rescale && frame_size_ok(*f) && (ow == 0 || oh == 0 || ow > 16384 || oh > 16384)) {
@@ -2349,10 +2330,14 @@ smr_status Renderer::preprocess_frame(const smr_input_frame *f, uint32_t ow, uin
     FrameView v;
     if (smr_status st = read_frame(*f, v); st != SMR_OK) return st;
     if (!rescale) { ow = f->width; oh = f->height; }
+    TargetPlane t = {rgba, pitch ? pitch : (size_t)ow * 4, (size_t)ow * 4, oh, mem_kind == SMR_MEM_DEVICE};
+    if (t.pitch < t.row_bytes) { set_error("output pitch smaller than a row"); return SMR_ERR_BUFFER_TOO_SMALL; }
+    if (t.device && ((t.pitch | (uintptr_t)t.p) & 3)) { set_error("device RGBA8 planes are 4-byte aligned"); return SMR_ERR_INVALID_ARGUMENT; }
     if (smr_status st = upload_pre_planes(*f, v); st != SMR_OK) return st;
+    if (smr_status st = place_targets(&t, 1); st != SMR_OK) return st;
     const int kind = premultiply ? 2 : (rescale ? 1 : 0);
-    return write_rgba(rgba, pitch, mem_kind, ow, oh, [&](uint8_t *dst, int dpitch) {
-        return dev::launch_preprocess(v.tex, opts_.rendering_mode, kind, dst, dpitch, (int)ow, (int)oh, stream_);
+    return launch_and_finish(&t, 1, -1, [&] {
+        return dev::launch_preprocess(v.tex, opts_.rendering_mode, kind, t.out, t.out_pitch, (int)ow, (int)oh, stream_);
     });
 }
 
@@ -2362,57 +2347,58 @@ smr_status Renderer::render_text(uint32_t w, uint32_t h, smr_rgba bg, const smr_
     static_assert(sizeof(smr_glyph) == sizeof(dev::GlyphDev), "smr_glyph is copied to the device as it is");
     if (!rgba || (n && !glyphs) || (color_mode != 0 && color_mode != 1)) return SMR_ERR_INVALID_ARGUMENT;
     std::lock_guard<std::mutex> g(mu_);
-    if (host_only_) { set_error("host-only handle (cuda_device = -1) has no device: no CPU fallback"); return SMR_ERR_CUDA; }
-    CUDA_OK(cudaSetDevice(opts_.cuda_device));
+    if (smr_status st = need_device(); st != SMR_OK) return st;
     // a zero-sized text texture is a transparent 1x1 one in the reference (text_renderer.rs:77-85); here the caller skips it
     if (w == 0 || h == 0 || w > 16384 || h > 16384) { set_error("text texture resolution out of range"); return SMR_ERR_INVALID_ARGUMENT; }
     if (n > (1u << 22)) { set_error("too many glyphs"); return SMR_ERR_INVALID_ARGUMENT; }
-    bool need_mask = false, need_color = false;
+    bool need[2] = {false, false};   // the mask atlas, the colour atlas
     for (uint32_t i = 0; i < n; i++) {
-        if (glyphs[i].content == SMR_GLYPH_MASK) need_mask = true;
-        else if (glyphs[i].content == SMR_GLYPH_COLOR) need_color = true;
+        if (glyphs[i].content == SMR_GLYPH_MASK) need[0] = true;
+        else if (glyphs[i].content == SMR_GLYPH_COLOR) need[1] = true;
         else { set_error("glyph content type must be SMR_GLYPH_COLOR or SMR_GLYPH_MASK"); return SMR_ERR_INVALID_ARGUMENT; }
     }
-    dev::TextJob J = {};
-    J.dst.width = (int)w; J.dst.height = (int)h; J.dst.mode = opts_.rendering_mode; J.color_mode = color_mode; J.n_glyphs = (int)n;
-    shader_color(RGBA{bg.r, bg.g, bg.b, bg.a}, J.bg);
     const smr_atlas *atl[2] = {mask, color};
-    const bool need[2] = {need_mask, need_color};
+    size_t atl_row[2] = {};
     for (int k = 0; k < 2; k++) {
-        if (!need[k]) continue;
         const smr_atlas *a = atl[k];
-        const size_t texel = k == 0 ? 1 : 4;
+        if (!need[k]) continue;
         if (!a || !a->data || a->width == 0 || a->height == 0 || a->width > 16384 || a->height > 16384) {
             set_error(k == 0 ? "mask glyphs need a mask atlas" : "colour glyphs need a colour atlas");
             return SMR_ERR_INVALID_ARGUMENT;
         }
-        const size_t row = (size_t)a->width * texel, sp = a->pitch ? a->pitch : row;
-        if (sp < row) { set_error("atlas pitch smaller than a row"); return SMR_ERR_INVALID_ARGUMENT; }
-        if (row * a->height > pre_planes_[k].cap) CUDA_OK(cudaStreamSynchronize(stream_));
-        CUDA_OK(pre_planes_[k].ensure(row * a->height));
-        CUDA_OK(cudaMemcpy2DAsync(pre_planes_[k].p, row, a->data, sp, row, a->height, cudaMemcpyHostToDevice, stream_));
-        stats_.h2d_bytes += row * a->height;
-        if (k == 0) { J.mask = pre_planes_[0].p; J.mask_w = (int)a->width; J.mask_h = (int)a->height; J.mask_pitch = (int)row; }
-        else { J.color = pre_planes_[1].p; J.color_w = (int)a->width; J.color_h = (int)a->height; J.color_pitch = (int)row; }
+        atl_row[k] = (size_t)a->width * (k == 0 ? 1 : 4);
+        if (a->pitch && a->pitch < atl_row[k]) { set_error("atlas pitch smaller than a row"); return SMR_ERR_INVALID_ARGUMENT; }
+    }
+    TargetPlane t = {rgba, pitch ? pitch : (size_t)w * 4, (size_t)w * 4, h, mem_kind == SMR_MEM_DEVICE};
+    if (t.pitch < t.row_bytes) { set_error("output pitch smaller than a row"); return SMR_ERR_BUFFER_TOO_SMALL; }
+    if (t.device && ((t.pitch | (uintptr_t)t.p) & 3)) { set_error("device RGBA8 planes are 4-byte aligned"); return SMR_ERR_INVALID_ARGUMENT; }
+
+    for (int k = 0; k < 2; k++) {
+        const smr_atlas *a = atl[k];
+        if (!need[k]) continue;
+        if (smr_status st = stage_in(pre_planes_[k], a->data, a->pitch ? a->pitch : atl_row[k], atl_row[k], a->height); st != SMR_OK)
+            return st;
     }
     if (n) {
-        const size_t bytes = sizeof(smr_glyph) * (size_t)n;
-        if (bytes > pre_planes_[2].cap) CUDA_OK(cudaStreamSynchronize(stream_));
-        CUDA_OK(pre_planes_[2].ensure(bytes));
-        CUDA_OK(cudaMemcpyAsync(pre_planes_[2].p, glyphs, bytes, cudaMemcpyHostToDevice, stream_));
-        stats_.h2d_bytes += bytes;
-        J.glyphs = reinterpret_cast<const dev::GlyphDev *>(pre_planes_[2].p);
+        if (smr_status st = stage_in(pre_planes_[2], glyphs, sizeof(smr_glyph) * n, sizeof(smr_glyph) * n, 1); st != SMR_OK)
+            return st;
     }
-    // the job and its tile table, as the tick's text launch reads them from the parameter arena
+    if (smr_status st = place_targets(&t, 1); st != SMR_OK) return st;
+    dev::TextJob J = {};
+    J.dst.width = (int)w; J.dst.height = (int)h; J.dst.mode = opts_.rendering_mode; J.color_mode = color_mode; J.n_glyphs = (int)n;
+    J.dst.out = t.out; J.dst.out_pitch = t.out_pitch;
+    shader_color(RGBA{bg.r, bg.g, bg.b, bg.a}, J.bg);
+    if (need[0]) { J.mask = pre_planes_[0].p; J.mask_w = (int)mask->width; J.mask_h = (int)mask->height; J.mask_pitch = (int)atl_row[0]; }
+    if (need[1]) { J.color = pre_planes_[1].p; J.color_w = (int)color->width; J.color_h = (int)color->height; J.color_pitch = (int)atl_row[1]; }
+    if (n) J.glyphs = reinterpret_cast<const dev::GlyphDev *>(pre_planes_[2].p);
+    // the job and its tile table, as the tick's text launch reads them from the parameter arena (pageable sources: staged
+    // before the copies return)
     const size_t begin_off = (sizeof(dev::TextJob) + 15) & ~(size_t)15;
     const int32_t begin[2] = {0, dev::node_tiles((int)w, (int)h)};
     CUDA_OK(text_job_.ensure(begin_off + sizeof(begin)));
-    return write_rgba(rgba, pitch, mem_kind, w, h, [&](uint8_t *dst, int dpitch) {
-        J.dst.out = dst; J.dst.out_pitch = dpitch;
-        // pageable sources: staged before the copies return; write_rgba waits for the launch
-        if (cudaMemcpyAsync(text_job_.p, &J, sizeof(J), cudaMemcpyHostToDevice, stream_) != cudaSuccess ||
-            cudaMemcpyAsync(text_job_.p + begin_off, begin, sizeof(begin), cudaMemcpyHostToDevice, stream_) != cudaSuccess)
-            return -1;
+    CUDA_OK(cudaMemcpyAsync(text_job_.p, &J, sizeof(J), cudaMemcpyHostToDevice, stream_));
+    CUDA_OK(cudaMemcpyAsync(text_job_.p + begin_off, begin, sizeof(begin), cudaMemcpyHostToDevice, stream_));
+    return launch_and_finish(&t, 1, -1, [&] {
         return dev::launch_tile_jobs(dev::node_kernel(dev::NODE_TEXT), text_job_.p, (const int32_t *)(text_job_.p + begin_off), 1,
                                      begin[1], "k_text", stream_);
     });

@@ -766,6 +766,11 @@ class Renderer:
                 f.planes[pi] = ptr
         return arr
 
+    def _one_frame(self, frame: Frame):
+        """the one source frame of a blocking call: (smr_input_frame array, the buffers it points into)"""
+        keep = []
+        return self._input_frames(FrameSet(frames={"_": frame}), keep), keep
+
     def render(self, input: FrameSet, outputs: Optional[List[str]] = None) -> FrameSet:
         """Renderer::render(FrameSet<InputId>) -> FrameSet<OutputId>.  Output planes are host numpy arrays."""
         keep = []
@@ -812,8 +817,7 @@ class Renderer:
     def preprocess_frame(self, frame: Frame, resolution: Optional[Resolution] = None) -> np.ndarray:
         """FramePreProcessor::process_to_bytes (state/frame_pre_processor.rs:81-100): one frame -> RGBA8 bytes of
         its node texture, optionally rescaled (linear sampler) to `resolution`.  Returns an (h, w, 4) uint8 array."""
-        keep = []
-        arr = self._input_frames(FrameSet(frames={"_": frame}), keep)
+        arr, keep = self._one_frame(frame)
         ow, oh = (resolution.width, resolution.height) if resolution else (0, 0)
         w, h = (ow, oh) if resolution else (frame.resolution.width, frame.resolution.height)
         out = np.empty((h, w, 4), np.uint8)
@@ -824,8 +828,7 @@ class Renderer:
         """VideoTranscoder's resize step (gpu-video vulkan_transcoder): one NV12 frame -> up to eight NV12 renditions in one
         launch.  `renditions` is a sequence of (width, height, ScalingAlgorithm); returns, per rendition, its (h, w) Y plane
         and its (h / 2, w / 2, 2) UV plane as host arrays."""
-        keep = []
-        arr = self._input_frames(FrameSet(frames={"_": frame}), keep)
+        arr, keep = self._one_frame(frame)
         outs = (F.Rendition * max(1, len(renditions)))()
         planes = []
         for i, (w, h, scaling) in enumerate(renditions):
@@ -842,8 +845,7 @@ class Renderer:
         """gpu-video's WgpuNv12ToRgbaConverter: one NV12 frame (its crop, origin (0, 0)) -> Rgba8Unorm bytes, bilinearly
         rescaled to `resolution` when it is given.  `converter` is the converter's (ColorSpace, ColorRange), `frame_color`
         the decoded frame's metadata.  Returns an (h, w, 4) uint8 array."""
-        keep = []
-        arr = self._input_frames(FrameSet(frames={"_": frame}), keep)
+        arr, keep = self._one_frame(frame)
         ow, oh = (resolution.width, resolution.height) if resolution else (0, 0)
         w, h = (ow, oh) if resolution else (frame.resolution.width, frame.resolution.height)
         out = np.empty((h, w, 4), np.uint8)
@@ -856,8 +858,7 @@ class Renderer:
         """gpu-video's WgpuRgbaToNv12Converter: one RGBA8 frame (raw bytes, alpha unused) -> NV12 planes, bilinearly
         rescaled to `resolution` (even sides; default: the frame's size).  Returns the (h, w) Y plane and the
         (h / 2, w / 2, 2) UV plane."""
-        keep = []
-        arr = self._input_frames(FrameSet(frames={"_": frame}), keep)
+        arr, keep = self._one_frame(frame)
         w, h = (resolution.width, resolution.height) if resolution else (frame.resolution.width, frame.resolution.height)
         y, uv = np.empty((h, w), np.uint8), np.empty((h // 2, w // 2, 2), np.uint8)
         planes = (C.c_void_p * 2)(y.ctypes.data, uv.ctypes.data)
@@ -880,8 +881,7 @@ class Renderer:
         premultiplied RGBA8 through the renderer's views; the result is a valid FrameData.Rgba8 input."""
         rgba = np.ascontiguousarray(rgba, np.uint8)
         h, w = rgba.shape[:2]
-        keep = []
-        arr = self._input_frames(FrameSet(frames={"_": Frame(FrameData.Rgba8(rgba), Resolution(w, h), 0.0)}), keep)
+        arr, keep = self._one_frame(Frame(FrameData.Rgba8(rgba), Resolution(w, h), 0.0))
         out = np.empty((h, w, 4), np.uint8)
         self._check(self._lib.smr_premultiply_rgba8(self._h, arr, out.ctypes.data, 0, F.MEM_HOST), RenderSceneError)
         return out
