@@ -179,6 +179,35 @@ struct PinnedBuf {
     }
 };
 
+// An owning CUDA handle, move-only: the resource is released when the handle is reset or destroyed, and a null handle
+// releases nothing.  It converts to the raw handle, so calls that take one are written as with a raw member.
+template <class H, auto Release> class Owned {
+    H h_ = nullptr;
+  public:
+    Owned() = default;
+    explicit Owned(H h) : h_(h) {}
+    Owned(Owned &&o) noexcept : h_(o.release()) {}
+    Owned &operator=(Owned &&o) noexcept { reset(o.release()); return *this; }
+    ~Owned() { reset(); }
+    operator H() const { return h_; }
+    H release() { H h = h_; h_ = nullptr; return h; }
+    void reset(H h = nullptr) { if (h_) Release(h_); h_ = h; }
+};
+using Stream = Owned<cudaStream_t, cudaStreamDestroy>;
+using Event = Owned<cudaEvent_t, cudaEventDestroy>;
+using MemPool = Owned<cudaMemPool_t, cudaMemPoolDestroy>;
+using Library = Owned<cudaLibrary_t, cudaLibraryUnload>;
+template <class T> using DevMem = Owned<T *, cudaFree>;
+using IpcMapping = Owned<void *, cudaIpcCloseMemHandle>;
+
+// `create`(&handle, args...) into `out`, with the status it returns
+template <class H, auto R, class Create, class... Args> static cudaError_t make(Owned<H, R> &out, Create create, Args... args) {
+    H h = nullptr;
+    cudaError_t e = create(&h, args...);
+    out.reset(e == cudaSuccess ? h : nullptr);
+    return e;
+}
+
 struct NcclId { char b[128]; };
 typedef int (*nccl_init_fn)(void **, int, NcclId, int);
 static struct {
@@ -194,6 +223,7 @@ static struct {
     int (*GroupEnd)() = nullptr;
     const char *(*GetErrorString)(int) = nullptr;
 } g_nccl;
+static int nccl_comm_destroy(void *comm) { return g_nccl.CommDestroy(comm); }
 
 // NVRTC (shader registration), also dlopen'ed on first use: the library does not link against it
 static struct {
@@ -507,12 +537,14 @@ class Renderer {
             return std::tie(scale_bits, offset_bits, n_out) < std::tie(o.scale_bits, o.offset_bits, o.n_out);
         }
     };
-    struct WeightEntry {
+    struct WeightEntry {         // one allocation: weights, inv and first, each from a 256-byte boundary
+        DevMem<uint8_t> mem;
         float *weights = nullptr, *inv = nullptr;
         int32_t *first = nullptr;
         int taps = 0;
         uint64_t last_used = 0;
     };
+    struct LaneTable { DevMem<uint8_t> perm; uint64_t last_used = 0; };
 
     // arenas ----------------------------------------------------------------------------------
     size_t param_alloc(size_t bytes) {  // returns offset in the param arena (256-byte aligned: tensor maps need 64)
@@ -578,7 +610,7 @@ class Renderer {
                            std::vector<dev::LayerDev> &layers, std::vector<dev::MaskDev> &masks);
     smr_status plan_layout_node(Output &o, size_t k, uint64_t pts);
     smr_status child_texture(Input &in, RenderLayout &l, int &tex_index, int &tex_w, int &tex_h);
-    smr_status get_weights(const KernelPass &p, WeightEntry &out);
+    smr_status get_weights(const KernelPass &p, const WeightEntry *&out);
     int materialised_input(Input &in);
     int try_fused_resample(Input &in, const struct AxisMapping &hm, const struct AxisMapping &vm, int dw, int dh);
     int source_tmaps(const dev::Tex &t, int src_class);
@@ -590,7 +622,20 @@ class Renderer {
     void shader_color(const RGBA &c, float out[4]) const;
 
     smr_options opts_;
-    cudaStream_t stream_ = nullptr;
+    // Members are destroyed in reverse order, so these come first: each stream outlives the work and the stream-ordered
+    // releases enqueued on it, web_pool_ outlives the web frames allocated from it, and retired_shaders_ outlives the
+    // shader programs that retire their modules into it.
+    Stream stream_;
+    Stream copy_stream_, copy_stream2_;   // uploads alternate between two streams (two DMA engines)
+    Stream d2h_stream_;                   // read-back of host outputs: overlaps the next tick's kernels
+    // the tick's exchange step overlaps the previous tick's kernels: NCCL runs on its own stream, ordered after
+    // everything submitted BEFORE the most recent tick and before the next one
+    Stream comm_stream_;
+    // Web frames: allocated on copy_stream_, released on stream_.  The pool never makes an allocation wait for a release
+    // that is still pending on stream_ (no internal dependencies), so a copy does not wait for the ticks in flight.
+    MemPool web_pool_;
+    // Shader modules whose last user is gone: each is unloaded once the event recorded on stream_ at that time completes
+    std::vector<std::pair<Library, Event>> retired_shaders_;
     SceneState scene_;
     std::map<std::string, Input> inputs_;
     std::map<std::string, Output> outputs_;
@@ -690,13 +735,8 @@ class Renderer {
     void plan_web_node(Output &o, WebNode &n);
     smr_status make_shader_node(const ShaderParams &p, std::unique_ptr<ShaderNode> &out);
     void plan_shader_node(Output &o, ShaderNode &n, uint64_t pts);
-    // Shader modules whose last user is gone: each is unloaded once the event recorded on stream_ at that time completes
-    std::vector<std::pair<void *, cudaEvent_t>> retired_shaders_;
     void reap_shaders(bool all);
-    cudaEvent_t web_ev_ = nullptr;             // the end of a web frame's copy: later launches on stream_ wait for it
-    // Web frames: allocated on copy_stream_, released on stream_.  The pool never makes an allocation wait for a release
-    // that is still pending on stream_ (no internal dependencies), so a copy does not wait for the ticks in flight.
-    cudaMemPool_t web_pool_ = nullptr;
+    Event web_ev_;                             // the end of a web frame's copy: later launches on stream_ wait for it
     smr_status alloc_on_stream(size_t bytes, std::shared_ptr<void> &buf);
     Output &install_output(const char *output_id, OutputNode &&node, int32_t fmt, uint32_t w, uint32_t h);
     void plan_node_textures(Output &o, uint64_t pts);
@@ -720,7 +760,8 @@ class Renderer {
     };
     std::map<TmapKey, CUtensorMap> tmap_cache_;
     // any-ratio TMA kernel: per (horizontal mapping, strip width) the lane <-> column-pair deal of every strip
-    std::map<std::tuple<uint32_t, uint32_t, int32_t, int32_t>, uint8_t *> lane_perms_;
+    std::map<std::tuple<uint32_t, uint32_t, int32_t, int32_t>, LaneTable> lane_perms_;
+    template <class Cache> void bound_cache(Cache &c);
     const uint8_t *lane_perm(float scale, float offset, int n_out, int cols);
     bool plane_tmap(const uint8_t *p, int pitch, int w, int h, int kind, CUtensorMap *out);
     bool direct_k11_ = true;                   // SMR_DIRECT_K11=0: A/B switch, every tile goes through the composite
@@ -733,16 +774,11 @@ class Renderer {
     DevBuf frame_dev_;
     std::map<WeightKey, WeightEntry> weights_;
     // up to two ticks in flight: uploads of tick n+1 (copy stream) overlap the kernels of tick n
-    cudaStream_t copy_stream_ = nullptr, copy_stream2_ = nullptr;   // uploads alternate between two streams (two DMA engines)
-    cudaStream_t d2h_stream_ = nullptr;      // read-back of host outputs: overlaps the next tick's kernels
-    cudaEvent_t kernels_done_[kTicksInFlight] = {};
-    cudaEvent_t h2d_done2_[kTicksInFlight] = {};
+    Event kernels_done_[kTicksInFlight];
+    Event h2d_done2_[kTicksInFlight];
     int upload_rr_ = 0;
-    cudaEvent_t h2d_done_[kTicksInFlight] = {}, tick_done_[kTicksInFlight] = {};
-    // the tick's exchange step overlaps the previous tick's kernels: NCCL runs on its own stream, ordered after
-    // everything submitted BEFORE the most recent tick and before the next one
-    cudaStream_t comm_stream_ = nullptr;
-    cudaEvent_t comm_done_ = nullptr, tick_start_ = nullptr;
+    Event h2d_done_[kTicksInFlight], tick_done_[kTicksInFlight];
+    Event comm_done_, tick_start_;
     bool comm_pending_ = false, tick_started_ = false;
     std::deque<int> inflight_;
     int slot_ = 0;
@@ -772,7 +808,7 @@ class Renderer {
     };
     smr_status place_targets(TargetPlane *t, size_t n);
     template <class Launch> smr_status launch_and_finish(const TargetPlane *t, size_t n, int kernel_class, Launch launch);
-    cudaEvent_t call_ev_[2] = {};      // launch_and_finish's profiling events
+    Event call_ev_[2];                 // launch_and_finish's profiling events
     // smr_transcode_resize's per-axis tables, per (source length, output length); at most kTranscodeTapTables are kept, the
     // least recently used beyond that are released when a call needs room (no call uses more than 32)
     struct TapTable { DevBuf buf; uint64_t used = 0; };
@@ -784,15 +820,18 @@ class Renderer {
     // optional per-kernel-class device timing (cudaEvents on the launching stream)
     void prof_mark(int kernel_class);
     bool profiling_ = false;
-    std::vector<cudaEvent_t> prof_events_;
+    std::vector<Event> prof_events_;
     size_t prof_next_event_ = 0;
     std::vector<std::pair<cudaEvent_t, int>> prof_marks_;
     smr_kernel_times prof_ = {};
     // NCCL communicator for shared-input replication (SURVEY 8e); libnccl is dlopen'ed on first use
-    void *nccl_comm_ = nullptr;
+    Owned<void *, nccl_comm_destroy> nccl_comm_;
     int comm_rank_ = 0, comm_size_ = 1;
-    int32_t *barrier_word_ = nullptr;            // 4 device bytes the per-tick all-reduce of the peer modes runs on
-    std::vector<void *> peer_own_, peer_opened_; // pools of smr_peer_pool_alloc / smr_peer_pool_open still alive
+    DevMem<int32_t> barrier_word_;               // 4 device bytes the per-tick all-reduce of the peer modes runs on
+    // pools of smr_peer_pool_alloc / smr_peer_pool_open still alive
+    std::vector<Owned<void *, cudaFree>> peer_own_;
+    std::vector<IpcMapping> peer_opened_;
+    template <class Pools> smr_status peer_pool_release(Pools &pools, void *dev_ptr);
   public:
     smr_status comm_init(const uint8_t *id, int rank, int nranks);
     smr_status comm_exchange(const smr_input_frame *frames, uint32_t n, const int32_t *roots, const uint64_t *consumers,
@@ -810,35 +849,15 @@ class Renderer {
 };
 
 Renderer::~Renderer() {
-    if (stream_) {
-        cudaSetDevice(opts_.cuda_device);
-        cudaStreamSynchronize(stream_);
-        if (copy_stream_) { cudaStreamSynchronize(copy_stream_); cudaStreamDestroy(copy_stream_); }
-        if (copy_stream2_) { cudaStreamSynchronize(copy_stream2_); cudaStreamDestroy(copy_stream2_); }
-        if (d2h_stream_) { cudaStreamSynchronize(d2h_stream_); cudaStreamDestroy(d2h_stream_); }
-        for (int i = 0; i < kTicksInFlight; i++) if (kernels_done_[i]) cudaEventDestroy(kernels_done_[i]);
-        for (int i = 0; i < kTicksInFlight; i++) if (h2d_done2_[i]) cudaEventDestroy(h2d_done2_[i]);
-        if (comm_stream_) { cudaStreamSynchronize(comm_stream_); cudaStreamDestroy(comm_stream_); }
-        if (comm_done_) cudaEventDestroy(comm_done_);
-        if (tick_start_) cudaEventDestroy(tick_start_);
-        if (web_ev_) cudaEventDestroy(web_ev_);
-        for (cudaEvent_t e : call_ev_) if (e) cudaEventDestroy(e);
-        for (int i = 0; i < kTicksInFlight; i++) { if (h2d_done_[i]) cudaEventDestroy(h2d_done_[i]); if (tick_done_[i]) cudaEventDestroy(tick_done_[i]); }
-        if (nccl_comm_) { g_nccl.CommDestroy(nccl_comm_); nccl_comm_ = nullptr; }
-        for (auto &kv : weights_) {
-            cudaFree(kv.second.weights); cudaFree(kv.second.inv); cudaFree(kv.second.first);
-        }
-        for (auto &kv : lane_perms_) cudaFree(kv.second);
-        outputs_.clear();   // text, image and web nodes, image assets and web frames free their memory on stream_
-        scene_ = SceneState();
-        cudaStreamSynchronize(stream_);
-        reap_shaders(true);
-        if (web_pool_) cudaMemPoolDestroy(web_pool_);   // after the web frames it holds were released above
-        for (void *p : peer_opened_) cudaIpcCloseMemHandle(p);
-        for (void *p : peer_own_) cudaFree(p);
-        if (barrier_word_) cudaFree(barrier_word_);
-        cudaStreamDestroy(stream_);
-    }
+    if (!stream_) return;   // host-only: nothing was made on a device
+    cudaSetDevice(opts_.cuda_device);   // the members below are released on this device
+    drain();   // no stream still runs work that reads what is released here
+    // node textures, image assets and web frames free themselves on stream_ (web frames into web_pool_), and dropping a
+    // shader program retires its module on stream_: all before the streams and the pool go
+    outputs_.clear();
+    scene_ = SceneState();
+    cudaStreamSynchronize(stream_);   // those releases have run
+    reap_shaders(true);   // every retired module's event has completed
 }
 
 static double eotf_f64(double c) { return c <= 0.04045 ? c / 12.92 : std::pow((c + 0.055) / 1.055, 2.4); }  // wgpu/utils.rs:74-81
@@ -874,22 +893,22 @@ smr_status Renderer::init() {
         return SMR_ERR_UNSUPPORTED;
     }
     CUDA_OK(cudaSetDevice(opts_.cuda_device));
-    CUDA_OK(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
-    CUDA_OK(cudaStreamCreateWithFlags(&copy_stream_, cudaStreamNonBlocking));
-    CUDA_OK(cudaStreamCreateWithFlags(&copy_stream2_, cudaStreamNonBlocking));
-    CUDA_OK(cudaStreamCreateWithFlags(&d2h_stream_, cudaStreamNonBlocking));
-    for (int i = 0; i < kTicksInFlight; i++) CUDA_OK(cudaEventCreateWithFlags(&kernels_done_[i], cudaEventDisableTiming));
-    for (int i = 0; i < kTicksInFlight; i++) CUDA_OK(cudaEventCreateWithFlags(&h2d_done2_[i], cudaEventDisableTiming));
-    CUDA_OK(cudaStreamCreateWithFlags(&comm_stream_, cudaStreamNonBlocking));
-    CUDA_OK(cudaEventCreateWithFlags(&comm_done_, cudaEventDisableTiming));
-    CUDA_OK(cudaEventCreateWithFlags(&tick_start_, cudaEventDisableTiming));
-    CUDA_OK(cudaEventCreateWithFlags(&web_ev_, cudaEventDisableTiming));
+    CUDA_OK(make(stream_, cudaStreamCreateWithFlags, cudaStreamNonBlocking));
+    CUDA_OK(make(copy_stream_, cudaStreamCreateWithFlags, cudaStreamNonBlocking));
+    CUDA_OK(make(copy_stream2_, cudaStreamCreateWithFlags, cudaStreamNonBlocking));
+    CUDA_OK(make(d2h_stream_, cudaStreamCreateWithFlags, cudaStreamNonBlocking));
+    for (int i = 0; i < kTicksInFlight; i++) CUDA_OK(make(kernels_done_[i], cudaEventCreateWithFlags, cudaEventDisableTiming));
+    for (int i = 0; i < kTicksInFlight; i++) CUDA_OK(make(h2d_done2_[i], cudaEventCreateWithFlags, cudaEventDisableTiming));
+    CUDA_OK(make(comm_stream_, cudaStreamCreateWithFlags, cudaStreamNonBlocking));
+    CUDA_OK(make(comm_done_, cudaEventCreateWithFlags, cudaEventDisableTiming));
+    CUDA_OK(make(tick_start_, cudaEventCreateWithFlags, cudaEventDisableTiming));
+    CUDA_OK(make(web_ev_, cudaEventCreateWithFlags, cudaEventDisableTiming));
     {
         cudaMemPoolProps props = {};
         props.allocType = cudaMemAllocationTypePinned;
         props.location.type = cudaMemLocationTypeDevice;
         props.location.id = opts_.cuda_device;
-        CUDA_OK(cudaMemPoolCreate(&web_pool_, &props));
+        CUDA_OK(make(web_pool_, cudaMemPoolCreate, &props));
         int no = 0;
         CUDA_OK(cudaMemPoolSetAttribute(web_pool_, cudaMemPoolReuseAllowInternalDependencies, &no));
         uint64_t keep = UINT64_MAX;   // released frames stay in the pool for the next ones
@@ -897,8 +916,8 @@ smr_status Renderer::init() {
     }
     CUDA_OK(cudaDeviceGetAttribute(&sm_count_, cudaDevAttrMultiProcessorCount, opts_.cuda_device));
     for (int i = 0; i < kTicksInFlight; i++) {
-        CUDA_OK(cudaEventCreateWithFlags(&h2d_done_[i], cudaEventDisableTiming));
-        CUDA_OK(cudaEventCreateWithFlags(&tick_done_[i], cudaEventDisableTiming));
+        CUDA_OK(make(h2d_done_[i], cudaEventCreateWithFlags, cudaEventDisableTiming));
+        CUDA_OK(make(tick_done_[i], cudaEventCreateWithFlags, cudaEventDisableTiming));
     }
     float u8n[256], dec[256];
     for (int b = 0; b < 256; b++) {
@@ -1081,16 +1100,8 @@ smr_status Renderer::unregister_output(const char *id) {
 }
 
 void Renderer::reap_shaders(bool all) {
-    for (size_t i = 0; i < retired_shaders_.size();) {
-        auto &r = retired_shaders_[i];
-        if (all || cudaEventQuery(r.second) == cudaSuccess) {
-            cudaLibraryUnload((cudaLibrary_t)r.first);
-            cudaEventDestroy(r.second);
-            retired_shaders_.erase(retired_shaders_.begin() + (long)i);
-        } else {
-            i++;
-        }
-    }
+    auto done = [all](const std::pair<Library, Event> &r) { return all || cudaEventQuery(r.second) == cudaSuccess; };
+    retired_shaders_.erase(std::remove_if(retired_shaders_.begin(), retired_shaders_.end(), done), retired_shaders_.end());
 }
 
 smr_status Renderer::register_shader(const char *id, const smr_shader_spec *spec) {
@@ -1131,7 +1142,7 @@ smr_status Renderer::add_shader(const char *id, std::unique_ptr<ShaderProgram> p
         reap_shaders(false);
         cudaLibrary_t lib = nullptr;
         CUDA_OK(cudaLibraryLoadData(&lib, program->cubin.data(), nullptr, nullptr, 0, nullptr, nullptr, 0));
-        program->library = lib;
+        Library owned(lib);   // unloaded if what follows fails
         cudaKernel_t k = nullptr;
         const void *src[5];
         size_t bytes[5];
@@ -1146,26 +1157,23 @@ smr_status Renderer::add_shader(const char *id, std::unique_ptr<ShaderProgram> p
         }
         if (e == cudaSuccess) e = cudaStreamSynchronize(stream_);
         if (e != cudaSuccess) {
-            cudaLibraryUnload(lib);
             set_error(std::string("loading the shader module: ") + cudaGetErrorString(e));
             return SMR_ERR_CUDA;
         }
+        program->library = owned.release();
         program->kernel = (const void *)k;
     }
     // the module is unloaded after the ticks submitted before its last user let go of it
     std::shared_ptr<ShaderProgram> shared(program.release(), [this](ShaderProgram *p) {
-        cudaEvent_t ev = nullptr;
-        if (p->library) {
-            cudaSetDevice(opts_.cuda_device);
-            if (cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) == cudaSuccess && cudaEventRecord(ev, stream_) == cudaSuccess) {
-                retired_shaders_.push_back({p->library, ev});
-            } else {   // no event: wait for the stream instead
-                if (ev) cudaEventDestroy(ev);
-                cudaStreamSynchronize(stream_);
-                cudaLibraryUnload((cudaLibrary_t)p->library);
-            }
-        }
+        Library lib((cudaLibrary_t)p->library);
         delete p;
+        if (!lib) return;
+        cudaSetDevice(opts_.cuda_device);
+        Event ev;
+        if (make(ev, cudaEventCreateWithFlags, cudaEventDisableTiming) == cudaSuccess && cudaEventRecord(ev, stream_) == cudaSuccess)
+            retired_shaders_.emplace_back(std::move(lib), std::move(ev));
+        else   // no event: wait for the stream instead, then unload
+            cudaStreamSynchronize(stream_);
     });
     if (!scene_.register_shader(id, std::move(shared))) { set_error("a shader with this id is already registered"); return SMR_ERR_INVALID_ARGUMENT; }
     return SMR_OK;
@@ -1733,14 +1741,14 @@ int Renderer::try_fused_resample(Input &in, const AxisMapping &hm_in, const Axis
             k = {dev::FusedKernel::TMA_ANY, 0, bucket, box ? 1 : 0};
     }
     if (box && k.kind != dev::FusedKernel::TMA_ANY) return -1;   // no other fused kernel reduces: generic passes
-    WeightEntry wh, wv;
+    const WeightEntry *wh, *wv;
     if (get_weights(passes[0], wh) != SMR_OK || get_weights(passes[1], wv) != SMR_OK) return -2;
     size_t dst_off = frame_alloc((size_t)dw * dh * 4);
     dev::FusedJob j{};
     j.dst_w = dw; j.dst_h = dh; j.dst_pitch = dw * 4;
-    j.taps_h = wh.taps; j.taps_v = wv.taps;
-    j.w_h = wh.weights; j.inv_h = wh.inv; j.first_h = wh.first;
-    j.w_v = wv.weights; j.inv_v = wv.inv; j.first_v = wv.first;
+    j.taps_h = wh->taps; j.taps_v = wv->taps;
+    j.w_h = wh->weights; j.inv_h = wh->inv; j.first_h = wh->first;
+    j.w_v = wv->weights; j.inv_v = wv->inv; j.first_v = wv->first;
     if (k.kind == dev::FusedKernel::TMA_INT) j.v_same = vm.crop_offset == 0.0f && sv == sh && tv == th;
     if (k.kind == dev::FusedKernel::TMA_ANY) {
         j.strip_cols = cols;
@@ -1777,12 +1785,11 @@ const uint8_t *Renderer::lane_perm(float scale, float offset, int n_out, int col
     memcpy(&sb, &scale, 4); memcpy(&ob, &offset, 4);
     auto key = std::make_tuple(sb, ob, (int32_t)n_out, (int32_t)cols);
     auto it = lane_perms_.find(key);
-    if (it != lane_perms_.end()) return it->second;
-    if (lane_perms_.size() > 4096) {
-        cudaStreamSynchronize(stream_);
-        for (auto &e : lane_perms_) cudaFree(e.second);
-        lane_perms_.clear();
+    if (it != lane_perms_.end()) {
+        it->second.last_used = tick_;
+        return it->second.perm;
     }
+    bound_cache(lane_perms_);
     const float ks = std::fmax(scale, 1.0f);
     auto first = [&](int o) {
         volatile float c = offset + ((float)o + 0.5f) * scale;
@@ -1804,13 +1811,22 @@ const uint8_t *Renderer::lane_perm(float scale, float offset, int n_out, int col
     }
     uint8_t *dev_perm = nullptr;
     if (cudaMalloc(&dev_perm, perm.size()) != cudaSuccess) { cudaGetLastError(); return nullptr; }
+    DevMem<uint8_t> owned(dev_perm);
     // pageable source: staged before the call returns
     if (cudaMemcpyAsync(dev_perm, perm.data(), perm.size(), cudaMemcpyHostToDevice, stream_) != cudaSuccess) {
-        cudaGetLastError(); cudaFree(dev_perm); return nullptr;
+        cudaGetLastError(); return nullptr;
     }
     cudaStreamSynchronize(stream_);   // once per geometry; keeps the pageable staging out of the steady state
-    lane_perms_[key] = dev_perm;
+    lane_perms_[key] = {std::move(owned), tick_};
     return dev_perm;
+}
+
+// Bounds a cache of device tables (weights_, lane_perms_): past 4096 entries, the entries this tick has not used are
+// dropped once stream_ no longer reads them.  Jobs planned earlier in the tick keep theirs.
+template <class Cache> void Renderer::bound_cache(Cache &c) {
+    if (c.size() <= 4096) return;
+    cudaStreamSynchronize(stream_);
+    for (auto i = c.begin(); i != c.end();) i = i->second.last_used == tick_ ? std::next(i) : c.erase(i);
 }
 
 bool Renderer::plane_tmap(const uint8_t *p, int pitch, int w, int h, int kind, CUtensorMap *out) {
@@ -1830,12 +1846,7 @@ bool Renderer::plane_tmap(const uint8_t *p, int pitch, int w, int h, int kind, C
 // Weight tables created by a tick whose k_weights launch was never enqueued hold uninitialised memory: drop them so that
 // the next tick computes them.
 void Renderer::rollback_weights() {
-    for (const WeightKey &k : new_weight_keys_) {
-        auto it = weights_.find(k);
-        if (it == weights_.end()) continue;
-        cudaFree(it->second.weights); cudaFree(it->second.inv); cudaFree(it->second.first);
-        weights_.erase(it);
-    }
+    for (const WeightKey &k : new_weight_keys_) weights_.erase(k);
     new_weight_keys_.clear();
     plan_.weight_jobs.clear();
 }
@@ -2077,8 +2088,8 @@ template <class Launch>
 smr_status Renderer::launch_and_finish(const TargetPlane *t, size_t n, int kernel_class, Launch launch) {
     const bool prof = profiling_ && kernel_class >= 0;
     if (prof && !call_ev_[0]) {
-        CUDA_OK(cudaEventCreate(&call_ev_[0]));
-        CUDA_OK(cudaEventCreate(&call_ev_[1]));
+        CUDA_OK(make(call_ev_[0], cudaEventCreateWithFlags, cudaEventDefault));
+        CUDA_OK(make(call_ev_[1], cudaEventCreateWithFlags, cudaEventDefault));
     }
     if (prof) CUDA_OK(cudaEventRecord(call_ev_[0], stream_));
     if (launch() < 0) { set_error(dev::last_launch_error()); return SMR_ERR_CUDA; }
@@ -2404,7 +2415,7 @@ smr_status Renderer::render_text(uint32_t w, uint32_t h, smr_rgba bg, const smr_
     });
 }
 
-smr_status Renderer::get_weights(const KernelPass &p, WeightEntry &out) {
+smr_status Renderer::get_weights(const KernelPass &p, const WeightEntry *&out) {
     WeightKey key;
     float scale = p.mapping.scale(), offset = p.mapping.crop_offset;
     memcpy(&key.scale_bits, &scale, 4);
@@ -2413,37 +2424,30 @@ smr_status Renderer::get_weights(const KernelPass &p, WeightEntry &out) {
     auto it = weights_.find(key);
     if (it != weights_.end()) {
         it->second.last_used = tick_;
-        out = it->second;
+        out = &it->second;
         return SMR_OK;
     }
-    if (weights_.size() > 4096) {  // bound the cache: drop entries not used this tick
-        cudaStreamSynchronize(stream_);
-        for (auto i = weights_.begin(); i != weights_.end();) {
-            if (i->second.last_used != tick_) {
-                cudaFree(i->second.weights); cudaFree(i->second.inv); cudaFree(i->second.first);
-                i = weights_.erase(i);
-            } else ++i;
-        }
-    }
-    WeightEntry e;
-    e.taps = resample_taps(scale);
-    if (e.taps < 1 || e.taps > 4096) { set_error("resampler tap count out of range"); return SMR_ERR_INVALID_ARGUMENT; }
-    e.last_used = tick_;
-    if (cudaMalloc(&e.weights, sizeof(float) * (size_t)e.taps * key.n_out) != cudaSuccess ||
-        cudaMalloc(&e.inv, sizeof(float) * key.n_out) != cudaSuccess ||
-        cudaMalloc(&e.first, sizeof(int32_t) * key.n_out) != cudaSuccess) {
-        cudaFree(e.weights); cudaFree(e.inv); cudaFree(e.first);
+    bound_cache(weights_);
+    const int taps = resample_taps(scale);
+    if (taps < 1 || taps > 4096) { set_error("resampler tap count out of range"); return SMR_ERR_INVALID_ARGUMENT; }
+    auto up256 = [](size_t n) { return (n + 255) & ~(size_t)255; };
+    const size_t w_bytes = up256(sizeof(float) * (size_t)taps * key.n_out), inv_bytes = up256(sizeof(float) * key.n_out);
+    uint8_t *d = nullptr;
+    if (cudaMalloc(&d, w_bytes + inv_bytes + sizeof(int32_t) * key.n_out) != cudaSuccess) {
         cudaGetLastError();
         set_error("out of device memory for resampler weight tables");
         return SMR_ERR_CUDA;
     }
+    WeightEntry &e = weights_[key];
+    e.mem.reset(d);
+    e.weights = (float *)d; e.inv = (float *)(d + w_bytes); e.first = (int32_t *)(d + w_bytes + inv_bytes);
+    e.taps = taps; e.last_used = tick_;
     new_weight_keys_.push_back(key);
     dev::WeightJob j;
     j.scale = scale; j.offset = offset; j.n_out = key.n_out; j.taps = e.taps;
     j.weights = e.weights; j.inv_wsum = e.inv; j.first = e.first;
     plan_.weight_jobs.push_back(j);
-    weights_[key] = e;
-    out = e;
+    out = &e;
     return SMR_OK;
 }
 
@@ -2686,12 +2690,12 @@ smr_status Renderer::child_texture(Input &in, RenderLayout &l, int &tex_index, i
         for (int pi = 0; pi < np; pi++) {
             const KernelPass &kp = passes[pi];
             bool last = pi == np - 1;
-            WeightEntry we;
+            const WeightEntry *we;
             smr_status st = get_weights(kp, we);
             if (st != SMR_OK) return st;
             dev::ResampleJob j{};
-            j.axis = kp.mapping.axis; j.perp_offset = kp.perp_offset; j.taps = we.taps;
-            j.weights = we.weights; j.inv_wsum = we.inv; j.first = we.first;
+            j.axis = kp.mapping.axis; j.perp_offset = kp.perp_offset; j.taps = we->taps;
+            j.weights = we->weights; j.inv_wsum = we->inv; j.first = we->first;
             j.box_fx = j.box_fy = 1;
             size_t out_off;
             if (last) {
@@ -3397,9 +3401,9 @@ void Renderer::prof_mark(int kernel_class) {
     if (!profiling_) return;
     if (kernel_class == -1) { prof_marks_.clear(); prof_next_event_ = 0; }
     if (prof_next_event_ >= prof_events_.size()) {
-        cudaEvent_t e;
-        if (cudaEventCreate(&e) != cudaSuccess) return;
-        prof_events_.push_back(e);
+        Event e;
+        if (make(e, cudaEventCreateWithFlags, cudaEventDefault) != cudaSuccess) return;
+        prof_events_.push_back(std::move(e));
     }
     cudaEvent_t e = prof_events_[prof_next_event_++];
     cudaEventRecord(e, stream_);
@@ -3420,8 +3424,11 @@ smr_status Renderer::comm_init(const uint8_t *id, int rank, int nranks) {
     CUDA_OK(cudaSetDevice(opts_.cuda_device));
     NcclId nid;
     memcpy(nid.b, id, 128);
-    int rc = g_nccl.CommInitRank(&nccl_comm_, nranks, nid, rank);
+    void *comm = nullptr;
+    int rc = g_nccl.CommInitRank(&comm, nranks, nid, rank);
     if (rc != 0) { set_error(std::string("ncclCommInitRank: ") + (g_nccl.GetErrorString ? g_nccl.GetErrorString(rc) : "error")); return SMR_ERR_CUDA; }
+    if (nccl_comm_) { cudaStreamSynchronize(comm_stream_); cudaStreamSynchronize(stream_); }   // as comm_destroy, for the one replaced
+    nccl_comm_.reset(comm);
     comm_rank_ = rank; comm_size_ = nranks;
     return SMR_OK;
 }
@@ -3498,7 +3505,9 @@ smr_status Renderer::comm_exchange(const smr_input_frame *frames, uint32_t n, co
 // place.  The only cross-GPU traffic of SMR_COMM_PEER_DIRECT besides the tile loads themselves.
 smr_status Renderer::comm_tick_barrier() {
     if (!barrier_word_) {
-        CUDA_OK(cudaMalloc(&barrier_word_, 256));
+        int32_t *word = nullptr;
+        CUDA_OK(cudaMalloc(&word, 256));
+        barrier_word_.reset(word);
         CUDA_OK(cudaMemsetAsync(barrier_word_, 0, 256, comm_stream_));
     }
     int rc = g_nccl.AllReduce(barrier_word_, barrier_word_, 1, /*ncclInt32*/ 2, /*ncclSum*/ 0, nccl_comm_, comm_stream_);
@@ -3553,10 +3562,11 @@ smr_status Renderer::peer_pool_alloc(size_t bytes, void **dev_ptr, uint8_t handl
     CUDA_OK(cudaSetDevice(opts_.cuda_device));
     void *p = nullptr;
     CUDA_OK(cudaMalloc(&p, bytes));   // its own allocation: an IPC handle names a whole cudaMalloc block
+    Owned<void *, cudaFree> owned(p);
     cudaIpcMemHandle_t h;
-    if (cudaIpcGetMemHandle(&h, p) != cudaSuccess) { cudaGetLastError(); cudaFree(p); set_error("cudaIpcGetMemHandle failed"); return SMR_ERR_CUDA; }
+    if (cudaIpcGetMemHandle(&h, p) != cudaSuccess) { cudaGetLastError(); set_error("cudaIpcGetMemHandle failed"); return SMR_ERR_CUDA; }
     memcpy(handle, &h, 64);
-    peer_own_.push_back(p);
+    peer_own_.push_back(std::move(owned));
     *dev_ptr = p;
     return SMR_OK;
 }
@@ -3570,34 +3580,24 @@ smr_status Renderer::peer_pool_open(const uint8_t handle[64], void **dev_ptr) {
     void *p = nullptr;
     cudaError_t e = cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess);
     if (e != cudaSuccess) { cudaGetLastError(); set_error(std::string("cudaIpcOpenMemHandle: ") + cudaGetErrorString(e)); return SMR_ERR_CUDA; }
-    peer_opened_.push_back(p);
+    peer_opened_.emplace_back(p);
     *dev_ptr = p;
     return SMR_OK;
 }
 
-smr_status Renderer::peer_pool_close(void *dev_ptr) {
-    std::lock_guard<std::mutex> g(mu_);
-    auto it = std::find(peer_opened_.begin(), peer_opened_.end(), dev_ptr);
-    if (it == peer_opened_.end()) return SMR_ERR_INVALID_ARGUMENT;
-    CUDA_OK(cudaSetDevice(opts_.cuda_device));
-    cudaStreamSynchronize(stream_);
-    if (comm_stream_) cudaStreamSynchronize(comm_stream_);
-    tmap_cache_.clear();   // descriptors of planes inside the mapping
-    cudaIpcCloseMemHandle(dev_ptr);
-    peer_opened_.erase(it);
-    return SMR_OK;
-}
+smr_status Renderer::peer_pool_close(void *dev_ptr) { return peer_pool_release(peer_opened_, dev_ptr); }
+smr_status Renderer::peer_pool_free(void *dev_ptr) { return peer_pool_release(peer_own_, dev_ptr); }
 
-smr_status Renderer::peer_pool_free(void *dev_ptr) {
+// Closes or frees a peer pool once no stream reads it
+template <class Pools> smr_status Renderer::peer_pool_release(Pools &pools, void *dev_ptr) {
     std::lock_guard<std::mutex> g(mu_);
-    auto it = std::find(peer_own_.begin(), peer_own_.end(), dev_ptr);
-    if (it == peer_own_.end()) return SMR_ERR_INVALID_ARGUMENT;
+    auto it = std::find_if(pools.begin(), pools.end(), [dev_ptr](const auto &p) { return (void *)p == dev_ptr; });
+    if (it == pools.end()) return SMR_ERR_INVALID_ARGUMENT;
     CUDA_OK(cudaSetDevice(opts_.cuda_device));
     cudaStreamSynchronize(stream_);
     if (comm_stream_) cudaStreamSynchronize(comm_stream_);
-    tmap_cache_.clear();
-    cudaFree(dev_ptr);
-    peer_own_.erase(it);
+    tmap_cache_.clear();   // descriptors of planes inside the pool
+    pools.erase(it);
     return SMR_OK;
 }
 
@@ -3607,8 +3607,7 @@ smr_status Renderer::comm_destroy() {
         cudaSetDevice(opts_.cuda_device);
         cudaStreamSynchronize(comm_stream_);   // the collectives run here
         cudaStreamSynchronize(stream_);
-        g_nccl.CommDestroy(nccl_comm_);
-        nccl_comm_ = nullptr;
+        nccl_comm_.reset();
     }
     return SMR_OK;
 }
