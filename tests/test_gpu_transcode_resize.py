@@ -8,7 +8,7 @@ import pytest
 
 import smelter_b200 as s
 from smelter_b200 import _ffi as F
-from tests.oracle_transcode import transcode_resize as oracle
+from tests.c_oracles import transcode_resize as oracle
 
 pytestmark = pytest.mark.gpu
 

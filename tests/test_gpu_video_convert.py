@@ -10,7 +10,7 @@ import pytest
 import smelter_b200 as s
 from oracle import oracle as orc
 from smelter_b200 import _ffi as F
-from tests.oracle_video_convert import nv12_to_rgba as oracle
+from tests.c_oracles import nv12_to_rgba as oracle
 from tests.test_color_conversion_space import yuv420_block_triples, yuv420_chroma_sums
 
 pytestmark = pytest.mark.gpu

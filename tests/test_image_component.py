@@ -18,7 +18,7 @@ from oracle import oracle as orc
 from smelter_b200 import _ffi as F
 from tests import harness
 from tests import layout_ref_image as LR
-from tests import oracle_image
+from tests import c_oracles
 from tests.parity import assert_identical, black, chroma_size, from_ref_layout, layouts_equal, node_texture, yuv_frame
 from tests.test_layout_independent import diff, product_layouts, ref_layouts
 
@@ -99,7 +99,7 @@ class Pair:
         ns = LR.LR.to_ns(pts)
         res = {k: (f.resolution.width, f.resolution.height) for k, f in frames.items()}
         layouts, (rw, rh) = self.ref.layouts(pts, res)
-        tex = {id(c): oracle_image.render_image(self.px[a][a.frame_at(ns, start)], w, h, m)
+        tex = {id(c): c_oracles.render_image(self.px[a][a.frame_at(ns, start)], w, h, m)
                for c, a, start, (w, h) in self.ref.image_nodes()}
         if isinstance(self.scene, IMG):
             return to_format(tex[id(self.scene)], self.out, self.fmt)
@@ -355,7 +355,7 @@ def test_image_oracle_at_equal_size_is_the_premultiply_oracle(mode):
     full[..., 3] = np.arange(256)[:, None]
     for src in (full, pixels(37, 23, 1, 5)[0], pixels(1, 1, 1, 6)[0]):
         h, w = src.shape[:2]
-        assert np.array_equal(oracle_image.render_image(src, w, h, mode), orc.add_premultiplied_alpha(src, mode))
+        assert np.array_equal(c_oracles.render_image(src, w, h, mode), orc.add_premultiplied_alpha(src, mode))
 
 
 # ---- GPU ------------------------------------------------------------------------------------------------------------

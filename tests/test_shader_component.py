@@ -21,7 +21,7 @@ import bench
 import smelter_b200 as s
 from smelter_b200 import _ffi as F
 from tests import layout_ref_shader as LS
-from tests import oracle_shader
+from tests import c_oracles
 from tests import test_web_view_component as TW
 from tests.test_gpu_bench_scenes import bench_frames
 from tests.test_image_component import pixels
@@ -154,8 +154,8 @@ class Pair(TW.Pair):
         if not isinstance(c, SH):
             return super().leaf_texture(c, frames, live)
         kids = [self.leaf_texture(k, frames, live, pts) for k in c.children]
-        return oracle_shader.render_shader(self.sources[c.shader_id], int(c.width), int(c.height), kids, pts,
-                                           param_bytes(c.shader_param), self.m)
+        return c_oracles.render_shader(self.sources[c.shader_id], int(c.width), int(c.height), kids, pts,
+                                       param_bytes(c.shader_param), self.m)
 
     def expected(self, pts, frames, stale=()):
         live = {k for k in frames if k not in stale}
@@ -354,8 +354,8 @@ def test_oracle_identity_shader_is_the_child():
             "{ return t.sample(0, in.tex_coords); }"
     px = TW.page(37, 23, 4, translucent=False)
     for m in (0, 1):
-        assert np.array_equal(oracle_shader.render_shader(ident, 37, 23, [px], mode=m), px)
-    assert not oracle_shader.render_shader(ident, 5, 4, [None]).any()
+        assert np.array_equal(c_oracles.render_shader(ident, 37, 23, [px], mode=m), px)
+    assert not c_oracles.render_shader(ident, 5, 4, [None]).any()
 
 
 # ---- GPU ------------------------------------------------------------------------------------------------------------

@@ -19,7 +19,7 @@ import pytest
 import smelter_b200 as s
 from smelter_b200 import _ffi as F
 from tests import layout_ref_image as LI
-from tests import oracle_svg
+from tests import c_oracles
 from tests import svg_standin
 from tests import test_shader_component as TS
 from tests import test_web_view_component as TW
@@ -73,7 +73,7 @@ class Pair(TWL.Pair):
         if isinstance(c, IMG) and c.image_id in self.svg:
             asset, fn = self.svg[c.image_id]
             w, h = LI.resolution(asset, c.width, c.height)
-            return oracle_svg.render_svg(fn(w, h), self.m)
+            return c_oracles.render_svg(fn(w, h), self.m)
         return super().leaf_texture(c, frames, live, pts)
 
     def expected(self, pts, frames, stale=()):
@@ -295,12 +295,12 @@ def test_oracle_conversion():
     the renderer accepts, which is what lets k_image take pass 1's bytes as pass 2's texel"""
     opaque = svg_standin.rasterize(40, 30)
     opaque[..., 3] = 255
-    assert np.array_equal(oracle_svg.render_svg(opaque, 0), opaque)
+    assert np.array_equal(c_oracles.render_svg(opaque, 0), opaque)
     raster = svg_standin.rasterize(67, 52)
-    assert np.array_equal(oracle_svg.render_svg(raster, 1), raster)
-    got = oracle_svg.render_svg(raster, 0)
+    assert np.array_equal(c_oracles.render_svg(raster, 1), raster)
+    got = c_oracles.render_svg(raster, 0)
     assert np.array_equal(got[..., 3], raster[..., 3]) and not got[raster[..., 3] == 0].any()
-    assert oracle_svg.same_size_taps_off_texel(16384) == 0
+    assert c_oracles.same_size_taps_off_texel(16384) == 0
 
 
 def test_standin_draws_partial_coverage_at_scale():
@@ -331,7 +331,7 @@ def test_exhaustive_conversion(mode):
     p.register_svg("full", size=(256, 256), fn=lambda w, h: full)
     p.update(IMG(image_id="full"))
     got = np.asarray(p.r.render(s.FrameSet(pts=0.0)).frames["output_1"].data.planes[0]).reshape(256, 256, 4)
-    exp = oracle_svg.render_svg(full, p.m)
+    exp = c_oracles.render_svg(full, p.m)
     assert np.array_equal(got, exp), np.argwhere(np.any(got != exp, axis=-1))[:8]
 
 

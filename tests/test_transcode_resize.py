@@ -8,7 +8,7 @@ import numpy as np
 import pytest
 
 from smelter_b200 import _ffi as F
-from tests.oracle_transcode import transcode_resize
+from tests.c_oracles import transcode_resize
 
 f32 = np.float32
 ALGOS = (F.SCALE_NEAREST, F.SCALE_BILINEAR, F.SCALE_LANCZOS3)

@@ -11,7 +11,7 @@ import pytest
 
 from oracle import oracle as orc
 from smelter_b200 import _ffi as F
-from tests.oracle_video_convert import nv12_to_rgba
+from tests.c_oracles import nv12_to_rgba
 from tests.test_color_conversion_space import (CHUNK, N, SIDE, coverage, report, tie_rule, upsample2_sum16,
                                                yuv420_block_triples, yuv420_chroma_sums)
 

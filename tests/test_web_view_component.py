@@ -19,8 +19,7 @@ from oracle import oracle as orc
 from smelter_b200 import _ffi as F
 from tests import harness
 from tests import layout_ref_web as LW
-from tests import oracle_image
-from tests import oracle_web
+from tests import c_oracles
 from tests.parity import assert_identical, black, chroma_size, from_ref_layout, layouts_equal, node_texture, nv12_frame, yuv_frame
 from tests.test_image_component import pixels
 from tests.test_layout_independent import diff, product_layouts, ref_layouts
@@ -120,7 +119,7 @@ class Pair:
         if isinstance(c, IMG):
             px = self.px[c.image_id]
             w, h = LW.LI.resolution(self.ref.images[c.image_id], c.width, c.height)
-            return oracle_image.render_image(px, w, h, self.m)
+            return c_oracles.render_image(px, w, h, self.m)
         if isinstance(c, TXT):
             return text_texture(c, self.m)
         return self.web_texture(c, frames, live)
@@ -129,7 +128,7 @@ class Pair:
         inst = self.ref.webs.get(c.instance_id) or self.gone[c.instance_id]   # an unregistered instance a scene still shows
         prev = self.tex.get(id(c), np.zeros((inst.height, inst.width, 4), np.uint8))
         kids = [self.leaf_texture(k, frames, live) for k in c.children]
-        t = oracle_web.render_web(prev, self.pages.get(c.instance_id), kids, self.rects[c.instance_id], inst.embedding, self.m)
+        t = c_oracles.render_web(prev, self.pages.get(c.instance_id), kids, self.rects[c.instance_id], inst.embedding, self.m)
         self.tex[id(c)] = t
         return t
 
@@ -293,9 +292,9 @@ def test_oracle_page_alone_is_the_swapped_page():
     """an opaque page with no child is its own bytes, b and r swapped, in both modes"""
     pg = page(37, 23, 4, translucent=False)
     for m in (orc.MODE_GPU_OPTIMIZED, orc.MODE_CPU_OPTIMIZED):
-        got = oracle_web.render_web(np.zeros((23, 37, 4), np.uint8), pg, [], [], OVER, m)
+        got = c_oracles.render_web(np.zeros((23, 37, 4), np.uint8), pg, [], [], OVER, m)
         assert np.array_equal(got, pg[..., [2, 1, 0, 3]])
-    assert not oracle_web.render_web(np.zeros((4, 4, 4), np.uint8), None, [], [], OVER).any()
+    assert not c_oracles.render_web(np.zeros((4, 4, 4), np.uint8), None, [], [], OVER).any()
 
 
 # ---- GPU ------------------------------------------------------------------------------------------------------------

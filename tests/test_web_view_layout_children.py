@@ -8,7 +8,7 @@ import pytest
 
 import smelter_b200 as s
 from tests import layout_ref_web_layout as LWL
-from tests import oracle_web
+from tests import c_oracles
 from tests import test_shader_component as TS
 from tests import test_web_view_component as TW
 from tests.test_image_component import pixels
@@ -42,7 +42,7 @@ class Pair(TS.Pair):
         inst = self.ref.webs.get(c.instance_id) or self.gone[c.instance_id]
         prev = self.tex.get(id(c), TW.np.zeros((inst.height, inst.width, 4), TW.np.uint8))
         kids = [self.leaf_texture(k, frames, live, pts) for k in c.children]
-        t = oracle_web.render_web(prev, self.pages.get(c.instance_id), kids, self.rects[c.instance_id], inst.embedding, self.m)
+        t = c_oracles.render_web(prev, self.pages.get(c.instance_id), kids, self.rects[c.instance_id], inst.embedding, self.m)
         self.tex[id(c)] = t
         return t
 

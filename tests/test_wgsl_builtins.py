@@ -15,7 +15,7 @@ import numpy as np
 import pytest
 
 import smelter_b200 as s
-from tests import oracle_shader, oracle_wgsl
+from tests import c_oracles
 from tests import test_web_view_component as TW
 from tests.test_wgsl_shader import HEADER, Pair, host, status, with_fs
 
@@ -707,8 +707,8 @@ static void wo_vs(const wo_base &, const void *, const float *p, const float *tc
 
 
 def render_vs(restatement, W, H, children, pts=0.0, params=b"", mode=0):
-    """oracle_wgsl.render through orc_render_wgsl_vs, so that wo_vs can sample the children"""
-    L = oracle_wgsl.lib(restatement)
+    """c_oracles.render_wgsl through orc_render_wgsl_vs, so that wo_vs can sample the children"""
+    L = c_oracles.wgsl_lib(restatement)
     L.orc_render_wgsl_vs.argtypes = L.orc_render_wgsl.argtypes
     out = np.zeros((H, W, 4), np.uint8)
     kids = [None if c is None else np.ascontiguousarray(c, np.uint8) for c in children]
@@ -716,7 +716,7 @@ def render_vs(restatement, W, H, children, pts=0.0, params=b"", mode=0):
     cw = (C.c_int * max(1, len(kids)))(*[1 if c is None else c.shape[1] for c in kids])
     ch = (C.c_int * max(1, len(kids)))(*[1 if c is None else c.shape[0] for c in kids])
     pb = C.create_string_buffer(bytes(params), max(1, len(params)))
-    L.orc_render_wgsl_vs(W, H, int(mode), float(oracle_shader.time_of(pts)), pb if params else None, ptrs, cw, ch, len(kids),
+    L.orc_render_wgsl_vs(W, H, int(mode), float(c_oracles.time_of(pts)), pb if params else None, ptrs, cw, ch, len(kids),
                          out.ctypes.data)
     return out
 

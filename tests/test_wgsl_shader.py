@@ -16,7 +16,7 @@ import pytest
 
 import smelter_b200 as s
 from smelter_b200 import _ffi as F
-from tests import oracle_wgsl
+from tests import c_oracles
 from tests import test_shader_component as TS
 from tests import test_web_view_component as TW
 from tests.test_oracle_kat import GRADIENT_RGBA_EXPECTED, GRADIENT_YUV_EXPECTED
@@ -252,7 +252,7 @@ class Pair(TS.Pair):
         if isinstance(c, SH) and c.shader_id in self.wgsl:
             kids = [self.leaf_texture(k, frames, live, pts) for k in c.children]
             pb = TS.param_bytes(c.shader_param)
-            return oracle_wgsl.render(self.wgsl[c.shader_id][0], int(c.width), int(c.height), kids, pts, pb.ljust(256, b"\0"), self.m)
+            return c_oracles.render_wgsl(self.wgsl[c.shader_id][0], int(c.width), int(c.height), kids, pts, pb.ljust(256, b"\0"), self.m)
         return super().leaf_texture(c, frames, live, pts)
 
 

@@ -1,12 +1,10 @@
 /* transcode_oracle.c -- CPU oracle of smr_transcode_resize: gpu-video's transcoder resize (vulkan_transcoder/shader.wgsl
- * `main` and its samplers) restated per output pixel, for one rendition.  Test infrastructure (tests/oracle_transcode.py
+ * `main` and its samplers) restated per output pixel, for one rendition.  Test infrastructure (tests/c_oracles.py
  * builds it with -ffp-contract=off, so every f32 operation rounds on its own, as DESIGN.md NC-10 requires).
  *
  * Texels are fetched as v / 255 (NC-1) and stored as rint(clamp(x) * 255) (NC-2); sin is evaluated in fp64 and rounded
  * to f32 (NC-8).  Written from the shader, not from the kernel: coordinates and weights are evaluated here per pixel. */
-#include <math.h>
-#include <stddef.h>
-#include <stdint.h>
+#include "oracle_nc.h"
 
 typedef struct {
     const uint8_t *p;
@@ -15,12 +13,6 @@ typedef struct {
 } plane;
 
 static float fetch(const plane *t, int x, int y, int c) { return (float)t->p[(size_t)y * t->pitch + x * t->ch + c] / 255.0f; }
-
-static uint8_t store(float x) {
-    if (!(x > 0.0f)) return 0;        /* NaN and below: 0 */
-    if (x > 1.0f) x = 1.0f;
-    return (uint8_t)rintf(x * 255.0f);
-}
 
 static float sinc(float x) {
     if (fabsf(x) < 1e-6f) return 1.0f;
@@ -80,13 +72,13 @@ void orc_transcode_resize(const uint8_t *y, int y_pitch, const uint8_t *uv, int 
     for (int oyy = 0; oyy < out_h; oyy++) {
         for (int ox = 0; ox < out_w; ox++) {
             const float fx = ((float)ox + 0.5f) / (float)out_w, fy = ((float)oyy + 0.5f) / (float)out_h;
-            oy[(size_t)oyy * out_w + ox] = store(sample(&ty, algo, fx, fy, 0));
+            oy[(size_t)oyy * out_w + ox] = store_unorm(sample(&ty, algo, fx, fy, 0));
             if (ox % 2 == 0 && oyy % 2 == 0) {
                 const int ux = ox / 2, uy = oyy / 2, uw = out_w / 2, uh = out_h / 2;
                 const float gx = ((float)ux + 0.5f) / (float)uw, gy = ((float)uy + 0.5f) / (float)uh;
                 uint8_t *d = ouv + ((size_t)uy * uw + ux) * 2;
-                d[0] = store(sample(&tuv, algo, gx, gy, 0));
-                d[1] = store(sample(&tuv, algo, gx, gy, 1));
+                d[0] = store_unorm(sample(&tuv, algo, gx, gy, 0));
+                d[1] = store_unorm(sample(&tuv, algo, gx, gy, 1));
             }
         }
     }

@@ -5,7 +5,7 @@
  *   wo_vs(b, params, position, tex_coords, pos, vary)          vs_main
  *   wo_fs(b, params, tex, fragment position, vary, out) -> bool fs_main (false: discard)
  * between this file's two parts (WO_PRE defined: the types; not defined: the rasteriser).  It is compiled after
- * shader_oracle_shim.h (tests/oracle_shader.py), whose sampling and blending it uses.  The rasteriser restates the
+ * shader_oracle_shim.h (tests/c_oracles.py), whose sampling and blending it uses.  The rasteriser restates the
  * contract of smr_register_wgsl_shader (include/smelter_b200.h) independently of the product's kernel:
  *   window x = fmaf(x/w, W/2, W/2), y = fmaf(-(y/w), H/2, H/2), snapped to 1/256 px; a plane with a vertex of w <= 0 or a
  *   window coordinate beyond 2^20 px is not drawn; triangles (0,1,2), (2,3,0); the doubled area from the snapped
@@ -84,7 +84,7 @@ extern "C" void orc_render_wgsl(int W, int H, int mode, float time, const void *
                     }
                     float fpos[4] = {(float)x + 0.5f, (float)y + 0.5f, depth, s};
                     float4 c;
-                    if (wo_fs(b, params, t, fpos, vary, c)) blend(out + ((size_t)y * W + x) * 4, c, mode);
+                    if (wo_fs(b, params, t, fpos, vary, c)) blend_fragment(out + ((size_t)y * W + x) * 4, c, mode);
                 }
         }
     }
