@@ -265,7 +265,8 @@ typedef enum {
     SMR_KERNEL_TRANSCODE = 12,     /* transcoder renditions (k_transcode, smr_transcode_resize) */
     SMR_KERNEL_VIDEO_CONVERT = 13, /* NV12 -> RGBA frame converter (k_video_nv12_to_rgba, smr_video_nv12_to_rgba); the
                                       reverse converter is k_output and counts as SMR_KERNEL_OUTPUT */
-    SMR_KERNEL_CLASSES = 14
+    SMR_KERNEL_DEINTERLACE = 14,   /* deinterlaced input planes (k_deinterlace, smr_set_input_deinterlace) */
+    SMR_KERNEL_CLASSES = 15
 } smr_kernel_class;
 typedef struct {
     double total_ms[SMR_KERNEL_CLASSES];
@@ -280,6 +281,48 @@ void smr_destroy(smr_renderer *r);
 /* Renderer::register_input / unregister_input                       state.rs:102-113 */
 smr_status smr_register_input(smr_renderer *r, const char *input_id);
 smr_status smr_unregister_input(smr_renderer *r, const char *input_id);
+
+/* Deinterlacing of an interlaced input (new: the reference has no deinterlacer).  Interlaced sources (1080i SDI capture,
+ * PAFF / MBAFF broadcast H.264) deliver woven frames: two fields, captured half a frame period apart, on alternate rows.
+ * Converted and resampled as they are, moving content combs, and a downscale aliases the combs.  With a mode set, every
+ * frame of the input is deinterlaced on the GPU before anything reads it (the rest of the tick is unchanged).
+ * The rule, byte for byte (DESIGN.md NC-12): each plane of the frame (the three planes of planar formats, NV12's luma and
+ * interleaved chroma planes, the one plane of UYVY / YUYV / BGRA / ARGB / RGBA8) is processed on its own, byte by byte
+ * along its row bytes; row parity within the plane decides the field, the half-height chroma planes of 4:2:0 included.
+ * SMR_FIELD_TOP_FIRST keeps the even rows and rebuilds the odd ones, SMR_FIELD_BOTTOM_FIRST keeps the odd rows and
+ * rebuilds the even ones.  For a rebuilt row y: a = row y - 1 (row y + 1 when y - 1 is outside the plane), b = row y + 1
+ * (row y - 1 when y + 1 is outside the plane); a plane of one row is copied unchanged.
+ *   SMR_DEINTERLACE_FIELD: out = (a + b + 1) >> 1.
+ *   SMR_DEINTERLACE_MOTION_ADAPTIVE: c = the current row y, p, pa, pb = rows y, a and b of the previous frame;
+ *     m = max(|c - p|, |a - pa|, |b - pb|), out = m <= motion_threshold ? c : (a + b + 1) >> 1.  Without a previous frame
+ *     the rebuilt rows follow FIELD.
+ * The previous frame is the last frame of the input with another pts_ns, kept by the library as a copy (the caller may
+ * rewrite its planes once the tick that read them has retired).  A frame with the same pts_ns, format and size as the last
+ * one is the same frame (the queue repeats frames when an input is slower than the output): it gives the same bytes and
+ * does not advance the history.  A change of format or size clears the history, and so does a call here that changes
+ * the mode or the field order (a call that only changes the threshold keeps it); a tick in which the input has no live
+ * frame leaves it alone.  The setting lasts until it is changed, or until smr_unregister_input, which drops it and the
+ * history.  SMR_DEINTERLACE_OFF (the default) leaves the input exactly as without this call.
+ * A shim maps DeckLink's detected field dominance (bmdUpperFieldFirst: TOP_FIRST, bmdLowerFieldFirst: BOTTOM_FIRST) and
+ * turns the mode off for progressive display modes (see INTEGRATION.md).
+ * SMR_ERR_INVALID_ARGUMENT: a NULL id or cfg, an id that is not registered, an unknown mode or field order,
+ * motion_threshold above 255.  A host-only handle stores the setting. */
+typedef enum { SMR_DEINTERLACE_OFF = 0, SMR_DEINTERLACE_FIELD = 1, SMR_DEINTERLACE_MOTION_ADAPTIVE = 2 } smr_deinterlace_mode;
+typedef enum { SMR_FIELD_TOP_FIRST = 0, SMR_FIELD_BOTTOM_FIRST = 1 } smr_field_order;
+typedef struct {
+    int32_t mode;                  /* smr_deinterlace_mode */
+    int32_t field_order;           /* smr_field_order */
+    uint32_t motion_threshold;     /* MOTION_ADAPTIVE: T, 0 .. 255 */
+} smr_deinterlace;
+smr_status smr_set_input_deinterlace(smr_renderer *r, const char *input_id, const smr_deinterlace *cfg);
+/* inspection (needs a device; blocking): the planes the kernels of the most recent tick that had a live frame of the input
+ * read for it, after deinterlacing, copied into planes[p] (rows of the frame's row bytes, at pitch[p], 0 = tightly packed;
+ * host or device memory per mem_kind).  The plane sizes are those of the frame (smr_input_frame).  Valid once that tick
+ * has retired.  For an input without deinterlacing these are the library's copy of a host frame, or the caller's device
+ * planes as they are now.  SMR_ERR_INVALID_ARGUMENT: a NULL id, planes or pitch, a NULL plane the format has, an id that
+ * is not registered or has had no live frame since it was registered, an unknown mem_kind. */
+smr_status smr_debug_input_planes(smr_renderer *r, const char *input_id, void *const planes[3], const uint32_t pitch[3],
+                                  int32_t mem_kind);
 
 /* Renderer::register_renderer / unregister_renderer for RendererSpec::Image   state.rs:123-166, registry.rs:57-68
  * An image asset arrives decoded, as straight-alpha RGBA8 frames of width x height in HOST memory (PNG / JPEG / GIF

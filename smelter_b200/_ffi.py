@@ -231,8 +231,16 @@ class VideoColor(C.Structure):   # smr_video_color
     _fields_ = [("color_space", C.c_int32), ("color_range", C.c_int32)]
 
 
+DEINTERLACE_OFF, DEINTERLACE_FIELD, DEINTERLACE_MOTION_ADAPTIVE = 0, 1, 2
+FIELD_TOP_FIRST, FIELD_BOTTOM_FIRST = 0, 1
+
+
+class Deinterlace(C.Structure):   # smr_deinterlace
+    _fields_ = [("mode", C.c_int32), ("field_order", C.c_int32), ("motion_threshold", C.c_uint32)]
+
+
 KERNEL_CLASSES = ["convert", "weights", "resample_box", "resample_first", "resample_last", "composite", "output",
-                  "fill", "resample_fused", "image", "web", "shader", "transcode", "video_convert"]
+                  "fill", "resample_fused", "image", "web", "shader", "transcode", "video_convert", "deinterlace"]
 
 
 class KernelTimes(C.Structure):
@@ -240,7 +248,8 @@ class KernelTimes(C.Structure):
 
 
 EXPORTS = [
-    "smr_create", "smr_destroy", "smr_register_input", "smr_unregister_input", "smr_register_image", "smr_unregister_image",
+    "smr_create", "smr_destroy", "smr_register_input", "smr_unregister_input", "smr_set_input_deinterlace",
+    "smr_debug_input_planes", "smr_register_image", "smr_unregister_image",
     "smr_register_svg_image",
     "smr_register_web_renderer", "smr_unregister_web_renderer", "smr_web_set_frame", "smr_web_set_child_rects", "smr_register_shader", "smr_unregister_shader", "smr_register_wgsl_shader", "smr_update_scene",
     "smr_unregister_output", "smr_set_layouts", "smr_render", "smr_render_begin", "smr_render_end", "smr_preprocess_frame", "smr_premultiply_rgba8", "smr_transcode_resize", "smr_video_nv12_to_rgba", "smr_video_rgba_to_nv12", "smr_render_text", "smr_debug_partition", "smr_debug_tile_plan", "smr_debug_weights", "smr_debug_sincos", "smr_debug_transcode_taps", "smr_debug_fused_jobs", "smr_debug_resample_stages", "smr_debug_composite_layers", "smr_debug_interior", "smr_output_plane_sizes",
@@ -268,6 +277,8 @@ def lib():
     L.smr_destroy.restype = None
     L.smr_register_input.argtypes = [vp, C.c_char_p]
     L.smr_unregister_input.argtypes = [vp, C.c_char_p]
+    L.smr_set_input_deinterlace.argtypes = [vp, C.c_char_p, C.POINTER(Deinterlace)]
+    L.smr_debug_input_planes.argtypes = [vp, C.c_char_p, C.POINTER(C.c_void_p * 3), C.POINTER(C.c_uint32 * 3), C.c_int32]
     L.smr_register_image.argtypes = [vp, C.c_char_p, C.POINTER(ImageSpec)]
     L.smr_unregister_image.argtypes = [vp, C.c_char_p]
     L.smr_register_svg_image.argtypes = [vp, C.c_char_p, C.POINTER(SvgSpec)]

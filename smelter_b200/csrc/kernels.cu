@@ -12,6 +12,7 @@
 //   k_fill        r8/rg8_fill_value.wgsl (black frame)                                  (K6)
 //   k_transcode   gpu-video's vulkan_transcoder/shader.wgsl: NV12 -> up to eight NV12 renditions (transcode.cuh)
 //   k_video_nv12_to_rgba  gpu-video's nv12_to_rgba.wgsl: NV12 -> RGBA8 at any size (video_convert.cuh)
+//   k_deinterlace field / motion-adaptive deinterlacing of interlaced input planes (deinterlace.cuh; the reference has none)
 //
 // Numeric contract: identical to oracle/smelter_oracle.c (DESIGN.md section 3).  Compiled with
 // -fmad=false: only explicit fmaf() is fused, every other operation rounds separately, division and
@@ -1534,6 +1535,9 @@ int launch_output(const OutputJob &job, Stream s) {
 
 // gpu-video's NV12 -> RGBA converter (smr_video_nv12_to_rgba, NC-11)
 #include "video_convert.cuh"
+
+// the deinterlacers of smr_set_input_deinterlace (NC-12)
+#include "deinterlace.cuh"
 
 // ------------------------------------------------------------------------------------------------
 // FramePreProcessor (state/frame_pre_processor.rs): K1..K4 to RGBA8, optional rescale (rgba_rescale.wgsl, blend: None)

@@ -313,6 +313,28 @@ struct VideoConvertJob {
 };
 constexpr int kVideoConvertTileX = 32, kVideoConvertTileY = 8;   // threads per block
 
+// One plane of a deinterlaced input (smr_set_input_deinterlace, DESIGN.md NC-12), processed byte by byte along its rows.
+// Row parity decides the field: rows of parity `rebuild` are rebuilt from the rows above and below, the others are kept.
+struct DeinterlaceJob {
+    const uint8_t *cur;           // the frame as the tick reads it (the caller's device plane or the library's staged copy)
+    const uint8_t *prev;          // the previous frame's plane (MOTION_ADAPTIVE history, 16-byte aligned rows); nullptr: FIELD
+    uint8_t *out;                 // the deinterlaced plane: 16-byte aligned rows
+    uint8_t *hist;                // the next history, a copy of `cur` (16-byte aligned rows); nullptr: not written
+    int32_t cur_pitch, prev_pitch, out_pitch, hist_pitch;
+    int32_t row_bytes, rows;
+    int32_t rebuild;              // 1: TOP_FIRST (odd rows rebuilt), 0: BOTTOM_FIRST (even rows rebuilt)
+    uint32_t threshold;           // MOTION_ADAPTIVE: T, 0 .. 255
+    int32_t tiles_x;              // blocks per row of tiles
+};
+// A block owns kDeinterlaceTileX 16-byte columns and kDeinterlaceTileY runs of kDeinterlaceRun row pairs of one job; a
+// thread one column of one run
+constexpr int kDeinterlaceTileX = 32, kDeinterlaceTileY = 8, kDeinterlaceRun = 4;
+inline int deinterlace_tiles_x(int row_bytes) { return (row_bytes + 16 * kDeinterlaceTileX - 1) / (16 * kDeinterlaceTileX); }
+inline int deinterlace_tiles(int row_bytes, int rows) {
+    const int pairs = (rows + 1) / 2, per_block = kDeinterlaceTileY * kDeinterlaceRun;
+    return deinterlace_tiles_x(row_bytes) * ((pairs + per_block - 1) / per_block);
+}
+
 // host tables pushed once per device (numeric contract NC-1/3/4)
 void upload_tables(const float *u8n, const float *srgb_dec, const float *srgb_enc_thr);
 // the device tables of node_sample.cuh in this module (c_u8n, c_dec, c_thr, c_yl, c_enc1): addresses and bytes, for the
@@ -355,6 +377,9 @@ int launch_output(const OutputJob &job, Stream s);
 int launch_transcode(const TranscodeLaunch &L, int n_blocks, Stream s);
 // k_video_nv12_to_rgba: a thread per 2 x 2 pixel quad when the target has the source's size, a thread per pixel otherwise
 int launch_video_nv12_to_rgba(const VideoConvertJob &J, Stream s);
+// k_deinterlace: every job of jobs_dev in one launch; job i owns the blocks [tile_begin_dev[i], tile_begin_dev[i + 1]) of
+// the grid (deinterlace_tiles of each job, prefix sums), n_tiles = tile_begin[n_jobs]
+int launch_deinterlace(const DeinterlaceJob *jobs_dev, const int32_t *tile_begin_dev, int n_jobs, int n_tiles, Stream s);
 int launch_fill_yuv(uint8_t *p0, uint8_t *p1, uint8_t *p2, int pitch0, int pitch1, int pitch2, int w, int h,
                     int out_format, uint8_t y, uint8_t u, uint8_t v, Stream s);
 const char *last_launch_error();

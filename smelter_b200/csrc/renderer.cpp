@@ -405,6 +405,8 @@ struct FrameView {
         size_t span() const { return pitch * (rows - 1) + row_bytes; }   // first to last byte of the plane
     } plane[3];
 };
+// row bytes and rows of plane `plane` of a width x height frame of format `fmt`; false: the format has no such plane
+static bool plane_layout(int fmt, uint32_t w, uint32_t h, int plane, size_t &row_bytes, size_t &rows);
 
 // ------------------------------------------------------------------------------------------------
 class Renderer {
@@ -415,6 +417,8 @@ class Renderer {
 
     smr_status register_input(const char *id);
     smr_status unregister_input(const char *id);
+    smr_status set_input_deinterlace(const char *id, const smr_deinterlace *cfg);
+    smr_status debug_input_planes(const char *id, void *const planes[3], const uint32_t pitch[3], int32_t mem_kind);
     smr_status register_image(const char *id, const smr_image_spec *spec);
     smr_status register_svg_image(const char *id, const smr_svg_spec *spec);
     smr_status unregister_image(const char *id);
@@ -458,6 +462,15 @@ class Renderer {
     std::mutex mu_;
 
   private:
+    // MOTION_ADAPTIVE's history: library copies of the input's last two frames of distinct pts, in hist[last] (the last
+    // frame) and hist[last ^ 1] (the one before it)
+    struct DeinterlaceHistory {
+        int frames = 0;         // distinct frames held: 0, 1 or 2
+        int last = 0;
+        uint64_t pts = 0;       // the last frame's pts, format and size
+        int32_t format = 0;
+        uint32_t width = 0, height = 0;
+    };
     struct Input {
         bool has_frame = false;
         dev::Tex tex;           // planes as they sit in HBM
@@ -465,6 +478,11 @@ class Renderer {
         Resolution res;
         int node_tex = -1;      // index in the tick's texture table of the materialised RGBA8 node texture
         int raw_tex = -1;       // index of the virtual (fused K1/K2) texture
+        int32_t format = -1;    // smr_frame_format of the last live frame (-1: none since registration)
+        smr_deinterlace deint = {SMR_DEINTERLACE_OFF, SMR_FIELD_TOP_FIRST, 10};
+        DeinterlaceHistory hist;
+        DevBuf deint_out[kTicksInFlight][3];   // the deinterlaced planes `tex` points at, one set per tick in flight
+        DevBuf hist_planes[2][3];
     };
     // A component node of an output's scene: its node texture as a layout child (premultiplied TEX_RGBA8, always live) and
     // the device memory behind it, allocated and freed in the order of stream_, so the ticks submitted before a scene update
@@ -596,6 +614,7 @@ class Renderer {
     smr_status read_frame(const smr_input_frame &f, FrameView &v);
     template <class Use> smr_status select_inputs(uint64_t pts, const smr_input_frame *in, uint32_t n_in, Use use);
     smr_status upload_input(Input &I, const smr_input_frame &f);
+    smr_status plan_deinterlace(Input &I, const smr_input_frame &f, FrameView &v);
     struct LayoutEval {
         std::vector<Input *> child_in;                      // the Input behind each child; nullptr: the empty view
         std::vector<std::optional<Resolution>> child_res;
@@ -713,6 +732,12 @@ class Renderer {
         std::map<std::tuple<int, uint32_t, uint32_t, uint32_t, uint32_t, int, int>, int> resample_cache;
         std::vector<FusedLaunch> fused_launches;
         std::vector<NodeLaunch> node_launches;   // the text, image, web and shader launches (pack_params)
+        // k_deinterlace: one job per plane of the deinterlaced inputs, and each input's history before the tick planned it
+        // (restored when the tick fails before its launches)
+        std::vector<dev::DeinterlaceJob> deint;
+        std::vector<std::pair<Input *, DeinterlaceHistory>> deint_history;
+        size_t deint_off, deint_begin_off;
+        int deint_tiles;
         size_t stage_off[3], weights_off, fused_off, composites_off;   // the packed job arrays in the parameter arena
         uint64_t launches, direct_tiles;
         bool nodes_enqueued;                  // the node launches before the conversions
@@ -723,6 +748,8 @@ class Renderer {
             composites.clear(); outputs.clear(); fills.clear(); d2h.clear(); texts.clear(); images.clear(); webs.clear(); shaders.clear(); phases.clear();
             resample_cache.clear();
             fused_launches.clear(); node_launches.clear();
+            deint.clear(); deint_history.clear();
+            deint_tiles = 0;
             launches = direct_tiles = 0;
             nodes_enqueued = false;
         }
@@ -941,6 +968,44 @@ smr_status Renderer::unregister_input(const char *id) {
     std::lock_guard<std::mutex> g(mu_);
     if (!host_only_) { cudaSetDevice(opts_.cuda_device); drain(); }
     inputs_.erase(id);
+    return SMR_OK;
+}
+
+smr_status Renderer::set_input_deinterlace(const char *id, const smr_deinterlace *cfg) {
+    if (!id || !cfg) return SMR_ERR_INVALID_ARGUMENT;
+    std::lock_guard<std::mutex> g(mu_);
+    auto it = inputs_.find(id);
+    if (it == inputs_.end()) { set_error(std::string("input \"") + id + "\" is not registered"); return SMR_ERR_INVALID_ARGUMENT; }
+    if (cfg->mode < SMR_DEINTERLACE_OFF || cfg->mode > SMR_DEINTERLACE_MOTION_ADAPTIVE) { set_error("unknown deinterlace mode"); return SMR_ERR_INVALID_ARGUMENT; }
+    if (cfg->field_order != SMR_FIELD_TOP_FIRST && cfg->field_order != SMR_FIELD_BOTTOM_FIRST) { set_error("unknown field order"); return SMR_ERR_INVALID_ARGUMENT; }
+    if (cfg->motion_threshold > 255) { set_error("motion threshold above 255"); return SMR_ERR_INVALID_ARGUMENT; }
+    Input &I = it->second;
+    if (cfg->mode != I.deint.mode || cfg->field_order != I.deint.field_order) I.hist = DeinterlaceHistory();
+    I.deint = *cfg;
+    return SMR_OK;
+}
+
+// inspection: the planes the last tick with a live frame of the input read for it, copied out on stream_ after that tick
+smr_status Renderer::debug_input_planes(const char *id, void *const planes[3], const uint32_t pitch[3], int32_t mem_kind) {
+    if (!id || !planes || !pitch || (mem_kind != SMR_MEM_HOST && mem_kind != SMR_MEM_DEVICE)) return SMR_ERR_INVALID_ARGUMENT;
+    std::lock_guard<std::mutex> g(mu_);
+    auto it = inputs_.find(id);
+    if (it == inputs_.end() || it->second.format < 0) { set_error("no live frame of this input since it was registered"); return SMR_ERR_INVALID_ARGUMENT; }
+    const Input &I = it->second;
+    const uint8_t *src[3] = {I.tex.p0, I.tex.p1, I.tex.p2};
+    const size_t spitch[3] = {(size_t)I.tex.pitch0, (size_t)I.tex.pitch1, (size_t)I.tex.pitch2};
+    size_t row_bytes[3] = {}, rows[3] = {};
+    for (int p = 0; p < 3; p++) {
+        if (!plane_layout(I.format, (uint32_t)I.tex.width, (uint32_t)I.tex.height, p, row_bytes[p], rows[p])) continue;
+        if (!planes[p] || (pitch[p] && pitch[p] < row_bytes[p])) { set_error("a target plane is null or its pitch is shorter than a row"); return SMR_ERR_INVALID_ARGUMENT; }
+    }
+    if (smr_status st = need_device(); st != SMR_OK) return st;
+    for (int p = 0; p < 3; p++) {
+        if (!rows[p]) continue;
+        CUDA_OK(cudaMemcpy2DAsync(planes[p], pitch[p] ? pitch[p] : row_bytes[p], src[p], spitch[p], row_bytes[p], rows[p],
+                                  cudaMemcpyDefault, stream_));
+    }
+    CUDA_OK(cudaStreamSynchronize(stream_));
     return SMR_OK;
 }
 
@@ -1652,26 +1717,81 @@ template <class Use> smr_status Renderer::select_inputs(uint64_t pts, const smr_
     return SMR_OK;
 }
 
-// a live frame, checked and uploaded: host planes go to the slot's buffers on alternating copy streams
+static size_t align16(size_t n) { return (n + 15) & ~(size_t)15; }
+
+// a live frame, checked and uploaded: host planes go to the slot's buffers on alternating copy streams.  A deinterlaced
+// input's planes are staged at 16-byte aligned pitches, which k_deinterlace reads with 16-byte loads.
 smr_status Renderer::upload_input(Input &I, const smr_input_frame &f) {
     FrameView v;
     if (smr_status st = read_frame(f, v); st != SMR_OK) return st;
+    const bool deint = I.deint.mode != SMR_DEINTERLACE_OFF;
     for (int p = 0; p < 3 && f.mem_kind != SMR_MEM_DEVICE; p++) {
-        const FrameView::Plane &P = v.plane[p];
+        FrameView::Plane &P = v.plane[p];
         if (!P.p) continue;
+        const size_t pitch = deint ? align16(P.row_bytes) : P.row_bytes;
         DevBuf &buf = I.planes[slot_][p];
-        CUDA_OK(buf.ensure(P.row_bytes * P.rows));
+        CUDA_OK(buf.ensure(pitch * P.rows));
         cudaStream_t cs = (upload_rr_++ & 1) ? copy_stream2_ : copy_stream_;
-        if (P.pitch == P.row_bytes)   // tightly packed (the reference's bytes::Bytes planes): one linear DMA
+        if (P.pitch == P.row_bytes && pitch == P.row_bytes)   // tightly packed (the reference's bytes::Bytes planes): one linear DMA
             CUDA_OK(cudaMemcpyAsync(buf.p, P.p, P.row_bytes * P.rows, cudaMemcpyHostToDevice, cs));
         else
-            CUDA_OK(cudaMemcpy2DAsync(buf.p, P.row_bytes, P.p, P.pitch, P.row_bytes, P.rows, cudaMemcpyHostToDevice, cs));
+            CUDA_OK(cudaMemcpy2DAsync(buf.p, pitch, P.p, P.pitch, P.row_bytes, P.rows, cudaMemcpyHostToDevice, cs));
         uploaded_ = true;
         stats_.h2d_bytes += P.row_bytes * P.rows;
-        set_tex_plane(v.tex, p, buf.p, P.row_bytes);
+        P.p = buf.p; P.pitch = pitch;
+        set_tex_plane(v.tex, p, buf.p, pitch);
     }
+    if (deint)
+        if (smr_status st = plan_deinterlace(I, f, v); st != SMR_OK) return st;
+    I.format = f.format;
     I.tex = v.tex;
     I.raw_tex = add_texture(v.tex, v.tex.kind == dev::TEX_YUV420 || v.tex.kind == dev::TEX_NV12 || v.tex.kind >= dev::TEX_YUV422);
+    return SMR_OK;
+}
+
+// The tick's k_deinterlace jobs for a live frame of a deinterlaced input (NC-12), one per plane; `v` is pointed at the
+// slot's deinterlaced planes.  MOTION_ADAPTIVE reads the previous frame from the history and, for a frame of a new pts,
+// copies the current one into the other history set, which becomes the last.  Two sets suffice: the ticks run in order on
+// stream_, and the set a tick writes is read only by later ticks.
+smr_status Renderer::plan_deinterlace(Input &I, const smr_input_frame &f, FrameView &v) {
+    DeinterlaceHistory &H = I.hist;
+    plan_.deint_history.push_back({&I, H});
+    int prev_set = -1;
+    DevBuf *next = nullptr;
+    if (I.deint.mode == SMR_DEINTERLACE_MOTION_ADAPTIVE) {
+        if (H.frames && (H.format != f.format || H.width != f.width || H.height != f.height)) H = DeinterlaceHistory();
+        const bool repeat = H.frames && H.pts == f.pts_ns;   // the same frame again: same bytes, history unchanged
+        if (repeat) {
+            prev_set = H.frames == 2 ? (H.last ^ 1) : -1;
+        } else {
+            prev_set = H.frames ? H.last : -1;
+            next = I.hist_planes[H.last ^ 1];
+            H.last ^= 1;
+            H.frames = std::min(H.frames + 1, 2);
+            H.pts = f.pts_ns; H.format = f.format; H.width = f.width; H.height = f.height;
+        }
+    }
+    for (int p = 0; p < 3; p++) {
+        const FrameView::Plane &P = v.plane[p];
+        if (!P.p) continue;
+        const size_t pitch = align16(P.row_bytes);
+        DevBuf &out = I.deint_out[slot_][p];
+        CUDA_OK(out.ensure(pitch * P.rows));
+        dev::DeinterlaceJob j{};
+        j.cur = P.p; j.cur_pitch = (int)P.pitch;
+        if (prev_set >= 0) { j.prev = I.hist_planes[prev_set][p].p; j.prev_pitch = (int)pitch; }
+        j.out = out.p; j.out_pitch = (int)pitch;
+        if (next) {
+            CUDA_OK(next[p].ensure(pitch * P.rows));
+            j.hist = next[p].p; j.hist_pitch = (int)pitch;
+        }
+        j.row_bytes = (int)P.row_bytes; j.rows = (int)P.rows;
+        j.rebuild = I.deint.field_order == SMR_FIELD_TOP_FIRST ? 1 : 0;
+        j.threshold = I.deint.motion_threshold;
+        j.tiles_x = dev::deinterlace_tiles_x(j.row_bytes);
+        plan_.deint.push_back(j);
+        set_tex_plane(v.tex, p, out.p, pitch);
+    }
     return SMR_OK;
 }
 
@@ -2915,6 +3035,7 @@ smr_status Renderer::render_begin(uint64_t pts, const smr_input_frame *in, uint3
             if (r.plan_.nodes_enqueued) return;
             for (TextNode *t : r.plan_.texts) t->rendered = false;
             for (ImageNode *n : r.plan_.images) n->held = n->held_before;
+            for (auto &h : r.plan_.deint_history) h.first->hist = h.second;
         }
     } guard{*this};
     smr_status st = plan_tick(pts, in, n_in, out, n_out);
@@ -3091,6 +3212,14 @@ smr_status Renderer::pack_params() {
     }
     plan_.fused_off = param_put_all(plan_.fused, &FusedRec::job);
     plan_.composites_off = param_put_all(plan_.composites, &CompositeRec::job);   // read by k_composite_multi
+    if (!plan_.deint.empty()) {   // the deinterlace jobs and the prefix table of their blocks
+        plan_.deint_off = param_put(plan_.deint.data(), sizeof(dev::DeinterlaceJob) * plan_.deint.size());
+        std::vector<int32_t> begin(plan_.deint.size() + 1, 0);
+        for (size_t i = 0; i < plan_.deint.size(); i++)
+            begin[i + 1] = begin[i] + dev::deinterlace_tiles(plan_.deint[i].row_bytes, plan_.deint[i].rows);
+        plan_.deint_tiles = begin.back();
+        plan_.deint_begin_off = param_put(begin.data(), sizeof(int32_t) * begin.size());
+    }
     for (WebNode *n : plan_.webs) {   // the children's textures, frame-arena addresses resolved
         for (size_t i = 0; i < n->planes.size(); i++)
             if (n->plane_child[i] >= 0) n->planes[i].tex = packed_node_tex(*n->owner, n->params.children[n->plane_child[i]]);
@@ -3152,7 +3281,8 @@ smr_status Renderer::pack_params() {
     return SMR_OK;
 }
 
-// Enqueues the tick's kernels on stream_, in this order: the text nodes, the image nodes and the web nodes of depth 1 (they
+// Enqueues the tick's kernels on stream_, in this order: k_deinterlace (it rewrites inputs before anything reads them); the
+// text nodes, the image nodes and the web nodes of depth 1 (they
 // read inputs, text and image nodes only); k_convert, k_weights, the fused resamples; per phase p, its generic resample
 // passes, its composite (the last phase's: ONE launch for every output) and then, after its layout nodes of depth p + 1, the
 // shader nodes of that depth (one launch per shader) and its web nodes; the output jobs; the fills.
@@ -3175,6 +3305,9 @@ smr_status Renderer::launch_tick() {
         return true;
     };
     prof_mark(-1);
+    if (!plan_.deint.empty() &&
+        !launched(dev::launch_deinterlace((const dev::DeinterlaceJob *)(pd + plan_.deint_off), (const int32_t *)(pd + plan_.deint_begin_off),
+                                          (int)plan_.deint.size(), plan_.deint_tiles, stream_), SMR_KERNEL_DEINTERLACE)) return SMR_ERR_CUDA;
     if (!launch_nodes(-1)) return SMR_ERR_CUDA;
     plan_.nodes_enqueued = true;
     for (auto &cv : plan_.convert_jobs) {
@@ -3737,6 +3870,12 @@ void smr_destroy(smr_renderer *r) { delete r; }
 
 smr_status smr_register_input(smr_renderer *r, const char *id) { SMR_GUARD(r->impl.register_input(id)) }
 smr_status smr_unregister_input(smr_renderer *r, const char *id) { SMR_GUARD(r->impl.unregister_input(id)) }
+smr_status smr_set_input_deinterlace(smr_renderer *r, const char *id, const smr_deinterlace *cfg) {
+    SMR_GUARD(r->impl.set_input_deinterlace(id, cfg))
+}
+smr_status smr_debug_input_planes(smr_renderer *r, const char *id, void *const planes[3], const uint32_t pitch[3], int32_t mem_kind) {
+    SMR_GUARD(r->impl.debug_input_planes(id, planes, pitch, mem_kind))
+}
 smr_status smr_register_image(smr_renderer *r, const char *id, const smr_image_spec *spec) { SMR_GUARD(r->impl.register_image(id, spec)) }
 smr_status smr_register_svg_image(smr_renderer *r, const char *id, const smr_svg_spec *spec) { SMR_GUARD(r->impl.register_svg_image(id, spec)) }
 smr_status smr_unregister_image(smr_renderer *r, const char *id) { SMR_GUARD(r->impl.unregister_image(id)) }

@@ -120,6 +120,35 @@ _FRAME_KIND = {"PlanarYuv420": F.FRAME_PLANAR_YUV420, "PlanarYuvJ420": F.FRAME_P
                "InterleavedUyvy422": F.FRAME_UYVY422, "InterleavedYuyv422": F.FRAME_YUYV422}
 
 
+def plane_shapes(fmt: int, width: int, height: int) -> List[Tuple[int, int]]:
+    """(rows, row bytes) of each plane of a width x height frame of smr_frame_format `fmt`, as the library reads it"""
+    cw, ch = width // 2, height // 2
+    if fmt in (F.FRAME_PLANAR_YUV420, F.FRAME_PLANAR_YUVJ420):
+        return [(height, width), (ch, cw), (ch, cw)]
+    if fmt == F.FRAME_NV12:
+        return [(height, width), (ch, 2 * cw)]
+    if fmt == F.FRAME_PLANAR_YUV422:
+        return [(height, width), (height, cw), (height, cw)]
+    if fmt == F.FRAME_PLANAR_YUV444:
+        return [(height, width)] * 3
+    if fmt in (F.FRAME_UYVY422, F.FRAME_YUYV422):
+        return [(height, 4 * cw)]
+    if fmt in (F.FRAME_BGRA, F.FRAME_ARGB, F.FRAME_RGBA8):
+        return [(height, 4 * width)]
+    raise ValueError(f"unknown frame format {fmt}")
+
+
+class DeinterlaceMode:   # smr_deinterlace_mode
+    Off = F.DEINTERLACE_OFF
+    Field = F.DEINTERLACE_FIELD
+    MotionAdaptive = F.DEINTERLACE_MOTION_ADAPTIVE
+
+
+class FieldOrder:        # smr_field_order
+    TopFirst = F.FIELD_TOP_FIRST
+    BottomFirst = F.FIELD_BOTTOM_FIRST
+
+
 @dataclass
 class Frame:
     data: FrameData
@@ -621,6 +650,7 @@ class Renderer:
         if st != F.SMR_OK:
             raise RendererError(st, (self._lib.smr_last_error(None) or b"").decode())
         self._outputs: Dict[str, Tuple[Resolution, int]] = {}
+        self._input_geometry: Dict[str, Tuple[int, int, int]] = {}   # the last rendered frame's (format, width, height)
         self._svg_rasterizers = {}
         self.opts = opts
 
@@ -647,6 +677,30 @@ class Renderer:
 
     def unregister_input(self, input_id: str):
         self._check(self._lib.smr_unregister_input(self._h, input_id.encode()))
+        self._input_geometry.pop(input_id, None)
+
+    def set_input_deinterlace(self, input_id: str, mode: int, field_order: int = FieldOrder.TopFirst, motion_threshold: int = 10):
+        """deinterlace every frame of a registered interlaced input before the scene reads it (smr_set_input_deinterlace):
+        `mode` a DeinterlaceMode, `field_order` the FieldOrder of the source, `motion_threshold` MotionAdaptive's T (0 .. 255)"""
+        cfg = F.Deinterlace(int(mode), int(field_order), int(motion_threshold))
+        self._check(self._lib.smr_set_input_deinterlace(self._h, input_id.encode(), C.byref(cfg)))
+
+    def debug_input_planes(self, input_id: str) -> List[np.ndarray]:
+        """the planes the kernels of the last render with a live frame of the input read for it, after deinterlacing: one
+        (rows, row bytes) uint8 array per plane of the input's last frame passed to render / render_raw"""
+        if input_id not in self._input_geometry:
+            raise RendererError(1, f"no frame of input \"{input_id}\" was rendered")   # SMR_ERR_INVALID_ARGUMENT
+        planes = [np.empty(shape, np.uint8) for shape in plane_shapes(*self._input_geometry[input_id])]
+        ptrs = (C.c_void_p * 3)(*[p.ctypes.data for p in planes])
+        self._check(self._lib.smr_debug_input_planes(self._h, input_id.encode(), C.byref(ptrs), C.byref((C.c_uint32 * 3)()),
+                                                     F.MEM_HOST))
+        return planes
+
+    def _note_inputs(self, in_arr, n_in):
+        for i in range(n_in):
+            f = in_arr[i]
+            if f.input_id:
+                self._input_geometry[f.input_id.decode()] = (f.format, f.width, f.height)
 
     def register_image(self, image_id: str, frames, delays=None):
         """Renderer::register_renderer for an image that arrives decoded: `frames` is one (h, w, 4) uint8 straight-alpha
@@ -795,6 +849,7 @@ class Renderer:
                     out_arr[i].planes[p] = planes[p].ctypes.data
         st = self._lib.smr_render(self._h, _secs_to_ns(input.pts), in_arr, len(input.frames), out_arr, len(ids))
         self._check(st, RenderSceneError)
+        self._note_inputs(in_arr, len(input.frames))
         result = FrameSet(pts=input.pts)
         for i, oid in enumerate(ids):
             w, h, fmt = out_arr[i].width, out_arr[i].height, out_arr[i].format
@@ -907,6 +962,7 @@ class Renderer:
     def render_raw(self, pts_ns, in_arr, n_in, out_arr, n_out, wait=True):
         st = self._lib.smr_render_begin(self._h, pts_ns, in_arr, n_in, out_arr, n_out)
         self._check(st, RenderSceneError)
+        self._note_inputs(in_arr, n_in)
         if wait:
             self._check(self._lib.smr_render_end(self._h), RenderSceneError)
 
