@@ -315,6 +315,28 @@ typedef struct {
     uint32_t motion_threshold;     /* MOTION_ADAPTIVE: T, 0 .. 255 */
 } smr_deinterlace;
 smr_status smr_set_input_deinterlace(smr_renderer *r, const char *input_id, const smr_deinterlace *cfg);
+/* The colour matrix and range of a YUV input (new: the reference reads every YUV input as BT.709, limited range except
+ * PlanarYuvJ420).  SD capture (NTSC / PAL), V4L2 webcams and MJPEG / JFIF sources are BT.601; screen capture and some
+ * cameras send full range.  The caller knows which from the source's metadata (ffmpeg's AVFrame colorspace / color_range,
+ * the DeckLink display mode, V4L2's ycbcr_enc / quantization; see INTEGRATION.md).
+ *   matrix: SMR_MATRIX_DEFAULT is BT.709; SMR_MATRIX_BT601 converts with r = y + 1.402 (v - .5),
+ *     g = y - 0.3441 (u - .5) - 0.7141 (v - .5), b = y + 1.772 (u - .5) (DESIGN.md NC-13): the matrix only, no change of
+ *     primaries.
+ *   range: SMR_RANGE_DEFAULT is full for SMR_FRAME_PLANAR_YUVJ420 and limited for every other YUV format; an explicit
+ *     value overrides that for every YUV format (planar 4:2:0, J420, NV12, 4:2:2, 4:4:4, UYVY, YUYV).
+ * RGB formats (BGRA, ARGB, RGBA8) store the setting and ignore it.  {DEFAULT, DEFAULT} leaves the input exactly as without
+ * this call.  The setting lasts until it is changed, or until smr_unregister_input, which drops it; a tick converts with
+ * the setting in force at its smr_render_begin (ticks in flight keep theirs).  The blocking calls take a frame, not an
+ * input, and keep their own rules (smr_preprocess_frame, the transcoder, the video converters).
+ * SMR_ERR_INVALID_ARGUMENT: a NULL id or c, an id that is not registered, an unknown matrix or range.  A host-only handle
+ * stores the setting. */
+typedef enum { SMR_MATRIX_DEFAULT = 0, SMR_MATRIX_BT709 = 1, SMR_MATRIX_BT601 = 2 } smr_yuv_matrix;
+typedef enum { SMR_RANGE_DEFAULT = 0, SMR_RANGE_LIMITED = 1, SMR_RANGE_FULL = 2 } smr_yuv_range;
+typedef struct {
+    int32_t matrix;                /* smr_yuv_matrix */
+    int32_t range;                 /* smr_yuv_range */
+} smr_input_color;
+smr_status smr_set_input_color(smr_renderer *r, const char *input_id, const smr_input_color *c);
 /* inspection (needs a device; blocking): the planes the kernels of the most recent tick that had a live frame of the input
  * read for it, after deinterlacing, copied into planes[p] (rows of the frame's row bytes, at pitch[p], 0 = tightly packed;
  * host or device memory per mem_kind).  The plane sizes are those of the frame (smr_input_frame).  Valid once that tick
@@ -688,9 +710,9 @@ smr_status smr_debug_tile_plan(const int32_t *boxes, uint32_t n_layers, uint32_t
  * composite because its piece of the launch was cut at an odd row.  *n is the job count; records go to `out` when they
  * fit in cap (SMR_ERR_BUFFER_TOO_SMALL otherwise; out = NULL asks for the count). */
 typedef enum {
-    SMR_FUSED_LDG = 0,             /* k_resample_fused_int<ratio, src_class> */
-    SMR_FUSED_TMA_INT = 1,         /* k_resample_tma3<ratio, src_class, full_range> */
-    SMR_FUSED_TMA_ANY = 2          /* k_resample_tma0<src_class, window, box> */
+    SMR_FUSED_LDG = 0,             /* k_resample_fused_int<ratio, src_class, matrix, full_range of UYVY / YUYV> */
+    SMR_FUSED_TMA_INT = 1,         /* k_resample_tma3<ratio, src_class, full_range, matrix> */
+    SMR_FUSED_TMA_ANY = 2          /* k_resample_tma0<src_class, window, box, matrix> */
 } smr_fused_kernel;
 typedef struct {
     int32_t kernel;                /* smr_fused_kernel */
@@ -704,6 +726,7 @@ typedef struct {
     uint32_t src_width, src_height, dst_width, dst_height;
     int32_t taps_h, taps_v;
     int32_t direct;                /* the job writes the output bytes of its direct tiles itself */
+    int32_t matrix;                /* the source's matrix: SMR_MATRIX_BT709 or SMR_MATRIX_BT601 */
 } smr_fused_job_info;
 smr_status smr_debug_fused_jobs(smr_renderer *r, smr_fused_job_info *out, uint32_t cap, uint32_t *n);
 
@@ -765,6 +788,7 @@ typedef struct {
     int32_t tex_align[3];          /* each plane's address mod 16 */
     int32_t width, height;         /* the job's target */
     int32_t out_format;            /* smr_output_format of the fused K10 / K11 stores, or -1: an RGBA8 frame for k_output */
+    int32_t tex_matrix;            /* a YUV texture's matrix: SMR_MATRIX_BT709 or SMR_MATRIX_BT601; 0 for other kinds */
 } smr_composite_layer_info;
 smr_status smr_debug_composite_layers(smr_renderer *r, smr_composite_layer_info *out, uint32_t cap, uint32_t *n);
 

@@ -9,5 +9,5 @@ from .renderer import (  # noqa: F401
     RendererOptions, RenderingMode, RenderSceneError, RescaleMode, RescalerComponent, Resolution, RGBAColor, ScalingAlgorithm, ShaderComponent,
     ShaderParam, ShaderParamType,
     TextComponent, TilesComponent, Transition, UpdateSceneError, VerticalAlign, ViewChildrenDirection, ViewComponent, WebViewComponent,
-    YuvPlanes,
+    YuvMatrix, YuvPlanes, YuvRange,
 )

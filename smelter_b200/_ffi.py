@@ -190,7 +190,7 @@ class FusedJobInfo(C.Structure):   # smr_fused_job_info
     _fields_ = [("kernel", C.c_int32), ("ratio", C.c_int32), ("window", C.c_int32), ("box", C.c_int32),
                 ("src_class", C.c_int32), ("full_range", C.c_int32), ("v_same", C.c_int32), ("strip_cols", C.c_int32),
                 ("src_width", C.c_uint32), ("src_height", C.c_uint32), ("dst_width", C.c_uint32), ("dst_height", C.c_uint32),
-                ("taps_h", C.c_int32), ("taps_v", C.c_int32), ("direct", C.c_int32)]
+                ("taps_h", C.c_int32), ("taps_v", C.c_int32), ("direct", C.c_int32), ("matrix", C.c_int32)]
 
 
 STAGE_BOX, STAGE_FIRST, STAGE_LAST = 0, 1, 2
@@ -211,7 +211,7 @@ class CompositeLayerInfo(C.Structure):   # smr_composite_layer_info
                 ("fast", C.c_int32), ("box", C.c_int32 * 12), ("tx_off", C.c_int32), ("ty_off", C.c_int32),
                 ("mask_count", C.c_int32), ("tex_kind", C.c_int32), ("tex_width", C.c_int32), ("tex_height", C.c_int32),
                 ("tex_pitch", C.c_int32 * 3), ("tex_align", C.c_int32 * 3), ("width", C.c_int32), ("height", C.c_int32),
-                ("out_format", C.c_int32)]
+                ("out_format", C.c_int32), ("tex_matrix", C.c_int32)]
 
 
 SCALE_NEAREST, SCALE_BILINEAR, SCALE_LANCZOS3 = 0, 1, 2
@@ -239,6 +239,14 @@ class Deinterlace(C.Structure):   # smr_deinterlace
     _fields_ = [("mode", C.c_int32), ("field_order", C.c_int32), ("motion_threshold", C.c_uint32)]
 
 
+MATRIX_DEFAULT, MATRIX_BT709, MATRIX_BT601 = 0, 1, 2
+RANGE_DEFAULT, RANGE_LIMITED, RANGE_FULL = 0, 1, 2
+
+
+class InputColor(C.Structure):   # smr_input_color
+    _fields_ = [("matrix", C.c_int32), ("range", C.c_int32)]
+
+
 KERNEL_CLASSES = ["convert", "weights", "resample_box", "resample_first", "resample_last", "composite", "output",
                   "fill", "resample_fused", "image", "web", "shader", "transcode", "video_convert", "deinterlace"]
 
@@ -248,7 +256,7 @@ class KernelTimes(C.Structure):
 
 
 EXPORTS = [
-    "smr_create", "smr_destroy", "smr_register_input", "smr_unregister_input", "smr_set_input_deinterlace",
+    "smr_create", "smr_destroy", "smr_register_input", "smr_unregister_input", "smr_set_input_deinterlace", "smr_set_input_color",
     "smr_debug_input_planes", "smr_register_image", "smr_unregister_image",
     "smr_register_svg_image",
     "smr_register_web_renderer", "smr_unregister_web_renderer", "smr_web_set_frame", "smr_web_set_child_rects", "smr_register_shader", "smr_unregister_shader", "smr_register_wgsl_shader", "smr_update_scene",
@@ -278,6 +286,7 @@ def lib():
     L.smr_register_input.argtypes = [vp, C.c_char_p]
     L.smr_unregister_input.argtypes = [vp, C.c_char_p]
     L.smr_set_input_deinterlace.argtypes = [vp, C.c_char_p, C.POINTER(Deinterlace)]
+    L.smr_set_input_color.argtypes = [vp, C.c_char_p, C.POINTER(InputColor)]
     L.smr_debug_input_planes.argtypes = [vp, C.c_char_p, C.POINTER(C.c_void_p * 3), C.POINTER(C.c_uint32 * 3), C.c_int32]
     L.smr_register_image.argtypes = [vp, C.c_char_p, C.POINTER(ImageSpec)]
     L.smr_unregister_image.argtypes = [vp, C.c_char_p]

@@ -23,6 +23,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <atomic>
+#include <type_traits>
 #include <cstring>
 
 #include "kernels.h"
@@ -356,7 +357,9 @@ __device__ __forceinline__ void prefetch_l2_span(const uint8_t *p, int bytes, co
 
 // SRC: 0 planar 4:2:0 (K1), 1 NV12 (K2), 2 UYVY, 3 YUYV (K3: texel-centre chroma, no interpolation -- for even
 // widths >= 8 the shader's coordinate round trip lands on pixel x's own texel (x >> 1) with weight exactly 1)
-template <int S, int SRC>
+// MAT: the matrix (Tex::matrix) of every source of the launch.  FULL: the range of every source of the launch for the
+// interleaved sources (the host keys their launches by it); 4:2:0 sources read the range per job, with FULL false.
+template <int S, int SRC, int MAT, bool FULL>
 __global__ void __launch_bounds__(32 * W64_WARPS, 3) k_resample_fused_int(const FusedJob *jobs, const FusedPiece *pieces,
                                                                             const int *piece_begin) {
     constexpr bool NV12 = SRC == 1, IL = SRC >= 2;
@@ -403,7 +406,7 @@ __global__ void __launch_bounds__(32 * W64_WARPS, 3) k_resample_fused_int(const 
     constexpr int NP = ((W64_TW - 1) * K::SS + TAPS + 2) >> 1, NIT = (NP + 31) / 32;
     const int npairs = S == 0 ? npairs_g : NP;
     const int full_range = src.full_range;
-    const float *ytab = full_range ? M.T.u8n : M.T.yl;
+    constexpr YuvCoef kc = yuv_coef(MAT);
     // pairs whose pixels and chroma taps need no clamping: x = xa_e + 2p >= 2 and x + 3 <= W - 1
     // (interleaved sources have no chroma neighbours: x >= 0 and x + 1 <= W - 1)
     const int p_in_lo = IL ? (xa_e >= 0 ? 0 : (1 - xa_e) >> 1) : (xa_e >= 2 ? 0 : (2 - xa_e + 1) >> 1);
@@ -486,9 +489,9 @@ __global__ void __launch_bounds__(32 * W64_WARPS, 3) k_resample_fused_int(const 
                         const float u = M.T.u8n[ub], v = M.T.u8n[vb];   // texel hit: exactly b / 255 (NC-1)
                         const int i = 2 * p - dsh;
                         int r8, g8, b8;
-                        yuv_to_rgb8n(M.T.yl[y0], u, v, 0, r8, g8, b8);
+                        yuv_to_rgb8n(FULL ? M.T.u8n[y0] : M.T.yl[y0], u, v, FULL, kc, r8, g8, b8);
                         if (i >= 0) put(i, r8, g8, b8);
-                        yuv_to_rgb8n(M.T.yl[y1], u, v, 0, r8, g8, b8);
+                        yuv_to_rgb8n(FULL ? M.T.u8n[y1] : M.T.yl[y1], u, v, FULL, kc, r8, g8, b8);
                         put(i + 1, r8, g8, b8);
                         return;
                     }
@@ -510,16 +513,16 @@ __global__ void __launch_bounds__(32 * W64_WARPS, 3) k_resample_fused_int(const 
                         const float yn = div255((float)yb, 1.0f);
                         return full_range ? yn : clamp01((yn - K16) * RCP_Y);
                     };
-                    yuv_to_rgb8n(luma(R.y & 0xffu), ue, ve, full_range, r8, g8, b8);
+                    yuv_to_rgb8n(luma(R.y & 0xffu), ue, ve, full_range, kc, r8, g8, b8);
                     if (i >= 0) put(i, r8, g8, b8);
-                    yuv_to_rgb8n(luma(R.y >> 8), uo, vo, full_range, r8, g8, b8);
+                    yuv_to_rgb8n(luma(R.y >> 8), uo, vo, full_range, kc, r8, g8, b8);
                     put(i + 1, r8, g8, b8);
                 };
                 auto inside = [&](int pp) { return pp >= p_in_lo && pp <= p_hi; };
                 auto border = [&](int p) {   // image border: resample.wgsl clamps the tap index
                     const int x = xa_e + 2 * p, i = 2 * p - dsh;
-                    const uchar4 pe = node_texel(M.T, src, min(max(x, 0), W - 1), r);
-                    const uchar4 po = node_texel(M.T, src, min(max(x + 1, 0), W - 1), r);
+                    const uchar4 pe = node_texel<MAT, FULL>(M.T, src, min(max(x, 0), W - 1), r);
+                    const uchar4 po = node_texel<MAT, FULL>(M.T, src, min(max(x + 1, 0), W - 1), r);
                     if (i >= 0) put(i, pe.x, pe.y, pe.z);
                     put(i + 1, po.x, po.y, po.z);
                 };
@@ -618,31 +621,42 @@ __global__ void __launch_bounds__(32 * W64_WARPS, 3) k_resample_fused_int(const 
     }  // pieces
 }
 
-template <int S, int SRC>
-static bool launch_fused_int(const FusedJob *jobs_dev, const FusedPiece *pieces, const int *piece_begin, int nblocks,
-                             cudaStream_t s) {
+template <int S, int SRC, int MAT, bool FULL>
+static bool launch_fused_kernel(const FusedJob *jobs_dev, const FusedPiece *pieces, const int *piece_begin, int nblocks,
+                                cudaStream_t s) {
     // the attribute is per device: several handles of one process may drive different GPUs from different threads
     static std::atomic<unsigned long long> done{0};
     int dev = 0;
     cudaGetDevice(&dev);
     const unsigned long long bit = 1ull << (dev & 63);
     if (!(done.load(std::memory_order_acquire) & bit)) {
-        cudaFuncSetAttribute(k_resample_fused_int<S, SRC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        cudaFuncSetAttribute(k_resample_fused_int<S, SRC, MAT, FULL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                              (int)sizeof(typename W64<S>::Smem));
         done.fetch_or(bit, std::memory_order_release);
     }
-    k_resample_fused_int<S, SRC><<<nblocks, dim3(32, W64_WARPS), sizeof(typename W64<S>::Smem), s>>>(jobs_dev, pieces, piece_begin);
+    k_resample_fused_int<S, SRC, MAT, FULL><<<nblocks, dim3(32, W64_WARPS), sizeof(typename W64<S>::Smem), s>>>(jobs_dev, pieces, piece_begin);
     return check_launch("k_resample_fused_int");
 }
 
+// the range is a template parameter for the interleaved sources only (k_resample_fused_int's FULL)
+template <int S, int SRC>
+static bool launch_fused_int(const FusedJob *jobs_dev, const FusedPiece *pieces, const int *piece_begin, int nblocks, int full_range,
+                             int matrix, cudaStream_t s) {
+    constexpr bool IL = SRC >= 2;
+    if (IL && full_range) return matrix ? launch_fused_kernel<S, SRC, 1, IL>(jobs_dev, pieces, piece_begin, nblocks, s)
+                                        : launch_fused_kernel<S, SRC, 0, IL>(jobs_dev, pieces, piece_begin, nblocks, s);
+    return matrix ? launch_fused_kernel<S, SRC, 1, false>(jobs_dev, pieces, piece_begin, nblocks, s)
+                  : launch_fused_kernel<S, SRC, 0, false>(jobs_dev, pieces, piece_begin, nblocks, s);
+}
+
 template <int S>
-static bool launch_fused_src(int src, const FusedJob *jobs_dev, const FusedPiece *pieces_dev, const int *piece_begin_dev,
-                             int nblocks, cudaStream_t st) {
+static bool launch_fused_src(int src, int full_range, int matrix, const FusedJob *jobs_dev, const FusedPiece *pieces_dev,
+                             const int *piece_begin_dev, int nblocks, cudaStream_t st) {
     switch (src) {
-        case 0: return launch_fused_int<S, 0>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, st);
-        case 1: return launch_fused_int<S, 1>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, st);
-        case 2: return launch_fused_int<S, 2>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, st);
-        default: return launch_fused_int<S, 3>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, st);
+        case 0: return launch_fused_int<S, 0>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, full_range, matrix, st);
+        case 1: return launch_fused_int<S, 1>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, full_range, matrix, st);
+        case 2: return launch_fused_int<S, 2>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, full_range, matrix, st);
+        default: return launch_fused_int<S, 3>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, full_range, matrix, st);
     }
 }
 
@@ -717,55 +731,62 @@ __device__ __forceinline__ void emit_yuv_2x2(const FusedJob &J, int X, int Y, ui
 #include "resample_tma3.cuh"
 #include "resample_tma0.cuh"
 
-template <int SRC, int WINP, int BOX>
-static bool launch_tma0(const FusedJob *jobs_dev, const FusedPiece *pieces, const int *piece_begin, int nblocks, cudaStream_t s) {
+template <int SRC, int WINP, int BOX, int MAT>
+static bool launch_tma0_mat(const FusedJob *jobs_dev, const FusedPiece *pieces, const int *piece_begin, int nblocks, cudaStream_t s) {
     static std::atomic<unsigned long long> done{0};
     int dev = 0;
     cudaGetDevice(&dev);
     const unsigned long long bit = 1ull << (dev & 63);
     if (!(done.load(std::memory_order_acquire) & bit)) {
-        cudaFuncSetAttribute(tma_any::k_resample_tma0<SRC, WINP, BOX>, cudaFuncAttributeMaxDynamicSharedMemorySize, tma_any::Cfg::SMEM);
+        cudaFuncSetAttribute(tma_any::k_resample_tma0<SRC, WINP, BOX, MAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, tma_any::Cfg::SMEM);
         done.fetch_or(bit, std::memory_order_release);
     }
     const int grid = (nblocks + tma_any::kGroups - 1) / tma_any::kGroups;
-    tma_any::k_resample_tma0<SRC, WINP, BOX><<<grid, dim3(32, tma::kWarps * tma_any::kGroups), tma_any::Cfg::SMEM, s>>>(jobs_dev, pieces, piece_begin, nblocks);
+    tma_any::k_resample_tma0<SRC, WINP, BOX, MAT><<<grid, dim3(32, tma::kWarps * tma_any::kGroups), tma_any::Cfg::SMEM, s>>>(jobs_dev, pieces, piece_begin, nblocks);
     return check_launch("k_resample_tma0");
+}
+template <int SRC, int WINP, int BOX>
+static bool launch_tma0(const FusedJob *jobs_dev, const FusedPiece *pieces, const int *piece_begin, int nblocks, int matrix, cudaStream_t s) {
+    return matrix ? launch_tma0_mat<SRC, WINP, BOX, 1>(jobs_dev, pieces, piece_begin, nblocks, s)
+                  : launch_tma0_mat<SRC, WINP, BOX, 0>(jobs_dev, pieces, piece_begin, nblocks, s);
 }
 
 template <int WINP>
-static bool launch_tma0_src(int src, int box, const FusedJob *jobs_dev, const FusedPiece *pieces, const int *piece_begin, int nblocks,
-                            cudaStream_t s) {
-    if (box) return src == 1 ? launch_tma0<1, WINP, 1>(jobs_dev, pieces, piece_begin, nblocks, s)
-                             : launch_tma0<0, WINP, 1>(jobs_dev, pieces, piece_begin, nblocks, s);
-    return src == 1 ? launch_tma0<1, WINP, 0>(jobs_dev, pieces, piece_begin, nblocks, s)
-                    : launch_tma0<0, WINP, 0>(jobs_dev, pieces, piece_begin, nblocks, s);
+static bool launch_tma0_src(int src, int box, int matrix, const FusedJob *jobs_dev, const FusedPiece *pieces, const int *piece_begin,
+                            int nblocks, cudaStream_t s) {
+    if (box) return src == 1 ? launch_tma0<1, WINP, 1>(jobs_dev, pieces, piece_begin, nblocks, matrix, s)
+                             : launch_tma0<0, WINP, 1>(jobs_dev, pieces, piece_begin, nblocks, matrix, s);
+    return src == 1 ? launch_tma0<1, WINP, 0>(jobs_dev, pieces, piece_begin, nblocks, matrix, s)
+                    : launch_tma0<0, WINP, 0>(jobs_dev, pieces, piece_begin, nblocks, matrix, s);
 }
 
-template <int S, int SRC, bool FULL>
+template <int S, int SRC, bool FULL, int MAT>
 static bool launch_tma3_range(const FusedJob *jobs_dev, const FusedPiece *pieces, const int *piece_begin, int nblocks, cudaStream_t s) {
     static std::atomic<unsigned long long> done{0};
     int dev = 0;
     cudaGetDevice(&dev);
     const unsigned long long bit = 1ull << (dev & 63);
     if (!(done.load(std::memory_order_acquire) & bit)) {
-        cudaFuncSetAttribute(tma_int::k_resample_tma3<S, SRC, FULL>, cudaFuncAttributeMaxDynamicSharedMemorySize, tma_int::Cfg<S>::SMEM);
+        cudaFuncSetAttribute(tma_int::k_resample_tma3<S, SRC, FULL, MAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, tma_int::Cfg<S>::SMEM);
         done.fetch_or(bit, std::memory_order_release);
     }
     const int grid = (nblocks + tma_int::kGroups - 1) / tma_int::kGroups;   // the host cut the work for `nblocks` eight-warp groups
-    tma_int::k_resample_tma3<S, SRC, FULL><<<grid, dim3(32, tma::kWarps * tma_int::kGroups), tma_int::Cfg<S>::SMEM, s>>>(jobs_dev, pieces, piece_begin,
-                                                                                                                  nblocks);
+    tma_int::k_resample_tma3<S, SRC, FULL, MAT><<<grid, dim3(32, tma::kWarps * tma_int::kGroups), tma_int::Cfg<S>::SMEM, s>>>(
+        jobs_dev, pieces, piece_begin, nblocks);
     return check_launch("k_resample_tma3");
 }
 template <int S, int SRC>
 static bool launch_tma3(const FusedJob *jobs_dev, const FusedPiece *pieces, const int *piece_begin, int nblocks, int full_range,
-                        cudaStream_t s) {
-    return full_range ? launch_tma3_range<S, SRC, true>(jobs_dev, pieces, piece_begin, nblocks, s)
-                      : launch_tma3_range<S, SRC, false>(jobs_dev, pieces, piece_begin, nblocks, s);
+                        int matrix, cudaStream_t s) {
+    if (matrix) return full_range ? launch_tma3_range<S, SRC, true, 1>(jobs_dev, pieces, piece_begin, nblocks, s)
+                                  : launch_tma3_range<S, SRC, false, 1>(jobs_dev, pieces, piece_begin, nblocks, s);
+    return full_range ? launch_tma3_range<S, SRC, true, 0>(jobs_dev, pieces, piece_begin, nblocks, s)
+                      : launch_tma3_range<S, SRC, false, 0>(jobs_dev, pieces, piece_begin, nblocks, s);
 }
 
 // src: 0 planar 4:2:0, 1 NV12, 2 UYVY, 3 YUYV (fused_source_class)
-int launch_resample_fused(const FusedKernel &k, int src, int full_range, const FusedJob *jobs_dev, const FusedPiece *pieces_dev,
-                          const int *piece_begin_dev, int nblocks, Stream s) {
+int launch_resample_fused(const FusedKernel &k, int src, int full_range, int matrix, const FusedJob *jobs_dev,
+                          const FusedPiece *pieces_dev, const int *piece_begin_dev, int nblocks, Stream s) {
     if (nblocks <= 0) return 0;
     cudaStream_t st = (cudaStream_t)s;
     bool ok = false;
@@ -778,24 +799,24 @@ int launch_resample_fused(const FusedKernel &k, int src, int full_range, const F
     switch (k.kind) {
         case FusedKernel::TMA_ANY:
             switch (k.window) {
-                case 0: ok = launch_tma0_src<kTma0Window[0]>(src, k.box, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
-                case 1: ok = launch_tma0_src<kTma0Window[1]>(src, k.box, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
-                case 2: ok = launch_tma0_src<kTma0Window[2]>(src, k.box, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
-                default: ok = launch_tma0_src<kTma0Window[3]>(src, k.box, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
+                case 0: ok = launch_tma0_src<kTma0Window[0]>(src, k.box, matrix, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
+                case 1: ok = launch_tma0_src<kTma0Window[1]>(src, k.box, matrix, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
+                case 2: ok = launch_tma0_src<kTma0Window[2]>(src, k.box, matrix, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
+                default: ok = launch_tma0_src<kTma0Window[3]>(src, k.box, matrix, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
             }
             break;
         case FusedKernel::TMA_INT:
-            if (k.ratio == 4) ok = src == 1 ? launch_tma3<4, 1>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, full_range, st)
-                                            : launch_tma3<4, 0>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, full_range, st);
-            else ok = src == 1 ? launch_tma3<2, 1>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, full_range, st)
-                               : launch_tma3<2, 0>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, full_range, st);
+            if (k.ratio == 4) ok = src == 1 ? launch_tma3<4, 1>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, full_range, matrix, st)
+                                            : launch_tma3<4, 0>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, full_range, matrix, st);
+            else ok = src == 1 ? launch_tma3<2, 1>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, full_range, matrix, st)
+                               : launch_tma3<2, 0>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, full_range, matrix, st);
             break;
         default:
             switch (k.ratio) {
-                case 2: ok = launch_fused_src<2>(src, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
-                case 3: ok = launch_fused_src<3>(src, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
-                case 4: ok = launch_fused_src<4>(src, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
-                default: ok = launch_fused_src<0>(src, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
+                case 2: ok = launch_fused_src<2>(src, full_range, matrix, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
+                case 3: ok = launch_fused_src<3>(src, full_range, matrix, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
+                case 4: ok = launch_fused_src<4>(src, full_range, matrix, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
+                default: ok = launch_fused_src<0>(src, full_range, matrix, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
             }
     }
     return ok ? 1 : -1;
@@ -808,11 +829,11 @@ int launch_resample_fused(const FusedKernel &k, int src, int full_range, const F
 // ------------------------------------------------------------------------------------------------
 // one source row: yw = its 8 luma bytes, v[k] = 3 * heavy + light chroma texel cx - 1 + k (u in bits 0..15, v in 16..31)
 __device__ __forceinline__ void half_row_convert(const uint32_t (&yw)[2], const uint32_t (&v)[6], float nk16, float rcp_y, float rcp_c,
-                                                 int (&sums)[4][3]) {
+                                                 const YuvCoef &kc, int (&sums)[4][3]) {
 #pragma unroll
     for (int p = 0; p < 4; p++) {
         float2 qr, qg, qb;
-        tma::convert_pair(yw, v, p, nk16, rcp_y, rcp_c, qr, qg, qb);
+        tma::convert_pair(yw, v, p, nk16, rcp_y, rcp_c, kc, qr, qg, qb);
         sums[p][0] += (int)(__float_as_uint(qr.x) & 0xffu) + (int)(__float_as_uint(qr.y) & 0xffu);
         sums[p][1] += (int)(__float_as_uint(qg.x) & 0xffu) + (int)(__float_as_uint(qg.y) & 0xffu);
         sums[p][2] += (int)(__float_as_uint(qb.x) & 0xffu) + (int)(__float_as_uint(qb.y) & 0xffu);
@@ -820,7 +841,8 @@ __device__ __forceinline__ void half_row_convert(const uint32_t (&yw)[2], const 
 }
 
 template <bool NV12>
-__device__ __forceinline__ void half_row_sums(const Tex &S, int x0, int r, float nk16, float rcp_y, float rcp_c, int (&sums)[4][3]) {
+__device__ __forceinline__ void half_row_sums(const Tex &S, int x0, int r, float nk16, float rcp_y, float rcp_c, const YuvCoef &kc,
+                                              int (&sums)[4][3]) {
     const uint8_t *yrow = S.p0 + (size_t)r * S.pitch0 + x0;
     const uint32_t yw[2] = {__ldg(reinterpret_cast<const uint32_t *>(yrow)), __ldg(reinterpret_cast<const uint32_t *>(yrow) + 1)};
     const int ch = r >> 1, cl = (r & 1) ? ch + 1 : ch - 1, cx = x0 >> 1;
@@ -838,12 +860,13 @@ __device__ __forceinline__ void half_row_sums(const Tex &S, int x0, int r, float
         }
         v[k] = 3u * h + l;
     }
-    half_row_convert(yw, v, nk16, rcp_y, rcp_c, sums);
+    half_row_convert(yw, v, nk16, rcp_y, rcp_c, kc, sums);
 }
 
 // NV12, x0 % 4 == 0, chroma plane 4-byte aligned: both source rows (r even, r + 1) of one output row.  The three chroma rows
 // they touch are loaded once as 16-byte windows [x0 - 4, x0 + 12) and spread once; the heavy row (r / 2) is shared.
-__device__ __forceinline__ void half_pair_sums_nv12(const Tex &S, int x0, int r, float nk16, float rcp_y, float rcp_c, int (&sums)[4][3]) {
+__device__ __forceinline__ void half_pair_sums_nv12(const Tex &S, int x0, int r, float nk16, float rcp_y, float rcp_c, const YuvCoef &kc,
+                                                    int (&sums)[4][3]) {
     const int ch = r >> 1;
     auto spread_row = [&](int crow, uint32_t (&t)[6]) {
         const uint32_t *w = reinterpret_cast<const uint32_t *>(S.p1 + (size_t)crow * S.pitch1 + x0 - 4);
@@ -862,7 +885,7 @@ __device__ __forceinline__ void half_pair_sums_nv12(const Tex &S, int x0, int r,
         for (int k = 0; k < 6; k++) v[k] = th[k] + tl[k];
         const uint32_t *yrow = reinterpret_cast<const uint32_t *>(S.p0 + (size_t)(r + half) * S.pitch0 + x0);
         const uint32_t yw[2] = {__ldg(yrow), __ldg(yrow + 1)};
-        half_row_convert(yw, v, nk16, rcp_y, rcp_c, sums);
+        half_row_convert(yw, v, nk16, rcp_y, rcp_c, kc, sums);
     }
 }
 
@@ -1169,30 +1192,36 @@ __device__ __forceinline__ void composite_body(const CompositeJob &J, const Laye
                 const Tex &S = J.textures[L.tex];
                 const int sx = 2 * (x0 + L.tx_off), sy = 2 * (y0 + L.ty_off);
                 if (sx >= 2 && sx + 9 <= S.width - 1 && sy >= 2 && sy + 5 <= S.height - 1) {
-                    const bool fr = S.full_range != 0;
-                    const float nk16 = fr ? 0.0f : -K16, rcp_y = fr ? 1.0f : RCP_Y, rcp_c = fr ? 1.0f : RCP_C;
+                    // one copy of the tile's conversion per matrix: the coefficients are immediates, as in the fused kernels
+                    auto half_tile = [&](auto mat) {
+                        constexpr YuvCoef kc = yuv_coef(decltype(mat)::value);
+                        const bool fr = S.full_range != 0;
+                        const float nk16 = fr ? 0.0f : -K16, rcp_y = fr ? 1.0f : RCP_Y, rcp_c = fr ? 1.0f : RCP_C;
 #pragma unroll
-                    for (int j = 0; j < CT_H; j++) {
-                        int sums[4][3];
+                        for (int j = 0; j < CT_H; j++) {
+                            int sums[4][3];
 #pragma unroll
-                        for (int i = 0; i < 4; i++) sums[i][0] = sums[i][1] = sums[i][2] = 0;
-                        if (S.kind == TEX_NV12 && (S.pitch1 & 3) == 0 && ((size_t)S.p1 & 3) == 0) {
-                            half_pair_sums_nv12(S, sx, sy + 2 * j, nk16, rcp_y, rcp_c, sums);
-                        } else if (S.kind == TEX_NV12) {
-                            half_row_sums<true>(S, sx, sy + 2 * j, nk16, rcp_y, rcp_c, sums);
-                            half_row_sums<true>(S, sx, sy + 2 * j + 1, nk16, rcp_y, rcp_c, sums);
-                        } else {
-                            half_row_sums<false>(S, sx, sy + 2 * j, nk16, rcp_y, rcp_c, sums);
-                            half_row_sums<false>(S, sx, sy + 2 * j + 1, nk16, rcp_y, rcp_c, sums);
+                            for (int i = 0; i < 4; i++) sums[i][0] = sums[i][1] = sums[i][2] = 0;
+                            if (S.kind == TEX_NV12 && (S.pitch1 & 3) == 0 && ((size_t)S.p1 & 3) == 0) {
+                                half_pair_sums_nv12(S, sx, sy + 2 * j, nk16, rcp_y, rcp_c, kc, sums);
+                            } else if (S.kind == TEX_NV12) {
+                                half_row_sums<true>(S, sx, sy + 2 * j, nk16, rcp_y, rcp_c, kc, sums);
+                                half_row_sums<true>(S, sx, sy + 2 * j + 1, nk16, rcp_y, rcp_c, kc, sums);
+                            } else {
+                                half_row_sums<false>(S, sx, sy + 2 * j, nk16, rcp_y, rcp_c, kc, sums);
+                                half_row_sums<false>(S, sx, sy + 2 * j + 1, nk16, rcp_y, rcp_c, kc, sums);
+                            }
+#pragma unroll
+                            for (int i = 0; i < CT_W; i++) {
+                                // filter_u8 at weights (128, 128): N = 16384 (t00 + t10 + t01 + t11), NC-6u, stored through NC-2
+                                px[j][i] = make_uchar4((unsigned char)unorm8(div255((float)(sums[i][0] << 14), 1.0f / 65536.0f)),
+                                                       (unsigned char)unorm8(div255((float)(sums[i][1] << 14), 1.0f / 65536.0f)),
+                                                       (unsigned char)unorm8(div255((float)(sums[i][2] << 14), 1.0f / 65536.0f)), 255);
+                            }
                         }
-#pragma unroll
-                        for (int i = 0; i < CT_W; i++) {
-                            // filter_u8 at weights (128, 128): N = 16384 (t00 + t10 + t01 + t11), NC-6u, stored through NC-2
-                            px[j][i] = make_uchar4((unsigned char)unorm8(div255((float)(sums[i][0] << 14), 1.0f / 65536.0f)),
-                                                   (unsigned char)unorm8(div255((float)(sums[i][1] << 14), 1.0f / 65536.0f)),
-                                                   (unsigned char)unorm8(div255((float)(sums[i][2] << 14), 1.0f / 65536.0f)), 255);
-                        }
-                    }
+                    };
+                    if (S.matrix == 1) half_tile(std::integral_constant<int, 1>());
+                    else half_tile(std::integral_constant<int, 0>());
                     break;
                 }
             }

@@ -40,6 +40,8 @@ struct Tex {
     int32_t full_range = 0;
     const uint8_t *p0 = nullptr, *p1 = nullptr, *p2 = nullptr;
     int32_t pitch0 = 0, pitch1 = 0, pitch2 = 0;  // bytes per row
+    // YUV kinds: 0 BT.709, 1 BT.601 (node_sample.cuh: yuv_coef).  Last, in what was tail padding: no other field moves.
+    int32_t matrix = 0;
 };
 
 struct MaskDev {
@@ -189,10 +191,17 @@ struct FusedKernel {
 // What a launch of a fused kernel needs to know: output columns per strip of job `j`, blocks (eight-warp groups) per SM
 // of the persistent grid, and the rows a block's share of the partition is a multiple of
 struct FusedShape { int strip_cols, groups_per_sm, row_gran; };
-// The source range a launch of kernel k is specialised for: the integer-ratio TMA kernel builds a luma table for one
-// range (1 full, 0 limited), so its launches are single-range; every other kernel reads the range per job (0)
+// source class of the fused kernel's template: 0 planar 4:2:0, 1 NV12, 2 UYVY, 3 YUYV; -1 not supported
+inline int fused_source_class(int tex_kind) {
+    return tex_kind == TEX_YUV420 ? 0 : tex_kind == TEX_NV12 ? 1 : tex_kind == TEX_UYVY ? 2 : tex_kind == TEX_YUYV ? 3 : -1;
+}
+// The source range a launch of kernel k is specialised for (1 full, 0 limited): the integer-ratio TMA kernel builds a luma
+// table for one range, and the LDG kernel's interleaved readers take it as a template parameter, so their launches are
+// single-range; every other reader takes the range per job (0).  The matrix (Tex::matrix) is a template parameter of every
+// fused kernel: a launch key is (kernel, source class, range, matrix).
 inline int fused_launch_range(const FusedKernel &k, const FusedJob &j) {
-    return k.kind == FusedKernel::TMA_INT && j.src.full_range ? 1 : 0;
+    const bool keyed = k.kind == FusedKernel::TMA_INT || (k.kind == FusedKernel::LDG && fused_source_class(j.src.kind) >= 2);
+    return keyed && j.src.full_range ? 1 : 0;
 }
 inline FusedShape fused_shape(const FusedKernel &k, const FusedJob &j) {
     switch (k.kind) {
@@ -352,10 +361,6 @@ int debug_weights(float scale, float offset, int n_out, float *w_host, size_t ca
 // NC-8's sin_cr / cos_cr (the functions k_weights calls) on n host values, synchronously.  1 done, -1 CUDA error
 int debug_sincos(const float *x_host, int n, float *s_host, float *c_host);
 int launch_resample(const ResampleJob *jobs_dev, const ResampleJob *jobs_host, int n_jobs, Stream s);
-// source class of the fused kernel's template: 0 planar 4:2:0, 1 NV12, 2 UYVY, 3 YUYV; -1 not supported
-inline int fused_source_class(int tex_kind) {
-    return tex_kind == TEX_YUV420 ? 0 : tex_kind == TEX_NV12 ? 1 : tex_kind == TEX_UYVY ? 2 : tex_kind == TEX_YUYV ? 3 : -1;
-}
 // FramePreProcessor: node texture of `src` (rescale = 0) or its linear-filtered rescale to out_w x out_h
 int launch_preprocess(const Tex &src, int mode, int rescale, uint8_t *out, int out_pitch, int out_w, int out_h, Stream s);
 // node textures: every job of jobs_dev in one launch of a 32 x 8 tile-job kernel, node_kernel's or a shader module's
@@ -366,9 +371,9 @@ int launch_tile_jobs(const void *kernel, const void *jobs_dev, const int32_t *ti
                      const char *name, Stream s);
 enum NodeKernel { NODE_TEXT, NODE_IMAGE, NODE_WEB };   // k_text (TextJob), k_image (ImageJob), k_web (WebJob)
 const void *node_kernel(NodeKernel k);
-// full_range: fused_launch_range of every job of the launch
-int launch_resample_fused(const FusedKernel &k, int src, int full_range, const FusedJob *jobs_dev, const FusedPiece *pieces_dev,
-                          const int *piece_begin_dev, int nblocks, Stream s);
+// full_range: fused_launch_range of every job of the launch; matrix: src.matrix of every job of the launch
+int launch_resample_fused(const FusedKernel &k, int src, int full_range, int matrix, const FusedJob *jobs_dev,
+                          const FusedPiece *pieces_dev, const int *piece_begin_dev, int nblocks, Stream s);
 // every output of a tick in one launch; jobs_dev[i] == jobs_host[i], layers / masks / textures device pointers.  One output
 // with a short layer list (layers0_host: host copy of jobs_host[0].layers) passes job and layers in the parameter block
 int launch_composite(const CompositeJob *jobs_dev, const CompositeJob *jobs_host, const LayerDev *layers0_host, int n, Stream s);

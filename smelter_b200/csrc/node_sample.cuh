@@ -107,45 +107,49 @@ __device__ __forceinline__ float sample_plane(const Tables &T, const uint8_t *p,
 #define RCP_Y (1.0f / 0.85882352941f)
 #define RCP_C (1.0f / 0.87843137254f)
 
-__device__ __forceinline__ uchar4 yuv_to_rgba8(float y, float u, float v, int full_range) {
+// The chroma coefficients of the YUV -> RGB matrix rows, by Tex::matrix: 0 BT.709 (K1-K3), 1 BT.601 (NC-13, from Kr = 0.299
+// and Kb = 0.114).  The only place they appear: every reader takes them from here, as immediates where the matrix is a
+// template parameter.
+struct YuvCoef {
+    float rv, gu, gv, bu;   // r = y + rv (v - .5); g = y + gu (u - .5) + gv (v - .5); b = y + bu (u - .5)
+};
+__host__ __device__ constexpr YuvCoef yuv_coef(int matrix) {
+    return matrix == 1 ? YuvCoef{1.402f, -0.3441f, -0.7141f, 1.772f} : YuvCoef{1.5748f, -0.1873f, -0.4681f, 1.8556f};
+}
+
+__device__ __forceinline__ uchar4 yuv_to_rgba8(float y, float u, float v, int full_range, int matrix) {
+    const YuvCoef k = yuv_coef(matrix);
     if (!full_range) {
         y = clamp01((y - K16) * RCP_Y);
         u = clamp01((u - K16) * RCP_C);
         v = clamp01((v - K16) * RCP_C);
     }
     float um = u - 0.5f, vm = v - 0.5f;
-    float r = fmaf(1.5748f, vm, y);
-    float g = fmaf(-0.4681f, vm, fmaf(-0.1873f, um, y));
-    float b = fmaf(1.8556f, um, y);
+    float r = fmaf(k.rv, vm, y);
+    float g = fmaf(k.gv, vm, fmaf(k.gu, um, y));
+    float b = fmaf(k.bu, um, y);
     return make_uchar4((unsigned char)unorm8(r), (unsigned char)unorm8(g), (unsigned char)unorm8(b), 255);
 }
 
-// same arithmetic, results as integers (no byte packing) for callers that index a table next
-__device__ __forceinline__ void yuv_to_rgb8i(float y, float u, float v, int full_range, int &r8, int &g8, int &b8) {
-    if (!full_range) {
-        y = clamp01((y - K16) * RCP_Y);
-        u = clamp01((u - K16) * RCP_C);
-        v = clamp01((v - K16) * RCP_C);
-    }
-    float um = u - 0.5f, vm = v - 0.5f;
-    r8 = unorm8(fmaf(1.5748f, vm, y));
-    g8 = unorm8(fmaf(-0.4681f, vm, fmaf(-0.1873f, um, y)));
-    b8 = unorm8(fmaf(1.8556f, um, y));
-}
-
-// luma already expanded (Tables::yl or Tables::u8n), chroma still raw
-__device__ __forceinline__ void yuv_to_rgb8n(float yn, float u, float v, int full_range, int &r8, int &g8, int &b8) {
+// luma already expanded (Tables::yl or Tables::u8n), chroma still raw; results as integers for callers that index a table next
+__device__ __forceinline__ void yuv_to_rgb8n(float yn, float u, float v, int full_range, const YuvCoef &k, int &r8, int &g8, int &b8) {
     if (!full_range) {
         u = clamp01((u - K16) * RCP_C);
         v = clamp01((v - K16) * RCP_C);
     }
     float um = u - 0.5f, vm = v - 0.5f;
-    r8 = unorm8(fmaf(1.5748f, vm, yn));
-    g8 = unorm8(fmaf(-0.4681f, vm, fmaf(-0.1873f, um, yn)));
-    b8 = unorm8(fmaf(1.8556f, um, yn));
+    r8 = unorm8(fmaf(k.rv, vm, yn));
+    g8 = unorm8(fmaf(k.gv, vm, fmaf(k.gu, um, yn)));
+    b8 = unorm8(fmaf(k.bu, um, yn));
 }
 
+// MAT: the matrix, or -1 for the texture's (s.matrix).  RANGE422: the range of the 4:2:2, 4:4:4 and interleaved kinds, or -1
+// for the texture's (s.full_range); the 4:2:0 kinds always read s.full_range.  Callers that are specialised for one
+// matrix and range pass them, so that the coefficients are immediates.
+template <int MAT = -1, int RANGE422 = -1>
 __device__ __forceinline__ uchar4 node_texel(const Tables &T, const Tex &s, int x, int y) {
+    const int mat = MAT < 0 ? s.matrix : MAT;
+    const int fr422 = RANGE422 < 0 ? s.full_range : RANGE422;
     switch (s.kind) {
         case TEX_RGBA8:
             return __ldg(reinterpret_cast<const uchar4 *>(s.p0 + (size_t)y * s.pitch0) + x);
@@ -183,7 +187,7 @@ __device__ __forceinline__ uchar4 node_texel(const Tables &T, const Tex &s, int 
                     nv = ((int)a.y * (4 - kx) + (int)b.y * kx) * (4 - ky) + ((int)c.y * (4 - kx) + (int)d.y * kx) * ky;
                 }
                 const float uu = div255((float)nu, 0.0625f), vv = div255((float)nv, 0.0625f);
-                return yuv_to_rgba8(yy, uu, vv, s.full_range);
+                return yuv_to_rgba8(yy, uu, vv, s.full_range, mat);
             }
             float tx = ((float)x + 0.5f) / (float)s.width, ty = ((float)y + 0.5f) / (float)s.height;
             LinTap ax = linear_tap(tx, s.width), ay = linear_tap(ty, s.height);
@@ -197,7 +201,7 @@ __device__ __forceinline__ uchar4 node_texel(const Tables &T, const Tex &s, int 
                 uu = sample_plane(T, s.p1, s.pitch1, 2, 0, cx, cy);
                 vv = sample_plane(T, s.p1, s.pitch1, 2, 1, cx, cy);
             }
-            return yuv_to_rgba8(yy, uu, vv, s.full_range);
+            return yuv_to_rgba8(yy, uu, vv, s.full_range, mat);
         }
         case TEX_YUV422:
         case TEX_YUV444: {   // the three planes are sampled at the same normalised coordinate (NC-6)
@@ -208,7 +212,7 @@ __device__ __forceinline__ uchar4 node_texel(const Tables &T, const Tex &s, int 
             float yy = sample_plane(T, s.p0, s.pitch0, 1, 0, ax, ay);
             float uu = sample_plane(T, s.p1, s.pitch1, 1, 0, cx, cy);
             float vv = sample_plane(T, s.p2, s.pitch2, 1, 0, cx, cy);
-            return yuv_to_rgba8(yy, uu, vv, 0);
+            return yuv_to_rgba8(yy, uu, vv, fr422, mat);
         }
         case TEX_UYVY:
         case TEX_YUYV: {   // K3 (interleaved_{uyvy,yuyv}_to_rgba.wgsl:24-61): column index back from the coordinate
@@ -223,8 +227,8 @@ __device__ __forceinline__ uchar4 node_texel(const Tables &T, const Tex &s, int 
 #pragma unroll
             for (int c = 0; c < 4; c++) t[c] = sample_plane(T, s.p0, s.pitch0, 4, c, ax, ay);
             const bool second = x_pos & 1u;
-            if (s.kind == TEX_YUYV) return yuv_to_rgba8(second ? t[2] : t[0], t[1], t[3], 0);
-            return yuv_to_rgba8(second ? t[3] : t[1], t[0], t[2], 0);
+            if (s.kind == TEX_YUYV) return yuv_to_rgba8(second ? t[2] : t[0], t[1], t[3], fr422, mat);
+            return yuv_to_rgba8(second ? t[3] : t[1], t[0], t[2], fr422, mat);
         }
         default:
             return make_uchar4(0, 0, 0, 0);
@@ -273,10 +277,10 @@ __device__ __forceinline__ void yuv_quad(const Tables &T, const Tex &s, int x, i
     const uchar2 y1 = __ldg(reinterpret_cast<const uchar2 *>(s.p0 + (size_t)(y + 1) * s.pitch0 + x));
     unsigned n00, n10, n01, n11;
     quad_chroma16(he, ho, n00, n10, n01, n11);
-    p00 = yuv_to_rgba8(T.u8n[y0.x], div255((float)(n00 & 0xffffu), 0.0625f), div255((float)(n00 >> 16), 0.0625f), s.full_range);
-    p10 = yuv_to_rgba8(T.u8n[y0.y], div255((float)(n10 & 0xffffu), 0.0625f), div255((float)(n10 >> 16), 0.0625f), s.full_range);
-    p01 = yuv_to_rgba8(T.u8n[y1.x], div255((float)(n01 & 0xffffu), 0.0625f), div255((float)(n01 >> 16), 0.0625f), s.full_range);
-    p11 = yuv_to_rgba8(T.u8n[y1.y], div255((float)(n11 & 0xffffu), 0.0625f), div255((float)(n11 >> 16), 0.0625f), s.full_range);
+    p00 = yuv_to_rgba8(T.u8n[y0.x], div255((float)(n00 & 0xffffu), 0.0625f), div255((float)(n00 >> 16), 0.0625f), s.full_range, s.matrix);
+    p10 = yuv_to_rgba8(T.u8n[y0.y], div255((float)(n10 & 0xffffu), 0.0625f), div255((float)(n10 >> 16), 0.0625f), s.full_range, s.matrix);
+    p01 = yuv_to_rgba8(T.u8n[y1.x], div255((float)(n01 & 0xffffu), 0.0625f), div255((float)(n01 >> 16), 0.0625f), s.full_range, s.matrix);
+    p11 = yuv_to_rgba8(T.u8n[y1.y], div255((float)(n11 & 0xffffu), 0.0625f), div255((float)(n11 >> 16), 0.0625f), s.full_range, s.matrix);
 }
 
 // textureSample of a child through NodeTextureState::view()

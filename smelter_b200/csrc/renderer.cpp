@@ -418,6 +418,7 @@ class Renderer {
     smr_status register_input(const char *id);
     smr_status unregister_input(const char *id);
     smr_status set_input_deinterlace(const char *id, const smr_deinterlace *cfg);
+    smr_status set_input_color(const char *id, const smr_input_color *c);
     smr_status debug_input_planes(const char *id, void *const planes[3], const uint32_t pitch[3], int32_t mem_kind);
     smr_status register_image(const char *id, const smr_image_spec *spec);
     smr_status register_svg_image(const char *id, const smr_svg_spec *spec);
@@ -480,6 +481,7 @@ class Renderer {
         int raw_tex = -1;       // index of the virtual (fused K1/K2) texture
         int32_t format = -1;    // smr_frame_format of the last live frame (-1: none since registration)
         smr_deinterlace deint = {SMR_DEINTERLACE_OFF, SMR_FIELD_TOP_FIRST, 10};
+        smr_input_color color = {SMR_MATRIX_DEFAULT, SMR_RANGE_DEFAULT};
         DeinterlaceHistory hist;
         DevBuf deint_out[kTicksInFlight][3];   // the deinterlaced planes `tex` points at, one set per tick in flight
         DevBuf hist_planes[2][3];
@@ -693,9 +695,11 @@ class Renderer {
         std::vector<uint32_t> list;
         size_t list_off = SIZE_MAX;       // param-arena offset of `list`
     };
-    struct FusedKey {           // the fused jobs one launch runs: same kernel, source class and launch range
-        dev::FusedKernel kernel; int src, range;
-        bool operator==(const FusedKey &o) const { return kernel == o.kernel && src == o.src && range == o.range; }
+    struct FusedKey {           // the fused jobs one launch runs: same kernel, source class, launch range and matrix
+        dev::FusedKernel kernel; int src, range, matrix;
+        bool operator==(const FusedKey &o) const {
+            return kernel == o.kernel && src == o.src && range == o.range && matrix == o.matrix;
+        }
     };
     struct FusedLaunch { FusedKey key; size_t pieces_off, begin_off; int nblocks; };
     // One launch of a node-texture kernel (launch_tile_jobs): launch_tick enqueues it after phase `phase`'s composite (-1:
@@ -982,6 +986,17 @@ smr_status Renderer::set_input_deinterlace(const char *id, const smr_deinterlace
     Input &I = it->second;
     if (cfg->mode != I.deint.mode || cfg->field_order != I.deint.field_order) I.hist = DeinterlaceHistory();
     I.deint = *cfg;
+    return SMR_OK;
+}
+
+smr_status Renderer::set_input_color(const char *id, const smr_input_color *c) {
+    if (!id || !c) return SMR_ERR_INVALID_ARGUMENT;
+    std::lock_guard<std::mutex> g(mu_);
+    auto it = inputs_.find(id);
+    if (it == inputs_.end()) { set_error(std::string("input \"") + id + "\" is not registered"); return SMR_ERR_INVALID_ARGUMENT; }
+    if (c->matrix < SMR_MATRIX_DEFAULT || c->matrix > SMR_MATRIX_BT601) { set_error("unknown colour matrix"); return SMR_ERR_INVALID_ARGUMENT; }
+    if (c->range < SMR_RANGE_DEFAULT || c->range > SMR_RANGE_FULL) { set_error("unknown colour range"); return SMR_ERR_INVALID_ARGUMENT; }
+    it->second.color = *c;
     return SMR_OK;
 }
 
@@ -1650,6 +1665,23 @@ static bool tex_kind_of_format(int fmt, dev::Tex &t) {   // FrameData variant ->
     }
 }
 
+static bool tex_is_yuv(const dev::Tex &t) {
+    return t.kind == dev::TEX_YUV420 || t.kind == dev::TEX_NV12 || t.kind >= dev::TEX_YUV422;
+}
+
+// An input's smr_input_color over its frame's texture: DEFAULT keeps the format's rule (tex_kind_of_format: BT.709, full
+// range for J420 only), an explicit value replaces it.  RGB kinds ignore the setting.
+static void apply_input_color(const smr_input_color &c, dev::Tex &t) {
+    if (!tex_is_yuv(t)) return;
+    if (c.matrix != SMR_MATRIX_DEFAULT) t.matrix = c.matrix == SMR_MATRIX_BT601 ? 1 : 0;
+    if (c.range != SMR_RANGE_DEFAULT) t.full_range = c.range == SMR_RANGE_FULL ? 1 : 0;
+}
+
+// Tex::matrix as smr_yuv_matrix, for inspection; 0 for a texture that is not YUV
+static int32_t public_matrix(const dev::Tex &t) {
+    return !tex_is_yuv(t) ? 0 : t.matrix == 1 ? SMR_MATRIX_BT601 : SMR_MATRIX_BT709;
+}
+
 static void set_tex_plane(dev::Tex &t, int p, const uint8_t *ptr, size_t pitch) {
     (p == 0 ? t.p0 : p == 1 ? t.p1 : t.p2) = ptr;
     (p == 0 ? t.pitch0 : p == 1 ? t.pitch1 : t.pitch2) = (int)pitch;
@@ -1724,6 +1756,7 @@ static size_t align16(size_t n) { return (n + 15) & ~(size_t)15; }
 smr_status Renderer::upload_input(Input &I, const smr_input_frame &f) {
     FrameView v;
     if (smr_status st = read_frame(f, v); st != SMR_OK) return st;
+    apply_input_color(I.color, v.tex);
     const bool deint = I.deint.mode != SMR_DEINTERLACE_OFF;
     for (int p = 0; p < 3 && f.mem_kind != SMR_MEM_DEVICE; p++) {
         FrameView::Plane &P = v.plane[p];
@@ -1745,7 +1778,7 @@ smr_status Renderer::upload_input(Input &I, const smr_input_frame &f) {
         if (smr_status st = plan_deinterlace(I, f, v); st != SMR_OK) return st;
     I.format = f.format;
     I.tex = v.tex;
-    I.raw_tex = add_texture(v.tex, v.tex.kind == dev::TEX_YUV420 || v.tex.kind == dev::TEX_NV12 || v.tex.kind >= dev::TEX_YUV422);
+    I.raw_tex = add_texture(v.tex, tex_is_yuv(v.tex));
     return SMR_OK;
 }
 
@@ -3150,11 +3183,11 @@ smr_status Renderer::resolve_frame_arena() {
     return SMR_OK;
 }
 
-// The tick's fused resamples over a persistent grid, one launch per kernel, source class and launch range; runs before the
+// The tick's fused resamples over a persistent grid, one launch per kernel, source class, launch range and matrix; runs before the
 // composites' tile lists are packed, as a job cut at an odd row gives its direct tiles back to its composite
 void Renderer::plan_fused_launches() {
     auto key_of = [](const FusedRec &f) {
-        return FusedKey{f.kernel, dev::fused_source_class(f.job.src.kind), dev::fused_launch_range(f.kernel, f.job)};
+        return FusedKey{f.kernel, dev::fused_source_class(f.job.src.kind), dev::fused_launch_range(f.kernel, f.job), f.job.src.matrix};
     };
     for (size_t i = 0; i < plan_.fused.size(); i++) {
         const FusedKey v = key_of(plan_.fused[i]);
@@ -3320,7 +3353,7 @@ smr_status Renderer::launch_tick() {
                                       (int)plan_.weight_jobs.size(), stream_), SMR_KERNEL_WEIGHTS)) return SMR_ERR_CUDA;
     new_weight_keys_.clear();   // the tables are being computed on the stream: the cache entries are good
     for (const FusedLaunch &fl : plan_.fused_launches)
-        if (!launched(dev::launch_resample_fused(fl.key.kernel, fl.key.src, fl.key.range, (const dev::FusedJob *)(pd + plan_.fused_off),
+        if (!launched(dev::launch_resample_fused(fl.key.kernel, fl.key.src, fl.key.range, fl.key.matrix, (const dev::FusedJob *)(pd + plan_.fused_off),
                                                  (const dev::FusedPiece *)(pd + fl.pieces_off), (const int *)(pd + fl.begin_off),
                                                  fl.nblocks, stream_), SMR_KERNEL_RESAMPLE_FUSED)) return SMR_ERR_CUDA;
     for (size_t p = 0; p + 1 < plan_.phases.size(); p++) {
@@ -3401,6 +3434,7 @@ smr_status Renderer::debug_fused_jobs(smr_fused_job_info *out, uint32_t cap, uin
         o.dst_width = (uint32_t)j.dst_w; o.dst_height = (uint32_t)j.dst_h;
         o.taps_h = j.taps_h; o.taps_v = j.taps_v;
         o.direct = f.direct_off != SIZE_MAX ? 1 : 0;
+        o.matrix = public_matrix(j.src);
     }
     return SMR_OK;
 }
@@ -3479,6 +3513,7 @@ smr_status Renderer::debug_composite_layers(smr_composite_layer_info *out, uint3
                 const uint8_t *p[3] = {t.p0, t.p1, t.p2};
                 const int32_t pitch[3] = {t.pitch0, t.pitch1, t.pitch2};
                 o.tex_kind = t.kind; o.tex_width = t.width; o.tex_height = t.height;
+                o.tex_matrix = public_matrix(t);
                 for (int pl = 0; pl < 3; pl++) {
                     o.tex_pitch[pl] = p[pl] ? pitch[pl] : 0;
                     o.tex_align[pl] = (int32_t)((uintptr_t)p[pl] & 15);
@@ -3872,6 +3907,9 @@ smr_status smr_register_input(smr_renderer *r, const char *id) { SMR_GUARD(r->im
 smr_status smr_unregister_input(smr_renderer *r, const char *id) { SMR_GUARD(r->impl.unregister_input(id)) }
 smr_status smr_set_input_deinterlace(smr_renderer *r, const char *id, const smr_deinterlace *cfg) {
     SMR_GUARD(r->impl.set_input_deinterlace(id, cfg))
+}
+smr_status smr_set_input_color(smr_renderer *r, const char *id, const smr_input_color *c) {
+    SMR_GUARD(r->impl.set_input_color(id, c))
 }
 smr_status smr_debug_input_planes(smr_renderer *r, const char *id, void *const planes[3], const uint32_t pitch[3], int32_t mem_kind) {
     SMR_GUARD(r->impl.debug_input_planes(id, planes, pitch, mem_kind))

@@ -336,11 +336,11 @@ __device__ __forceinline__ uint32_t luma_base(unsigned char *tail) {
 
 // K1/K2 -> u8 of pixels 2p and 2p + 1 of an 8-pixel run (yw: its luma bytes, v: its combined chroma as fetch_row makes it),
 // two pixels per instruction: q = 1.5 * 2^23 + the byte.  nk16, rcp_y, rcp_c: -16/255 and the limited-range scales, or
-// 0, 1, 1 for a full-range source.  YTAB: the luma comes from the luma table (ybase from luma_base, filled for the same
+// 0, 1, 1 for a full-range source; k: the matrix's coefficients (yuv_coef).  YTAB: the luma comes from the luma table (ybase from luma_base, filled for the same
 // nk16 and rcp_y) instead of the arithmetic.
 template <bool YTAB = false>
 __device__ __forceinline__ void convert_pair(const uint32_t (&yw)[2], const uint32_t (&v)[6], int p, float nk16, float rcp_y,
-                                             float rcp_c, float2 &qr, float2 &qg, float2 &qb, uint32_t ybase = 0) {
+                                             float rcp_c, const YuvCoef &k, float2 &qr, float2 &qg, float2 &qb, uint32_t ybase = 0) {
     // 16 x chroma of the even / odd pixel of the pair (NC-6u with the .25 / .75 taps)
     const uint32_t ne = v[p] + 3u * v[p + 1], no = 3u * v[p + 1] + v[p + 2];
     const float m23 = -8388608.0f;
@@ -371,10 +371,10 @@ __device__ __forceinline__ void convert_pair(const uint32_t (&yw)[2], const uint
     w = make_float2(__saturatef(w.x * rcp_c), __saturatef(w.y * rcp_c));
     const float2 um = add2(u, splat(-0.5f)), vm = add2(w, splat(-0.5f));
     // clamp01 (NC-2) as the .SAT of the matrix row's last fma
-    const float2 gi = fma2(splat(-0.1873f), um, y);
-    const float2 rr = make_float2(__saturatef(fmaf(1.5748f, vm.x, y.x)), __saturatef(fmaf(1.5748f, vm.y, y.y)));
-    const float2 gg = make_float2(__saturatef(fmaf(-0.4681f, vm.x, gi.x)), __saturatef(fmaf(-0.4681f, vm.y, gi.y)));
-    const float2 bb = make_float2(__saturatef(fmaf(1.8556f, um.x, y.x)), __saturatef(fmaf(1.8556f, um.y, y.y)));
+    const float2 gi = fma2(splat(k.gu), um, y);
+    const float2 rr = make_float2(__saturatef(fmaf(k.rv, vm.x, y.x)), __saturatef(fmaf(k.rv, vm.y, y.y)));
+    const float2 gg = make_float2(__saturatef(fmaf(k.gv, vm.x, gi.x)), __saturatef(fmaf(k.gv, vm.y, gi.y)));
+    const float2 bb = make_float2(__saturatef(fmaf(k.bu, um.x, y.x)), __saturatef(fmaf(k.bu, um.y, y.y)));
     // NC-2 rounding: the add rounds to the nearest-even integer
     qr = add2_after_mul(mul2(rr, splat(255.0f)), splat(kMagicRound));
     qg = add2_after_mul(mul2(gg, splat(255.0f)), splat(kMagicRound));
@@ -382,14 +382,14 @@ __device__ __forceinline__ void convert_pair(const uint32_t (&yw)[2], const uint
 }
 
 // K1/K2 -> u8 -> sRGB decode of the node-texture fetch (NC-3) of an 8-pixel run: (r, g) and b of pixel i, looked up in
-// this lane's copy of the decode table (kaddr from setup_block); YTAB, ybase: as in convert_pair
+// this lane's copy of the decode table (kaddr from setup_block); k, YTAB, ybase: as in convert_pair
 template <bool YTAB = false>
 __device__ __forceinline__ void convert_run(const uint32_t (&yw)[2], const uint32_t (&v)[6], float nk16, float rcp_y, float rcp_c,
-                                            uint32_t kaddr, float2 (&prg)[8], float (&pb)[8], uint32_t ybase = 0) {
+                                            const YuvCoef &k, uint32_t kaddr, float2 (&prg)[8], float (&pb)[8], uint32_t ybase = 0) {
 #pragma unroll
     for (int p = 0; p < 4; p++) {
         float2 qr, qg, qb;
-        convert_pair<YTAB>(yw, v, p, nk16, rcp_y, rcp_c, qr, qg, qb, ybase);
+        convert_pair<YTAB>(yw, v, p, nk16, rcp_y, rcp_c, k, qr, qg, qb, ybase);
         prg[2 * p] = make_float2(lds_tab((__float_as_uint(qr.x) << 7) + kaddr), lds_tab((__float_as_uint(qg.x) << 7) + kaddr));
         prg[2 * p + 1] = make_float2(lds_tab((__float_as_uint(qr.y) << 7) + kaddr), lds_tab((__float_as_uint(qg.y) << 7) + kaddr));
         pb[2 * p] = lds_tab((__float_as_uint(qb.x) << 7) + kaddr);

@@ -37,7 +37,8 @@ struct Cfg {
 // WINP: slots of a lane's window the tap loop walks (host: >= taps + widest distance of two adjacent columns + pads)
 // BOX: the source is box-reduced 2:1 on both axes first (downsample.wgsl:28-41, one pre-decimation level of resampler.rs:56-67):
 // the two source rows of a reduced row are converted back to back, summed in the shader's order, quantised to f16
-template <int SRC, int WINP, int BOX>
+// MAT: the matrix (Tex::matrix) of every source of the launch (the host keys the launches by it); the range is read per job
+template <int SRC, int WINP, int BOX, int MAT>
 __global__ void __launch_bounds__(32 * kWarps * kGroups, 1) k_resample_tma0(const FusedJob *jobs, const FusedPiece *pieces, const int *piece_begin,
                                                                             int n_virtual_blocks) {
     using K = Cfg;
@@ -133,7 +134,7 @@ __global__ void __launch_bounds__(32 * kWarps * kGroups, 1) k_resample_tma0(cons
                     // A1: K1/K2 -> u8 -> sRGB decode, two pixels per instruction
                     float2 crg[P];   // (r, g) of source pixel i of this row
                     float cb[P];     // b
-                    convert_run(yw, v, nk16, rcp_y, rcp_c, kaddr, crg, cb);
+                    convert_run(yw, v, nk16, rcp_y, rcp_c, yuv_coef(MAT), kaddr, crg, cb);
                     if (!BOX) {
 #pragma unroll
                         for (int i = 0; i < P; i++) { prg[i] = crg[i]; pb[i] = cb[i]; }

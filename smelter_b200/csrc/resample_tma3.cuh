@@ -15,8 +15,9 @@
 //     consecutive output rows share TAPS - S of their ring rows, every row is loaded once for both.
 //
 // Template parameter S in {2, 4}: integer horizontal ratio with zero crop offset (first(o) = S * o + const).
-// SRC: 0 planar 4:2:0, 1 NV12.  FULL: the range of every source of the launch (the host keys the launches by it), so the
-// range constants of K1/K2 are immediates of the row loop and take no registers there.
+// SRC: 0 planar 4:2:0, 1 NV12.  FULL, MAT: the range and the matrix (Tex::matrix) of every source of the launch (the host
+// keys the launches by both), so the range constants and the matrix coefficients of K1/K2 are immediates of the row loop
+// and take no registers there.  The luma table depends on the range alone.
 #pragma once
 
 namespace tma_int {
@@ -74,7 +75,7 @@ struct Cfg {
     static constexpr int SMEM = kGroups * GROUP_BYTES + kTailBytes + kLumaTabBytes;
 };
 
-template <int S, int SRC, bool FULL>
+template <int S, int SRC, bool FULL, int MAT>
 __global__ void __launch_bounds__(32 * kWarps * kGroups, 1) k_resample_tma3(const FusedJob *jobs, const FusedPiece *pieces, const int *piece_begin,
                                                                             int n_virtual_blocks) {
     using K = Cfg<S>;
@@ -91,6 +92,7 @@ __global__ void __launch_bounds__(32 * kWarps * kGroups, 1) k_resample_tma3(cons
     const uint32_t bar0 = smem_u32(tail + kBarOff) + 16u * (uint32_t)grp;
     // every source of the launch has the range FULL: the luma table is the block's
     constexpr float nk16 = FULL ? 0.0f : -K16, rcp_y = FULL ? 1.0f : RCP_Y, rcp_c = FULL ? 1.0f : RCP_C;
+    constexpr YuvCoef kc = yuv_coef(MAT);
     const uint32_t kaddr = setup_block<kGroups>(tail, [&] { fill_luma_table(tail, nk16, rcp_y); });
     const uint32_t ybase = luma_base(tail);
     const int vb = blockIdx.x * kGroups + grp;         // the host cut the launch for SMs x 3 eight-warp blocks
@@ -142,7 +144,7 @@ __global__ void __launch_bounds__(32 * kWarps * kGroups, 1) k_resample_tma3(cons
                 // A1: K1/K2 -> u8 -> sRGB decode, two pixels per instruction, luma from the luma table
                 float2 prg[P];   // (r, g) of pixel i
                 float pb[P];     // b of pixel i
-                convert_run<true>(yw, v, nk16, rcp_y, rcp_c, kaddr, prg, pb, ybase);
+                convert_run<true>(yw, v, nk16, rcp_y, rcp_c, kc, kaddr, prg, pb, ybase);
                 // A2: horizontal Lanczos along the warp.  acc j of the lane that owns tap 0 of output OUT * lane + j.
                 // The weights are compile-time constants (int_weights.h): every FFMA takes its weight as an immediate.
                 float2 arg[OUT];          // (r, g)

@@ -15,9 +15,10 @@ constexpr float kVcScaleC = 255.0f / 224.0f;  // f32(255 / 224)
 // store, alpha 255.  Packed RGBA, r in the low byte.
 __device__ __forceinline__ uint32_t vc_bt709_limited(float y, float cb, float cr) {
     const float s0 = (y - kVcBiasY) * kVcScaleY, s1 = (cb - 0.5f) * kVcScaleC, s2 = (cr - 0.5f) * kVcScaleC;
-    const uint32_t r = (uint32_t)unorm8(s0 + s2 * 1.5748f);
-    const uint32_t g = (uint32_t)unorm8((s0 + s1 * -0.1873f) + s2 * -0.4681f);
-    const uint32_t b = (uint32_t)unorm8(s0 + s1 * 1.8556f);
+    constexpr YuvCoef k = yuv_coef(0);
+    const uint32_t r = (uint32_t)unorm8(s0 + s2 * k.rv);
+    const uint32_t g = (uint32_t)unorm8((s0 + s1 * k.gu) + s2 * k.gv);
+    const uint32_t b = (uint32_t)unorm8(s0 + s1 * k.bu);
     return r | (g << 8) | (b << 16) | 0xff000000u;
 }
 

@@ -149,6 +149,18 @@ class FieldOrder:        # smr_field_order
     BottomFirst = F.FIELD_BOTTOM_FIRST
 
 
+class YuvMatrix:         # smr_yuv_matrix
+    Default = F.MATRIX_DEFAULT   # BT.709
+    BT709 = F.MATRIX_BT709
+    BT601 = F.MATRIX_BT601
+
+
+class YuvRange:          # smr_yuv_range
+    Default = F.RANGE_DEFAULT    # full for PLANAR_YUVJ420, limited for every other YUV format
+    Limited = F.RANGE_LIMITED
+    Full = F.RANGE_FULL
+
+
 @dataclass
 class Frame:
     data: FrameData
@@ -685,6 +697,12 @@ class Renderer:
         cfg = F.Deinterlace(int(mode), int(field_order), int(motion_threshold))
         self._check(self._lib.smr_set_input_deinterlace(self._h, input_id.encode(), C.byref(cfg)))
 
+    def set_input_color(self, input_id: str, matrix: int = YuvMatrix.Default, range: int = YuvRange.Default):
+        """the colour matrix (YuvMatrix) and range (YuvRange) a registered YUV input is converted with (smr_set_input_color);
+        Default keeps the format's rule, RGB inputs ignore the setting"""
+        c = F.InputColor(int(matrix), int(range))
+        self._check(self._lib.smr_set_input_color(self._h, input_id.encode(), C.byref(c)))
+
     def debug_input_planes(self, input_id: str) -> List[np.ndarray]:
         """the planes the kernels of the last render with a live frame of the input read for it, after deinterlacing: one
         (rows, row bytes) uint8 array per plane of the input's last frame passed to render / render_raw"""
@@ -1018,7 +1036,7 @@ class Renderer:
     def debug_fused_jobs(self):
         """The fused resample jobs of the last planned tick (smr_debug_fused_jobs), one dict per job in plan order:
         kernel ("ldg" / "tma_int" / "tma_any"), ratio, window, box, src_class, full_range, v_same, strip_cols,
-        src (w, h), dst (w, h), taps_h, taps_v, direct."""
+        src (w, h), dst (w, h), taps_h, taps_v, direct, matrix (YuvMatrix.BT709 / BT601)."""
         n = C.c_uint32()
         self._check(self._lib.smr_debug_fused_jobs(self._h, None, 0, C.byref(n)))
         arr = (F.FusedJobInfo * max(1, n.value))()
@@ -1060,7 +1078,7 @@ class Renderer:
         """The layers of the last planned tick's composite jobs (smr_debug_composite_layers), one dict per layer in job
         order, then painter's order: job, kernel ("p" / "multi"), layer, type, rotated, fast, box (12 ints: pixel box and
         both interior bars), tx_off, ty_off, mask_count, tex_kind, tex_width, tex_height, tex_pitch, tex_align, width,
-        height, out_format."""
+        height, out_format, tex_matrix (YuvMatrix.BT709 / BT601 for a YUV texture, else 0)."""
         n = C.c_uint32()
         self._check(self._lib.smr_debug_composite_layers(self._h, None, 0, C.byref(n)))
         arr = (F.CompositeLayerInfo * max(1, n.value))()

@@ -1,7 +1,7 @@
 """Instruction budget of the integer-ratio TMA resample kernel, read from the compiler's output (no GPU needed).
 
 Compiles smelter_b200/csrc/kernels.cu alone with the library's nvcc flags into a temporary cubin and prints, for every
-k_resample_tma3<S, SRC, FULL>: registers, spill stores / loads (ptxas -v), the kernel's SASS instruction count, and the
+k_resample_tma3<S, SRC, FULL, MAT>: registers, spill stores / loads (ptxas -v), the kernel's SASS instruction count, and the
 instruction count of the phase-A row loop (one warp, one source row: fetch, K1/K2, decode, horizontal pass, ring
 store) by opcode.  The row loop is the backward-branch loop of the kernel that holds the SHFL.UP of the horizontal pass.
 Then the same-ratio vertical pass of one step (one warp, two output rows): it is unrolled, so it is the branch-free run
@@ -136,8 +136,8 @@ def vertical_pass(ins, loop):
 
 
 def demangle_tma3(name):
-    m = re.search(r"k_resample_tma3ILi(\d)ELi(\d)ELb(\d)E", name)
-    return (int(m.group(1)), int(m.group(2)), int(m.group(3))) if m else None
+    m = re.search(r"k_resample_tma3ILi(\d)ELi(\d)ELb(\d)E(?:Li(\d)E)?", name)   # kernels without MAT are BT.709
+    return tuple(int(g or 0) for g in m.groups()) if m else None
 
 
 def short_names(names, cuobjdump_dir):
@@ -162,10 +162,10 @@ def main():
     regs = parse_ptxas(ptxas)
     funcs = parse_sass(sass)
     tma3 = sorted((demangle_tma3(n), n) for n in funcs if demangle_tma3(n))
-    for (S, SRC, FULL), name in tma3:
+    for (S, SRC, FULL, MAT), name in tma3:
         r, st, ld = regs.get(name, (0, 0, 0))
         loop = row_loop(funcs[name])
-        print(f"k_resample_tma3<{S},{SRC},{FULL}>: {r} registers, spill {st}/{ld} B, {len(funcs[name])} SASS; "
+        print(f"k_resample_tma3<{S},{SRC},{FULL},{MAT}>: {r} registers, spill {st}/{ld} B, {len(funcs[name])} SASS; "
               f"phase-A row loop {len(loop)} instructions")
         ops = collections.Counter(op for _, op, _ in loop)
         const = sum(n for op, n in ops.items() if op.startswith(("ULDC", "LDC")))
