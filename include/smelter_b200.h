@@ -729,6 +729,20 @@ typedef struct {
     int32_t matrix;                /* the source's matrix: SMR_MATRIX_BT709 or SMR_MATRIX_BT601 */
 } smr_fused_job_info;
 smr_status smr_debug_fused_jobs(smr_renderer *r, smr_fused_job_info *out, uint32_t cap, uint32_t *n);
+/* inspection (no handle, no device access): the fused resample kernel instantiations the library is compiled with, one
+ * record per instantiation.  A fused launch runs the jobs of one record, and a job whose record is missing fails its tick
+ * with SMR_ERR_CUDA.  *n is the record count; records go to `out` when they fit in cap (SMR_ERR_BUFFER_TOO_SMALL
+ * otherwise; out = NULL asks for the count). */
+typedef struct {
+    int32_t kernel;                /* smr_fused_kernel */
+    int32_t ratio;                 /* as in smr_fused_job_info */
+    int32_t window;                /* as in smr_fused_job_info: 20, 25, 29 or 33 slots for SMR_FUSED_TMA_ANY, else 0 */
+    int32_t box;                   /* as in smr_fused_job_info */
+    int32_t src_class;             /* 0 planar 4:2:0, 1 NV12, 2 UYVY, 3 YUYV */
+    int32_t range;                 /* the range the kernel is specialised for: 1 full; 0 limited, or read per job */
+    int32_t matrix;                /* smr_yuv_matrix: SMR_MATRIX_BT709 or SMR_MATRIX_BT601 */
+} smr_fused_variant_info;
+smr_status smr_debug_fused_variants(smr_fused_variant_info *out, uint32_t cap, uint32_t *n);
 
 /* inspection (no device access): the generic resample passes of the handle's most recently planned tick -- every
  * resampled child the fused kernels do not take -- one record per pass: box passes, then first passes, then last passes,

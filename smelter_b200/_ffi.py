@@ -193,6 +193,11 @@ class FusedJobInfo(C.Structure):   # smr_fused_job_info
                 ("taps_h", C.c_int32), ("taps_v", C.c_int32), ("direct", C.c_int32), ("matrix", C.c_int32)]
 
 
+class FusedVariantInfo(C.Structure):   # smr_fused_variant_info
+    _fields_ = [("kernel", C.c_int32), ("ratio", C.c_int32), ("window", C.c_int32), ("box", C.c_int32),
+                ("src_class", C.c_int32), ("range", C.c_int32), ("matrix", C.c_int32)]
+
+
 STAGE_BOX, STAGE_FIRST, STAGE_LAST = 0, 1, 2
 STAGE_SRC_RAW, STAGE_SRC_CONVERTED, STAGE_SRC_F16 = 0, 1, 2
 
@@ -260,7 +265,7 @@ EXPORTS = [
     "smr_debug_input_planes", "smr_register_image", "smr_unregister_image",
     "smr_register_svg_image",
     "smr_register_web_renderer", "smr_unregister_web_renderer", "smr_web_set_frame", "smr_web_set_child_rects", "smr_register_shader", "smr_unregister_shader", "smr_register_wgsl_shader", "smr_update_scene",
-    "smr_unregister_output", "smr_set_layouts", "smr_render", "smr_render_begin", "smr_render_end", "smr_preprocess_frame", "smr_premultiply_rgba8", "smr_transcode_resize", "smr_video_nv12_to_rgba", "smr_video_rgba_to_nv12", "smr_render_text", "smr_debug_partition", "smr_debug_tile_plan", "smr_debug_weights", "smr_debug_sincos", "smr_debug_transcode_taps", "smr_debug_fused_jobs", "smr_debug_resample_stages", "smr_debug_composite_layers", "smr_debug_interior", "smr_output_plane_sizes",
+    "smr_unregister_output", "smr_set_layouts", "smr_render", "smr_render_begin", "smr_render_end", "smr_preprocess_frame", "smr_premultiply_rgba8", "smr_transcode_resize", "smr_video_nv12_to_rgba", "smr_video_rgba_to_nv12", "smr_render_text", "smr_debug_partition", "smr_debug_tile_plan", "smr_debug_weights", "smr_debug_sincos", "smr_debug_transcode_taps", "smr_debug_fused_jobs", "smr_debug_fused_variants", "smr_debug_resample_stages", "smr_debug_composite_layers", "smr_debug_interior", "smr_output_plane_sizes",
     "smr_component_default", "smr_debug_layouts", "smr_debug_node_layouts", "smr_debug_image_nodes", "smr_debug_set_inputs", "smr_get_stats", "smr_set_profiling", "smr_get_kernel_times",
     "smr_comm_get_unique_id", "smr_comm_init", "smr_comm_broadcast_inputs", "smr_comm_exchange_inputs", "smr_comm_pull_inputs", "smr_peer_pool_alloc", "smr_peer_pool_open", "smr_peer_pool_close", "smr_peer_pool_free", "smr_comm_destroy", "smr_host_register", "smr_host_unregister", "smr_cuda_stream", "smr_last_error",
     "smr_version",
@@ -333,6 +338,8 @@ def lib():
     L.smr_debug_transcode_taps.restype = C.c_int32
     L.smr_debug_fused_jobs.argtypes = [vp, C.POINTER(FusedJobInfo), C.c_uint32, C.POINTER(C.c_uint32)]
     L.smr_debug_fused_jobs.restype = C.c_int32
+    L.smr_debug_fused_variants.argtypes = [C.POINTER(FusedVariantInfo), C.c_uint32, C.POINTER(C.c_uint32)]
+    L.smr_debug_fused_variants.restype = C.c_int32
     L.smr_debug_resample_stages.argtypes = [vp, C.POINTER(ResampleStageInfo), C.c_uint32, C.POINTER(C.c_uint32),
                                             C.POINTER(C.c_int32), C.c_uint32, C.POINTER(C.c_uint32)]
     L.smr_debug_resample_stages.restype = C.c_int32

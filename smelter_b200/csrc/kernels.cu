@@ -22,9 +22,12 @@
 
 #include <cstdio>
 #include <cstdlib>
+#include <algorithm>
 #include <atomic>
 #include <type_traits>
 #include <cstring>
+#include <utility>
+#include <vector>
 
 #include "kernels.h"
 #include "interior.h"
@@ -621,45 +624,6 @@ __global__ void __launch_bounds__(32 * W64_WARPS, 3) k_resample_fused_int(const 
     }  // pieces
 }
 
-template <int S, int SRC, int MAT, bool FULL>
-static bool launch_fused_kernel(const FusedJob *jobs_dev, const FusedPiece *pieces, const int *piece_begin, int nblocks,
-                                cudaStream_t s) {
-    // the attribute is per device: several handles of one process may drive different GPUs from different threads
-    static std::atomic<unsigned long long> done{0};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    const unsigned long long bit = 1ull << (dev & 63);
-    if (!(done.load(std::memory_order_acquire) & bit)) {
-        cudaFuncSetAttribute(k_resample_fused_int<S, SRC, MAT, FULL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             (int)sizeof(typename W64<S>::Smem));
-        done.fetch_or(bit, std::memory_order_release);
-    }
-    k_resample_fused_int<S, SRC, MAT, FULL><<<nblocks, dim3(32, W64_WARPS), sizeof(typename W64<S>::Smem), s>>>(jobs_dev, pieces, piece_begin);
-    return check_launch("k_resample_fused_int");
-}
-
-// the range is a template parameter for the interleaved sources only (k_resample_fused_int's FULL)
-template <int S, int SRC>
-static bool launch_fused_int(const FusedJob *jobs_dev, const FusedPiece *pieces, const int *piece_begin, int nblocks, int full_range,
-                             int matrix, cudaStream_t s) {
-    constexpr bool IL = SRC >= 2;
-    if (IL && full_range) return matrix ? launch_fused_kernel<S, SRC, 1, IL>(jobs_dev, pieces, piece_begin, nblocks, s)
-                                        : launch_fused_kernel<S, SRC, 0, IL>(jobs_dev, pieces, piece_begin, nblocks, s);
-    return matrix ? launch_fused_kernel<S, SRC, 1, false>(jobs_dev, pieces, piece_begin, nblocks, s)
-                  : launch_fused_kernel<S, SRC, 0, false>(jobs_dev, pieces, piece_begin, nblocks, s);
-}
-
-template <int S>
-static bool launch_fused_src(int src, int full_range, int matrix, const FusedJob *jobs_dev, const FusedPiece *pieces_dev,
-                             const int *piece_begin_dev, int nblocks, cudaStream_t st) {
-    switch (src) {
-        case 0: return launch_fused_int<S, 0>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, full_range, matrix, st);
-        case 1: return launch_fused_int<S, 1>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, full_range, matrix, st);
-        case 2: return launch_fused_int<S, 2>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, full_range, matrix, st);
-        default: return launch_fused_int<S, 3>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, full_range, matrix, st);
-    }
-}
-
 }  // namespace dev
 }  // namespace smr
 namespace smr {
@@ -731,95 +695,91 @@ __device__ __forceinline__ void emit_yuv_2x2(const FusedJob &J, int X, int Y, ui
 #include "resample_tma3.cuh"
 #include "resample_tma0.cuh"
 
-template <int SRC, int WINP, int BOX, int MAT>
-static bool launch_tma0_mat(const FusedJob *jobs_dev, const FusedPiece *pieces, const int *piece_begin, int nblocks, cudaStream_t s) {
-    static std::atomic<unsigned long long> done{0};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    const unsigned long long bit = 1ull << (dev & 63);
-    if (!(done.load(std::memory_order_acquire) & bit)) {
-        cudaFuncSetAttribute(tma_any::k_resample_tma0<SRC, WINP, BOX, MAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, tma_any::Cfg::SMEM);
-        done.fetch_or(bit, std::memory_order_release);
-    }
-    const int grid = (nblocks + tma_any::kGroups - 1) / tma_any::kGroups;
-    tma_any::k_resample_tma0<SRC, WINP, BOX, MAT><<<grid, dim3(32, tma::kWarps * tma_any::kGroups), tma_any::Cfg::SMEM, s>>>(jobs_dev, pieces, piece_begin, nblocks);
-    return check_launch("k_resample_tma0");
+// ------------------------------------------------------------------------------------------------
+// The compiled instantiations of the three fused kernel families, one table built once from each family's template
+// parameter lists: launch_resample_fused looks a launch's variant up here and launches the entry's kernel
+// ------------------------------------------------------------------------------------------------
+struct FusedEntry {
+    FusedVariant key;
+    const void *fn;     // the __global__ function
+    int smem;           // dynamic shared memory, bytes
+    dim3 block;
+    int groups;         // eight-warp groups per block: the host cuts a launch's work for nblocks groups
+    const char *name;   // in a launch error
+};
+
+template <int... V> using ints = std::integer_sequence<int, V...>;
+// f(a, b, ...) for every combination of a in the first list, b in the second, ..., each a std::integral_constant
+template <class F> static void each(F &&f) { f(); }
+template <class F, int... V, class... Lists> static void each(F &&f, ints<V...>, Lists... rest);
+template <class F, class C, class... Lists> static void each_with(F &f, C c, Lists... rest) {   // f(c, ...) over the rest
+    each([&](auto... tail) { f(c, tail...); }, rest...);
 }
-template <int SRC, int WINP, int BOX>
-static bool launch_tma0(const FusedJob *jobs_dev, const FusedPiece *pieces, const int *piece_begin, int nblocks, int matrix, cudaStream_t s) {
-    return matrix ? launch_tma0_mat<SRC, WINP, BOX, 1>(jobs_dev, pieces, piece_begin, nblocks, s)
-                  : launch_tma0_mat<SRC, WINP, BOX, 0>(jobs_dev, pieces, piece_begin, nblocks, s);
+template <class F, int... V, class... Lists> static void each(F &&f, ints<V...>, Lists... rest) {
+    (each_with(f, std::integral_constant<int, V>{}, rest...), ...);
 }
 
-template <int WINP>
-static bool launch_tma0_src(int src, int box, int matrix, const FusedJob *jobs_dev, const FusedPiece *pieces, const int *piece_begin,
-                            int nblocks, cudaStream_t s) {
-    if (box) return src == 1 ? launch_tma0<1, WINP, 1>(jobs_dev, pieces, piece_begin, nblocks, matrix, s)
-                             : launch_tma0<0, WINP, 1>(jobs_dev, pieces, piece_begin, nblocks, matrix, s);
-    return src == 1 ? launch_tma0<1, WINP, 0>(jobs_dev, pieces, piece_begin, nblocks, matrix, s)
-                    : launch_tma0<0, WINP, 0>(jobs_dev, pieces, piece_begin, nblocks, matrix, s);
+static const std::vector<FusedEntry> &fused_table() {
+    static const std::vector<FusedEntry> table = [] {
+        std::vector<FusedEntry> t;
+        using two = ints<0, 1>;
+        // k_resample_fused_int: any ratio (0) or 2 / 3 / 4, every source class; the range is a parameter of the interleaved
+        // sources only
+        each([&](auto S, auto SRC, auto MAT, auto FULL) {
+            if constexpr (!FULL || SRC >= 2)
+                t.push_back({{FusedVariant::LDG, S, 0, 0, SRC, FULL, MAT}, (const void *)k_resample_fused_int<S, SRC, MAT, FULL != 0>,
+                             (int)sizeof(typename W64<S>::Smem), dim3(32, W64_WARPS), 1, "k_resample_fused_int"});
+        }, ints<0, 2, 3, 4>{}, ints<0, 1, 2, 3>{}, two{}, two{});
+        // k_resample_tma3: ratio 2 / 4 on planar 4:2:0 and NV12
+        each([&](auto S, auto SRC, auto FULL, auto MAT) {
+            t.push_back({{FusedVariant::TMA_INT, S, 0, 0, SRC, FULL, MAT}, (const void *)tma_int::k_resample_tma3<S, SRC, FULL != 0, MAT>,
+                         tma_int::Cfg<S>::SMEM, dim3(32, tma::kWarps * tma_int::kGroups), tma_int::kGroups, "k_resample_tma3"});
+        }, ints<2, 4>{}, two{}, two{}, two{});
+        // k_resample_tma0: planar 4:2:0 and NV12, every window of kTma0Window, with and without the box reduction
+        each([&](auto SRC, auto W, auto BOX, auto MAT) {
+            t.push_back({{FusedVariant::TMA_ANY, 0, W, BOX, SRC, 0, MAT}, (const void *)tma_any::k_resample_tma0<SRC, kTma0Window[W], BOX, MAT>,
+                         tma_any::Cfg::SMEM, dim3(32, tma::kWarps * tma_any::kGroups), tma_any::kGroups, "k_resample_tma0"});
+        }, two{}, ints<0, 1, 2, 3>{}, two{}, two{});
+        return t;
+    }();
+    return table;
 }
 
-template <int S, int SRC, bool FULL, int MAT>
-static bool launch_tma3_range(const FusedJob *jobs_dev, const FusedPiece *pieces, const int *piece_begin, int nblocks, cudaStream_t s) {
-    static std::atomic<unsigned long long> done{0};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    const unsigned long long bit = 1ull << (dev & 63);
-    if (!(done.load(std::memory_order_acquire) & bit)) {
-        cudaFuncSetAttribute(tma_int::k_resample_tma3<S, SRC, FULL, MAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, tma_int::Cfg<S>::SMEM);
-        done.fetch_or(bit, std::memory_order_release);
-    }
-    const int grid = (nblocks + tma_int::kGroups - 1) / tma_int::kGroups;   // the host cut the work for `nblocks` eight-warp groups
-    tma_int::k_resample_tma3<S, SRC, FULL, MAT><<<grid, dim3(32, tma::kWarps * tma_int::kGroups), tma_int::Cfg<S>::SMEM, s>>>(
-        jobs_dev, pieces, piece_begin, nblocks);
-    return check_launch("k_resample_tma3");
-}
-template <int S, int SRC>
-static bool launch_tma3(const FusedJob *jobs_dev, const FusedPiece *pieces, const int *piece_begin, int nblocks, int full_range,
-                        int matrix, cudaStream_t s) {
-    if (matrix) return full_range ? launch_tma3_range<S, SRC, true, 1>(jobs_dev, pieces, piece_begin, nblocks, s)
-                                  : launch_tma3_range<S, SRC, false, 1>(jobs_dev, pieces, piece_begin, nblocks, s);
-    return full_range ? launch_tma3_range<S, SRC, true, 0>(jobs_dev, pieces, piece_begin, nblocks, s)
-                      : launch_tma3_range<S, SRC, false, 0>(jobs_dev, pieces, piece_begin, nblocks, s);
+int fused_variants(FusedVariant *out, int cap) {
+    const std::vector<FusedEntry> &table = fused_table();
+    for (int i = 0; i < cap && i < (int)table.size(); i++) out[i] = table[i].key;
+    return (int)table.size();
 }
 
-// src: 0 planar 4:2:0, 1 NV12, 2 UYVY, 3 YUYV (fused_source_class)
-int launch_resample_fused(const FusedKernel &k, int src, int full_range, int matrix, const FusedJob *jobs_dev,
-                          const FusedPiece *pieces_dev, const int *piece_begin_dev, int nblocks, Stream s) {
-    if (nblocks <= 0) return 0;
-    cudaStream_t st = (cudaStream_t)s;
-    bool ok = false;
+int launch_resample_fused(const FusedVariant &v, const FusedJob *jobs_dev, const FusedPiece *pieces_dev, const int *piece_begin_dev,
+                          int nblocks, Stream s) {
     static_assert(tma_int::Cfg<4>::NOUT == kTmaStripCols4 && tma_int::Cfg<2>::NOUT == kTmaStripCols2 &&
                   tma_int::Cfg<4>::RROWS == kTmaRing4 && tma_int::Cfg<2>::RROWS == kTmaRing2, "integer-ratio kernel");
     static_assert(tma_any::kGroups == kTma0Groups && tma_any::Cfg::MAXT == kTma0MaxTaps && tma_any::Cfg::WINP_MAX == kTma0Window[3] &&
                   tma_any::Cfg::RROWS == kTmaRing4, "any-ratio kernel");
     static_assert(tma::kLumaBox == 2 * kTmaLumaBoxW && tma::kChunkRows == kTmaLumaBoxH && tma::kNv12Box == 2 * kTmaNv12BoxW &&
                   tma::kPlanarBox == kTmaPlanarBoxW && tma::kChromaRows == kTmaChromaBoxH, "TMA boxes");
-    switch (k.kind) {
-        case FusedKernel::TMA_ANY:
-            switch (k.window) {
-                case 0: ok = launch_tma0_src<kTma0Window[0]>(src, k.box, matrix, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
-                case 1: ok = launch_tma0_src<kTma0Window[1]>(src, k.box, matrix, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
-                case 2: ok = launch_tma0_src<kTma0Window[2]>(src, k.box, matrix, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
-                default: ok = launch_tma0_src<kTma0Window[3]>(src, k.box, matrix, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
-            }
-            break;
-        case FusedKernel::TMA_INT:
-            if (k.ratio == 4) ok = src == 1 ? launch_tma3<4, 1>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, full_range, matrix, st)
-                                            : launch_tma3<4, 0>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, full_range, matrix, st);
-            else ok = src == 1 ? launch_tma3<2, 1>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, full_range, matrix, st)
-                               : launch_tma3<2, 0>(jobs_dev, pieces_dev, piece_begin_dev, nblocks, full_range, matrix, st);
-            break;
-        default:
-            switch (k.ratio) {
-                case 2: ok = launch_fused_src<2>(src, full_range, matrix, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
-                case 3: ok = launch_fused_src<3>(src, full_range, matrix, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
-                case 4: ok = launch_fused_src<4>(src, full_range, matrix, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
-                default: ok = launch_fused_src<0>(src, full_range, matrix, jobs_dev, pieces_dev, piece_begin_dev, nblocks, st); break;
-            }
+    if (nblocks <= 0) return 0;
+    const std::vector<FusedEntry> &table = fused_table();
+    const auto e = std::find_if(table.begin(), table.end(), [&](const FusedEntry &x) { return x.key == v; });
+    if (e == table.end()) {
+        snprintf(g_err, sizeof(g_err), "no fused resample kernel for kind %d, ratio %d, window %d, box %d, source class %d, range %d, matrix %d",
+                 (int)v.kind, v.ratio, v.window, v.box, v.src, v.range, v.matrix);
+        return -1;
     }
-    return ok ? 1 : -1;
+    // the attribute is per device: several handles of one process may drive different GPUs from different threads
+    static std::vector<std::atomic<unsigned long long>> attr_set(table.size());
+    std::atomic<unsigned long long> &done = attr_set[e - table.begin()];
+    int dev = 0;
+    cudaGetDevice(&dev);
+    const unsigned long long bit = 1ull << (dev & 63);
+    if (!(done.load(std::memory_order_acquire) & bit)) {
+        cudaFuncSetAttribute(e->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, e->smem);
+        done.fetch_or(bit, std::memory_order_release);
+    }
+    void *args[] = {(void *)&jobs_dev, (void *)&pieces_dev, (void *)&piece_begin_dev, (void *)&nblocks};   // k_resample_fused_int takes the first three
+    cudaLaunchKernel(e->fn, dim3((nblocks + e->groups - 1) / e->groups), e->block, args, (size_t)e->smem, (cudaStream_t)s);
+    return check_launch(e->name) ? 1 : -1;
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -176,9 +176,9 @@ constexpr int kTmaLumaBoxW = 136, kTmaLumaBoxH = 32, kTmaNv12BoxW = 144, kTmaPla
 constexpr int kTma0Groups = 2, kTma0MaxSpan = 256, kTma0MaxTaps = 25;
 constexpr int kTma0Window[4] = {20, 25, 29, 33};
 
-// Which kernel resamples a FusedJob (host side only; every job of one launch has the same kernel, source class and
-// launch range)
-struct FusedKernel {
+// Which kernel instantiation resamples a FusedJob, and so the key of a launch: every job of one launch has the same
+// variant (host side only)
+struct FusedVariant {
     enum Kind : int32_t {
         LDG,      // k_resample_fused_int: LDG-staged, weights from smem (ratio 0) or from int_weights.h (integer ratio 2 / 3 / 4)
         TMA_INT,  // k_resample_tma3 (resample_tma3.cuh): integer ratio 2 / 4, TMA-staged, weights from int_weights.h
@@ -186,7 +186,13 @@ struct FusedKernel {
                   // with `box` on a source box-reduced 2:1
     } kind = LDG;
     int32_t ratio = 0, window = 0, box = 0;
-    bool operator==(const FusedKernel &o) const { return kind == o.kind && ratio == o.ratio && window == o.window && box == o.box; }
+    int32_t src = 0;      // source class (fused_source_class)
+    int32_t range = 0;    // fused_launch_range
+    int32_t matrix = 0;   // Tex::matrix of the source
+    bool operator==(const FusedVariant &o) const {
+        return kind == o.kind && ratio == o.ratio && window == o.window && box == o.box && src == o.src && range == o.range &&
+               matrix == o.matrix;
+    }
 };
 // What a launch of a fused kernel needs to know: output columns per strip of job `j`, blocks (eight-warp groups) per SM
 // of the persistent grid, and the rows a block's share of the partition is a multiple of
@@ -195,18 +201,18 @@ struct FusedShape { int strip_cols, groups_per_sm, row_gran; };
 inline int fused_source_class(int tex_kind) {
     return tex_kind == TEX_YUV420 ? 0 : tex_kind == TEX_NV12 ? 1 : tex_kind == TEX_UYVY ? 2 : tex_kind == TEX_YUYV ? 3 : -1;
 }
-// The source range a launch of kernel k is specialised for (1 full, 0 limited): the integer-ratio TMA kernel builds a luma
-// table for one range, and the LDG kernel's interleaved readers take it as a template parameter, so their launches are
-// single-range; every other reader takes the range per job (0).  The matrix (Tex::matrix) is a template parameter of every
-// fused kernel: a launch key is (kernel, source class, range, matrix).
-inline int fused_launch_range(const FusedKernel &k, const FusedJob &j) {
-    const bool keyed = k.kind == FusedKernel::TMA_INT || (k.kind == FusedKernel::LDG && fused_source_class(j.src.kind) >= 2);
-    return keyed && j.src.full_range ? 1 : 0;
+// The source range a launch of variant v (its kind and src) is specialised for, given the source's full_range (1 full, 0
+// limited): the integer-ratio TMA kernel builds a luma table for one range, and the LDG kernel's interleaved readers take it
+// as a template parameter, so their launches are single-range; every other reader takes the range per job (0).  The matrix
+// (Tex::matrix) is a template parameter of every fused kernel.
+inline int fused_launch_range(const FusedVariant &v, int full_range) {
+    const bool keyed = v.kind == FusedVariant::TMA_INT || (v.kind == FusedVariant::LDG && v.src >= 2);
+    return keyed && full_range ? 1 : 0;
 }
-inline FusedShape fused_shape(const FusedKernel &k, const FusedJob &j) {
+inline FusedShape fused_shape(const FusedVariant &k, const FusedJob &j) {
     switch (k.kind) {
-        case FusedKernel::TMA_INT: return {k.ratio == 4 ? kTmaStripCols4 : kTmaStripCols2, 3, 2};
-        case FusedKernel::TMA_ANY: return {j.strip_cols, kTma0Groups, 8};
+        case FusedVariant::TMA_INT: return {k.ratio == 4 ? kTmaStripCols4 : kTmaStripCols2, 3, 2};
+        case FusedVariant::TMA_ANY: return {j.strip_cols, kTma0Groups, 8};
         default: return {kFusedStripCols, 3, 8};
     }
 }
@@ -371,9 +377,13 @@ int launch_tile_jobs(const void *kernel, const void *jobs_dev, const int32_t *ti
                      const char *name, Stream s);
 enum NodeKernel { NODE_TEXT, NODE_IMAGE, NODE_WEB };   // k_text (TextJob), k_image (ImageJob), k_web (WebJob)
 const void *node_kernel(NodeKernel k);
-// full_range: fused_launch_range of every job of the launch; matrix: src.matrix of every job of the launch
-int launch_resample_fused(const FusedKernel &k, int src, int full_range, int matrix, const FusedJob *jobs_dev,
-                          const FusedPiece *pieces_dev, const int *piece_begin_dev, int nblocks, Stream s);
+// the fused resample of every job of a launch, all of variant v, on `nblocks` eight-warp groups.  -1 with a launch error
+// naming v when the library compiles no instantiation of v
+int launch_resample_fused(const FusedVariant &v, const FusedJob *jobs_dev, const FusedPiece *pieces_dev, const int *piece_begin_dev,
+                          int nblocks, Stream s);
+// the variants launch_resample_fused accepts, one per compiled kernel instantiation: the first min(count, cap) go to
+// `out`; returns the count
+int fused_variants(FusedVariant *out, int cap);
 // every output of a tick in one launch; jobs_dev[i] == jobs_host[i], layers / masks / textures device pointers.  One output
 // with a short layer list (layers0_host: host copy of jobs_host[0].layers) passes job and layers in the parameter block
 int launch_composite(const CompositeJob *jobs_dev, const CompositeJob *jobs_host, const LayerDev *layers0_host, int n, Stream s);

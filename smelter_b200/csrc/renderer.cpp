@@ -674,7 +674,7 @@ class Renderer {
     };
     struct FusedRec {
         dev::FusedJob job;
-        dev::FusedKernel kernel;
+        dev::FusedVariant key;  // its kernel instantiation: the key of its launch
         int src_tex;            // the job's source (texture table)
         size_t dst_off;         // frame-arena offset of its RGBA8 output
         int tmap_idx;           // first of its three entries in `tmaps`, or -1
@@ -695,13 +695,7 @@ class Renderer {
         std::vector<uint32_t> list;
         size_t list_off = SIZE_MAX;       // param-arena offset of `list`
     };
-    struct FusedKey {           // the fused jobs one launch runs: same kernel, source class, launch range and matrix
-        dev::FusedKernel kernel; int src, range, matrix;
-        bool operator==(const FusedKey &o) const {
-            return kernel == o.kernel && src == o.src && range == o.range && matrix == o.matrix;
-        }
-    };
-    struct FusedLaunch { FusedKey key; size_t pieces_off, begin_off; int nblocks; };
+    struct FusedLaunch { dev::FusedVariant key; size_t pieces_off, begin_off; int nblocks; };
     // One launch of a node-texture kernel (launch_tile_jobs): launch_tick enqueues it after phase `phase`'s composite (-1:
     // before the conversions)
     struct NodeLaunch {
@@ -1681,6 +1675,17 @@ static void apply_input_color(const smr_input_color &c, dev::Tex &t) {
 static int32_t public_matrix(const dev::Tex &t) {
     return !tex_is_yuv(t) ? 0 : t.matrix == 1 ? SMR_MATRIX_BT601 : SMR_MATRIX_BT709;
 }
+static smr_fused_variant_info public_variant(const dev::FusedVariant &v) {
+    smr_fused_variant_info o{};
+    o.kernel = v.kind == dev::FusedVariant::TMA_INT ? SMR_FUSED_TMA_INT : v.kind == dev::FusedVariant::TMA_ANY ? SMR_FUSED_TMA_ANY : SMR_FUSED_LDG;
+    o.ratio = v.ratio;
+    o.window = v.kind == dev::FusedVariant::TMA_ANY ? dev::kTma0Window[v.window] : 0;
+    o.box = v.box;
+    o.src_class = v.src;
+    o.range = v.range;
+    o.matrix = v.matrix == 1 ? SMR_MATRIX_BT601 : SMR_MATRIX_BT709;
+    return o;
+}
 
 static void set_tex_plane(dev::Tex &t, int p, const uint8_t *ptr, size_t pitch) {
     (p == 0 ? t.p0 : p == 1 ? t.p1 : t.p2) = ptr;
@@ -1871,12 +1876,12 @@ int Renderer::try_fused_resample(Input &in, const AxisMapping &hm_in, const Axis
     // descriptor can address (16-byte aligned rows), even target width, the vertical footprint of 8 output rows inside the ring
     const bool tma = src_class < 2 && (dw & 1) == 0;
     const int rows8 = (int)std::ceil((dev::kFusedWarps - 1) * sv) + tv + 1;
-    dev::FusedKernel k;   // LDG, weights from smem
+    dev::FusedVariant k;   // LDG, weights from smem
     int tmap_idx = -1, cols = 64;
     if (!box && hm.crop_offset == 0.0f && (sh == 2.0f || sh == 3.0f || sh == 4.0f)) k.ratio = (int)sh;   // LDG, int_weights.h
     if (tma && (k.ratio == 2 || k.ratio == 4) && rows8 <= (k.ratio == 4 ? dev::kTmaRing4 : dev::kTmaRing2) &&
         (tmap_idx = source_tmaps(t, src_class)) >= 0) {
-        k.kind = dev::FusedKernel::TMA_INT;
+        k.kind = dev::FusedVariant::TMA_INT;
     } else if (tma && th <= dev::kTma0MaxTaps && rows8 <= dev::kTmaRing4) {
         // any other ratio <= 4 (fractional, 3, with a crop offset, box-reduced): the any-ratio TMA kernel; its strips are
         // narrowed so that a strip's source span fits the 256 pixels a warp converts per row (= 128 reduced ones)
@@ -1891,9 +1896,12 @@ int Renderer::try_fused_resample(Input &in, const AxisMapping &hm_in, const Axis
         int bucket = 0;
         while (bucket < 4 && dev::kTma0Window[bucket] < winp) bucket++;
         if (bucket < 4 && span(cols) <= max_span && (tmap_idx = source_tmaps(t, src_class)) >= 0)
-            k = {dev::FusedKernel::TMA_ANY, 0, bucket, box ? 1 : 0};
+            k = {dev::FusedVariant::TMA_ANY, 0, bucket, box ? 1 : 0};
     }
-    if (box && k.kind != dev::FusedKernel::TMA_ANY) return -1;   // no other fused kernel reduces: generic passes
+    if (box && k.kind != dev::FusedVariant::TMA_ANY) return -1;   // no other fused kernel reduces: generic passes
+    k.src = src_class;
+    k.range = dev::fused_launch_range(k, t.full_range);
+    k.matrix = t.matrix;
     const WeightEntry *wh, *wv;
     if (get_weights(passes[0], wh) != SMR_OK || get_weights(passes[1], wv) != SMR_OK) return -2;
     size_t dst_off = frame_alloc((size_t)dw * dh * 4);
@@ -1902,8 +1910,8 @@ int Renderer::try_fused_resample(Input &in, const AxisMapping &hm_in, const Axis
     j.taps_h = wh->taps; j.taps_v = wv->taps;
     j.w_h = wh->weights; j.inv_h = wh->inv; j.first_h = wh->first;
     j.w_v = wv->weights; j.inv_v = wv->inv; j.first_v = wv->first;
-    if (k.kind == dev::FusedKernel::TMA_INT) j.v_same = vm.crop_offset == 0.0f && sv == sh && tv == th;
-    if (k.kind == dev::FusedKernel::TMA_ANY) {
+    if (k.kind == dev::FusedVariant::TMA_INT) j.v_same = vm.crop_offset == 0.0f && sv == sh && tv == th;
+    if (k.kind == dev::FusedVariant::TMA_ANY) {
         j.strip_cols = cols;
         j.lane_perm = lane_perm(sh, hm.crop_offset, dw, cols);   // nullptr (identity) if the table could not be made
     }
@@ -2705,7 +2713,7 @@ void Renderer::plan_tiles(Output &o, CompositeRec &pc, const std::vector<dev::La
             // 4:1 only: per OUTPUT pixel the emission costs the resample kernel about what it saves the composite; at 2:1 a
             // quarter as many source pixels stand behind each output pixel and the vertical pass (four of a group's eight
             // warps) becomes the longer leg -- measured: 4:1 grid +4 %, 2:1 grid -2 %
-            if (f.kernel.kind != dev::FusedKernel::TMA_INT || f.kernel.ratio != 4 || !fj.v_same || ((fj.dst_w | fj.dst_h) & 1)) continue;
+            if (f.key.kind != dev::FusedVariant::TMA_INT || f.key.ratio != 4 || !fj.v_same || ((fj.dst_w | fj.dst_h) & 1)) continue;
             if ((L.tx_off & 1) || (L.ty_off & 1)) continue;   // frame position of texel (0, 0) = (-tx_off, -ty_off)
             // the whole child inside the frame: the kernel maps EVERY pixel of the job to a tile of the map, so a child hanging
             // over an edge (overflow: visible, absolute positions) would index tiles that do not exist
@@ -3183,21 +3191,18 @@ smr_status Renderer::resolve_frame_arena() {
     return SMR_OK;
 }
 
-// The tick's fused resamples over a persistent grid, one launch per kernel, source class, launch range and matrix; runs before the
-// composites' tile lists are packed, as a job cut at an odd row gives its direct tiles back to its composite
+// The tick's fused resamples over a persistent grid, one launch per kernel variant; runs before the composites' tile lists
+// are packed, as a job cut at an odd row gives its direct tiles back to its composite
 void Renderer::plan_fused_launches() {
-    auto key_of = [](const FusedRec &f) {
-        return FusedKey{f.kernel, dev::fused_source_class(f.job.src.kind), dev::fused_launch_range(f.kernel, f.job), f.job.src.matrix};
-    };
     for (size_t i = 0; i < plan_.fused.size(); i++) {
-        const FusedKey v = key_of(plan_.fused[i]);
-        if (std::any_of(plan_.fused.begin(), plan_.fused.begin() + i, [&](const FusedRec &f) { return key_of(f) == v; })) continue;
+        const dev::FusedVariant &v = plan_.fused[i].key;
+        if (std::any_of(plan_.fused.begin(), plan_.fused.begin() + i, [&](const FusedRec &f) { return f.key == v; })) continue;
         std::vector<int> idx, widths, heights, cols;
         dev::FusedShape shape{};
         for (size_t ji = i; ji < plan_.fused.size(); ji++) {
             const FusedRec &f = plan_.fused[ji];
-            if (!(key_of(f) == v)) continue;
-            shape = dev::fused_shape(f.kernel, f.job);
+            if (!(f.key == v)) continue;
+            shape = dev::fused_shape(f.key, f.job);
             idx.push_back((int)ji); widths.push_back(f.job.dst_w); heights.push_back(f.job.dst_h); cols.push_back(shape.strip_cols);
         }
         std::vector<dev::FusedPiece> pieces;
@@ -3353,9 +3358,9 @@ smr_status Renderer::launch_tick() {
                                       (int)plan_.weight_jobs.size(), stream_), SMR_KERNEL_WEIGHTS)) return SMR_ERR_CUDA;
     new_weight_keys_.clear();   // the tables are being computed on the stream: the cache entries are good
     for (const FusedLaunch &fl : plan_.fused_launches)
-        if (!launched(dev::launch_resample_fused(fl.key.kernel, fl.key.src, fl.key.range, fl.key.matrix, (const dev::FusedJob *)(pd + plan_.fused_off),
-                                                 (const dev::FusedPiece *)(pd + fl.pieces_off), (const int *)(pd + fl.begin_off),
-                                                 fl.nblocks, stream_), SMR_KERNEL_RESAMPLE_FUSED)) return SMR_ERR_CUDA;
+        if (!launched(dev::launch_resample_fused(fl.key, (const dev::FusedJob *)(pd + plan_.fused_off), (const dev::FusedPiece *)(pd + fl.pieces_off),
+                                                 (const int *)(pd + fl.begin_off), fl.nblocks, stream_), SMR_KERNEL_RESAMPLE_FUSED))
+            return SMR_ERR_CUDA;
     for (size_t p = 0; p + 1 < plan_.phases.size(); p++) {
         const TickPlan::Phase &b = plan_.phases[p], &e = plan_.phases[p + 1];
         for (int s = 0; s < 3; s++) {
@@ -3420,16 +3425,11 @@ smr_status Renderer::debug_fused_jobs(smr_fused_job_info *out, uint32_t cap, uin
         const FusedRec &f = plan_.fused[i];
         const dev::FusedJob &j = f.job;
         smr_fused_job_info &o = out[i];
-        o.kernel = f.kernel.kind == dev::FusedKernel::TMA_INT   ? SMR_FUSED_TMA_INT
-                   : f.kernel.kind == dev::FusedKernel::TMA_ANY ? SMR_FUSED_TMA_ANY
-                                                                : SMR_FUSED_LDG;
-        o.ratio = f.kernel.ratio;
-        o.window = f.kernel.kind == dev::FusedKernel::TMA_ANY ? dev::kTma0Window[f.kernel.window] : 0;
-        o.box = f.kernel.box;
-        o.src_class = dev::fused_source_class(j.src.kind);
+        const smr_fused_variant_info v = public_variant(f.key);
+        o.kernel = v.kernel; o.ratio = v.ratio; o.window = v.window; o.box = v.box; o.src_class = v.src_class;
         o.full_range = j.src.full_range;
         o.v_same = j.v_same;
-        o.strip_cols = dev::fused_shape(f.kernel, j).strip_cols;
+        o.strip_cols = dev::fused_shape(f.key, j).strip_cols;
         o.src_width = (uint32_t)j.src.width; o.src_height = (uint32_t)j.src.height;
         o.dst_width = (uint32_t)j.dst_w; o.dst_height = (uint32_t)j.dst_h;
         o.taps_h = j.taps_h; o.taps_v = j.taps_v;
@@ -4024,6 +4024,16 @@ smr_status smr_debug_image_nodes(smr_renderer *r, const char *output_id, uint64_
                                  uint32_t *n) { SMR_GUARD(r->impl.debug_image_nodes(output_id, pts, out, cap, n)) }
 smr_status smr_debug_set_inputs(smr_renderer *r, uint64_t pts, const smr_input_frame *in, uint32_t n_in) { SMR_GUARD(r->impl.debug_set_inputs(pts, in, n_in)) }
 smr_status smr_debug_fused_jobs(smr_renderer *r, smr_fused_job_info *out, uint32_t cap, uint32_t *n) { SMR_GUARD(r->impl.debug_fused_jobs(out, cap, n)) }
+smr_status smr_debug_fused_variants(smr_fused_variant_info *out, uint32_t cap, uint32_t *n) {
+    if (!n) return SMR_ERR_INVALID_ARGUMENT;
+    std::vector<smr::dev::FusedVariant> v(smr::dev::fused_variants(nullptr, 0));
+    smr::dev::fused_variants(v.data(), (int)v.size());
+    *n = (uint32_t)v.size();
+    if (!out) return SMR_OK;
+    if (cap < v.size()) return SMR_ERR_BUFFER_TOO_SMALL;
+    for (size_t i = 0; i < v.size(); i++) out[i] = smr::public_variant(v[i]);
+    return SMR_OK;
+}
 smr_status smr_debug_composite_layers(smr_renderer *r, smr_composite_layer_info *out, uint32_t cap, uint32_t *n) {
     SMR_GUARD(r->impl.debug_composite_layers(out, cap, n))
 }

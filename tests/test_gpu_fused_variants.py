@@ -9,8 +9,8 @@ RGBA output byte for byte with the oracle fed the same layouts.  The children ar
 the output bytes are the fused kernel's bytes.
 
 - `REGISTRY`: one scene per reachable (kernel, ratio or window, box, source class) instantiation, for k_resample_tma3
-  also per source range and per vertical path (`v_same`).  `test_registry_covers_every_instantiation` derives the set of
-  instantiations from the launch switch in kernels.cu and fails when one has no scene.
+  also per source range and per vertical path (`v_same`).  `test_registry_covers_every_compiled_variant` reads the set of
+  instantiations from the library (`smr_debug_fused_variants`) and fails when one has no scene.
 - Geometry edges of each kernel family on planar and NV12 sources: the last strip, tiny and odd sizes, sources smaller
   than one TMA box, tiles that end at the image edge, crop offsets, two crops of one input.
 - Content that hits every byte code in each plane, with runs of alternating 0 / 255 across strip and tile boundaries.
@@ -19,8 +19,6 @@ the output bytes are the fused kernel's bytes.
 - Direct tiles (the fused kernel writing output YUV itself) in a launch whose partition cuts the second job at odd rows.
 """
 import ctypes as C
-import os
-import re
 from dataclasses import dataclass, field
 from typing import Optional, Tuple
 
@@ -33,7 +31,6 @@ from smelter_b200.renderer import _FRAME_KIND
 from tests import harness
 from tests.parity import OUTPUT_ID, node_texture, to_oracle_layout
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 YUV = s.OutputFrameFormat.PlanarYuv420Bytes
 NV12 = s.OutputFrameFormat.Nv12WgpuTexture
 RGBA = s.OutputFrameFormat.RgbaWgpuTexture
@@ -336,33 +333,31 @@ def _registry():
 REGISTRY = _registry()
 
 
+FUSED_KERNEL = {F.FUSED_LDG: "ldg", F.FUSED_TMA_INT: "tma_int", F.FUSED_TMA_ANY: "tma_any"}
+
+
+def fused_variants():
+    """(kernel, ratio, window, box, src_class, matrix, launch range) of every fused kernel instantiation the library
+    compiles (smr_debug_fused_variants, no device needed), one per launch key; matrix 1 is BT.601"""
+    L, n = F.lib(), C.c_uint32()
+    assert L.smr_debug_fused_variants(None, 0, C.byref(n)) == 0
+    arr = (F.FusedVariantInfo * n.value)()
+    assert L.smr_debug_fused_variants(arr, n.value, C.byref(n)) == 0 and n.value == len(arr)
+    return [(FUSED_KERNEL[v.kernel], v.ratio, v.window, v.box, v.src_class, int(v.matrix == F.MATRIX_BT601), v.range)
+            for v in arr]
+
+
 def launchable_instantiations():
-    """The (kernel, ratio, window, box, src_class) template instantiations the launch switch of kernels.cu compiles"""
-    src = open(os.path.join(ROOT, "smelter_b200", "csrc", "kernels.cu")).read()
-    hdr = open(os.path.join(ROOT, "smelter_b200", "csrc", "kernels.h")).read()
-    windows = [int(v) for v in re.search(r"kTma0Window\[4\]\s*=\s*\{([^}]*)\}", hdr).group(1).split(",")]
-    used_windows = sorted({windows[int(i)] for i in re.findall(r"launch_tma0_src<kTma0Window\[(\d)\]>", src)})
-    tma0 = set(re.findall(r"launch_tma0<(\d), WINP, (\d)>", src))
-    tma3 = set(re.findall(r"launch_tma3<(\d), (\d)>\(", src))
-    int_s = set(re.findall(r"launch_fused_src<(\d)>\(", src))
-    int_src = set(re.findall(r"launch_fused_int<S, (\d)>\(", src))
-    assert used_windows == windows and tma0 and tma3 and int_s and int_src, "the launch switch of kernels.cu changed shape"
-    out = set()
-    for w in used_windows:
-        for sc, box in tma0:
-            out.add(("tma_any", 0, w, int(box), int(sc)))
-    for S, sc in tma3:
-        out.add(("tma_int", int(S), 0, 0, int(sc)))
-    for S in int_s:
-        for sc in int_src:
-            out.add(("ldg", int(S), 0, 0, int(sc)))
-    return out
+    """The (kernel, ratio, window, box, src_class) template instantiations the library compiles"""
+    return {v[:5] for v in fused_variants()}
 
 
-def test_registry_covers_every_instantiation():
+def test_registry_covers_every_compiled_variant():
     """36 kernels: k_resample_tma3 <2|4, planar|NV12>, k_resample_tma0 <planar|NV12, 20|25|29|33, box 0|1>,
     k_resample_fused_int <2|3|4|0, planar|NV12|UYVY|YUYV>; k_resample_tma3 also on both source ranges (NV12 is limited
-    only) and both vertical paths"""
+    only) and both vertical paths.  The library compiles 96 distinct instantiations in all."""
+    variants = fused_variants()
+    assert len(variants) == len(set(variants)) == 96, sorted(variants)
     inst = launchable_instantiations()
     assert len(inst) == 36, sorted(inst)
     have = {(e.kernel, e.ratio, e.window, e.box, e.src_class) for e in REGISTRY}

@@ -2,17 +2,14 @@
 against the colour oracle `tests/input_color_oracle.c` (DESIGN.md NC-13), and an input left at the default converts as before.
 
 - the composite's 1:1 reader over the joint byte space of every YUV format, for BT.709 / BT.601 x limited / full;
-- every fused-kernel instantiation with a BT.601 source (and the interleaved sources at full range), derived from the
-  launch switch of kernels.cu, with the same kernel choice as the BT.709 child of the same geometry;
+- every fused-kernel instantiation with a BT.601 source (and the interleaved sources at full range), as the library
+  lists them (smr_debug_fused_variants), with the same kernel choice as the BT.709 child of the same geometry;
 - one tick that mixes matrices and ranges on k_resample_tma3 with direct tiles and on k_resample_tma0: one launch per
   (kernel, source class, range, matrix) key;
 - the composite's fast readers (FAST_HALF, FAST_IDENT), rotated and masked layers and the generic reader;
 - defaults, and explicit settings equal to a format's own rule, give the bytes of a handle that never made the call;
 - a setting changed between ticks, an input registered again, deinterlacing with BT.601, RGB inputs.
 """
-import os
-import re
-
 import numpy as np
 import pytest
 
@@ -24,8 +21,8 @@ from tests.test_color_conversion_space import yuv420_block_triples
 from tests.test_gpu_color_conversion import interleaved_frame, reader_frames, run_one, yuv_frame
 from tests.parity import to_oracle_layout
 from tests.test_gpu_composite_classes import child
-from tests.test_gpu_fused_variants import (ALIGNED, REGISTRY, ROOT, Job, launchable_instantiations, make_frame,
-                                           mismatch_report, render, scene_of)
+from tests.test_gpu_fused_variants import (ALIGNED, REGISTRY, Job, fused_variants, make_frame, mismatch_report, render,
+                                           scene_of)
 
 pytestmark = pytest.mark.gpu
 
@@ -119,31 +116,6 @@ def test_passthrough_every_tuple(kind, color):
 # ------------------------------------------------------------------------------------------------
 # 2. / 3. every fused-kernel instantiation with BT.601, and the same kernel choice as BT.709
 # ------------------------------------------------------------------------------------------------
-def color_instantiations():
-    """(kernel, ratio, window, box, src_class, matrix, launch range) of every fused kernel the launch switch compiles: the
-    base instantiations of test_gpu_fused_variants times the matrix, and for k_resample_tma3 and the LDG kernel's
-    interleaved sources times the range"""
-    src = open(os.path.join(ROOT, "smelter_b200", "csrc", "kernels.cu")).read()
-    mats_tma0 = {int(m) for m in re.findall(r"launch_tma0_mat<SRC, WINP, BOX, (\d)>\(", src)}
-    tma3 = {(fr == "true", int(m)) for fr, m in re.findall(r"launch_tma3_range<S, SRC, (true|false), (\d)>\(", src)}
-    ldg = {(fr != "false", int(m)) for m, fr in re.findall(r"launch_fused_kernel<S, SRC, (\d), (IL|false)>\(", src)}
-    assert mats_tma0 == {0, 1} and tma3 == {(f, m) for f in (False, True) for m in (0, 1)} and \
-        ldg == {(f, m) for f in (False, True) for m in (0, 1)}, "the matrix dispatch of kernels.cu changed shape"
-    out = set()
-    for kernel, ratio, window, box, sc in launchable_instantiations():
-        for m in (0, 1):
-            if kernel == "tma_any":
-                out.add((kernel, ratio, window, box, sc, m, 0))
-            elif kernel == "tma_int":
-                for fr in (0, 1):
-                    if sc == 0 or fr == 0 or m == 1:   # NV12 full range: only with BT.601 here (J420 is planar)
-                        out.add((kernel, ratio, window, box, sc, m, fr))
-            else:
-                for fr in ((0, 1) if sc >= 2 else (0,)):
-                    out.add((kernel, ratio, window, box, sc, m, fr))
-    return out
-
-
 def color_registry():
     """one (REGISTRY entry, (matrix, range)) per colour instantiation; DEFAULT keeps the entry's format rule"""
     R = []
@@ -160,17 +132,20 @@ def color_registry():
 COLOR_REGISTRY = color_registry()
 
 
-def key_of(e, color):
+def key_of(e, color, compiled):
+    """the launch key of entry e's job under `color`: a kernel compiled for one range runs a full-range source at range 1,
+    any other reads the range per job (0)"""
     fr = (1 if e.fmt == "yuvj" else 0) if color[1] == s.YuvRange.Default else int(color[1] == FULL)
-    m = 1 if color[0] == BT601 else 0
-    keyed_range = fr if (e.kernel == "tma_int" or (e.kernel == "ldg" and e.src_class >= 2)) else 0
-    return (e.kernel, e.ratio, e.window, e.box, e.src_class, m, keyed_range)
+    key = (e.kernel, e.ratio, e.window, e.box, e.src_class, 1 if color[0] == BT601 else 0)
+    return key + (fr if key + (1,) in compiled else 0,)
 
 
-def test_color_registry_covers_every_new_instantiation():
+def test_color_registry_covers_every_new_compiled_variant():
     """every instantiation a BT.601 source (or an interleaved source at full range) reaches has a scene"""
-    have = {key_of(e, c) for e, c in COLOR_REGISTRY}
-    want = {k for k in color_instantiations() if k[5] == 1 or (k[0] == "ldg" and k[6] == 1)}
+    compiled = set(fused_variants())
+    have = {key_of(e, c, compiled) for e, c in COLOR_REGISTRY}
+    want = {k for k in compiled if k[5] == 1 or (k[0] == "ldg" and k[6] == 1)}
+    assert len(want) == 56, sorted(want)
     assert want <= have, f"instantiations without a scene: {sorted(want - have)}"
 
 
